@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py -- panoptic images/sec of the UPSNet-50 Cityscapes inference hot path (BASELINE.json
-configs[1]: synthetic 1x3x1024x2048, batch 1 per GPU) on N B200s, one process per GPU.
+configs[1]: synthetic 1x3x1024x2048, batch 1 per GPU) on N H100s, one process per GPU.
 
     python bench.py --gpus 1 --steps 20 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
@@ -43,7 +43,8 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d["bf16_tflops_sustained"],
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "source": "fallback"}
+    # H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- a ceiling, not a measured rate
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class NvmlSampler(threading.Thread):
@@ -112,7 +113,7 @@ def bind_to_gpu_numa(index):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons (B200_PROFILING.md recipe); fallback when NVML is not importable."""
+    """nvidia-smi clocks + throttle reasons; fallback when NVML is not importable."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -278,6 +279,31 @@ def parity_block(gpu_model, cpu_out, dev):
     return blk
 
 
+DUMP_BYTES = 64 << 20          # --dump-outputs: total size of the written arrays
+DUMP_SAMPLE = 1 << 20          # elements kept (fixed seeded sample) of an array that would not fit
+
+
+def dump_outputs(out, path):
+    """Results of one engine step as the public forward() returns them (model.py: sizes from out["counts"]), written as
+    <path>/<name>.npy: floating outputs as float32, integer labels / indices as float64 (exact).  An array larger than
+    its share of DUMP_BYTES is replaced by a fixed sample (seed 0) of DUMP_SAMPLE flat elements, in flat-index order."""
+    import numpy as np
+    n1, n2, k = (int(v) for v in out["counts"].tolist())
+    keep = out["keep"][:k]
+    res = {"cls_probs": out["cls_probs"][:n1], "pred_boxes": out["pred_boxes"][:n1], "mask_probs": out["mask_probs"][:n1],
+           "cls_inds": out["cls_inds"][:n1], "fcn_outputs": out["fcn_outputs"], "panoptic_cls_inds": out["p_cls"][:n2][keep],
+           "panoptic_cls_probs": out["p_scores"][:n2][keep], "panoptic_outputs": out["panoptic_outputs"]}
+    os.makedirs(path, exist_ok=True)
+    share = DUMP_BYTES // len(res)
+    for name, t in res.items():
+        a = t.detach().cpu().numpy()
+        a = a.astype(np.float32) if np.issubdtype(a.dtype, np.floating) else a.astype(np.float64)
+        if a.nbytes > share:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_SAMPLE, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -285,13 +311,16 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--precision", default=os.environ.get("UPSNET_PRECISION", "bf16x3"), choices=["fp32", "bf16x3", "bf16"],
-                    help="bf16x3 (default, the configuration the parity tests certify at 'fp32 logits within 1e-3'): tcgen05 "
-                         "hi/lo split on the hi/lo bf16 pair stream; bf16: tcgen05 single pass + bf16 activation storage "
+                    help="bf16x3 (default, the configuration the parity tests certify at 'fp32 logits within 1e-3'): wgmma "
+                         "hi/lo split on the hi/lo bf16 pair stream; bf16: wgmma single pass + bf16 activation storage "
                          "(secondary figure, bf16-level error); fp32: CUDA-core tiles")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-other-configs", action="store_true", help="skip the configs[2] / configs[4] extras of the default run")
     ap.add_argument("--lanes", type=int, default=int(os.environ.get("UPSNET_LANES", "2")),
                     help="images in flight per GPU: independent engine instances (CUDA-graph instance + pool + scratch) on their own streams")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the results of the last timed step (what a caller of the engine receives) "
+                         "as DIR/<name>.npy (float32 / float64, at most 64 MB in all) for output-by-output comparison of two builds")
     ap.add_argument("--workload", default="cityscapes", choices=["cityscapes", "coco"],
                     help="cityscapes = BASELINE configs[1] (the metric); coco = configs[2] UPSNet-101-DCN 800x1344 (extra)")
     args = ap.parse_args()
@@ -326,7 +355,7 @@ def main():
         model = synthetic_model(UPSNetConfig.coco_r101_dcn(), depth=(3, 4, 23, 3), seed=0, device=dev)
     else:
         model = synthetic_model(UPSNetConfig.cityscapes_r50(), seed=0, device=dev)
-    n_img = 4  # rotate distinct images; one step touches >1 GB of activations (>> 126 MB L2)
+    n_img = 4  # rotate distinct images; one step touches >1 GB of activations (>> 50 MB L2)
     host_imgs = [synthetic_input(H, W, seed=100 * rank + s)["data"].pin_memory() for s in range(n_img)]
     dev_imgs = [h.to(dev) for h in host_imgs]
     im_info = synthetic_input(8, 8)["im_info"]; im_info[0, :2] = (H, W)
@@ -347,11 +376,14 @@ def main():
     LANES = max(1, int(args.lanes))
     lane_streams = [torch.cuda.Stream(dev) for _ in range(LANES)]
 
+    last = {}
+
     def step_graph(i):
         l = i % LANES
         with torch.cuda.stream(lane_streams[l]):
             out, _ = model._run_static(dev_imgs[i % n_img], im_info[0], lane=l)
             counts_host[i % counts_host.shape[0]].copy_(out["counts"], non_blocking=True)
+        last["out"] = out
         return out
 
     # end-to-end leg: the pipelined serving front end (upsnet_b200/pipeline.py).  Every step submits one PINNED HOST
@@ -419,6 +451,8 @@ def main():
     counts_host.zero_()
     ms, launches, per_rank = timed(step_graph, args.steps)
     assert int(counts_host[:args.steps, 0].min()) >= 1, "every image must yield at least the dummy detection"
+    if args.dump_outputs and rank == 0:
+        dump_outputs(last["out"], args.dump_outputs)
     ms_e2e, _, per_rank_e2e = timed(step_e2e, args.steps, finish=drain_e2e)
     clocks = sampler.stop() if sampler else None
     h2d, d2h = engine.bytes_per_image()
@@ -495,19 +529,13 @@ def main():
     algo = sum(w.get("algo_flops", w.get("flops", 0.0)) for k_, _, _, w in trace if k_ == "conv2d")
     achieved = algo / (conv["ms"] * 1e-3) / 1e12 if conv["ms"] > 0 else 0.0   # ALGORITHMIC flops (x3 MMAs not counted)
     dcn_algo = sum(w.get("algo_flops", 0.0) for k_, _, _, w in trace if k_ == "dcn")
-    kname = {"bf16": "igemm_tma_kernel (TMA-fed tcgen05 implicit GEMM; dense conv / FC family incl. stem)",
-             "bf16x3": "igemm_tma2_kernel / igemm_tma_kernel on hi/lo bf16 pairs (TMA-fed tcgen05 implicit GEMM, 3 MMAs per "
-                       "k-slice: hi*hi + lo*hi + hi*lo; 2-CTA cta_group::2 variant for tiles with >= 8 k-blocks, 1-CTA "
-                       "otherwise; dense conv / FC family incl. the RGB stem)",
+    kname = {"bf16": "igemm_tma_kernel (TMA-fed wgmma implicit GEMM; dense conv / FC family incl. stem)",
+             "bf16x3": "igemm_tma_kernel on hi/lo bf16 pairs (TMA-fed wgmma implicit GEMM, 3 MMAs per k-slice: "
+                       "hi*hi + lo*hi + hi*lo; dense conv / FC family incl. the RGB stem)",
              "fp32": "igemm_simt_kernel (fp32 CUDA-core tiles)"}[args.precision]
     roofline = {"kernel": kname + ", precision=%s" % args.precision, "bound": "tensor",
                 "achieved": achieved, "peak": pk["tf_sustained"], "unit": "TFLOP/s",
-                "frac": achieved / pk["tf_sustained"], "peak_source": pk["source"] + " (sustained bf16)",
-                # dram__bytes_read.sum + dram__bytes_write.sum of ONE representative launch of the family under `ncu --set full`
-                # (profiles/r2_pair_full.md: FPN / RPN 3x3 256->256 @256x512 on pairs, 136.7 MB read + 93.7 MB written against
-                # algorithmic x + y = 268 MB: no re-reads from HBM); null for the other precisions (not captured)
-                "traffic": 230.4e6 if args.precision == "bf16x3" else None,
-                "traffic_launch": "FPN / RPN 3x3 256->256 @256x512 (154.6 GFLOP algorithmic, 268 MB algorithmic bytes)" if args.precision == "bf16x3" else None,
+                "frac": achieved / pk["tf_sustained"], "peak_source": pk["source"] + " (bf16)",
                 "share_of_step": conv["ms"] / tot_ms if tot_ms else None,
                 "avg_launch_ms": conv["ms"] / max(conv["calls"], 1),
                 "flops_per_step": algo / n_trace, "mma_flops_per_step": conv["flops"] / n_trace,
@@ -534,7 +562,7 @@ def main():
             step_graph(i)
         ms3, _, _ = timed(step_graph, max(5, args.steps // 2))
         other = {"precision": "bf16", "value": world * max(5, args.steps // 2) / (ms3 * 1e-3), "unit": "images/s",
-                 "note": "single tcgen05 pass on bf16 activations: bf16-level error (tests hold it to 4e-2..8e-2), reported "
+                 "note": "single wgmma pass on bf16 activations: bf16-level error (tests hold it to 4e-2..8e-2), reported "
                          "for reference only -- the headline is the bf16x3 pair stream that meets 'fp32 logits within 1e-3'"}
         U.set_precision(args.precision)
     # The other BASELINE configurations, measured in the same (driver-run) process: configs[2] UPSNet-101-DCN at 800x1344
@@ -600,7 +628,7 @@ def main():
                 "scaling": "weak", "vs_baseline": None, "dtype": {"fp32": "fp32", "bf16x3": "bf16x3", "bf16": "bf16"}[args.precision],
                 "data": "synthetic",
                 "config": {"workload": WORKLOAD, "parallelism": "replicas x%d (one image per GPU, no collective)" % world,
-                           "l2": "no flush: each step streams >1 GB of activations (>> 126 MB L2) and rotates %d images" % n_img,
+                           "l2": "no flush: each step streams >1 GB of activations (>> 50 MB L2) and rotates %d images" % n_img,
                            "weights": "random-init (upsnet_b200/synthetic.py), frozen BN folded",
                            "engine": "static shapes, device-side counts, CUDA graph replay=%s; value = sync-free engine entry "
                                      "(result sizes read back asynchronously), e2e = public PipelinedEngine API; %d engine lane(s): consecutive images "
@@ -645,7 +673,7 @@ def run_ops(args):
             fn()
         tot = 0.0
         for _ in range(iters):
-            flush.zero_()                                   # L2 flush (256 MB > 126 MB L2)
+            flush.zero_()                                   # L2 flush (256 MB > 50 MB L2)
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record(); fn(); b.record(); torch.cuda.synchronize()
             tot += a.elapsed_time(b)
@@ -736,7 +764,7 @@ def run_ops(args):
     row("dcn v1 fp32 simt", "FCN L1@P2 256->128 3x3, 256x512", gpu_ms(lambda: U.deform_conv(x, off, w, b, 1, 1, 1, precision=0), iters=5), by, fl, rm)
     for name, prec in (("bf16x3", 1), ("bf16", 2)):
         got = U.deform_conv(x, off, w, b, 1, 1, 1, precision=prec)
-        row("dcn v1 tcgen05 " + name, "FCN L1@P2 256->128 3x3, 256x512",
+        row("dcn v1 wgmma " + name, "FCN L1@P2 256->128 3x3, 256x512",
             gpu_ms(lambda: U.deform_conv(x, off, w, b, 1, 1, 1, precision=prec)), by, fl, None, None,
             (got.float() - base).abs().max().item())
     x2 = torch.randn(2, 256, 50, 84, device=dev); om = torch.randn(2, 27, 50, 84, device=dev)
@@ -755,7 +783,7 @@ def run_ops(args):
     xcl = x.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
     for name, prec in (("bf16x3", 1), ("bf16", 2)):
         got = U.conv2d(xcl, wc, None, 1, 1, 1, precision=prec)
-        row("conv3x3 tcgen05 " + name, "256->256 @256x512", gpu_ms(lambda: U.conv2d(xcl, wc, None, 1, 1, 1, precision=prec)),
+        row("conv3x3 wgmma " + name, "256->256 @256x512", gpu_ms(lambda: U.conv2d(xcl, wc, None, 1, 1, 1, precision=prec)),
             None, flc, None, None, (got.float() - basec).abs().max().item())
 
     # ---- config 5: panoptic-head sweep at 1024x2048 ----

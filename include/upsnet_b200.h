@@ -1,5 +1,5 @@
 /*
- * upsnet_b200.h -- C ABI of libupsnet_b200.so: hand-written sm_100a CUDA for the UPSNet
+ * upsnet_b200.h -- C ABI of libupsnet_b200.so: hand-written sm_90a (H100) CUDA for the UPSNet
  * per-image inference hot path (SURVEY.md section 8).  Plain pointers and sizes only; no
  * torch types.  Every entry point
  *   - takes DEVICE pointers unless the name ends in _host,
@@ -51,10 +51,10 @@ extern "C" {
 
 /* precision of the tensor-core convolution path */
 #define UPSNET_PREC_FP32_SIMT 0 /* fp32 FFMA tiles (exact-order-free fp32)            */
-#define UPSNET_PREC_BF16X3 1    /* tcgen05 kind::f16, 3-term bf16 split (~fp32 result) */
-#define UPSNET_PREC_BF16 2      /* tcgen05 kind::f16, single bf16 pass                 */
+#define UPSNET_PREC_BF16X3 1    /* wgmma bf16, 3-term bf16 split (~fp32 result)     */
+#define UPSNET_PREC_BF16 2      /* wgmma bf16, single bf16 pass                     */
 
-/* library / build identification: returns e.g. 100 for sm_100a, fills `n_sm` if non-NULL */
+/* library / build identification: returns 90 for sm_90a, fills `n_sm` if non-NULL */
 int upsnet_version(int *n_sm);
 
 /* ---------------------------------------------------------------------------------------
@@ -129,7 +129,7 @@ int upsnet_conv2d_forward(const float *x, const float *weight, const float *bias
                           void *stream);
 
 /* ---------------------------------------------------------------------------------------
- * tcgen05 implicit-GEMM convolution / deformable convolution (engine entry point).
+ * wgmma implicit-GEMM convolution / deformable convolution (engine entry point).
  * Same arithmetic contract as upsnet_conv2d_forward / upsnet_dcn_forward, but
  *   - x is NHWC [N,H,W,Cin] (Cin % 64 == 0) stored as fp32 or bf16 (x_dtype) -- or, for a tiny Cin <= 8 (the
  *     RGB stem), the fp32 NCHW image itself: K = kh*kw*Cin is flattened and zero-padded to a multiple of 64; y and residual are NHWC or
@@ -171,7 +171,7 @@ int upsnet_dcn_pair_forward(const void *x_pair, const float *offset, const float
                             int pad_h, int pad_w, int dil_h, int dil_w, int epi_flags, void *stream);
 /* Dense 3x3 / stride-1 convolution on hi/lo PAIR activations through the same window pipeline (csrc/dcn_win.cu, DENSE mode):
  * the input window of a 16x8-pixel tile is staged once per 16-channel sub-chunk by TMA and feeds all nine taps, the A operand
- * is copied window -> TMEM.  Meant for the small-N layers (18-channel offset convs of the semantic head, 64->64 bottleneck
+ * is copied window -> A operand tile in shared memory.  Meant for the small-N layers (18-channel offset convs of the semantic head, 64->64 bottleneck
  * convs) whose per-tap TMA boxes make upsnet_igemm_forward L2->SM-bandwidth-bound.  x [N,H,W,2*Cin] pair NHWC; `packed`
  * from upsnet_dcn_pack_weight; y = fp32 NCHW [N,Cout,Ho,Wo] (UPSNET_LAYOUT_NCHW, any Cout) or pair NHWC [N,Ho,Wo,2*Cout]
  * (UPSNET_LAYOUT_NHWC, Cout % 16 == 0); epi_flags: UPSNET_EPI_RELU.  Same arithmetic contract as upsnet_igemm_forward
@@ -228,7 +228,7 @@ int upsnet_mask_removal(const float *boxes, const float *cls_prob, const float *
  * [N,Ho,Wo,2*Cout] computed with the three-pass split from hi/lo copies of the image -- fused bias + ReLU (UPSNET_EPI_RELU).
  * replaces: models/resnet.py:155-162 conv1 + bn1 (folded) + relu.
  * The call first packs the image to a zero-padded bf16 NHWC8 copy in `workspace` (upsnet_stem_workspace_bytes),
- * then runs the tcgen05 kernel whose A tiles are boxes of a 5-D tensor map over that copy; weights are packed
+ * then runs the wgmma kernel whose A tiles are boxes of a 5-D tensor map over that copy; weights are packed
  * once with upsnet_stem_pack_weight ([Cout][kh][8][8] bf16, upsnet_stem_packed_weight_bytes).
  * Returns UPSNET_E_UNSUPPORTED if the driver rejects the tensor map (callers fall back to upsnet_igemm_forward). */
 int upsnet_stem_workspace_bytes(int N, int H, int W, int kh, int kw, int pad, size_t *bytes);

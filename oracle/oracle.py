@@ -9,7 +9,7 @@ import this module; the product package ``upsnet_b200`` never does.
   materialises the [k,H,W] planes exactly like the reference does; it pins the fused C version
   at small sizes.
 * ``RefKernels`` loads oracle/_ref/libupsnet_ref.so = the reference's own .cu kernels compiled
-  for sm_100a (GPU box only).
+  for sm_90a (where the reference checkout is present).
 """
 import ctypes as C
 import os
@@ -33,7 +33,8 @@ def build(force=False):
         subprocess.check_call(["make", "-C", _HERE, os.path.join(_HERE, "libupsnet_oracle.so")])
     if os.path.isdir("/root/reference/upsnet/operators/src") and (
             force or not os.path.exists(os.path.join(_HERE, "_ref", "libupsnet_ref.so"))):
-        subprocess.check_call(["make", "-C", _HERE, "ref"])
+        from upsnet_b200.build import nvcc
+        subprocess.check_call(["make", "-C", _HERE, "ref", "NVCC=" + nvcc()])
     return so
 
 

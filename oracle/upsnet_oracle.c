@@ -9,7 +9,7 @@
  * (SURVEY.md section 4), so the oracle is pinned against
  *   (i)   the reference's own pure-numpy NMS (upsnet/nms/py_cpu_nms.py), imported
  *         in the build container by tests/golden/make_golden.py -> committed fixtures;
- *   (ii)  the reference's own CUDA kernels compiled for sm_100a (oracle/_ref, built
+ *   (ii)  the reference's own CUDA kernels compiled for sm_90a (oracle/_ref, built
  *         by oracle/Makefile from the sources where they lie) on the GPU box;
  *   (iii) torchvision.ops.roi_align / deform_conv2d (same Caffe2 / MSRA lineage).
  * The panoptic head's cv2.resize step is NOT bit-reproducible from any formula

@@ -70,7 +70,7 @@ CASES = [
     dict(N=1, Cin=128, Cout=128, H=8, W=16, pd=1, off="large"),        # single tile
     dict(N=1, Cin=128, Cout=128, H=40, W=64, pd=1, off="huge"),        # almost everything is an outlier / outside the image
     dict(N=1, Cin=64, Cout=64, H=6, W=5, pd=1, off="zero"),            # map smaller than a tile, zero offsets == dense conv
-    dict(N=3, Cin=64, Cout=128, H=64, W=96, pd=1, off="tapbias"),      # > 148 tiles: persistent CTAs run several tiles
+    dict(N=3, Cin=64, Cout=128, H=64, W=96, pd=1, off="tapbias"),      # > 132 tiles: persistent CTAs run several tiles
 ]
 
 
@@ -134,7 +134,7 @@ DENSE_CASES = [
     dict(N=2, Cin=64, Cout=64, H=40, W=56, pd=1, nchw=False, relu=True),       # res2 conv2 shape class: pair out + ReLU
     dict(N=1, Cin=64, Cout=32, H=20, W=20, pd=2, nchw=False, relu=False),      # dilation 2, N tile 32, pair out
     dict(N=1, Cin=128, Cout=27, H=9, W=7, pd=1, nchw=True, relu=True),         # map smaller than a tile, odd Cout
-    dict(N=3, Cin=64, Cout=18, H=64, W=96, pd=1, nchw=True, relu=False),       # > 148 tiles
+    dict(N=3, Cin=64, Cout=18, H=64, W=96, pd=1, nchw=True, relu=False),       # > 132 tiles
     dict(N=1, Cin=512, Cout=18, H=16, W=24, pd=1, nchw=True, relu=False),      # 72 k-blocks
 ]
 

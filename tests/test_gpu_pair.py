@@ -1,4 +1,4 @@
-"""GPU parity of the hi/lo bf16 PAIR activation stream (precision bf16x3 on the TMA-fed tcgen05 kernel, VERDICT r1 item 1):
+"""GPU parity of the hi/lo bf16 PAIR activation stream (precision bf16x3 on the TMA-fed wgmma kernel):
 every layer shape class of the engine against the CPU oracle at the "fp32 logits within 1e-3" contract -- in practice
 held to ~1e-5 relative, which is what makes the pair stream an fp32-grade format.  Own file = own process (a trap in a
 tensor-core kernel poisons the CUDA context)."""
@@ -51,10 +51,25 @@ def test_pair_roundtrip(dev, pair_mode):
     assert err <= 2.0 ** -16 * x.abs().max().item(), err
 
 
+def _conv_kernels(fn):
+    """fn() under torch.profiler: its result and the names of the implicit-GEMM conv kernels it launched."""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        out = fn()
+        torch.cuda.synchronize()
+    return out, {e.key for e in prof.key_averages() if "igemm_" in e.key}
+
+
+def _assert_kernel(names, tma):
+    """The TMA-fed kernel serves the layer when it is enabled (no silent fall-back to the gather kernel), else the gather one."""
+    want, other = ("igemm_tma_kernel", "igemm_tc_kernel") if tma else ("igemm_tc_kernel", "igemm_tma_kernel")
+    assert any(want in n for n in names) and not any(other in n for n in names), names
+
+
 CONV_CASES = [
     dict(N=1, Cin=64, Cout=64, H=16, W=16, k=1, stride=1, pad=0, dil=1),      # one k-block
     dict(N=1, Cin=256, Cout=64, H=16, W=24, k=1, stride=1, pad=0, dil=1),     # ring wrap
-    dict(N=1, Cin=64, Cout=128, H=20, W=28, k=3, stride=1, pad=1, dil=1),     # 3x3 halo candidate, ragged tiles
+    dict(N=1, Cin=64, Cout=128, H=20, W=28, k=3, stride=1, pad=1, dil=1),     # 3x3, ragged tiles
     dict(N=1, Cin=256, Cout=256, H=32, W=48, k=3, stride=1, pad=1, dil=1),    # FPN / RPN 3x3 shape class
     dict(N=2, Cin=128, Cout=256, H=15, W=17, k=3, stride=1, pad=1, dil=1),    # batch, odd sizes
     dict(N=1, Cin=256, Cout=512, H=16, W=20, k=1, stride=2, pad=0, dil=1),    # strided 1x1 (down-sampling conv)
@@ -82,22 +97,26 @@ def test_pair_conv_vs_oracle(dev, pair_mode, cfg, tma):
     ops.USE_TMA["on"] = tma
     try:
         xp = Pair.from_float(t(x, dev))
-        got = U.conv2d(xp, t(w, dev), t(b, dev), cfg["stride"], cfg["pad"], cfg["dil"], precision=X3)
+        got, k1 = _conv_kernels(lambda: U.conv2d(xp, t(w, dev), t(b, dev), cfg["stride"], cfg["pad"], cfg["dil"], precision=X3))
+        _assert_kernel(k1, tma)
         assert isinstance(got, Pair) and got.shape == want.shape
         g = got.float().cpu().numpy()
         # 3 MMAs drop only lo*lo (2^-18 of sum|x||w|); pair storage of x and y adds 2^-17 each
         err = np.abs(g - want)
         assert (err <= 4e-5 * bound + 2e-5 * np.abs(want) + 1e-6).all(), float((err / (bound + 1e-3)).max())
         assert err.max() < 1e-3
-        got2 = U.conv2d(xp, t(w, dev), t(b, dev), cfg["stride"], cfg["pad"], cfg["dil"], residual=Pair.from_float(t(res, dev)),
-                        relu=True, precision=X3)
+        rp = Pair.from_float(t(res, dev))
+        got2, k2 = _conv_kernels(lambda: U.conv2d(xp, t(w, dev), t(b, dev), cfg["stride"], cfg["pad"], cfg["dil"], residual=rp,
+                                                  relu=True, precision=X3))
+        _assert_kernel(k2, tma)
         want2 = np.maximum(want + res, 0)
         err2 = np.abs(got2.float().cpu().numpy() - want2)
         assert (err2 <= 4e-5 * bound + 4e-5 * (np.abs(want) + np.abs(res)) + 1e-6).all(), float(err2.max())
         # fp32 plane-wise head output from a pair input (direct-store epilogue), Cout clipped to a head-like count
         co = min(cfg["Cout"], 19)
-        got3 = U.conv2d(xp, t(w[:co].copy(), dev), t(b[:co].copy(), dev), cfg["stride"], cfg["pad"], cfg["dil"], precision=X3,
-                        out_format="nchw")
+        got3, k3 = _conv_kernels(lambda: U.conv2d(xp, t(w[:co].copy(), dev), t(b[:co].copy(), dev), cfg["stride"], cfg["pad"],
+                                                  cfg["dil"], precision=X3, out_format="nchw"))
+        _assert_kernel(k3, tma)
         assert got3.dtype == torch.float32 and got3.is_contiguous()
         err3 = np.abs(got3.cpu().numpy() - want[:, :co])
         assert (err3 <= 4e-5 * bound[:, :co] + 1e-6).all(), float(err3.max())

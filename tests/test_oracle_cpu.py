@@ -167,11 +167,11 @@ def test_cabi_library_exports_every_declared_symbol():
     declared = sorted(set(re.findall(r"\bint\s+(upsnet_\w+)\s*\(", header)))
     assert declared, "no declarations parsed"
     assert sorted(_lib.EXPORTED_SYMBOLS) == declared
-    so = build.build()  # nvcc cross-compiles for sm_100a without a GPU
+    so = build.build()  # nvcc cross-compiles for sm_90a without a GPU
     L = ctypes.CDLL(so)
     for name in declared:
         assert hasattr(L, name), name
-    assert L.upsnet_version(None) == 100
+    assert L.upsnet_version(None) == 90
 
 
 def test_ops_fail_loudly_without_cuda_tensors():

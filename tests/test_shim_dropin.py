@@ -4,13 +4,9 @@
    model code (:36-37 config, :43-44 `from upsnet.models import *`, :162 `eval(config.symbol)()`, :190-193
    `load_state_dict(..., resume=True)` with DataParallel's `module.` prefix, and the backbone-only torchvision key
    remapping of models/resnet.py:213-222), then a forward through the engine (CPU ops plugged in: no GPU here).
-2. overlay: a scratch COPY of the reference tree with `upsnet/{models,operators,nms}` overlaid by this repository's shim
-   files (never `upsnet/config`): the reference's OWN config module + experiment yaml drive the zero-argument factory.
-   Needs /root/reference, i.e. runs in the build container only."""
+2. the reference's operator module paths and constructor signatures, and the shim modules against the stored
+   outputs of the reference's own modules (tests/golden/reference_modules.npz)."""
 import os
-import shutil
-import subprocess
-import sys
 import textwrap
 
 import numpy as np
@@ -18,7 +14,6 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
 
 
 def test_standalone_script_lines_and_state_dict(tmp_path):
@@ -126,51 +121,3 @@ def test_shim_modules_vs_reference_fixtures():
                      class_agnostic=bool(c["agnostic"]), score_thresh=float(c["score_thresh"]))
         s, b, ci = mr(torch.from_numpy(c["rois"]), torch.from_numpy(c["delta"]), torch.from_numpy(c["prob"]), ref["mroi_im_info"])
         _check_mroi(c, s.numpy(), b.numpy(), ci.numpy())
-
-
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "upsnet")), reason="needs the reference checkout (build container)")
-def test_overlay_on_reference_tree(tmp_path):
-    """Overlay scenario in a subprocess: scratch copy of the reference + this repository's shim over models / operators /
-    nms; the reference's own `upsnet/config/config.py` and experiment yaml configure `eval(config.symbol)()`."""
-    tree = tmp_path / "ref"
-    shutil.copytree(os.path.join(REF, "upsnet"), tree / "upsnet", ignore=shutil.ignore_patterns("*.so", "*.o", "build", "_ext"))
-    shutil.copytree(os.path.join(REF, "lib"), tree / "lib")
-    for sub in ("models", "operators", "nms"):
-        shutil.copytree(os.path.join(ROOT, "upsnet", sub), tree / "upsnet" / sub, dirs_exist_ok=True)
-    code = textwrap.dedent("""
-        import sys, types
-        import numpy as np
-        np.float = float; np.int = int
-        class ED(dict):                       # easydict is not installed in this image; the reference config needs it
-            def __init__(s, d=None, **k):
-                super().__init__()
-                for a, b in dict(d or {}, **k).items(): s[a] = b
-            def __setitem__(s, a, b): super().__setitem__(a, ED(b) if isinstance(b, dict) and not isinstance(b, ED) else b)
-            __setattr__ = __setitem__
-            def __getattr__(s, a):
-                try: return s[a]
-                except KeyError: raise AttributeError(a)
-        m = types.ModuleType("easydict"); m.EasyDict = ED; sys.modules["easydict"] = m
-        import yaml; _load = yaml.load
-        yaml.load = lambda f, Loader=None: _load(f, Loader=Loader or yaml.SafeLoader)    # PyYAML >= 6 (SURVEY Appendix B)
-        sys.path.insert(0, %r)                 # what upsnet_end2end_test.py:33-34 do with its own location
-        sys.path.append(%r)                    # this repository (upsnet_b200) via PYTHONPATH
-        from upsnet.config.config import config, update_config
-        import upsnet.config.config as C
-        assert C.__file__.startswith(%r), C.__file__                         # the REFERENCE's config module
-        update_config(%r)
-        from upsnet.models import *
-        test_model = eval(config.symbol)()
-        import upsnet_b200.model as M
-        assert isinstance(test_model, M.resnet_upsnet), type(test_model)
-        assert test_model.cfg.fcn_num_layers == config.network.fcn_num_layers == 2
-        assert test_model.cfg.num_seg_classes == 19 and test_model.cfg.max_det == config.test.max_det
-        sd = {"module." + k: v for k, v in test_model.state_dict().items()}
-        test_model.load_state_dict(sd, resume=True)
-        from upsnet.operators.modules.deform_conv import DeformConv
-        import upsnet_b200.operators as O
-        assert DeformConv is O.DeformConv
-        print("OVERLAY_OK", config.symbol)
-    """) % (str(tree), ROOT, str(tree), os.path.join(REF, "upsnet", "experiments", "upsnet_resnet50_cityscapes_16gpu.yaml"))
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "OVERLAY_OK resnet_50_upsnet" in r.stdout, r.stdout + r.stderr

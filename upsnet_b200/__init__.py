@@ -1,4 +1,4 @@
-"""upsnet_b200 -- B200-native (sm_100a) implementation of the UPSNet per-image inference hot path
+"""upsnet_b200 -- H100-native (sm_90a) implementation of the UPSNet per-image inference hot path
 behind the reference's own operator API.  All compute lives in libupsnet_b200.so (C ABI:
 include/upsnet_b200.h); this package is the thin PyTorch-facing host layer."""
 from .operators import (DeformConv, DeformConvWithOffset, ModDeformConv, ModDeformConvWithOffsetMask,  # noqa: F401

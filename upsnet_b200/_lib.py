@@ -121,7 +121,7 @@ def ptr(t):
 def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise UpsnetError("upsnet_b200 ops are CUDA-only (sm_100a); got a %s tensor" % t.device)
+            raise UpsnetError("upsnet_b200 ops are CUDA-only (sm_90a); got a %s tensor" % t.device)
 
 
 def f32c(t):

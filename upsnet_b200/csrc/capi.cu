@@ -1,5 +1,5 @@
 // capi.cu -- convolution / deformable-convolution entry points of the C ABI and dispatch
-// between the fp32 CUDA-core tiles (igemm_simt.cu) and the tcgen05 tensor-core tiles
+// between the fp32 CUDA-core tiles (igemm_simt.cu) and the wgmma tensor-core tiles
 // (igemm_tc.cu).  See include/upsnet_b200.h for the contract of every symbol.
 #include "common.cuh"
 #include "tc_params.cuh"
@@ -23,7 +23,7 @@ extern "C" int upsnet_version(int* n_sm) {
     else
       *n_sm = -1;
   }
-  return 100;
+  return 90;
 }
 
 static int conv_common(const float* x, const float* offset, const float* mask, const float* weight,

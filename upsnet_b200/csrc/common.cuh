@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the sm_100a kernels of libupsnet_b200.so
+// common.cuh -- shared helpers for the sm_90a kernels of libupsnet_b200.so
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -19,7 +19,7 @@
 
 namespace ups {
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // cudaFuncSetAttribute is per device (and context): remember which devices a kernel has been configured on, so that a
 // process driving several GPUs (the reference's thread-per-GPU DataParallel, gpu_nms(device_id)) opts in on each of them.

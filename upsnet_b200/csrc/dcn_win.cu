@@ -1,25 +1,26 @@
 // dcn_win.cu -- fused deformable convolution (v1 / v2) on hi/lo bf16 PAIR activations with the bilinear corners
-// gathered from a SHARED-MEMORY WINDOW instead of global memory (sm_100a).
+// gathered from a SHARED-MEMORY WINDOW instead of global memory (sm_90a).
 //
 // Reference semantics: operators/src/deform_conv_kernel.cu:89-118 (bilinear corner rule), :194-242 (im2col, the
 // h > -1 && w > -1 && h < H && w < W test at :229), operators/functions/deform_conv.py:44-57 (im2col + torch.mm);
 // v2 mask: operators/src/mod_deform_conv_kernel.cu.  Same arithmetic contract as igemm_tc_kernel<1,2> (igemm_tc.cu),
-// which this kernel replaces for 3x3 / stride-1 layers on the pair stream: round 2's profile of that kernel
-// (profiles/r2_pair_full.md) shows the gather ISSUE-bound -- ~300 instructions per (pixel, tap, 8 channels), a third of
-// them 64-bit address arithmetic and unpacking around eight long-latency LDG.128 -- with the tensor pipe at 18 %.
+// which this kernel replaces for 3x3 / stride-1 layers on the pair stream: that kernel's gather is issue-bound -- a few
+// hundred instructions per (pixel, tap, 8 channels), much of it 64-bit address arithmetic and unpacking around eight
+// long-latency global loads.
 //
 // Here the K axis is ordered (16-channel sub-chunk, tap, channel): for one sub-chunk the nine taps x four corners of a
 // 16 x 8-pixel tile touch one small window of the input -- (16 + 3 + offset range) x (8 + 3 + offset range) pixels x
-// 16 channels x (hi, lo) -- which ONE TMA box pair stages in shared memory (30 x 20 pixels, 2 x 19.2 KB, double buffered).
+// 16 channels x (hi, lo) -- which ONE TMA box pair stages in shared memory (32 x 20 pixels, 2 x 20 KB, double buffered).
 // The 16 gather warps then read corners with LDS.128 at immediate offsets (+32 B = x+1, +960 B = y+1), blend (hi plane:
-// packed fp32x2 FMAs, lo plane: packed bf16x2 HFMA2), re-split and store the A tile in the SWIZZLE_128B K-major layout
-// tcgen05 consumes; weights (packed in the same K order by dcn_win_pack_weight) arrive by TMA.  Samples that fall
+// fp32 FMAs, lo plane: packed bf16x2 HFMA2), re-split and store the A tile in the SWIZZLE_128B K-major layout
+// wgmma consumes; weights (packed in the same K order by dcn_win_pack_weight) arrive by TMA.  Samples that fall
 // outside the window (large offsets) are flagged in the per-tile sample table and gathered from global memory by the
 // same thread, so the result never depends on the window size -- only the speed does.
 //
-// Warp roles (23 warps): 0-3 epilogue (TMEM -> bias / ReLU -> hi/lo split -> NHWC pair stores), 4 MMA issuer (three
-// tcgen05.mma per K=16 slice: lo*hi, hi*lo, hi*hi; two TMEM accumulator buffers), 5 weight TMA, 6 window TMA,
-// 7-22 gather producers in two groups that fill alternate k-blocks.
+// Warp roles (22 warps): 0-3 consumers (one warpgroup: per K=16 slice three wgmma pairs -- lo*hi, hi*lo, hi*hi for tile
+// rows 0-63 and 64-127 -- accumulators in registers, then staged through shared memory -> bias / ReLU -> hi/lo split ->
+// NHWC pair stores, thread = tile pixel), 4 weight TMA, 5 window TMA, 6-21 gather producers in two groups that fill
+// alternate k-blocks.
 // Roofline: tensor pipe (2*P*Cout*Cin*9 flop x 3 passes); per k-block and SM the gather costs ~4 K warp instructions
 // and 128 KB of shared-memory reads against 12 MMAs of 128x128x16 -- see DESIGN.md section 4.
 #include <cuda.h>
@@ -34,19 +35,24 @@ namespace ups {
 
 constexpr int DW_BM = 128;            // pixels per M tile
 constexpr int DW_BK = 64;             // K elements per k-block = 4 slices of 16 channels
-constexpr int DW_STAGES = 3;          // operand ring depth: A stages live in TMEM (gather warps), B stages in smem (TMA)
-constexpr int DW_WW = 32, DW_WH = 24; // window box in pixels; the row pitch (32 px = 1024 B) keeps bank = f(x) only
+constexpr int DW_STAGES = 3;          // operand ring depth: A stages (gather warps) and B stages (TMA), both in smem
+constexpr int DW_WW = 32, DW_WH = 20; // window box in pixels; the row pitch (32 px = 1024 B) keeps bank = f(x) only
 constexpr int DW_PLANE = DW_WW * DW_WH * 32;      // one plane (hi or lo) of a window: 16 channels x 2 B per pixel
 constexpr int DW_WIN_BYTES = 2 * DW_PLANE;
 constexpr int DW_KHW = 9;
 constexpr int DW_GROUP = 256, DW_GROUPS = 2, DW_PRODUCERS = DW_GROUP * DW_GROUPS;
-constexpr int DW_WARP_MMA = 4, DW_WARP_TMAB = 5, DW_WARP_TMAW = 6, DW_WARP_PROD0 = 7;
-constexpr int DW_THREADS = (DW_WARP_PROD0 + DW_PRODUCERS / 32) * 32;   // 736
-constexpr uint32_t DW_TMEM_A0 = 256;  // TMEM columns [0,256): two accumulators; [256 + 64 s, +64): A stage s (hi 32 cols, lo 32 cols)
+constexpr int DW_CONSUMERS = 128, DW_WARP_TMAB = 4, DW_WARP_TMAW = 5, DW_WARP_PROD0 = 6;
+constexpr int DW_THREADS = (DW_WARP_PROD0 + DW_PRODUCERS / 32) * 32;   // 704
+// N tile: the two m64 accumulator fragments of a consumer thread (DW_BN floats) have to fit next to the addressing in the
+// registers 22 warps per SM leave (ptxas -v: 80 used per thread).  Measured on H100 SXM (400 W), bf16x3 bench: N = 32 runs the semantic head's deformable convs in
+// 6.2 ms per image, N = 64 (fragments spilled to local memory) in 15.6 ms.
+constexpr int DW_BN = 32;
+constexpr uint32_t DW_A_BYTES = 2 * DW_BM * 128;   // A stage: hi tile, lo tile (128 rows x 64 bf16, SWIZZLE_128B)
+constexpr int DW_EPI_PITCH = 36;      // floats per row of the accumulator staging buffer (32 columns + pad)
+constexpr uint32_t DW_EPI_BYTES = DW_BM * DW_EPI_PITCH * 4;
 
 // shared-memory map (byte offsets from the 1024-aligned base)
 constexpr uint32_t DW_OFF_BARS = 0;        // 18 mbarriers
-constexpr uint32_t DW_OFF_TMEM = 160;
 constexpr uint32_t DW_OFF_STATS = 192;     // 2 x int[8]: min w, min h, max w, max h, sum w, sum h, count, -
 constexpr uint32_t DW_OFF_ORG = 256;       // 2 x int4: window origin (w, h), image, -
 constexpr uint32_t DW_OFF_TW = 512;        // float4 [9][128] corner weights
@@ -63,7 +69,7 @@ struct DwParams {
   int N, H, W, Cin, Cout, Cout_pad, Ho, Wo, ph, pw, dh, dw, relu, BN, tile_w, tile_h;
   // DENSE mode (offset == null): plain 3x3 / stride-1 convolution through the same pipeline -- the window of a tile is its
   // receptive field (origin = tile origin - pad, known without a sample table), a "gather" is one LDS.128 per plane copied
-  // to the TMEM A operand, no blend.  Serves the small-N 3x3 layers of the pair stream (18-channel offset convs, 64->64
+  // to the A operand tile, no blend.  Serves the small-N 3x3 layers of the pair stream (18-channel offset convs, 64->64
   // bottleneck convs), which the per-tap TMA boxes of igemm_tma.cu make L2->SM-bandwidth-bound (A re-fetched per tap).
   int dense;
   int out_nchw;           // y = fp32 NCHW [N,Cout,Ho,Wo] (offset maps) instead of the pair NHWC tensor
@@ -75,6 +81,7 @@ struct DwParams {
   int win_plane;          // bytes of one plane of a window buffer
   int win_buf;            // bytes of one window buffer (both planes)
   int stages;             // operand ring depth (2 or 3)
+  int win_nbuf;           // window buffers (2: the next fill streams in while the current one is gathered; dense mode: 1)
 };
 
 __device__ __forceinline__ void dw_expect_tx(uint32_t bar, uint32_t bytes) {
@@ -99,21 +106,6 @@ __device__ __forceinline__ uint4 dw_lds128(uint32_t addr) {
   return v;
 }
 __device__ __forceinline__ void dw_producer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(DW_PRODUCERS) : "memory"); }
-// registers -> TMEM: lane i of the warp writes four consecutive 32-bit columns of TMEM lane (quadrant base + i)
-__device__ __forceinline__ void dw_tmem_st4(uint32_t taddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ void dw_tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// D[tmem] (+)= A[tmem] * B[smem desc]^T, kind::f16: A = 128 TMEM lanes x 8 columns (16 bf16 of K, two per column)
-__device__ __forceinline__ void dw_umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint32_t b_lo, uint32_t desc_hi, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 db;\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(desc_hi) : "memory");
-}
 
 __global__ void __launch_bounds__(DW_THREADS, 1)
 dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const DwParams p) {
@@ -123,20 +115,19 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
   uint8_t* sm = smem_dyn + (base - raw);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t b_bytes = (uint32_t)p.BN * 128;
-  const uint32_t stage_bytes = 2 * b_bytes;                                 // weight tile: hi plane, lo plane
+  const uint32_t b_bytes = (uint32_t)DW_BN * 128;
+  const uint32_t stage_bytes = 2 * b_bytes + DW_A_BYTES;                    // weight tile (hi, lo planes), then the A tiles
   const uint32_t NST = (uint32_t)p.stages;
   const uint32_t win_base = base + DW_OFF_STAGES + NST * stage_bytes;       // 1024-aligned (stage_bytes % 1024 == 0)
+  const uint32_t NWB = (uint32_t)p.win_nbuf;
+  float* stf = reinterpret_cast<float*>(sm + (win_base - base) + NWB * (uint32_t)p.win_buf);   // accumulator staging
   // barriers
-  const uint32_t bar_fa = base + DW_OFF_BARS;            // full_a[3]: 8 producer warps each (A stage written to TMEM)
+  const uint32_t bar_fa = base + DW_OFF_BARS;            // full_a[3]: 8 producer warps each (A stage written)
   const uint32_t bar_fb = bar_fa + 24;                   // full_b[3]: weight TMA (tx)
-  const uint32_t bar_em = bar_fa + 48;                   // empty[3]: tcgen05.commit (A stage in TMEM + B stage in smem consumed)
-  const uint32_t bar_tf = bar_fa + 72;                   // tmem_full[2]
-  const uint32_t bar_te = bar_fa + 88;                   // tmem_empty[2]: 4 epilogue warps
+  const uint32_t bar_em = bar_fa + 48;                   // empty[3]: 4 consumer warps (their wgmmas have read A and B)
   const uint32_t bar_wf = bar_fa + 104;                  // win_full[2]: window TMA (tx)
   const uint32_t bar_we = bar_fa + 120;                  // win_empty[2]: 16 producer warps
   const uint32_t bar_og = bar_fa + 136;                  // org_full[2]: window origin of a tile published
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(sm + DW_OFF_TMEM);
   int* stats = reinterpret_cast<int*>(sm + DW_OFF_STATS);
   int4* org = reinterpret_cast<int4*>(sm + DW_OFF_ORG);
   float4* tw = reinterpret_cast<float4*>(sm + DW_OFF_TW);
@@ -147,23 +138,20 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
   const int spf = p.dense ? 4 : 1;                    // sub-chunks per window fill
   const int nfill = nsc / spf;                        // window fills per tile
   const int num_kb = nsc * DW_KHW / 4;                // Cin % 64 == 0 -> integral
-  const int n_tiles = p.Cout_pad / p.BN;
+  const int n_tiles = p.Cout_pad / DW_BN;
   const int TW = p.tile_w, TH = p.tile_h;
   const int tw_shift = TW == 16 ? 4 : 3;
   const int tiles_w = (p.Wo + TW - 1) / TW, tiles_h = (p.Ho + TH - 1) / TH;
   const long long num_tiles = (long long)p.N * tiles_w * tiles_h * n_tiles;
-  constexpr uint32_t tmem_cols = 512;
 
-  if (warp == DW_WARP_MMA) {
+  if (warp == 0) {
     if (lane == 0) {
       for (int s = 0; s < DW_STAGES; ++s) {
         mbar_init(bar_fa + 8 * s, DW_GROUP / 32);
         mbar_init(bar_fb + 8 * s, 1);
-        mbar_init(bar_em + 8 * s, 1);
+        mbar_init(bar_em + 8 * s, DW_CONSUMERS / 32);
       }
       for (int s = 0; s < 2; ++s) {
-        mbar_init(bar_tf + 8 * s, 1);
-        mbar_init(bar_te + 8 * s, 4);
         mbar_init(bar_wf + 8 * s, 1);
         mbar_init(bar_we + 8 * s, DW_PRODUCERS / 32);
         mbar_init(bar_og + 8 * s, 1);
@@ -176,19 +164,15 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
       }
     }
     __syncwarp();
-    tmem_alloc(smem_u32(tmem_ptr_smem), tmem_cols);
   }
   if (warp == DW_WARP_TMAB && lane == 0) dw_prefetch_tmap(&tm_w);
   if (warp == DW_WARP_TMAW && lane == 0) dw_prefetch_tmap(&tm_x);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   if (warp >= DW_WARP_PROD0) {
     // =============================== GATHER PRODUCERS ===============================
-    // A warp owns the 32 rows of ITS TMEM lane quadrant (hardware rule: warp w reaches lanes 32 (w % 4) .. +31), lane = row:
-    // the 32 lanes of an LDS.128 read one (slice, 8-channel half) of 32 consecutive tile pixels.  The window is stored by
+    // A warp owns 32 rows of the A tile (quadrant = producer warp % 4), lane = row: the 32 lanes of an LDS.128 read one
+    // (slice, 8-channel half) of 32 consecutive tile pixels.  The window is stored by
     // TMA with SWIZZLE_32B (16-byte chunk ^= address bit 7, i.e. pixel bit 2), so eight horizontally consecutive pixels of
     // one half occupy eight different 16-byte bank groups: a quarter-warp wavefront is conflict-free whenever its samples
     // stay on consecutive pixels of any rows (row pitch 1024 B).
@@ -196,7 +180,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     const int pw = warp - DW_WARP_PROD0;         // 0..15
     const int group = pw >> 3;                   // alternate k-blocks
     const int u = (pw >> 2) & 1;                 // which two of the k-block's four slices this warp gathers
-    const int quad = warp & 3;                   // TMEM lane quadrant
+    const int quad = pw & 3;                     // A rows [32 quad, 32 quad + 32)
     const int r = quad * 32 + lane;              // A row = tile pixel
     const __nv_bfloat16* xh = reinterpret_cast<const __nv_bfloat16*>(p.x);
     uint32_t g0 = 0, wf0 = 0;                    // running k-block / window-fill counters at the start of the tile
@@ -307,8 +291,8 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         const uint32_t g = g0 + (uint32_t)kb;
         const uint32_t s = g % NST, it = g / NST;
         mbar_wait(bar_em + 8 * s, (it & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t a_col = tmem_base + ((uint32_t)(quad * 32) << 16) + DW_TMEM_A0 + s * 64u;
+        // A stage s: hi tile then lo tile, row r = 128 bytes, 16-byte chunk j of K at (j ^ (r & 7)) (SWIZZLE_128B)
+        const uint32_t a_row = base + DW_OFF_STAGES + s * stage_bytes + 2 * b_bytes + (uint32_t)r * 128u;
 #pragma unroll 1
         for (int pass = 0; pass < 4; ++pass) {
           const int sl = 2 * u + (pass >> 1), half = pass & 1;
@@ -316,19 +300,19 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
           const int sc = q / DW_KHW, tap = q - sc * DW_KHW;
           const uint32_t wf = wf0 + (uint32_t)(dense ? (sc >> 2) : sc);      // dense: one fill per 64-channel chunk
           if (wf >= wf_ready) {                         // first touch of this window fill
-            mbar_wait(bar_wf + 8 * (wf & 1u), (wf >> 1) & 1u);
+            mbar_wait(bar_wf + 8 * (wf % NWB), (wf / NWB) & 1u);
             wf_ready = wf + 1;
           }
-          const uint32_t wbuf = win_base + (wf & 1u) * (uint32_t)p.win_buf;
+          const uint32_t wbuf = win_base + (wf % NWB) * (uint32_t)p.win_buf;
           const int code = tp[tap * DW_BM + r];
-          if (dense) {        // plain copy of the tap's pixel: window -> TMEM A operand
+          const uint32_t a_off = (((uint32_t)(sl * 2 + half) ^ (uint32_t)(r & 7)) << 4);   // K elements 16 sl + 8 half ..
+          if (dense) {        // plain copy of the tap's pixel: window -> A operand
             // SWIZZLE_128B window: a pixel is one 128-byte row (64 channels), 16-byte chunk c sits at c ^ (pixel & 7)
             const uint32_t pix = (uint32_t)code, ch = (uint32_t)((sc & 3) * 2 + half);
             const uint32_t al = wbuf + pix * 128u + ((ch ^ (pix & 7u)) << 4);
             const uint4 h4 = dw_lds128(al), l4 = dw_lds128(al + (uint32_t)p.win_plane);
-            const uint32_t col = a_col + (uint32_t)(sl * 8 + half * 4);
-            dw_tmem_st4(col, h4.x, h4.y, h4.z, h4.w);
-            dw_tmem_st4(col + 32u, l4.x, l4.y, l4.z, l4.w);
+            sts128(a_row + a_off, h4);
+            sts128(a_row + DW_BM * 128u + a_off, l4);
             continue;
           }
           const float4 wv = tw[tap * DW_BM + r];
@@ -356,7 +340,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
             hc[2] = __ldg(reinterpret_cast<const uint4*>(b10)); lc[2] = __ldg(reinterpret_cast<const uint4*>(b10 + p.Cin));
             hc[3] = __ldg(reinterpret_cast<const uint4*>(b11)); lc[3] = __ldg(reinterpret_cast<const uint4*>(b11 + p.Cin));
           }
-          // blend: hi plane in packed fp32x2 (exact products of bf16 values), lo plane in packed bf16x2 (2^-9 of the
+          // blend: hi plane in fp32 on channel pairs (exact products of bf16 values), lo plane in packed bf16x2 (2^-9 of the
           // value: its blend needs 2^-9 relative accuracy only), summed in fp32 and split again
           const float wf4[4] = {wv.x, wv.y, wv.z, wv.w};
           unsigned long long acc[4] = {0ull, 0ull, 0ull, 0ull};
@@ -372,7 +356,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
             for (int qq = 0; qq < 4; ++qq) {
               unsigned long long hp;
               asm("mov.b64 %0, {%1, %2};" : "=l"(hp) : "r"(hw_[qq] << 16), "r"(hw_[qq] & 0xffff0000u));
-              asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(acc[qq]) : "l"(wp), "l"(hp), "l"(acc[qq]));
+              acc[qq] = f32x2_fma(wp, hp, acc[qq]);
               const __nv_bfloat162 lv = *reinterpret_cast<const __nv_bfloat162*>(&lw_[qq]);
               lacc[qq] = i == 0 ? __hmul2(wb, lv) : __hfma2(wb, lv, lacc[qq]);
             }
@@ -383,33 +367,30 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
             const uint32_t lw = *reinterpret_cast<const uint32_t*>(&lacc[qq]);
             unsigned long long lp;
             asm("mov.b64 %0, {%1, %2};" : "=l"(lp) : "r"(lw << 16), "r"(lw & 0xffff0000u));
-            asm("add.rn.f32x2 %0, %1, %2;" : "=l"(acc[qq]) : "l"(acc[qq]), "l"(lp));
+            acc[qq] = f32x2_add(acc[qq], lp);
             uint32_t a0, a1;
             asm("mov.b64 {%0, %1}, %2;" : "=r"(a0), "=r"(a1) : "l"(acc[qq]));
             const float v0 = __uint_as_float(a0), v1 = __uint_as_float(a1);
             ohi[qq] = pack_bf16x2(v0, v1);
             olo[qq] = pack_bf16x2(v0 - __uint_as_float(ohi[qq] << 16), v1 - __uint_as_float(ohi[qq] & 0xffff0000u));
           }
-          // A operand in TMEM: K element k of the k-block = 16-bit slot k of the row's 32 columns (slice sl = columns 8 sl .. +7)
-          const uint32_t col = a_col + (uint32_t)(sl * 8 + half * 4);
-          dw_tmem_st4(col, ohi[0], ohi[1], ohi[2], ohi[3]);
-          dw_tmem_st4(col + 32u, olo[0], olo[1], olo[2], olo[3]);
+          sts128(a_row + a_off, make_uint4(ohi[0], ohi[1], ohi[2], ohi[3]));
+          sts128(a_row + DW_BM * 128u + a_off, make_uint4(olo[0], olo[1], olo[2], olo[3]));
         }
-        dw_tmem_st_wait();
-        tc_fence_before();
+        fence_proxy_async();    // generic-proxy stores -> visible to wgmma (async proxy)
         __syncwarp();
         if (lane == 0) {
           mbar_arrive(bar_fa + 8 * s);
           // window buffers this warp will not read again: its next k-block (kb + 2) starts at slice 4 * (kb + 2)
           while (rel < nfill && DW_KHW * spf * (rel + 1) <= 4 * (kb + DW_GROUPS)) {
-            mbar_arrive(bar_we + 8 * ((wf0 + (uint32_t)rel) & 1u));
+            mbar_arrive(bar_we + 8 * ((wf0 + (uint32_t)rel) % NWB));
             ++rel;
           }
         }
         rel = __shfl_sync(0xffffffffu, rel, 0);
       }
       if (lane == 0) {
-        while (rel < nfill) { mbar_arrive(bar_we + 8 * ((wf0 + (uint32_t)rel) & 1u)); ++rel; }
+        while (rel < nfill) { mbar_arrive(bar_we + 8 * ((wf0 + (uint32_t)rel) % NWB)); ++rel; }
       }
       __syncwarp();
       g0 += (uint32_t)num_kb;
@@ -433,8 +414,8 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         }
         const int cstep = 16 * spf;
         for (int f = 0; f < nfill; ++f, ++wf) {
-          const uint32_t b = wf & 1u;
-          mbar_wait(bar_we + 8 * b, ((wf >> 1) & 1u) ^ 1u);
+          const uint32_t b = wf % NWB;
+          mbar_wait(bar_we + 8 * b, ((wf / NWB) & 1u) ^ 1u);
           dw_expect_tx(bar_wf + 8 * b, (uint32_t)p.win_bytes);
           const uint32_t dst = win_base + b * (uint32_t)p.win_buf;
           dw_tma_4d(dst, &tm_x, bar_wf + 8 * b, f * cstep, o.x, o.y, o.z);
@@ -448,7 +429,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     if (lane == 0) {
       uint32_t g = 0;
       for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int n0 = (int)(tile % n_tiles) * p.BN;
+        const int n0 = (int)(tile % n_tiles) * DW_BN;
         for (int kb = 0; kb < num_kb; ++kb, ++g) {
           const uint32_t s = g % NST, it = g / NST;
           mbar_wait(bar_em + 8 * s, (it & 1u) ^ 1u);
@@ -460,111 +441,112 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
       }
     }
     __syncwarp();
-  } else if (warp == DW_WARP_MMA) {
-    // =============================== MMA ISSUER ===============================
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc(DW_BM, p.BN);
-      const uint32_t desc_hi = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);
-      const uint32_t b0 = ((base + DW_OFF_STAGES) >> 4) & 0x3fffu, stage16 = stage_bytes >> 4, b16 = b_bytes >> 4;
-      uint32_t s = 0, ph = 0, b_hi = b0, ti = 0;
-      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++ti) {
-        const uint32_t buf = ti & 1u, use = ti >> 1;
-        mbar_wait(bar_te + 8 * buf, (use & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + buf * (uint32_t)p.BN;
-        uint32_t acc = 0u;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(bar_fb + 8 * s, ph);
-          mbar_wait(bar_fa + 8 * s, ph);
-          tc_fence_after();
-          const uint32_t a_hi = tmem_base + DW_TMEM_A0 + s * 64u, a_lo = a_hi + 32u, b_lo = b_hi + b16;
-#pragma unroll
-          for (uint32_t k = 0; k < DW_BK / 16; ++k) {
-            dw_umma_ts(tmem_d, a_lo + 8 * k, b_hi + 2 * k, desc_hi, idesc, acc);
-            dw_umma_ts(tmem_d, a_hi + 8 * k, b_lo + 2 * k, desc_hi, idesc, 1u);
-            dw_umma_ts(tmem_d, a_hi + 8 * k, b_hi + 2 * k, desc_hi, idesc, 1u);
-            acc = 1u;
-          }
-          umma_commit(bar_em + 8 * s);
-          b_hi += stage16;
-          if (++s == NST) { s = 0; ph ^= 1u; b_hi = b0; }
-        }
-        umma_commit(bar_tf + 8 * buf);
-      }
-    }
-    __syncwarp();
   } else {
-    // =============================== EPILOGUE (warps 0-3) ===============================
-    const int q = warp & 3;
-    uint32_t ti = 0;
+    // =============================== CONSUMERS (warps 0-3) ===============================
+    const uint32_t dhi = wg_desc_hi(1024);
+    float d0[DW_BN / 2], d1[DW_BN / 2];                   // tile rows [0, 64) and [64, 128)
+    constexpr uint32_t h16 = 64u * 128u / 16u;      // rows 64-127: 64 rows of 128 bytes further
     __nv_bfloat16* yb = reinterpret_cast<__nv_bfloat16*>(p.y);
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++ti) {
+    uint32_t s = 0, ph = 0;
+    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const long long mt = tile / n_tiles;
-      const int n0 = (int)(tile % n_tiles) * p.BN;
+      const int n0 = (int)(tile % n_tiles) * DW_BN;
       const int tx = (int)(mt % tiles_w), ty = (int)((mt / tiles_w) % tiles_h), n = (int)(mt / ((long long)tiles_w * tiles_h));
-      const uint32_t buf = ti & 1u, use = ti >> 1;
-      mbar_wait(bar_tf + 8 * buf, use & 1u);
-      tc_fence_after();
-      const int m = q * 32 + lane;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(bar_fb + 8 * s, ph);
+        mbar_wait(bar_fa + 8 * s, ph);
+        const uint32_t st0 = base + DW_OFF_STAGES + s * stage_bytes;
+        const uint32_t b_hi = wg_desc_lo(st0), b_lo = wg_desc_lo(st0 + b_bytes);
+        const uint32_t a_hi = wg_desc_lo(st0 + 2 * b_bytes), a_lo = wg_desc_lo(st0 + 2 * b_bytes + DW_BM * 128u);
+        wgmma_fence();
+#pragma unroll
+        for (uint32_t k = 0; k < DW_BK / 16; ++k) {
+          const uint32_t acc = (kb | k) ? 1u : 0u;
+          const uint64_t bh = wg_desc(b_hi + 2 * k, dhi), bl = wg_desc(b_lo + 2 * k, dhi);
+          Wgmma<DW_BN>::mma(d0, wg_desc(a_lo + 2 * k, dhi), bh, acc);
+          Wgmma<DW_BN>::mma(d1, wg_desc(a_lo + h16 + 2 * k, dhi), bh, acc);
+          Wgmma<DW_BN>::mma(d0, wg_desc(a_hi + 2 * k, dhi), bl, 1u);
+          Wgmma<DW_BN>::mma(d1, wg_desc(a_hi + h16 + 2 * k, dhi), bl, 1u);
+          Wgmma<DW_BN>::mma(d0, wg_desc(a_hi + 2 * k, dhi), bh, 1u);
+          Wgmma<DW_BN>::mma(d1, wg_desc(a_hi + h16 + 2 * k, dhi), bh, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                // the previous k-block's wgmmas have read their stage
+        wgmma_fence_acc(d0);
+        wgmma_fence_acc(d1);
+        if (prev >= 0 && lane == 0) mbar_arrive(bar_em + 8 * prev);
+        prev = (int)s;
+        if (++s == NST) { s = 0; ph ^= 1u; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(d0);
+      wgmma_fence_acc(d1);
+      if (prev >= 0 && lane == 0) mbar_arrive(bar_em + 8 * prev);
+
+      // ---- epilogue: 32 accumulator columns at a time through shared memory, thread = tile pixel ----
+      const int m = warp * 32 + lane;
       const int ry = m >> tw_shift;
       const int wo = tx * TW + (m & (TW - 1)), ho = ty * TH + ry;
       const bool row_ok = ry < TH && wo < p.Wo && ho < p.Ho;
       __nv_bfloat16* yp = yb + (((size_t)n * p.Ho + ho) * p.Wo + wo) * (size_t)(2 * p.Cout);
-      const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + buf * (uint32_t)p.BN;
-      for (int cb = 0; cb < p.BN; cb += 16) {
-        if (n0 + cb >= p.Cout) break;              // zero-padded weight rows (warp-uniform)
-        uint32_t rr[16];
-        tmem_ld16(trow + (uint32_t)cb, rr);
-        if (!row_ok) continue;
-        const int co = n0 + cb;
-        float o[16];
+      const uint32_t trow = smem_u32(stf + (size_t)m * DW_EPI_PITCH);
+      for (int c32 = 0; c32 < DW_BN; c32 += 32) {
+        if (n0 + c32 >= p.Cout) break;                 // zero-padded weight rows (CTA-uniform)
+        named_bar(2, DW_CONSUMERS);                    // the previous chunk has been read
 #pragma unroll
-        for (int e = 0; e < 16; ++e) o[e] = __uint_as_float(rr[e]);
-        if (p.bias) {
-          if (co + 16 <= p.Cout) {
+        for (int c = 0; c < DW_BN; c += 32)
+          if (c == c32) {
+            acc_stage<DW_BN, 32>(d0, stf, DW_EPI_PITCH, 0, c);
+            acc_stage<DW_BN, 32>(d1, stf, DW_EPI_PITCH, 64, c);
+          }
+        named_bar(2, DW_CONSUMERS);
+        for (int cb = c32; cb < c32 + 32 && cb < DW_BN; cb += 16) {
+          if (n0 + cb >= p.Cout) break;
+          uint32_t rr[16];
+          acc_ld16(trow + (uint32_t)(cb - c32) * 4u, rr);
+          if (!row_ok) continue;
+          const int co = n0 + cb;
+          float o[16];
 #pragma unroll
-            for (int e4 = 0; e4 < 4; ++e4) {
-              const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + co) + e4);
-              o[4 * e4] += bv.x; o[4 * e4 + 1] += bv.y; o[4 * e4 + 2] += bv.z; o[4 * e4 + 3] += bv.w;
+          for (int e = 0; e < 16; ++e) o[e] = __uint_as_float(rr[e]);
+          if (p.bias) {
+            if (co + 16 <= p.Cout) {
+#pragma unroll
+              for (int e4 = 0; e4 < 4; ++e4) {
+                const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + co) + e4);
+                o[4 * e4] += bv.x; o[4 * e4 + 1] += bv.y; o[4 * e4 + 2] += bv.z; o[4 * e4 + 3] += bv.w;
+              }
+            } else {
+#pragma unroll
+              for (int e = 0; e < 16; ++e)
+                if (co + e < p.Cout) o[e] += __ldg(p.bias + co + e);
             }
-          } else {
+          }
+          if (p.relu) {
+#pragma unroll
+            for (int e = 0; e < 16; ++e) o[e] = fmaxf(o[e], 0.f);
+          }
+          if (p.out_nchw) {     // plane-wise fp32 output (offset maps): for a fixed channel the lanes write consecutive pixels
+            float* yf = reinterpret_cast<float*>(p.y) + ((size_t)n * p.Cout + co) * HoWo + (size_t)ho * p.Wo + wo;
 #pragma unroll
             for (int e = 0; e < 16; ++e)
-              if (co + e < p.Cout) o[e] += __ldg(p.bias + co + e);
+              if (co + e < p.Cout) yf[(size_t)e * HoWo] = o[e];
+            continue;
           }
-        }
-        if (p.relu) {
+          uint32_t hw[8], lw[8];
 #pragma unroll
-          for (int e = 0; e < 16; ++e) o[e] = fmaxf(o[e], 0.f);
+          for (int e = 0; e < 8; ++e) {
+            hw[e] = pack_bf16x2(o[2 * e], o[2 * e + 1]);
+            lw[e] = pack_bf16x2(o[2 * e] - __uint_as_float(hw[e] << 16), o[2 * e + 1] - __uint_as_float(hw[e] & 0xffff0000u));
+          }
+          uint4* dh_ = reinterpret_cast<uint4*>(yp + co);
+          uint4* dl_ = reinterpret_cast<uint4*>(yp + p.Cout + co);
+          dh_[0] = make_uint4(hw[0], hw[1], hw[2], hw[3]); dh_[1] = make_uint4(hw[4], hw[5], hw[6], hw[7]);
+          dl_[0] = make_uint4(lw[0], lw[1], lw[2], lw[3]); dl_[1] = make_uint4(lw[4], lw[5], lw[6], lw[7]);
         }
-        if (p.out_nchw) {     // plane-wise fp32 output (offset maps): for a fixed channel the lanes write consecutive pixels
-          float* yf = reinterpret_cast<float*>(p.y) + ((size_t)n * p.Cout + co) * HoWo + (size_t)ho * p.Wo + wo;
-#pragma unroll
-          for (int e = 0; e < 16; ++e)
-            if (co + e < p.Cout) yf[(size_t)e * HoWo] = o[e];
-          continue;
-        }
-        uint32_t hw[8], lw[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          hw[e] = pack_bf16x2(o[2 * e], o[2 * e + 1]);
-          lw[e] = pack_bf16x2(o[2 * e] - __uint_as_float(hw[e] << 16), o[2 * e + 1] - __uint_as_float(hw[e] & 0xffff0000u));
-        }
-        uint4* dh_ = reinterpret_cast<uint4*>(yp + co);
-        uint4* dl_ = reinterpret_cast<uint4*>(yp + p.Cout + co);
-        dh_[0] = make_uint4(hw[0], hw[1], hw[2], hw[3]); dh_[1] = make_uint4(hw[4], hw[5], hw[6], hw[7]);
-        dl_[0] = make_uint4(lw[0], lw[1], lw[2], lw[3]); dl_[1] = make_uint4(lw[4], lw[5], lw[6], lw[7]);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_te + 8 * buf);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == DW_WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
   }
 }
 
@@ -652,7 +634,7 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
   p.Wo = conv_out_size(W, pad_w, dil_w, 3, 1);
   if (p.Ho <= 0 || p.Wo <= 0) return UPSNET_E_BADARG;
   p.relu = (epi_flags & UPSNET_EPI_RELU) ? 1 : 0;
-  p.BN = p.Cout_pad % 128 == 0 ? 128 : (p.Cout_pad % 64 == 0 ? 64 : 32);
+  p.BN = DW_BN;
   p.dense = dense ? 1 : 0; p.out_nchw = out_nchw ? 1 : 0;
   static int sms = 0;
   if (sms == 0) {
@@ -676,7 +658,7 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
   if (num_tiles <= 0) return 0;
   // dense: the window box is the tile's receptive field: 24 pixels x (tile + halo) rows x 64 channels (128-byte pixels)
   int win_h = DW_WH;
-  p.win_pitch = DW_WW; p.win_plane = DW_PLANE; p.win_buf = DW_WIN_BYTES; p.stages = DW_STAGES;
+  p.win_pitch = DW_WW; p.win_plane = DW_PLANE; p.win_buf = DW_WIN_BYTES; p.stages = DW_STAGES; p.win_nbuf = 2;
   if (dense) {
     win_h = p.tile_h + 2 * dil_h;
     p.win_pitch = 24;
@@ -684,6 +666,7 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
     p.win_plane = p.win_pitch * win_h * 128;
     p.win_plane = (p.win_plane + 1023) / 1024 * 1024;     // SWIZZLE_128B destinations: 1024-byte aligned planes
     p.win_buf = 2 * p.win_plane;
+    p.win_nbuf = 1;       // one 64-channel fill serves 36 k-slices: a second buffer does not fit next to the A stages
   }
   if (!dense) {     // tuning hook: UPSNET_DCN_WIN_H = rows of the deformable window box (12..24)
     static int wh_env = -1;
@@ -692,7 +675,9 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
   }
   p.win_bytes = dense ? 2 * p.win_pitch * win_h * 128 : 2 * DW_WW * win_h * 32;
   p.win_h = win_h;
-  auto smem_need = [&]() { return (size_t)DW_OFF_STAGES + (size_t)p.stages * 2 * (p.BN * 128) + 2 * (size_t)p.win_buf + 1024; };
+  auto smem_need = [&]() {
+    return (size_t)DW_OFF_STAGES + (size_t)p.stages * (2 * (p.BN * 128) + DW_A_BYTES) + (size_t)p.win_nbuf * p.win_buf + DW_EPI_BYTES + 1024;
+  };
   if (smem_need() > 227 * 1024 && p.stages > 2) p.stages = 2;
   if (smem_need() > 227 * 1024) return UPSNET_E_UNSUPPORTED;
   DwEncodeFn enc = dw_encoder();

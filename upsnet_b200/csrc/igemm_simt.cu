@@ -13,7 +13,7 @@
 // (tap, pixel) the four bilinear corner offsets + weights are computed ONCE (they do not
 // depend on the channel) and reused for all Cin channels of the deformable group.
 // NCHW fp32 in/out like the reference.  This path is bounded by the fp32 FFMA rate, not by
-// tensor cores; the tcgen05 path lives in igemm_tc.cu.
+// tensor cores; the wgmma path lives in igemm_tc.cu.
 #include "common.cuh"
 
 namespace ups {

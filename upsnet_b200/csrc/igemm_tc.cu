@@ -1,22 +1,24 @@
-// igemm_tc.cu -- tcgen05 implicit-GEMM convolution / deformable convolution for sm_100a.
+// igemm_tc.cu -- wgmma implicit-GEMM convolution / deformable convolution for sm_90a.
 //
 // One warp-specialised kernel covers the dense k x k convolutions of the backbone / FPN / RPN /
 // heads, the fully connected layers and the FUSED deformable conv v1/v2 (im2col never leaves the
 // SM; reference: deformable_im2col -> 1.2 GB col buffer -> torch.mm, operators/functions/
 // deform_conv.py:44-57 + operators/src/deform_conv_kernel.cu:194-242).
 //
-//   D[128 pixels x BN couts] (fp32, TMEM)  +=  A[128 x 64] (bf16, smem)  *  B[BN x 64]^T (bf16, smem)
+//   D[128 pixels x BN couts] (fp32, registers)  +=  A[128 x 64] (bf16, smem)  *  B[BN x 64]^T (bf16, smem)
 //
 // * A (activations, NHWC fp32 in HBM) is GATHERED by 8 producer warps: for k-block (tap, 64
 //   channels) every (pixel,8-channel) item is one or -- when deformable -- four 32-byte reads
 //   (the four bilinear corners; weights/offsets come from a per-tile sample table computed once
 //   per (tap,pixel), reused by all channels), blended in fp32, converted to bf16 and stored with
-//   one 16-byte st.shared into the K-major SWIZZLE_128B layout tcgen05 consumes.
+//   one 16-byte st.shared into the K-major SWIZZLE_128B layout wgmma consumes.
 // * B (weights) is pre-packed once to bf16 [Cout_pad][tap][Cin] and copied by the same warps.
-// * One elected thread issues tcgen05.mma (kind::f16, M=128, N=BN, K=16) per 16-column slice;
-//   tcgen05.commit releases the smem stage to the producers through an mbarrier; accumulators
-//   live in TMEM (two buffers) and are drained with tcgen05.ld (32x32b.x16) by 4 epilogue warps
-//   while the next tile's main loop is already running (persistent CTAs, static tile schedule).
+// * One consumer warpgroup issues two wgmma (M=64 each: rows 0-63 and 64-127 of the tile, N=BN,
+//   K=16) per 16-column slice with the accumulators in registers; a stage goes back to the producers through an
+//   mbarrier once the wgmmas that read it have completed.  At the end of a tile the accumulators
+//   are staged through shared memory 32 columns at a time and written out by the same 4 warps
+//   (thread = output pixel) while the producers already fill the ring for the next tile
+//   (persistent CTAs, static tile schedule).
 // * Precision modes: BF16 (one pass) and BF16X3 (x = hi + lo split of both operands, three
 //   MMAs: hi*hi + lo*hi + hi*lo; error ~2^-16 relative, i.e. fp32-grade results for the
 //   "fp32 logits within 1e-3" contract at 3x the tensor work).
@@ -37,19 +39,18 @@ constexpr int TC_BK = 64;          // bf16 elements per k-block row (= 128 bytes
 constexpr int TC_GROUP = 256;       // producer threads that fill one smem stage together (8 warps)
 constexpr int TC_GROUPS = 2;        // producer groups work on alternate k-blocks (two stages in flight)
 constexpr int TC_PRODUCERS = TC_GROUP * TC_GROUPS;  // 16 warps
-constexpr int TC_EPILOGUE = 128;      // 4 warps: TMEM lane quadrant = warp & 3 (x TC_EPI_SPLIT column slices)
-constexpr int TC_EPI_SPLIT = TC_EPILOGUE / 128;
+constexpr int TC_CONSUMERS = 128;     // 4 warps = one wgmma warpgroup; in the epilogue thread = tile row
 constexpr int TC_EPI_PITCH = 36;      // floats per staged row: 32 columns + 4 pad (16-byte aligned, conflict-free)
-constexpr int TC_THREADS = TC_EPILOGUE + 32 + TC_PRODUCERS;  // 21 warps
+constexpr int TC_THREADS = TC_CONSUMERS + TC_PRODUCERS;  // 20 warps
 constexpr int TC_MAX_STAGES = 6;
 
 
 
 // shared-memory carve-up (offsets from the 1024-aligned base)
 struct TcSmem {
-  uint32_t bars;      // full[6], empty[6], tmem_full[2], tmem_empty[2] (16 x 8 B) then tmem ptr
+  uint32_t bars;      // full[6], empty[6]
   uint32_t rowbase;   // long long [128]
-  uint32_t epi;       // epilogue staging: 4 warps x 32 rows x 36 floats (coalesced NHWC stores)
+  uint32_t epi;       // accumulator staging: 128 rows x 36 floats (32 columns at a time)
   uint32_t table;     // deform: float4 [KHW][128] + int4 [KHW][128]; dense: int [KHW][128]
   uint32_t stages;    // 1024-aligned
   uint32_t a_bytes, b_bytes, stage_bytes, total;
@@ -59,7 +60,7 @@ __host__ __device__ inline TcSmem tc_smem_layout(bool deform, int KHW, int BN, i
   s.bars = 0;
   s.rowbase = 256;
   s.epi = s.rowbase + 2 * TC_BM * 8;     // two row-info buffers, then the epilogue staging area
-  s.table = s.epi + (TC_EPILOGUE / 32) * 32 * TC_EPI_PITCH * 4;
+  s.table = s.epi + TC_BM * TC_EPI_PITCH * 4;
   const uint32_t tbytes = deform ? KHW * TC_BM * 32 : KHW * TC_BM * 4;
   s.stages = (uint32_t)((s.table + tbytes + 1023) / 1024 * 1024);
   s.a_bytes = TC_BM * 128;
@@ -69,23 +70,24 @@ __host__ __device__ inline TcSmem tc_smem_layout(bool deform, int KHW, int BN, i
   return s;
 }
 
-// Named barrier among the producer warps only (ids 1.. ; id 0 is __syncthreads)
+// Named barriers (id 0 is __syncthreads): 1 = the producer warps, 2 = the consumer warps
 __device__ __forceinline__ void producer_bar_sync() {
   asm volatile("bar.sync 1, %0;" ::"n"(TC_PRODUCERS) : "memory");
 }
 
-// Persistent, warp-specialised kernel.  Roles (21 warps):
-//   warps 0-3   epilogue: TMEM -> registers -> bias/residual/ReLU -> global (TMEM lane quadrant = warp)
-//   warp  4     MMA issuer (one elected lane), owns TMEM alloc/dealloc and barrier init
-//   warps 5-20  producers, two groups of 8 warps filling alternate k-blocks (two smem stages in flight):
+// Persistent, warp-specialised kernel.  Roles (20 warps):
+//   warps 0-3   consumers: one warpgroup issues wgmma (accumulators in registers), then stages the accumulators
+//               through shared memory and applies bias/residual/ReLU and stores (thread = tile row)
+//   warps 4-19  producers, two groups of 8 warps filling alternate k-blocks (two smem stages in flight):
 //               sample table, B via cp.async, A gather (loads issued first, then bf16 conversion)
-// Pipelines: smem ring full[s]/empty[s] (producers <-> MMA) runs across tiles; two TMEM accumulator
-// buffers tmem_full[b]/tmem_empty[b] (MMA <-> epilogue) overlap tile i's epilogue with tile i+1's
-// main loop.  Tiles: id = blockIdx.x + it*gridDim.x, n-tile fastest (concurrent CTAs share the A rows in L2).
+// Pipeline: smem ring full[s]/empty[s] (producers <-> consumers) runs across tiles, so the producers fill the
+// next tile's stages while the consumers write the previous tile out.
+// Tiles: id = blockIdx.x + it*gridDim.x, n-tile fastest (concurrent CTAs share the A rows in L2).
 // MODE: 0 = dense (Cin % 64 == 0, NHWC), 1 = deformable, 2 = tiny Cin (stem: NCHW fp32 image, K = kh*kw*Cin
 // flattened and zero-padded to a multiple of 64, element-wise gather through a per-k table)
 // XM: activation storage of x -- 0 fp32, 1 bf16, 2 hi/lo bf16 pairs (NHWC with 2*Cin channels; always the 3-MMA split)
-template <int MODE, int XM>
+// BN: N tile (== p.BN), the width of the wgmma instruction and of the register accumulators
+template <int MODE, int XM, int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 igemm_tc_kernel(const TcParams p) {
   constexpr bool XBF16 = XM == 1;
@@ -101,8 +103,6 @@ igemm_tc_kernel(const TcParams p) {
   const bool x3 = p.x3 != 0;
   const TcSmem L = tc_smem_layout(DEFORM, SMALLC ? 2 : KHW, p.BN, p.stages, x3);
   const uint32_t bar_full = base + L.bars, bar_empty = bar_full + 8 * TC_MAX_STAGES;
-  const uint32_t bar_tfull = bar_empty + 8 * TC_MAX_STAGES, bar_tempty = bar_tfull + 16;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(sm + L.bars + 8 * (2 * TC_MAX_STAGES + 4));
   long long* rowbase = reinterpret_cast<long long*>(sm + L.rowbase);
   float4* tw = reinterpret_cast<float4*>(sm + L.table);
   int4* to = reinterpret_cast<int4*>(sm + L.table + (DEFORM ? KHW * TC_BM * 16 : 0));
@@ -137,24 +137,14 @@ igemm_tc_kernel(const TcParams p) {
     const long long pg = mt * TC_BM + r;
     return pg < Ptot ? pg : -1ll;
   };
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < 2 * p.BN) tmem_cols <<= 1;
 
   // ---------------- one-time setup ----------------
-  if (warp == TC_EPILOGUE / 32) {
-    if (lane == 0) {
-      for (int s = 0; s < p.stages; ++s) {
-        mbar_init(bar_full + 8 * s, TC_GROUP / 32);
-        mbar_init(bar_empty + 8 * s, 1);
-      }
-      for (int b = 0; b < 2; ++b) {
-        mbar_init(bar_tfull + 8 * b, 1);
-        mbar_init(bar_tempty + 8 * b, TC_EPILOGUE / 32);   // one arrive per epilogue warp
-      }
-      fence_mbar_init();
+  if (tid == 0) {
+    for (int s = 0; s < p.stages; ++s) {
+      mbar_init(bar_full + 8 * s, TC_GROUP / 32);
+      mbar_init(bar_empty + 8 * s, TC_CONSUMERS / 32);   // one arrive per consumer warp
     }
-    __syncwarp();
-    tmem_alloc(smem_u32(tmem_ptr_smem), tmem_cols);
+    fence_mbar_init();
   }
   if (SMALLC) {   // per-k table: k -> (dy, dx, channel) packed, -1 for the zero padding of K
     for (int k = tid; k < Kp; k += TC_THREADS) {
@@ -167,14 +157,11 @@ igemm_tc_kernel(const TcParams p) {
       ti[k] = v;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp > TC_EPILOGUE / 32) {
+  if (warp >= TC_CONSUMERS / 32) {
     // =============================== PRODUCERS ===============================
-    const int pt = tid - (TC_EPILOGUE + 32);  // 0..511
+    const int pt = tid - TC_CONSUMERS;    // 0..511
     const int group = pt / TC_GROUP;      // which alternate k-blocks this thread fills
     const int gt = pt - group * TC_GROUP; // 0..255 inside the group
     const int j = gt & 7;                 // 16-byte chunk (8 channels) inside the 128-byte row
@@ -333,8 +320,8 @@ igemm_tc_kernel(const TcParams p) {
           }
         } else if (DEFORM && XPAIR) {
           // deformable, hi/lo pair activations: 8 lanes x 16 B cover a row's 64 channels of one plane; per corner one hi and
-          // one lo load.  The gather is ISSUE-bound (ncu: 2.4 IPC, tensor pipe 18 %), so the blend is written for instruction
-          // count: hi plane = packed fp32x2 FMAs (FFMA2: two channels per instruction, exact fp32 products of the bf16 values),
+          // one lo load.  The gather is issue-bound, so the blend is written for instruction count: hi plane = fp32 FMAs on
+          // channel pairs (exact fp32 products of the bf16 values),
           // lo plane = packed bf16x2 HFMA2 with bf16-rounded weights (the lo plane is 2^-9 of the value, its blend only needs
           // 2^-9 relative accuracy -> 2^-18 overall); the two sums are added in fp32 and the result is split again.
           const __nv_bfloat16* xh = reinterpret_cast<const __nv_bfloat16*>(p.x);
@@ -364,7 +351,7 @@ igemm_tc_kernel(const TcParams p) {
                 for (int q = 0; q < 4; ++q) {
                   unsigned long long hp;
                   asm("mov.b64 %0, {%1, %2};" : "=l"(hp) : "r"(H[i][q] << 16), "r"(H[i][q] & 0xffff0000u));
-                  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(acc[q]) : "l"(wp), "l"(hp), "l"(acc[q]));
+                  acc[q] = f32x2_fma(wp, hp, acc[q]);
                   const __nv_bfloat162 lv = *reinterpret_cast<const __nv_bfloat162*>(&Lo[i][q]);
                   lacc[q] = i == 0 ? __hmul2(wb, lv) : __hfma2(wb, lv, lacc[q]);
                 }
@@ -374,7 +361,7 @@ igemm_tc_kernel(const TcParams p) {
                 const uint32_t lw = *reinterpret_cast<const uint32_t*>(&lacc[q]);
                 unsigned long long lp;
                 asm("mov.b64 %0, {%1, %2};" : "=l"(lp) : "r"(lw << 16), "r"(lw & 0xffff0000u));
-                asm("add.rn.f32x2 %0, %1, %2;" : "=l"(acc[q]) : "l"(acc[q]), "l"(lp));
+                acc[q] = f32x2_add(acc[q], lp);
               }
             }
             const uint32_t soff = (uint32_t)r * 128u + (uint32_t)((j ^ (r & 7)) << 4);
@@ -441,8 +428,8 @@ igemm_tc_kernel(const TcParams p) {
           // deformable, bf16 activations: 4 lanes x 32 B cover a row's 64 channels (two 16-byte loads per corner,
           // one address computation); the four corners are blended in packed bf16x2 (HFMA2.BF16: 4 ops per 8
           // channels and corner pair instead of 8 unpack + 8 FMA + pack) with the tile's sample table, whose
-          // weights are stored as replicated bf16 pairs.  This kernel is issue-bound (ncu: 2.3 IPC, L2 16 %), so
-          // instructions per gathered element are what matters.
+          // weights are stored as replicated bf16 pairs.  This kernel is issue-bound, so instructions per gathered
+          // element are what matters.
           const __nv_bfloat16* xh = reinterpret_cast<const __nv_bfloat16*>(p.x);
           const int j2 = gt & 3, rr0 = gt >> 2;              // 64 rows per pass
           const int cp0 = c0 - j * 8 + j2 * 16;              // first channel of this lane's 16-channel slice
@@ -456,7 +443,7 @@ igemm_tc_kernel(const TcParams p) {
               const __nv_bfloat16* xb = xh + rb + cp0;
               const uint4 wv = twp[tap * TC_BM + r];
               const int4 ov = to[tap * TC_BM + r];
-              // one 256-bit load per corner (LDG.E.256): 4 lanes cover a row's full 128-byte line, so the L1
+              // 32 bytes per corner (two 16-byte loads): 4 lanes cover a row's full 128-byte line, so the L1
               // wavefront count stays that of the 8-lane x 16-byte mapping while the address work is halved
               uint4 a0, a1, b0, b1, d0, d1, e0, e1;
               ldg256(xb + ov.x, a0, a1);
@@ -533,80 +520,86 @@ igemm_tc_kernel(const TcParams p) {
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_full + 8 * pend_s);
     }
-  } else if (warp == TC_EPILOGUE / 32) {
-    // =============================== MMA ISSUER ===============================
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc(TC_BM, p.BN);
-      // descriptors: constant high word (SBO 1024 B, version 1, SWIZZLE_128B) + running low word (address >> 4);
-      // ring position / phase are running counters (no division on this single thread's per-k-block path)
-      const uint32_t desc_hi = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);
-      const uint32_t a_lo0 = ((base + L.stages) >> 4) & 0x3fffu, stage16 = L.stage_bytes >> 4;
-      const uint32_t a16 = L.a_bytes >> 4, b16 = L.b_bytes >> 4;
-      uint32_t s = 0, ph = 0, a_hi = a_lo0, ti_local = 0;
-      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++ti_local) {
-        const uint32_t buf = ti_local & 1u, use = ti_local >> 1;
-        mbar_wait(bar_tempty + 8 * buf, (use & 1u) ^ 1u);   // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + buf * (uint32_t)p.BN;
-        uint32_t acc = 0u;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(bar_full + 8 * s, ph);
-          tc_fence_after();
-          const uint32_t b_hi = a_hi + a16, a_lo = b_hi + b16, b_lo = a_lo + a16;
-#pragma unroll
-          for (uint32_t k = 0; k < TC_BK / 16; ++k) {       // 16 bf16 = 32 bytes = 2 descriptor units
-            if (x3) {
-              umma_bf16_lohi(tmem_d, a_lo + 2 * k, b_hi + 2 * k, desc_hi, idesc, acc);
-              umma_bf16_lohi(tmem_d, a_hi + 2 * k, b_lo + 2 * k, desc_hi, idesc, 1u);
-              umma_bf16_lohi(tmem_d, a_hi + 2 * k, b_hi + 2 * k, desc_hi, idesc, 1u);
-            } else {
-              umma_bf16_lohi(tmem_d, a_hi + 2 * k, b_hi + 2 * k, desc_hi, idesc, acc);
-            }
-            acc = 1u;
-          }
-          umma_commit(bar_empty + 8 * s);   // frees the stage once the MMAs above have read it
-          a_hi += stage16;
-          if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1u; a_hi = a_lo0; }
-        }
-        umma_commit(bar_tfull + 8 * buf);   // accumulator complete -> epilogue
-      }
-    }
-    __syncwarp();
   } else {
-    // =============================== EPILOGUE (warps 0-3) ===============================
-    const int q = warp & 3;        // TMEM lane quadrant
-    const int half = warp >> 2;    // which slice of the BN accumulator columns (TC_EPI_SPLIT slices)
+    // =============================== CONSUMERS (warps 0-3) ===============================
+    const uint32_t dhi = wg_desc_hi(1024);          // 8-row groups of 128-byte rows
     const bool vec_ptrs_ok = (((uintptr_t)p.y) & 15) == 0 && (!p.residual || (((uintptr_t)p.residual) & 15) == 0);
-    uint32_t ti_local = 0;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++ti_local) {
+    float* stf = reinterpret_cast<float*>(sm + L.epi);
+    float d0[BN / 2], d1[BN / 2];                   // tile rows [0, 64) and [64, 128)
+    uint32_t s = 0, ph = 0;
+    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const long long mt = tile / n_tiles;
-      const int n0 = (int)(tile % n_tiles) * p.BN;
-      const uint32_t buf = ti_local & 1u, use = ti_local >> 1;
-      mbar_wait(bar_tfull + 8 * buf, use & 1u);
-      tc_fence_after();
+      const int n0 = (int)(tile % n_tiles) * BN;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(bar_full + 8 * s, ph);
+        const uint32_t st0 = base + L.stages + s * L.stage_bytes;
+        const uint32_t a_hi = wg_desc_lo(st0), b_hi = wg_desc_lo(st0 + L.a_bytes);
+        const uint32_t a_lo = wg_desc_lo(st0 + L.a_bytes + L.b_bytes), b_lo = wg_desc_lo(st0 + 2 * L.a_bytes + L.b_bytes);
+        constexpr uint32_t h16 = 64u * 128u / 16u;      // rows 64-127: 64 rows of 128 bytes further
+        wgmma_fence();
+#pragma unroll
+        for (uint32_t k = 0; k < TC_BK / 16; ++k) {       // 16 bf16 = 32 bytes = 2 descriptor units
+          const uint32_t acc = (kb | k) ? 1u : 0u;
+          const uint64_t bh = wg_desc(b_hi + 2 * k, dhi);
+          if (x3) {
+            const uint64_t bl = wg_desc(b_lo + 2 * k, dhi);
+            Wgmma<BN>::mma(d0, wg_desc(a_lo + 2 * k, dhi), bh, acc);
+            Wgmma<BN>::mma(d1, wg_desc(a_lo + h16 + 2 * k, dhi), bh, acc);
+            Wgmma<BN>::mma(d0, wg_desc(a_hi + 2 * k, dhi), bl, 1u);
+            Wgmma<BN>::mma(d1, wg_desc(a_hi + h16 + 2 * k, dhi), bl, 1u);
+            Wgmma<BN>::mma(d0, wg_desc(a_hi + 2 * k, dhi), bh, 1u);
+            Wgmma<BN>::mma(d1, wg_desc(a_hi + h16 + 2 * k, dhi), bh, 1u);
+          } else {
+            Wgmma<BN>::mma(d0, wg_desc(a_hi + 2 * k, dhi), bh, acc);
+            Wgmma<BN>::mma(d1, wg_desc(a_hi + h16 + 2 * k, dhi), bh, acc);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                // the previous k-block's wgmmas have read their stage
+        wgmma_fence_acc(d0);
+        wgmma_fence_acc(d1);
+        if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+        prev = (int)s;
+        if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1u; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(d0);
+      wgmma_fence_acc(d1);
+      if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+
+      // ---- epilogue: 32 accumulator columns at a time through shared memory, thread = tile row ----
+      const int q = warp;
       const int m = q * 32 + lane;
       const long long pg = tile_pixel(mt, m);
       const bool row_ok = pg >= 0;
       const int n_img = row_ok ? (int)(pg / HoWo) : 0;
       const int pp = row_ok ? (int)(pg - (long long)n_img * HoWo) : 0;
-      const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + buf * (uint32_t)p.BN;
-      if (p.out_nhwc && (p.Cout & 7) == 0 && vec_ptrs_ok) {
-        // ---- NHWC: stage 32 rows x 32 columns (fp32, +bias) per warp in shared memory, then write them out
-        //      row-wise: 4 (bf16) or 8 (fp32) lanes cover one row's 64 / 128 contiguous bytes, so every store
-        //      -- and every residual read -- is made of fully used 32-byte sectors instead of one 16-byte
-        //      fragment per 512-byte-strided row. ----
-        float* st = reinterpret_cast<float*>(sm + L.epi) + (size_t)warp * 32 * TC_EPI_PITCH;
-        const bool y16 = p.y_bf16 || p.y_pair;          // 16-bit storage: 8 columns (16 B) per lane
-        const size_t ypitch = p.y_pair ? 2 * (size_t)p.Cout : (size_t)p.Cout;   // elements per stored pixel
-        const int lpr = y16 ? 4 : 8;                    // lanes per row in the write-out phase
-        const int rpi = 32 / lpr;                       // rows per iteration
-        const int sub = lane % lpr, rsub = lane / lpr;
-        for (int cb = 0; cb < p.BN; cb += 32) {
-          if (n0 + cb >= p.Cout) break;                 // zero-padded weight rows beyond Cout
+      const uint32_t trow = smem_u32(stf + (size_t)m * TC_EPI_PITCH);
+      for (int cb = 0; cb < BN; cb += 32) {
+        if (n0 + cb >= p.Cout) break;                   // zero-padded weight rows beyond Cout (CTA-uniform)
+        named_bar(2, TC_CONSUMERS);                     // the previous chunk has been read
+#pragma unroll
+        for (int c = 0; c < BN; c += 32)
+          if (c == cb) {
+            acc_stage<BN, 32>(d0, stf, TC_EPI_PITCH, 0, c);
+            acc_stage<BN, 32>(d1, stf, TC_EPI_PITCH, 64, c);
+          }
+        named_bar(2, TC_CONSUMERS);
+        if (p.out_nhwc && (p.Cout & 7) == 0 && vec_ptrs_ok) {
+          // ---- NHWC: this warp's 32 staged rows x 32 columns (+bias, in place) are written out row-wise: 4 (bf16) or
+          //      8 (fp32) lanes cover one row's 64 / 128 contiguous bytes, so every store -- and every residual read -- is
+          //      made of fully used 32-byte sectors instead of one 16-byte fragment per 512-byte-strided row. ----
+          float* st = stf + (size_t)q * 32 * TC_EPI_PITCH;
+          const bool y16 = p.y_bf16 || p.y_pair;          // 16-bit storage: 8 columns (16 B) per lane
+          const size_t ypitch = p.y_pair ? 2 * (size_t)p.Cout : (size_t)p.Cout;   // elements per stored pixel
+          const int lpr = y16 ? 4 : 8;                    // lanes per row in the write-out phase
+          const int rpi = 32 / lpr;                       // rows per iteration
+          const int sub = lane % lpr, rsub = lane / lpr;
 #pragma unroll
           for (int c = 0; c < 2; ++c) {
             uint32_t rr[16];
-            tmem_ld16(trow + (uint32_t)(cb + c * 16), rr);   // warp-collective
+            acc_ld16(trow + (uint32_t)(c * 16) * 4u, rr);
             const int co0 = n0 + cb + c * 16;
             float4* dst = reinterpret_cast<float4*>(st + lane * TC_EPI_PITCH + c * 16);
 #pragma unroll
@@ -693,126 +686,113 @@ igemm_tc_kernel(const TcParams p) {
               }
             }
           }
-          __syncwarp();
+          continue;
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_tempty + 8 * buf);
-        continue;
-      }
-      // ---- legacy per-lane path (NCHW outputs, odd channel counts) ----
-      for (int col = 0; col < p.BN; col += 16) {
-        uint32_t rr[16];
-        tmem_ld16(trow + (uint32_t)col, rr);  // warp-collective
-        if (!row_ok) continue;
-        const int co0 = n0 + col;
-        if (co0 >= p.Cout) continue;
-        float o16[16];
+        // ---- per-lane path (NCHW outputs, odd channel counts) ----
+        for (int col = cb; col < cb + 32; col += 16) {
+          uint32_t rr[16];
+          acc_ld16(trow + (uint32_t)(col - cb) * 4u, rr);
+          if (!row_ok) continue;
+          const int co0 = n0 + col;
+          if (co0 >= p.Cout) continue;
+          float o16[16];
 #pragma unroll
-        for (int e = 0; e < 16; ++e) o16[e] = __uint_as_float(rr[e]);
-        if (p.bias) {
+          for (int e = 0; e < 16; ++e) o16[e] = __uint_as_float(rr[e]);
+          if (p.bias) {
 #pragma unroll
-          for (int e = 0; e < 16; ++e) if (co0 + e < p.Cout) o16[e] += __ldg(p.bias + co0 + e);
-        }
-        if (p.out_nhwc) {
-          const size_t oidx = (size_t)pg * p.Cout + co0;
-          // FPN top-down path (models/fpn.py:88-93): lateral conv + nearest-2x-upsampled coarser map, fused:
-          // the residual is indexed at (ho/2, wo/2) of the half-resolution tensor instead of being materialised.
-          size_t ridx = oidx;
-          if (p.res_up2) {
-            const int ho = pp / p.Wo, wo = pp - ho * p.Wo;
-            ridx = (((size_t)n_img * (p.Ho >> 1) + (ho >> 1)) * (p.Wo >> 1) + (wo >> 1)) * p.Cout + co0;
+            for (int e = 0; e < 16; ++e) if (co0 + e < p.Cout) o16[e] += __ldg(p.bias + co0 + e);
           }
-          const bool full = (co0 + 15 < p.Cout) && ((p.Cout & 7) == 0) && vec_ptrs_ok;
-          if (p.y_bf16) {
-            __nv_bfloat16* yo = reinterpret_cast<__nv_bfloat16*>(p.y) + oidx;
-            const __nv_bfloat16* ro = p.residual ? reinterpret_cast<const __nv_bfloat16*>(p.residual) + ridx : nullptr;
-            if (full) {
-              if (ro) {
-                const uint4 r0 = __ldg(reinterpret_cast<const uint4*>(ro)), r1 = __ldg(reinterpret_cast<const uint4*>(ro) + 1);
-                const uint32_t rw[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                  o16[2 * q] += __uint_as_float(rw[q] << 16);
-                  o16[2 * q + 1] += __uint_as_float(rw[q] & 0xffff0000u);
-                }
-              }
-              if (p.relu) {
-#pragma unroll
-                for (int e = 0; e < 16; ++e) o16[e] = fmaxf(o16[e], 0.f);
-              }
-              uint4 w0, w1;
-              w0.x = pack_bf16x2(o16[0], o16[1]); w0.y = pack_bf16x2(o16[2], o16[3]);
-              w0.z = pack_bf16x2(o16[4], o16[5]); w0.w = pack_bf16x2(o16[6], o16[7]);
-              w1.x = pack_bf16x2(o16[8], o16[9]); w1.y = pack_bf16x2(o16[10], o16[11]);
-              w1.z = pack_bf16x2(o16[12], o16[13]); w1.w = pack_bf16x2(o16[14], o16[15]);
-              reinterpret_cast<uint4*>(yo)[0] = w0;
-              reinterpret_cast<uint4*>(yo)[1] = w1;
-            } else {
-#pragma unroll
-              for (int e = 0; e < 16; ++e) {
-                if (co0 + e >= p.Cout) break;
-                float o = o16[e];
-                if (ro) o += __bfloat162float(ro[e]);
-                if (p.relu) o = fmaxf(o, 0.f);
-                yo[e] = __float2bfloat16_rn(o);
-              }
+          if (p.out_nhwc) {
+            const size_t oidx = (size_t)pg * p.Cout + co0;
+            // FPN top-down path (models/fpn.py:88-93): lateral conv + nearest-2x-upsampled coarser map, fused:
+            // the residual is indexed at (ho/2, wo/2) of the half-resolution tensor instead of being materialised.
+            size_t ridx = oidx;
+            if (p.res_up2) {
+              const int ho = pp / p.Wo, wo = pp - ho * p.Wo;
+              ridx = (((size_t)n_img * (p.Ho >> 1) + (ho >> 1)) * (p.Wo >> 1) + (wo >> 1)) * p.Cout + co0;
             }
-          } else {
-            float* yo = reinterpret_cast<float*>(p.y) + oidx;
-            const float* ro = p.residual ? reinterpret_cast<const float*>(p.residual) + ridx : nullptr;
-            if (full) {
-#pragma unroll
-              for (int g4 = 0; g4 < 4; ++g4) {
-                float4 o = make_float4(o16[g4 * 4], o16[g4 * 4 + 1], o16[g4 * 4 + 2], o16[g4 * 4 + 3]);
-                if (ro) {
-                  const float4 rv = __ldg(reinterpret_cast<const float4*>(ro + g4 * 4));
-                  o.x += rv.x; o.y += rv.y; o.z += rv.z; o.w += rv.w;
-                }
-                if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                *reinterpret_cast<float4*>(yo + g4 * 4) = o;
-              }
-            } else {
-#pragma unroll
-              for (int e = 0; e < 16; ++e) {
-                if (co0 + e >= p.Cout) break;
-                float o = o16[e];
-                if (ro) o += __ldg(ro + e);
-                if (p.relu) o = fmaxf(o, 0.f);
-                yo[e] = o;
-              }
-            }
-          }
-        } else {  // NCHW: for a fixed cout the 32 lanes of a warp write 32 consecutive pixels
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const int co = co0 + e;
-            if (co >= p.Cout) break;
-            const size_t oidx = ((size_t)n_img * p.Cout + co) * HoWo + pp;
-            float o = o16[e];
+            const bool full = (co0 + 15 < p.Cout) && ((p.Cout & 7) == 0) && vec_ptrs_ok;
             if (p.y_bf16) {
-              if (p.residual) o += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[oidx]);
-              if (p.relu) o = fmaxf(o, 0.f);
-              reinterpret_cast<__nv_bfloat16*>(p.y)[oidx] = __float2bfloat16_rn(o);
+              __nv_bfloat16* yo = reinterpret_cast<__nv_bfloat16*>(p.y) + oidx;
+              const __nv_bfloat16* ro = p.residual ? reinterpret_cast<const __nv_bfloat16*>(p.residual) + ridx : nullptr;
+              if (full) {
+                if (ro) {
+                  const uint4 r0 = __ldg(reinterpret_cast<const uint4*>(ro)), r1 = __ldg(reinterpret_cast<const uint4*>(ro) + 1);
+                  const uint32_t rw[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+#pragma unroll
+                  for (int q = 0; q < 8; ++q) {
+                    o16[2 * q] += __uint_as_float(rw[q] << 16);
+                    o16[2 * q + 1] += __uint_as_float(rw[q] & 0xffff0000u);
+                  }
+                }
+                if (p.relu) {
+#pragma unroll
+                  for (int e = 0; e < 16; ++e) o16[e] = fmaxf(o16[e], 0.f);
+                }
+                uint4 w0, w1;
+                w0.x = pack_bf16x2(o16[0], o16[1]); w0.y = pack_bf16x2(o16[2], o16[3]);
+                w0.z = pack_bf16x2(o16[4], o16[5]); w0.w = pack_bf16x2(o16[6], o16[7]);
+                w1.x = pack_bf16x2(o16[8], o16[9]); w1.y = pack_bf16x2(o16[10], o16[11]);
+                w1.z = pack_bf16x2(o16[12], o16[13]); w1.w = pack_bf16x2(o16[14], o16[15]);
+                reinterpret_cast<uint4*>(yo)[0] = w0;
+                reinterpret_cast<uint4*>(yo)[1] = w1;
+              } else {
+#pragma unroll
+                for (int e = 0; e < 16; ++e) {
+                  if (co0 + e >= p.Cout) break;
+                  float o = o16[e];
+                  if (ro) o += __bfloat162float(ro[e]);
+                  if (p.relu) o = fmaxf(o, 0.f);
+                  yo[e] = __float2bfloat16_rn(o);
+                }
+              }
             } else {
-              if (p.residual) o += __ldg(reinterpret_cast<const float*>(p.residual) + oidx);
-              if (p.relu) o = fmaxf(o, 0.f);
-              if (p.sig_from >= 0 && co >= p.sig_from) o = 1.f / (1.f + expf(-o));
-              reinterpret_cast<float*>(p.y)[oidx] = o;
+              float* yo = reinterpret_cast<float*>(p.y) + oidx;
+              const float* ro = p.residual ? reinterpret_cast<const float*>(p.residual) + ridx : nullptr;
+              if (full) {
+#pragma unroll
+                for (int g4 = 0; g4 < 4; ++g4) {
+                  float4 o = make_float4(o16[g4 * 4], o16[g4 * 4 + 1], o16[g4 * 4 + 2], o16[g4 * 4 + 3]);
+                  if (ro) {
+                    const float4 rv = __ldg(reinterpret_cast<const float4*>(ro + g4 * 4));
+                    o.x += rv.x; o.y += rv.y; o.z += rv.z; o.w += rv.w;
+                  }
+                  if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+                  *reinterpret_cast<float4*>(yo + g4 * 4) = o;
+                }
+              } else {
+#pragma unroll
+                for (int e = 0; e < 16; ++e) {
+                  if (co0 + e >= p.Cout) break;
+                  float o = o16[e];
+                  if (ro) o += __ldg(ro + e);
+                  if (p.relu) o = fmaxf(o, 0.f);
+                  yo[e] = o;
+                }
+              }
+            }
+          } else {  // NCHW: for a fixed cout the 32 lanes of a warp write 32 consecutive pixels
+#pragma unroll
+            for (int e = 0; e < 16; ++e) {
+              const int co = co0 + e;
+              if (co >= p.Cout) break;
+              const size_t oidx = ((size_t)n_img * p.Cout + co) * HoWo + pp;
+              float o = o16[e];
+              if (p.y_bf16) {
+                if (p.residual) o += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[oidx]);
+                if (p.relu) o = fmaxf(o, 0.f);
+                reinterpret_cast<__nv_bfloat16*>(p.y)[oidx] = __float2bfloat16_rn(o);
+              } else {
+                if (p.residual) o += __ldg(reinterpret_cast<const float*>(p.residual) + oidx);
+                if (p.relu) o = fmaxf(o, 0.f);
+                if (p.sig_from >= 0 && co >= p.sig_from) o = 1.f / (1.f + expf(-o));
+                reinterpret_cast<float*>(p.y)[oidx] = o;
+              }
             }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * buf);   // accumulator buffer may be overwritten
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == TC_EPILOGUE / 32) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
   }
 }
 
@@ -858,6 +838,35 @@ bool tc_supported(int Cin, int kh, int kw, int dg) {
   return ((Cin % TC_BK) == 0 || Cin <= 8) && dg == 1 && kh * kw <= 49 && kh <= 15 && kw <= 15;
 }
 
+template <int BN>
+static cudaError_t tc_configure() {
+  const void* k[] = {(const void*)igemm_tc_kernel<0, 0, BN>, (const void*)igemm_tc_kernel<0, 1, BN>, (const void*)igemm_tc_kernel<0, 2, BN>,
+                     (const void*)igemm_tc_kernel<1, 0, BN>, (const void*)igemm_tc_kernel<1, 1, BN>, (const void*)igemm_tc_kernel<1, 2, BN>,
+                     (const void*)igemm_tc_kernel<2, 0, BN>};
+  for (const void* f : k) {
+    const cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+  }
+  // deformable instantiations: prefer the smallest shared-memory carve-out that fits, the rest of the 256 KB is L1
+  for (int i = 3; i < 6; ++i) (void)cudaFuncSetAttribute(k[i], cudaFuncAttributePreferredSharedMemoryCarveout, 60);
+  return cudaSuccess;
+}
+
+template <int BN>
+static void tc_launch(const TcParams& p, bool deform, bool smallc, dim3 grid, size_t smem, cudaStream_t stream) {
+  if (smallc) igemm_tc_kernel<2, 0, BN><<<grid, TC_THREADS, smem, stream>>>(p);
+  else if (p.x_pair) {
+    if (deform) igemm_tc_kernel<1, 2, BN><<<grid, TC_THREADS, smem, stream>>>(p);
+    else igemm_tc_kernel<0, 2, BN><<<grid, TC_THREADS, smem, stream>>>(p);
+  } else if (p.x_bf16) {
+    if (deform) igemm_tc_kernel<1, 1, BN><<<grid, TC_THREADS, smem, stream>>>(p);
+    else igemm_tc_kernel<0, 1, BN><<<grid, TC_THREADS, smem, stream>>>(p);
+  } else {
+    if (deform) igemm_tc_kernel<1, 0, BN><<<grid, TC_THREADS, smem, stream>>>(p);
+    else igemm_tc_kernel<0, 0, BN><<<grid, TC_THREADS, smem, stream>>>(p);
+  }
+}
+
 int launch_igemm_tc(TcParams p, const void* packed, cudaStream_t stream) {
   const int KHW = p.kh * p.kw;
   if (!tc_supported(p.Cin, p.kh, p.kw, 1)) return UPSNET_E_UNSUPPORTED;
@@ -875,15 +884,16 @@ int launch_igemm_tc(TcParams p, const void* packed, cudaStream_t stream) {
   if (smallc && (deform || p.x_bf16 || p.x_pair || p.dh * (p.kh - 1) > 255 || p.dw * (p.kw - 1) > 255)) return UPSNET_E_UNSUPPORTED;
   if (p.x_pair && !p.x3) return UPSNET_E_UNSUPPORTED;          // pairs are the storage format of precision bf16x3
   if (p.sig_from >= 0 && (p.out_nhwc || p.y_bf16)) return UPSNET_E_UNSUPPORTED;   // sigmoid lives in the fp32 NCHW per-lane epilogue
+  if (p.x_bf16 && !p.x_pair && p.x3) return UPSNET_E_UNSUPPORTED;   // the hi/lo split needs fp32 or pair activations
   if (p.y_pair) {
     // pair output: the staged NHWC epilogue only (16-byte vectors), plain [hi Cout][lo Cout] grouping
     if (!p.out_nhwc || (p.Cout & 7) || (p.pair_group && p.pair_group != p.Cout)) return UPSNET_E_UNSUPPORTED;
     if (p.residual && (((uintptr_t)p.residual) & 15)) return UPSNET_E_UNSUPPORTED;
   }
-  // tile N: as wide as possible (each gathered A tile is reused by BN couts)
-  int BN = p.Cout_pad;
-  const int bn_cap = p.x3 ? 128 : 256;
-  if (BN > bn_cap) BN = (p.Cout_pad % bn_cap == 0) ? bn_cap : ((p.Cout_pad % 128 == 0) ? 128 : 64);
+  // tile N: as wide as the register file allows (each gathered A tile is reused by BN couts).  20 warps leave 96 registers
+  // per thread (ptxas -v: 96 used); the consumer holds two m64nBN fragments = BN floats, so BN = 64 (64 floats next to the
+  // addressing, a few hundred bytes spilled) is the widest that fits -- BN = 128 would need 128 registers for the fragments.
+  int BN = p.Cout_pad > 64 ? 64 : p.Cout_pad;
   {  // few output tiles (FC layers, coarse pyramid levels): narrower N tiles so that every SM gets work
     const long long mt = ((long long)p.N * p.Ho * p.Wo + TC_BM - 1) / TC_BM;
     while (BN > 64 && (BN % 32) == 0 && mt * (p.Cout_pad / BN) < kNumSMs && p.Cout_pad % (BN / 2) == 0 && ((BN / 2) % 32) == 0) BN /= 2;
@@ -891,7 +901,7 @@ int launch_igemm_tc(TcParams p, const void* packed, cudaStream_t stream) {
   p.BN = BN;
   // One persistent CTA per SM: give the smem ring everything that is left after the sample table.
   const int khw_l = smallc ? 2 : KHW;   // table region: [KHW][128] entries, or the 1 KB per-k table of the stem mode
-  // deformable: a short ring leaves ~100 KB of the SM's 256 KB as L1 for the corner gathers (see the producer)
+  // deformable: a short ring leaves ~100 KB of the SM's 256 KB of L1 / shared memory to the corner gathers (see the producer)
   int stages = deform ? 3 : TC_MAX_STAGES;
   TcSmem L = tc_smem_layout(deform, khw_l, BN, stages, p.x3 != 0);
   while (stages > 2 && L.total + 1024 > 220 * 1024) { --stages; L = tc_smem_layout(deform, khw_l, BN, stages, p.x3 != 0); }
@@ -924,34 +934,16 @@ int launch_igemm_tc(TcParams p, const void* packed, cudaStream_t stream) {
     if (extra < 0) { const char* e = getenv("UPSNET_DCN_EXTRA_SMEM_KB"); extra = e ? atoi(e) : 0; }
     if (extra > 0 && smem + (size_t)extra * 1024 <= 227 * 1024) smem += (size_t)extra * 1024;
   }
-  // opt in to the full 227 KB once per process (kept out of the per-launch path: CUDA-graph capture)
   // opt in to the full 227 KB once per device (kept out of the per-launch path: CUDA-graph capture)
   static PerDeviceOnce configured;
   if (configured.need()) {
-    UPS_CUDA(cudaFuncSetAttribute(igemm_tc_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    UPS_CUDA(cudaFuncSetAttribute(igemm_tc_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    UPS_CUDA(cudaFuncSetAttribute(igemm_tc_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    UPS_CUDA(cudaFuncSetAttribute(igemm_tc_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    UPS_CUDA(cudaFuncSetAttribute(igemm_tc_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    UPS_CUDA(cudaFuncSetAttribute(igemm_tc_kernel<0, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    UPS_CUDA(cudaFuncSetAttribute(igemm_tc_kernel<2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    // deformable instantiations: prefer the smallest shared-memory carve-out that fits, the rest of the 256 KB is L1
-    (void)cudaFuncSetAttribute(igemm_tc_kernel<1, 1>, cudaFuncAttributePreferredSharedMemoryCarveout, 60);
-    (void)cudaFuncSetAttribute(igemm_tc_kernel<1, 0>, cudaFuncAttributePreferredSharedMemoryCarveout, 60);
-    (void)cudaFuncSetAttribute(igemm_tc_kernel<1, 2>, cudaFuncAttributePreferredSharedMemoryCarveout, 60);
+    UPS_CUDA(tc_configure<32>());
+    UPS_CUDA(tc_configure<64>());
   }
-  if (smallc) {
-    igemm_tc_kernel<2, 0><<<grid, TC_THREADS, smem, stream>>>(p);
-  } else if (p.x_pair) {
-    if (deform) igemm_tc_kernel<1, 2><<<grid, TC_THREADS, smem, stream>>>(p);
-    else igemm_tc_kernel<0, 2><<<grid, TC_THREADS, smem, stream>>>(p);
-  } else if (p.x_bf16) {
-    if (p.x3) return UPSNET_E_UNSUPPORTED;   // the hi/lo split needs fp32 or pair activations
-    if (deform) igemm_tc_kernel<1, 1><<<grid, TC_THREADS, smem, stream>>>(p);
-    else igemm_tc_kernel<0, 1><<<grid, TC_THREADS, smem, stream>>>(p);
-  } else {
-    if (deform) igemm_tc_kernel<1, 0><<<grid, TC_THREADS, smem, stream>>>(p);
-    else igemm_tc_kernel<0, 0><<<grid, TC_THREADS, smem, stream>>>(p);
+  switch (BN) {
+    case 32: tc_launch<32>(p, deform, smallc, grid, smem, stream); break;
+    case 64: tc_launch<64>(p, deform, smallc, grid, smem, stream); break;
+    default: return UPSNET_E_UNSUPPORTED;
   }
   UPS_CHECK_LAUNCH();
   return 0;

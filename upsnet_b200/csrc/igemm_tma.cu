@@ -1,4 +1,4 @@
-// igemm_tma.cu -- TMA-fed tcgen05 implicit-GEMM convolution for sm_100a (dense, stride 1, bf16 NHWC in / out).
+// igemm_tma.cu -- TMA-fed wgmma implicit-GEMM convolution for sm_90a (dense, stride 1, bf16 NHWC in / out).
 //
 // The layers that dominate the UPSNet backbone / FPN / RPN / mask head / FC path (1x1 and 3x3, stride 1,
 // Cin % 64 == 0, Cout % 64 == 0; reference: models/resnet.py, models/fpn.py, models/rcnn.py) need no gather
@@ -8,13 +8,14 @@
 //
 //   A[<=128 pixels x 64 ch]  cp.async.bulk.tensor.4d  box (64, bw, bh, bn) at (c0, w0 + kj*dw - pw, h0 + ki*dh - ph, n0)
 //   B[BN couts x 64 k]       cp.async.bulk.tensor.2d  box (64, BN) of the packed weights [Cout][tap*Cin + c]
-//   D[128 x BN] fp32 in TMEM (two buffers)  +=  A * B^T     tcgen05.mma kind::f16, one elected thread
-//   epilogue (8 warps, thread = accumulator row): tcgen05.ld -> +bias (+residual slab, TMA-prefetched) -> ReLU
-//            -> bf16 -> SWIZZLE_128B slab in smem -> cp.async.bulk.tensor.4d store (clips the box at the borders)
+//   D[128 x BN] fp32 in registers  +=  A * B^T     wgmma m64nBNk16, two warpgroups (tile rows 0-63 / 64-127)
+//   epilogue (same 8 warps): accumulators -> fp32 staging rows in smem -> thread = accumulator row: +bias (+residual
+//            slab, TMA-prefetched) -> ReLU -> bf16 -> SWIZZLE_128B slab in smem -> cp.async.bulk.tensor.4d store
+//            (clips the box at the borders)
 //
-// Both operands land in the K-major SWIZZLE_128B layout the UMMA descriptors expect (the TMA swizzle mode and
-// the smem descriptor's layout type are the same permutation), so no thread touches the operands: 3 service
-// warps (TMA loads, MMA issue, residual loads) + 8 epilogue warps per persistent CTA, one CTA per SM.
+// Both operands land in the K-major SWIZZLE_128B layout the wgmma descriptors expect (the TMA swizzle mode and
+// the smem descriptor's layout type are the same permutation), so no thread touches the operands: 2 service
+// warps (TMA loads, residual loads) + 8 consumer warps per persistent CTA, one CTA per SM.
 // Roofline: tensor pipe for the 3x3 layers (2*P*Cout*Cin*9 flop), HBM for the 1x1 (+residual) layers
 // (x + residual + y bytes); per-SM L2->smem operand traffic is (128 + BN) * 128 B per k-block.
 #include <cuda.h>   // CUtensorMap + enums only; the encoder is resolved at run time (no libcuda link dependency)
@@ -27,11 +28,12 @@
 
 namespace ups {
 
-constexpr int TM_EPI_WARPS = 8;
-constexpr int TM_WARP_TMA = 8, TM_WARP_MMA = 9, TM_WARP_RES = 10;
-constexpr int TM_THREADS = 11 * 32;
+constexpr int TM_EPI_WARPS = 8;                 // consumers: two wgmma warpgroups, then the epilogue
+constexpr int TM_WARP_TMA = 8, TM_WARP_RES = 9;
+constexpr int TM_THREADS = 10 * 32;
 constexpr int TM_MAX_STAGES = 8;
 constexpr int TM_SLAB_BYTES = 128 * 128;   // 128 rows x 64 bf16
+constexpr int TM_MMA_BF16 = 0, TM_MMA_WIDE = 1;   // bf16 stream: hi*hi | pair stream: hi*[hi;lo] + lo*hi
 
 struct TmaGeom {
   const float* bias;
@@ -45,13 +47,7 @@ struct TmaGeom {
   int direct, y_bf16, out_nhwc;
   void* y;
   int stem;                             // stride-2 tiny-Cin stem: A boxes come from the packed / padded image (5-D map)
-  // halo mode (k x k, stride 1): one (16 x PH)-pixel input PATCH per (tile, channel chunk) feeds all taps -- the A operand
-  // of tap (ky, kx) is the patch seen through a descriptor that starts (ky*dh*16 + kx*dw) rows further (tile = 8 x 16 px)
-  int halo, patch_rows, pstages, kh;
-  int rotate;                           // tile-dependent start of the K loop (see producer)
-  int wres, wtiles;                     // halo mode with the n-tile's whole weight set (wtiles tiles) resident in smem, loaded once per CTA
   int sig_from;                         // direct epilogue: channels >= sig_from get a logistic sigmoid (-1 = none)
-  int dbg;                              // timing experiments only (UPSNET_TMA_DEBUG): 1 alternate accumulators, 2 one MMA per k-block, 3 no MMAs
   // PAIR mode (precision bf16x3 on the TMA kernel): activations are hi/lo bf16 PAIRS -- an NHWC tensor with 2*C channels,
   // channels [0,C) = bf16(x), [C,2C) = bf16(x - hi) -- weights are the packed hi/lo planes, every k-slice issues three
   // MMAs (lo*hi, hi*lo, hi*hi) and the epilogue splits the fp32 result into a pair again.
@@ -61,11 +57,9 @@ struct TmaGeom {
   int pg;                               // output / residual pair group G: channels stored [hi G][lo G] per group (G = Cout normally)
   int res_inplace;                      // residual slabs are TMA-loaded into the (double-buffered) output slabs and updated in place
   int opairs;                           // output slab pairs that alternate (2, or 1 when shared memory is short)
-  // 2-CTA kernel, N tile <= 64: the hi*hi and hi*lo products share ONE instruction -- B operand = [W_hi ; W_lo] (N = 2 BN, CTA 0
-  // stages the hi rows, CTA 1 the lo rows), accumulated in columns [0, 2 BN); lo*hi goes to columns [0, BN); the epilogue adds
-  // the two column groups.  A tcgen05.mma of M = 256 takes ~100 cycles whatever N <= 128 is (measured: the 18-channel offset
-  // convs and the 64->64 3x3 convs run at 12 instructions x ~100 cycles per k-block), so two instructions per K slice instead
-  // of three is a third less time on these instruction-bound layers.
+  // pair mode (N tile <= 64): the hi*hi and hi*lo products share ONE instruction -- B operand = the contiguous [W_hi ; W_lo]
+  // tile of the stage (N = 2 BN), accumulated in columns [0, 2 BN); lo*hi goes to columns [0, BN); the consumers add the two
+  // column groups in registers before the accumulators are staged.  Two wgmma per K slice instead of three.
   int wide;
 };
 
@@ -103,36 +97,49 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) {
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void sts128(uint32_t addr, const uint4& v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-
 // pair tensors: channel coordinate of channel n's hi value when channels are stored [hi G][lo G] per group of G (lo = +G)
 __device__ __forceinline__ int pair_chan(int n, int G) { return (n / G) * 2 * G + (n % G); }
 
 struct TmaSmem {
-  uint32_t stages, out, res, a_bytes, b_bytes, stage_bytes, total;
-  uint32_t patch, patch_bytes;                               // halo mode: patch ring in front of a B-only ring
-  uint32_t a_half, b_half, patch_half;                       // pair mode: offset of the lo tile inside an A / B / patch slot
+  uint32_t stages, out, res, acc, a_bytes, b_bytes, stage_bytes, total;
+  uint32_t a_half, b_half;                                   // pair mode: offset of the lo tile inside an A / B slot
   uint32_t oslabs, res_slab;                                 // pair mode: number of (hi, lo) output slab pairs; bytes per residual slab
 };
-__host__ __device__ inline TmaSmem tma_smem_layout(int BN, int stages, bool has_res, int patch_rows = 0, int pstages = 0,
-                                                  bool direct = false, bool x3 = false, bool res_up2 = false,
-                                                  bool res_inplace = false, int opairs = 2) {
+// Accumulator staging: 128 rows of BN fp32 (wide mode adds its two column groups in registers first), no padding -- the
+// 16-byte chunk j of row r sits at chunk j ^ (r & 7), so the row-per-lane reads of the epilogue are conflict-free.
+template <int N, int W>   // fragment of m64nN, columns [0, W) staged
+__device__ __forceinline__ void acc_stage_sw(const float (&d)[N / 2], float* buf, int row0) {
+  const int t = threadIdx.x & 127, l = t & 31;
+  const int r = row0 + 16 * (t >> 5) + (l >> 2);
+#pragma unroll
+  for (int i = 0; i < W / 8; ++i) {
+    const int c = 8 * i + 2 * (l & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int rr = r + 8 * h;
+      const int pc = ((((c >> 2) ^ (rr & 7))) << 2) | (c & 3);
+      *reinterpret_cast<float2*>(buf + (size_t)rr * W + pc) = make_float2(d[4 * i + 2 * h], d[4 * i + 2 * h + 1]);
+    }
+  }
+}
+// 16 consecutive staged fp32 of `row` from column `col` (multiple of 4); rowaddr = shared address of the row
+__device__ __forceinline__ void acc_ld16_sw(uint32_t rowaddr, int row, int col, uint32_t (&r)[16]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint32_t a = rowaddr + ((uint32_t)(((col >> 2) + i) ^ (row & 7)) << 4);
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[4 * i]), "=r"(r[4 * i + 1]), "=r"(r[4 * i + 2]), "=r"(r[4 * i + 3]) : "r"(a));
+  }
+}
+__host__ __device__ inline TmaSmem tma_smem_layout(int BN, int stages, bool has_res, bool direct, bool x3, bool res_up2,
+                                                  bool res_inplace, int opairs) {
   TmaSmem s;
   const uint32_t mul = x3 ? 2u : 1u;
-  s.a_half = 128 * 128; s.b_half = (uint32_t)BN * 128; s.patch_half = (uint32_t)patch_rows * 128u;
-  s.a_bytes = patch_rows ? 0u : s.a_half * mul;
+  s.a_half = 128 * 128; s.b_half = (uint32_t)BN * 128;
+  s.a_bytes = s.a_half * mul;
   s.b_bytes = s.b_half * mul;
   s.stage_bytes = s.a_bytes + s.b_bytes;
-  s.patch = 1024;                                            // barriers live in the first KB
-  s.patch_bytes = s.patch_half * mul;                        // multiple of 2048 (16-pixel patch rows)
-  s.stages = s.patch + s.patch_bytes * (uint32_t)pstages;
+  s.stages = 1024;                                           // barriers live in the first KB
   s.out = s.stages + s.stage_bytes * (uint32_t)stages;
   s.res_slab = (x3 && res_up2) ? 4096u : (uint32_t)TM_SLAB_BYTES;
   if (x3) {
@@ -140,20 +147,24 @@ __host__ __device__ inline TmaSmem tma_smem_layout(int BN, int stages, bool has_
     // store can still be reading the first while the second is written); in-place residual: one pair per slab and buffer
     s.oslabs = direct ? 0u : (res_inplace ? 2u * (uint32_t)(BN / 64) : (uint32_t)opairs);
     s.res = s.out + s.oslabs * 2u * TM_SLAB_BYTES;
-    s.total = s.res + ((has_res && !res_inplace) ? 2u * (uint32_t)(BN / 64) * 2u * s.res_slab : 0u);
-    return s;
+    s.acc = s.res + ((has_res && !res_inplace) ? 2u * (uint32_t)(BN / 64) * 2u * s.res_slab : 0u);
+  } else {
+    s.oslabs = 0;
+    const uint32_t out_slabs = direct ? 0 : (BN == 64 ? 1 : 2);   // one output slab per epilogue group (TMA-store epilogue only)
+    s.res = s.out + out_slabs * TM_SLAB_BYTES;
+    s.acc = s.res + (has_res ? 2u * (uint32_t)(BN / 64) * TM_SLAB_BYTES : 0u);   // two residual buffers (prefetch)
   }
-  s.oslabs = 0;
-  const uint32_t out_slabs = direct ? 0 : (BN == 64 ? 1 : 2);   // one output slab per epilogue group (TMA-store epilogue only)
-  s.res = s.out + out_slabs * TM_SLAB_BYTES;
-  s.total = s.res + (has_res ? 2u * (uint32_t)(BN / 64) * TM_SLAB_BYTES : 0u);   // two residual buffers (prefetch)
+  s.total = s.acc + 128u * (uint32_t)BN * 4u;
   return s;
 }
 
-// Roles (11 warps): warps 0-7 epilogue (TMEM lane quadrant = warp & 3; column half = warp >> 2), warp 8 TMA
-// operand loads, warp 9 MMA issue + TMEM ownership, warp 10 residual-slab loads.
-// Barriers: full[s]/empty[s] smem ring (TMA <-> MMA), tfull[b]/tempty[b] TMEM buffers (MMA <-> epilogue),
-// rfull/rempty residual slabs (TMA <-> epilogue).
+// Roles (10 warps): warps 0-7 consumers -- two wgmma warpgroups (tile rows [64 wg, 64 wg + 64)), then the epilogue
+// (thread = accumulator row q * 32 + lane with q = warp & 3; column half = warp >> 2); warp 8 TMA operand loads, warp 9
+// residual-slab loads.
+// Barriers: full[s]/empty[s] smem ring (TMA <-> consumers), rfull/rempty residual slabs (TMA <-> epilogue).
+// N: accumulator columns (BN, or 2 BN in wide mode), the width of the wgmma instructions.  MMA: TM_MMA_* (the products
+// issued per K slice), a template parameter so that no run-time branch sits between the wgmmas of a k-block.
+template <int N, int MMA>
 __global__ void __launch_bounds__(TM_THREADS, 1)
 igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
                  const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ CUtensorMap tm_r, const TmaGeom g) {
@@ -161,13 +172,10 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
   const uint32_t raw = smem_u32(smem_dyn);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* sm = smem_dyn + (base - raw);
-  const TmaSmem L = tma_smem_layout(g.BN, g.wres ? g.wtiles : g.stages, g.has_res != 0, g.halo ? g.patch_rows : 0, g.pstages,
-                                    g.direct != 0, g.x3 != 0, g.res_up2 != 0, g.res_inplace != 0, g.opairs);
+  const TmaSmem L = tma_smem_layout(g.BN, g.stages, g.has_res != 0, g.direct != 0, g.x3 != 0, g.res_up2 != 0, g.res_inplace != 0,
+                                    g.opairs);
   const uint32_t bar_full = base, bar_empty = base + 8 * TM_MAX_STAGES;
-  const uint32_t bar_tfull = bar_empty + 8 * TM_MAX_STAGES, bar_tempty = bar_tfull + 16;
-  const uint32_t bar_rfull = bar_tempty + 16, bar_rempty = bar_rfull + 16;     // two residual buffers
-  const uint32_t bar_pfull = bar_rempty + 16, bar_pempty = bar_pfull + 32;     // up to four patch slots (halo mode)
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(sm + 8 * (2 * TM_MAX_STAGES + 16));
+  const uint32_t bar_rfull = bar_empty + 8 * TM_MAX_STAGES, bar_rempty = bar_rfull + 16;     // two residual buffers
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cchunks = g.Cin / 64;
@@ -175,50 +183,30 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
   const long long m_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n;
   const long long num_tiles = m_tiles * g.n_tiles;
   const uint32_t box_bytes = (uint32_t)(g.bw * g.bh * g.bn) * 128u;
-  // wide-B (pair mode, N tile <= 64, per-tap boxes / stem): B operand = the contiguous [W_hi ; W_lo] tile of the stage (N = 2 BN)
-  const uint32_t acc_cols = (uint32_t)(g.wide ? 2 * g.BN : g.BN);      // TMEM columns of one accumulator buffer
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < 2 * acc_cols) tmem_cols <<= 1;
 
-  if (warp == TM_WARP_MMA) {
-    if (lane == 0) {
-      for (int s = 0; s < g.stages; ++s) {
-        mbar_init(bar_full + 8 * s, 1);
-        mbar_init(bar_empty + 8 * s, 1);
-      }
-      for (int b = 0; b < 2; ++b) {
-        mbar_init(bar_tfull + 8 * b, 1);
-        mbar_init(bar_tempty + 8 * b, TM_EPI_WARPS);
-      }
-      for (int b = 0; b < 2; ++b) {
-        mbar_init(bar_rfull + 8 * b, 1);
-        mbar_init(bar_rempty + 8 * b, g.res_inplace ? 1 : TM_EPI_WARPS);
-      }
-      for (int b = 0; b < 4; ++b) {
-        mbar_init(bar_pfull + 8 * b, 1);
-        mbar_init(bar_pempty + 8 * b, 1);
-      }
-      fence_mbar_init();
+  if (tid == 0) {
+    for (int s = 0; s < g.stages; ++s) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, TM_EPI_WARPS);
     }
-    __syncwarp();
-    tmem_alloc(smem_u32(tmem_ptr_smem), tmem_cols);
+    for (int b = 0; b < 2; ++b) {
+      mbar_init(bar_rfull + 8 * b, 1);
+      mbar_init(bar_rempty + 8 * b, g.res_inplace ? 1 : TM_EPI_WARPS);
+    }
+    fence_mbar_init();
   } else if (warp == TM_WARP_TMA && lane == 0) {
     prefetch_tmap(&tm_x);
     prefetch_tmap(&tm_w);
     prefetch_tmap(&tm_y);
     if (g.has_res || (g.stem && g.x3)) prefetch_tmap(&tm_r);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   if (warp == TM_WARP_TMA) {
     // =============================== OPERAND LOADS ===============================
     if (lane == 0) {
       // ring position / phase are running counters: no division on the per-k-block path of this single thread
-      uint32_t s = 0, ph = 0, sp = 0, php = 0;
-      bool first_tile = true;
+      uint32_t s = 0, ph = 0;
       uint32_t a_dst = base + L.stages;
       const uint32_t tx_bytes = (g.x3 ? 2u * box_bytes : box_bytes) + L.b_bytes;
       for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -228,67 +216,8 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
         const int h0 = (int)((mt / g.tiles_w) % g.tiles_h) * g.bh;
         const int i0 = (int)(mt / ((long long)g.tiles_w * g.tiles_h)) * g.bn;
         const int n0 = nt * g.BN;
-        if (g.halo) {
-          // Units (tile, channel chunk) in order.  The PATCH of unit u+1 is requested before the weight tiles of unit u
-          // (its latency would otherwise be exposed once per unit: the weight ring is shorter than a unit's KHW tiles).
-          // Resident-weight mode: the n-tile's whole weight set is loaded once, up front.
-          if (first_tile) {
-            first_tile = false;
-            if (g.wres) {
-              mbar_arrive_expect_tx(bar_full, (uint32_t)(g.KHW * cchunks) * L.b_bytes);
-              for (int cc = 0; cc < cchunks; ++cc)
-                for (int tap = 0; tap < g.KHW; ++tap) {
-                  const uint32_t wd = base + L.stages + (uint32_t)(cc * g.KHW + tap) * L.b_bytes;
-                  tma_load_2d(wd, &tm_w, bar_full, tap * g.Cin + cc * 64, n0);
-                  if (g.x3) tma_load_2d(wd + L.b_half, &tm_w, bar_full, tap * g.Cin + cc * 64, g.w_lo + n0);
-                }
-            }
-            mbar_wait(bar_pempty + 8 * sp, php ^ 1u);
-            mbar_arrive_expect_tx(bar_pfull + 8 * sp, L.patch_bytes);
-            tma_load_4d(base + L.patch + sp * L.patch_bytes, &tm_x, bar_pfull + 8 * sp, 0, w0 - g.pw, h0 - g.ph, i0);
-            if (g.x3) tma_load_4d(base + L.patch + sp * L.patch_bytes + L.patch_half, &tm_x, bar_pfull + 8 * sp, g.x_lo, w0 - g.pw, h0 - g.ph, i0);
-            if (++sp == (uint32_t)g.pstages) { sp = 0; php ^= 1u; }
-          }
-          const long long ntile = tile + gridDim.x;
-          for (int cc = 0; cc < cchunks; ++cc) {
-            // next unit: next chunk of this tile, or chunk 0 of this CTA's next tile
-            if (cc + 1 < cchunks || ntile < num_tiles) {
-              int nw0 = w0, nh0 = h0, ni0 = i0, ncc = cc + 1;
-              if (cc + 1 == cchunks) {
-                const long long nmt = ntile / g.n_tiles;
-                nw0 = (int)(nmt % g.tiles_w) * g.bw;
-                nh0 = (int)((nmt / g.tiles_w) % g.tiles_h) * g.bh;
-                ni0 = (int)(nmt / ((long long)g.tiles_w * g.tiles_h)) * g.bn;
-                ncc = 0;
-              }
-              mbar_wait(bar_pempty + 8 * sp, php ^ 1u);
-              mbar_arrive_expect_tx(bar_pfull + 8 * sp, L.patch_bytes);
-              tma_load_4d(base + L.patch + sp * L.patch_bytes, &tm_x, bar_pfull + 8 * sp, ncc * 64, nw0 - g.pw, nh0 - g.ph, ni0);
-              if (g.x3) tma_load_4d(base + L.patch + sp * L.patch_bytes + L.patch_half, &tm_x, bar_pfull + 8 * sp, g.x_lo + ncc * 64, nw0 - g.pw, nh0 - g.ph, ni0);
-              if (++sp == (uint32_t)g.pstages) { sp = 0; php ^= 1u; }
-            }
-            if (g.wres) continue;
-            for (int t_ = 0; t_ < g.KHW; ++t_) {
-              int tap = t_ + (g.rotate ? (int)(mt % g.KHW) : 0);     // same rotation as the MMA loop
-              if (tap >= g.KHW) tap -= g.KHW;
-              const uint32_t bf = bar_full + 8 * s;
-              mbar_wait(bar_empty + 8 * s, ph ^ 1u);
-              mbar_arrive_expect_tx(bf, L.b_bytes);
-              tma_load_2d(a_dst, &tm_w, bf, tap * g.Cin + cc * 64, n0);
-              if (g.x3) tma_load_2d(a_dst + L.b_half, &tm_w, bf, tap * g.Cin + cc * 64, g.w_lo + n0);
-              a_dst += L.stage_bytes;
-              if (++s == (uint32_t)g.stages) { s = 0; ph ^= 1u; a_dst = base + L.stages; }
-            }
-          }
-          continue;
-        }
-        // Optional (UPSNET_TMA_ROTATE=1, default off): start the K loop at a tile-dependent k-block and wrap.  Measured
-        // on B200: SLOWER by 2.5 % end to end -- lock-step CTAs asking for the same weight tile at the same moment is
-        // what lets L2 merge their requests, so the natural order stays the default.
-        int kbr = g.rotate ? (int)((mt * 5) % num_kb) : 0;
-        int tap0 = kbr / cchunks;
-        int cc = kbr - tap0 * cchunks, ki = tap0 / g.kw, kj = tap0 - ki * g.kw;
-        int cw = w0 - g.pw + kj * g.dw, ch = h0 - g.ph + ki * g.dh;         // box origin of the current tap
+        int kbr = 0, cc = 0, kj = 0;
+        int cw = w0 - g.pw, ch = h0 - g.ph;         // box origin of the current tap
         for (int kb = 0; kb < num_kb; ++kb) {
           const uint32_t bf = bar_full + 8 * s;
           mbar_wait(bar_empty + 8 * s, ph ^ 1u);
@@ -305,126 +234,14 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
               tma_load_4d(a_dst + L.a_half, &tm_x, bf, g.x_lo + cc * 64, cw, ch, i0);
             tma_load_2d(a_dst + L.a_bytes + L.b_half, &tm_w, bf, kbr * 64, g.w_lo + n0);
           }
-          if (++kbr == num_kb) { kbr = 0; cc = 0; kj = 0; cw = w0 - g.pw; ch = h0 - g.ph; }
-          else if (++cc == cchunks) {
+          ++kbr;
+          if (++cc == cchunks) {
             cc = 0; cw += g.dw;
             if (++kj == g.kw) { kj = 0; cw = w0 - g.pw; ch += g.dh; }
           }
           a_dst += L.stage_bytes;
           if (++s == (uint32_t)g.stages) { s = 0; ph ^= 1u; a_dst = base + L.stages; }
         }
-      }
-    }
-    __syncwarp();
-  } else if (warp == TM_WARP_MMA) {
-    // =============================== MMA ISSUER ===============================
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc(128, g.BN), idesc_w = umma_idesc(128, 2 * g.BN);
-      // smem descriptors: constant high word (SBO = 1024 B, version 1, SWIZZLE_128B), the low word carries
-      // (address >> 4) and is advanced by running adds -- the issue loop of this single thread paces every tile
-      // whose MMAs are short (N <= 128), so it is kept to a handful of instructions per k-block.
-      const uint32_t desc_hi = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);
-      const uint32_t a_lo0 = ((base + L.stages) >> 4) & 0x3fffu, stage16 = L.stage_bytes >> 4, a16 = L.a_bytes >> 4;
-      const uint32_t ah16 = L.a_half >> 4, bh16 = L.b_half >> 4, ph16 = L.patch_half >> 4;   // pair mode: lo-tile offsets
-      uint32_t s = 0, ph = 0, a_lo = a_lo0, ti_local = 0, sp = 0, php = 0;
-      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++ti_local) {
-        const uint32_t buf = ti_local & 1u, use = ti_local >> 1;
-        mbar_wait(bar_tempty + 8 * buf, (use & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + buf * acc_cols;
-        uint32_t acc = 0u;
-        if (g.halo) {
-          // A descriptors: 8-row groups = 8 consecutive patch pixels of one patch row, group stride = one patch row
-          // (16 px = 2048 B); a tap shifts the START by whole 128-byte rows.  Measured on B200: the SWIZZLE_128B XOR is
-          // taken from the shared-memory ADDRESS bits [7,10) -- exactly what the TMA write used -- so a start that is
-          // not 1024-byte aligned needs no base-offset (field = 0; a non-zero value double-shifts and corrupts the tile).
-          const uint32_t hi_a0 = (uint32_t)(2048 >> 4) | (1u << 14) | (2u << 29);
-          if (g.wres && ti_local == 0) {     // the resident weight set: one barrier, once per CTA
-            mbar_wait(bar_full, 0u);
-            tc_fence_after();
-          }
-          for (int cc = 0; cc < cchunks; ++cc) {
-            mbar_wait(bar_pfull + 8 * sp, php);
-            tc_fence_after();
-            const uint32_t patch = base + L.patch + sp * L.patch_bytes;
-            int ky = 0, kx = 0;
-            if (g.wres) {
-              uint32_t b_lo = a_lo0 + (uint32_t)(cc * g.KHW) * (L.b_bytes >> 4);
-              for (int tap = 0; tap < g.KHW; ++tap) {
-                const uint32_t a_start = patch + (uint32_t)((ky * g.dh * 16 + kx * g.dw) * 128);
-                const uint32_t pa_lo = (a_start >> 4) & 0x3fffu;
-#pragma unroll
-                for (uint32_t k = 0; k < 4; ++k) {
-                  if (g.x3) {
-                    umma_bf16_lohi2(tmem_d, pa_lo + ph16 + 2 * k, hi_a0, b_lo + 2 * k, desc_hi, idesc, acc);
-                    umma_bf16_lohi2(tmem_d, pa_lo + 2 * k, hi_a0, b_lo + bh16 + 2 * k, desc_hi, idesc, 1u);
-                    acc = 1u;
-                  }
-                  umma_bf16_lohi2(tmem_d, pa_lo + 2 * k, hi_a0, b_lo + 2 * k, desc_hi, idesc, acc);
-                  acc = 1u;
-                }
-                b_lo += L.b_bytes >> 4;
-                if (++kx == g.kw) { kx = 0; ++ky; }
-              }
-              umma_commit(bar_pempty + 8 * sp);
-              if (++sp == (uint32_t)g.pstages) { sp = 0; php ^= 1u; }
-              continue;
-            }
-            const int trot = g.rotate ? (int)((tile / g.n_tiles) % g.KHW) : 0;
-            ky = trot / g.kw; kx = trot - ky * g.kw;
-            for (int t_ = 0; t_ < g.KHW; ++t_) {
-              mbar_wait(bar_full + 8 * s, ph);
-              tc_fence_after();
-              const uint32_t a_start = patch + (uint32_t)((ky * g.dh * 16 + kx * g.dw) * 128);
-              const uint32_t pa_lo = (a_start >> 4) & 0x3fffu, pa_hi = hi_a0;
-#pragma unroll
-              for (uint32_t k = 0; k < 4; ++k) {
-                if (g.x3) {
-                  umma_bf16_lohi2(tmem_d, pa_lo + ph16 + 2 * k, pa_hi, a_lo + 2 * k, desc_hi, idesc, acc);
-                  umma_bf16_lohi2(tmem_d, pa_lo + 2 * k, pa_hi, a_lo + bh16 + 2 * k, desc_hi, idesc, 1u);
-                  acc = 1u;
-                }
-                umma_bf16_lohi2(tmem_d, pa_lo + 2 * k, pa_hi, a_lo + 2 * k, desc_hi, idesc, acc);
-                acc = 1u;
-              }
-              umma_commit(bar_empty + 8 * s);
-              a_lo += stage16;
-              if (++s == (uint32_t)g.stages) { s = 0; ph ^= 1u; a_lo = a_lo0; }
-              if (++kx == g.kw) { kx = 0; if (++ky == g.kh) ky = 0; }
-            }
-            umma_commit(bar_pempty + 8 * sp);     // every tap of this chunk has been issued: the patch slot may be refilled
-            if (++sp == (uint32_t)g.pstages) { sp = 0; php ^= 1u; }
-          }
-          umma_commit(bar_tfull + 8 * buf);
-          continue;
-        }
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(bar_full + 8 * s, ph);
-          tc_fence_after();
-          const uint32_t b_lo = a_lo + a16;
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k) {       // 16 bf16 = 32 bytes = 2 descriptor units inside the swizzle span
-            if (g.dbg == 3 || (g.dbg == 2 && k)) continue;
-            const uint32_t td = (g.dbg == 1 && (k & 1)) ? (tmem_base + (buf ^ 1u) * acc_cols) : tmem_d;
-            if (g.wide) {    // two instructions per K slice: hi * [hi ; lo] -> columns [0, 2 BN), lo * hi -> columns [0, BN)
-              umma_bf16_lohi(td, a_lo + 2 * k, b_lo + 2 * k, desc_hi, idesc_w, acc);
-              umma_bf16_lohi(td, a_lo + ah16 + 2 * k, b_lo + 2 * k, desc_hi, idesc, 1u);
-              acc = 1u;
-              continue;
-            }
-            if (g.x3) {      // (hi + lo) * (hi + lo) without the lo * lo term: relative error ~2^-16
-              umma_bf16_lohi(td, a_lo + ah16 + 2 * k, b_lo + 2 * k, desc_hi, idesc, acc);
-              umma_bf16_lohi(td, a_lo + 2 * k, b_lo + bh16 + 2 * k, desc_hi, idesc, 1u);
-              acc = 1u;
-            }
-            umma_bf16_lohi(td, a_lo + 2 * k, b_lo + 2 * k, desc_hi, idesc, acc);
-            acc = 1u;
-          }
-          umma_commit(bar_empty + 8 * s);
-          a_lo += stage16;
-          if (++s == (uint32_t)g.stages) { s = 0; ph ^= 1u; a_lo = a_lo0; }
-        }
-        umma_commit(bar_tfull + 8 * buf);
       }
     }
     __syncwarp();
@@ -466,9 +283,54 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
     }
     __syncwarp();
   } else {
-    // =============================== EPILOGUE (warps 0-7) ===============================
+    // =============================== CONSUMERS (warps 0-7) ===============================
+    const int wg = warp >> 2;
+    const uint32_t dhi = wg_desc_hi(1024);
+    const uint32_t a_row0 = (uint32_t)wg * 64u * 128u;       // this warpgroup's 64 rows of the A tile
+    const uint32_t ah16 = L.a_half >> 4;       // pair mode: lo A tile offset (descriptor units)
+    float* accbuf = reinterpret_cast<float*>(sm + L.acc);
+    constexpr int SW = MMA == TM_MMA_WIDE ? N / 2 : N;        // staged columns (= BN)
+    float d[N / 2];
+    uint32_t s = 0, ph = 0;
+    // main loop of one tile, then its accumulators -> staging rows (all eight warps take part)
+    auto mainloop = [&]() {
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(bar_full + 8 * s, ph);
+        const uint32_t st0 = base + L.stages + s * L.stage_bytes;
+        const uint32_t a = wg_desc_lo(st0 + a_row0), b = wg_desc_lo(st0 + L.a_bytes);
+        wgmma_fence();
+#pragma unroll
+        for (uint32_t k = 0; k < 4; ++k) {       // 16 bf16 = 32 bytes = 2 descriptor units inside the swizzle span
+          const uint32_t acc = (kb | k) ? 1u : 0u;
+          if constexpr (MMA == TM_MMA_WIDE) {   // hi * [hi ; lo] -> columns [0, 2 BN), lo * hi -> columns [0, BN)
+            Wgmma<N>::mma(d, wg_desc(a + 2 * k, dhi), wg_desc(b + 2 * k, dhi), acc);
+            Wgmma<N / 2>::mma(*reinterpret_cast<float(*)[N / 4]>(&d[0]), wg_desc(a + ah16 + 2 * k, dhi), wg_desc(b + 2 * k, dhi), 1u);
+          } else {
+            Wgmma<N>::mma(d, wg_desc(a + 2 * k, dhi), wg_desc(b + 2 * k, dhi), acc);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                         // the previous k-block's wgmmas have read their stage
+        wgmma_fence_acc(d);
+        if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+        prev = (int)s;
+        if (++s == (uint32_t)g.stages) { s = 0; ph ^= 1u; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(d);
+      if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+      if constexpr (MMA == TM_MMA_WIDE) {        // hi*hi + lo*hi (columns [0, BN)) + hi*lo (columns [BN, 2 BN)): same thread
+#pragma unroll
+        for (int i = 0; i < N / 4; ++i) d[i] += d[N / 4 + i];
+      }
+      named_bar_sync(3, 256);                    // the previous tile's epilogue has read the staging rows
+      acc_stage_sw<N, SW>(d, accbuf, wg * 64);
+      named_bar_sync(3, 256);
+    };
     const int q = warp & 3, half = warp >> 2;
     const int row = q * 32 + lane;
+    const uint32_t trow = smem_u32(accbuf + (size_t)row * SW);
     const int units = g.BN / 32;                       // 32-column units of the accumulator
     const int upw = units >= 4 ? units / 2 : 1;        // units per half (BN = 64: one each)
     const int bar_id = g.BN == 64 ? 1 : 1 + half;
@@ -492,10 +354,8 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
       const int i0 = (int)(mt / ((long long)g.tiles_w * g.tiles_h)) * g.bn;
       const int n0 = nt * g.BN;
       const uint32_t buf = ti_local & 1u, use = ti_local >> 1;
-      mbar_wait(bar_tfull + 8 * buf, use & 1u);
-      tc_fence_after();
+      mainloop();
       if (g.has_res) mbar_wait(bar_rfull + 8 * buf, use & 1u);
-      const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + buf * acc_cols;
       if (g.direct) {
         // thread = accumulator row = one output pixel of the box; the two halves split the columns
         const int wq = row % g.bw, hq = (row / g.bw) % g.bh, nq = row / (g.bw * g.bh);
@@ -506,16 +366,7 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
         const int cbeg = half * (g.BN / 2), cend = cbeg + g.BN / 2;
         for (int cb = cbeg; cb < cend; cb += 16) {
           uint32_t v[16];
-          if (g.wide) {       // hi*hi + lo*hi in column cb, hi*lo in column BN + cb
-            uint32_t v2[16];
-            tmem_ld16_issue(trow + (uint32_t)cb, v);
-            tmem_ld16_issue(trow + (uint32_t)(g.BN + cb), v2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(v2[e]));
-          } else {
-            tmem_ld16(trow + (uint32_t)cb, v);         // warp-collective
-          }
+          acc_ld16_sw(trow, row, cb, v);
           const int co0 = n0 + cb;
           if (!ok || co0 >= g.Cout) continue;
 #pragma unroll
@@ -531,9 +382,6 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
             else reinterpret_cast<float*>(g.y)[oi] = o;
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_tempty + 8 * buf);
         continue;
       }
       if (g.x3) {
@@ -545,8 +393,8 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
         for (int sl = 0; sl < nslab; ++sl, ++oc) {
           const int u = 2 * sl + half;
           uint32_t v0[16], v1[16];
-          tmem_ld16_issue(trow + (uint32_t)(u * 32), v0);
-          tmem_ld16_issue(trow + (uint32_t)(u * 32 + 16), v1);
+          acc_ld16_sw(trow, row, u * 32, v0);
+          acc_ld16_sw(trow, row, u * 32 + 16, v1);
           uint32_t ob;
           if (g.res_inplace) {
             ob = base + L.out + (buf * (uint32_t)nslab + (uint32_t)sl) * 2u * TM_SLAB_BYTES;   // holds this slab's residual
@@ -557,17 +405,9 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
             }
             named_bar_sync(1, 256);
           }
-          tmem_ld_wait();
           float o[32];
 #pragma unroll
           for (int e = 0; e < 16; ++e) { o[e] = __uint_as_float(v0[e]); o[16 + e] = __uint_as_float(v1[e]); }
-          if (g.wide) {       // + the hi*lo column group
-            tmem_ld16_issue(trow + (uint32_t)(g.BN + u * 32), v0);
-            tmem_ld16_issue(trow + (uint32_t)(g.BN + u * 32 + 16), v1);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) { o[e] += __uint_as_float(v0[e]); o[16 + e] += __uint_as_float(v1[e]); }
-          }
           if (g.bias) {
             const float4* bp = reinterpret_cast<const float4*>(g.bias + n0 + u * 32);
 #pragma unroll
@@ -616,12 +456,8 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
             bulk_commit();
           }
         }
-        tc_fence_before();
         __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(bar_tempty + 8 * buf);
-          if (g.has_res && !g.res_inplace) mbar_arrive(bar_rempty + 8 * buf);
-        }
+        if (lane == 0 && g.has_res && !g.res_inplace) mbar_arrive(bar_rempty + 8 * buf);
         if (g.res_inplace && lead) {     // the slab pairs of this tile may be refilled once their stores have been read out
           bulk_wait_read0();
           mbar_arrive(bar_rempty + 8 * buf);
@@ -633,14 +469,13 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
         const int slab = u >> 1;
         const uint32_t jb = (uint32_t)(u & 1) * 4u;     // first 16-byte chunk of this unit inside the slab row
         uint32_t v0[16], v1[16];
-        tmem_ld16_issue(trow + (uint32_t)(u * 32), v0);
-        tmem_ld16_issue(trow + (uint32_t)(u * 32 + 16), v1);
+        acc_ld16_sw(trow, row, u * 32, v0);
+        acc_ld16_sw(trow, row, u * 32 + 16, v1);
         if ((u & 1) == 0 || g.BN == 64) {
           // the output slab is about to be overwritten: its previous TMA store must have finished reading it
           if (leader) bulk_wait_read0();
           named_bar_sync(bar_id, bar_cnt);
         }
-        tmem_ld_wait();
         float o[32];
 #pragma unroll
         for (int e = 0; e < 16; ++e) { o[e] = __uint_as_float(v0[e]); o[16 + e] = __uint_as_float(v1[e]); }
@@ -685,414 +520,10 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
           }
         }
       }
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(bar_tempty + 8 * buf);
-        if (g.has_res) mbar_arrive(bar_rempty + 8 * buf);
-      }
+      if (lane == 0 && g.has_res) mbar_arrive(bar_rempty + 8 * buf);
     }
     if (leader || (g.x3 && warp == 0 && lane == 0)) bulk_wait0();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == TM_WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
-  }
-}
-
-// ----------------------------------------------------------------------------------------------
-// 2-CTA variant (cta_group::2) for the latency-bound layers of the PAIR stream.
-//
-// A cluster of two CTAs (one TPC) works on an M = 256 tile: CTA r owns output rows [128 r, 128 r + 128) -- m-tile 2p + r of
-// the same n-tile -- and stages its OWN A tiles (hi, lo) but only HALF of the weight tile (rows [n0 + r*BN/2, +BN/2) of both
-// planes); `tcgen05.mma.cta_group::2` (issued by the leader CTA's single MMA thread, M = 256) reads the B halves from both
-// CTAs' shared memory.  A pair k-block is then 48 KB per CTA instead of 64 KB, so FOUR ring stages fit next to the output
-// slab pair instead of three -- the ring is latency-bound (profiles/r2_mma_probe_pair.md), stages are throughput.
-// Protocol (CUTLASS sm100 2-SM scheme): every CTA's TMA thread issues its loads with `.cta_group::2`, their complete_tx
-// bytes go to the LEADER's full barrier (which expects the bytes of both CTAs); `tcgen05.commit ... multicast::cluster`
-// releases the stage / publishes the accumulator in BOTH CTAs; both CTAs' epilogue warps arrive on the leader's
-// tmem-empty barrier (remote mbarrier arrive for CTA 1).  Per-tap boxes only, no residual (the +res layers keep the 1-CTA
-// kernel with in-place slab pairs); slab (pair) or direct (fp32) epilogue as in the 1-CTA kernel.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t addr, uint32_t rank) {   // shared::cta address -> shared::cluster address in CTA `rank`
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(uint32_t dst, const CUtensorMap* tm, uint32_t bar_leader, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar_leader), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma2_load_2d(uint32_t dst, const CUtensorMap* tm, uint32_t bar_leader, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar_leader), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma2_bf16_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi, uint32_t idesc,
-                                                uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(desc_hi) : "memory");
-}
-__device__ __forceinline__ void umma2_commit_mc(uint32_t bar) {      // arrive on `bar` (same offset) in both CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-
-struct Tma2Smem { uint32_t stages, out, res, res_slab, a_half, b_half, a_bytes, b_bytes, stage_bytes, total; };
-__host__ __device__ inline Tma2Smem tma2_smem_layout(int BN, int stages, bool direct, int opairs, bool has_res = false,
-                                                    bool res_up2 = false, bool res_inplace = false, bool wide = false) {
-  Tma2Smem s;
-  s.a_half = 128 * 128; s.b_half = (uint32_t)(BN / 2) * 128;      // this CTA's half of the weight tile, per plane
-  // wide: [Y: BN rows = this CTA's half of [W_hi ; W_lo]] [X: BN/2 rows = this CTA's half of W_hi]
-  s.a_bytes = 2 * s.a_half; s.b_bytes = (wide ? 3u : 2u) * s.b_half;
-  s.stage_bytes = s.a_bytes + s.b_bytes;
-  s.stages = 1024;
-  s.out = s.stages + s.stage_bytes * (uint32_t)stages;
-  s.res_slab = res_up2 ? 4096u : (uint32_t)TM_SLAB_BYTES;
-  const uint32_t pairs = direct ? 0u : (res_inplace ? 2u * (uint32_t)(BN / 64) : (uint32_t)opairs);
-  s.res = s.out + pairs * 2u * TM_SLAB_BYTES;
-  s.total = s.res + ((has_res && !res_inplace) ? 2u * (uint32_t)(BN / 64) * 2u * s.res_slab : 0u);
-  return s;
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TM_THREADS, 1)
-igemm_tma2_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
-                  const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ CUtensorMap tm_r, const TmaGeom g) {
-  extern __shared__ __align__(1024) uint8_t smem_dyn[];
-  const uint32_t raw = smem_u32(smem_dyn);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* sm = smem_dyn + (base - raw);
-  const Tma2Smem L = tma2_smem_layout(g.BN, g.stages, g.direct != 0, g.opairs, g.has_res != 0, g.res_up2 != 0, g.res_inplace != 0,
-                                      g.wide != 0);
-  const uint32_t acc_cols = (uint32_t)(g.wide ? 2 * g.BN : g.BN);      // TMEM columns of one accumulator buffer
-  const uint32_t bar_full = base, bar_empty = base + 8 * TM_MAX_STAGES;
-  const uint32_t bar_tfull = bar_empty + 8 * TM_MAX_STAGES, bar_tempty = bar_tfull + 16;
-  const uint32_t bar_rfull = bar_tempty + 16, bar_rempty = bar_rfull + 16;     // residual slabs: CTA-local protocol
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(sm + 8 * (2 * TM_MAX_STAGES + 16));
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader_cta = rank == 0;
-  const int cchunks = g.Cin / 64;
-  const int num_kb = g.KHW * cchunks;
-  const long long m_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n;
-  const long long p_tiles = (m_tiles + 1) / 2;                      // pairs of m-tiles
-  const long long num_tiles = p_tiles * g.n_tiles;
-  const long long cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-  const uint32_t box_bytes = (uint32_t)(g.bw * g.bh * g.bn) * 128u;
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < 2 * acc_cols) tmem_cols <<= 1;
-
-  if (warp == TM_WARP_MMA) {
-    if (lane == 0) {
-      for (int s = 0; s < g.stages; ++s) {
-        mbar_init(bar_full + 8 * s, 1);
-        mbar_init(bar_empty + 8 * s, 1);
-      }
-      for (int b = 0; b < 2; ++b) {
-        mbar_init(bar_tfull + 8 * b, 1);
-        mbar_init(bar_tempty + 8 * b, 2 * TM_EPI_WARPS);      // the epilogue warps of BOTH CTAs (used in the leader only)
-        mbar_init(bar_rfull + 8 * b, 1);
-        mbar_init(bar_rempty + 8 * b, g.res_inplace ? 1 : TM_EPI_WARPS);
-      }
-      fence_mbar_init();
-    }
-    __syncwarp();
-    tmem_alloc2(smem_u32(tmem_ptr_smem), tmem_cols);
-  } else if (warp == TM_WARP_TMA && lane == 0) {
-    prefetch_tmap(&tm_x);
-    prefetch_tmap(&tm_w);
-    prefetch_tmap(&tm_y);
-    if (g.has_res) prefetch_tmap(&tm_r);
-  }
-  tc_fence_before();
-  cluster_sync_all();          // barriers of both CTAs initialised, TMEM allocated in both
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  if (warp == TM_WARP_TMA) {
-    if (lane == 0) {
-      uint32_t s = 0, ph = 0;
-      uint32_t a_dst = base + L.stages;
-      const uint32_t tx_both = 2u * (2u * box_bytes + L.b_bytes);       // both CTAs' A (hi, lo) boxes + B parts
-      for (long long tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        const int nt = (int)(tile % g.n_tiles);
-        const long long mt = 2 * (tile / g.n_tiles) + rank;
-        const int w0 = (int)(mt % g.tiles_w) * g.bw;
-        const int h0 = (int)((mt / g.tiles_w) % g.tiles_h) * g.bh;
-        const int i0 = (int)(mt / ((long long)g.tiles_w * g.tiles_h)) * g.bn;     // >= N for the odd tail tile: all-zero boxes
-        const int nrow = nt * g.BN + (int)rank * (g.BN / 2);                      // this CTA's half of the weight rows
-        int cc = 0, kj = 0, cw = w0 - g.pw, ch = h0 - g.ph;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          const uint32_t bf_local = bar_full + 8 * s;
-          const uint32_t bf = mapa_rank(bf_local, 0);                 // complete_tx goes to the leader CTA's barrier
-          mbar_wait(bar_empty + 8 * s, ph ^ 1u);
-          if (leader_cta) mbar_arrive_expect_tx(bf_local, tx_both);
-          tma2_load_4d(a_dst, &tm_x, bf, cc * 64, cw, ch, i0);
-          tma2_load_4d(a_dst + L.a_half, &tm_x, bf, g.x_lo + cc * 64, cw, ch, i0);
-          if (g.wide) {
-            const int yrow = (rank ? g.w_lo : 0) + nt * g.BN;              // CTA 0: the hi rows of the n-tile, CTA 1: its lo rows
-            tma2_load_2d(a_dst + L.a_bytes, &tm_w, bf, kb * 64, yrow);
-            tma2_load_2d(a_dst + L.a_bytes + L.b_half, &tm_w, bf, kb * 64, yrow + g.BN / 2);
-            tma2_load_2d(a_dst + L.a_bytes + 2 * L.b_half, &tm_w, bf, kb * 64, nrow);     // X: this CTA's half of W_hi
-          } else {
-            tma2_load_2d(a_dst + L.a_bytes, &tm_w, bf, kb * 64, nrow);
-            tma2_load_2d(a_dst + L.a_bytes + L.b_half, &tm_w, bf, kb * 64, g.w_lo + nrow);
-          }
-          if (++cc == cchunks) {
-            cc = 0; cw += g.dw;
-            if (++kj == g.kw) { kj = 0; cw = w0 - g.pw; ch += g.dh; }
-          }
-          a_dst += L.stage_bytes;
-          if (++s == (uint32_t)g.stages) { s = 0; ph ^= 1u; a_dst = base + L.stages; }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == TM_WARP_MMA) {
-    if (lane == 0 && leader_cta) {
-      const uint32_t idesc = umma_idesc(256, g.BN), idesc_w = umma_idesc(256, 2 * g.BN);
-      const uint32_t desc_hi = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);
-      const uint32_t a_lo0 = ((base + L.stages) >> 4) & 0x3fffu, stage16 = L.stage_bytes >> 4, a16 = L.a_bytes >> 4;
-      const uint32_t ah16 = L.a_half >> 4, bh16 = L.b_half >> 4;
-      uint32_t s = 0, ph = 0, a_lo = a_lo0, ti_local = 0;
-      for (long long tile = cluster_id; tile < num_tiles; tile += num_clusters, ++ti_local) {
-        const uint32_t buf = ti_local & 1u, use = ti_local >> 1;
-        mbar_wait(bar_tempty + 8 * buf, (use & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + buf * acc_cols;
-        uint32_t acc = 0u;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(bar_full + 8 * s, ph);
-          tc_fence_after();
-          const uint32_t b_lo = a_lo + a16;
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k) {
-            if (g.wide) {
-              umma2_bf16_lohi(tmem_d, a_lo + 2 * k, b_lo + 2 * k, desc_hi, idesc_w, acc);                 // hi * [hi ; lo] -> columns [0, 2 BN)
-              umma2_bf16_lohi(tmem_d, a_lo + ah16 + 2 * k, b_lo + 2 * bh16 + 2 * k, desc_hi, idesc, 1u);  // lo * hi      -> columns [0, BN)
-            } else {
-              umma2_bf16_lohi(tmem_d, a_lo + ah16 + 2 * k, b_lo + 2 * k, desc_hi, idesc, acc);
-              umma2_bf16_lohi(tmem_d, a_lo + 2 * k, b_lo + bh16 + 2 * k, desc_hi, idesc, 1u);
-              umma2_bf16_lohi(tmem_d, a_lo + 2 * k, b_lo + 2 * k, desc_hi, idesc, 1u);
-            }
-            acc = 1u;
-          }
-          umma2_commit_mc(bar_empty + 8 * s);
-          a_lo += stage16;
-          if (++s == (uint32_t)g.stages) { s = 0; ph ^= 1u; a_lo = a_lo0; }
-        }
-        umma2_commit_mc(bar_tfull + 8 * buf);
-      }
-    }
-    __syncwarp();
-  } else if (warp == TM_WARP_RES) {
-    // residual slab pairs of this CTA's own m-tile: a CTA-local producer / consumer pair, exactly as in the 1-CTA kernel
-    if (lane == 0 && g.has_res) {
-      uint32_t ti_local = 0;
-      const int slabs = g.BN / 64;
-      for (long long tile = cluster_id; tile < num_tiles; tile += num_clusters, ++ti_local) {
-        const int nt = (int)(tile % g.n_tiles);
-        const long long mt = 2 * (tile / g.n_tiles) + rank;
-        const int w0 = (int)(mt % g.tiles_w) * g.bw;
-        const int h0 = (int)((mt / g.tiles_w) % g.tiles_h) * g.bh;
-        const int i0 = (int)(mt / ((long long)g.tiles_w * g.tiles_h)) * g.bn;
-        const uint32_t rb = ti_local & 1u, ruse = ti_local >> 1;
-        mbar_wait(bar_rempty + 8 * rb, (ruse & 1u) ^ 1u);
-        const uint32_t lo_off = g.res_inplace ? (uint32_t)TM_SLAB_BYTES : L.res_slab;
-        const uint32_t pdst = g.res_inplace ? base + L.out + rb * (uint32_t)slabs * 2u * TM_SLAB_BYTES
-                                            : base + L.res + rb * (uint32_t)slabs * 2u * L.res_slab;
-        mbar_arrive_expect_tx(bar_rfull + 8 * rb, (g.res_up2 ? box_bytes / 4 : box_bytes) * (uint32_t)slabs * 2u);
-        for (int sl = 0; sl < slabs; ++sl) {
-          const int c = pair_chan(nt * g.BN + sl * 64, g.pg);
-          tma_load_4d(pdst + (uint32_t)sl * 2u * lo_off, &tm_r, bar_rfull + 8 * rb, c, w0 >> g.res_up2, h0 >> g.res_up2, i0);
-          tma_load_4d(pdst + (uint32_t)sl * 2u * lo_off + lo_off, &tm_r, bar_rfull + 8 * rb, c + g.pg, w0 >> g.res_up2,
-                      h0 >> g.res_up2, i0);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp < TM_EPI_WARPS) {
-    const int q = warp & 3, half = warp >> 2;
-    const int row = q * 32 + lane;
-    const uint32_t sw_row = (uint32_t)row * 128u;
-    const uint32_t rx = (uint32_t)(row & 7);
-    int rrow = row;
-    if (g.res_up2) {
-      const int w = row % g.bw, h = (row / g.bw) % g.bh, n = row / (g.bw * g.bh);
-      rrow = (w >> 1) + (g.bw >> 1) * ((h >> 1) + (g.bh >> 1) * n);
-    }
-    const uint32_t rs_row = (uint32_t)rrow * 128u, rrx = (uint32_t)(rrow & 7);
-    const uint32_t tempty_leader = mapa_rank(bar_tempty, 0);
-    uint32_t ti_local = 0, oc = 0;
-    for (long long tile = cluster_id; tile < num_tiles; tile += num_clusters, ++ti_local) {
-      const int nt = (int)(tile % g.n_tiles);
-      const long long mt = 2 * (tile / g.n_tiles) + rank;
-      const int w0 = (int)(mt % g.tiles_w) * g.bw;
-      const int h0 = (int)((mt / g.tiles_w) % g.tiles_h) * g.bh;
-      const int i0 = (int)(mt / ((long long)g.tiles_w * g.tiles_h)) * g.bn;
-      const int n0 = nt * g.BN;
-      const uint32_t buf = ti_local & 1u, use = ti_local >> 1;
-      mbar_wait(bar_tfull + 8 * buf, use & 1u);
-      tc_fence_after();
-      if (g.has_res) mbar_wait(bar_rfull + 8 * buf, use & 1u);
-      const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + buf * acc_cols;
-      if (g.direct) {
-        const int wq = row % g.bw, hq = (row / g.bw) % g.bh, nq = row / (g.bw * g.bh);
-        const int wo = w0 + wq, ho = h0 + hq, ni = i0 + nq;
-        const bool ok = nq < g.bn && wo < g.Wo && ho < g.Ho && ni < g.N;
-        const size_t HoWo = (size_t)g.Ho * g.Wo;
-        const size_t pix = ((size_t)ni * g.Ho + ho) * g.Wo + wo;
-        const int cbeg = half * (g.BN / 2), cend = cbeg + g.BN / 2;
-        for (int cb = cbeg; cb < cend; cb += 16) {
-          uint32_t v[16];
-          if (g.wide) {       // hi*hi + lo*hi in column cb, hi*lo in column BN + cb
-            uint32_t v2[16];
-            tmem_ld16_issue(trow + (uint32_t)cb, v);
-            tmem_ld16_issue(trow + (uint32_t)(g.BN + cb), v2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(v2[e]));
-          } else {
-            tmem_ld16(trow + (uint32_t)cb, v);
-          }
-          const int co0 = n0 + cb;
-          if (!ok || co0 >= g.Cout) continue;
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const int co = co0 + e;
-            if (co >= g.Cout) break;
-            float o = __uint_as_float(v[e]);
-            if (g.bias) o += __ldg(g.bias + co);
-            if (g.relu) o = fmaxf(o, 0.f);
-            if (g.sig_from >= 0 && co >= g.sig_from) o = 1.f / (1.f + expf(-o));
-            const size_t oi = g.out_nhwc ? pix * g.Cout + co : ((size_t)ni * g.Cout + co) * HoWo + (size_t)ho * g.Wo + wo;
-            reinterpret_cast<float*>(g.y)[oi] = o;
-          }
-        }
-      } else {
-        const int nslab = g.BN / 64;
-        const uint32_t jb = (uint32_t)half * 4u;
-        const bool lead = warp == 0 && lane == 0;
-        for (int sl = 0; sl < nslab; ++sl, ++oc) {
-          const int u = 2 * sl + half;
-          uint32_t v0[16], v1[16];
-          tmem_ld16_issue(trow + (uint32_t)(u * 32), v0);
-          tmem_ld16_issue(trow + (uint32_t)(u * 32 + 16), v1);
-          uint32_t ob;
-          if (g.res_inplace) {
-            ob = base + L.out + (buf * (uint32_t)nslab + (uint32_t)sl) * 2u * TM_SLAB_BYTES;   // holds this slab's residual
-          } else {
-            ob = base + L.out + (g.opairs == 2 ? (oc & 1u) : 0u) * 2u * TM_SLAB_BYTES;
-            if (lead) {
-              if (g.opairs == 2) bulk_wait_read1(); else bulk_wait_read0();
-            }
-            named_bar_sync(1, 256);
-          }
-          tmem_ld_wait();
-          float o[32];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) { o[e] = __uint_as_float(v0[e]); o[16 + e] = __uint_as_float(v1[e]); }
-          if (g.wide) {       // + the hi*lo column group
-            tmem_ld16_issue(trow + (uint32_t)(g.BN + u * 32), v0);
-            tmem_ld16_issue(trow + (uint32_t)(g.BN + u * 32 + 16), v1);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) { o[e] += __uint_as_float(v0[e]); o[16 + e] += __uint_as_float(v1[e]); }
-          }
-          if (g.bias) {
-            const float4* bp = reinterpret_cast<const float4*>(g.bias + n0 + u * 32);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const float4 b4 = __ldg(bp + e);
-              o[4 * e] += b4.x; o[4 * e + 1] += b4.y; o[4 * e + 2] += b4.z; o[4 * e + 3] += b4.w;
-            }
-          }
-          if (g.has_res) {
-            uint32_t rh, rl, xr;
-            if (g.res_inplace) { rh = ob + sw_row; rl = rh + TM_SLAB_BYTES; xr = rx; }
-            else { rh = base + L.res + (buf * (uint32_t)nslab + (uint32_t)sl) * 2u * L.res_slab + rs_row; rl = rh + L.res_slab; xr = rrx; }
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const uint4 hv = lds128(rh + (((jb + c) ^ xr) << 4)), lv = lds128(rl + (((jb + c) ^ xr) << 4));
-              const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w}, lw[4] = {lv.x, lv.y, lv.z, lv.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                o[c * 8 + 2 * e] += __uint_as_float(hw[e] << 16) + __uint_as_float(lw[e] << 16);
-                o[c * 8 + 2 * e + 1] += __uint_as_float(hw[e] & 0xffff0000u) + __uint_as_float(lw[e] & 0xffff0000u);
-              }
-            }
-          }
-          if (g.relu) {
-#pragma unroll
-            for (int e = 0; e < 32; ++e) o[e] = fmaxf(o[e], 0.f);
-          }
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint32_t hw[4], lw[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float a = o[c * 8 + 2 * e], b = o[c * 8 + 2 * e + 1];
-              hw[e] = pack_bf16x2(a, b);
-              lw[e] = pack_bf16x2(a - __uint_as_float(hw[e] << 16), b - __uint_as_float(hw[e] & 0xffff0000u));
-            }
-            sts128(ob + sw_row + (((jb + c) ^ rx) << 4), make_uint4(hw[0], hw[1], hw[2], hw[3]));
-            sts128(ob + TM_SLAB_BYTES + sw_row + (((jb + c) ^ rx) << 4), make_uint4(lw[0], lw[1], lw[2], lw[3]));
-          }
-          fence_proxy_async();
-          named_bar_sync(1, 256);
-          if (lead) {
-            const int c = pair_chan(n0 + sl * 64, g.pg);
-            tma_store_4d(&tm_y, ob, c, w0, h0, i0);
-            tma_store_4d(&tm_y, ob + TM_SLAB_BYTES, c + g.pg, w0, h0, i0);
-            bulk_commit();
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive_cluster(tempty_leader + 8 * buf);     // leader's barrier: 16 arrivals = both CTAs drained
-        if (g.has_res && !g.res_inplace) mbar_arrive(bar_rempty + 8 * buf);
-      }
-      if (g.res_inplace && warp == 0 && lane == 0) {      // slab pairs may be refilled once their stores have been read out
-        bulk_wait_read0();
-        mbar_arrive(bar_rempty + 8 * buf);
-      }
-    }
-    if (warp == 0 && lane == 0) bulk_wait0();
-  }
-  tc_fence_before();
-  cluster_sync_all();          // no CTA may exit (or free TMEM) while its peer still reads its shared memory / signals its barriers
-  if (warp == TM_WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, tmem_cols);
   }
 }
 
@@ -1155,6 +586,48 @@ static void tma_pick_box(int N, int Ho, int Wo, int kh, int kw, int dh, int dw, 
   *bw_o = bbw; *bh_o = bbh; *bn_o = bbn;
 }
 
+template <int N, int MMA>
+static int tma_launch_n(dim3 grid, size_t smem, cudaStream_t stream, const CUtensorMap& tm_x, const CUtensorMap& tm_w,
+                        const CUtensorMap& tm_y, const CUtensorMap& tm_r, const TmaGeom& g) {
+  static ups::PerDeviceOnce configured;     // opt in to 227 KB once per device (outside CUDA-graph capture)
+  if (configured.need())
+    UPS_CUDA(cudaFuncSetAttribute(igemm_tma_kernel<N, MMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  igemm_tma_kernel<N, MMA><<<grid, TM_THREADS, smem, stream>>>(tm_x, tm_w, tm_y, tm_r, g);
+  UPS_CHECK_LAUNCH();
+  return 0;
+}
+// kernel instance for the N tile BN and the geometry's products: bf16 stream N = BN; pairs (wide) N = 2 BN
+static int tma_launch(int BN, dim3 grid, size_t smem, cudaStream_t stream, const CUtensorMap& tm_x, const CUtensorMap& tm_w,
+                      const CUtensorMap& tm_y, const CUtensorMap& tm_r, const TmaGeom& g) {
+  if (g.wide) {
+    if (BN == 32) return tma_launch_n<64, TM_MMA_WIDE>(grid, smem, stream, tm_x, tm_w, tm_y, tm_r, g);
+    if (BN == 64) return tma_launch_n<128, TM_MMA_WIDE>(grid, smem, stream, tm_x, tm_w, tm_y, tm_r, g);
+  } else {
+    if (BN == 32) return tma_launch_n<32, TM_MMA_BF16>(grid, smem, stream, tm_x, tm_w, tm_y, tm_r, g);
+    if (BN == 64) return tma_launch_n<64, TM_MMA_BF16>(grid, smem, stream, tm_x, tm_w, tm_y, tm_r, g);
+    if (BN == 128) return tma_launch_n<128, TM_MMA_BF16>(grid, smem, stream, tm_x, tm_w, tm_y, tm_r, g);
+  }
+  return UPSNET_E_UNSUPPORTED;
+}
+
+// Ring depth and output slab pairs for an N tile: the deepest ring that fits (<= TM_MAX_STAGES, >= 2); pair mode: when two
+// alternating output slab pairs leave fewer than four stages (or do not fit at all), one pair buys stages -- the main loop
+// needs the depth more than the epilogue does.
+static bool tma_fit(int BN, bool has_res, bool direct, bool pair, bool res_up2, bool res_inplace, int* stages, int* opairs,
+                    TmaSmem* L) {
+  const uint32_t cap = 227 * 1024 - 1024;
+  auto lay = [&](int st, int op) { return tma_smem_layout(BN, st, has_res, direct, pair, res_up2, res_inplace, op); };
+  int st = TM_MAX_STAGES, op = 2;
+  while (st > 2 && lay(st, op).total > cap) --st;
+  if (pair && !direct && !res_inplace && (st < 4 || lay(st, op).total > cap)) {
+    int st1 = 4;
+    while (st1 > 2 && lay(st1, 1).total > cap) --st1;
+    if (st1 > st || lay(st, op).total > cap) { st = st1; op = 1; }
+  }
+  *stages = st; *opairs = op; *L = lay(st, op);
+  return L->total <= cap;
+}
+
 int launch_igemm_tma(const TcParams& p, const void* packed, cudaStream_t stream) {
   if (p.no_tma || p.offset) return UPSNET_E_UNSUPPORTED;
   // precision bf16 runs on bf16 activations, precision bf16x3 on hi/lo bf16 pairs (same tile pipeline, three MMAs)
@@ -1192,100 +665,32 @@ int launch_igemm_tma(const TcParams& p, const void* packed, cudaStream_t stream)
   g.kw = p.kw; g.KHW = p.kh * p.kw; g.ph = p.ph; g.pw = p.pw; g.dh = p.dh; g.dw = p.dw;
   g.relu = p.relu; g.has_res = p.residual ? 1 : 0; g.res_up2 = p.res_up2 ? 1 : 0; g.sig_from = p.sig_from;
   tma_pick_box(p.N, p.Ho, p.Wo, p.kh, p.kw, p.dh, p.dw, g.res_up2 != 0, &g.bw, &g.bh, &g.bn);
-  // halo mode for k x k filters (UPSNET_TMA_HALO=0 disables it, =2 also enables it for BN = 256): 8 x 16-pixel tiles,
-  // 16-pixel-wide patch rows; the patch must cover 8 + (kw-1)*dw <= 16 pixels per row
-  static int halo_env = -1;
-  if (halo_env < 0) { const char* e = getenv("UPSNET_TMA_HALO"); halo_env = e ? atoi(e) : 1; }
-  const int patch_h = 16 + (p.kh - 1) * p.dh;
-  bool halo = halo_env > 0 && !strided && p.kh * p.kw > 1 && (p.kw - 1) * p.dw <= 8 && patch_h <= 48 && !g.res_up2 &&
-              p.Wo >= 8 && p.Ho >= 8;
-  // pair mode (measured, profiles/r2_mma_probe_pair.md): the patch slots of a hi/lo pair (2 x 36 KB per 3x3 slot) only fit next
-  // to N tiles <= 64, and there the tap-shifted (not 1024-byte aligned) A descriptors make the short N <= 64 MMAs ~2x slower
-  // than the per-tap boxes -- halo mode stays a bf16-stream optimisation (UPSNET_TMA_HALO=3 forces it for pairs)
-  if (pair && halo_env < 3) halo = false;
-  if (halo) { g.bw = 8; g.bh = 16; g.bn = 1; }
   g.tiles_w = (p.Wo + g.bw - 1) / g.bw;
   g.tiles_h = (p.Ho + g.bh - 1) / g.bh;
   g.tiles_n = (p.N + g.bn - 1) / g.bn;
-  long long m_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n;
+  const long long m_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n;
   const int Cout_pad = p.Cout <= 32 ? 32 : (p.Cout + 63) / 64 * 64;      // rows of the packed weight planes (tc_cout_pad)
-  int BN = (Cout_pad % 256 == 0 && !g.has_res) ? 256 : ((Cout_pad % 128 == 0) ? 128 : (Cout_pad % 64 == 0 ? 64 : 32));
-  // pair mode: operand tiles are twice as large -- N tile <= 128, and 64 next to residual slab pairs (shared memory)
+  // N tile <= 128: the accumulators are m64nBN register fragments of two warpgroups (64 floats per thread at 128) and are
+  // staged as 128 x BN fp32 rows in shared memory for the epilogue
+  int BN = (Cout_pad % 128 == 0) ? 128 : (Cout_pad % 64 == 0 ? 64 : 32);
   g.x3 = pair ? 1 : 0; g.x_lo = p.Cin; g.w_lo = Cout_pad; g.pg = pg;
   g.res_inplace = (pair && g.has_res && !g.res_up2) ? 1 : 0;
   g.opairs = 2;
-  if (pair && BN > 128) BN = 128;
-  if (pair && g.has_res && BN > 64) BN = 64;
-  // N tile: as wide as possible (operand bytes per flop fall with BN) while ~2/3 of the SMs still get a tile; measured
-  // on B200 (profiles/r1_bn_sweep.md): 64 m-tiles x Cout 256 -> BN 128 (128 CTAs) beats BN 64 (256 tiles) by 38 %
-  // and BN 256 (64 CTAs) by 11 %; 16 m-tiles x Cout 512 -> BN 64 (128 CTAs) stays best.
-  while (BN > 64 && m_tiles * (Cout_pad / BN) < 96) BN /= 2;
-  (void)sms;
-  if (const char* fb = getenv("UPSNET_TMA_FORCE_BN")) {     // tuning hook (scripts/bn_sweep.py): force the N tile
-    const int v = atoi(fb);
-    if ((v == 64 || v == 128 || v == 256) && Cout_pad % v == 0 && !(g.has_res && v > 128) && !(pair && (v > 128 || (g.has_res && v > 64)))) BN = v;
+  // pair mode: N tile <= 64, i.e. always wide (two wgmma per K slice).  Measured on H100 SXM, bf16x3 bench: the N = 128 tiles
+  // (2-stage ring, one output slab pair) ran the dense conv family in 9.1-9.2 ms per image, N <= 64 in 8.4-8.5 ms.
+  if (pair && BN > 64) BN = 64;
+  // N tile: as wide as possible (operand bytes per flop fall with BN) while ~2/3 of the SMs still get a tile
+  while (BN > 64 && m_tiles * (Cout_pad / BN) < 88) BN /= 2;
+  g.direct = direct ? 1 : 0; g.y_bf16 = p.y_bf16; g.out_nhwc = p.out_nhwc; g.y = p.y;
+  TmaSmem L;
+  bool ok = tma_fit(BN, g.has_res != 0, direct, pair, g.res_up2 != 0, g.res_inplace != 0, &g.stages, &g.opairs, &L);
+  while (!ok && BN > 64) {    // a narrower N tile frees staging and operand space
+    BN /= 2;
+    ok = tma_fit(BN, g.has_res != 0, direct, pair, g.res_up2 != 0, g.res_inplace != 0, &g.stages, &g.opairs, &L);
   }
-  if (halo && BN == 256 && halo_env < 2) {     // wide-N layers are MMA-bound: keep the fewest-tiles box for them
-    halo = false;
-    tma_pick_box(p.N, p.Ho, p.Wo, p.kh, p.kw, p.dh, p.dw, false, &g.bw, &g.bh, &g.bn);
-    g.tiles_w = (p.Wo + g.bw - 1) / g.bw;
-    g.tiles_h = (p.Ho + g.bh - 1) / g.bh;
-    g.tiles_n = (p.N + g.bn - 1) / g.bn;
-    m_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n;
-  }
+  if (!ok) return UPSNET_E_UNSUPPORTED;
   g.BN = BN;
   g.n_tiles = Cout_pad / BN;
-  g.direct = direct ? 1 : 0; g.y_bf16 = p.y_bf16; g.out_nhwc = p.out_nhwc; g.y = p.y;
-  { const char* e = getenv("UPSNET_TMA_DEBUG"); g.dbg = e ? atoi(e) : 0; }
-  { static int rot_env = -1; if (rot_env < 0) { const char* e = getenv("UPSNET_TMA_ROTATE"); rot_env = e ? atoi(e) : 0; } g.rotate = rot_env; }
-  g.halo = halo ? 1 : 0; g.patch_rows = halo ? 16 * patch_h : 0; g.pstages = halo ? 3 : 0; g.kh = p.kh;
-  int stages = TM_MAX_STAGES;
-  TmaSmem L;
-  // resident weights: the n-tile's KHW * Cin/64 weight tiles stay in smem for the life of the (persistent) CTA when they
-  // fit next to >= 2 patch slots -- the 64->64 3x3 bottleneck convs and the 18-channel offset convs of the semantic head
-  g.wres = 0;
-  if (halo && Cout_pad == BN) {
-    const int wtiles = g.KHW * (p.Cin / 64);
-    for (int ps = 4; ps >= 2 && !g.wres; --ps) {
-      L = tma_smem_layout(BN, wtiles, g.has_res != 0, g.patch_rows, ps, direct, pair, g.res_up2 != 0, g.res_inplace != 0, g.opairs);
-      if (L.total + 1024 <= 227 * 1024) { g.wres = 1; g.wtiles = wtiles; g.pstages = ps; stages = 1; }
-    }
-  }
-  if (!g.wres) {
-    const uint32_t cap = 227 * 1024 - 1024;
-    auto lay = [&](int st) { return tma_smem_layout(BN, st, g.has_res != 0, g.patch_rows, g.pstages, direct, pair, g.res_up2 != 0, g.res_inplace != 0, g.opairs); };
-    // deepest ring that fits (<= TM_MAX_STAGES, >= 2); pair mode: if two alternating output slab pairs leave fewer than
-    // four stages, one pair buys another stage -- the main loop needs the depth more than the epilogue does
-    auto fit = [&]() {
-      g.opairs = 2;
-      stages = TM_MAX_STAGES;
-      while (stages > 2 && lay(stages).total > cap) --stages;
-      if (pair && !direct && !g.res_inplace && stages < 4) {
-        g.opairs = 1;
-        int st1 = 4;
-        while (st1 > 2 && lay(st1).total > cap) --st1;
-        if (st1 > stages || lay(stages).total > cap) stages = st1; else g.opairs = 2;
-      }
-      L = lay(stages);
-      return L.total <= cap;
-    };
-    if (pair && halo) g.pstages = 2;       // pair patches are 2 x 36 KB (3x3): two slots, the rest goes to the weight ring
-    bool ok = fit();
-    if (!ok && g.pstages > 2) { g.pstages = 2; ok = fit(); }
-    if (!ok && pair && halo) {
-      // pair mode: the patch slots do not fit next to a weight ring for this N tile -- plain per-tap boxes instead
-      halo = false;
-      g.halo = 0; g.patch_rows = 0; g.pstages = 0;
-      tma_pick_box(p.N, p.Ho, p.Wo, p.kh, p.kw, p.dh, p.dw, g.res_up2 != 0, &g.bw, &g.bh, &g.bn);
-      g.tiles_w = (p.Wo + g.bw - 1) / g.bw;
-      g.tiles_h = (p.Ho + g.bh - 1) / g.bh;
-      g.tiles_n = (p.N + g.bn - 1) / g.bn;
-      m_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n;
-      ok = fit();
-    }
-    if (!ok) return UPSNET_E_UNSUPPORTED;
-  }
-  g.stages = stages;
 
   const int Kp = g.KHW * p.Cin;
   CUtensorMap tm_x, tm_w, tm_y, tm_r;
@@ -1298,9 +703,8 @@ int launch_igemm_tma(const TcParams& p, const void* packed, cudaStream_t stream)
     const cuuint64_t dy[4] = {(cuuint64_t)p.Cout * xm, (cuuint64_t)p.Wo, (cuuint64_t)p.Ho, (cuuint64_t)p.N};
     const cuuint64_t dwt[2] = {(cuuint64_t)Kp, (cuuint64_t)Cout_pad * xm};       // the packed weights ARE [hi plane][lo plane]
     const cuuint32_t box[4] = {64, (cuuint32_t)g.bw, (cuuint32_t)g.bh, (cuuint32_t)g.bn};
-    const cuuint32_t boxp[4] = {64, 16, (cuuint32_t)patch_h, 1};            // halo mode: the input patch of a tile
     const cuuint32_t boxw[2] = {64, (cuuint32_t)BN};
-    if (!encode_bf16(enc, &tm_x, p.x, 4, dx, halo ? boxp : box, sx)) return UPSNET_E_UNSUPPORTED;
+    if (!encode_bf16(enc, &tm_x, p.x, 4, dx, box, sx)) return UPSNET_E_UNSUPPORTED;
     if (!encode_bf16(enc, &tm_w, packed, 2, dwt, boxw)) return UPSNET_E_UNSUPPORTED;
     if (direct) {   // no TMA store / residual in the direct-store epilogue: the two maps are placeholders
       tm_y = tm_x;
@@ -1318,61 +722,9 @@ int launch_igemm_tma(const TcParams& p, const void* packed, cudaStream_t stream)
   }
   const long long num_tiles = m_tiles * g.n_tiles;
   if (num_tiles <= 0) return 0;
-  // ---- 2-CTA variant (cta_group::2): pair stream, per-tap boxes, no residual; each CTA stages half of the weight tile ----
-  static int two_env = -1;
-  if (two_env < 0) { const char* e = getenv("UPSNET_TMA_2CTA"); two_env = e ? atoi(e) : 1; }
-  // measured (profiles/r2_2cta_ab.md): -10..-20 % on the long-K tiles (3x3, FC, 1x1 with Cin >= 512), but the cross-CTA
-  // accumulator hand-shake costs more than the deeper ring buys when a tile has only 1-4 k-blocks (the HBM-bound 1x1 layers
-  // of res2 / res3, +res or not): those keep the 1-CTA kernel.  UPSNET_TMA_2CTA=2 forces the pair kernel everywhere.
-  const int num_kb_h = g.KHW * (p.Cin / 64);
-  if (two_env > 0 && (two_env > 1 || num_kb_h >= 8) && pair && !g.halo && !g.stem && BN >= 32 && m_tiles >= 2 && sms >= 2 &&
-      !(direct && g.has_res)) {
-    const int opairs_1cta = g.opairs;
-    int st2 = TM_MAX_STAGES;
-    g.opairs = 2;
-    static int wide_env = -1;
-    if (wide_env < 0) { const char* e = getenv("UPSNET_TMA_WIDE"); wide_env = e ? atoi(e) : 1; }
-    g.wide = (wide_env > 0 && BN <= 64 && !g.has_res) ? 1 : 0;
-    auto lay2 = [&](int st, int op) { return tma2_smem_layout(BN, st, direct, op, g.has_res != 0, g.res_up2 != 0, g.res_inplace != 0, g.wide != 0); };
-    Tma2Smem L2 = lay2(st2, g.opairs);
-    while (st2 > 2 && L2.total + 1024 > 227 * 1024) { --st2; L2 = lay2(st2, g.opairs); }
-    if (!direct && !g.res_inplace && st2 < 5) {           // one output slab pair buys a stage
-      int st1 = st2;
-      while (st1 < TM_MAX_STAGES && lay2(st1 + 1, 1).total + 1024 <= 227 * 1024) ++st1;
-      if (st1 > st2) { st2 = st1; g.opairs = 1; L2 = lay2(st2, 1); }
-    }
-    if (L2.total + 1024 <= 227 * 1024) {
-      g.stages = st2;
-      CUtensorMap tm_w2;
-      const cuuint64_t dwt2[2] = {(cuuint64_t)Kp, (cuuint64_t)Cout_pad * 2};
-      const cuuint32_t boxw2[2] = {64, (cuuint32_t)(BN / 2)};
-      if (encode_bf16(enc, &tm_w2, packed, 2, dwt2, boxw2)) {
-        static ups::PerDeviceOnce configured2;
-        if (configured2.need()) {
-          UPS_CUDA(cudaFuncSetAttribute(igemm_tma2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        }
-        const long long ctiles = ((m_tiles + 1) / 2) * g.n_tiles;
-        const long long clusters = ctiles < sms / 2 ? ctiles : sms / 2;
-        igemm_tma2_kernel<<<dim3((unsigned)(2 * clusters)), TM_THREADS, L2.total + 1024, stream>>>(tm_x, tm_w2, tm_y, tm_r, g);
-        UPS_CHECK_LAUNCH();
-        return 0;
-      }
-    }
-    g.stages = stages; g.opairs = opairs_1cta; g.wide = 0;     // fall through to the 1-CTA kernel with its own geometry
-  }
-  {   // 1-CTA kernel, pair stream, N tile <= 64, per-tap boxes (incl. the in-place +res layers): two MMAs per K slice
-    static int wide1_env = -1;
-    if (wide1_env < 0) { const char* e = getenv("UPSNET_TMA_WIDE"); wide1_env = e ? atoi(e) : 1; }
-    g.wide = (wide1_env > 0 && pair && BN <= 64 && !g.halo && !g.wres) ? 1 : 0;
-  }
-  static ups::PerDeviceOnce configured;
-  if (configured.need()) {
-    UPS_CUDA(cudaFuncSetAttribute(igemm_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-  }
+  g.wide = pair ? 1 : 0;    // pair stream: two wgmma per K slice (see TmaGeom::wide)
   dim3 grid((unsigned)(num_tiles < sms ? num_tiles : sms));
-  igemm_tma_kernel<<<grid, TM_THREADS, L.total + 1024, stream>>>(tm_x, tm_w, tm_y, tm_r, g);
-  UPS_CHECK_LAUNCH();
-  return 0;
+  return tma_launch(BN, grid, L.total + 1024, stream, tm_x, tm_w, tm_y, tm_r, g);
 }
 
 
@@ -1484,17 +836,11 @@ extern "C" int upsnet_stem_forward(const float* x, const void* packed_w, const f
   g.tiles_w = (Wo + g.bw - 1) / g.bw;
   g.tiles_h = (Ho + g.bh - 1) / g.bh;
   g.tiles_n = (N + g.bn - 1) / g.bn;
-  g.BN = Cout % 256 == 0 ? 256 : (Cout % 128 == 0 ? 128 : 64);
-  if (pair && g.BN > 128) g.BN = 128;
+  g.BN = (Cout % 128 == 0 && !pair) ? 128 : 64;
   g.n_tiles = Cout / g.BN;
-  {   // pair stem, N tile 64: two MMAs per K slice over [W_hi ; W_lo] (see TmaGeom::wide)
-    const char* e = getenv("UPSNET_TMA_WIDE");
-    g.wide = (pair && g.BN <= 64 && (!e || atoi(e) > 0)) ? 1 : 0;
-  }
-  int stages = TM_MAX_STAGES;
-  TmaSmem L = tma_smem_layout(g.BN, stages, false, 0, 0, false, pair, false, false, g.opairs);
-  while (stages > 2 && L.total + 1024 > 227 * 1024) { --stages; L = tma_smem_layout(g.BN, stages, false, 0, 0, false, pair, false, false, g.opairs); }
-  g.stages = stages;
+  g.wide = pair ? 1 : 0;     // pair stem: two wgmma per K slice over [W_hi ; W_lo] (see TmaGeom::wide)
+  TmaSmem L;
+  if (!tma_fit(g.BN, false, false, pair, false, false, &g.stages, &g.opairs, &L)) return UPSNET_E_UNSUPPORTED;
   CUtensorMap tm_x, tm_w, tm_y, tm_lo;
   {
     const cuuint64_t pitch = (cuuint64_t)Wp * 16;
@@ -1519,10 +865,6 @@ extern "C" int upsnet_stem_forward(const float* x, const void* packed_w, const f
                                                              N, Cin, H, W, pad, Hp, Wp);
     UPS_CHECK_LAUNCH();
   }
-  static ups::PerDeviceOnce configured;
-  if (configured.need()) {
-    UPS_CUDA(cudaFuncSetAttribute(igemm_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-  }
   static int sms = 0;
   if (sms == 0) {
     int dev = 0, v = kNumSMs;
@@ -1531,7 +873,5 @@ extern "C" int upsnet_stem_forward(const float* x, const void* packed_w, const f
   }
   const long long num_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n * g.n_tiles;
   dim3 grid((unsigned)(num_tiles < sms ? num_tiles : sms));
-  igemm_tma_kernel<<<grid, TM_THREADS, L.total + 1024, st>>>(tm_x, tm_w, tm_y, pair ? tm_lo : tm_y, g);
-  UPS_CHECK_LAUNCH();
-  return 0;
+  return tma_launch(g.BN, grid, L.total + 1024, st, tm_x, tm_w, tm_y, pair ? tm_lo : tm_y, g);
 }

@@ -1,4 +1,4 @@
-// nms.cu -- device-resident, segmented greedy NMS for sm_100a.
+// nms.cu -- device-resident, segmented greedy NMS for sm_90a.
 //
 // Semantics: nms/nms_kernel.cu:30-38 (devIoU with +1 areas), :77 (suppress IoU > thresh) and
 // the greedy sweep of :130-146 -- which the reference runs on the HOST after a D2H copy of the

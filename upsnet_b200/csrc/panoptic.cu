@@ -1,4 +1,4 @@
-// panoptic.cu -- fused parameter-free panoptic head for sm_100a.
+// panoptic.cu -- fused parameter-free panoptic head for sm_90a.
 //
 // Restates models/resnet_upsnet.py:223-240 of the reference:
 //   MaskRemoval  (operators/modules/mask_removal.py:29-93)  score-ordered overlap pruning
@@ -374,7 +374,7 @@ pan_decide_kernel(int n_max, const int* __restrict__ n_dev, int H, int W, double
     const unsigned int ms = (unsigned int)s_msum[li];
     // mask_removal.py:82: int/int true division (float64) compared with the python float 0.3; decided without the division
     // whenever ov is clear of thr*ms by more than rounding could account for (1e-12 relative >> 2^-52) -- every thread of the
-    // group evaluates the same expression on the same operands (B200 has few fp64 units, but this is 3 flops per thread)
+    // group evaluates the same expression on the same operands (fp64 is slow on the SM, but this is 3 flops per thread)
     bool drop;
     {
       const double t = (double)ms * fraction_threshold, dov = (double)ov;

@@ -1,4 +1,4 @@
-// roi_align.cu -- ROIAlign / FPN-ROIAlign forward for sm_100a.
+// roi_align.cu -- ROIAlign / FPN-ROIAlign forward for sm_90a.
 //
 // Semantics follow operators/src/roi_align_kernel.cu:43-95 (bilinear) and :163-235 (forward)
 // of the reference: no half-pixel shift, roi extent forced >= 1, sampling grid sr x sr,

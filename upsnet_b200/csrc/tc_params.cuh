@@ -1,4 +1,4 @@
-// tc_params.cuh -- launch parameters shared by the tcgen05 convolution kernels and the C-ABI dispatcher.
+// tc_params.cuh -- launch parameters shared by the wgmma convolution kernels and the C-ABI dispatcher.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

@@ -1,5 +1,5 @@
 """resnet_upsnet inference engine: the host-side mirror of upsnet/models/{resnet,fpn,rpn,rcnn,fcn,
-resnet_upsnet}.py running on the sm_100a C ABI.
+resnet_upsnet}.py running on the sm_90a C ABI.
 
 * Same module tree / parameter names as the reference, so its checkpoints load with
   load_state_dict (e.g. resnet_backbone.res3.layers.0.conv2_offset.weight,

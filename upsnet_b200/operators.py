@@ -1,5 +1,5 @@
 """Host-side mirror of the reference's operator API (upsnet/operators/modules/*, upsnet/nms/nms.py)
-on top of the sm_100a C ABI.  Same class names, constructor arguments, parameter names/shapes
+on top of the sm_90a C ABI.  Same class names, constructor arguments, parameter names/shapes
 (so reference checkpoints load) and forward signatures; all compute is in libupsnet_b200.so.
 
 Reference interfaces mirrored (paths relative to /root/reference/upsnet/):
@@ -31,17 +31,17 @@ from ._lib import check, f32c, lib, ptr, require_cuda, stream_ptr
 _PRECISION = {"conv": _lib.PREC_FP32_SIMT}
 ACT_BF16 = {"on": False}   # engine switch: store activations as bf16 (precision 'bf16' only)
 ACT_PAIR = {"on": False}   # engine switch: store activations as hi/lo bf16 pairs (precision 'bf16x3': fp32-grade results)
-# pair-stream deformable convs gather from a shared-memory window with the A operand in TMEM (csrc/dcn_win.cu); maps with fewer
+# pair-stream deformable convs gather from a shared-memory window into shared-memory A tiles (csrc/dcn_win.cu); maps with fewer
 # than min_pixels output pixels keep the global-gather kernel (measured: 0.058 vs 0.048 ms at 32x64, 0.060 vs 0.075 ms at 64x128)
 DCN_WINDOW = {"on": True, "min_pixels": 4096}
 USE_TMA = {"on": True}     # False forces the cp.async gather kernel where the TMA-fed one would qualify (A/B tests)
 
 
 def set_precision(name, bf16_activations=None, pair_activations=None):
-    """'fp32' (CUDA-core fp32 tiles), 'bf16x3' or 'bf16' (tcgen05 tiles).  With 'bf16' the engine also stores
+    """'fp32' (CUDA-core fp32 tiles), 'bf16x3' or 'bf16' (wgmma tiles).  With 'bf16' the engine also stores
     the NHWC activation stream as bf16 (halves HBM traffic; the gather becomes a cp.async copy) unless
     bf16_activations=False.  With 'bf16x3' -- the configuration that meets "fp32 logits within 1e-3" -- the stream is
-    stored as hi/lo bf16 PAIRS (class Pair: same bytes as fp32, ~16 mantissa bits) so that the TMA-fed tcgen05 kernel can
+    stored as hi/lo bf16 PAIRS (class Pair: same bytes as fp32, ~16 mantissa bits) so that the TMA-fed wgmma kernel can
     run the three-term split (hi*hi + lo*hi + hi*lo) without any gather threads; pair_activations=False keeps fp32
     activations and the gather-fed kernel (round-1 behaviour, kept for A/B tests)."""
     _PRECISION["conv"] = {"fp32": _lib.PREC_FP32_SIMT, "bf16x3": _lib.PREC_BF16X3, "bf16": _lib.PREC_BF16}[name]
@@ -141,7 +141,7 @@ def _conv_out(n, pad, dil, k, stride):
 
 
 # ------------------------------------------------------------------------------------------------
-# tensor-core (tcgen05) path plumbing: NHWC views and the packed-weight cache
+# tensor-core (wgmma) path plumbing: NHWC views and the packed-weight cache
 # ------------------------------------------------------------------------------------------------
 def _nhwc(x):
     """[N,C,H,W] logical tensor -> contiguous [N,H,W,C] storage (no copy if already channels_last)."""
@@ -202,8 +202,7 @@ def _packed_weight_dcn(weight):
 
 
 # small-N dense 3x3 / stride-1 convs on the pair stream through the window pipeline (csrc/dcn_win.cu DENSE mode): Cout <= max_cout
-# measured on B200 (scripts/exp_offset_conv.py): 0.18 vs 0.15 ms for the 256->18 offset conv at 256x512 -- the 32-byte rows of the
-# window boxes run into the TMA request rate (~4-5 cycles per box row and SM) -> off by default, kept for the record / tests
+# off by default: the per-tap TMA boxes of the dense conv kernel serve these layers; kept as an entry point and for the tests
 DENSE_WINDOW = {"on": False, "max_cout": 64, "min_pixels": 4096}
 
 
@@ -398,7 +397,7 @@ def _igemm_tc(kind, x, offset, mask, weight, bias, residual, stride, padding, di
 def conv2d(x, weight, bias=None, stride=1, padding=0, dilation=1, residual=None, relu=False, precision=None,
            out_format=None, out_dtype=None, residual_up2=False, pair_group=0, sigmoid_from=None):
     """Dense conv + fused bias / residual / ReLU epilogue.  fp32 precision -> upsnet_conv2d_forward
-    (NCHW CUDA-core tiles); bf16x3 / bf16 -> upsnet_igemm_forward (tcgen05 tiles, NHWC storage)."""
+    (NCHW CUDA-core tiles); bf16x3 / bf16 -> upsnet_igemm_forward (wgmma tiles, NHWC storage)."""
     require_cuda(x, weight, bias, residual)
     prec = _PRECISION["conv"] if precision is None else precision
     if prec != _lib.PREC_FP32_SIMT and _tc_ok(weight.shape[1], weight.shape[2], weight.shape[3], 1):

@@ -1,12 +1,12 @@
 """Training-side pieces of the hot path (BASELINE config #4: UPSNet-50 end2end_train, bf16, 8 GPUs, NCCL all-reduce):
 
-* autograd Functions for the custom operators with hand-written sm_100a BACKWARD kernels (csrc/backward.cu):
+* autograd Functions for the custom operators with hand-written sm_90a BACKWARD kernels (csrc/backward.cu):
     DeformConvFunction / ModDeformConvFunction   operators/functions/deform_conv.py:26-108, mod_deform_conv.py:25-118
     RoIAlignFunction                             operators/functions/roialign.py:21-58
   The dense GEMMs of the deformable backward (d(weight) = dY col^T, d(col) = W^T dY) are library calls (torch.mm), like the
   reference's; the gather / scatter / coordinate-gradient kernels are ours.
 * FlatBucketAllReduce: the gradient all-reduce of `upsnet_end2end_train.py:121` (hvd.DistributedOptimizer) as flat bf16
-  buckets over torch.distributed (NCCL over NVLink on the B200 box, gloo in the CPU tests): gradients are packed per bucket,
+  buckets over torch.distributed (NCCL between the GPUs, gloo in the CPU tests): gradients are packed per bucket,
   reduced asynchronously while the rest of backward runs, averaged and unpacked before the optimiser step.
 
 Scope note: this is the operator / communication layer of the training configuration.  Losses, target assignment and the
@@ -125,13 +125,13 @@ class RoIAlignFunction(torch.autograd.Function):
 
 
 # ------------------------------------------------------------------------------------------------
-# gradient all-reduce (config #4: "bf16, 8xB200, NCCL allreduce over NVLink")
+# gradient all-reduce (config #4: "bf16, NCCL allreduce")
 # ------------------------------------------------------------------------------------------------
 class FlatBucketAllReduce:
     """Averages the gradients of `params` over the process group through flat buckets.
 
     * buckets are filled in REVERSE parameter order (the order backward produces gradients), `bucket_bytes` each;
-    * `reduce_dtype` (bf16 on the NCCL path: half the NVLink bytes; the accumulation of 8 ranks in bf16 costs ~3 bits, the
+    * `reduce_dtype` (bf16 on the NCCL path: half the interconnect bytes; the accumulation of 8 ranks in bf16 costs ~3 bits, the
       configuration BASELINE.json names) -- gradients are packed with a cast, reduced with SUM, and unpacked with 1/world;
     * `start()` launches every bucket's all_reduce asynchronously (NCCL: on its own stream, overlapping the optimiser's
       host work and, when called from autograd hooks, the rest of backward); `finish()` waits and writes p.grad back.
