@@ -169,6 +169,11 @@ int upsnet_dcn_pack_weight(const float *weight, int Cout, int Cin, int kh, int k
 int upsnet_dcn_pair_forward(const void *x_pair, const float *offset, const float *mask, const void *packed,
                             const float *bias, void *y_pair, int N, int H, int W, int Cin, int Cout, int kh, int kw,
                             int pad_h, int pad_w, int dil_h, int dil_w, int epi_flags, void *stream);
+/* Tuning hook of upsnet_dcn_pair_forward: output-channel tile of the following launches in this process.  0 (default) =
+ * chosen per launch (128 when Cout is a multiple of 128 and the layer has at least a quarter as many 16x8-pixel tiles as
+ * the GPU has SMs, else 32); 32 or 128 = that tile wherever it applies (128 needs Cout rounded up to 64 to be a multiple of 128).  Results are
+ * the same for every choice.  UPSNET_E_BADARG for other values. */
+int upsnet_dcn_set_tile_n(int bn);
 /* Dense 3x3 / stride-1 convolution on hi/lo PAIR activations through the same window pipeline (csrc/dcn_win.cu, DENSE mode):
  * the input window of a 16x8-pixel tile is staged once per 16-channel sub-chunk by TMA and feeds all nine taps, the A operand
  * is copied window -> A operand tile in shared memory.  Meant for the small-N layers (18-channel offset convs of the semantic head, 64->64 bottleneck

@@ -1,5 +1,7 @@
 """Timing / ncu driver for the window-staged deformable conv on pairs (csrc/dcn_win.cu) next to the global-gather kernel.
-  python scripts/prof_dcn_win.py            -> CUDA-event timings of both kernels for several offset distributions
+  python scripts/prof_dcn_win.py            -> CUDA-event timings for several offset distributions: the window kernel with
+                                               N tile 128 and 32 (forced; "-" where 128 does not apply) and as chosen per
+                                               launch, and the global-gather kernel; algorithmic TFLOP/s (one pass)
   ncu --set full --clock-control none --import-source on -k regex:dcn_win -s 2 -c 1 python scripts/prof_dcn_win.py ncu
 """
 import os, sys
@@ -7,6 +9,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import upsnet_b200 as U
 from upsnet_b200 import operators as ops
+from upsnet_b200._lib import lib
 from upsnet_b200.operators import Pair
 dev = torch.device("cuda", 0)
 torch.manual_seed(0)
@@ -43,7 +46,8 @@ def gpu_ms(fn, iters=10):
     return e0.elapsed_time(e1) / iters
 
 
-shapes = [(256, 128, 256, 512), (128, 128, 256, 512), (256, 128, 128, 256), (256, 128, 64, 128), (256, 128, 32, 64)]
+shapes = [(256, 128, 256, 512), (128, 128, 256, 512), (256, 128, 128, 256), (256, 128, 64, 128), (256, 128, 32, 64),
+          (256, 256, 100, 168), (512, 512, 50, 84)]
 if len(sys.argv) > 1 and sys.argv[1] == "ncu":
     x, w = act(1, 256, 256, 512), wgt(128, 256, 3)
     off = offsets(sys.argv[2] if len(sys.argv) > 2 else "tapbias", 256, 512)
@@ -51,14 +55,25 @@ if len(sys.argv) > 1 and sys.argv[1] == "ncu":
         U.deform_conv(x, off, w, None, 1, 1, 1, relu=True)
     torch.cuda.synchronize()
     sys.exit(0)
+def window_ms(bn, fn):
+    assert lib().upsnet_dcn_set_tile_n(bn) == 0
+    try:
+        return gpu_ms(fn)
+    finally:
+        lib().upsnet_dcn_set_tile_n(0)
+
+
 for cin, cout, h, w_ in shapes:
     x, w = act(1, cin, h, w_), wgt(cout, cin, 3)
+    fl = 2.0 * h * w_ * cout * cin * 9
     for kind in ("zero", "small", "tapbias", "rand1.5", "rand4"):
         off = offsets(kind, h, w_)
+        run = lambda: U.deform_conv(x, off, w, None, 1, 1, 1, relu=True)
         ops.DCN_WINDOW["on"] = True
-        a = gpu_ms(lambda: U.deform_conv(x, off, w, None, 1, 1, 1, relu=True))
+        t = {bn: window_ms(bn, run) for bn in (128, 32, 0)}
         ops.DCN_WINDOW["on"] = False
-        b = gpu_ms(lambda: U.deform_conv(x, off, w, None, 1, 1, 1, relu=True))
+        g = gpu_ms(run)
         ops.DCN_WINDOW["on"] = True
-        fl = 2.0 * h * w_ * cout * cin * 9
-        print("Cin%d->%d @%dx%d off=%-8s window %.3f ms (%.0f TF/s algo)   global-gather %.3f ms" % (cin, cout, h, w_, kind, a, fl / a / 1e9, b), flush=True)
+        wide = "  N128 %.3f ms (%4.0f TF/s)" % (t[128], fl / t[128] / 1e9) if cout % 128 == 0 else "  N128 -"
+        print("Cin%d->%d @%dx%d off=%-8s%s  N32 %.3f ms (%4.0f TF/s)  auto %.3f ms   global-gather %.3f ms"
+              % (cin, cout, h, w_, kind, wide, t[32], fl / t[32] / 1e9, t[0], g), flush=True)

@@ -17,12 +17,20 @@
 // outside the window (large offsets) are flagged in the per-tile sample table and gathered from global memory by the
 // same thread, so the result never depends on the window size -- only the speed does.
 //
-// Warp roles (22 warps): 0-3 consumers (one warpgroup: per K=16 slice three wgmma pairs -- lo*hi, hi*lo, hi*hi for tile
-// rows 0-63 and 64-127 -- accumulators in registers, then staged through shared memory -> bias / ReLU -> hi/lo split ->
-// NHWC pair stores, thread = tile pixel), 4 weight TMA, 5 window TMA, 6-21 gather producers in two groups that fill
-// alternate k-blocks.
-// Roofline: tensor pipe (2*P*Cout*Cin*9 flop x 3 passes); per k-block and SM the gather costs ~4 K warp instructions
-// and 128 KB of shared-memory reads against 12 MMAs of 128x128x16 -- see DESIGN.md section 4.
+// Two instantiations, chosen per launch (DwCfg below):
+//   N tile 128 (semantic head, res3-5 DCN): 20 warps.  0-7 consumers (two warpgroups, tile rows 0-63 / 64-127, one
+//     m64n128 fragment per thread; per K=16 slice three wgmma -- lo*hi, hi*lo, hi*hi), 8 weight TMA, 9 window TMA,
+//     10-11 idle, 12-19 gather producers.  K = 32 per stage (SWIZZLE_64B), three stages.  The A tile is gathered once
+//     per 128 output channels.
+//   N tile 32 (small maps, Cout not a multiple of 128, DENSE mode): 24 warps.  0-3 consumers (one warpgroup holding both
+//     m64n32 fragments), 4 weight TMA, 5 window TMA, 6-7 idle, 8-23 gather producers.  K = 64 per stage (SWIZZLE_128B).
+//   The TMA warps and the idle ones form a warpgroup that hands registers to the consumers (setmaxnreg, DwCfg).
+// In both, a producer warp gathers two K=16 slices of 32 tile rows per k-block, and the producers form two groups that
+// fill alternate k-blocks.  After the last k-block of a tile each consumer warpgroup stages its accumulators through
+// shared memory (32 columns at a time) -> bias / ReLU -> hi/lo split -> NHWC pair stores, thread = tile pixel.
+// Every output element sums the same K=16 slices in the same order in both instantiations.
+// Roofline: tensor pipe (2*P*Cout*Cin*9 flop x 3 passes); per 64 K and SM the gather costs ~4 K warp instructions and
+// 128 KB of shared-memory reads -- per 128 output channels at N = 128, per 32 at N = 32 -- see DESIGN.md section 4.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cstdlib>
@@ -34,22 +42,50 @@
 namespace ups {
 
 constexpr int DW_BM = 128;            // pixels per M tile
-constexpr int DW_BK = 64;             // K elements per k-block = 4 slices of 16 channels
 constexpr int DW_STAGES = 3;          // operand ring depth: A stages (gather warps) and B stages (TMA), both in smem
 constexpr int DW_WW = 32, DW_WH = 20; // window box in pixels; the row pitch (32 px = 1024 B) keeps bank = f(x) only
 constexpr int DW_PLANE = DW_WW * DW_WH * 32;      // one plane (hi or lo) of a window: 16 channels x 2 B per pixel
 constexpr int DW_WIN_BYTES = 2 * DW_PLANE;
 constexpr int DW_KHW = 9;
-constexpr int DW_GROUP = 256, DW_GROUPS = 2, DW_PRODUCERS = DW_GROUP * DW_GROUPS;
-constexpr int DW_CONSUMERS = 128, DW_WARP_TMAB = 4, DW_WARP_TMAW = 5, DW_WARP_PROD0 = 6;
-constexpr int DW_THREADS = (DW_WARP_PROD0 + DW_PRODUCERS / 32) * 32;   // 704
-// N tile: the two m64 accumulator fragments of a consumer thread (DW_BN floats) have to fit next to the addressing in the
-// registers 22 warps per SM leave (ptxas -v: 80 used per thread).  Measured on H100 SXM (400 W), bf16x3 bench: N = 32 runs the semantic head's deformable convs in
-// 6.2 ms per image, N = 64 (fragments spilled to local memory) in 15.6 ms.
-constexpr int DW_BN = 32;
-constexpr uint32_t DW_A_BYTES = 2 * DW_BM * 128;   // A stage: hi tile, lo tile (128 rows x 64 bf16, SWIZZLE_128B)
+constexpr int DW_GROUPS = 2;          // producer groups: alternate k-blocks
 constexpr int DW_EPI_PITCH = 36;      // floats per row of the accumulator staging buffer (32 columns + pad)
 constexpr uint32_t DW_EPI_BYTES = DW_BM * DW_EPI_PITCH * 4;
+
+// Per-instantiation geometry.  N tile 32: one consumer warpgroup holds both m64 fragments (2 x 16 floats) next to 16
+// gather warps.  N tile 128: an m64n128 fragment is 64 floats per thread, so each tile half gets its own consumer
+// warpgroup and the gather runs on 8 warps (16 gather warps would leave the consumers too few registers); its stages
+// hold K = 32 so that three of them, two windows and the staging buffer fit in 227 KB of shared memory.
+template <int BN> struct DwCfg {
+  static constexpr int NCW = BN == 128 ? 2 : 1;                  // consumer warpgroups
+  static constexpr int FRAGS = 2 / NCW;                          // m64 accumulator fragments per consumer thread
+  static constexpr int BK = BN == 128 ? 32 : 64;                 // K elements per k-block
+  static constexpr int SPK = BK / 16;                            // K=16 slices per k-block
+  static constexpr int ROWB = BK * 2;                            // bytes of one A / B row in a stage (= swizzle span)
+  static constexpr int CONSUMERS = 128 * NCW;
+  // one warpgroup for the two TMA warps (and two idle warps), so that setmaxnreg can move its registers to the consumers
+  static constexpr int WARP_TMAB = CONSUMERS / 32, WARP_TMAW = WARP_TMAB + 1, WARP_PROD0 = WARP_TMAB + 4;
+  static constexpr int GROUP = 4 * (SPK / 2) * 32;                // producer threads per group: 4 row quadrants x SPK/2
+  static constexpr int PRODUCERS = GROUP * DW_GROUPS;
+  static constexpr int THREADS = WARP_PROD0 * 32 + PRODUCERS;     // 768 (N = 32), 640 (N = 128)
+  // registers per thread: the launch budget (80 for 24 warps, 96 for 20: 16 K registers per SM sub-partition) stays
+  // with the producers; the TMA warpgroup drops to REGS_TMA and the consumer warpgroups take what it frees.  setmaxnreg
+  // moves registers inside the CTA's own allocation, so the warpgroup budgets must add up to what the launch gave.
+  // ptxas -v: no spills in either instantiation (N = 128: 64 accumulators per consumer thread).
+  static constexpr int WARPGROUPS = THREADS / 128;
+  static constexpr int REGS_LAUNCH = 16384 / (32 * ((THREADS / 32 + 3) / 4)) / 8 * 8;
+  static constexpr int REGS_TMA = 32, REGS_CONSUMER = 128;
+  static_assert(NCW * REGS_CONSUMER + REGS_TMA + (PRODUCERS / 128) * REGS_LAUNCH <= WARPGROUPS * REGS_LAUNCH,
+                "setmaxnreg budgets exceed the CTA's register allocation");
+  static constexpr int TABLE_IT = (DW_KHW * DW_BM + PRODUCERS - 1) / PRODUCERS;   // sample-table entries per producer
+  static constexpr uint32_t A_BYTES = 2 * DW_BM * ROWB;          // A stage: hi tile, lo tile (128 rows x BK bf16)
+  static constexpr uint32_t B_BYTES = BN * ROWB;                 // one weight plane of a stage
+  static constexpr uint32_t STAGE_BYTES = 2 * B_BYTES + A_BYTES;
+  static_assert(STAGE_BYTES % 1024 == 0, "stages must keep the 1024-byte alignment of the swizzled tiles");
+};
+// 16-byte chunk j of A / B row r in a stage: SWIZZLE_128B (128-byte rows) or SWIZZLE_64B (64-byte rows)
+template <int ROWB> __device__ __forceinline__ uint32_t dw_chunk(uint32_t j, uint32_t r) {
+  return ROWB == 128 ? (j ^ (r & 7u)) : (j ^ ((r >> 1) & 3u));
+}
 
 // shared-memory map (byte offsets from the 1024-aligned base)
 constexpr uint32_t DW_OFF_BARS = 0;        // 18 mbarriers
@@ -105,28 +141,35 @@ __device__ __forceinline__ uint4 dw_lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
 }
-__device__ __forceinline__ void dw_producer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(DW_PRODUCERS) : "memory"); }
+template <int R> __device__ __forceinline__ void dw_setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void dw_setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int N> __device__ __forceinline__ void dw_producer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(N) : "memory"); }
 
-__global__ void __launch_bounds__(DW_THREADS, 1)
+template <int BN>
+__global__ void __launch_bounds__(DwCfg<BN>::THREADS, 1)
 dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const DwParams p) {
+  using C = DwCfg<BN>;
+  constexpr int DW_PRODUCERS = C::PRODUCERS, DW_CONSUMERS = C::CONSUMERS;
+  constexpr int DW_WARP_TMAB = C::WARP_TMAB, DW_WARP_TMAW = C::WARP_TMAW, DW_WARP_PROD0 = C::WARP_PROD0;
+  constexpr int DW_BK = C::BK, SPK = C::SPK, ROWB = C::ROWB;
   extern __shared__ __align__(1024) uint8_t smem_dyn[];
   const uint32_t raw = smem_u32(smem_dyn);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* sm = smem_dyn + (base - raw);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t b_bytes = (uint32_t)DW_BN * 128;
-  const uint32_t stage_bytes = 2 * b_bytes + DW_A_BYTES;                    // weight tile (hi, lo planes), then the A tiles
+  const uint32_t b_bytes = C::B_BYTES;
+  const uint32_t stage_bytes = C::STAGE_BYTES;                              // weight tile (hi, lo planes), then the A tiles
   const uint32_t NST = (uint32_t)p.stages;
   const uint32_t win_base = base + DW_OFF_STAGES + NST * stage_bytes;       // 1024-aligned (stage_bytes % 1024 == 0)
   const uint32_t NWB = (uint32_t)p.win_nbuf;
   float* stf = reinterpret_cast<float*>(sm + (win_base - base) + NWB * (uint32_t)p.win_buf);   // accumulator staging
   // barriers
-  const uint32_t bar_fa = base + DW_OFF_BARS;            // full_a[3]: 8 producer warps each (A stage written)
+  const uint32_t bar_fa = base + DW_OFF_BARS;            // full_a[3]: the producer warps of one group (A stage written)
   const uint32_t bar_fb = bar_fa + 24;                   // full_b[3]: weight TMA (tx)
-  const uint32_t bar_em = bar_fa + 48;                   // empty[3]: 4 consumer warps (their wgmmas have read A and B)
+  const uint32_t bar_em = bar_fa + 48;                   // empty[3]: every consumer warp (its wgmmas have read A and B)
   const uint32_t bar_wf = bar_fa + 104;                  // win_full[2]: window TMA (tx)
-  const uint32_t bar_we = bar_fa + 120;                  // win_empty[2]: 16 producer warps
+  const uint32_t bar_we = bar_fa + 120;                  // win_empty[2]: every producer warp
   const uint32_t bar_og = bar_fa + 136;                  // org_full[2]: window origin of a tile published
   int* stats = reinterpret_cast<int*>(sm + DW_OFF_STATS);
   int4* org = reinterpret_cast<int4*>(sm + DW_OFF_ORG);
@@ -137,8 +180,8 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
   const int nsc = p.Cin / 16;                         // 16-channel sub-chunks
   const int spf = p.dense ? 4 : 1;                    // sub-chunks per window fill
   const int nfill = nsc / spf;                        // window fills per tile
-  const int num_kb = nsc * DW_KHW / 4;                // Cin % 64 == 0 -> integral
-  const int n_tiles = p.Cout_pad / DW_BN;
+  const int num_kb = nsc * DW_KHW / SPK;              // Cin % 64 == 0 -> integral
+  const int n_tiles = p.Cout_pad / BN;
   const int TW = p.tile_w, TH = p.tile_h;
   const int tw_shift = TW == 16 ? 4 : 3;
   const int tiles_w = (p.Wo + TW - 1) / TW, tiles_h = (p.Ho + TH - 1) / TH;
@@ -147,7 +190,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
   if (warp == 0) {
     if (lane == 0) {
       for (int s = 0; s < DW_STAGES; ++s) {
-        mbar_init(bar_fa + 8 * s, DW_GROUP / 32);
+        mbar_init(bar_fa + 8 * s, C::GROUP / 32);
         mbar_init(bar_fb + 8 * s, 1);
         mbar_init(bar_em + 8 * s, DW_CONSUMERS / 32);
       }
@@ -176,10 +219,10 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     // TMA with SWIZZLE_32B (16-byte chunk ^= address bit 7, i.e. pixel bit 2), so eight horizontally consecutive pixels of
     // one half occupy eight different 16-byte bank groups: a quarter-warp wavefront is conflict-free whenever its samples
     // stay on consecutive pixels of any rows (row pitch 1024 B).
-    const int pt = tid - DW_WARP_PROD0 * 32;     // 0..511: sample-table work is spread over all producer threads
-    const int pw = warp - DW_WARP_PROD0;         // 0..15
-    const int group = pw >> 3;                   // alternate k-blocks
-    const int u = (pw >> 2) & 1;                 // which two of the k-block's four slices this warp gathers
+    const int pt = tid - DW_WARP_PROD0 * 32;     // sample-table work is spread over all producer threads
+    const int pw = warp - DW_WARP_PROD0;
+    const int group = pw / (C::GROUP / 32);      // alternate k-blocks
+    const int u = (pw >> 2) & (SPK / 2 - 1);     // which two of the k-block's slices this warp gathers
     const int quad = pw & 3;                     // A rows [32 quad, 32 quad + 32)
     const int r = quad * 32 + lane;              // A row = tile pixel
     const __nv_bfloat16* xh = reinterpret_cast<const __nv_bfloat16*>(p.x);
@@ -195,20 +238,21 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         const int ry = min(rr >> tw_shift, TH - 1), rx = rr & (TW - 1);      // rows past the block read a valid (unused) pixel
         tp[e] = (ry + ki * p.dh) * p.win_pitch + rx + kj * p.dw;      // window PIXEL index
       }
-      dw_producer_bar();
+      dw_producer_bar<DW_PRODUCERS>();
     }
     for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tile_it) {
       const long long mt = tile / n_tiles;
       const int tx = (int)(mt % tiles_w), ty = (int)((mt / tiles_w) % tiles_h), n = (int)(mt / ((long long)tiles_w * tiles_h));
       const int par = (int)(tile_it & 1u);
       if (!dense) {
-      // ---- sample table, phase 1: every thread computes up to three (tap, pixel) entries in registers ----
-      float4 ewv[3];
-      int ehl[3], ewl[3];
-      bool evalid[3];
+      // ---- sample table, phase 1: every thread computes up to TABLE_IT (tap, pixel) entries in registers ----
+      constexpr int TIT = C::TABLE_IT;
+      float4 ewv[TIT];
+      int ehl[TIT], ewl[TIT];
+      bool evalid[TIT];
       int mnw = 0x7fffffff, mnh = 0x7fffffff, mxw = -0x7fffffff, mxh = -0x7fffffff, sw_ = 0, sh_ = 0, cnt = 0;
 #pragma unroll
-      for (int it = 0; it < 3; ++it) {
+      for (int it = 0; it < TIT; ++it) {
         const int e = pt + it * DW_PRODUCERS;
         ewv[it] = make_float4(0.f, 0.f, 0.f, 0.f);
         ehl[it] = 0; ewl[it] = 0; evalid[it] = false;
@@ -249,7 +293,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         atomicMin(st + 0, mnw); atomicMin(st + 1, mnh); atomicMax(st + 2, mxw); atomicMax(st + 3, mxh);
         atomicAdd(st + 4, sw_); atomicAdd(st + 5, sh_); atomicAdd(st + 6, cnt);
       }
-      dw_producer_bar();      // (B) statistics complete; every producer has also finished the previous tile's gather
+      dw_producer_bar<DW_PRODUCERS>();      // (B) statistics complete; every producer has also finished the previous tile's gather
       // ---- window origin (same integer arithmetic in every thread), table phase 2 ----
       int ox = 0, oy = 0;
       {
@@ -263,7 +307,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         }
       }
 #pragma unroll
-      for (int it = 0; it < 3; ++it) {
+      for (int it = 0; it < TIT; ++it) {
         const int e = pt + it * DW_PRODUCERS;
         if (e < DW_KHW * DW_BM) {
           int code = 0;
@@ -282,7 +326,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         so[0] = 0x7fffffff; so[1] = 0x7fffffff; so[2] = -0x7fffffff; so[3] = -0x7fffffff; so[4] = 0; so[5] = 0; so[6] = 0;
         mbar_arrive(bar_og + 8 * par);        // release: the window TMA thread may read the origin
       }
-      dw_producer_bar();      // (C) table visible
+      dw_producer_bar<DW_PRODUCERS>();      // (C) table visible
       }                       // !dense
       const __nv_bfloat16* ximg = xh + (size_t)n * p.H * p.W * (size_t)(2 * p.Cin);
 
@@ -291,12 +335,12 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         const uint32_t g = g0 + (uint32_t)kb;
         const uint32_t s = g % NST, it = g / NST;
         mbar_wait(bar_em + 8 * s, (it & 1u) ^ 1u);
-        // A stage s: hi tile then lo tile, row r = 128 bytes, 16-byte chunk j of K at (j ^ (r & 7)) (SWIZZLE_128B)
-        const uint32_t a_row = base + DW_OFF_STAGES + s * stage_bytes + 2 * b_bytes + (uint32_t)r * 128u;
+        // A stage s: hi tile then lo tile, row r = ROWB bytes, 16-byte chunk j of K at dw_chunk(j, r)
+        const uint32_t a_row = base + DW_OFF_STAGES + s * stage_bytes + 2 * b_bytes + (uint32_t)r * (uint32_t)ROWB;
 #pragma unroll 1
         for (int pass = 0; pass < 4; ++pass) {
           const int sl = 2 * u + (pass >> 1), half = pass & 1;
-          const int q = kb * 4 + sl;                    // slice index: (sub-chunk, tap)
+          const int q = kb * SPK + sl;                  // slice index: (sub-chunk, tap)
           const int sc = q / DW_KHW, tap = q - sc * DW_KHW;
           const uint32_t wf = wf0 + (uint32_t)(dense ? (sc >> 2) : sc);      // dense: one fill per 64-channel chunk
           if (wf >= wf_ready) {                         // first touch of this window fill
@@ -305,14 +349,14 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
           }
           const uint32_t wbuf = win_base + (wf % NWB) * (uint32_t)p.win_buf;
           const int code = tp[tap * DW_BM + r];
-          const uint32_t a_off = (((uint32_t)(sl * 2 + half) ^ (uint32_t)(r & 7)) << 4);   // K elements 16 sl + 8 half ..
+          const uint32_t a_off = dw_chunk<ROWB>((uint32_t)(sl * 2 + half), (uint32_t)r) << 4;   // K elements 16 sl + 8 half ..
           if (dense) {        // plain copy of the tap's pixel: window -> A operand
             // SWIZZLE_128B window: a pixel is one 128-byte row (64 channels), 16-byte chunk c sits at c ^ (pixel & 7)
             const uint32_t pix = (uint32_t)code, ch = (uint32_t)((sc & 3) * 2 + half);
             const uint32_t al = wbuf + pix * 128u + ((ch ^ (pix & 7u)) << 4);
             const uint4 h4 = dw_lds128(al), l4 = dw_lds128(al + (uint32_t)p.win_plane);
             sts128(a_row + a_off, h4);
-            sts128(a_row + DW_BM * 128u + a_off, l4);
+            sts128(a_row + DW_BM * ROWB + a_off, l4);
             continue;
           }
           const float4 wv = tw[tap * DW_BM + r];
@@ -375,14 +419,14 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
             olo[qq] = pack_bf16x2(v0 - __uint_as_float(ohi[qq] << 16), v1 - __uint_as_float(ohi[qq] & 0xffff0000u));
           }
           sts128(a_row + a_off, make_uint4(ohi[0], ohi[1], ohi[2], ohi[3]));
-          sts128(a_row + DW_BM * 128u + a_off, make_uint4(olo[0], olo[1], olo[2], olo[3]));
+          sts128(a_row + DW_BM * ROWB + a_off, make_uint4(olo[0], olo[1], olo[2], olo[3]));
         }
         fence_proxy_async();    // generic-proxy stores -> visible to wgmma (async proxy)
         __syncwarp();
         if (lane == 0) {
           mbar_arrive(bar_fa + 8 * s);
-          // window buffers this warp will not read again: its next k-block (kb + 2) starts at slice 4 * (kb + 2)
-          while (rel < nfill && DW_KHW * spf * (rel + 1) <= 4 * (kb + DW_GROUPS)) {
+          // window buffers this warp will not read again: its next k-block (kb + 2) starts at slice SPK * (kb + 2)
+          while (rel < nfill && DW_KHW * spf * (rel + 1) <= SPK * (kb + DW_GROUPS)) {
             mbar_arrive(bar_we + 8 * ((wf0 + (uint32_t)rel) % NWB));
             ++rel;
           }
@@ -396,9 +440,12 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
       g0 += (uint32_t)num_kb;
       wf0 += (uint32_t)nfill;
     }
-  } else if (warp == DW_WARP_TMAW) {
+  } else if (warp >= DW_WARP_TMAB) {
+    // The TMA warpgroup (weight TMA, window TMA, two idle warps) keeps a minimal register budget so that the consumer
+    // warpgroups can raise theirs.
+    dw_setmaxnreg_dec<C::REGS_TMA>();
+    if (warp == DW_WARP_TMAW && lane == 0) {
     // =============================== WINDOW TMA ===============================
-    if (lane == 0) {
       uint32_t wf = 0, ti = 0;
       for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++ti) {
         const uint32_t par = ti & 1u;
@@ -422,14 +469,11 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
           dw_tma_4d(dst + (uint32_t)p.win_plane, &tm_x, bar_wf + 8 * b, p.Cin + f * cstep, o.x, o.y, o.z);
         }
       }
-    }
-    __syncwarp();
-  } else if (warp == DW_WARP_TMAB) {
-    // =============================== WEIGHT TMA ===============================
-    if (lane == 0) {
+    } else if (warp == DW_WARP_TMAB && lane == 0) {
+      // =============================== WEIGHT TMA ===============================
       uint32_t g = 0;
       for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int n0 = (int)(tile % n_tiles) * DW_BN;
+        const int n0 = (int)(tile % n_tiles) * BN;
         for (int kb = 0; kb < num_kb; ++kb, ++g) {
           const uint32_t s = g % NST, it = g / NST;
           mbar_wait(bar_em + 8 * s, (it & 1u) ^ 1u);
@@ -442,15 +486,19 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     }
     __syncwarp();
   } else {
-    // =============================== CONSUMERS (warps 0-3) ===============================
-    const uint32_t dhi = wg_desc_hi(1024);
-    float d0[DW_BN / 2], d1[DW_BN / 2];                   // tile rows [0, 64) and [64, 128)
-    constexpr uint32_t h16 = 64u * 128u / 16u;      // rows 64-127: 64 rows of 128 bytes further
+    // =============================== CONSUMERS (warpgroups 0 .. NCW-1) ===============================
+    dw_setmaxnreg_inc<C::REGS_CONSUMER>();
+    // Warpgroup wg owns m64 fragment f (tile rows [64 (wg FRAGS + f), +64)) for f < FRAGS.
+    constexpr int FRAGS = C::FRAGS;
+    const int wg = warp >> 2;
+    const uint32_t dhi = ROWB == 128 ? wg_desc_hi(8 * ROWB) : wg_desc_hi_sw64(8 * ROWB);
+    float d[FRAGS][BN / 2];
+    constexpr uint32_t h16 = 64u * ROWB / 16u;      // the next 64 tile rows: 64 rows of ROWB bytes further
     __nv_bfloat16* yb = reinterpret_cast<__nv_bfloat16*>(p.y);
     uint32_t s = 0, ph = 0;
     for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const long long mt = tile / n_tiles;
-      const int n0 = (int)(tile % n_tiles) * DW_BN;
+      const int n0 = (int)(tile % n_tiles) * BN;
       const int tx = (int)(mt % tiles_w), ty = (int)((mt / tiles_w) % tiles_h), n = (int)(mt / ((long long)tiles_w * tiles_h));
       int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
@@ -458,50 +506,55 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         mbar_wait(bar_fa + 8 * s, ph);
         const uint32_t st0 = base + DW_OFF_STAGES + s * stage_bytes;
         const uint32_t b_hi = wg_desc_lo(st0), b_lo = wg_desc_lo(st0 + b_bytes);
-        const uint32_t a_hi = wg_desc_lo(st0 + 2 * b_bytes), a_lo = wg_desc_lo(st0 + 2 * b_bytes + DW_BM * 128u);
+        const uint32_t a_hi = wg_desc_lo(st0 + 2 * b_bytes) + (uint32_t)(wg * FRAGS) * h16;
+        const uint32_t a_lo = wg_desc_lo(st0 + 2 * b_bytes + DW_BM * ROWB) + (uint32_t)(wg * FRAGS) * h16;
         wgmma_fence();
 #pragma unroll
-        for (uint32_t k = 0; k < DW_BK / 16; ++k) {
+        for (uint32_t k = 0; k < SPK; ++k) {
           const uint32_t acc = (kb | k) ? 1u : 0u;
           const uint64_t bh = wg_desc(b_hi + 2 * k, dhi), bl = wg_desc(b_lo + 2 * k, dhi);
-          Wgmma<DW_BN>::mma(d0, wg_desc(a_lo + 2 * k, dhi), bh, acc);
-          Wgmma<DW_BN>::mma(d1, wg_desc(a_lo + h16 + 2 * k, dhi), bh, acc);
-          Wgmma<DW_BN>::mma(d0, wg_desc(a_hi + 2 * k, dhi), bl, 1u);
-          Wgmma<DW_BN>::mma(d1, wg_desc(a_hi + h16 + 2 * k, dhi), bl, 1u);
-          Wgmma<DW_BN>::mma(d0, wg_desc(a_hi + 2 * k, dhi), bh, 1u);
-          Wgmma<DW_BN>::mma(d1, wg_desc(a_hi + h16 + 2 * k, dhi), bh, 1u);
+#pragma unroll
+          for (int f = 0; f < FRAGS; ++f) Wgmma<BN>::mma(d[f], wg_desc(a_lo + f * h16 + 2 * k, dhi), bh, acc);
+#pragma unroll
+          for (int f = 0; f < FRAGS; ++f) Wgmma<BN>::mma(d[f], wg_desc(a_hi + f * h16 + 2 * k, dhi), bl, 1u);
+#pragma unroll
+          for (int f = 0; f < FRAGS; ++f) Wgmma<BN>::mma(d[f], wg_desc(a_hi + f * h16 + 2 * k, dhi), bh, 1u);
         }
         wgmma_commit();
         wgmma_wait<1>();                                // the previous k-block's wgmmas have read their stage
-        wgmma_fence_acc(d0);
-        wgmma_fence_acc(d1);
+#pragma unroll
+        for (int f = 0; f < FRAGS; ++f) wgmma_fence_acc(d[f]);
         if (prev >= 0 && lane == 0) mbar_arrive(bar_em + 8 * prev);
         prev = (int)s;
         if (++s == NST) { s = 0; ph ^= 1u; }
       }
       wgmma_wait<0>();
-      wgmma_fence_acc(d0);
-      wgmma_fence_acc(d1);
+#pragma unroll
+      for (int f = 0; f < FRAGS; ++f) wgmma_fence_acc(d[f]);
       if (prev >= 0 && lane == 0) mbar_arrive(bar_em + 8 * prev);
 
-      // ---- epilogue: 32 accumulator columns at a time through shared memory, thread = tile pixel ----
-      const int m = warp * 32 + lane;
+      // ---- epilogue per warpgroup: 32 accumulator columns at a time through shared memory, thread = tile pixel ----
+      // One warpgroup: thread t has tile row t and both 16-column halves of a chunk.  Two: warpgroup wg has rows
+      // [64 wg, 64 wg + 64), thread t of it row 64 wg + t % 64 and the chunk's 16-column half t / 64.
+      const int t = tid & 127;
+      const int m = FRAGS == 2 ? t : 64 * wg + (t & 63);
+      const int csub = FRAGS == 2 ? 0 : 16 * (t >> 6), cstep = FRAGS == 2 ? 16 : 32;
       const int ry = m >> tw_shift;
       const int wo = tx * TW + (m & (TW - 1)), ho = ty * TH + ry;
       const bool row_ok = ry < TH && wo < p.Wo && ho < p.Ho;
       __nv_bfloat16* yp = yb + (((size_t)n * p.Ho + ho) * p.Wo + wo) * (size_t)(2 * p.Cout);
       const uint32_t trow = smem_u32(stf + (size_t)m * DW_EPI_PITCH);
-      for (int c32 = 0; c32 < DW_BN; c32 += 32) {
+      for (int c32 = 0; c32 < BN; c32 += 32) {
         if (n0 + c32 >= p.Cout) break;                 // zero-padded weight rows (CTA-uniform)
-        named_bar(2, DW_CONSUMERS);                    // the previous chunk has been read
+        named_bar(2 + wg, 128);                        // the previous chunk has been read
 #pragma unroll
-        for (int c = 0; c < DW_BN; c += 32)
+        for (int c = 0; c < BN; c += 32)
           if (c == c32) {
-            acc_stage<DW_BN, 32>(d0, stf, DW_EPI_PITCH, 0, c);
-            acc_stage<DW_BN, 32>(d1, stf, DW_EPI_PITCH, 64, c);
+#pragma unroll
+            for (int f = 0; f < FRAGS; ++f) acc_stage<BN, 32>(d[f], stf, DW_EPI_PITCH, 64 * (wg * FRAGS + f), c);
           }
-        named_bar(2, DW_CONSUMERS);
-        for (int cb = c32; cb < c32 + 32 && cb < DW_BN; cb += 16) {
+        named_bar(2 + wg, 128);
+        for (int cb = c32 + csub; cb < c32 + 32 && cb < BN; cb += cstep) {
           if (n0 + cb >= p.Cout) break;
           uint32_t rr[16];
           acc_ld16(trow + (uint32_t)(cb - c32) * 4u, rr);
@@ -615,6 +668,16 @@ extern "C" int upsnet_dcn_pack_weight(const float* weight, int Cout, int Cin, in
   return 0;
 }
 
+// N tile of the next launches: 0 = chosen per launch (above), 32 or 128 = that N tile wherever it applies (128 needs a
+// deformable layer with Cout_pad % 128 == 0).  For tests and tuning: lets one process compare both instantiations.
+static int g_dw_force_bn = 0;
+
+extern "C" int upsnet_dcn_set_tile_n(int bn) {
+  if (bn != 0 && bn != 32 && bn != 128) return UPSNET_E_BADARG;
+  g_dw_force_bn = bn;
+  return 0;
+}
+
 static int dw_launch(const void* x_pair, const float* offset, const float* mask, const void* packed,
                      const float* bias, void* y_pair, int N, int H, int W, int Cin, int Cout, int kh,
                      int kw, int pad_h, int pad_w, int dil_h, int dil_w, int epi_flags, bool dense, bool out_nchw, void* stream) {
@@ -634,7 +697,6 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
   p.Wo = conv_out_size(W, pad_w, dil_w, 3, 1);
   if (p.Ho <= 0 || p.Wo <= 0) return UPSNET_E_BADARG;
   p.relu = (epi_flags & UPSNET_EPI_RELU) ? 1 : 0;
-  p.BN = DW_BN;
   p.dense = dense ? 1 : 0; p.out_nchw = out_nchw ? 1 : 0;
   static int sms = 0;
   if (sms == 0) {
@@ -644,9 +706,17 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
   }
   p.tile_w = 16; p.tile_h = 8;
   auto dtiles = [&]() { return (long long)p.N * ((p.Wo + p.tile_w - 1) / p.tile_w) * ((p.Ho + p.tile_h - 1) / p.tile_h) * (p.Cout_pad / p.BN); };
+  // N tile: 128 (A tile gathered once per 128 output channels) when Cout_pad allows it and there are at least sms / 4
+  // of its 16 x 8-pixel tiles; otherwise 32, whose smaller pixel blocks (below) spread tiny maps over more SMs.  Measured
+  // on H100 SXM (400 W), 256 -> 128 channels: 64 x 128 map (64 tiles) 0.128 ms at N = 128 vs 0.221 ms at N = 32;
+  // 32 x 64 map (16 tiles) 0.138 vs 0.115 ms.  DENSE mode: always 32.
+  p.BN = 128;
+  const bool wide_ok = !dense && p.Cout_pad % 128 == 0;
+  const bool wide = wide_ok && (g_dw_force_bn == 128 || (g_dw_force_bn == 0 && dtiles() >= sms / 4));
+  if (!wide) p.BN = 32;
   // few tiles (coarse pyramid levels): smaller pixel blocks -> more CTAs share the serial k-block chain
-  if (dtiles() < sms / 2) { p.tile_w = 8; p.tile_h = 8; }
-  if (dtiles() < sms / 2) { p.tile_h = 4; }
+  if (!wide && dtiles() < sms / 2) { p.tile_w = 8; p.tile_h = 8; }
+  if (!wide && dtiles() < sms / 2) { p.tile_h = 4; }
   {
     static int tile_env = -1;     // tuning hook shared with igemm_tc.cu
     if (tile_env < 0) { const char* e = getenv("UPSNET_DCN_TILE"); tile_env = e ? atoi(e) : 0; }
@@ -675,8 +745,12 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
   }
   p.win_bytes = dense ? 2 * p.win_pitch * win_h * 128 : 2 * DW_WW * win_h * 32;
   p.win_h = win_h;
+  // shared memory: N = 32 -> 23 KB tables + 2 x 40 KB stages (3 do not fit) + 2 x 40 KB windows + 18 KB staging;
+  //                N = 128 -> 23 KB tables + 3 x 32 KB stages + 2 x 40 KB windows + 18 KB staging (218 KB)
+  const uint32_t stage_bytes = wide ? DwCfg<128>::STAGE_BYTES : DwCfg<32>::STAGE_BYTES;
+  const int bk = wide ? DwCfg<128>::BK : DwCfg<32>::BK;
   auto smem_need = [&]() {
-    return (size_t)DW_OFF_STAGES + (size_t)p.stages * (2 * (p.BN * 128) + DW_A_BYTES) + (size_t)p.win_nbuf * p.win_buf + DW_EPI_BYTES + 1024;
+    return (size_t)DW_OFF_STAGES + (size_t)p.stages * stage_bytes + (size_t)p.win_nbuf * p.win_buf + DW_EPI_BYTES + 1024;
   };
   if (smem_need() > 227 * 1024 && p.stages > 2) p.stages = 2;
   if (smem_need() > 227 * 1024) return UPSNET_E_UNSUPPORTED;
@@ -691,20 +765,26 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
     if (enc(&tm_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x_pair), dx, sx, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
             dense ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return UPSNET_E_UNSUPPORTED;
+    // weight box: BK x BN, rows of BK bf16 in the swizzle the stage's wgmma descriptors expect
     const cuuint64_t dwt[2] = {(cuuint64_t)(9 * Cin), (cuuint64_t)(2 * p.Cout_pad)};
     const cuuint64_t sw[1] = {(cuuint64_t)(9 * Cin) * 2};
-    const cuuint32_t bw[2] = {64, (cuuint32_t)p.BN};
+    const cuuint32_t bw[2] = {(cuuint32_t)bk, (cuuint32_t)p.BN};
     if (enc(&tm_w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(packed), dwt, sw, bw, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+            bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return UPSNET_E_UNSUPPORTED;
   }
   const size_t smem = smem_need();
   static PerDeviceOnce configured;
   if (configured.need()) {
-    UPS_CUDA(cudaFuncSetAttribute(dcn_win_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    UPS_CUDA(cudaFuncSetAttribute(dcn_win_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    UPS_CUDA(cudaFuncSetAttribute(dcn_win_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   }
   dim3 grid((unsigned)(num_tiles < sms ? num_tiles : sms));
-  dcn_win_kernel<<<grid, DW_THREADS, smem, (cudaStream_t)stream>>>(tm_x, tm_w, p);
+  if (wide)
+    dcn_win_kernel<128><<<grid, DwCfg<128>::THREADS, smem, (cudaStream_t)stream>>>(tm_x, tm_w, p);
+  else
+    dcn_win_kernel<32><<<grid, DwCfg<32>::THREADS, smem, (cudaStream_t)stream>>>(tm_x, tm_w, p);
   UPS_CHECK_LAUNCH();
   return 0;
 }

@@ -101,6 +101,8 @@ template <int R> __device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) 
 // Given as (low word, high word): one 32-bit add of 2 advances K by 16 bf16 inside the 128-byte swizzle span.
 __device__ __forceinline__ uint32_t wg_desc_lo(uint32_t smem_addr) { return ((smem_addr >> 4) & 0x3fffu) | (1u << 16); }
 __device__ __forceinline__ uint32_t wg_desc_hi(uint32_t sbo_bytes) { return (sbo_bytes >> 4) | (1u << 30); }
+// the same for K-major SWIZZLE_64B tiles (64-byte rows, layout type 2): K advances by 16 bf16 with the same add of 2
+__device__ __forceinline__ uint32_t wg_desc_hi_sw64(uint32_t sbo_bytes) { return (sbo_bytes >> 4) | (2u << 30); }
 __device__ __forceinline__ uint64_t wg_desc(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
 
 // Accumulator staging: the warpgroup's 64 x N fragment (rows [row0, row0 + 64) of the tile) is written to a row-major fp32
