@@ -21,6 +21,17 @@ namespace ups {
 
 constexpr int kNumSMs = 132;  // H100 SXM
 
+// SM count of the device current at the first call, cached for the process; kNumSMs if the query fails
+inline int num_sms() {
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0, v = kNumSMs;
+    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    sms = v > 0 ? v : kNumSMs;
+  }
+  return sms;
+}
+
 // cudaFuncSetAttribute is per device (and context): remember which devices a kernel has been configured on, so that a
 // process driving several GPUs (the reference's thread-per-GPU DataParallel, gpu_nms(device_id)) opts in on each of them.
 struct PerDeviceOnce {

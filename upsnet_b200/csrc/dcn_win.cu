@@ -33,7 +33,6 @@
 // 128 KB of shared-memory reads -- per 128 output channels at N = 128, per 32 at N = 32 -- see DESIGN.md section 4.
 #include <cuda.h>
 #include <cuda_bf16.h>
-#include <cstdlib>
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -120,31 +119,6 @@ struct DwParams {
   int win_nbuf;           // window buffers (2: the next fill streams in while the current one is gathered; dense mode: 1)
 };
 
-__device__ __forceinline__ void dw_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void dw_tma_4d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void dw_tma_2d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void dw_prefetch_tmap(const CUtensorMap* tm) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
-}
-__device__ __forceinline__ uint4 dw_lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
-template <int R> __device__ __forceinline__ void dw_setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
-template <int R> __device__ __forceinline__ void dw_setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
-template <int N> __device__ __forceinline__ void dw_producer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(N) : "memory"); }
-
 template <int BN>
 __global__ void __launch_bounds__(DwCfg<BN>::THREADS, 1)
 dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const DwParams p) {
@@ -208,8 +182,8 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     }
     __syncwarp();
   }
-  if (warp == DW_WARP_TMAB && lane == 0) dw_prefetch_tmap(&tm_w);
-  if (warp == DW_WARP_TMAW && lane == 0) dw_prefetch_tmap(&tm_x);
+  if (warp == DW_WARP_TMAB && lane == 0) prefetch_tmap(&tm_w);
+  if (warp == DW_WARP_TMAW && lane == 0) prefetch_tmap(&tm_x);
   __syncthreads();
 
   if (warp >= DW_WARP_PROD0) {
@@ -238,7 +212,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         const int ry = min(rr >> tw_shift, TH - 1), rx = rr & (TW - 1);      // rows past the block read a valid (unused) pixel
         tp[e] = (ry + ki * p.dh) * p.win_pitch + rx + kj * p.dw;      // window PIXEL index
       }
-      dw_producer_bar<DW_PRODUCERS>();
+      named_bar<1, DW_PRODUCERS>();
     }
     for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tile_it) {
       const long long mt = tile / n_tiles;
@@ -293,7 +267,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         atomicMin(st + 0, mnw); atomicMin(st + 1, mnh); atomicMax(st + 2, mxw); atomicMax(st + 3, mxh);
         atomicAdd(st + 4, sw_); atomicAdd(st + 5, sh_); atomicAdd(st + 6, cnt);
       }
-      dw_producer_bar<DW_PRODUCERS>();      // (B) statistics complete; every producer has also finished the previous tile's gather
+      named_bar<1, DW_PRODUCERS>();      // (B) statistics complete; every producer has also finished the previous tile's gather
       // ---- window origin (same integer arithmetic in every thread), table phase 2 ----
       int ox = 0, oy = 0;
       {
@@ -326,7 +300,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         so[0] = 0x7fffffff; so[1] = 0x7fffffff; so[2] = -0x7fffffff; so[3] = -0x7fffffff; so[4] = 0; so[5] = 0; so[6] = 0;
         mbar_arrive(bar_og + 8 * par);        // release: the window TMA thread may read the origin
       }
-      dw_producer_bar<DW_PRODUCERS>();      // (C) table visible
+      named_bar<1, DW_PRODUCERS>();      // (C) table visible
       }                       // !dense
       const __nv_bfloat16* ximg = xh + (size_t)n * p.H * p.W * (size_t)(2 * p.Cin);
 
@@ -354,7 +328,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
             // SWIZZLE_128B window: a pixel is one 128-byte row (64 channels), 16-byte chunk c sits at c ^ (pixel & 7)
             const uint32_t pix = (uint32_t)code, ch = (uint32_t)((sc & 3) * 2 + half);
             const uint32_t al = wbuf + pix * 128u + ((ch ^ (pix & 7u)) << 4);
-            const uint4 h4 = dw_lds128(al), l4 = dw_lds128(al + (uint32_t)p.win_plane);
+            const uint4 h4 = lds128(al), l4 = lds128(al + (uint32_t)p.win_plane);
             sts128(a_row + a_off, h4);
             sts128(a_row + DW_BM * ROWB + a_off, l4);
             continue;
@@ -366,9 +340,9 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
             const uint32_t cl = (uint32_t)code, cr = cl + 32u;
             const uint32_t al = wbuf + cl + ((((cl >> 7) & 1u) ^ (uint32_t)half) << 4);
             const uint32_t ar = wbuf + cr + ((((cr >> 7) & 1u) ^ (uint32_t)half) << 4);
-            hc[0] = dw_lds128(al); hc[1] = dw_lds128(ar); hc[2] = dw_lds128(al + DW_WW * 32); hc[3] = dw_lds128(ar + DW_WW * 32);
-            lc[0] = dw_lds128(al + DW_PLANE); lc[1] = dw_lds128(ar + DW_PLANE);
-            lc[2] = dw_lds128(al + DW_PLANE + DW_WW * 32); lc[3] = dw_lds128(ar + DW_PLANE + DW_WW * 32);
+            hc[0] = lds128(al); hc[1] = lds128(ar); hc[2] = lds128(al + DW_WW * 32); hc[3] = lds128(ar + DW_WW * 32);
+            lc[0] = lds128(al + DW_PLANE); lc[1] = lds128(ar + DW_PLANE);
+            lc[2] = lds128(al + DW_PLANE + DW_WW * 32); lc[3] = lds128(ar + DW_PLANE + DW_WW * 32);
           } else {
             // outlier sample: the four corners come from global memory (clamped addresses; invalid corners carry weight 0)
             const int hl = (int)(((uint32_t)code >> 15) & 0xffffu) - 1, wl = (int)((uint32_t)code & 0x7fffu) - 1;
@@ -443,7 +417,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
   } else if (warp >= DW_WARP_TMAB) {
     // The TMA warpgroup (weight TMA, window TMA, two idle warps) keeps a minimal register budget so that the consumer
     // warpgroups can raise theirs.
-    dw_setmaxnreg_dec<C::REGS_TMA>();
+    setmaxnreg_dec<C::REGS_TMA>();
     if (warp == DW_WARP_TMAW && lane == 0) {
     // =============================== WINDOW TMA ===============================
       uint32_t wf = 0, ti = 0;
@@ -463,10 +437,10 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         for (int f = 0; f < nfill; ++f, ++wf) {
           const uint32_t b = wf % NWB;
           mbar_wait(bar_we + 8 * b, ((wf / NWB) & 1u) ^ 1u);
-          dw_expect_tx(bar_wf + 8 * b, (uint32_t)p.win_bytes);
+          mbar_arrive_expect_tx(bar_wf + 8 * b, (uint32_t)p.win_bytes);
           const uint32_t dst = win_base + b * (uint32_t)p.win_buf;
-          dw_tma_4d(dst, &tm_x, bar_wf + 8 * b, f * cstep, o.x, o.y, o.z);
-          dw_tma_4d(dst + (uint32_t)p.win_plane, &tm_x, bar_wf + 8 * b, p.Cin + f * cstep, o.x, o.y, o.z);
+          tma_load_4d(dst, &tm_x, bar_wf + 8 * b, f * cstep, o.x, o.y, o.z);
+          tma_load_4d(dst + (uint32_t)p.win_plane, &tm_x, bar_wf + 8 * b, p.Cin + f * cstep, o.x, o.y, o.z);
         }
       }
     } else if (warp == DW_WARP_TMAB && lane == 0) {
@@ -478,16 +452,16 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
           const uint32_t s = g % NST, it = g / NST;
           mbar_wait(bar_em + 8 * s, (it & 1u) ^ 1u);
           const uint32_t stage = base + DW_OFF_STAGES + s * stage_bytes;
-          dw_expect_tx(bar_fb + 8 * s, 2 * b_bytes);
-          dw_tma_2d(stage, &tm_w, bar_fb + 8 * s, kb * DW_BK, n0);
-          dw_tma_2d(stage + b_bytes, &tm_w, bar_fb + 8 * s, kb * DW_BK, p.Cout_pad + n0);
+          mbar_arrive_expect_tx(bar_fb + 8 * s, 2 * b_bytes);
+          tma_load_2d(stage, &tm_w, bar_fb + 8 * s, kb * DW_BK, n0);
+          tma_load_2d(stage + b_bytes, &tm_w, bar_fb + 8 * s, kb * DW_BK, p.Cout_pad + n0);
         }
       }
     }
     __syncwarp();
   } else {
     // =============================== CONSUMERS (warpgroups 0 .. NCW-1) ===============================
-    dw_setmaxnreg_inc<C::REGS_CONSUMER>();
+    setmaxnreg_inc<C::REGS_CONSUMER>();
     // Warpgroup wg owns m64 fragment f (tile rows [64 (wg FRAGS + f), +64)) for f < FRAGS.
     constexpr int FRAGS = C::FRAGS;
     const int wg = warp >> 2;
@@ -620,29 +594,9 @@ __global__ void dcn_win_pack_kernel(const float* __restrict__ w, int Cout, int C
   }
 }
 
-static int dw_cout_pad(int Cout) { return Cout <= 32 ? 32 : (Cout + 63) / 64 * 64; }
-
 // packing / kernel: any Cout (rows are zero-padded); the pair NHWC epilogue additionally needs Cout % 16 == 0
 static bool dw_supported(int Cin, int Cout, int kh, int kw) {
   return kh == 3 && kw == 3 && Cin % 64 == 0 && Cin >= 64 && Cout >= 1;
-}
-
-typedef CUresult (*DwEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static DwEncodeFn dw_encoder() {
-  static DwEncodeFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    void* q = nullptr;
-    cudaDriverEntryPointQueryResult qr = cudaDriverEntryPointSymbolNotFound;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &q, cudaEnableDefault, &qr) == cudaSuccess && qr == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<DwEncodeFn>(q);
-    else
-      (void)cudaGetLastError();
-    tried = true;
-  }
-  return fn;
 }
 
 }  // namespace ups
@@ -650,14 +604,14 @@ static DwEncodeFn dw_encoder() {
 extern "C" int upsnet_dcn_packed_weight_bytes(int Cout, int Cin, int kh, int kw, size_t* bytes) {
   if (!bytes || Cout <= 0 || Cin <= 0) return UPSNET_E_BADARG;
   if (!ups::dw_supported(Cin, Cout, kh, kw)) return UPSNET_E_UNSUPPORTED;
-  *bytes = (size_t)2 * ups::dw_cout_pad(Cout) * (size_t)(9 * Cin) * sizeof(uint16_t);
+  *bytes = (size_t)2 * ups::cout_pad(Cout) * (size_t)(9 * Cin) * sizeof(uint16_t);
   return 0;
 }
 
 extern "C" int upsnet_dcn_pack_weight(const float* weight, int Cout, int Cin, int kh, int kw, void* packed, void* stream) {
   if (!weight || !packed || Cout <= 0 || Cin <= 0) return UPSNET_E_BADARG;
   if (!ups::dw_supported(Cin, Cout, kh, kw)) return UPSNET_E_UNSUPPORTED;
-  const int Cout_pad = ups::dw_cout_pad(Cout), K = 9 * Cin;
+  const int Cout_pad = ups::cout_pad(Cout), K = 9 * Cin;
   uint16_t* hi = reinterpret_cast<uint16_t*>(packed);
   uint16_t* lo = hi + (size_t)Cout_pad * K;
   const size_t total = (size_t)Cout_pad * K;
@@ -691,19 +645,14 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
     return UPSNET_E_UNSUPPORTED;
   DwParams p{};
   p.x = x_pair; p.offset = offset; p.mask = mask; p.bias = bias; p.y = y_pair;
-  p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.Cout_pad = dw_cout_pad(Cout);
+  p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.Cout_pad = cout_pad(Cout);
   p.ph = pad_h; p.pw = pad_w; p.dh = dil_h; p.dw = dil_w;
   p.Ho = conv_out_size(H, pad_h, dil_h, 3, 1);
   p.Wo = conv_out_size(W, pad_w, dil_w, 3, 1);
   if (p.Ho <= 0 || p.Wo <= 0) return UPSNET_E_BADARG;
   p.relu = (epi_flags & UPSNET_EPI_RELU) ? 1 : 0;
   p.dense = dense ? 1 : 0; p.out_nchw = out_nchw ? 1 : 0;
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0, v = kNumSMs;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    sms = v > 0 ? v : kNumSMs;
-  }
+  const int sms = num_sms();
   p.tile_w = 16; p.tile_h = 8;
   auto dtiles = [&]() { return (long long)p.N * ((p.Wo + p.tile_w - 1) / p.tile_w) * ((p.Ho + p.tile_h - 1) / p.tile_h) * (p.Cout_pad / p.BN); };
   // N tile: 128 (A tile gathered once per 128 output channels) when Cout_pad allows it and there are at least sms / 4
@@ -717,13 +666,6 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
   // few tiles (coarse pyramid levels): smaller pixel blocks -> more CTAs share the serial k-block chain
   if (!wide && dtiles() < sms / 2) { p.tile_w = 8; p.tile_h = 8; }
   if (!wide && dtiles() < sms / 2) { p.tile_h = 4; }
-  {
-    static int tile_env = -1;     // tuning hook shared with igemm_tc.cu
-    if (tile_env < 0) { const char* e = getenv("UPSNET_DCN_TILE"); tile_env = e ? atoi(e) : 0; }
-    if (tile_env == 168) { p.tile_w = 16; p.tile_h = 8; }
-    if (tile_env == 88) { p.tile_w = 8; p.tile_h = 8; }
-    if (tile_env == 84) { p.tile_w = 8; p.tile_h = 4; }
-  }
   const long long num_tiles = dtiles();
   if (num_tiles <= 0) return 0;
   // dense: the window box is the tile's receptive field: 24 pixels x (tile + halo) rows x 64 channels (128-byte pixels)
@@ -738,11 +680,6 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
     p.win_buf = 2 * p.win_plane;
     p.win_nbuf = 1;       // one 64-channel fill serves 36 k-slices: a second buffer does not fit next to the A stages
   }
-  if (!dense) {     // tuning hook: UPSNET_DCN_WIN_H = rows of the deformable window box (12..24)
-    static int wh_env = -1;
-    if (wh_env < 0) { const char* e = getenv("UPSNET_DCN_WIN_H"); wh_env = e ? atoi(e) : 0; }
-    if (wh_env >= 12 && wh_env <= DW_WH) win_h = wh_env;
-  }
   p.win_bytes = dense ? 2 * p.win_pitch * win_h * 128 : 2 * DW_WW * win_h * 32;
   p.win_h = win_h;
   // shared memory: N = 32 -> 23 KB tables + 2 x 40 KB stages (3 do not fit) + 2 x 40 KB windows + 18 KB staging;
@@ -754,7 +691,7 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
   };
   if (smem_need() > 227 * 1024 && p.stages > 2) p.stages = 2;
   if (smem_need() > 227 * 1024) return UPSNET_E_UNSUPPORTED;
-  DwEncodeFn enc = dw_encoder();
+  EncodeTiledFn enc = tma_encoder();
   if (!enc) return UPSNET_E_UNSUPPORTED;
   CUtensorMap tm_x, tm_w;
   {

@@ -26,7 +26,6 @@
 // LSU gather rate of the producers (4 corner reads per element) -- see DESIGN.md.
 #include <cuda_bf16.h>
 #include <cstdio>
-#include <cstdlib>
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -43,6 +42,7 @@ constexpr int TC_CONSUMERS = 128;     // 4 warps = one wgmma warpgroup; in the e
 constexpr int TC_EPI_PITCH = 36;      // floats per staged row: 32 columns + 4 pad (16-byte aligned, conflict-free)
 constexpr int TC_THREADS = TC_CONSUMERS + TC_PRODUCERS;  // 20 warps
 constexpr int TC_MAX_STAGES = 6;
+// named barriers (id 0 is __syncthreads): 1 = the producer warps, 2 = the consumer warps
 
 
 
@@ -68,11 +68,6 @@ __host__ __device__ inline TcSmem tc_smem_layout(bool deform, int KHW, int BN, i
   s.stage_bytes = (s.a_bytes + s.b_bytes) * (x3 ? 2 : 1);
   s.total = s.stages + s.stage_bytes * stages;
   return s;
-}
-
-// Named barriers (id 0 is __syncthreads): 1 = the producer warps, 2 = the consumer warps
-__device__ __forceinline__ void producer_bar_sync() {
-  asm volatile("bar.sync 1, %0;" ::"n"(TC_PRODUCERS) : "memory");
 }
 
 // Persistent, warp-specialised kernel.  Roles (20 warps):
@@ -179,7 +174,7 @@ igemm_tc_kernel(const TcParams p) {
       // producer barrier per tile suffices for the dense / stem modes; the deformable sample table is a single
       // buffer and needs the extra barrier before it is overwritten.
       long long* rowinfo = rowbase + (tile_it & 1) * TC_BM;
-      if (DEFORM) producer_bar_sync();   // every producer is done with the previous tile's sample table
+      if (DEFORM) named_bar<1, TC_PRODUCERS>();   // every producer is done with the previous tile's sample table
       for (int r = pt; r < TC_BM; r += TC_PRODUCERS) {
         const long long pg = tile_pixel(mt, r);
         long long v = -1;
@@ -237,7 +232,7 @@ igemm_tc_kernel(const TcParams p) {
           to[e] = ov;
         }
       }
-      producer_bar_sync();   // row info (and sample table) visible to all producers
+      named_bar<1, TC_PRODUCERS>();   // row info (and sample table) visible to all producers
       ++tile_it;
 
       for (int kb = (int)((uint32_t)(group - (int)g0) & 1u); kb < num_kb; kb += TC_GROUPS) {  // ring parity == group
@@ -814,15 +809,14 @@ __global__ void pack_weight_kernel(const float* __restrict__ w, int Cout, int Ci
   }
 }
 
-static int tc_cout_pad(int Cout) { return Cout <= 32 ? 32 : (Cout + 63) / 64 * 64; }
 static int tc_kp(int Cin, int KHW) { return (KHW * Cin + TC_BK - 1) / TC_BK * TC_BK; }
 
 size_t tc_packed_weight_bytes(int Cout, int Cin, int kh, int kw) {
-  return (size_t)2 * tc_cout_pad(Cout) * tc_kp(Cin, kh * kw) * sizeof(uint16_t);
+  return (size_t)2 * cout_pad(Cout) * tc_kp(Cin, kh * kw) * sizeof(uint16_t);
 }
 
 int tc_pack_weight(const float* w, int Cout, int Cin, int kh, int kw, void* packed, cudaStream_t stream) {
-  const int Cout_pad = tc_cout_pad(Cout), KHW = kh * kw, Kp = tc_kp(Cin, KHW);
+  const int Cout_pad = cout_pad(Cout), KHW = kh * kw, Kp = tc_kp(Cin, KHW);
   uint16_t* hi = reinterpret_cast<uint16_t*>(packed);
   uint16_t* lo = hi + (size_t)Cout_pad * Kp;
   const size_t total = (size_t)Cout_pad * Kp;
@@ -875,7 +869,7 @@ int launch_igemm_tc(TcParams p, const void* packed, cudaStream_t stream) {
     if (rc != UPSNET_E_UNSUPPORTED) return rc;
   }
   if ((((uintptr_t)p.x) & 15) || (((uintptr_t)packed) & 15) || (((uintptr_t)p.y) & 15)) return UPSNET_E_BADARG;
-  p.Cout_pad = tc_cout_pad(p.Cout);
+  p.Cout_pad = cout_pad(p.Cout);
   p.w_hi = reinterpret_cast<const uint16_t*>(packed);
   p.w_lo = p.w_hi + (size_t)p.Cout_pad * tc_kp(p.Cin, KHW);
   const bool deform = p.offset != nullptr;
@@ -909,31 +903,16 @@ int launch_igemm_tc(TcParams p, const void* packed, cudaStream_t stream) {
   p.stages = stages;
   const long long Ptot = (long long)p.N * p.Ho * p.Wo;
   if (Ptot <= 0) return 0;
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0, v = kNumSMs;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    sms = v > 0 ? v : kNumSMs;
-  }
+  const int sms = num_sms();
   p.tile_w = 16; p.tile_h = 8;
   auto dtiles = [&]() { return (long long)p.N * ((p.Wo + p.tile_w - 1) / p.tile_w) * ((p.Ho + p.tile_h - 1) / p.tile_h) * (p.Cout_pad / BN); };
   if (deform) {   // few tiles (coarse pyramid levels): smaller pixel blocks -> more CTAs, proportionally less gather work each
     if (dtiles() < sms / 2) { p.tile_w = 8; p.tile_h = 8; }
     if (dtiles() < sms / 2) { p.tile_h = 4; }
-    static int tile_env = -1;     // tuning hook: UPSNET_DCN_TILE=168 | 88 | 84 forces the pixel block (pair / bf16 experiments)
-    if (tile_env < 0) { const char* e = getenv("UPSNET_DCN_TILE"); tile_env = e ? atoi(e) : 0; }
-    if (tile_env == 168) { p.tile_w = 16; p.tile_h = 8; }
-    if (tile_env == 88) { p.tile_w = 8; p.tile_h = 8; }
-    if (tile_env == 84) { p.tile_w = 8; p.tile_h = 4; }
   }
   const long long num_tiles = (deform ? dtiles() : ((Ptot + TC_BM - 1) / TC_BM) * (p.Cout_pad / BN));
   dim3 grid((unsigned)(num_tiles < sms ? num_tiles : sms));
-  size_t smem = L.total + 1024;
-  if (deform) {     // experiment hook: extra (unused) dynamic shared memory shrinks L1 -- measures the gather's L1 sensitivity
-    static int extra = -1;
-    if (extra < 0) { const char* e = getenv("UPSNET_DCN_EXTRA_SMEM_KB"); extra = e ? atoi(e) : 0; }
-    if (extra > 0 && smem + (size_t)extra * 1024 <= 227 * 1024) smem += (size_t)extra * 1024;
-  }
+  const size_t smem = L.total + 1024;
   // opt in to the full 227 KB once per device (kept out of the per-launch path: CUDA-graph capture)
   static PerDeviceOnce configured;
   if (configured.need()) {

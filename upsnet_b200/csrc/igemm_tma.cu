@@ -63,40 +63,6 @@ struct TmaGeom {
   int wide;
 };
 
-// ---- PTX: TMA (bulk tensor) copies ----
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-      ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
-}
-__device__ __forceinline__ void named_bar_sync(int id, int count) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
-}
 // pair tensors: channel coordinate of channel n's hi value when channels are stored [hi G][lo G] per group of G (lo = +G)
 __device__ __forceinline__ int pair_chan(int n, int G) { return (n / G) * 2 * G + (n % G); }
 
@@ -324,9 +290,9 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
 #pragma unroll
         for (int i = 0; i < N / 4; ++i) d[i] += d[N / 4 + i];
       }
-      named_bar_sync(3, 256);                    // the previous tile's epilogue has read the staging rows
+      named_bar(3, 256);                    // the previous tile's epilogue has read the staging rows
       acc_stage_sw<N, SW>(d, accbuf, wg * 64);
-      named_bar_sync(3, 256);
+      named_bar(3, 256);
     };
     const int q = warp & 3, half = warp >> 2;
     const int row = q * 32 + lane;
@@ -403,7 +369,7 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
             if (lead) {                             // the stores that last used this pair have finished reading it
               if (g.opairs == 2) bulk_wait_read1(); else bulk_wait_read0();
             }
-            named_bar_sync(1, 256);
+            named_bar(1, 256);
           }
           float o[32];
 #pragma unroll
@@ -448,7 +414,7 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
             sts128(ob + TM_SLAB_BYTES + sw_row + (((jb + c) ^ rx) << 4), make_uint4(lw[0], lw[1], lw[2], lw[3]));
           }
           fence_proxy_async();
-          named_bar_sync(1, 256);
+          named_bar(1, 256);
           if (lead) {
             const int c = pair_chan(n0 + sl * 64, g.pg);
             tma_store_4d(&tm_y, ob, c, w0, h0, i0);
@@ -474,7 +440,7 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
         if ((u & 1) == 0 || g.BN == 64) {
           // the output slab is about to be overwritten: its previous TMA store must have finished reading it
           if (leader) bulk_wait_read0();
-          named_bar_sync(bar_id, bar_cnt);
+          named_bar(bar_id, bar_cnt);
         }
         float o[32];
 #pragma unroll
@@ -513,7 +479,7 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
         }
         if ((u & 1) == 1 || g.BN == 64) {
           fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA store
-          named_bar_sync(bar_id, bar_cnt);
+          named_bar(bar_id, bar_cnt);
           if (leader) {
             tma_store_4d(&tm_y, out_slab, n0 + slab * 64, w0, h0, i0);
             bulk_commit();
@@ -530,26 +496,6 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
 // ----------------------------------------------------------------------------------------------
 // host side: tensor maps, tile geometry, launch
 // ----------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn tma_encoder() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qr = cudaDriverEntryPointSymbolNotFound;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qr) == cudaSuccess &&
-        qr == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-    else
-      (void)cudaGetLastError();
-    tried = true;
-  }
-  return fn;
-}
-
 // bf16 tensor, innermost dimension first; box[0] = 64 elements = one 128-byte swizzle span
 static bool encode_bf16(EncodeTiledFn enc, CUtensorMap* tm, const void* ptr, int rank, const cuuint64_t* dims,
                         const cuuint32_t* box, const cuuint64_t* byte_strides = nullptr) {
@@ -653,12 +599,7 @@ int launch_igemm_tma(const TcParams& p, const void* packed, cudaStream_t stream)
   if (p.bias && (((uintptr_t)p.bias) & 15)) return UPSNET_E_UNSUPPORTED;
   EncodeTiledFn enc = tma_encoder();
   if (!enc) return UPSNET_E_UNSUPPORTED;
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0, v = kNumSMs;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    sms = v > 0 ? v : kNumSMs;
-  }
+  const int sms = num_sms();
   TmaGeom g{};
   g.bias = p.bias;
   g.N = p.N; g.Ho = p.Ho; g.Wo = p.Wo; g.Cout = p.Cout; g.Cin = p.Cin;
@@ -669,7 +610,7 @@ int launch_igemm_tma(const TcParams& p, const void* packed, cudaStream_t stream)
   g.tiles_h = (p.Ho + g.bh - 1) / g.bh;
   g.tiles_n = (p.N + g.bn - 1) / g.bn;
   const long long m_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n;
-  const int Cout_pad = p.Cout <= 32 ? 32 : (p.Cout + 63) / 64 * 64;      // rows of the packed weight planes (tc_cout_pad)
+  const int Cout_pad = cout_pad(p.Cout);
   // N tile <= 128: the accumulators are m64nBN register fragments of two warpgroups (64 floats per thread at 128) and are
   // staged as 128 x BN fp32 rows in shared memory for the epilogue
   int BN = (Cout_pad % 128 == 0) ? 128 : (Cout_pad % 64 == 0 ? 64 : 32);
@@ -865,12 +806,7 @@ extern "C" int upsnet_stem_forward(const float* x, const void* packed_w, const f
                                                              N, Cin, H, W, pad, Hp, Wp);
     UPS_CHECK_LAUNCH();
   }
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0, v = kNumSMs;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    sms = v > 0 ? v : kNumSMs;
-  }
+  const int sms = num_sms();
   const long long num_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n * g.n_tiles;
   dim3 grid((unsigned)(num_tiles < sms ? num_tiles : sms));
   return tma_launch(g.BN, grid, L.total + 1024, st, tm_x, tm_w, tm_y, pair ? tm_lo : tm_y, g);

@@ -1,9 +1,34 @@
-// tc_params.cuh -- launch parameters shared by the wgmma convolution kernels and the C-ABI dispatcher.
+// tc_params.cuh -- launch parameters and host helpers shared by the wgmma convolution kernels and the C-ABI dispatcher.
 #pragma once
+#include <cuda.h>   // CUtensorMap + enums only; the encoder is resolved at run time (no libcuda link dependency)
 #include <cuda_runtime.h>
 #include <cstdint>
 
 namespace ups {
+
+// Rows of each packed weight plane (hi, lo) of the tensor-core convs: Cout zero-padded to a whole number of N tiles.
+inline int cout_pad(int Cout) { return Cout <= 32 ? 32 : (Cout + 63) / 64 * 64; }
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// cuTensorMapEncodeTiled from the driver, looked up once; null when the driver does not have it
+inline EncodeTiledFn tma_encoder() {
+  static EncodeTiledFn fn = nullptr;
+  static bool tried = false;
+  if (!tried) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qr = cudaDriverEntryPointSymbolNotFound;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qr) == cudaSuccess &&
+        qr == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+    else
+      (void)cudaGetLastError();
+    tried = true;
+  }
+  return fn;
+}
 
 struct TcParams {
   const void* x;         // NHWC [N,H,W,Cin], fp32 or bf16 (x_bf16)

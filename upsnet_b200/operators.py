@@ -151,16 +151,31 @@ def _nhwc(x):
 
 import weakref
 
-# keyed on the weight TENSOR OBJECT (weak): a data_ptr key would alias a freed weight whose storage the
-# caching allocator handed to a new tensor.  Entries die with their tensor; _version catches in-place updates.
-_packed_cache = {}   # id(tensor) -> (weakref to the tensor, version, packed buffer)
+
+def _per_weight(cache, weight, make, device=None, versioned=True):
+    """make() once per weight tensor, kept in `cache`: id(tensor) -> (weakref to the tensor, version, value).
+    Keyed on the weight TENSOR OBJECT (weak): a data_ptr key would alias a freed weight whose storage the caching
+    allocator handed to a new tensor.  Entries die with their tensor; with `versioned`, _version catches in-place
+    updates; with `device`, a value (None allowed) made for another device is made again."""
+    hit = cache.get(id(weight))
+    if (hit is not None and hit[0]() is weight and (not versioned or hit[1] == weight._version) and
+            (device is None or hit[2] is None or hit[2].device == device)):
+        return hit[2]
+    value = make()
+    wid = id(weight)
+    cache[wid] = (weakref.ref(weight, lambda _r, _k=wid: cache.pop(_k, None)), weight._version, value)
+    return value
+
+
+_packed_cache = {}
 
 
 def _packed_weight(weight):
     """bf16 hi/lo planes [Cout_pad][kh*kw][Cin] (upsnet_igemm_pack_weight), cached per weight tensor+version."""
-    hit = _packed_cache.get(id(weight))
-    if hit is not None and hit[0]() is weight and hit[1] == weight._version and hit[2].device == weight.device:
-        return hit[2]
+    return _per_weight(_packed_cache, weight, lambda: _pack_igemm(weight), device=weight.device)
+
+
+def _pack_igemm(weight):
     Cout, Cin, kh, kw = weight.shape
     nbytes = C.c_size_t(0)
     check(lib().upsnet_igemm_packed_weight_bytes(Cout, Cin, kh, kw, C.byref(nbytes)), "igemm_packed_weight_bytes")
@@ -170,8 +185,6 @@ def _packed_weight(weight):
         check(lib().upsnet_igemm_pack_weight(ptr(w), Cout, Cin, kh, kw, ptr(buf), stream_ptr(weight.device)),
               "igemm_pack_weight")
     STATS["launches"] += 1
-    wid = id(weight)
-    _packed_cache[wid] = (weakref.ref(weight, lambda _r, _k=wid: _packed_cache.pop(_k, None)), weight._version, buf)
     return buf
 
 
@@ -180,10 +193,11 @@ _dcn_packed_cache = {}
 
 def _packed_weight_dcn(weight):
     """upsnet_dcn_pack_weight: bf16 hi/lo planes in the window kernel's K order (16-channel sub-chunk, tap, channel);
-    None when the layer shape is not supported by that kernel.  Cached like _packed_weight."""
-    hit = _dcn_packed_cache.get(id(weight))
-    if hit is not None and hit[0]() is weight and hit[1] == weight._version and (hit[2] is None or hit[2].device == weight.device):
-        return hit[2]
+    None when the layer shape is not supported by that kernel (cached too).  Cached like _packed_weight."""
+    return _per_weight(_dcn_packed_cache, weight, lambda: _pack_dcn(weight), device=weight.device)
+
+
+def _pack_dcn(weight):
     Cout, Cin, kh, kw = weight.shape
     nbytes = C.c_size_t(0)
     rc = lib().upsnet_dcn_packed_weight_bytes(Cout, Cin, kh, kw, C.byref(nbytes))
@@ -196,8 +210,6 @@ def _packed_weight_dcn(weight):
         STATS["launches"] += 1
     elif rc != -2:
         check(rc, "dcn_packed_weight_bytes")
-    wid = id(weight)
-    _dcn_packed_cache[wid] = (weakref.ref(weight, lambda _r, _k=wid: _dcn_packed_cache.pop(_k, None)), weight._version, buf)
     return buf
 
 
@@ -259,7 +271,7 @@ def _dcn_window(x, offset, mask, weight, bias, padding, dilation, relu):
     return Pair(store)
 
 
-_stem_cache = {}   # id(weight) -> (weakref, version, packed bf16 [Cout][kh][8][8])
+_stem_cache = {}   # packed bf16 [Cout][kh][8][8] per weight
 _stem_ws = None
 
 
@@ -274,10 +286,8 @@ def stem_conv(x, weight, bias, padding, relu=True, pair=False):
     N, Cin, H, W = x.shape
     Cout, _, kh, kw = weight.shape
     dev = x.device
-    hit = _stem_cache.get(id(weight))
-    if hit is not None and hit[0]() is weight and hit[1] == weight._version and hit[2].device == dev:
-        packed = hit[2]
-    else:
+
+    def pack():
         nb = C.c_size_t(0)
         check(lib().upsnet_stem_packed_weight_bytes(Cout, kh, C.byref(nb)), "stem_packed_weight_bytes")
         packed = torch.empty(nb.value, dtype=torch.uint8, device=dev)
@@ -285,8 +295,9 @@ def stem_conv(x, weight, bias, padding, relu=True, pair=False):
             check(lib().upsnet_stem_pack_weight(ptr(f32c(weight.detach())), Cout, Cin, kh, kw, ptr(packed), stream_ptr(dev)),
                   "stem_pack_weight")
         STATS["launches"] += 1
-        wid = id(weight)
-        _stem_cache[wid] = (weakref.ref(weight, lambda _r, _k=wid: _stem_cache.pop(_k, None)), weight._version, packed)
+        return packed
+
+    packed = _per_weight(_stem_cache, weight, pack, device=dev)
     nb = C.c_size_t(0)
     check(lib().upsnet_stem_workspace_bytes(N, H, W, kh, kw, int(padding), C.byref(nb)), "stem_workspace_bytes")
     if _stem_ws is None:
@@ -462,13 +473,7 @@ _view_cache = {}
 def _as_1x1(weight):
     """[Cout,K] -> [Cout,K,1,1] view, cached per weight tensor so the packed-weight cache (keyed on tensor
     identity) hits on every call."""
-    hit = _view_cache.get(id(weight))
-    if hit is not None and hit[0]() is weight:
-        return hit[1]
-    v = weight.reshape(weight.shape[0], weight.shape[1], 1, 1)
-    wid = id(weight)
-    _view_cache[wid] = (weakref.ref(weight, lambda _r, _k=wid: _view_cache.pop(_k, None)), v)
-    return v
+    return _per_weight(_view_cache, weight, lambda: weight.reshape(weight.shape[0], weight.shape[1], 1, 1), versioned=False)
 
 
 def deform_conv(data, offset, weight, bias=None, stride=1, padding=0, dilation=1, deformable_groups=1,
