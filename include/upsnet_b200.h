@@ -348,6 +348,44 @@ int upsnet_unified_pan_result(const long long *seg, const long long *pan, const 
 int upsnet_prep_image(const unsigned char *image_hwc, int h, int w, double scale, int out_h, int out_w, int pad_h,
                       int pad_w, const double pixel_means[3], float *blob, void *stream);
 
+/* upsnet_label_restore: a network-resolution label map back to the original image size.
+ * replaces: upsnet_end2end_test.py:259-266 -- crop [:h,:w], astype(uint8) (values wrap mod 256), cv2.resize(fx = fy,
+ *           INTER_NEAREST) on the host.
+ * src0 / src1 int64 [Hp,Wp] (src1 / dst1 may be NULL: both maps of an image in one launch); (h,w) <= (Hp,Wp) the crop;
+ * fx the resize factor (the caller passes cv2's double); out_h = rint(h*fx), out_w = rint(w*fx) (half to even, cvRound).
+ * dst int64 [out_h,out_w] = (uint8) src[min(floor(y/fx),h-1)][min(floor(x/fx),w-1)] with 1/fx taken in double. */
+int upsnet_label_restore(const long long *src0, const long long *src1, int Hp, int Wp, int h, int w, double fx,
+                         int out_h, int out_w, long long *dst0, long long *dst1, void *stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Panoptic quality statistics of one image on the device (SURVEY section 8 row f4, evaluation half).
+ * replaces: dataset/base_dataset.py:462-511 _converter_2ch_single_core + :513-608 _pq_compute_single_core (numpy on the
+ *           host: np.unique over the 2-channel map, one full-image mask per segment, np.unique over a uint64 pair map).
+ * pan_2ch uint8 [H,W,3] (class, instance, -) as upsnet_unified_pan_result writes it; class 255 = void.  A prediction
+ *   segment is (class, instance) for a thing class and the class alone for a stuff class (stuff instances merge).
+ * gt_rgb uint8 [H,W,3], id = R + 256 G + 65536 B; id 0 = VOID.
+ * gt_table int64 [5][num_gt] (structure of arrays): id, category_id, iscrowd, area, order.  Rows sorted by strictly
+ *   ascending id in [1, 2^24); `order` = the row's position in the ground truth's segment list after duplicate ids are
+ *   merged the way a Python dict does (the later entry wins, the first position is kept); category_id in [0,255).
+ * cat_flags uint8 [256]: bit 0 = category known, bit 1 = isthing.
+ * acc_counts int64 [3][256] (tp, fp, fn per category id) and acc_iou fp64 [256] are ADDED to; the per-match IoUs are
+ *   summed in ascending (gt id, prediction segment) order, so repeated runs give bit-identical sums.
+ * err (DEVICE int, sticky: bits are OR-ed in, never cleared): UPSNET_PQ_E_* below.  The call never synchronises.
+ * Workspace: upsnet_pq_workspace_bytes. */
+#define UPSNET_PQ_MAX_GT 4096        /* ground-truth segments per image */
+#define UPSNET_PQ_MAX_PAIRS 65536    /* distinct (ground-truth segment, prediction segment) pairs per image */
+#define UPSNET_PQ_MAX_PRED 2048      /* prediction segments per image */
+#define UPSNET_PQ_E_PRED_CATEGORY 1  /* a prediction class that is neither 255 nor a known category */
+#define UPSNET_PQ_E_GT_COUNT 2       /* num_gt > UPSNET_PQ_MAX_GT */
+#define UPSNET_PQ_E_PAIRS 4          /* more than UPSNET_PQ_MAX_PAIRS distinct pairs */
+#define UPSNET_PQ_E_GT_TABLE 8       /* ids not strictly ascending in [1,2^24), or a category id outside [0,255) */
+#define UPSNET_PQ_E_PRED_COUNT 16    /* more than UPSNET_PQ_MAX_PRED prediction segments */
+#define UPSNET_PQ_E_MATCHES 32       /* more than UPSNET_PQ_MAX_GT matches (only when table areas undercount pixels) */
+int upsnet_pq_workspace_bytes(size_t *bytes);
+int upsnet_pq_update(const unsigned char *pan_2ch, const unsigned char *gt_rgb, int H, int W, const long long *gt_table,
+                     int num_gt, const unsigned char *cat_flags, long long *acc_counts, double *acc_iou, int *err,
+                     void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---------------------------------------------------------------------------------------
  * Instance-mask post-processing of the test loop on the device (SURVEY section 8 row f4).
  * replaces: upsnet_end2end_test.py:95-152 `im_post` (expand_boxes bbox/bbox_transform.py:365-381 -> int32 boxes,

@@ -7,7 +7,9 @@
 //  * upsnet_prep_image: dataset/base_dataset.py:143-174 prep_im_for_blob + :898-923 im_list_to_blob -- mean subtraction,
 //    bilinear resize (cv2.INTER_LINEAR rule) and zero padding to a multiple of the FPN stride, uint8 HWC BGR in, fp32 NCHW
 //    out.  Reference: numpy + cv2 on the host, then a 4x larger fp32 H2D copy.
-// Both are HBM-bound streaming kernels (bytes: 16*H*W + 3*H*W resp. 3*h*w + 12*Hp*Wp).
+//  * upsnet_label_restore: upsnet_end2end_test.py:259-266 (row f4) -- both label maps cropped to im_info[:2], wrapped to
+//    uint8 and resized back to the original image size with cv2's INTER_NEAREST rule, in one launch.
+// All are HBM-bound streaming kernels (bytes: 16*H*W + 3*H*W; 3*h*w + 12*Hp*Wp; 16*oh*ow per map).
 #include "common.cuh"
 
 namespace ups {
@@ -168,6 +170,23 @@ prep_image_kernel(const unsigned char* __restrict__ src, int h, int w, int ho, i
   }
 }
 
+// ---- label maps back to the original image size (upsnet_end2end_test.py:259-266) ----
+// cv2.resize INTER_NEAREST (imgproc/resize.cpp resizeNN): ifx = 1 / fx in double, sx = min(cvFloor(x * ifx), w - 1).
+// blockIdx.y picks the map; the crop [:h,:w] is the clamp, astype(uint8) the & 0xff.
+__global__ void __launch_bounds__(256)
+label_restore_kernel(const long long* __restrict__ src0, const long long* __restrict__ src1, int Wp, int h, int w,
+                     double ifx, int out_h, int out_w, long long* __restrict__ dst0, long long* __restrict__ dst1) {
+  const long long* src = blockIdx.y ? src1 : src0;
+  long long* dst = blockIdx.y ? dst1 : dst0;
+  const size_t n = (size_t)out_h * out_w;
+  for (size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (size_t)gridDim.x * blockDim.x) {
+    const int y = (int)(p / out_w), x = (int)(p - (size_t)y * out_w);
+    const int sy = min((int)floor(__dmul_rn((double)y, ifx)), h - 1);
+    const int sx = min((int)floor(__dmul_rn((double)x, ifx)), w - 1);
+    dst[p] = (long long)(unsigned char)src[(size_t)sy * Wp + sx];
+  }
+}
+
 }  // namespace ups
 
 extern "C" int upsnet_unified_pan_workspace_bytes(int num_seg_classes, size_t* bytes) {
@@ -213,6 +232,19 @@ extern "C" int upsnet_prep_image(const unsigned char* image_hwc, int h, int w, d
   if (blocks > (size_t)ups::kNumSMs * 16) blocks = (size_t)ups::kNumSMs * 16;
   ups::prep_image_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(image_hwc, h, w, out_h, out_w, pad_h, pad_w, 1.0 / scale,
                                                                               pixel_means[0], pixel_means[1], pixel_means[2], blob);
+  UPS_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int upsnet_label_restore(const long long* src0, const long long* src1, int Hp, int Wp, int h, int w, double fx,
+                                    int out_h, int out_w, long long* dst0, long long* dst1, void* stream) {
+  if (!src0 || !dst0 || (!src1) != (!dst1)) return UPSNET_E_BADARG;
+  if (h <= 0 || w <= 0 || h > Hp || w > Wp || out_h <= 0 || out_w <= 0 || !(fx > 0.0)) return UPSNET_E_BADARG;
+  const size_t n = (size_t)out_h * out_w;
+  size_t blocks = (n + 255) / 256;
+  if (blocks > (size_t)ups::kNumSMs * 8) blocks = (size_t)ups::kNumSMs * 8;
+  const dim3 grid((unsigned)blocks, src1 ? 2 : 1);
+  ups::label_restore_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src0, src1, Wp, h, w, 1.0 / fx, out_h, out_w, dst0, dst1);
   UPS_CHECK_LAUNCH();
   return 0;
 }

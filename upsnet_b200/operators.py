@@ -1244,6 +1244,42 @@ def prep_image(image_hwc_u8, pixel_means, scale=1.0, stride=32):
     return blob, (ho, wo)
 
 
+def label_restore_geometry(im_info):
+    """(h, w, fx, out_h, out_w) of upsnet_end2end_test.py:259-266 for one im_info row [h, w, scale].  im_info is float32
+    in the reference (coco.py:145-147), so fx = 1 / im_info[2] is a float32 that cv2 receives as a double, and the crop
+    is int() of the float32 entries; the output size is cv2's cvRound(h * fx) (half to even)."""
+    info = np.asarray(im_info, dtype=np.float32).reshape(-1)[:3]
+    h, w = int(info[0]), int(info[1])
+    fx = float(np.float32(1) / info[2])
+    return h, w, fx, int(np.rint(h * fx)), int(np.rint(w * fx))
+
+
+def label_restore(label_map, im_info, *more_maps):
+    """upsnet_end2end_test.py:259-266 on the device: crop an int64 label map [Hp,Wp] (or [1,Hp,Wp]) to im_info[:2],
+    wrap it to uint8 like astype('uint8') and resize it back to the original image size with cv2's INTER_NEAREST rule.
+    Returns int64 with the input's leading dimensions and [out_h,out_w] last, so it feeds unified_pan_result unchanged.
+    A second map of the same shape may follow im_info: both are restored in one launch and a tuple is returned."""
+    assert len(more_maps) <= 1, "label_restore takes one or two maps"
+    maps = (label_map,) + tuple(more_maps)
+    require_cuda(*maps)
+    Hp, Wp = int(label_map.shape[-2]), int(label_map.shape[-1])
+    lead = tuple(label_map.shape[:-2])
+    srcs = []
+    for m in maps:
+        assert tuple(m.shape) == tuple(label_map.shape) and m.numel() == Hp * Wp, "one [Hp,Wp] map per call"
+        srcs.append(m.reshape(Hp, Wp).to(torch.int64).contiguous())
+    h, w, fx, oh, ow = label_restore_geometry(im_info)
+    if not (0 < h <= Hp and 0 < w <= Wp):
+        raise ValueError("im_info crop (%d, %d) outside the %dx%d label map" % (h, w, Hp, Wp))
+    dev = srcs[0].device
+    outs = [torch.empty(lead + (oh, ow), dtype=torch.int64, device=dev) for _ in srcs]
+    two = len(srcs) == 2
+    with torch.cuda.device(dev), _Timed("label_restore", 1, {"bytes": 16.0 * oh * ow * len(srcs)}, dev):
+        check(lib().upsnet_label_restore(ptr(srcs[0]), ptr(srcs[1] if two else None), Hp, Wp, h, w, fx, oh, ow,
+                                         ptr(outs[0]), ptr(outs[1] if two else None), stream_ptr(dev)), "label_restore")
+    return tuple(outs) if two else outs[0]
+
+
 # ------------------------------------------------------------------------------------------------
 # Row f4: im_post (upsnet_end2end_test.py:95-152) -- mask paste + COCO RLE
 # ------------------------------------------------------------------------------------------------

@@ -23,10 +23,14 @@ class PipelinedEngine:
     PIXEL_MEANS = (102.9801, 115.9465, 122.7717)     # config.network.pixel_means (BGR, caffe models)
 
     def __init__(self, model, im_info, depth=2, with_masks=False, with_unified=False, stuff_area_limit=4 * 64 * 64,
-                 pixel_means=None, im_scale=1.0, lanes=None, label_maps=True):
+                 pixel_means=None, im_scale=1.0, lanes=None, label_maps=True, restore_size=False):
         """with_unified: also run get_unified_pan_result on the device (base_dataset.py:332-371) and return its uint8
         [H,W,3] map as 'pan_2ch'.  submit() also accepts the RAW uint8 [h,w,3] BGR image (pinned): mean subtraction,
-        resize by im_scale and padding (prep_im_for_blob / im_list_to_blob) then run on the device after a 4x smaller H2D."""
+        resize by im_scale and padding (prep_im_for_blob / im_list_to_blob) then run on the device after a 4x smaller H2D.
+        restore_size: crop the two label maps to im_info[:2] and resize them back to the original image size
+        (upsnet_end2end_test.py:259-266, one label_restore launch) before they are returned and before pan_2ch is
+        computed from them, as the reference does before its PQ evaluation; needed whenever im_info's scale != 1 or
+        the network input is padded."""
         self.model, self.depth = model, depth
         # engine lanes: slot i computes on lane i % lanes (own CUDA-graph instance, activation pool, scratch, stream), so the
         # forward passes of `lanes` consecutive images overlap on the GPU; lanes=1 is the strictly serial compute of round 1
@@ -36,7 +40,7 @@ class PipelinedEngine:
         if not label_maps:      # serving format: the unified 2-channel map replaces the two int64 label maps on the way out
             assert with_unified, "label_maps=False needs with_unified=True (pan_2ch carries class and instance id)"
             self.keys = tuple(k for k in self.keys if k not in ("panoptic_outputs", "fcn_outputs"))
-        self.with_unified, self.stuff_area_limit = with_unified, stuff_area_limit
+        self.with_unified, self.stuff_area_limit, self.restore_size = with_unified, stuff_area_limit, restore_size
         self.pixel_means, self.im_scale = (pixel_means or self.PIXEL_MEANS), float(im_scale)
         self.dev = None
         self._t = 0
@@ -112,8 +116,11 @@ class PipelinedEngine:
         return self._t - 1
 
     def _post(self, out):
+        from . import operators as ops
+        if self.restore_size:
+            out["fcn_outputs"], out["panoptic_outputs"] = ops.label_restore(out["fcn_outputs"], self.im_info,
+                                                                            out["panoptic_outputs"])
         if self.with_unified:
-            from . import operators as ops
             m = self.model
             out["pan_2ch"] = ops.unified_pan_result(out["fcn_outputs"], out["panoptic_outputs"], out["p_cls"][out["keep"]],
                                                     m.num_seg_classes, m.num_classes, self.stuff_area_limit,
