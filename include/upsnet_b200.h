@@ -152,6 +152,12 @@ int upsnet_igemm_forward(const void *x_nhwc, const float *offset, const float *m
                          int N, int H, int W, int Cin, int Cout, int kh, int kw, int stride_h,
                          int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int out_layout,
                          int x_dtype, int y_dtype, int epi_flags, int precision, void *stream);
+/* Tuning hook of the TMA-fed dense path of upsnet_igemm_forward (csrc/igemm_tma.cu): output-channel tile of the following
+ * launches in this process.  0 (default) = chosen per launch (the widest tile that still gives ~2/3 of the SMs a tile and,
+ * for pair activations, a ring of at least three stages); 64 or 128 = that tile wherever Cout rounded up is a multiple of it.
+ * A forced tile that does not fit in shared memory is narrowed as the launch's own choice is.  Results are the same for
+ * every choice.  UPSNET_E_BADARG for other values. */
+int upsnet_tma_set_tile_n(int bn);
 
 /* ---------------------------------------------------------------------------------------
  * Deformable convolution v1 / v2 on hi/lo PAIR activations with the bilinear corners gathered from a shared-memory

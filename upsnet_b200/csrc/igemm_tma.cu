@@ -11,7 +11,8 @@
 //   D[128 x BN] fp32 in registers  +=  A * B^T     wgmma m64nBNk16, two warpgroups (tile rows 0-63 / 64-127)
 //   epilogue (same 8 warps): accumulators -> fp32 staging rows in smem -> thread = accumulator row: +bias (+residual
 //            slab, TMA-prefetched) -> ReLU -> bf16 -> SWIZZLE_128B slab in smem -> cp.async.bulk.tensor.4d store
-//            (clips the box at the borders)
+//            (clips the box at the borders); hi/lo pair outputs skip the staging: the same steps run on the fragments
+//            and write the (hi, lo) slabs from registers
 //
 // Both operands land in the K-major SWIZZLE_128B layout the wgmma descriptors expect (the TMA swizzle mode and
 // the smem descriptor's layout type are the same permutation), so no thread touches the operands: 2 service
@@ -57,9 +58,9 @@ struct TmaGeom {
   int pg;                               // output / residual pair group G: channels stored [hi G][lo G] per group (G = Cout normally)
   int res_inplace;                      // residual slabs are TMA-loaded into the (double-buffered) output slabs and updated in place
   int opairs;                           // output slab pairs that alternate (2, or 1 when shared memory is short)
-  // pair mode (N tile <= 64): the hi*hi and hi*lo products share ONE instruction -- B operand = the contiguous [W_hi ; W_lo]
-  // tile of the stage (N = 2 BN), accumulated in columns [0, 2 BN); lo*hi goes to columns [0, BN); the consumers add the two
-  // column groups in registers before the accumulators are staged.  Two wgmma per K slice instead of three.
+  // pair mode: the hi*hi and hi*lo products share ONE instruction -- B operand = the contiguous [W_hi ; W_lo] tile of the
+  // stage (N = 2 BN <= 256), accumulated in columns [0, 2 BN); lo*hi goes to columns [0, BN); the consumers add the two
+  // column groups in registers and the slab epilogue works on the fragments.  Two wgmma per K slice instead of three.
   int wide;
 };
 
@@ -71,8 +72,9 @@ struct TmaSmem {
   uint32_t a_half, b_half;                                   // pair mode: offset of the lo tile inside an A / B slot
   uint32_t oslabs, res_slab;                                 // pair mode: number of (hi, lo) output slab pairs; bytes per residual slab
 };
-// Accumulator staging: 128 rows of BN fp32 (wide mode adds its two column groups in registers first), no padding -- the
-// 16-byte chunk j of row r sits at chunk j ^ (r & 7), so the row-per-lane reads of the epilogue are conflict-free.
+// Accumulator staging (bf16-stream slab epilogue, direct-store epilogue): 128 rows of BN fp32 (wide mode adds its two column
+// groups in registers first), no padding -- the 16-byte chunk j of row r sits at chunk j ^ (r & 7), so the row-per-lane reads
+// of the epilogue are conflict-free.
 template <int N, int W>   // fragment of m64nN, columns [0, W) staged
 __device__ __forceinline__ void acc_stage_sw(const float (&d)[N / 2], float* buf, int row0) {
   const int t = threadIdx.x & 127, l = t & 31;
@@ -120,13 +122,14 @@ __host__ __device__ inline TmaSmem tma_smem_layout(int BN, int stages, bool has_
     s.res = s.out + out_slabs * TM_SLAB_BYTES;
     s.acc = s.res + (has_res ? 2u * (uint32_t)(BN / 64) * TM_SLAB_BYTES : 0u);   // two residual buffers (prefetch)
   }
-  s.total = s.acc + 128u * (uint32_t)BN * 4u;
+  // the pair slab epilogue writes the slabs straight from the fragments: no staging rows
+  s.total = s.acc + ((x3 && !direct) ? 0u : 128u * (uint32_t)BN * 4u);
   return s;
 }
 
 // Roles (10 warps): warps 0-7 consumers -- two wgmma warpgroups (tile rows [64 wg, 64 wg + 64)), then the epilogue
-// (thread = accumulator row q * 32 + lane with q = warp & 3; column half = warp >> 2); warp 8 TMA operand loads, warp 9
-// residual-slab loads.
+// (pair slabs: on the fragments; staged epilogues: thread = accumulator row q * 32 + lane with q = warp & 3, column
+// half = warp >> 2); warp 8 TMA operand loads, warp 9 residual-slab loads.
 // Barriers: full[s]/empty[s] smem ring (TMA <-> consumers), rfull/rempty residual slabs (TMA <-> epilogue).
 // N: accumulator columns (BN, or 2 BN in wide mode), the width of the wgmma instructions.  MMA: TM_MMA_* (the products
 // issued per K slice), a template parameter so that no run-time branch sits between the wgmmas of a k-block.
@@ -256,9 +259,11 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
     const uint32_t ah16 = L.a_half >> 4;       // pair mode: lo A tile offset (descriptor units)
     float* accbuf = reinterpret_cast<float*>(sm + L.acc);
     constexpr int SW = MMA == TM_MMA_WIDE ? N / 2 : N;        // staged columns (= BN)
+    // the pair slab epilogue reads the fragments; the bf16-stream and direct-store epilogues read staged rows
+    const bool staged = MMA != TM_MMA_WIDE || g.direct;
     float d[N / 2];
     uint32_t s = 0, ph = 0;
-    // main loop of one tile, then its accumulators -> staging rows (all eight warps take part)
+    // main loop of one tile, then (staged epilogues) its accumulators -> staging rows (all eight warps take part)
     auto mainloop = [&]() {
       int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
@@ -287,12 +292,16 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
       wgmma_fence_acc(d);
       if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
       if constexpr (MMA == TM_MMA_WIDE) {        // hi*hi + lo*hi (columns [0, BN)) + hi*lo (columns [BN, 2 BN)): same thread
+        // Zeroing the folded group ends its live range here (the next tile's first wgmma overwrites it, but the compiler
+        // cannot see that): with N = 256 the epilogue then holds 64 accumulators instead of 128 and nothing spills.
 #pragma unroll
-        for (int i = 0; i < N / 4; ++i) d[i] += d[N / 4 + i];
+        for (int i = 0; i < N / 4; ++i) { d[i] += d[N / 4 + i]; d[N / 4 + i] = 0.f; }
       }
-      named_bar(3, 256);                    // the previous tile's epilogue has read the staging rows
-      acc_stage_sw<N, SW>(d, accbuf, wg * 64);
-      named_bar(3, 256);
+      if (staged) {
+        named_bar(3, 256);                  // the previous tile's epilogue has read the staging rows
+        acc_stage_sw<N, SW>(d, accbuf, wg * 64);
+        named_bar(3, 256);
+      }
     };
     const int q = warp & 3, half = warp >> 2;
     const int row = q * 32 + lane;
@@ -305,12 +314,20 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
     const uint32_t out_slab = base + L.out + (g.BN == 64 ? 0u : (uint32_t)half * TM_SLAB_BYTES);
     const uint32_t sw_row = (uint32_t)row * 128u;
     const uint32_t rx = (uint32_t)(row & 7);
-    int rrow = row;                                    // row of the residual slab this accumulator row reads
-    if (g.res_up2) {
-      const int w = row % g.bw, h = (row / g.bw) % g.bh, n = row / (g.bw * g.bh);
-      rrow = (w >> 1) + (g.bw >> 1) * ((h >> 1) + (g.bh >> 1) * n);
-    }
+    auto res_row = [&](int r) {                        // row of the residual slab that accumulator row r reads
+      if (!g.res_up2) return r;
+      const int w = r % g.bw, h = (r / g.bw) % g.bh, n = r / (g.bw * g.bh);
+      return (w >> 1) + (g.bw >> 1) * ((h >> 1) + (g.bh >> 1) * n);
+    };
+    const int rrow = res_row(row);
     const uint32_t rs_row = (uint32_t)rrow * 128u, rrx = (uint32_t)(rrow & 7);
+    // pair slab epilogue: byte offsets of this thread's two fragment rows in a slab, and of the residual rows they read
+    uint32_t fr_row[2], fr_res[2], fr_rx[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * h, rr = res_row(r);
+      fr_row[h] = (uint32_t)r * 128u; fr_res[h] = (uint32_t)rr * 128u; fr_rx[h] = (uint32_t)(rr & 7);
+    }
     uint32_t ti_local = 0, oc = 0;
     for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++ti_local) {
       const int nt = (int)(tile % g.n_tiles);
@@ -350,20 +367,19 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
         }
         continue;
       }
-      if (g.x3) {
-        // ---- pair epilogue: all eight warps share one 64-channel (hi, lo) slab pair at a time; half h owns its columns
-        //      [32h, 32h + 32).  fp32 result -> hi = bf16(o), lo = bf16(o - hi) -> two swizzled slabs -> two TMA stores ----
-        const int nslab = g.BN / 64;
-        const uint32_t jb = (uint32_t)half * 4u;
+      if constexpr (MMA == TM_MMA_WIDE) {
+        // ---- pair slab epilogue, on the fragments: all eight warps share one 64-channel (hi, lo) slab pair at a time, each
+        //      thread holds rows fr[h] and, per 8-column group j of the slab, columns 8 j + cq + {0, 1}.
+        //      fp32 result -> hi = bf16(o), lo = bf16(o - hi) -> one bf16x2 word per slab, at chunk j ^ (row & 7): the 8 rows
+        //      of a store instruction hit 8 distinct chunks (conflict-free) -> two TMA stores per slab pair ----
         const bool lead = warp == 0 && lane == 0;
-        for (int sl = 0; sl < nslab; ++sl, ++oc) {
-          const int u = 2 * sl + half;
-          uint32_t v0[16], v1[16];
-          acc_ld16_sw(trow, row, u * 32, v0);
-          acc_ld16_sw(trow, row, u * 32 + 16, v1);
+        const uint32_t cq4 = (uint32_t)(lane & 3) * 4u;      // byte offset of the column pair inside a 16-byte chunk
+        const uint32_t fx = (uint32_t)(lane >> 2);           // fragment row & 7 (both rows)
+#pragma unroll
+        for (int sl = 0; sl < SW / 64; ++sl, ++oc) {
           uint32_t ob;
           if (g.res_inplace) {
-            ob = base + L.out + (buf * (uint32_t)nslab + (uint32_t)sl) * 2u * TM_SLAB_BYTES;   // holds this slab's residual
+            ob = base + L.out + (buf * (uint32_t)(SW / 64) + (uint32_t)sl) * 2u * TM_SLAB_BYTES;   // holds this slab's residual
           } else {
             ob = base + L.out + (g.opairs == 2 ? (oc & 1u) : 0u) * 2u * TM_SLAB_BYTES;
             if (lead) {                             // the stores that last used this pair have finished reading it
@@ -371,47 +387,32 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
             }
             named_bar(1, 256);
           }
-          float o[32];
 #pragma unroll
-          for (int e = 0; e < 16; ++e) { o[e] = __uint_as_float(v0[e]); o[16 + e] = __uint_as_float(v1[e]); }
-          if (g.bias) {
-            const float4* bp = reinterpret_cast<const float4*>(g.bias + n0 + u * 32);
+          for (int j = 0; j < 8; ++j) {
+            const int i = 8 * sl + j;                        // fragment column group
+            float2 bv = make_float2(0.f, 0.f);
+            if (g.bias) bv = __ldg(reinterpret_cast<const float2*>(g.bias + n0 + 8 * i) + (lane & 3));
 #pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const float4 b4 = __ldg(bp + e);
-              o[4 * e] += b4.x; o[4 * e + 1] += b4.y; o[4 * e + 2] += b4.z; o[4 * e + 3] += b4.w;
-            }
-          }
-          if (g.has_res) {
-            uint32_t rh, rl, xr;
-            if (g.res_inplace) { rh = ob + sw_row; rl = rh + TM_SLAB_BYTES; xr = rx; }
-            else { rh = base + L.res + (buf * (uint32_t)nslab + (uint32_t)sl) * 2u * L.res_slab + rs_row; rl = rh + L.res_slab; xr = rrx; }
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const uint4 hv = lds128(rh + (((jb + c) ^ xr) << 4)), lv = lds128(rl + (((jb + c) ^ xr) << 4));
-              const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w}, lw[4] = {lv.x, lv.y, lv.z, lv.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                o[c * 8 + 2 * e] += __uint_as_float(hw[e] << 16) + __uint_as_float(lw[e] << 16);
-                o[c * 8 + 2 * e + 1] += __uint_as_float(hw[e] & 0xffff0000u) + __uint_as_float(lw[e] & 0xffff0000u);
+            for (int h = 0; h < 2; ++h) {
+              float a = d[4 * i + 2 * h], b = d[4 * i + 2 * h + 1];
+              const uint32_t oa = ob + fr_row[h] + (((uint32_t)j ^ fx) << 4) + cq4;
+              if (g.bias) { a += bv.x; b += bv.y; }
+              if (g.has_res) {
+                uint32_t hw, lw;
+                if (g.res_inplace) { hw = lds32(oa); lw = lds32(oa + TM_SLAB_BYTES); }
+                else {
+                  const uint32_t ra = base + L.res + (buf * (uint32_t)(SW / 64) + (uint32_t)sl) * 2u * L.res_slab + fr_res[h];
+                  hw = lds32(ra + (((uint32_t)j ^ fr_rx[h]) << 4) + cq4);
+                  lw = lds32(ra + L.res_slab + (((uint32_t)j ^ fr_rx[h]) << 4) + cq4);
+                }
+                a += __uint_as_float(hw << 16) + __uint_as_float(lw << 16);
+                b += __uint_as_float(hw & 0xffff0000u) + __uint_as_float(lw & 0xffff0000u);
               }
+              if (g.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
+              const uint32_t hw = pack_bf16x2(a, b);
+              sts32(oa, hw);
+              sts32(oa + TM_SLAB_BYTES, pack_bf16x2(a - __uint_as_float(hw << 16), b - __uint_as_float(hw & 0xffff0000u)));
             }
-          }
-          if (g.relu) {
-#pragma unroll
-            for (int e = 0; e < 32; ++e) o[e] = fmaxf(o[e], 0.f);
-          }
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint32_t hw[4], lw[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float a = o[c * 8 + 2 * e], b = o[c * 8 + 2 * e + 1];
-              hw[e] = pack_bf16x2(a, b);
-              lw[e] = pack_bf16x2(a - __uint_as_float(hw[e] << 16), b - __uint_as_float(hw[e] & 0xffff0000u));
-            }
-            sts128(ob + sw_row + (((jb + c) ^ rx) << 4), make_uint4(hw[0], hw[1], hw[2], hw[3]));
-            sts128(ob + TM_SLAB_BYTES + sw_row + (((jb + c) ^ rx) << 4), make_uint4(lw[0], lw[1], lw[2], lw[3]));
           }
           fence_proxy_async();
           named_bar(1, 256);
@@ -428,66 +429,66 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
           bulk_wait_read0();
           mbar_arrive(bar_rempty + 8 * buf);
         }
-        continue;
-      }
-      for (int ui = 0; ui < upw; ++ui) {
-        const int u = half * upw + ui;
-        const int slab = u >> 1;
-        const uint32_t jb = (uint32_t)(u & 1) * 4u;     // first 16-byte chunk of this unit inside the slab row
-        uint32_t v0[16], v1[16];
-        acc_ld16_sw(trow, row, u * 32, v0);
-        acc_ld16_sw(trow, row, u * 32 + 16, v1);
-        if ((u & 1) == 0 || g.BN == 64) {
-          // the output slab is about to be overwritten: its previous TMA store must have finished reading it
-          if (leader) bulk_wait_read0();
-          named_bar(bar_id, bar_cnt);
-        }
-        float o[32];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) { o[e] = __uint_as_float(v0[e]); o[16 + e] = __uint_as_float(v1[e]); }
-        if (g.bias) {
-          const float4* bp = reinterpret_cast<const float4*>(g.bias + n0 + u * 32);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const float4 b4 = __ldg(bp + e);
-            o[4 * e] += b4.x; o[4 * e + 1] += b4.y; o[4 * e + 2] += b4.z; o[4 * e + 3] += b4.w;
+      } else {
+        for (int ui = 0; ui < upw; ++ui) {
+          const int u = half * upw + ui;
+          const int slab = u >> 1;
+          const uint32_t jb = (uint32_t)(u & 1) * 4u;     // first 16-byte chunk of this unit inside the slab row
+          uint32_t v0[16], v1[16];
+          acc_ld16_sw(trow, row, u * 32, v0);
+          acc_ld16_sw(trow, row, u * 32 + 16, v1);
+          if ((u & 1) == 0 || g.BN == 64) {
+            // the output slab is about to be overwritten: its previous TMA store must have finished reading it
+            if (leader) bulk_wait_read0();
+            named_bar(bar_id, bar_cnt);
           }
-        }
-        if (g.has_res) {
-          const uint32_t rs = base + L.res + (buf * (uint32_t)(g.BN / 64) + (uint32_t)slab) * TM_SLAB_BYTES + rs_row;
-#pragma unroll
+          float o[32];
+  #pragma unroll
+          for (int e = 0; e < 16; ++e) { o[e] = __uint_as_float(v0[e]); o[16 + e] = __uint_as_float(v1[e]); }
+          if (g.bias) {
+            const float4* bp = reinterpret_cast<const float4*>(g.bias + n0 + u * 32);
+  #pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const float4 b4 = __ldg(bp + e);
+              o[4 * e] += b4.x; o[4 * e + 1] += b4.y; o[4 * e + 2] += b4.z; o[4 * e + 3] += b4.w;
+            }
+          }
+          if (g.has_res) {
+            const uint32_t rs = base + L.res + (buf * (uint32_t)(g.BN / 64) + (uint32_t)slab) * TM_SLAB_BYTES + rs_row;
+  #pragma unroll
+            for (int c = 0; c < 4; ++c) {
+              const uint4 rv = lds128(rs + (((jb + c) ^ rrx) << 4));
+              const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
+  #pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                o[c * 8 + 2 * e] += __uint_as_float(rw[e] << 16);
+                o[c * 8 + 2 * e + 1] += __uint_as_float(rw[e] & 0xffff0000u);
+              }
+            }
+          }
+          if (g.relu) {
+  #pragma unroll
+            for (int e = 0; e < 32; ++e) o[e] = fmaxf(o[e], 0.f);
+          }
+  #pragma unroll
           for (int c = 0; c < 4; ++c) {
-            const uint4 rv = lds128(rs + (((jb + c) ^ rrx) << 4));
-            const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              o[c * 8 + 2 * e] += __uint_as_float(rw[e] << 16);
-              o[c * 8 + 2 * e + 1] += __uint_as_float(rw[e] & 0xffff0000u);
+            uint4 w;
+            w.x = pack_bf16x2(o[c * 8], o[c * 8 + 1]); w.y = pack_bf16x2(o[c * 8 + 2], o[c * 8 + 3]);
+            w.z = pack_bf16x2(o[c * 8 + 4], o[c * 8 + 5]); w.w = pack_bf16x2(o[c * 8 + 6], o[c * 8 + 7]);
+            sts128(out_slab + sw_row + (((jb + c) ^ rx) << 4), w);
+          }
+          if ((u & 1) == 1 || g.BN == 64) {
+            fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA store
+            named_bar(bar_id, bar_cnt);
+            if (leader) {
+              tma_store_4d(&tm_y, out_slab, n0 + slab * 64, w0, h0, i0);
+              bulk_commit();
             }
           }
         }
-        if (g.relu) {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) o[e] = fmaxf(o[e], 0.f);
-        }
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint4 w;
-          w.x = pack_bf16x2(o[c * 8], o[c * 8 + 1]); w.y = pack_bf16x2(o[c * 8 + 2], o[c * 8 + 3]);
-          w.z = pack_bf16x2(o[c * 8 + 4], o[c * 8 + 5]); w.w = pack_bf16x2(o[c * 8 + 6], o[c * 8 + 7]);
-          sts128(out_slab + sw_row + (((jb + c) ^ rx) << 4), w);
-        }
-        if ((u & 1) == 1 || g.BN == 64) {
-          fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA store
-          named_bar(bar_id, bar_cnt);
-          if (leader) {
-            tma_store_4d(&tm_y, out_slab, n0 + slab * 64, w0, h0, i0);
-            bulk_commit();
-          }
-        }
+        __syncwarp();
+        if (lane == 0 && g.has_res) mbar_arrive(bar_rempty + 8 * buf);
       }
-      __syncwarp();
-      if (lane == 0 && g.has_res) mbar_arrive(bar_rempty + 8 * buf);
     }
     if (leader || (g.x3 && warp == 0 && lane == 0)) bulk_wait0();
   }
@@ -548,6 +549,7 @@ static int tma_launch(int BN, dim3 grid, size_t smem, cudaStream_t stream, const
   if (g.wide) {
     if (BN == 32) return tma_launch_n<64, TM_MMA_WIDE>(grid, smem, stream, tm_x, tm_w, tm_y, tm_r, g);
     if (BN == 64) return tma_launch_n<128, TM_MMA_WIDE>(grid, smem, stream, tm_x, tm_w, tm_y, tm_r, g);
+    if (BN == 128) return tma_launch_n<256, TM_MMA_WIDE>(grid, smem, stream, tm_x, tm_w, tm_y, tm_r, g);
   } else {
     if (BN == 32) return tma_launch_n<32, TM_MMA_BF16>(grid, smem, stream, tm_x, tm_w, tm_y, tm_r, g);
     if (BN == 64) return tma_launch_n<64, TM_MMA_BF16>(grid, smem, stream, tm_x, tm_w, tm_y, tm_r, g);
@@ -573,6 +575,10 @@ static bool tma_fit(int BN, bool has_res, bool direct, bool pair, bool res_up2, 
   *stages = st; *opairs = op; *L = lay(st, op);
   return L->total <= cap;
 }
+
+// N tile of the next launches: 0 = chosen per launch (below), 64 or 128 = that N tile wherever Cout rounded up allows it and
+// it fits (else the launch narrows it as it does its own choice).  For tests and tuning: lets one process compare the tiles.
+static int g_tma_force_bn = 0;
 
 int launch_igemm_tma(const TcParams& p, const void* packed, cudaStream_t stream) {
   if (p.no_tma || p.offset) return UPSNET_E_UNSUPPORTED;
@@ -611,21 +617,24 @@ int launch_igemm_tma(const TcParams& p, const void* packed, cudaStream_t stream)
   g.tiles_n = (p.N + g.bn - 1) / g.bn;
   const long long m_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n;
   const int Cout_pad = cout_pad(p.Cout);
-  // N tile <= 128: the accumulators are m64nBN register fragments of two warpgroups (64 floats per thread at 128) and are
-  // staged as 128 x BN fp32 rows in shared memory for the epilogue
+  // N tile <= 128: the accumulators are m64nBN register fragments of two warpgroups (bf16 stream: 64 floats per thread at
+  // 128; pairs: m64n2BN, 128 floats per thread at 128)
   int BN = (Cout_pad % 128 == 0) ? 128 : (Cout_pad % 64 == 0 ? 64 : 32);
   g.x3 = pair ? 1 : 0; g.x_lo = p.Cin; g.w_lo = Cout_pad; g.pg = pg;
   g.res_inplace = (pair && g.has_res && !g.res_up2) ? 1 : 0;
   g.opairs = 2;
-  // pair mode: N tile <= 64, i.e. always wide (two wgmma per K slice).  Measured on H100 SXM, bf16x3 bench: the N = 128 tiles
-  // (2-stage ring, one output slab pair) ran the dense conv family in 9.1-9.2 ms per image, N <= 64 in 8.4-8.5 ms.
-  if (pair && BN > 64) BN = 64;
-  // N tile: as wide as possible (operand bytes per flop fall with BN) while ~2/3 of the SMs still get a tile
-  while (BN > 64 && m_tiles * (Cout_pad / BN) < 88) BN /= 2;
+  if (g_tma_force_bn && Cout_pad % g_tma_force_bn == 0) {
+    BN = g_tma_force_bn;
+  } else {
+    // N tile: as wide as possible (operand bytes per flop fall with BN) while ~2/3 of the SMs still get a tile
+    while (BN > 64 && m_tiles * (Cout_pad / BN) < 88) BN /= 2;
+  }
   g.direct = direct ? 1 : 0; g.y_bf16 = p.y_bf16; g.out_nhwc = p.out_nhwc; g.y = p.y;
   TmaSmem L;
   bool ok = tma_fit(BN, g.has_res != 0, direct, pair, g.res_up2 != 0, g.res_inplace != 0, &g.stages, &g.opairs, &L);
-  while (!ok && BN > 64) {    // a narrower N tile frees staging and operand space
+  // a narrower N tile frees operand, slab and staging space.  Pairs: a 2-stage ring at N = 128 loses to a deeper one at 64
+  // (measured on H100 SXM, bf16x3 bench: N = 128 pair tiles with 2 stages ran the dense conv family 8 % slower than N = 64)
+  while (BN > 64 && (!ok || (pair && g.stages < 3))) {
     BN /= 2;
     ok = tma_fit(BN, g.has_res != 0, direct, pair, g.res_up2 != 0, g.res_inplace != 0, &g.stages, &g.opairs, &L);
   }
@@ -722,6 +731,12 @@ static void stem_geometry(int H, int W, int kh, int kw, int pad, int* Ho, int* W
 }
 
 }  // namespace ups
+
+extern "C" int upsnet_tma_set_tile_n(int bn) {
+  if (bn != 0 && bn != 64 && bn != 128) return UPSNET_E_BADARG;
+  ups::g_tma_force_bn = bn;
+  return 0;
+}
 
 extern "C" int upsnet_stem_workspace_bytes(int N, int H, int W, int kh, int kw, int pad, size_t* bytes) {
   if (!bytes || N <= 0 || H <= 0 || W <= 0 || kh <= 0 || kw <= 0 || kw > 8 || pad < 0) return UPSNET_E_BADARG;
