@@ -180,17 +180,6 @@ int upsnet_dcn_pair_forward(const void *x_pair, const float *offset, const float
  * the GPU has SMs, else 32); 32 or 128 = that tile wherever it applies (128 needs Cout rounded up to 64 to be a multiple of 128).  Results are
  * the same for every choice.  UPSNET_E_BADARG for other values. */
 int upsnet_dcn_set_tile_n(int bn);
-/* Dense 3x3 / stride-1 convolution on hi/lo PAIR activations through the same window pipeline (csrc/dcn_win.cu, DENSE mode):
- * the input window of a 16x8-pixel tile is staged once per 16-channel sub-chunk by TMA and feeds all nine taps, the A operand
- * is copied window -> A operand tile in shared memory.  Meant for the small-N layers (18-channel offset convs of the semantic head, 64->64 bottleneck
- * convs) whose per-tap TMA boxes make upsnet_igemm_forward L2->SM-bandwidth-bound.  x [N,H,W,2*Cin] pair NHWC; `packed`
- * from upsnet_dcn_pack_weight; y = fp32 NCHW [N,Cout,Ho,Wo] (UPSNET_LAYOUT_NCHW, any Cout) or pair NHWC [N,Ho,Wo,2*Cout]
- * (UPSNET_LAYOUT_NHWC, Cout % 16 == 0); epi_flags: UPSNET_EPI_RELU.  Same arithmetic contract as upsnet_igemm_forward
- * (precision UPSNET_PREC_BF16X3).  UPSNET_E_UNSUPPORTED for other shapes (dilation > 7, Cin % 64 != 0).
- * replaces: the cuDNN 3x3 convs of models/fcn.py:40-55 (conv_offset) and models/resnet.py:80-100 (conv2). */
-int upsnet_conv3x3_pair_forward(const void *x_pair, const void *packed, const float *bias, void *y, int N, int H, int W,
-                                int Cin, int Cout, int pad_h, int pad_w, int dil_h, int dil_w, int out_layout,
-                                int epi_flags, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * Parameter-free panoptic head, fused: MaskRemoval + SegTerm + void/concat/argmax.

@@ -126,44 +126,3 @@ def test_window_dcn_c_abi_rejects_other_shapes(dev):
     assert lib().upsnet_dcn_packed_weight_bytes(128, 256, 1, 1, C.byref(nb)) == -2      # 3x3 only
     assert lib().upsnet_dcn_packed_weight_bytes(128, 96, 3, 3, C.byref(nb)) == -2       # Cin % 64
     assert lib().upsnet_dcn_packed_weight_bytes(20, 64, 3, 3, C.byref(nb)) == 0 and nb.value == 2 * 32 * 9 * 64 * 2   # rows padded to 32
-
-
-DENSE_CASES = [
-    dict(N=1, Cin=256, Cout=18, H=32, W=48, pd=1, nchw=True, relu=False),      # offset conv of the semantic head (a12)
-    dict(N=1, Cin=128, Cout=18, H=25, W=42, pd=1, nchw=True, relu=False),      # ragged tiles
-    dict(N=2, Cin=64, Cout=64, H=40, W=56, pd=1, nchw=False, relu=True),       # res2 conv2 shape class: pair out + ReLU
-    dict(N=1, Cin=64, Cout=32, H=20, W=20, pd=2, nchw=False, relu=False),      # dilation 2, N tile 32, pair out
-    dict(N=1, Cin=128, Cout=27, H=9, W=7, pd=1, nchw=True, relu=True),         # map smaller than a tile, odd Cout
-    dict(N=3, Cin=64, Cout=18, H=64, W=96, pd=1, nchw=True, relu=False),       # > 132 tiles
-    dict(N=1, Cin=512, Cout=18, H=16, W=24, pd=1, nchw=True, relu=False),      # 72 k-blocks
-]
-
-
-@pytest.mark.parametrize("cfg", DENSE_CASES)
-def test_window_dense_conv_vs_oracle(dev, pair_mode, cfg):
-    """DENSE mode of the window kernel (upsnet_conv3x3_pair_forward) against the CPU oracle convolution and against the
-    per-tap TMA kernel it replaces for small-N layers."""
-    U = pair_mode
-    from upsnet_b200 import operators as ops
-    rng = np.random.default_rng(33)
-    N, Cin, Cout, H, W, pd = cfg["N"], cfg["Cin"], cfg["Cout"], cfg["H"], cfg["W"], cfg["pd"]
-    x, w, b = _case(rng, N, Cin, Cout, H, W)
-    want = O.conv2d(x, w, b, 1, pd, pd)
-    if cfg["relu"]:
-        want = np.maximum(want, 0)
-    xp = ops.Pair.from_float(t(x, dev))
-    was = dict(ops.DENSE_WINDOW)
-    ops.DENSE_WINDOW.update(on=True, min_pixels=0)
-    try:
-        l0 = ops.STATS["launches"]
-        got = U.conv2d(xp, t(w, dev), t(b, dev), 1, pd, pd, relu=cfg["relu"], precision=X3, out_format="nchw" if cfg["nchw"] else None)
-        assert ops.STATS["launches"] > l0
-        ops.DENSE_WINDOW["on"] = False
-        ref = U.conv2d(xp, t(w, dev), t(b, dev), 1, pd, pd, relu=cfg["relu"], precision=X3, out_format="nchw" if cfg["nchw"] else None)
-    finally:
-        ops.DENSE_WINDOW.update(was)
-    assert isinstance(got, ops.Pair) != cfg["nchw"]
-    g = got.float().cpu().numpy()
-    assert g.shape == want.shape
-    assert np.abs(g - want).max() < 1e-4
-    assert np.abs(ref.float().cpu().numpy() - g).max() < 1e-4

@@ -58,7 +58,6 @@ def lib():
         L.upsnet_dcn_pair_forward.argtypes = [vp] * 6 + [i] * 12 + [vp]
         L.upsnet_dcn_set_tile_n.argtypes = [i]
         L.upsnet_tma_set_tile_n.argtypes = [i]
-        L.upsnet_conv3x3_pair_forward.argtypes = [vp] * 4 + [i] * 11 + [vp]
         L.upsnet_panoptic_workspace_bytes.argtypes = [i, i, i, i, C.POINTER(sz)]
         L.upsnet_panoptic_workspace_min_bytes.argtypes = [i, i, i, i, C.POINTER(sz)]
         L.upsnet_panoptic_head.argtypes = [vp, i, i, i, vp, vp, vp, vp, i, vp, i, d, vp, vp, vp, vp, vp, sz, vp]
@@ -102,7 +101,7 @@ EXPORTED_SYMBOLS = [
     "upsnet_rpn_decode", "upsnet_maskroi_prepare", "upsnet_maskroi_finish", "upsnet_maxpool2d_nhwc", "upsnet_upsample_bilinear_nchw", "upsnet_rpn_topk_workspace_bytes", "upsnet_rpn_topk", "upsnet_rpn_collect", "upsnet_stem_workspace_bytes",
     "upsnet_stem_packed_weight_bytes", "upsnet_stem_pack_weight", "upsnet_stem_forward",
     "upsnet_dcn_im2col", "upsnet_dcn_col2im", "upsnet_dcn_col2im_coord", "upsnet_roi_align_backward",
-    "upsnet_dcn_packed_weight_bytes", "upsnet_dcn_pack_weight", "upsnet_dcn_pair_forward", "upsnet_dcn_set_tile_n", "upsnet_tma_set_tile_n", "upsnet_conv3x3_pair_forward",
+    "upsnet_dcn_packed_weight_bytes", "upsnet_dcn_pack_weight", "upsnet_dcn_pair_forward", "upsnet_dcn_set_tile_n", "upsnet_tma_set_tile_n",
     "upsnet_fcn_score_fuse", "upsnet_unified_pan_workspace_bytes", "upsnet_unified_pan_result", "upsnet_prep_image", "upsnet_im_post_workspace_bytes", "upsnet_im_post_rle",
     "upsnet_label_restore", "upsnet_pq_workspace_bytes", "upsnet_pq_update",
 ]

@@ -22,8 +22,9 @@
 //     m64n128 fragment per thread; per K=16 slice three wgmma -- lo*hi, hi*lo, hi*hi), 8 weight TMA, 9 window TMA,
 //     10-11 idle, 12-19 gather producers.  K = 32 per stage (SWIZZLE_64B), three stages.  The A tile is gathered once
 //     per 128 output channels.
-//   N tile 32 (small maps, Cout not a multiple of 128, DENSE mode): 24 warps.  0-3 consumers (one warpgroup holding both
-//     m64n32 fragments), 4 weight TMA, 5 window TMA, 6-7 idle, 8-23 gather producers.  K = 64 per stage (SWIZZLE_128B).
+//   N tile 32 (small maps, Cout not a multiple of 128): 24 warps.  0-3 consumers (one warpgroup holding both m64n32
+//     fragments), 4 weight TMA, 5 window TMA, 6-7 idle, 8-23 gather producers.  K = 64 per stage (SWIZZLE_128B), two
+//     stages.
 //   The TMA warps and the idle ones form a warpgroup that hands registers to the consumers (setmaxnreg, DwCfg).
 // In both, a producer warp gathers two K=16 slices of 32 tile rows per k-block, and the producers form two groups that
 // fill alternate k-blocks.  After the last k-block of a tile each consumer warpgroup stages its accumulators through
@@ -41,14 +42,23 @@
 namespace ups {
 
 constexpr int DW_BM = 128;            // pixels per M tile
-constexpr int DW_STAGES = 3;          // operand ring depth: A stages (gather warps) and B stages (TMA), both in smem
 constexpr int DW_WW = 32, DW_WH = 20; // window box in pixels; the row pitch (32 px = 1024 B) keeps bank = f(x) only
 constexpr int DW_PLANE = DW_WW * DW_WH * 32;      // one plane (hi or lo) of a window: 16 channels x 2 B per pixel
 constexpr int DW_WIN_BYTES = 2 * DW_PLANE;
+constexpr int DW_WIN_BUFS = 2;        // window buffers: the next fill streams in while the current one is gathered
 constexpr int DW_KHW = 9;
 constexpr int DW_GROUPS = 2;          // producer groups: alternate k-blocks
 constexpr int DW_EPI_PITCH = 36;      // floats per row of the accumulator staging buffer (32 columns + pad)
 constexpr uint32_t DW_EPI_BYTES = DW_BM * DW_EPI_PITCH * 4;
+
+// shared-memory map (byte offsets from the 1024-aligned base); the stages, windows and staging buffer follow (DwCfg)
+constexpr uint32_t DW_OFF_BARS = 0;        // 18 mbarriers
+constexpr uint32_t DW_OFF_STATS = 192;     // 2 x int[8]: min w, min h, max w, max h, sum w, sum h, count, -
+constexpr uint32_t DW_OFF_ORG = 256;       // 2 x int4: window origin (w, h), image, -
+constexpr uint32_t DW_OFF_TW = 512;        // float4 [9][128] corner weights
+constexpr uint32_t DW_OFF_TP = DW_OFF_TW + DW_KHW * DW_BM * 16;   // int [9][128] window byte offset / outlier code
+constexpr uint32_t DW_OFF_STAGES = DW_OFF_TP + DW_KHW * DW_BM * 4;   // 23552 = 23 * 1024
+static_assert(DW_OFF_STAGES % 1024 == 0, "stage buffers need 1024-byte alignment (SWIZZLE_128B)");
 
 // Per-instantiation geometry.  N tile 32: one consumer warpgroup holds both m64 fragments (2 x 16 floats) next to 16
 // gather warps.  N tile 128: an m64n128 fragment is 64 floats per thread, so each tile half gets its own consumer
@@ -80,20 +90,20 @@ template <int BN> struct DwCfg {
   static constexpr uint32_t B_BYTES = BN * ROWB;                 // one weight plane of a stage
   static constexpr uint32_t STAGE_BYTES = 2 * B_BYTES + A_BYTES;
   static_assert(STAGE_BYTES % 1024 == 0, "stages must keep the 1024-byte alignment of the swizzled tiles");
+  // operand ring depth (A stages from the gather warps, B stages from TMA): as many as fit next to the tables, the two
+  // windows and the staging buffer.  N = 32: 23 KB tables + 2 x 40 KB stages (3 do not fit) + 2 x 40 KB windows + 18 KB
+  // staging; N = 128: 23 KB tables + 3 x 32 KB stages + 2 x 40 KB windows + 18 KB staging.
+  static constexpr int STAGES = BN == 128 ? 3 : 2;
+  static_assert(STAGES <= 3, "the barrier map holds three stages");
+  static constexpr uint32_t OFF_WIN = DW_OFF_STAGES + STAGES * STAGE_BYTES;   // window buffers (1024-aligned)
+  static constexpr uint32_t OFF_EPI = OFF_WIN + DW_WIN_BUFS * DW_WIN_BYTES;   // accumulator staging buffer
+  static constexpr uint32_t SMEM = OFF_EPI + DW_EPI_BYTES + 1024;             // + alignment slack of the dynamic base
+  static_assert(SMEM <= 227 * 1024, "shared memory exceeds 227 KB");
 };
 // 16-byte chunk j of A / B row r in a stage: SWIZZLE_128B (128-byte rows) or SWIZZLE_64B (64-byte rows)
 template <int ROWB> __device__ __forceinline__ uint32_t dw_chunk(uint32_t j, uint32_t r) {
   return ROWB == 128 ? (j ^ (r & 7u)) : (j ^ ((r >> 1) & 3u));
 }
-
-// shared-memory map (byte offsets from the 1024-aligned base)
-constexpr uint32_t DW_OFF_BARS = 0;        // 18 mbarriers
-constexpr uint32_t DW_OFF_STATS = 192;     // 2 x int[8]: min w, min h, max w, max h, sum w, sum h, count, -
-constexpr uint32_t DW_OFF_ORG = 256;       // 2 x int4: window origin (w, h), image, -
-constexpr uint32_t DW_OFF_TW = 512;        // float4 [9][128] corner weights
-constexpr uint32_t DW_OFF_TP = DW_OFF_TW + DW_KHW * DW_BM * 16;   // int [9][128] window byte offset / outlier code
-constexpr uint32_t DW_OFF_STAGES = DW_OFF_TP + DW_KHW * DW_BM * 4;   // 23552 = 23 * 1024
-static_assert(DW_OFF_STAGES % 1024 == 0, "stage buffers need 1024-byte alignment (SWIZZLE_128B)");
 
 struct DwParams {
   const void* x;          // pair NHWC [N,H,W,2*Cin] (outlier gathers)
@@ -102,26 +112,13 @@ struct DwParams {
   const float* bias;
   void* y;                // pair NHWC [N,Ho,Wo,2*Cout]
   int N, H, W, Cin, Cout, Cout_pad, Ho, Wo, ph, pw, dh, dw, relu, BN, tile_w, tile_h;
-  // DENSE mode (offset == null): plain 3x3 / stride-1 convolution through the same pipeline -- the window of a tile is its
-  // receptive field (origin = tile origin - pad, known without a sample table), a "gather" is one LDS.128 per plane copied
-  // to the A operand tile, no blend.  Serves the small-N 3x3 layers of the pair stream (18-channel offset convs, 64->64
-  // bottleneck convs), which the per-tap TMA boxes of igemm_tma.cu make L2->SM-bandwidth-bound (A re-fetched per tap).
-  int dense;
-  int out_nchw;           // y = fp32 NCHW [N,Cout,Ho,Wo] (offset maps) instead of the pair NHWC tensor
-  int win_bytes;          // bytes one window fill delivers (both planes): the dense box is only tile + halo rows high
-  int win_h;              // rows of the window box (<= DW_WH)
-  // DENSE mode window geometry: one fill = a 64-channel chunk (four 16-channel sub-chunks), 128-byte pixels, SWIZZLE_128B --
-  // the 32-byte box rows of the deformable window would make the plain copy loop TMA-request-bound (~4.5 cycles per box row)
-  int win_pitch;          // pixels per window row (dense: 24)
-  int win_plane;          // bytes of one plane of a window buffer
-  int win_buf;            // bytes of one window buffer (both planes)
-  int stages;             // operand ring depth (2 or 3)
-  int win_nbuf;           // window buffers (2: the next fill streams in while the current one is gathered; dense mode: 1)
 };
 
+// p is __grid_constant__ so that each field is read from the parameter bank where it is used.  Passed as a plain value,
+// nvcc 12.9 loads the whole struct into registers at kernel entry and keeps it live, and both instantiations spill.
 template <int BN>
 __global__ void __launch_bounds__(DwCfg<BN>::THREADS, 1)
-dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const DwParams p) {
+dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ DwParams p) {
   using C = DwCfg<BN>;
   constexpr int DW_PRODUCERS = C::PRODUCERS, DW_CONSUMERS = C::CONSUMERS;
   constexpr int DW_WARP_TMAB = C::WARP_TMAB, DW_WARP_TMAW = C::WARP_TMAW, DW_WARP_PROD0 = C::WARP_PROD0;
@@ -134,10 +131,9 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t b_bytes = C::B_BYTES;
   const uint32_t stage_bytes = C::STAGE_BYTES;                              // weight tile (hi, lo planes), then the A tiles
-  const uint32_t NST = (uint32_t)p.stages;
-  const uint32_t win_base = base + DW_OFF_STAGES + NST * stage_bytes;       // 1024-aligned (stage_bytes % 1024 == 0)
-  const uint32_t NWB = (uint32_t)p.win_nbuf;
-  float* stf = reinterpret_cast<float*>(sm + (win_base - base) + NWB * (uint32_t)p.win_buf);   // accumulator staging
+  constexpr uint32_t NST = C::STAGES, NWB = DW_WIN_BUFS;
+  const uint32_t win_base = base + C::OFF_WIN;
+  float* stf = reinterpret_cast<float*>(sm + C::OFF_EPI);                   // accumulator staging
   // barriers
   const uint32_t bar_fa = base + DW_OFF_BARS;            // full_a[3]: the producer warps of one group (A stage written)
   const uint32_t bar_fb = bar_fa + 24;                   // full_b[3]: weight TMA (tx)
@@ -151,9 +147,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
   int* tp = reinterpret_cast<int*>(sm + DW_OFF_TP);
 
   const int HoWo = p.Ho * p.Wo;
-  const int nsc = p.Cin / 16;                         // 16-channel sub-chunks
-  const int spf = p.dense ? 4 : 1;                    // sub-chunks per window fill
-  const int nfill = nsc / spf;                        // window fills per tile
+  const int nsc = p.Cin / 16;                         // 16-channel sub-chunks = window fills per tile
   const int num_kb = nsc * DW_KHW / SPK;              // Cin % 64 == 0 -> integral
   const int n_tiles = p.Cout_pad / BN;
   const int TW = p.tile_w, TH = p.tile_h;
@@ -163,7 +157,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
 
   if (warp == 0) {
     if (lane == 0) {
-      for (int s = 0; s < DW_STAGES; ++s) {
+      for (int s = 0; s < C::STAGES; ++s) {
         mbar_init(bar_fa + 8 * s, C::GROUP / 32);
         mbar_init(bar_fb + 8 * s, 1);
         mbar_init(bar_em + 8 * s, DW_CONSUMERS / 32);
@@ -203,22 +197,10 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     uint32_t g0 = 0, wf0 = 0;                    // running k-block / window-fill counters at the start of the tile
     uint32_t wf_ready = 0;                       // window fills [0, wf_ready) have been observed complete by this thread
     uint32_t tile_it = 0;
-    const bool dense = p.dense != 0;
-    if (dense) {
-      // tile-independent table: window offset of (tap, tile pixel) relative to the tile's receptive-field origin
-      for (int e = pt; e < DW_KHW * DW_BM; e += DW_PRODUCERS) {
-        const int tap = e >> 7, rr = e & 127;
-        const int ki = tap / 3, kj = tap - ki * 3;
-        const int ry = min(rr >> tw_shift, TH - 1), rx = rr & (TW - 1);      // rows past the block read a valid (unused) pixel
-        tp[e] = (ry + ki * p.dh) * p.win_pitch + rx + kj * p.dw;      // window PIXEL index
-      }
-      named_bar<1, DW_PRODUCERS>();
-    }
     for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tile_it) {
       const long long mt = tile / n_tiles;
       const int tx = (int)(mt % tiles_w), ty = (int)((mt / tiles_w) % tiles_h), n = (int)(mt / ((long long)tiles_w * tiles_h));
       const int par = (int)(tile_it & 1u);
-      if (!dense) {
       // ---- sample table, phase 1: every thread computes up to TABLE_IT (tap, pixel) entries in registers ----
       constexpr int TIT = C::TABLE_IT;
       float4 ewv[TIT];
@@ -277,7 +259,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
           const int a = st[0], b = st[1], cc = st[2], d = st[3];
           // the bounding box of all corners fits: start the window there; otherwise centre it on the mean sample
           ox = (cc - a + 1 <= DW_WW) ? a : (int)floorf((float)st[4] / (float)c + 1.0f) - DW_WW / 2;
-          oy = (d - b + 1 <= p.win_h) ? b : (int)floorf((float)st[5] / (float)c + 1.0f) - p.win_h / 2;
+          oy = (d - b + 1 <= DW_WH) ? b : (int)floorf((float)st[5] / (float)c + 1.0f) - DW_WH / 2;
         }
       }
 #pragma unroll
@@ -287,7 +269,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
           int code = 0;
           if (evalid[it]) {
             const int dx = ewl[it] - ox, dy = ehl[it] - oy;
-            if (dx >= 0 && dx + 1 < DW_WW && dy >= 0 && dy + 1 < p.win_h) code = (dy * DW_WW + dx) * 32;
+            if (dx >= 0 && dx + 1 < DW_WW && dy >= 0 && dy + 1 < DW_WH) code = (dy * DW_WW + dx) * 32;
             else code = (int)(0x80000000u | ((uint32_t)(ehl[it] + 1) << 15) | (uint32_t)(ewl[it] + 1));   // outlier: global gather
           }
           tw[e] = ewv[it];
@@ -301,7 +283,6 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         mbar_arrive(bar_og + 8 * par);        // release: the window TMA thread may read the origin
       }
       named_bar<1, DW_PRODUCERS>();      // (C) table visible
-      }                       // !dense
       const __nv_bfloat16* ximg = xh + (size_t)n * p.H * p.W * (size_t)(2 * p.Cin);
 
       int rel = 0;            // sub-chunks of this tile this WARP has released
@@ -316,23 +297,14 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
           const int sl = 2 * u + (pass >> 1), half = pass & 1;
           const int q = kb * SPK + sl;                  // slice index: (sub-chunk, tap)
           const int sc = q / DW_KHW, tap = q - sc * DW_KHW;
-          const uint32_t wf = wf0 + (uint32_t)(dense ? (sc >> 2) : sc);      // dense: one fill per 64-channel chunk
+          const uint32_t wf = wf0 + (uint32_t)sc;
           if (wf >= wf_ready) {                         // first touch of this window fill
             mbar_wait(bar_wf + 8 * (wf % NWB), (wf / NWB) & 1u);
             wf_ready = wf + 1;
           }
-          const uint32_t wbuf = win_base + (wf % NWB) * (uint32_t)p.win_buf;
+          const uint32_t wbuf = win_base + (wf % NWB) * (uint32_t)DW_WIN_BYTES;
           const int code = tp[tap * DW_BM + r];
           const uint32_t a_off = dw_chunk<ROWB>((uint32_t)(sl * 2 + half), (uint32_t)r) << 4;   // K elements 16 sl + 8 half ..
-          if (dense) {        // plain copy of the tap's pixel: window -> A operand
-            // SWIZZLE_128B window: a pixel is one 128-byte row (64 channels), 16-byte chunk c sits at c ^ (pixel & 7)
-            const uint32_t pix = (uint32_t)code, ch = (uint32_t)((sc & 3) * 2 + half);
-            const uint32_t al = wbuf + pix * 128u + ((ch ^ (pix & 7u)) << 4);
-            const uint4 h4 = lds128(al), l4 = lds128(al + (uint32_t)p.win_plane);
-            sts128(a_row + a_off, h4);
-            sts128(a_row + DW_BM * ROWB + a_off, l4);
-            continue;
-          }
           const float4 wv = tw[tap * DW_BM + r];
           uint4 hc[4], lc[4];
           if (code >= 0) {
@@ -400,7 +372,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         if (lane == 0) {
           mbar_arrive(bar_fa + 8 * s);
           // window buffers this warp will not read again: its next k-block (kb + 2) starts at slice SPK * (kb + 2)
-          while (rel < nfill && DW_KHW * spf * (rel + 1) <= SPK * (kb + DW_GROUPS)) {
+          while (rel < nsc && DW_KHW * (rel + 1) <= SPK * (kb + DW_GROUPS)) {
             mbar_arrive(bar_we + 8 * ((wf0 + (uint32_t)rel) % NWB));
             ++rel;
           }
@@ -408,11 +380,11 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         rel = __shfl_sync(0xffffffffu, rel, 0);
       }
       if (lane == 0) {
-        while (rel < nfill) { mbar_arrive(bar_we + 8 * ((wf0 + (uint32_t)rel) % NWB)); ++rel; }
+        while (rel < nsc) { mbar_arrive(bar_we + 8 * ((wf0 + (uint32_t)rel) % NWB)); ++rel; }
       }
       __syncwarp();
       g0 += (uint32_t)num_kb;
-      wf0 += (uint32_t)nfill;
+      wf0 += (uint32_t)nsc;
     }
   } else if (warp >= DW_WARP_TMAB) {
     // The TMA warpgroup (weight TMA, window TMA, two idle warps) keeps a minimal register budget so that the consumer
@@ -423,24 +395,16 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
       uint32_t wf = 0, ti = 0;
       for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++ti) {
         const uint32_t par = ti & 1u;
-        int4 o;
-        if (p.dense) {       // receptive-field origin of the tile: no sample table, no hand-shake
-          const long long mt = tile / n_tiles;
-          o = make_int4((int)(mt % tiles_w) * TW - p.pw, (int)((mt / tiles_w) % tiles_h) * TH - p.ph,
-                        (int)(mt / ((long long)tiles_w * tiles_h)), 0);
-        } else {
-          mbar_wait(bar_og + 8 * par, (ti >> 1) & 1u);
-          const volatile int* ov = reinterpret_cast<const volatile int*>(&org[par]);
-          o = make_int4(ov[0], ov[1], ov[2], 0);
-        }
-        const int cstep = 16 * spf;
-        for (int f = 0; f < nfill; ++f, ++wf) {
+        mbar_wait(bar_og + 8 * par, (ti >> 1) & 1u);
+        const volatile int* ov = reinterpret_cast<const volatile int*>(&org[par]);
+        const int4 o = make_int4(ov[0], ov[1], ov[2], 0);
+        for (int f = 0; f < nsc; ++f, ++wf) {
           const uint32_t b = wf % NWB;
           mbar_wait(bar_we + 8 * b, ((wf / NWB) & 1u) ^ 1u);
-          mbar_arrive_expect_tx(bar_wf + 8 * b, (uint32_t)p.win_bytes);
-          const uint32_t dst = win_base + b * (uint32_t)p.win_buf;
-          tma_load_4d(dst, &tm_x, bar_wf + 8 * b, f * cstep, o.x, o.y, o.z);
-          tma_load_4d(dst + (uint32_t)p.win_plane, &tm_x, bar_wf + 8 * b, p.Cin + f * cstep, o.x, o.y, o.z);
+          mbar_arrive_expect_tx(bar_wf + 8 * b, (uint32_t)DW_WIN_BYTES);
+          const uint32_t dst = win_base + b * (uint32_t)DW_WIN_BYTES;
+          tma_load_4d(dst, &tm_x, bar_wf + 8 * b, f * 16, o.x, o.y, o.z);
+          tma_load_4d(dst + (uint32_t)DW_PLANE, &tm_x, bar_wf + 8 * b, p.Cin + f * 16, o.x, o.y, o.z);
         }
       }
     } else if (warp == DW_WARP_TMAB && lane == 0) {
@@ -554,13 +518,6 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
 #pragma unroll
             for (int e = 0; e < 16; ++e) o[e] = fmaxf(o[e], 0.f);
           }
-          if (p.out_nchw) {     // plane-wise fp32 output (offset maps): for a fixed channel the lanes write consecutive pixels
-            float* yf = reinterpret_cast<float*>(p.y) + ((size_t)n * p.Cout + co) * HoWo + (size_t)ho * p.Wo + wo;
-#pragma unroll
-            for (int e = 0; e < 16; ++e)
-              if (co + e < p.Cout) yf[(size_t)e * HoWo] = o[e];
-            continue;
-          }
           uint32_t hw[8], lw[8];
 #pragma unroll
           for (int e = 0; e < 8; ++e) {
@@ -622,8 +579,8 @@ extern "C" int upsnet_dcn_pack_weight(const float* weight, int Cout, int Cin, in
   return 0;
 }
 
-// N tile of the next launches: 0 = chosen per launch (above), 32 or 128 = that N tile wherever it applies (128 needs a
-// deformable layer with Cout_pad % 128 == 0).  For tests and tuning: lets one process compare both instantiations.
+// N tile of the next launches: 0 = chosen per launch (below), 32 or 128 = that N tile wherever it applies (128 needs
+// Cout_pad % 128 == 0).  For tests and tuning: lets one process compare both instantiations.
 static int g_dw_force_bn = 0;
 
 extern "C" int upsnet_dcn_set_tile_n(int bn) {
@@ -632,14 +589,14 @@ extern "C" int upsnet_dcn_set_tile_n(int bn) {
   return 0;
 }
 
-static int dw_launch(const void* x_pair, const float* offset, const float* mask, const void* packed,
-                     const float* bias, void* y_pair, int N, int H, int W, int Cin, int Cout, int kh,
-                     int kw, int pad_h, int pad_w, int dil_h, int dil_w, int epi_flags, bool dense, bool out_nchw, void* stream) {
+extern "C" int upsnet_dcn_pair_forward(const void* x_pair, const float* offset, const float* mask, const void* packed,
+                                       const float* bias, void* y_pair, int N, int H, int W, int Cin, int Cout, int kh,
+                                       int kw, int pad_h, int pad_w, int dil_h, int dil_w, int epi_flags, void* stream) {
   using namespace ups;
-  if (!x_pair || (!dense && !offset) || !packed || !y_pair) return UPSNET_E_BADARG;
+  if (!x_pair || !offset || !packed || !y_pair) return UPSNET_E_BADARG;
   if (N <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0 || pad_h < 0 || pad_w < 0 || dil_h <= 0 || dil_w <= 0) return UPSNET_E_BADARG;
   if (!dw_supported(Cin, Cout, kh, kw)) return UPSNET_E_UNSUPPORTED;
-  if (!out_nchw && (Cout % 16) != 0) return UPSNET_E_UNSUPPORTED;
+  if ((Cout % 16) != 0) return UPSNET_E_UNSUPPORTED;
   if (H >= 32767 || W >= 32767) return UPSNET_E_UNSUPPORTED;                 // outlier code packs (h, w) into 16 + 15 bits
   if ((((uintptr_t)x_pair) & 15) || (((uintptr_t)packed) & 15) || (((uintptr_t)y_pair) & 15) || (bias && (((uintptr_t)bias) & 15)))
     return UPSNET_E_UNSUPPORTED;
@@ -651,16 +608,15 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
   p.Wo = conv_out_size(W, pad_w, dil_w, 3, 1);
   if (p.Ho <= 0 || p.Wo <= 0) return UPSNET_E_BADARG;
   p.relu = (epi_flags & UPSNET_EPI_RELU) ? 1 : 0;
-  p.dense = dense ? 1 : 0; p.out_nchw = out_nchw ? 1 : 0;
   const int sms = num_sms();
   p.tile_w = 16; p.tile_h = 8;
   auto dtiles = [&]() { return (long long)p.N * ((p.Wo + p.tile_w - 1) / p.tile_w) * ((p.Ho + p.tile_h - 1) / p.tile_h) * (p.Cout_pad / p.BN); };
   // N tile: 128 (A tile gathered once per 128 output channels) when Cout_pad allows it and there are at least sms / 4
   // of its 16 x 8-pixel tiles; otherwise 32, whose smaller pixel blocks (below) spread tiny maps over more SMs.  Measured
   // on H100 SXM (400 W), 256 -> 128 channels: 64 x 128 map (64 tiles) 0.128 ms at N = 128 vs 0.221 ms at N = 32;
-  // 32 x 64 map (16 tiles) 0.138 vs 0.115 ms.  DENSE mode: always 32.
+  // 32 x 64 map (16 tiles) 0.138 vs 0.115 ms.
   p.BN = 128;
-  const bool wide_ok = !dense && p.Cout_pad % 128 == 0;
+  const bool wide_ok = p.Cout_pad % 128 == 0;
   const bool wide = wide_ok && (g_dw_force_bn == 128 || (g_dw_force_bn == 0 && dtiles() >= sms / 4));
   if (!wide) p.BN = 32;
   // few tiles (coarse pyramid levels): smaller pixel blocks -> more CTAs share the serial k-block chain
@@ -668,39 +624,18 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
   if (!wide && dtiles() < sms / 2) { p.tile_h = 4; }
   const long long num_tiles = dtiles();
   if (num_tiles <= 0) return 0;
-  // dense: the window box is the tile's receptive field: 24 pixels x (tile + halo) rows x 64 channels (128-byte pixels)
-  int win_h = DW_WH;
-  p.win_pitch = DW_WW; p.win_plane = DW_PLANE; p.win_buf = DW_WIN_BYTES; p.stages = DW_STAGES; p.win_nbuf = 2;
-  if (dense) {
-    win_h = p.tile_h + 2 * dil_h;
-    p.win_pitch = 24;
-    if (win_h > 16 || p.tile_w + 2 * dil_w > p.win_pitch) return UPSNET_E_UNSUPPORTED;
-    p.win_plane = p.win_pitch * win_h * 128;
-    p.win_plane = (p.win_plane + 1023) / 1024 * 1024;     // SWIZZLE_128B destinations: 1024-byte aligned planes
-    p.win_buf = 2 * p.win_plane;
-    p.win_nbuf = 1;       // one 64-channel fill serves 36 k-slices: a second buffer does not fit next to the A stages
-  }
-  p.win_bytes = dense ? 2 * p.win_pitch * win_h * 128 : 2 * DW_WW * win_h * 32;
-  p.win_h = win_h;
-  // shared memory: N = 32 -> 23 KB tables + 2 x 40 KB stages (3 do not fit) + 2 x 40 KB windows + 18 KB staging;
-  //                N = 128 -> 23 KB tables + 3 x 32 KB stages + 2 x 40 KB windows + 18 KB staging (218 KB)
-  const uint32_t stage_bytes = wide ? DwCfg<128>::STAGE_BYTES : DwCfg<32>::STAGE_BYTES;
   const int bk = wide ? DwCfg<128>::BK : DwCfg<32>::BK;
-  auto smem_need = [&]() {
-    return (size_t)DW_OFF_STAGES + (size_t)p.stages * stage_bytes + (size_t)p.win_nbuf * p.win_buf + DW_EPI_BYTES + 1024;
-  };
-  if (smem_need() > 227 * 1024 && p.stages > 2) p.stages = 2;
-  if (smem_need() > 227 * 1024) return UPSNET_E_UNSUPPORTED;
+  const size_t smem = wide ? DwCfg<128>::SMEM : DwCfg<32>::SMEM;
   EncodeTiledFn enc = tma_encoder();
   if (!enc) return UPSNET_E_UNSUPPORTED;
   CUtensorMap tm_x, tm_w;
   {
     const cuuint64_t dx[4] = {(cuuint64_t)(2 * Cin), (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
     const cuuint64_t sx[3] = {(cuuint64_t)(2 * Cin) * 2, (cuuint64_t)W * (2 * Cin) * 2, (cuuint64_t)H * W * (2 * Cin) * 2};
-    const cuuint32_t bx[4] = {(cuuint32_t)(dense ? 64 : 16), (cuuint32_t)p.win_pitch, (cuuint32_t)win_h, 1};
+    const cuuint32_t bx[4] = {16, DW_WW, DW_WH, 1};
     const cuuint32_t es[4] = {1, 1, 1, 1};
     if (enc(&tm_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x_pair), dx, sx, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            dense ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+            CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return UPSNET_E_UNSUPPORTED;
     // weight box: BK x BN, rows of BK bf16 in the swizzle the stage's wgmma descriptors expect
     const cuuint64_t dwt[2] = {(cuuint64_t)(9 * Cin), (cuuint64_t)(2 * p.Cout_pad)};
@@ -711,7 +646,6 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return UPSNET_E_UNSUPPORTED;
   }
-  const size_t smem = smem_need();
   static PerDeviceOnce configured;
   if (configured.need()) {
     UPS_CUDA(cudaFuncSetAttribute(dcn_win_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -724,20 +658,4 @@ static int dw_launch(const void* x_pair, const float* offset, const float* mask,
     dcn_win_kernel<32><<<grid, DwCfg<32>::THREADS, smem, (cudaStream_t)stream>>>(tm_x, tm_w, p);
   UPS_CHECK_LAUNCH();
   return 0;
-}
-
-extern "C" int upsnet_dcn_pair_forward(const void* x_pair, const float* offset, const float* mask, const void* packed,
-                                       const float* bias, void* y_pair, int N, int H, int W, int Cin, int Cout, int kh,
-                                       int kw, int pad_h, int pad_w, int dil_h, int dil_w, int epi_flags, void* stream) {
-  if (!offset) return UPSNET_E_BADARG;
-  return dw_launch(x_pair, offset, mask, packed, bias, y_pair, N, H, W, Cin, Cout, kh, kw, pad_h, pad_w, dil_h, dil_w, epi_flags,
-                   false, false, stream);
-}
-
-extern "C" int upsnet_conv3x3_pair_forward(const void* x_pair, const void* packed, const float* bias, void* y, int N, int H, int W,
-                                           int Cin, int Cout, int pad_h, int pad_w, int dil_h, int dil_w, int out_layout,
-                                           int epi_flags, void* stream) {
-  if (out_layout != UPSNET_LAYOUT_NCHW && out_layout != UPSNET_LAYOUT_NHWC) return UPSNET_E_BADARG;
-  return dw_launch(x_pair, nullptr, nullptr, packed, bias, y, N, H, W, Cin, Cout, 3, 3, pad_h, pad_w, dil_h, dil_w, epi_flags,
-                   true, out_layout == UPSNET_LAYOUT_NCHW, stream);
 }

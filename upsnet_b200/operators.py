@@ -213,39 +213,6 @@ def _pack_dcn(weight):
     return buf
 
 
-# small-N dense 3x3 / stride-1 convs on the pair stream through the window pipeline (csrc/dcn_win.cu DENSE mode): Cout <= max_cout
-# off by default: the per-tap TMA boxes of the dense conv kernel serve these layers; kept as an entry point and for the tests
-DENSE_WINDOW = {"on": False, "max_cout": 64, "min_pixels": 4096}
-
-
-def _dense_window(x, weight, bias, padding, dilation, relu, nchw_out):
-    """upsnet_conv3x3_pair_forward: Pair in; fp32 NCHW (offset maps) or Pair out.  None when the layer does not qualify."""
-    N, Cin, H, W = x.shape
-    Cout, _, kh, kw = weight.shape
-    ph, pw = padding; dh, dw = dilation
-    if N * H * W < DENSE_WINDOW["min_pixels"] or Cout > DENSE_WINDOW["max_cout"] or (not nchw_out and Cout % 16):
-        return None
-    packed = _packed_weight_dcn(weight)
-    if packed is None:
-        return None
-    Ho, Wo = _conv_out(H, ph, dh, 3, 1), _conv_out(W, pw, dw, 3, 1)
-    if nchw_out:
-        store = torch.empty((N, Cout, Ho, Wo), device=x.device, dtype=torch.float32)
-    else:
-        store = torch.empty((N, Ho, Wo, 2 * Cout), device=x.device, dtype=torch.bfloat16)
-    work = {"flops": 2.0 * N * Ho * Wo * Cout * Cin * 9 * 3, "algo_flops": 2.0 * N * Ho * Wo * Cout * Cin * 9,
-            "shape": "N%d %dx%d Cin%d->Cout%d k3 s1 pair->%s (window)" % (N, H, W, Cin, Cout, "float32" if nchw_out else "pair"),
-            "bytes": float(x.store.numel() * 2 + 4 * weight.numel() + store.numel() * store.element_size())}
-    with torch.cuda.device(x.device), _Timed("conv2d", 1, work, x.device):
-        rc = lib().upsnet_conv3x3_pair_forward(ptr(x.store), ptr(packed), ptr(bias), ptr(store), N, H, W, Cin, Cout, ph, pw, dh, dw,
-                                               _lib.LAYOUT_NCHW if nchw_out else _lib.LAYOUT_NHWC,
-                                               _lib.EPI_RELU if relu else 0, stream_ptr(x.device))
-    if rc == -2:
-        return None
-    check(rc, "conv3x3_pair_forward")
-    return store if nchw_out else Pair(store)
-
-
 def _dcn_window(x, offset, mask, weight, bias, padding, dilation, relu):
     """upsnet_dcn_pair_forward (csrc/dcn_win.cu): Pair in, Pair out, 3x3 / stride 1.  Returns None when the layer does
     not qualify (the caller then takes upsnet_igemm_forward)."""
@@ -414,14 +381,6 @@ def conv2d(x, weight, bias=None, stride=1, padding=0, dilation=1, residual=None,
     if prec != _lib.PREC_FP32_SIMT and _tc_ok(weight.shape[1], weight.shape[2], weight.shape[3], 1):
         if residual_up2 and out_format == "nchw":
             residual, residual_up2 = torch.nn.functional.interpolate(as_float(residual), scale_factor=2, mode="nearest"), False
-        if (DENSE_WINDOW["on"] and isinstance(x, Pair) and prec == _lib.PREC_BF16X3 and ACT_PAIR["on"] and USE_TMA["on"] and
-                weight.shape[2] == 3 and weight.shape[3] == 3 and _pair(stride) == (1, 1) and residual is None and
-                sigmoid_from is None and not pair_group and
-                ((out_format == "nchw" and out_dtype in (None, torch.float32)) or (out_format != "nchw" and out_dtype in (None, "pair")))):
-            y = _dense_window(x, weight, None if bias is None else f32c(bias), _pair(padding), _pair(dilation), relu,
-                              out_format == "nchw")
-            if y is not None:
-                return y
         return _igemm_tc("conv2d", x, None, None, weight, None if bias is None else f32c(bias), residual,
                          _pair(stride), _pair(padding), _pair(dilation), relu, prec, out_format, out_dtype,
                          residual_up2, pair_group, sigmoid_from)
