@@ -382,6 +382,23 @@ int upsnet_pq_update(const unsigned char *pan_2ch, const unsigned char *gt_rgb, 
                      void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Semantic-segmentation confusion matrix of one image on the device (SURVEY section 8 row f4, evaluation half).
+ * replaces: dataset/cityscapes.py:445-514 / coco.py:225-293 evaluate_ssegs + write_segmentation_result and
+ *           base_dataset.py:806-824 get_confusion_matrix (a PNG per prediction, PIL NEAREST resize to the ground-truth
+ *           size, np.bincount on the host).
+ * pred [rows][pred_pitch] elements of pred_bytes = 1 (uint8) or 8 (int64); each value is wrapped to uint8 (np.uint8).
+ * row_src int32 [H], col_src int32 [W]: the prediction element of gt pixel (y, x) is pred[row_src[y] * pred_pitch +
+ *   col_src[x]]; every resize / restore rule lives in these tables, which the caller builds (indices are not checked).
+ * gt uint8 [H,W]; pixels with gt == 255 are ignored.  A pixel counts in bin gt * C + pred only if that is < C*C (so gt
+ *   rows >= C drop and predictions >= C alias into later rows, as in the reference).
+ * acc int64 [C*C] (row = gt, column = prediction) is ADDED to with integer atomics: the result is order independent.
+ * 1 <= num_classes <= UPSNET_SSEG_MAX_CLASSES (a C*C uint32 histogram per block in shared memory).  No workspace; the
+ * call never synchronises. */
+#define UPSNET_SSEG_MAX_CLASSES 224
+int upsnet_sseg_update(const void *pred, int pred_bytes, int pred_pitch, const int *row_src, const int *col_src,
+                       const unsigned char *gt, int H, int W, int num_classes, long long *acc, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Instance-mask post-processing of the test loop on the device (SURVEY section 8 row f4).
  * replaces: upsnet_end2end_test.py:95-152 `im_post` (expand_boxes bbox/bbox_transform.py:365-381 -> int32 boxes,
  *           (M+2)x(M+2) zero-padded mask -> cv2.resize -> > 0.5 -> paste into [H,W] -> pycocotools.mask.encode), run by the

@@ -1,4 +1,4 @@
-"""Panoptic quality (PQ / SQ / RQ) evaluation on the device.
+"""Panoptic quality (PQ / SQ / RQ) and semantic-segmentation IoU evaluation on the device.
 
 The reference evaluates on the host (dataset/base_dataset.py:209-330 evaluate_panoptic): `_converter_2ch_single_core`
 turns every 2-channel prediction into segments, `_pq_compute_single_core` counts the (ground truth, prediction)
@@ -14,13 +14,29 @@ image per `update()` with the kernels of csrc/pq.cu; only `pq_stat()` / `summari
 The semantics are those of the reference, quirks included: stuff segments with different instance numbers merge, the
 ground truth's `area` field (not its pixel count) enters the union, only the last crowd segment of a category counts,
 ids in the PNG that are missing from `segments_info` take part in nothing, and a later duplicate id wins.
+
+`SegmentationIoU` does the same for the semantic-segmentation mIoU of the reference's `evaluate_ssegs`
+(dataset/cityscapes.py:445-514, coco.py:225-293, base_dataset.py:806-824 get_confusion_matrix).  The [C, C] confusion
+matrix stays on the device as int64 and grows by one image per `update()` (csrc/sseg.cu); only `confusion_matrix()` /
+`summarize()` copy it back.
+
+    miou = SegmentationIoU(19)
+    for pred, seg_gt in zip(fcn_outputs, gt_pngs):          # pred: int64 / uint8 label map; seg_gt: uint8 trainId PNG
+        miou.update(pred, seg_gt)                           # or update(network_map, seg_gt, im_info) before the restore
+    results = miou.summarize()                              # {'meanIU', 'IU_array', 'confusion_matrix'}
+
+The reference's quirks are kept: prediction values wrap mod 256 (np.uint8), the prediction is resized to the ground truth
+with Pillow's NEAREST rule (not cv2's), only gt == 255 is ignored, and a pixel counts in bin gt * C + pred only when
+that bin exists, so gt rows >= C are dropped and predictions >= C alias into later rows.
 """
+import collections
 import ctypes as C
 
 import numpy as np
 import torch
 
 from ._lib import UpsnetError, check, lib, ptr, stream_ptr
+from .operators import label_restore_geometry, label_restore_index
 
 MAX_GT = 4096          # UPSNET_PQ_MAX_GT: ground-truth segments per image
 MAX_PAIRS = 65536      # UPSNET_PQ_MAX_PAIRS: distinct (ground truth, prediction) segment pairs per image
@@ -179,3 +195,117 @@ class PanopticQuality:
         self._counts.zero_()
         self._iou.zero_()
         self._err.zero_()
+
+
+MAX_SSEG_CLASSES = 224     # UPSNET_SSEG_MAX_CLASSES: a C*C uint32 histogram per block fits in shared memory
+
+
+def pil_nearest_index(n_in, n_out):
+    """Source indices of PIL's Image.resize(..., Image.NEAREST) along one axis (ImagingScaleAffine): with a = n_in / n_out,
+    output i reads int(acc_i), acc_0 = a / 2 and acc_{i+1} = acc_i + a summed one after the other in double.  This is
+    neither cv2's rule nor floor((i + 0.5) * a); equal sizes give the identity."""
+    a = n_in / n_out
+    idx = np.add.accumulate(np.r_[a * 0.5, np.full(n_out - 1, a)]).astype(np.int64)       # sequential, then truncated
+    assert idx[0] >= 0 and idx[-1] < n_in
+    return idx
+
+
+def sseg_index_tables(pred_hw, gt_hw, im_info=None):
+    """int32 (row_src [H], col_src [W]) for upsnet_sseg_update.  Without im_info the prediction is resized from pred_hw to
+    the ground-truth size gt_hw by Pillow's rule.  With im_info the prediction is the network-resolution map (padded
+    [Hp, Wp]); the tables then compose the test script's crop + cv2 restore (label_restore, upsnet_end2end_test.py:259-266)
+    with Pillow's resize from the restored size to gt_hw, so they pick the pixels the reference's loop would."""
+    (ph, pw), (H, W) = (int(v) for v in pred_hw), (int(v) for v in gt_hw)
+    if im_info is None:
+        rows, cols = pil_nearest_index(ph, H), pil_nearest_index(pw, W)
+    else:
+        h, w, fx, oh, ow = label_restore_geometry(im_info)
+        if not (0 < h <= ph and 0 < w <= pw):
+            raise ValueError("im_info crop (%d, %d) outside the %dx%d label map" % (h, w, ph, pw))
+        if oh <= 0 or ow <= 0:
+            raise ValueError("im_info restores the map to an empty %dx%d image" % (oh, ow))
+        rows = label_restore_index(oh, fx, h)[pil_nearest_index(oh, H)]
+        cols = label_restore_index(ow, fx, w)[pil_nearest_index(ow, W)]
+    return rows.astype(np.int32), cols.astype(np.int32)
+
+
+class SegmentationIoU:
+    """Semantic-segmentation confusion matrix and mIoU of the reference's evaluate_ssegs, accumulated on one CUDA device.
+    1 <= num_classes <= 224 (19 for Cityscapes, 133 for COCO).  Calls on one object must be issued on one stream."""
+
+    TABLE_CACHE = 16       # index-table geometries kept on the device (LRU)
+
+    def __init__(self, num_classes, device=None):
+        if not 1 <= int(num_classes) <= MAX_SSEG_CLASSES:
+            raise ValueError("num_classes %r outside [1, %d]" % (num_classes, MAX_SSEG_CLASSES))
+        self.num_classes = int(num_classes)
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        assert self.device.type == "cuda", "SegmentationIoU runs on a CUDA device (no CPU fallback)"
+        self._acc = torch.zeros((self.num_classes ** 2,), dtype=torch.int64, device=self.device)
+        self._tables = collections.OrderedDict()
+        self._captured = []    # tables a captured CUDA graph reads at replay: never freed by the LRU
+
+    def _map(self, x, name, dtypes, max_dim):
+        if isinstance(x, np.ndarray):
+            x = torch.from_numpy(np.ascontiguousarray(x))
+        if x.dtype not in dtypes or not 2 <= x.dim() <= max_dim or any(int(s) != 1 for s in x.shape[:-2]):
+            raise ValueError("%s must be %s [h,w]%s, got %s %s"
+                             % (name, "/".join(str(d).replace("torch.", "") for d in dtypes),
+                                " / [1,h,w] / [1,1,h,w]" if max_dim > 2 else "", x.dtype, tuple(x.shape)))
+        if x.numel() == 0:
+            raise ValueError("%s is empty: %s" % (name, tuple(x.shape)))
+        return x.reshape(x.shape[-2:]).to(self.device, non_blocking=True).contiguous()
+
+    def _index_tables(self, pred_hw, gt_hw, im_info):
+        info = None if im_info is None else tuple(np.asarray(im_info, np.float32).reshape(-1)[:3].tolist())
+        key = (pred_hw, gt_hw, info)
+        tab = self._tables.get(key)
+        if tab is not None:
+            self._tables.move_to_end(key)
+            return tab
+        if torch.cuda.is_current_stream_capturing():
+            raise UpsnetError("SegmentationIoU: new geometry %s inside a CUDA-graph capture; call update() once outside "
+                              "the capture" % (key,))
+        rows, cols = sseg_index_tables(pred_hw, gt_hw, im_info)
+        host = torch.from_numpy(np.concatenate([rows, cols])).pin_memory()
+        tab = host.to(self.device, non_blocking=True)
+        self._tables[key] = tab
+        while len(self._tables) > self.TABLE_CACHE:
+            self._tables.popitem(last=False)
+        return tab
+
+    def update(self, pred, seg_gt, im_info=None):
+        """Adds one image.  pred int64 or uint8 [h,w] / [1,h,w] / [1,1,h,w]: the semantic label map at any size (it is
+        resized to seg_gt by Pillow's rule), or with im_info ([h, w, scale] as the data loader gives it) the
+        network-resolution map before the restore.  seg_gt uint8 [H,W], the trainId PNG as decoded.  Host arrays are
+        copied to the device once; nothing waits for the device."""
+        p = self._map(pred, "pred", (torch.int64, torch.uint8), 4)
+        g = self._map(seg_gt, "seg_gt", (torch.uint8,), 2)
+        pred_hw, gt_hw = tuple(int(s) for s in p.shape), tuple(int(s) for s in g.shape)
+        tab = self._index_tables(pred_hw, gt_hw, im_info)
+        if torch.cuda.is_current_stream_capturing():
+            self._captured.append(tab)
+        H, W = gt_hw
+        with torch.cuda.device(self.device):
+            check(lib().upsnet_sseg_update(ptr(p), p.element_size(), pred_hw[1], ptr(tab), C.c_void_p(tab.data_ptr() + 4 * H),
+                                           ptr(g), H, W, self.num_classes, ptr(self._acc), stream_ptr(self.device)),
+                  "sseg_update")
+
+    def confusion_matrix(self):
+        """float64 [C, C] (row = ground truth, column = prediction): the matrix the reference accumulates."""
+        C_ = self.num_classes
+        return self._acc.cpu().numpy().reshape(C_, C_).astype(np.float64)
+
+    def summarize(self):
+        """evaluate_ssegs's evaluation_results: {'meanIU', 'IU_array', 'confusion_matrix'}, with its arithmetic (the mean
+        runs over all C classes, so a class that never appears counts as 0)."""
+        confusion_matrix = self.confusion_matrix()
+        pos = confusion_matrix.sum(1)
+        res = confusion_matrix.sum(0)
+        tp = np.diag(confusion_matrix)
+        IU_array = (tp / np.maximum(1.0, pos + res - tp))
+        mean_IU = IU_array.mean()
+        return {'meanIU': mean_IU, 'IU_array': IU_array, 'confusion_matrix': confusion_matrix}
+
+    def reset(self):
+        self._acc.zero_()

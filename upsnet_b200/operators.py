@@ -1213,6 +1213,12 @@ def label_restore_geometry(im_info):
     return h, w, fx, int(np.rint(h * fx)), int(np.rint(w * fx))
 
 
+def label_restore_index(n_out, fx, n_crop):
+    """Source indices of one axis of the restore (the rule upsnet_label_restore applies on the device): cv2's
+    INTER_NEAREST min(floor(i * (1 / fx)), n_crop - 1) for i < n_out, with 1 / fx and the product in double."""
+    return np.minimum(np.floor(np.arange(n_out, dtype=np.float64) * (1.0 / fx)).astype(np.int64), n_crop - 1)
+
+
 def label_restore(label_map, im_info, *more_maps):
     """upsnet_end2end_test.py:259-266 on the device: crop an int64 label map [Hp,Wp] (or [1,Hp,Wp]) to im_info[:2],
     wrap it to uint8 like astype('uint8') and resize it back to the original image size with cv2's INTER_NEAREST rule.
