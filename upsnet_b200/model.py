@@ -149,25 +149,17 @@ class Stem(nn.Module):
         self.conv1 = nn.Conv2d(3, 64, 7, 2, 3, bias=False)
         self.bn1 = nn.BatchNorm2d(64)
         self._f = None
-        self._stem_tma = None    # None = not probed yet, True / False = TMA stem path usable
 
     def prepare(self):
         w, b = _fold_bn(self.conv1.weight, self.bn1)
         self._f = (w.detach(), b.detach())
 
     def forward(self, x):
-        bf16_stream = ops.ACT_BF16["on"] and ops._PRECISION["conv"] == ops._lib.PREC_BF16
-        pair_stream = ops.ACT_PAIR["on"] and ops._PRECISION["conv"] == ops._lib.PREC_BF16X3
-        if x.is_cuda and (bf16_stream or pair_stream) and self._stem_tma is not False:
-            try:    # TMA-fed stem; a driver that rejects the overlapping-stride tensor map leaves the gather kernel in charge
-                y = ops.stem_conv(x, self._f[0], self._f[1], 3, relu=True, pair=pair_stream)
-                self._stem_tma = True
-                return ops.max_pool2d(y, 3, 2, 1)
-            except ops._lib.UpsnetError:
-                if self._stem_tma:      # it worked before: a real failure, not a capability probe
-                    raise
-                self._stem_tma = False
-        x = ops.conv2d(x, self._f[0], self._f[1], stride=2, padding=3, relu=True)
+        stream = ops._stream()
+        if x.is_cuda and stream != "f32":       # bf16 / pair stream: the TMA-fed stem
+            x = ops.stem_conv(x, self._f[0], self._f[1], 3, relu=True, pair=stream == "pair")
+        else:       # fp32 stream, and CPU tensors (oracle.cpu_model.cpu_ops swaps in CPU versions of ops.conv2d & co.)
+            x = ops.conv2d(x, self._f[0], self._f[1], stride=2, padding=3, relu=True)
         return ops.max_pool2d(x, 3, 2, 1)
 
 
@@ -437,7 +429,6 @@ class FCNHead(nn.Module):
         self.score = nn.Conv2d(512, num_classes, 1)
         nn.init.normal_(self.score.weight.data, 0, 0.01)
         self.score.bias.data.zero_()
-        self.fuse_score = True   # inference: score each level at its own resolution (see forward)
         self.overlap_levels = False   # measured: no gain over the serial P2..P5 order (the side-stream fork already fills the gaps)
         self._streams = None
         self._f = None
@@ -476,7 +467,7 @@ class FCNHead(nn.Module):
         """score_only (static engine): stop at the quarter-resolution score map 'fcn_score' -- the x4 up-sampling is then
         evaluated inside the panoptic fusion kernel (ops.panoptic_fuse(..., up4=True)) and fcn_output is never materialised."""
         p2, p3, p4, p5 = self._subnets(p2, p3, p4, p5)
-        if self.fuse_score and self._f is not None:
+        if self._f is not None:     # prepared (inference): score each level at its own resolution
             # models/fcn.py:94-101 computes score(cat(p2, up2(p3), up4(p4), up8(p5))).  The 1x1 score conv and the
             # bilinear upsampling are both linear and act on different axes, so they commute:
             #   score = W2*p2 + up2(W3*p3) + up4(W4*p4) + up8(W5*p5) + b
@@ -541,7 +532,6 @@ class resnet_upsnet(nn.Module):
         self.mask_roi_panoptic_static = StaticMaskROI(cfg.max_det, self.num_classes, 0.5, True,
                                                       cfg.panoptic_score_thresh, cfg.bbox_reg_weights)
         self.static_engine = True     # fixed shapes + device-side counts: no host sync inside the forward
-        self.fuse_upsample = True     # panoptic fusion kernel up-samples the quarter-resolution semantic score map itself
         self.use_cuda_graph = True    # capture the static forward once per (shape, precision) and replay it
         self.overlap_heads = True     # semantic head on a side stream, concurrent with the detection chain
         self._side = {}
@@ -725,7 +715,7 @@ class resnet_upsnet(nn.Module):
         """Semantic head of the static engine: (fcn_output or None, fcn_score or None).  With the fused score path and the
         reference's x4 up-sampling the full-resolution logits are only materialised when a test asks for intermediates."""
         head = self.fcn_head
-        fuse_up = on_gpu and head.fuse_score and head._f is not None and head.upsample_rate == 4 and self.fuse_upsample
+        fuse_up = on_gpu and head._f is not None and head.upsample_rate == 4
         if not fuse_up:
             return head(p2, p3, p4, p5)["fcn_output"].float(), None
         ret = head(p2, p3, p4, p5, score_only=not getattr(self, "keep_intermediates", False))
@@ -754,8 +744,8 @@ class resnet_upsnet(nn.Module):
     def _run_static_lane(self, x, im_info, lane):
         if not (self.use_cuda_graph and x.is_cuda):
             return self._forward_static(x, im_info), None
-        key = (tuple(x.shape), str(x.device), ops._PRECISION["conv"], ops.ACT_BF16["on"], ops.ACT_PAIR["on"],
-               bool(getattr(self, "keep_intermediates", False)), tuple(float(v) for v in im_info), lane)
+        key = (tuple(x.shape), str(x.device), ops._PRECISION["conv"], bool(getattr(self, "keep_intermediates", False)),
+               tuple(float(v) for v in im_info), lane)
         ent = self._graphs.get(key)
         if ent is None:
             static_x = torch.empty(x.shape, dtype=torch.float32, device=x.device)

@@ -29,24 +29,26 @@ from ._lib import check, f32c, lib, ptr, require_cuda, stream_ptr
 
 # default arithmetic of the convolution tiles; switched by upsnet_b200.set_precision()
 _PRECISION = {"conv": _lib.PREC_FP32_SIMT}
-ACT_BF16 = {"on": False}   # engine switch: store activations as bf16 (precision 'bf16' only)
-ACT_PAIR = {"on": False}   # engine switch: store activations as hi/lo bf16 pairs (precision 'bf16x3': fp32-grade results)
 # pair-stream deformable convs gather from a shared-memory window into shared-memory A tiles (csrc/dcn_win.cu); maps with fewer
 # than min_pixels output pixels keep the global-gather kernel (measured: 0.058 vs 0.048 ms at 32x64, 0.060 vs 0.075 ms at 64x128)
 DCN_WINDOW = {"on": True, "min_pixels": 4096}
 USE_TMA = {"on": True}     # False forces the cp.async gather kernel where the TMA-fed one would qualify (A/B tests)
 
 
-def set_precision(name, bf16_activations=None, pair_activations=None):
-    """'fp32' (CUDA-core fp32 tiles), 'bf16x3' or 'bf16' (wgmma tiles).  With 'bf16' the engine also stores
-    the NHWC activation stream as bf16 (halves HBM traffic; the gather becomes a cp.async copy) unless
-    bf16_activations=False.  With 'bf16x3' -- the configuration that meets "fp32 logits within 1e-3" -- the stream is
-    stored as hi/lo bf16 PAIRS (class Pair: same bytes as fp32, ~16 mantissa bits) so that the TMA-fed wgmma kernel can
-    run the three-term split (hi*hi + lo*hi + hi*lo) without any gather threads; pair_activations=False keeps fp32
-    activations and the gather-fed kernel (round-1 behaviour, kept for A/B tests)."""
+def set_precision(name):
+    """Default precision of the convolutions, which also fixes how the engine stores its activation stream:
+    'fp32': CUDA-core fp32 tiles on fp32 NCHW activations.
+    'bf16': single-pass wgmma tiles; activations stored NHWC as bf16 (half the HBM traffic of fp32).
+    'bf16x3': the configuration that meets "fp32 logits within 1e-3"; activations stored NHWC as hi/lo bf16 PAIRS
+      (class Pair: same bytes as fp32, ~16 mantissa bits) so that the TMA-fed wgmma kernel runs the three-term split
+      (hi*hi + lo*hi + hi*lo) without gather threads.
+    An explicit precision= on conv2d / deform_conv changes the arithmetic of that call only, not the stream format."""
     _PRECISION["conv"] = {"fp32": _lib.PREC_FP32_SIMT, "bf16x3": _lib.PREC_BF16X3, "bf16": _lib.PREC_BF16}[name]
-    ACT_BF16["on"] = (name == "bf16") if bf16_activations is None else (bool(bf16_activations) and name == "bf16")
-    ACT_PAIR["on"] = (name == "bf16x3") if pair_activations is None else (bool(pair_activations) and name == "bf16x3")
+
+
+def _stream():
+    """Storage format of the engine's activation stream under the global precision: 'f32', 'bf16' or 'pair'."""
+    return {_lib.PREC_BF16: "bf16", _lib.PREC_BF16X3: "pair"}.get(_PRECISION["conv"], "f32")
 
 
 class Pair:
@@ -291,8 +293,8 @@ def _igemm_tc(kind, x, offset, mask, weight, bias, residual, stride, padding, di
               out_dtype=None, residual_up2=False, pair_group=0, sigmoid_from=None):
     """upsnet_igemm_forward: x logical NCHW (any memory format; fp32 or bf16) or a Pair; result logical NCHW whose
     storage is NHWC (channels_last view, the engine layout) unless out_format == 'nchw'.
-    Output: bf16 when the engine stores bf16 activations (ACT_BF16) / a Pair when it stores pairs (ACT_PAIR) and the
-    result stays in the NHWC activation stream; fp32 for plane-wise (NCHW) head outputs or when asked via out_dtype.
+    Output: bf16 / a Pair when the engine's activation stream (_stream()) is bf16 / pairs and the
+    result stays in that NHWC stream; fp32 for plane-wise (NCHW) head outputs or when asked via out_dtype.
     pair_group=G (Pair output only): channels are written as [hi G][lo G] groups and the result is returned as the Pair
     of logical shape [N, G, Ho, Wo*Cout/G] that this storage also is (see MaskBranch)."""
     sh, sw = stride; ph, pw = padding; dh, dw = dilation
@@ -301,10 +303,11 @@ def _igemm_tc(kind, x, offset, mask, weight, bias, residual, stride, padding, di
     Ho, Wo = _conv_out(H, ph, dh, kh, sh), _conv_out(W, pw, dw, kw, sw)
     nhwc_out = out_format != "nchw"
     x3 = prec == _lib.PREC_BF16X3
+    stream = _stream()
     pair_in = isinstance(x, Pair)
     if pair_in:
         assert x3, "Pair activations belong to precision bf16x3"
-    elif x3 and ACT_PAIR["on"] and Cin % 64 == 0:
+    elif x3 and stream == "pair" and Cin % 64 == 0:
         x = Pair.from_float(x)                               # entry into the pair stream (API-level callers)
         pair_in = True
     elif x3 and x.dtype != torch.float32:
@@ -314,10 +317,10 @@ def _igemm_tc(kind, x, offset, mask, weight, bias, residual, stride, padding, di
     dev = x.device
     pair_out = False
     if out_dtype is None:
-        if x3 and ACT_PAIR["on"] and nhwc_out and Cout % 8 == 0:
+        if x3 and stream == "pair" and nhwc_out and Cout % 8 == 0:
             pair_out = True
         else:
-            out_dtype = torch.bfloat16 if (ACT_BF16["on"] and prec == _lib.PREC_BF16 and nhwc_out) else torch.float32
+            out_dtype = torch.bfloat16 if (stream == "bf16" and prec == _lib.PREC_BF16 and nhwc_out) else torch.float32
     elif out_dtype == "pair":
         pair_out = True
     if pair_in:
@@ -454,7 +457,7 @@ def deform_conv(data, offset, weight, bias=None, stride=1, padding=0, dilation=1
         if mask is not None:
             assert tuple(mask.shape) == (N, kh * kw, Ho, Wo), mask.shape
         if (DCN_WINDOW["on"] and isinstance(data, Pair) and prec == _lib.PREC_BF16X3 and (sh, sw) == (1, 1) and
-                out_format != "nchw" and out_dtype in (None, "pair") and ACT_PAIR["on"]):
+                out_format != "nchw" and out_dtype in (None, "pair") and _stream() == "pair"):
             y = _dcn_window(data, offset, mask, weight, bias, (ph, pw), (dh, dw), relu)
             if y is not None:
                 return y
