@@ -399,6 +399,59 @@ int upsnet_sseg_update(const void *pred, int pred_bytes, int pred_pitch, const i
                        const unsigned char *gt, int H, int W, int num_classes, long long *acc, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * COCO box and mask AP on the device (SURVEY section 8 row f4, evaluation half).
+ * replaces: dataset/base_dataset.py:181-204 evaluate_boxes / coco.py:194-222 evaluate_masks -- a results JSON written,
+ *           reloaded with COCO.loadRes and scored by pycocotools' COCOeval.evaluate() / accumulate() on the host.
+ * Semantics: COCOeval with its default Params (iouThrs linspace(.5,.95,10), recThrs linspace(0,1,101), maxDets 1/10/100,
+ *   area ranges all / small / medium / large, useCats), none of which is a parameter here.
+ *
+ * upsnet_cocoeval_image: evaluate() of one image.  Detections: boxes fp32 [n][4] xyxy, scores fp32 [n], cls_inds int64 [n]
+ *   (class j in [1, num_categories]; K index class_to_k[j], class_to_k int32 [num_categories + 1] on the device); only
+ *   the first min(n, *n_dev) count when n_dev (device int) is given.  segm != 0: masks are counts uint32 [n][cap] /
+ *   run_len int32 [n] exactly as upsnet_im_post_rle leaves them, of an H x W image.
+ *   gt_table fp64 [9][num_gt] (structure of arrays): K index, iscrowd, area (the annotation's field), x, y, w, h, and for
+ *   segm the RLE's h, w.  segm: gt_counts uint32 (uncompressed run lengths, all ground truths back to back), gt_offsets
+ *   int64 [num_gt + 1].  The workspace (segm only) is upsnet_cocoeval_workspace_bytes(n, cap, gt_offsets[num_gt]).
+ *   Writes one record per kept detection (the first 100 of its category by descending score, ties in input order) at
+ *   records[atomicAdd(n_records, ...)]; bit a * 10 + t of matched / ignored is evaluateImg's dtMatches != 0 / dtIgnore for
+ *   IoU threshold t and area range a.  npig int64 [num_categories][4] is ADDED to (non-ignored ground truths).
+ *   Limits: UPSNET_COCOEVAL_MAX_DET detections, UPSNET_COCOEVAL_MAX_GT ground truths per image, UPSNET_COCOEVAL_MAX_GT_CAT
+ *   per (image, category), record_cap records.  err (DEVICE int, sticky) gets UPSNET_COCOEVAL_E_*; nothing is truncated
+ *   silently.  The call never synchronises.
+ * upsnet_cocoeval_accumulate: accumulate() over records [n_records].  image_rank int32 [image slot] = rank of the slot's
+ *   image id among all image ids (< UPSNET_COCOEVAL_MAX_IMAGES).  Writes precision / scores fp64 [10][101][K][4][3] and
+ *   recall fp64 [10][K][4][3], numpy's C order.  Workspace: upsnet_cocoeval_accumulate_workspace_bytes(n_records). */
+#define UPSNET_COCOEVAL_MAX_DET 2048
+#define UPSNET_COCOEVAL_MAX_GT 1024
+#define UPSNET_COCOEVAL_MAX_GT_CAT 192
+#define UPSNET_COCOEVAL_MAX_CATEGORIES 256
+#define UPSNET_COCOEVAL_MAX_IMAGES (1 << 17)
+#define UPSNET_COCOEVAL_E_DET_COUNT 1   /* more than UPSNET_COCOEVAL_MAX_DET detections */
+#define UPSNET_COCOEVAL_E_GT_COUNT 2    /* num_gt > UPSNET_COCOEVAL_MAX_GT */
+#define UPSNET_COCOEVAL_E_GT_CAT 4      /* more than UPSNET_COCOEVAL_MAX_GT_CAT ground truths of one category */
+#define UPSNET_COCOEVAL_E_CLASS 8       /* a detection class outside [1, num_categories] */
+#define UPSNET_COCOEVAL_E_RECORDS 16    /* more than record_cap records */
+#define UPSNET_COCOEVAL_E_RLE_SIZE 32   /* an RLE that does not cover the H x W image, or run_len > cap */
+typedef struct {
+  float score;
+  int category;                         /* K index */
+  int image;                            /* image slot */
+  int rank;                             /* rank in (image, category), < 100 */
+  unsigned long long matched, ignored;  /* bit a * 10 + t */
+} upsnet_coco_record;
+int upsnet_cocoeval_workspace_bytes(int n, int cap, long long gt_counts_total, size_t *bytes);
+int upsnet_cocoeval_image(int segm, const float *boxes, const float *scores, const int64_t *cls_inds, int n,
+                          const int *n_dev, const uint32_t *counts, int cap, const int *run_len, int H, int W,
+                          const double *gt_table, int num_gt, const uint32_t *gt_counts, const int64_t *gt_offsets,
+                          int num_categories, const int *class_to_k, int image_slot, upsnet_coco_record *records,
+                          int record_cap, int *n_records, long long *npig, int *err, void *workspace,
+                          size_t workspace_bytes, void *stream);
+int upsnet_cocoeval_accumulate_workspace_bytes(int n_records, size_t *bytes);
+int upsnet_cocoeval_accumulate(const upsnet_coco_record *records, int n_records, const int *image_rank,
+                               const long long *npig, int num_categories, double *precision, double *recall,
+                               double *scores, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Instance-mask post-processing of the test loop on the device (SURVEY section 8 row f4).
  * replaces: upsnet_end2end_test.py:95-152 `im_post` (expand_boxes bbox/bbox_transform.py:365-381 -> int32 boxes,
  *           (M+2)x(M+2) zero-padded mask -> cv2.resize -> > 0.5 -> paste into [H,W] -> pycocotools.mask.encode), run by the

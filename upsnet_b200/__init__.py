@@ -9,11 +9,11 @@ from .operators import (DeformConv, DeformConvWithOffset, ModDeformConv, ModDefo
                         label_restore)
 
 from .pipeline import PipelinedEngine  # noqa: F401,E402
-from .evaluation import PanopticQuality, SegmentationIoU  # noqa: F401,E402
+from .evaluation import PanopticQuality, SegmentationIoU, DetectionAP  # noqa: F401,E402
 
 __all__ = ["PipelinedEngine", "DeformConv", "DeformConvWithOffset", "ModDeformConv", "ModDeformConvWithOffsetMask",
            "ModulatedDeformConv", "RoIAlign", "ROIAlign", "RoIAlignFunction", "FPNRoIAlign", "PanopticHead",
            "MaskRemoval", "SegTerm", "MaskTerm", "MaskMatching",
            "conv2d", "linear", "deform_conv", "roi_align", "fpn_roi_align", "nms", "nms_segmented", "gpu_nms",
            "gpu_nms_wrapper", "panoptic_fuse", "set_precision", "unified_pan_result", "prep_image", "im_post", "im_post_rle",
-           "label_restore", "PanopticQuality", "SegmentationIoU"]
+           "label_restore", "PanopticQuality", "SegmentationIoU", "DetectionAP"]

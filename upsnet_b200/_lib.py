@@ -90,6 +90,11 @@ def lib():
         L.upsnet_pq_workspace_bytes.argtypes = [C.POINTER(sz)]
         L.upsnet_pq_update.argtypes = [vp, vp, i, i, vp, i, vp, vp, vp, vp, vp, sz, vp]
         L.upsnet_sseg_update.argtypes = [vp, i, i, vp, vp, vp, i, i, i, vp, vp]
+        L.upsnet_cocoeval_workspace_bytes.argtypes = [i, i, C.c_longlong, C.POINTER(sz)]
+        L.upsnet_cocoeval_image.argtypes = [i, vp, vp, vp, i, vp, vp, i, vp, i, i, vp, i, vp, vp, i, vp, i, vp, i, vp, vp,
+                                            vp, vp, sz, vp]
+        L.upsnet_cocoeval_accumulate_workspace_bytes.argtypes = [i, C.POINTER(sz)]
+        L.upsnet_cocoeval_accumulate.argtypes = [vp, i, vp, vp, i, vp, vp, vp, vp, sz, vp]
         _lib = L
     return _lib
 
@@ -105,7 +110,8 @@ EXPORTED_SYMBOLS = [
     "upsnet_dcn_packed_weight_bytes", "upsnet_dcn_pack_weight", "upsnet_dcn_pair_forward", "upsnet_dcn_set_tile_n", "upsnet_tma_set_tile_n",
     "upsnet_fcn_score_fuse", "upsnet_unified_pan_workspace_bytes", "upsnet_unified_pan_result", "upsnet_prep_image", "upsnet_im_post_workspace_bytes", "upsnet_im_post_rle",
     "upsnet_label_restore", "upsnet_pq_workspace_bytes", "upsnet_pq_update",
-    "upsnet_sseg_update",
+    "upsnet_sseg_update", "upsnet_cocoeval_workspace_bytes", "upsnet_cocoeval_image",
+    "upsnet_cocoeval_accumulate_workspace_bytes", "upsnet_cocoeval_accumulate",
 ]
 
 

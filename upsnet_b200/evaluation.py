@@ -28,6 +28,11 @@ matrix stays on the device as int64 and grows by one image per `update()` (csrc/
 The reference's quirks are kept: prediction values wrap mod 256 (np.uint8), the prediction is resized to the ground truth
 with Pillow's NEAREST rule (not cv2's), only gt == 255 is ignored, and a pixel counts in bin gt * C + pred only when
 that bin exists, so gt rows >= C are dropped and predictions >= C alias into later rows.
+
+`DetectionAP` computes the COCO box or mask AP of the reference's evaluate_boxes / evaluate_masks (pycocotools COCOeval
+with its default Params) without the results JSON: update() matches one image on the device (csrc/cocoeval.cu), reading
+the masks from im_post_rle's run lengths, and summarize() accumulates every image's records on the device and copies
+precision / recall / scores back once.
 """
 import collections
 import ctypes as C
@@ -309,3 +314,300 @@ class SegmentationIoU:
 
     def reset(self):
         self._acc.zero_()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# COCO box / mask AP: pycocotools COCOeval ('bbox' / 'segm', default Params) as the reference's evaluate_boxes
+# (base_dataset.py:181-204) and evaluate_masks (coco.py:194-222) run it, on the device (csrc/cocoeval.cu).
+# ---------------------------------------------------------------------------------------------------------------------
+MAX_AP_DET = 2048          # UPSNET_COCOEVAL_MAX_DET: detections per update()
+MAX_AP_GT = 1024           # UPSNET_COCOEVAL_MAX_GT: ground truths per image
+MAX_AP_GT_CAT = 192        # UPSNET_COCOEVAL_MAX_GT_CAT: ground truths per (image, category)
+MAX_AP_CATEGORIES = 256    # UPSNET_COCOEVAL_MAX_CATEGORIES
+MAX_AP_IMAGES = 1 << 17    # UPSNET_COCOEVAL_MAX_IMAGES
+IOU_THRS = np.linspace(.5, 0.95, int(np.round((0.95 - .5) / .05)) + 1, endpoint=True)    # COCOeval Params.setDetParams
+MAX_DETS = [1, 10, 100]
+
+_AP_ERRORS = ((1, "more than %d detections in one image" % MAX_AP_DET),
+              (2, "more than %d ground truths in one image" % MAX_AP_GT),
+              (4, "more than %d ground truths of one category in one image" % MAX_AP_GT_CAT),
+              (8, "a detection class index outside [1, number of categories]"),
+              (16, "more records than record_capacity (kept detections over all images)"),
+              (32, "a mask RLE that does not cover the image (size mismatch, or im_post_rle's buffer overflowed)"))
+
+
+def _mask_counts(mask):
+    """maskApi.c rleEncode of a [H,W] mask: run lengths of the column-major flattening, starting with the zeros run."""
+    v = (np.asarray(mask) != 0).astype(np.uint8).flatten(order="F")
+    if v.size == 0:
+        return np.zeros(0, np.uint32)
+    edges = np.concatenate([[0], np.flatnonzero(v[1:] != v[:-1]) + 1, [v.size]])
+    cnts = np.diff(edges)
+    if v[0]:
+        cnts = np.concatenate([[0], cnts])
+    return cnts.astype(np.uint32)
+
+
+def gt_rle(segmentation):
+    """A ground-truth `segmentation` -> (h, w, uint32 run lengths).  Accepts a compressed or uncompressed COCO RLE dict or
+    a [H,W] mask.  Polygons are rejected: rasterise them first (COCO.annToRLE(ann))."""
+    from .operators import rle_from_string
+    if isinstance(segmentation, dict):
+        h, w = (int(v) for v in segmentation["size"])
+        cnts = segmentation["counts"]
+        counts = rle_from_string(cnts) if isinstance(cnts, (str, bytes)) else np.asarray(cnts, np.int64).astype(np.uint32)
+        return h, w, counts
+    if isinstance(segmentation, list):
+        raise ValueError("polygon segmentations are not rasterised here: pass COCO.annToRLE(ann) as the segmentation")
+    if isinstance(segmentation, torch.Tensor):
+        segmentation = segmentation.cpu().numpy()
+    m = np.asarray(segmentation)
+    if m.ndim != 2:
+        raise ValueError("a mask segmentation must be [H,W], got shape %s" % (m.shape,))
+    return int(m.shape[0]), int(m.shape[1]), _mask_counts(m)
+
+
+def summarize_stats(precision, recall):
+    """COCOeval.summarize()'s 12 stats (_summarizeDets) from precision [T,R,K,A,M] and recall [T,K,A,M]."""
+    area_lbl = ['all', 'small', 'medium', 'large']
+
+    def _summarize(ap=1, iouThr=None, areaRng='all', maxDets=100):
+        aind = [i for i, aRng in enumerate(area_lbl) if aRng == areaRng]
+        mind = [i for i, mDet in enumerate(MAX_DETS) if mDet == maxDets]
+        s = precision if ap == 1 else recall
+        if iouThr is not None:
+            s = s[np.where(iouThr == IOU_THRS)[0]]
+        s = s[:, :, :, aind, mind] if ap == 1 else s[:, :, aind, mind]
+        return -1 if len(s[s > -1]) == 0 else np.mean(s[s > -1])
+    stats = np.zeros((12,))
+    stats[0] = _summarize(1)
+    stats[1] = _summarize(1, iouThr=.5, maxDets=MAX_DETS[2])
+    stats[2] = _summarize(1, iouThr=.75, maxDets=MAX_DETS[2])
+    stats[3] = _summarize(1, areaRng='small', maxDets=MAX_DETS[2])
+    stats[4] = _summarize(1, areaRng='medium', maxDets=MAX_DETS[2])
+    stats[5] = _summarize(1, areaRng='large', maxDets=MAX_DETS[2])
+    stats[6] = _summarize(0, maxDets=MAX_DETS[0])
+    stats[7] = _summarize(0, maxDets=MAX_DETS[1])
+    stats[8] = _summarize(0, maxDets=MAX_DETS[2])
+    stats[9] = _summarize(0, areaRng='small', maxDets=MAX_DETS[2])
+    stats[10] = _summarize(0, areaRng='medium', maxDets=MAX_DETS[2])
+    stats[11] = _summarize(0, areaRng='large', maxDets=MAX_DETS[2])
+    return stats
+
+
+def per_class_ap(precision):
+    """The AP values log_detection_eval_metrics (base_dataset.py:674-716) logs: for IoU [0.50, 0.95] and [0.50, 0.50], the
+    mean over precision[lo:hi+1, :, :, 0, 2] > -1 and the same per K index (the reference slices class j at K index
+    j - 1).  {'0.50:0.95': {'mean', 'per_class'}, '0.50:0.50': {...}}; an empty selection gives nan, as np.mean does."""
+    def thr_ind(thr):
+        return int(np.where((IOU_THRS > thr - 1e-5) & (IOU_THRS < thr + 1e-5))[0][0])
+
+    def mean(p):
+        sel = p[p > -1]
+        return float(np.mean(sel)) if sel.size else float("nan")
+    out = {}
+    lo = thr_ind(0.5)
+    for hi_thr in (0.95, 0.5):
+        hi = thr_ind(hi_thr)
+        p = precision[lo:hi + 1, :, :, 0, 2]
+        out["0.50:%.2f" % hi_thr] = {"mean": mean(p), "per_class": [mean(p[:, :, k]) for k in range(p.shape[2])]}
+    return out
+
+
+class DetectionAP:
+    """COCO box ('bbox') or mask ('segm') AP of the reference's evaluate_boxes / evaluate_masks, computed on one CUDA
+    device.  `categories`: the gt json's category list (or {id: info}).  The K axis of the results is the category ids
+    sorted (COCOeval's p.catIds); a detection of class j (JsonDataset order: the j-th category of `categories`, 1-based)
+    counts for that category's id.  Every image of the dataset must be passed to update() once, with or without
+    detections.  Calls on one object must be issued on one stream.
+
+        ap = DetectionAP(gt_json["categories"], iou_type="segm")
+        for image_id, anns, (boxes, scores, cls_inds, counts, run_len) in data:
+            ap.update(image_id, anns, boxes, scores, cls_inds, rle=(counts, run_len))
+        res = ap.summarize()            # {'stats', 'precision', 'recall', 'scores', 'per_class_ap'}
+    """
+
+    STAGING_SLOTS = 8
+
+    def __init__(self, categories, iou_type="segm", device=None, record_capacity=1 << 20):
+        if iou_type not in ("bbox", "segm"):
+            raise ValueError("iou_type must be 'bbox' or 'segm', got %r" % (iou_type,))
+        if isinstance(categories, dict):
+            categories = [dict(v, id=k) for k, v in categories.items()]
+        ids = [int(c["id"]) for c in categories]
+        if not 1 <= len(ids) <= MAX_AP_CATEGORIES or len(set(ids)) != len(ids):
+            raise ValueError("need 1 to %d distinct category ids, got %d (%d distinct)"
+                             % (MAX_AP_CATEGORIES, len(ids), len(set(ids))))
+        self.iou_type = iou_type
+        self.cat_ids = sorted(ids)
+        self._cat_to_k = {cid: k for k, cid in enumerate(self.cat_ids)}
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        assert self.device.type == "cuda", "DetectionAP runs on a CUDA device (no CPU fallback)"
+        K = len(ids)
+        self._cls_to_k = torch.tensor([-1] + [self._cat_to_k[c] for c in ids], dtype=torch.int32, device=self.device)
+        self.record_capacity = int(record_capacity)
+        self._records = torch.empty((self.record_capacity, 4), dtype=torch.int64, device=self.device)   # 32-byte records
+        self._n_rec = torch.zeros((1,), dtype=torch.int32, device=self.device)
+        self._npig = torch.zeros((K, 4), dtype=torch.int64, device=self.device)
+        self._err = torch.zeros((1,), dtype=torch.int32, device=self.device)
+        self._ws = torch.empty((0,), dtype=torch.uint8, device=self.device)
+        self._stage = [[torch.empty((0,), dtype=torch.uint8), torch.empty((0,), dtype=torch.uint8, device=self.device), None]
+                       for _ in range(self.STAGING_SLOTS)]
+        self._next = 0
+        self._image_ids = []
+        self._seen = set()
+
+    def _det(self, x, dtype, shape, name):
+        if isinstance(x, np.ndarray):
+            x = torch.from_numpy(np.ascontiguousarray(x))
+        x = torch.as_tensor(x)
+        if tuple(x.shape) != shape:
+            raise ValueError("%s must have shape %s, got %s" % (name, shape, tuple(x.shape)))
+        return x.to(self.device, dtype, non_blocking=True).contiguous()
+
+    def _gt_table(self, gt_anns):
+        """fp64 [9][G] (K index, iscrowd, area, x, y, w, h, rle h, rle w) and, for segm, the run lengths and offsets."""
+        G = len(gt_anns)
+        table = np.zeros((9, G), np.float64)
+        runs = []
+        for j, ann in enumerate(gt_anns):
+            cid = int(ann["category_id"])
+            if cid not in self._cat_to_k:
+                raise KeyError("ground-truth category_id %d is not in the categories" % cid)
+            table[0, j] = self._cat_to_k[cid]
+            table[1, j] = 1.0 if ann.get("iscrowd", 0) else 0.0        # _prepare: ignore = iscrowd
+            table[2, j] = float(ann["area"])
+            if self.iou_type == "bbox":
+                table[3:7, j] = [float(v) for v in ann["bbox"]]
+            else:
+                h, w, cnts = gt_rle(ann["segmentation"])
+                table[7, j], table[8, j] = h, w
+                runs.append(cnts)
+        offs = np.zeros(G + 1, np.int64)
+        if runs:
+            offs[1:] = np.cumsum([r.size for r in runs])
+        counts = np.concatenate(runs).astype(np.uint32) if runs else np.zeros(0, np.uint32)
+        return table, offs, counts
+
+    def _stage_gt(self, table, offs, counts):
+        """Copies the ground truths through a ring of pinned buffers; returns device pointers (table, offsets, counts)."""
+        G = table.shape[1]
+        nt, no = 8 * table.size, 8 * offs.size
+        nbytes = nt + no + 4 * counts.size
+        k = self._next % len(self._stage)
+        self._next += 1
+        host, dev, ev = self._stage[k]
+        if ev is not None:
+            ev.synchronize()           # the H2D copy that last read this pinned slot (STAGING_SLOTS updates ago)
+        if host.numel() < nbytes:
+            size = max(nbytes, 2 * host.numel(), 1 << 16)
+            host = torch.empty((size,), dtype=torch.uint8, pin_memory=True)
+            dev = torch.empty((size,), dtype=torch.uint8, device=self.device)
+        h = host.numpy()
+        h[:nt] = table.reshape(-1).view(np.uint8)
+        h[nt:nt + no] = offs.view(np.uint8)
+        h[nt + no:nbytes] = counts.view(np.uint8)
+        if nbytes:
+            dev[:nbytes].copy_(host[:nbytes], non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(self.device))
+        self._stage[k] = [host, dev, ev]
+        base = dev.data_ptr()
+        return (C.c_void_p(base), C.c_void_p(base + nt), C.c_void_p(base + nt + no)) if G else (None, None, None)
+
+    def update(self, image_id, gt_anns, boxes, scores, cls_inds, rle=None, n_dev=None, im_size=None):
+        """Adds one image: COCOeval.evaluate() for its detections and ground truths.
+        gt_anns: the image's instance annotations (category_id, iscrowd, area, and bbox for 'bbox' / segmentation for
+        'segm', as a compressed or uncompressed RLE or a [H,W] mask).  boxes fp32 [n,4] x1 y1 x2 y2, scores fp32 [n],
+        cls_inds int64 [n] class indices in [1, K], in im_post order.  rle = (counts, run_len) as ops.im_post_rle returns
+        them (segm only; they stay on the device).  n_dev: optional device int32 count, as for im_post_rle.  im_size:
+        (H, W) of the detection masks, by default the ground truths' RLE size.  Nothing waits for the device."""
+        if image_id in self._seen:
+            raise ValueError("image id %r was already added" % (image_id,))
+        if len(self._image_ids) >= MAX_AP_IMAGES:
+            raise ValueError("more than %d images" % MAX_AP_IMAGES)
+        n = int(boxes.shape[0]) if hasattr(boxes, "shape") else len(boxes)
+        b = self._det(boxes, torch.float32, (n, 4), "boxes")
+        s = self._det(scores, torch.float32, (n,), "scores")
+        c = self._det(cls_inds, torch.int64, (n,), "cls_inds")
+        segm = self.iou_type == "segm"
+        if segm and rle is None:
+            raise ValueError("iou_type 'segm' needs rle=(counts, run_len)")
+        table, offs, counts = self._gt_table(gt_anns)
+        G = table.shape[1]
+        cnt, rl, cap, H, W = None, None, 0, 0, 0
+        if segm:
+            cnt, rl = rle[0], rle[1]
+            if not (cnt.is_cuda and rl.is_cuda) or cnt.dim() != 2 or cnt.shape[0] < n or rl.numel() < n \
+                    or cnt.element_size() != 4 or rl.dtype != torch.int32:
+                raise ValueError("rle must be im_post_rle's device tensors (counts [n, cap] 32-bit, run_len int32 [n])")
+            cnt, rl, cap = cnt.contiguous(), rl.contiguous(), int(cnt.shape[1])
+            if im_size is not None:
+                H, W = (int(v) for v in im_size)
+            elif G:
+                H, W = int(table[7, 0]), int(table[8, 0])
+            nb = C.c_size_t(0)
+            check(lib().upsnet_cocoeval_workspace_bytes(n, cap, int(counts.size), C.byref(nb)), "cocoeval_workspace_bytes")
+            if self._ws.numel() < nb.value:
+                self._ws = torch.empty((nb.value,), dtype=torch.uint8, device=self.device)
+        if n_dev is not None and (not n_dev.is_cuda or n_dev.dtype != torch.int32):
+            raise ValueError("n_dev must be a device int32 tensor")
+        if G <= MAX_AP_GT:
+            t_ptr, o_ptr, c_ptr = self._stage_gt(table, offs, counts)
+        else:                          # only counted: the device raises the error flag without reading the table
+            t_ptr = o_ptr = c_ptr = None
+        slot = len(self._image_ids)
+        with torch.cuda.device(self.device):
+            check(lib().upsnet_cocoeval_image(int(segm), ptr(b), ptr(s), ptr(c), n, ptr(n_dev), ptr(cnt), cap, ptr(rl), H, W,
+                                              t_ptr, G, c_ptr, o_ptr, len(self.cat_ids), ptr(self._cls_to_k), slot,
+                                              ptr(self._records), self.record_capacity, ptr(self._n_rec), ptr(self._npig),
+                                              ptr(self._err), ptr(self._ws), self._ws.numel(), stream_ptr(self.device)),
+                  "cocoeval_image")
+        self._image_ids.append(image_id)
+        self._seen.add(image_id)
+
+    def check_errors(self):
+        """Raises if any update() so far hit an error (the flags are sticky until reset())."""
+        e = int(self._err.item())
+        for bit, msg in _AP_ERRORS:
+            if e & bit:
+                raise UpsnetError("cocoeval: " + msg)
+
+    def accumulate(self):
+        """COCOeval.accumulate(): {'precision' [10,101,K,4,3], 'recall' [10,K,4,3], 'scores' [10,101,K,4,3]} fp64 numpy."""
+        self.check_errors()
+        N = int(self._n_rec.item())
+        K = len(self.cat_ids)
+        rank = np.empty(len(self._image_ids), np.int32)
+        rank[np.argsort(np.asarray(self._image_ids), kind="stable")] = np.arange(len(self._image_ids), dtype=np.int32)
+        rank_d = torch.from_numpy(rank).to(self.device)
+        nb = C.c_size_t(0)
+        check(lib().upsnet_cocoeval_accumulate_workspace_bytes(N, C.byref(nb)), "cocoeval_accumulate_workspace_bytes")
+        ws = torch.empty((max(nb.value, 1),), dtype=torch.uint8, device=self.device)
+        f64 = dict(dtype=torch.float64, device=self.device)
+        out = torch.empty((2 * 10 * 101 * K * 12 + 10 * K * 12,), **f64)
+        precision = out[:10 * 101 * K * 12].view(10, 101, K, 4, 3)
+        scores = out[10 * 101 * K * 12:2 * 10 * 101 * K * 12].view(10, 101, K, 4, 3)
+        recall = out[2 * 10 * 101 * K * 12:].view(10, K, 4, 3)
+        with torch.cuda.device(self.device):
+            check(lib().upsnet_cocoeval_accumulate(ptr(self._records), N, ptr(rank_d), ptr(self._npig), K, ptr(precision),
+                                                   ptr(recall), ptr(scores), ptr(ws), ws.numel(), stream_ptr(self.device)),
+                  "cocoeval_accumulate")
+        host = out.cpu().numpy()                                         # the one copy back
+        n1 = 10 * 101 * K * 12
+        return {"precision": host[:n1].reshape(10, 101, K, 4, 3), "scores": host[n1:2 * n1].reshape(10, 101, K, 4, 3),
+                "recall": host[2 * n1:].reshape(10, K, 4, 3)}
+
+    def summarize(self):
+        """{'stats': COCOeval.stats (12 floats), 'precision', 'recall', 'scores', 'per_class_ap'} (per_class_ap: the values
+        log_detection_eval_metrics logs, see per_class_ap())."""
+        ev = self.accumulate()
+        return {"stats": summarize_stats(ev["precision"], ev["recall"]), "precision": ev["precision"],
+                "recall": ev["recall"], "scores": ev["scores"], "per_class_ap": per_class_ap(ev["precision"])}
+
+    def reset(self):
+        self._n_rec.zero_()
+        self._npig.zero_()
+        self._err.zero_()
+        self._image_ids = []
+        self._seen = set()

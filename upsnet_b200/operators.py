@@ -1273,6 +1273,28 @@ def rle_to_string(cnts):
     return bytes(out)
 
 
+def rle_from_string(s):
+    """pycocotools maskApi.c rleFrString, the inverse of rle_to_string: uint32 run lengths from the compressed `counts`
+    of a COCO RLE (str or bytes)."""
+    if isinstance(s, str):
+        s = s.encode()
+    cnts, p = [], 0
+    while p < len(s):
+        x, k, more = 0, 0, True
+        while more:
+            c = s[p] - 48
+            x |= (c & 0x1f) << (5 * k)
+            more = bool(c & 0x20)
+            p += 1
+            k += 1
+            if not more and (c & 0x10):
+                x |= -1 << (5 * k)
+        if len(cnts) > 2:
+            x += cnts[-2]
+        cnts.append(x)
+    return np.asarray(cnts, np.int64).astype(np.uint32)
+
+
 def im_post_rle(pred_boxes, pred_masks, cls_inds, im_h, im_w, n_dev=None, cap=None):
     """upsnet_im_post_rle: the COCO run lengths of every detection's pasted mask, computed on the device without
     materialising the [H,W] images.  pred_boxes [n,4] or [n,5] (batch index first, like the model's `pred_boxes`),
