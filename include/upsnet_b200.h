@@ -452,6 +452,38 @@ int upsnet_cocoeval_accumulate(const upsnet_coco_record *records, int n_records,
                                double *scores, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * upsnet_combined_pan_result: the combined panoptic result (instance output merged heuristically with the semantic head).
+ * replaces: dataset/base_dataset.py:373-449 get_combined_pan_result + _merge_pred_single_core (every detection decoded
+ *           to a full [H,W] image with pycocotools and three full-image boolean passes per detection, on the host).
+ * sem [H,W] of sem_elem_size = 1 (uint8) or 8 (int64, each value wrapped to uint8), the restored semantic map;
+ *   H * W <= 2^24 (the float32 pixel counts of the reference are exact up to there).
+ * Detections: scores fp32 [n], cls_inds int64 [n]; only the first min(n, *n_dev) count when n_dev (device int) is given,
+ *   and of those only classes in [1, num_classes) (the ones im_post keeps).  Masks: counts uint32 [n][cap] / run_len
+ *   int32 [n] exactly as upsnet_im_post_rle leaves them, of an H x W image.
+ * Order: descending score; among equal scores the detection later in the class-ascending concatenation of im_post's
+ *   per-class lists first, i.e. (score desc, class desc, index desc) -- np.argsort(score, kind='stable')[::-1].
+ * A detection is skipped when score < score_threshold, when its mask is empty, or when (float32) remain / area <
+ *   fraction_threshold, remain = its pixels not claimed by an earlier kept detection.  A kept detection of class c gets
+ *   instance number (++count[c]) mod 256 and claims its free pixels; number 0 (the 256th, ...) claims nothing.
+ * pan_2ch uint8 [H,W,3]: channel 0 = the semantic class, 255 where a class <= id_last_stuff (= num_seg_classes -
+ *   num_classes) has fewer than stuff_area_limit pixels or where a class > id_last_stuff has no instance, and
+ *   (c + id_last_stuff) mod 256 on the pixels of an instance of class c; channel 1 = the instance number; channel 2 = 0.
+ * err (DEVICE int, sticky): UPSNET_COMBINED_E_* below; a detection whose runs are unusable is skipped, more than
+ *   UPSNET_COMBINED_MAX_DET detections skips them all.  The call never synchronises.
+ * Workspace: upsnet_combined_pan_workspace_bytes(n, H, W) (a histogram, an H*W-bit occupancy bitmap and a 2-byte owner
+ * per pixel). */
+#define UPSNET_COMBINED_MAX_DET 2048
+#define UPSNET_COMBINED_E_RUN_LEN 1     /* run_len > cap (upsnet_im_post_rle overflowed its buffer) or < 0 */
+#define UPSNET_COMBINED_E_RLE_SIZE 2    /* runs that do not sum to H * W */
+#define UPSNET_COMBINED_E_DET_COUNT 4   /* more than UPSNET_COMBINED_MAX_DET detections */
+int upsnet_combined_pan_workspace_bytes(int n, int H, int W, size_t *bytes);
+int upsnet_combined_pan_result(const void *sem, int sem_elem_size, int H, int W, const float *scores,
+                               const int64_t *cls_inds, int n, const int *n_dev, const uint32_t *counts, int cap,
+                               const int *run_len, int num_seg_classes, int num_classes, float score_threshold,
+                               float fraction_threshold, int stuff_area_limit, unsigned char *pan_2ch, int *err,
+                               void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Instance-mask post-processing of the test loop on the device (SURVEY section 8 row f4).
  * replaces: upsnet_end2end_test.py:95-152 `im_post` (expand_boxes bbox/bbox_transform.py:365-381 -> int32 boxes,
  *           (M+2)x(M+2) zero-padded mask -> cv2.resize -> > 0.5 -> paste into [H,W] -> pycocotools.mask.encode), run by the

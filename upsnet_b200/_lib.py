@@ -95,6 +95,8 @@ def lib():
                                             vp, vp, sz, vp]
         L.upsnet_cocoeval_accumulate_workspace_bytes.argtypes = [i, C.POINTER(sz)]
         L.upsnet_cocoeval_accumulate.argtypes = [vp, i, vp, vp, i, vp, vp, vp, vp, sz, vp]
+        L.upsnet_combined_pan_workspace_bytes.argtypes = [i, i, i, C.POINTER(sz)]
+        L.upsnet_combined_pan_result.argtypes = [vp, i, i, i, vp, vp, i, vp, vp, i, vp, i, i, f, f, i, vp, vp, vp, sz, vp]
         _lib = L
     return _lib
 
@@ -112,6 +114,7 @@ EXPORTED_SYMBOLS = [
     "upsnet_label_restore", "upsnet_pq_workspace_bytes", "upsnet_pq_update",
     "upsnet_sseg_update", "upsnet_cocoeval_workspace_bytes", "upsnet_cocoeval_image",
     "upsnet_cocoeval_accumulate_workspace_bytes", "upsnet_cocoeval_accumulate",
+    "upsnet_combined_pan_workspace_bytes", "upsnet_combined_pan_result",
 ]
 
 

@@ -1339,3 +1339,107 @@ def im_post(boxes_all, masks_all, scores, pred_boxes, pred_masks, cls_inds, num_
         segms = [{"size": [H, W], "counts": rle_to_string(cn[d, :rl[d]]).decode()} for d in sel]
         boxes_all[idx].append(cls_boxes)
         masks_all[idx].append(segms)
+
+
+# ------------------------------------------------------------------------------------------------
+# combined panoptic result (dataset/base_dataset.py:373-449): instance output merged with the semantic head
+# ------------------------------------------------------------------------------------------------
+_comb_ws = _Workspace()
+COMBINED_ERRORS = ((1, "a detection needs more RLE counts than im_post_rle's buffer holds"),
+                   (2, "an RLE whose runs do not cover the semantic map (mask size != semantic map size)"),
+                   (4, "more than 2048 detections"))
+
+
+def combined_pan_result(sem, scores, cls_inds, rle, num_seg_classes, num_classes, score_threshold=0.6,
+                        fraction_threshold=0.7, stuff_area_limit=4 * 64 * 64, n_dev=None, check_errors=True):
+    """dataset/base_dataset.py:373-449 get_combined_pan_result + _merge_pred_single_core for one image, on the device.
+    sem int64 or uint8 [H,W] / [1,H,W] (the restored semantic map; int64 values wrap to uint8); scores fp32 [n] and
+    cls_inds [n] of the detections (classes outside [1, num_classes) are ignored, as im_post drops them); rle = (counts,
+    run_len) as im_post_rle returns them, of an H x W image; n_dev optional device count <= n.  Detections are taken by
+    descending score, ties by the later position in im_post's class-ascending concatenation (class desc, index desc).
+    -> uint8 [H,W,3] (class, instance number, 0).  Sync-free unless check_errors (one int D2H: raises ValueError for a
+    mask size that differs from the map's, UpsnetError for the other error bits)."""
+    counts, run_len = rle[0], rle[1]
+    require_cuda(sem, scores, cls_inds, counts, run_len, n_dev)
+    if sem.dtype not in (torch.uint8, torch.int64):
+        sem = sem.to(torch.int64)
+    sem = sem.reshape(sem.shape[-2:]).contiguous()
+    H, W = int(sem.shape[0]), int(sem.shape[1])
+    if H * W > 1 << 24:
+        raise ValueError("combined_pan_result: %dx%d image: the reference's float32 pixel counts are exact up to 2^24 "
+                         "pixels only" % (H, W))
+    sc = f32c(scores.reshape(-1))
+    cls = cls_inds.reshape(-1).to(torch.int64).contiguous()
+    n = int(sc.numel())
+    assert cls.numel() == n and run_len.numel() >= n and (n == 0 or counts.shape[0] >= n)
+    cap = int(counts.shape[1]) if counts.dim() == 2 else 1
+    cn, rl = counts.contiguous(), run_len.to(torch.int32).contiguous()
+    dev = sem.device
+    nb = C.c_size_t(0)
+    check(lib().upsnet_combined_pan_workspace_bytes(n, H, W, C.byref(nb)), "combined_pan_workspace_bytes")
+    ws = _comb_ws.get(dev, nb.value)
+    out = torch.empty((H, W, 3), dtype=torch.uint8, device=dev)
+    err = torch.zeros((1,), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev), _Timed("combined_pan", 3, {"bytes": (sem.element_size() * 2 + 3.25) * H * W}, dev):
+        check(lib().upsnet_combined_pan_result(ptr(sem), sem.element_size(), H, W, ptr(sc), ptr(cls), n, ptr(n_dev),
+                                               ptr(cn), cap, ptr(rl), int(num_seg_classes), int(num_classes),
+                                               float(score_threshold), float(fraction_threshold), int(stuff_area_limit),
+                                               ptr(out), ptr(err), ptr(ws), ws.numel(), stream_ptr(dev)),
+              "combined_pan_result")
+    if check_errors:
+        e = int(err.item())
+        if e & 2:
+            raise ValueError("combined_pan_result: " + COMBINED_ERRORS[1][1])
+        if e:
+            raise _lib.UpsnetError("combined_pan_result: " + "; ".join(m for b, m in COMBINED_ERRORS if e & b))
+    return out
+
+
+def combined_inputs(boxes, masks, i, H, W):
+    """Host side of get_combined_pan_result for image i: the per-class lists concatenated in ascending class order (the
+    reference's order before its sort) -> scores fp32 [n], classes int64 [n], counts uint32 [max(n,1), cap] and run_len
+    int32 [max(n,1)] in im_post_rle's layout.  Compressed `counts` strings are parsed with rle_from_string; lists of run
+    lengths are taken as they are.  A mask whose size is not (H, W) raises ValueError (the reference fails to broadcast)."""
+    sc, cl, runs = [], [], []
+    for j in range(1, len(boxes)):
+        b = np.asarray(boxes[j][i], np.float32).reshape(-1, 5)
+        ms = masks[j][i]
+        assert len(ms) == b.shape[0], "boxes[%d][%d] and masks[%d][%d] differ in length" % (j, i, j, i)
+        for m in ms:
+            if [int(v) for v in m["size"]] != [int(H), int(W)]:
+                raise ValueError("mask size %s != semantic map size %s (image %d)" % (list(m["size"]), [H, W], i))
+            c = m["counts"]
+            runs.append(rle_from_string(c) if isinstance(c, (str, bytes)) else np.asarray(c, np.int64).astype(np.uint32))
+        sc.append(b[:, 4])
+        cl.append(np.full(b.shape[0], j, np.int64))
+    n = len(runs)
+    cap = max([r.size for r in runs] + [1])
+    cn = np.zeros((max(n, 1), cap), np.uint32)
+    rl = np.zeros(max(n, 1), np.int32)
+    for d, r in enumerate(runs):
+        cn[d, :r.size] = r
+        rl[d] = r.size
+    sc = np.concatenate(sc).astype(np.float32) if sc else np.zeros(0, np.float32)
+    cl = np.concatenate(cl) if cl else np.zeros(0, np.int64)
+    return sc, cl, cn, rl
+
+
+def get_combined_pan_result(segs, boxes, masks, num_seg_classes, num_classes, score_threshold=0.6,
+                            fraction_threshold=0.7, stuff_area_limit=4 * 64 * 64, device=None):
+    """Drop-in for dataset/base_dataset.py:373-403 get_combined_pan_result on the test script's results (all_ssegs,
+    all_boxes, all_masks): segs[i] uint8 [H,W]; boxes[j][i] [n_ij,5] (score in column 4) and masks[j][i] COCO RLE dicts
+    for classes j = 1 .. len(boxes) - 1.  Each image's compressed strings are parsed on the host and uploaded once; the
+    merge runs on the device.  -> list of uint8 [H,W,3] numpy maps.  The reference's num_seg_classes / num_classes come
+    from config.dataset; here they are arguments.  `segs` is not modified."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    out = []
+    for i, seg in enumerate(segs):
+        seg = np.ascontiguousarray(seg)
+        sc, cl, cn, rl = combined_inputs(boxes, masks, i, seg.shape[0], seg.shape[1])
+        # one pinned upload of everything the image needs
+        tensors = [torch.from_numpy(a) for a in (seg, sc, cl, cn.view(np.int32), rl)]
+        seg_d, sc_d, cl_d, cn_d, rl_d = [t.pin_memory().to(dev, non_blocking=True) for t in tensors]
+        pan = combined_pan_result(seg_d, sc_d, cl_d, (cn_d, rl_d), num_seg_classes, num_classes, score_threshold,
+                                  fraction_threshold, stuff_area_limit)
+        out.append(pan.cpu().numpy())
+    return out

@@ -23,25 +23,45 @@ class PipelinedEngine:
     PIXEL_MEANS = (102.9801, 115.9465, 122.7717)     # config.network.pixel_means (BGR, caffe models)
 
     def __init__(self, model, im_info, depth=2, with_masks=False, with_unified=False, stuff_area_limit=4 * 64 * 64,
-                 pixel_means=None, im_scale=1.0, lanes=None, label_maps=True, restore_size=False):
+                 pixel_means=None, im_scale=1.0, lanes=None, label_maps=True, restore_size=False, with_combined=False,
+                 combined_score_threshold=0.6, combined_fraction_threshold=0.7):
         """with_unified: also run get_unified_pan_result on the device (base_dataset.py:332-371) and return its uint8
         [H,W,3] map as 'pan_2ch'.  submit() also accepts the RAW uint8 [h,w,3] BGR image (pinned): mean subtraction,
         resize by im_scale and padding (prep_im_for_blob / im_list_to_blob) then run on the device after a 4x smaller H2D.
         restore_size: crop the two label maps to im_info[:2] and resize them back to the original image size
         (upsnet_end2end_test.py:259-266, one label_restore launch) before they are returned and before pan_2ch is
         computed from them, as the reference does before its PQ evaluation; needed whenever im_info's scale != 1 or
-        the network input is padded."""
+        the network input is padded.
+        with_combined: also build the combined panoptic map (base_dataset.py:373-449 get_combined_pan_result, the
+        instance output merged with the semantic head) on the device and return it as 'pan_2ch_combined'.  It does what
+        the test script's im_detect + im_post + the merge do: pred_boxes[:, 1:] / im_info[2] in fp32, the masks' run
+        lengths at round(im_info[:2] / im_info[2]) (upsnet_im_post_rle), then upsnet_combined_pan_result on the restored
+        semantic map.  Needs restore_size=True and an im_info whose im_post size equals the restored size."""
         self.model, self.depth = model, depth
         # engine lanes: slot i computes on lane i % lanes (own CUDA-graph instance, activation pool, scratch, stream), so the
         # forward passes of `lanes` consecutive images overlap on the GPU; lanes=1 is the strictly serial compute of round 1
         self.lanes = depth if lanes is None else max(1, min(int(lanes), depth))
         self.im_info = np.asarray(im_info, dtype=np.float32).reshape(-1, 3)[0]
-        self.keys = self.RESULT_KEYS + (("mask_probs",) if with_masks else ()) + (("pan_2ch",) if with_unified else ())
+        self.keys = self.RESULT_KEYS + (("mask_probs",) if with_masks else ()) + (("pan_2ch",) if with_unified else ()) + \
+            (("pan_2ch_combined",) if with_combined else ())
         if not label_maps:      # serving format: the unified 2-channel map replaces the two int64 label maps on the way out
             assert with_unified, "label_maps=False needs with_unified=True (pan_2ch carries class and instance id)"
             self.keys = tuple(k for k in self.keys if k not in ("panoptic_outputs", "fcn_outputs"))
         self.with_unified, self.stuff_area_limit, self.restore_size = with_unified, stuff_area_limit, restore_size
         self.pixel_means, self.im_scale = (pixel_means or self.PIXEL_MEANS), float(im_scale)
+        self.with_combined = with_combined
+        if with_combined:
+            from . import operators as ops
+            if not restore_size:
+                raise ValueError("with_combined needs restore_size=True: the merge runs on the restored semantic map")
+            # upsnet_end2end_test.py passes np.round(im_info[:2] / im_info[2]) to im_post, while the restore follows cv2's
+            # dsize rule; the reference fails to broadcast where the two differ
+            self.combined_size = tuple(int(v) for v in np.round(self.im_info[:2] / self.im_info[2]))
+            restored = ops.label_restore_geometry(self.im_info)[3:]
+            if self.combined_size != restored:
+                raise ValueError("im_post size %s != restored label size %s for im_info %s"
+                                 % (self.combined_size, restored, self.im_info.tolist()))
+            self.combined_thresholds = (float(combined_score_threshold), float(combined_fraction_threshold))
         self.dev = None
         self._t = 0
         self._slots = None
@@ -125,6 +145,16 @@ class PipelinedEngine:
             out["pan_2ch"] = ops.unified_pan_result(out["fcn_outputs"], out["panoptic_outputs"], out["p_cls"][out["keep"]],
                                                     m.num_seg_classes, m.num_classes, self.stuff_area_limit,
                                                     k_dev=out["counts"][2:3], check_errors=False)
+        if self.with_combined:
+            m, n_dev = self.model, out["counts"][0:1]
+            pb = out["pred_boxes"]
+            # im_detect's pred_boxes[:, 1:] / im_info[2]: an elementwise fp32 division (a scalar divisor would be turned
+            # into a multiplication by its reciprocal)
+            boxes = pb[:, 1:] / torch.full((1, 1), float(self.im_info[2]), dtype=torch.float32, device=pb.device)
+            rle = ops.im_post_rle(boxes, out["mask_probs"], out["cls_inds"], *self.combined_size, n_dev=n_dev)[:2]
+            out["pan_2ch_combined"] = ops.combined_pan_result(out["fcn_outputs"], out["cls_probs"], out["cls_inds"], rle,
+                                                              m.num_seg_classes, m.num_classes, *self.combined_thresholds,
+                                                              self.stuff_area_limit, n_dev=n_dev, check_errors=False)
         return out
 
     def result(self, ticket):
@@ -146,6 +176,8 @@ class PipelinedEngine:
             res["mask_probs"] = h["mask_probs"][:n1]
         if "pan_2ch" in h:
             res["pan_2ch"] = h["pan_2ch"]
+        if "pan_2ch_combined" in h:
+            res["pan_2ch_combined"] = h["pan_2ch_combined"]
         return res
 
     def bytes_per_image(self):
