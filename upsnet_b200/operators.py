@@ -823,6 +823,18 @@ def gpu_nms_wrapper(thresh, device_id):
 # ------------------------------------------------------------------------------------------------
 # modules (reference names / signatures / parameter names)
 # ------------------------------------------------------------------------------------------------
+def _needs_grad(*tensors):
+    """True when autograd records and one of the (plain tensor) inputs or parameters requires grad."""
+    return torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in tensors)
+
+
+def _check_dg_for_grad(deformable_groups):
+    if deformable_groups != 1:
+        raise NotImplementedError("DeformConv / ModDeformConv backward supports deformable_groups=1 only (got %d); run "
+                                  "the forward under torch.no_grad() or with parameters that do not require grad"
+                                  % deformable_groups)
+
+
 class DeformConv(nn.Module):
     """operators/modules/deform_conv.py:27-64.  Parameters are created on CUDA like the reference."""
 
@@ -854,8 +866,8 @@ class DeformConv(nn.Module):
             self.bias.data.uniform_(-stdv, stdv)
 
     def forward(self, data, offset):
-        if torch.is_grad_enabled() and self.deformable_groups == 1 and \
-                any(t is not None and t.requires_grad for t in (data, offset, self.weight, self.bias)):
+        if _needs_grad(data, offset, self.weight, self.bias):
+            _check_dg_for_grad(self.deformable_groups)
             from .training import DeformConvFunction      # training path: hand-written backward kernels (csrc/backward.cu)
             return DeformConvFunction.apply(data, offset, self.weight, self.bias, self.stride, self.padding, self.dilation)
         return deform_conv(data, offset, self.weight, self.bias, self.stride, self.padding, self.dilation,
@@ -877,6 +889,9 @@ class DeformConvWithOffset(nn.Module):
                                deformable_groups=deformable_groups, bias=bias)
 
     def forward(self, x):
+        if _needs_grad(x, self.conv_offset.weight, self.conv_offset.bias):
+            from .training import OffsetConvFunction      # differentiable offsets, same forward
+            return self.conv(x, OffsetConvFunction.apply(x, self.conv_offset.weight, self.conv_offset.bias))
         offset = conv2d(x, self.conv_offset.weight, self.conv_offset.bias, 1, 1, 1, out_format="nchw")
         return self.conv(x, offset)
 
@@ -889,8 +904,8 @@ class ModDeformConv(DeformConv):
         offset_1, offset_2, mask = torch.chunk(offset_mask, 3, dim=1)
         offset = torch.cat((offset_1, offset_2), dim=1)
         mask = torch.sigmoid(mask) * 2
-        if torch.is_grad_enabled() and self.deformable_groups == 1 and \
-                any(t is not None and t.requires_grad for t in (data, offset_mask, self.weight, self.bias)):
+        if _needs_grad(data, offset_mask, self.weight, self.bias):
+            _check_dg_for_grad(self.deformable_groups)
             from .training import ModDeformConvFunction
             return ModDeformConvFunction.apply(data, offset, mask, self.weight, self.bias, self.stride, self.padding, self.dilation)
         return deform_conv(data, offset, self.weight, self.bias, self.stride, self.padding, self.dilation,
@@ -915,6 +930,9 @@ class ModDeformConvWithOffsetMask(nn.Module):
                                   deformable_groups=deformable_groups, bias=bias)
 
     def forward(self, x):
+        if _needs_grad(x, self.conv_offset_mask.weight, self.conv_offset_mask.bias):
+            from .training import OffsetConvFunction
+            return self.conv(x, OffsetConvFunction.apply(x, self.conv_offset_mask.weight, self.conv_offset_mask.bias))
         om = conv2d(x, self.conv_offset_mask.weight, self.conv_offset_mask.bias, 1, 1, 1, out_format="nchw")
         return self.conv(x, om)
 
@@ -961,7 +979,14 @@ class FPNRoIAlign(nn.Module):
         self.with_expand = with_expand
 
     def forward(self, feat, rois):
-        return fpn_roi_align(list(feat), rois, self.pooled_height, self.pooled_width, self.spatial_scale,
+        feat = list(feat)
+        if torch.is_grad_enabled() and any(getattr(f, "requires_grad", False) for f in feat):
+            if not all(isinstance(f, torch.Tensor) and f.dtype == torch.float32 for f in feat):
+                raise TypeError("FPNRoIAlign: the backward kernel takes fp32 features; pair / bf16 features cannot "
+                                "require grad")
+            from .training import FPNRoIAlignFunction     # training path: upsnet_roi_align_backward per level
+            return FPNRoIAlignFunction.apply(rois, self.pooled_height, self.pooled_width, self.spatial_scale, 2, *feat)
+        return fpn_roi_align(feat, rois, self.pooled_height, self.pooled_width, self.spatial_scale,
                              layout="auto")
 
 

@@ -3,8 +3,10 @@
 * autograd Functions for the custom operators with hand-written sm_90a BACKWARD kernels (csrc/backward.cu):
     DeformConvFunction / ModDeformConvFunction   operators/functions/deform_conv.py:26-108, mod_deform_conv.py:25-118
     RoIAlignFunction                             operators/functions/roialign.py:21-58
+    FPNRoIAlignFunction                          operators/modules/fpn_roi_align.py:32-62 (four RoIAlignFunction calls)
   The dense GEMMs of the deformable backward (d(weight) = dY col^T, d(col) = W^T dY) are library calls (torch.mm), like the
-  reference's; the gather / scatter / coordinate-gradient kernels are ours.
+  reference's; the gather / scatter / coordinate-gradient kernels are ours.  OffsetConvFunction makes the offset conv of
+  the *WithOffset* modules differentiable; its backward convs are library calls too.
 * FlatBucketAllReduce: the gradient all-reduce of `upsnet_end2end_train.py:121` (hvd.DistributedOptimizer) as flat bf16
   buckets over torch.distributed (NCCL between the GPUs, gloo in the CPU tests): gradients are packed per bucket,
   reduced asynchronously while the rest of backward runs, averaged and unpacked before the optimiser step.
@@ -116,12 +118,80 @@ class RoIAlignFunction(torch.autograd.Function):
     def backward(ctx, grad_out):
         (rois,) = ctx.saved_tensors
         (B, Cc, H, W), ph, pw, scale, sr = ctx.cfg
+        if rois.shape[0] == 0:          # an empty grad_out has no data pointer for the C ABI; nothing to scatter
+            return torch.zeros((B, Cc, H, W), dtype=torch.float32, device=grad_out.device), None, None, None, None, None
         grad_out, rois = f32c(grad_out), f32c(rois)
         dfeat = torch.empty((B, Cc, H, W), dtype=torch.float32, device=grad_out.device)
         with torch.cuda.device(grad_out.device):
             check(lib().upsnet_roi_align_backward(ptr(grad_out), ptr(rois), rois.shape[0], B, Cc, H, W, ph, pw, sr, scale,
                                                   ptr(dfeat), stream_ptr(grad_out.device)), "roi_align_backward")
         return dfeat, None, None, None, None, None
+
+
+class OffsetConvFunction(torch.autograd.Function):
+    """The 3x3 / pad 1 offset (and mask) conv of DeformConvWithOffset / ModDeformConvWithOffsetMask: forward is the same
+    ops.conv2d the no-grad path runs (so the offsets, and where the samples land, do not depend on requires_grad); backward
+    is the library's fp32 conv gradients with TF32 off, plus the bias sum."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        from . import operators as ops
+        ctx.save_for_backward(x, weight)
+        ctx.has_bias = bias is not None
+        return ops.conv2d(x, weight, bias, 1, 1, 1, out_format="nchw")
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        x, weight = ctx.saved_tensors
+        grad_out = grad_out.float()
+        dx = dw_ = None
+        with torch.backends.cudnn.flags(enabled=torch.backends.cudnn.enabled, benchmark=torch.backends.cudnn.benchmark,
+                                        deterministic=torch.backends.cudnn.deterministic, allow_tf32=False):
+            if ctx.needs_input_grad[0]:
+                dx = torch.nn.grad.conv2d_input(x.shape, weight, grad_out, stride=1, padding=1)
+            if ctx.needs_input_grad[1]:
+                dw_ = torch.nn.grad.conv2d_weight(x, weight.shape, grad_out, stride=1, padding=1)
+        db = grad_out.sum(dim=(0, 2, 3)) if ctx.has_bias and ctx.needs_input_grad[2] else None
+        return dx, dw_, db
+
+
+class FPNRoIAlignFunction(torch.autograd.Function):
+    """FPNRoIAlign on fp32 features [P2..P5]: forward = upsnet_roi_align_fpn_forward, which also writes the level it chose
+    for every roi; backward = upsnet_roi_align_backward once per level on the output gradient with the rows of the other
+    levels zeroed.  The levels come from the forward kernel, never recomputed on the host: a rounding difference at a level
+    boundary would send a roi's gradient to the wrong level."""
+
+    @staticmethod
+    def forward(ctx, rois, pooled_height, pooled_width, spatial_scales, sampling_ratio, *feats):
+        from . import operators as ops
+        out, levels = ops.fpn_roi_align(list(feats), rois, pooled_height, pooled_width, spatial_scales, sampling_ratio,
+                                        layout="auto", return_levels=True)
+        ctx.save_for_backward(rois, levels)
+        ctx.cfg = ([tuple(f.shape) for f in feats], int(pooled_height), int(pooled_width),
+                   [float(s) for s in spatial_scales], int(sampling_ratio))
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        rois, levels = ctx.saved_tensors
+        shapes, ph, pw, scales, sr = ctx.cfg
+        grad_out, rois = f32c(grad_out), f32c(rois)
+        R = rois.shape[0]
+        dfeats = []
+        with torch.cuda.device(grad_out.device):
+            for lv, (B, Cc, H, W) in enumerate(shapes):
+                if not ctx.needs_input_grad[5 + lv]:
+                    dfeats.append(None)
+                    continue
+                if R == 0:
+                    dfeats.append(torch.zeros((B, Cc, H, W), dtype=torch.float32, device=grad_out.device))
+                    continue
+                g = torch.where((levels == lv).view(R, 1, 1, 1), grad_out, 0.0).contiguous()
+                dfeat = torch.empty((B, Cc, H, W), dtype=torch.float32, device=grad_out.device)
+                check(lib().upsnet_roi_align_backward(ptr(g), ptr(rois), R, B, Cc, H, W, ph, pw, sr, scales[lv],
+                                                      ptr(dfeat), stream_ptr(grad_out.device)), "roi_align_backward")
+                dfeats.append(dfeat)
+        return (None, None, None, None, None) + tuple(dfeats)
 
 
 # ------------------------------------------------------------------------------------------------
