@@ -75,11 +75,13 @@ int upsnet_roi_align_forward(const void *feat, int B, int C, int H, int W, int l
  * replaces: operators/modules/fpn_roi_align.py:32-62 FPNRoIAlign.forward (host bucketing,
  *           4 launches, cat, index_select).  feats[l] has spatial size (Hs[l],Ws[l]) and
  *           scale scales[l]; level(roi) = clip(floor(2+log2(sqrt(w*h)/224+1e-6)),0,3).
- * levels_out (optional, may be NULL): int32 [R] chosen level per roi. */
+ * levels_out (optional, may be NULL): int32 [R] chosen level per roi.
+ * n_dev (optional, may be NULL; UPSNET_DTYPE_PAIR only): int32 device count -- rois >= *n_dev are neither read nor
+ * written (the launch keeps R blocks, so a captured graph does not change shape). */
 int upsnet_roi_align_fpn_forward(const void *const feats[4], const int Hs[4], const int Ws[4],
                                  const float scales[4], int B, int C, int layout, int dtype,
                                  const float *rois, int R, int PH, int PW, int sampling_ratio,
-                                 void *out, int *levels_out, void *stream);
+                                 void *out, int *levels_out, const int *n_dev, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * NMS (IoU with the legacy +1 box area, suppress when IoU > thresh).
@@ -141,7 +143,10 @@ int upsnet_conv2d_forward(const float *x, const float *weight, const float *bias
  *     [Cout_pad][kh*kw][Cin]); `packed` must hold upsnet_igemm_packed_weight_bytes bytes,
  *   - offset [N,2*kh*kw,Ho,Wo] / mask [N,kh*kw,Ho,Wo] stay NCHW (reference layout), NULL for a
  *     dense convolution; deformable_groups must be 1,
- *   - precision is UPSNET_PREC_BF16X3 (fp32-grade result) or UPSNET_PREC_BF16.
+ *   - precision is UPSNET_PREC_BF16X3 (fp32-grade result) or UPSNET_PREC_BF16,
+ *   - n_dev (optional, may be NULL): int32 device count of the images to compute.  On the TMA-fed dense path the tiles
+ *     whose first image is >= *n_dev are skipped (a tile holding images on both sides runs in full) and every computed
+ *     output is bit-identical to the unbounded launch; the other paths compute all N images.
  * replaces: the same reference call sites as upsnet_conv2d_forward / upsnet_dcn_forward.
  */
 int upsnet_igemm_packed_weight_bytes(int Cout, int Cin, int kh, int kw, size_t *bytes);
@@ -151,7 +156,7 @@ int upsnet_igemm_forward(const void *x_nhwc, const float *offset, const float *m
                          const void *packed, const float *bias, const void *residual, void *y,
                          int N, int H, int W, int Cin, int Cout, int kh, int kw, int stride_h,
                          int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int out_layout,
-                         int x_dtype, int y_dtype, int epi_flags, int precision, void *stream);
+                         int x_dtype, int y_dtype, int epi_flags, int precision, const int *n_dev, void *stream);
 /* Tuning hook of the TMA-fed dense path of upsnet_igemm_forward (csrc/igemm_tma.cu): output-channel tile of the following
  * launches in this process.  0 (default) = chosen per launch (the widest tile that still gives ~2/3 of the SMs a tile and,
  * for pair activations, a ring of at least three stages); 64 or 128 = that tile wherever Cout rounded up is a multiple of it.
@@ -312,6 +317,16 @@ int upsnet_maskroi_prepare(const float *rois, const unsigned char *roi_valid, co
 int upsnet_maskroi_finish(const int *keep, const int *keep_cnt, const int *seg_offsets, const float *sc,
                           const int *cls, const float *bx, int nseg, int max_seg_len, int top_n, int cap,
                           float *out_sc, float *out_bx, long long *out_cls, int *n_out, void *stream);
+
+/* upsnet_mask_rows: the rows the mask branch has to compute for one image, from the two MaskROI outputs (b1 [cap1,5], device
+ * count n1: detections; b2 [cap2,5], device count n2: panoptic candidates).  A row's logits depend on its box alone, so a
+ * candidate whose box (all five floats, compared bit for bit) equals a detection's box takes that detection's row.
+ * rows [cap1+cap2,5]: the n1 detections in order, then the candidates that match no detection in order, then zeros;
+ * u int32 device scalar: the number of rows written before the zeros; pan_row int32 [cap2]: the row of candidate j's logits
+ * (0 for j >= n2).  Counts are clamped to [0, cap].  One CTA, deterministic, no host read (graph-capturable).
+ * replaces: models/resnet_upsnet.py:203-222 running the mask branch once on the detections and once on the candidates. */
+int upsnet_mask_rows(const float *b1, const int *n1, int cap1, const float *b2, const int *n2, int cap2, float *rows,
+                     int *u, int *pan_row, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * Callers either side of the per-image forward (SURVEY section 8f), device resident.

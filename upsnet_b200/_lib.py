@@ -44,7 +44,7 @@ def lib():
         L.upsnet_version.argtypes = [C.POINTER(i)]
         L.upsnet_roi_align_forward.argtypes = [vp, i, i, i, i, i, i, vp, i, i, i, i, f, vp, vp]
         L.upsnet_roi_align_fpn_forward.argtypes = [C.POINTER(vp), C.POINTER(i), C.POINTER(i), C.POINTER(f),
-                                                   i, i, i, i, vp, i, i, i, i, vp, vp, vp]
+                                                   i, i, i, i, vp, i, i, i, i, vp, vp, vp, vp]
         L.upsnet_nms_workspace_bytes.argtypes = [i, i, C.POINTER(sz)]
         L.upsnet_nms_segmented.argtypes = [vp, vp, i, i, f, vp, vp, vp, sz, vp]
         L.upsnet_nms_host.argtypes = [vp, vp, vp, i, i, f, i]
@@ -52,7 +52,7 @@ def lib():
         L.upsnet_conv2d_forward.argtypes = [vp] * 5 + [i] * 15 + [vp]
         L.upsnet_igemm_packed_weight_bytes.argtypes = [i, i, i, i, C.POINTER(sz)]
         L.upsnet_igemm_pack_weight.argtypes = [vp, i, i, i, i, vp, vp]
-        L.upsnet_igemm_forward.argtypes = [vp] * 7 + [i] * 18 + [vp]
+        L.upsnet_igemm_forward.argtypes = [vp] * 7 + [i] * 18 + [vp, vp]
         L.upsnet_dcn_packed_weight_bytes.argtypes = [i, i, i, i, C.POINTER(sz)]
         L.upsnet_dcn_pack_weight.argtypes = [vp, i, i, i, i, vp, vp]
         L.upsnet_dcn_pair_forward.argtypes = [vp] * 6 + [i] * 12 + [vp]
@@ -67,6 +67,7 @@ def lib():
                                         C.POINTER(i), vp, i, i, f, f, vp, vp]
         L.upsnet_maskroi_prepare.argtypes = [vp, vp, vp, vp, i, i, i, f, C.POINTER(f), f, f, vp, vp, vp, vp, vp]
         L.upsnet_maskroi_finish.argtypes = [vp] * 6 + [i] * 4 + [vp] * 5
+        L.upsnet_mask_rows.argtypes = [vp, vp, i, vp, vp, i, vp, vp, vp, vp]
         L.upsnet_maxpool2d_nhwc.argtypes = [vp, vp] + [i] * 8 + [vp]
         L.upsnet_upsample_bilinear_nchw.argtypes = [vp, vp, i, i, i, i, vp]
         L.upsnet_rpn_topk_workspace_bytes.argtypes = [i, C.POINTER(sz)]
@@ -106,7 +107,7 @@ EXPORTED_SYMBOLS = [
     "upsnet_nms_workspace_bytes", "upsnet_nms_segmented", "upsnet_nms_host", "upsnet_dcn_forward",
     "upsnet_conv2d_forward", "upsnet_igemm_packed_weight_bytes", "upsnet_igemm_pack_weight",
     "upsnet_igemm_forward", "upsnet_panoptic_workspace_bytes", "upsnet_panoptic_workspace_min_bytes", "upsnet_panoptic_head", "upsnet_panoptic_head_up4", "upsnet_mask_removal",
-    "upsnet_rpn_decode", "upsnet_maskroi_prepare", "upsnet_maskroi_finish", "upsnet_maxpool2d_nhwc", "upsnet_upsample_bilinear_nchw", "upsnet_rpn_topk_workspace_bytes", "upsnet_rpn_topk", "upsnet_rpn_collect", "upsnet_stem_workspace_bytes",
+    "upsnet_rpn_decode", "upsnet_maskroi_prepare", "upsnet_maskroi_finish", "upsnet_mask_rows", "upsnet_maxpool2d_nhwc", "upsnet_upsample_bilinear_nchw", "upsnet_rpn_topk_workspace_bytes", "upsnet_rpn_topk", "upsnet_rpn_collect", "upsnet_stem_workspace_bytes",
     "upsnet_stem_packed_weight_bytes", "upsnet_stem_pack_weight", "upsnet_stem_forward",
     "upsnet_dcn_im2col", "upsnet_dcn_col2im", "upsnet_dcn_col2im_coord", "upsnet_roi_align_backward",
     "upsnet_dcn_packed_weight_bytes", "upsnet_dcn_pack_weight", "upsnet_dcn_pair_forward", "upsnet_dcn_set_tile_n", "upsnet_tma_set_tile_n",

@@ -93,7 +93,7 @@ extern "C" int upsnet_igemm_forward(const void* x_nhwc, const float* offset, con
                                     void* y, int N, int H, int W, int Cin, int Cout, int kh, int kw,
                                     int stride_h, int stride_w, int pad_h, int pad_w, int dil_h,
                                     int dil_w, int out_layout, int x_dtype, int y_dtype, int epi_flags,
-                                    int precision, void* stream) {
+                                    int precision, const int* n_dev, void* stream) {
   if (!x_nhwc || !packed || !y) return UPSNET_E_BADARG;
   if (N <= 0 || Cin <= 0 || H <= 0 || W <= 0 || Cout <= 0 || kh <= 0 || kw <= 0 || stride_h <= 0 ||
       stride_w <= 0 || pad_h < 0 || pad_w < 0 || dil_h <= 0 || dil_w <= 0)
@@ -104,6 +104,7 @@ extern "C" int upsnet_igemm_forward(const void* x_nhwc, const float* offset, con
   if ((size_t)H * W >= (1ull << 31)) return UPSNET_E_UNSUPPORTED;
   ups::TcParams p{};
   p.x = x_nhwc; p.offset = offset; p.mask = mask; p.bias = bias; p.residual = residual; p.y = y;
+  p.n_dev = n_dev;
   p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.kh = kh; p.kw = kw; p.sh = stride_h;
   p.sw = stride_w; p.ph = pad_h; p.pw = pad_w; p.dh = dil_h; p.dw = dil_w;
   p.Ho = ups::conv_out_size(H, pad_h, dil_h, kh, stride_h);

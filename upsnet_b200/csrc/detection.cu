@@ -708,3 +708,70 @@ extern "C" int upsnet_rpn_collect(const int* keep, const int* keep_cnt, const in
   UPS_CHECK_LAUNCH();
   return 0;
 }
+
+// ----------------------------------------------------------------------------------------------
+// Mask-branch row plan.  The branch maps a box (batch index + 4 coordinates) to its logits with no dependence on the
+// other rows, so the panoptic candidates whose box is bit-identical to a detection's box reuse that detection's row:
+//   rows [0, n1)  = the detections, in order;  rows [n1, u) = the candidates that match no detection, in order;
+//   pan_row[j]    = the row candidate j's logits come from (0 for j >= n2);  rows [u, cap1 + cap2) are zeroed.
+// One CTA, candidates in chunks of the block: ballot + per-warp counts keep the candidate order (deterministic).
+// ----------------------------------------------------------------------------------------------
+namespace ups {
+
+constexpr int kRowThreads = 128;
+
+__global__ void __launch_bounds__(kRowThreads)
+mask_rows_kernel(const float* __restrict__ b1, const int* __restrict__ n1p, int cap1, const float* __restrict__ b2,
+                 const int* __restrict__ n2p, int cap2, float* __restrict__ rows, int* __restrict__ u_out,
+                 int* __restrict__ pan_row) {
+  __shared__ int s_cnt[kRowThreads / 32];
+  const int n1 = min(max(*n1p, 0), cap1), n2 = min(max(*n2p, 0), cap2);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t* d = reinterpret_cast<const uint32_t*>(b1);
+  for (int k = tid; k < n1 * 5; k += kRowThreads) rows[k] = b1[k];
+  int base = n1;
+  for (int j0 = 0; j0 < cap2; j0 += kRowThreads) {
+    const int j = j0 + tid;
+    int src = 0;
+    bool fresh = false;
+    if (j < n2) {
+      const uint32_t* c = reinterpret_cast<const uint32_t*>(b2) + (size_t)j * 5;
+      const uint32_t c0 = c[0], c1 = c[1], c2 = c[2], c3 = c[3], c4 = c[4];
+      src = -1;
+      for (int i = 0; i < n1; ++i) {
+        const uint32_t* e = d + (size_t)i * 5;
+        if (e[0] == c0 && e[1] == c1 && e[2] == c2 && e[3] == c3 && e[4] == c4) { src = i; break; }
+      }
+      fresh = src < 0;
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, fresh);
+    if (lane == 0) s_cnt[warp] = __popc(bal);
+    __syncthreads();
+    int off = base, tot = 0;
+#pragma unroll
+    for (int w = 0; w < kRowThreads / 32; ++w) {
+      if (w < warp) off += s_cnt[w];
+      tot += s_cnt[w];
+    }
+    if (fresh) {
+      src = off + __popc(bal & ((1u << lane) - 1u));
+      for (int k = 0; k < 5; ++k) rows[(size_t)src * 5 + k] = b2[(size_t)j * 5 + k];
+    }
+    if (j < cap2) pan_row[j] = src;
+    base += tot;
+    __syncthreads();      // s_cnt is rewritten by the next chunk
+  }
+  for (int k = base * 5 + tid; k < (cap1 + cap2) * 5; k += kRowThreads) rows[k] = 0.f;
+  if (tid == 0) *u_out = base;
+}
+
+}  // namespace ups
+
+extern "C" int upsnet_mask_rows(const float* b1, const int* n1, int cap1, const float* b2, const int* n2, int cap2,
+                                float* rows, int* u, int* pan_row, void* stream) {
+  if (!b1 || !n1 || !b2 || !n2 || !rows || !u || !pan_row || cap1 <= 0 || cap2 <= 0) return UPSNET_E_BADARG;
+  if ((long long)cap1 + cap2 > (1 << 20)) return UPSNET_E_UNSUPPORTED;
+  ups::mask_rows_kernel<<<1, ups::kRowThreads, 0, (cudaStream_t)stream>>>(b1, n1, cap1, b2, n2, cap2, rows, u, pan_row);
+  UPS_CHECK_LAUNCH();
+  return 0;
+}

@@ -42,6 +42,10 @@ struct TmaGeom {
   int kw, KHW, ph, pw, dh, dw;
   int bw, bh, bn;                       // M-tile box: pixels along W, along H, images (bw*bh*bn <= 128)
   int tiles_w, tiles_h, tiles_n, n_tiles;
+  // optional device-side image count (<= N): tiles whose first image is >= *n_dev are skipped (the grid stays the static
+  // maximum, so a captured graph keeps its shape).  Read by every role at kernel start: the TMA producer, the residual warp
+  // and the consumers must walk the same tile sequence or the mbarrier rings would never drain.
+  const int* n_dev;
   int BN, stages, relu, has_res;
   int res_up2;                          // residual = half-resolution map, nearest 2x up-sampling (FPN top-down)
   // direct-store epilogue (small / odd Cout, fp32 or NCHW outputs: offset convs, RPN / score / mask-logit heads)
@@ -149,7 +153,9 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cchunks = g.Cin / 64;
   const int num_kb = g.KHW * cchunks;
-  const long long m_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_n;
+  // images are the slowest tile coordinate, so the tiles of images < n are a prefix of the tile sequence
+  const int tiles_n = g.n_dev ? (min(max(*g.n_dev, 0), g.N) + g.bn - 1) / g.bn : g.tiles_n;
+  const long long m_tiles = (long long)g.tiles_w * g.tiles_h * tiles_n;
   const long long num_tiles = m_tiles * g.n_tiles;
   const uint32_t box_bytes = (uint32_t)(g.bw * g.bh * g.bn) * 128u;
 
@@ -611,6 +617,7 @@ int launch_igemm_tma(const TcParams& p, const void* packed, cudaStream_t stream)
   g.N = p.N; g.Ho = p.Ho; g.Wo = p.Wo; g.Cout = p.Cout; g.Cin = p.Cin;
   g.kw = p.kw; g.KHW = p.kh * p.kw; g.ph = p.ph; g.pw = p.pw; g.dh = p.dh; g.dw = p.dw;
   g.relu = p.relu; g.has_res = p.residual ? 1 : 0; g.res_up2 = p.res_up2 ? 1 : 0; g.sig_from = p.sig_from;
+  g.n_dev = p.n_dev;
   tma_pick_box(p.N, p.Ho, p.Wo, p.kh, p.kw, p.dh, p.dw, g.res_up2 != 0, &g.bw, &g.bh, &g.bn);
   g.tiles_w = (p.Wo + g.bw - 1) / g.bw;
   g.tiles_h = (p.Ho + g.bh - 1) / g.bh;

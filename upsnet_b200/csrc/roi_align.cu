@@ -284,10 +284,11 @@ roi_align_nhwc_bf16_roi_kernel(FpnFeats f, int C, const float* __restrict__ rois
 __global__ void __launch_bounds__(256)
 roi_align_nhwc_pair_roi_kernel(FpnFeats f, int C, const float* __restrict__ rois, int R, int PH, int PW, int sr,
                                __nv_bfloat16* __restrict__ out, long long roi_stride, int pix_stride, long long lo_off,
-                               int* __restrict__ levels_out) {
+                               int* __restrict__ levels_out, const int* __restrict__ n_dev) {
   __shared__ int4 s_off[kRoiMaxSamples];
   __shared__ float4 s_w[kRoiMaxSamples];
   const int n = blockIdx.x;
+  if (n_dev && n >= *n_dev) return;     // rois beyond the device-side count: neither read nor written
   const float* r = rois + (size_t)n * 5;
   const int b = (int)roundf(r[0]);
   const float rx1 = r[1], ry1 = r[2], rx2 = r[3], ry2 = r[4];
@@ -358,10 +359,11 @@ roi_align_nhwc_pair_roi_kernel(FpnFeats f, int C, const float* __restrict__ rois
 }
 
 static int launch_roi_align(const FpnFeats& f, int B, int C, int layout, int dtype, const float* rois, int R,
-                            int PH, int PW, int sr, void* out_v, int* levels_out,
+                            int PH, int PW, int sr, void* out_v, int* levels_out, const int* n_dev,
                             cudaStream_t stream) {
   if (R < 0 || C <= 0 || PH <= 0 || PW <= 0 || B <= 0) return UPSNET_E_BADARG;
   if (R == 0) return 0;
+  if (n_dev && dtype != UPSNET_DTYPE_PAIR) return UPSNET_E_UNSUPPORTED;
   if (dtype == UPSNET_DTYPE_PAIR) {
     if (layout != UPSNET_LAYOUT_NHWC && layout != UPSNET_LAYOUT_FLAT_PAIR) return UPSNET_E_UNSUPPORTED;
     if (sr <= 0 || (C & 7) || (long long)PH * PW * sr * sr > kRoiMaxSamples || (((uintptr_t)out_v) & 15)) return UPSNET_E_UNSUPPORTED;
@@ -370,7 +372,7 @@ static int launch_roi_align(const FpnFeats& f, int B, int C, int layout, int dty
     const long long plane = (long long)PH * PW * C;
     const bool flat = layout == UPSNET_LAYOUT_FLAT_PAIR;
     roi_align_nhwc_pair_roi_kernel<<<R, 256, 0, stream>>>(f, C, rois, R, PH, PW, sr, (__nv_bfloat16*)out_v, 2 * plane,
-                                                          flat ? C : 2 * C, flat ? plane : (long long)C, levels_out);
+                                                          flat ? C : 2 * C, flat ? plane : (long long)C, levels_out, n_dev);
     UPS_CHECK_LAUNCH();
     return 0;
   }
@@ -427,7 +429,7 @@ extern "C" int upsnet_roi_align_forward(const void* feat, int B, int C, int H, i
   if (!feat || !out || (!rois && R > 0)) return UPSNET_E_BADARG;
   ups::FpnFeats f{};
   f.p[0] = feat; f.H[0] = H; f.W[0] = W; f.scale[0] = spatial_scale; f.nlevels = 1;
-  return ups::launch_roi_align(f, B, C, layout, dtype, rois, R, PH, PW, sampling_ratio, out, nullptr,
+  return ups::launch_roi_align(f, B, C, layout, dtype, rois, R, PH, PW, sampling_ratio, out, nullptr, nullptr,
                                (cudaStream_t)stream);
 }
 
@@ -435,7 +437,7 @@ extern "C" int upsnet_roi_align_fpn_forward(const void* const feats[4], const in
                                             const int Ws[4], const float scales[4], int B, int C,
                                             int layout, int dtype, const float* rois, int R, int PH, int PW,
                                             int sampling_ratio, void* out, int* levels_out,
-                                            void* stream) {
+                                            const int* n_dev, void* stream) {
   if (!feats || !Hs || !Ws || !scales || !out || (!rois && R > 0)) return UPSNET_E_BADARG;
   ups::FpnFeats f{};
   for (int l = 0; l < 4; ++l) {
@@ -443,6 +445,6 @@ extern "C" int upsnet_roi_align_fpn_forward(const void* const feats[4], const in
     f.p[l] = feats[l]; f.H[l] = Hs[l]; f.W[l] = Ws[l]; f.scale[l] = scales[l];
   }
   f.nlevels = 4;
-  return ups::launch_roi_align(f, B, C, layout, dtype, rois, R, PH, PW, sampling_ratio, out, levels_out,
+  return ups::launch_roi_align(f, B, C, layout, dtype, rois, R, PH, PW, sampling_ratio, out, levels_out, n_dev,
                                (cudaStream_t)stream);
 }

@@ -47,6 +47,7 @@ struct TcParams {
   int res_up2;           // residual is a half-resolution NHWC map read with nearest-neighbour 2x upsampling
   int no_tma;            // UPSNET_EPI_NO_TMA: force the cp.async gather kernel (A/B comparisons, tests)
   int tile_w, tile_h;    // deformable mode: pixel block of an M-tile (16x8 = all 128 rows; 8x8 / 8x4 leave rows unused)
+  const int* n_dev;      // optional device-side image count (<= N): the TMA kernel skips the tiles of images >= *n_dev
 };
 
 size_t tc_packed_weight_bytes(int Cout, int Cin, int kh, int kw);

@@ -353,23 +353,31 @@ class MaskBranch(nn.Module):
         b1 = self.mask_deconv1[0].bias.repeat(4).detach().contiguous()
         self._f = (w1, b1, cout)
 
-    def forward(self, feat, rois):
-        x = self.roi_pooling(feat, rois)
+    def forward(self, feat, rois, n_dev=None):
+        """n_dev (static engine): int32 device count of the rois that are needed -- the pair-stream ROIAlign and the
+        tensor-core convs skip the rest, whose logits are then unspecified."""
+        bound = {} if n_dev is None else {"n_dev": n_dev}     # (the CPU stand-ins of the ops take no count)
+        if n_dev is None or not isinstance(feat[0], ops.Pair):
+            x = self.roi_pooling(feat, rois)
+        else:
+            r = self.roi_pooling
+            x = ops.fpn_roi_align(list(feat), rois, r.pooled_height, r.pooled_width, r.spatial_scale, layout="auto", **bound)
         for i in range(1, 5):
             c = getattr(self, "mask_conv%d" % i)[0]
-            x = ops.conv2d(x, c.weight, c.bias, padding=1, relu=True)
+            x = ops.conv2d(x, c.weight, c.bias, padding=1, relu=True, **bound)
         w1, b1, cout = self._f
         if isinstance(x, ops.Pair):
             # pair stream: the deconv-as-1x1 conv writes its four (a, b) groups as [hi Cout][lo Cout] each, i.e. directly
             # as the Pair of 4w 'pixels' per row that mask_score (1x1) then scores -- same commutation as below
-            yv = ops.conv2d(x, w1, b1, relu=True, pair_group=cout)                                # Pair [n, Cout, h, 4w]
+            yv = ops.conv2d(x, w1, b1, relu=True, pair_group=cout, **bound)                     # Pair [n, Cout, h, 4w]
             n, _, h, w4 = yv.shape
             w = w4 // 4
-            z = ops.conv2d(yv, self.mask_score.weight, self.mask_score.bias, out_format="nhwc", out_dtype=torch.float32)
+            z = ops.conv2d(yv, self.mask_score.weight, self.mask_score.bias, out_format="nhwc", out_dtype=torch.float32,
+                           **bound)
             K = z.shape[1]
             z = z.permute(0, 2, 3, 1).reshape(n, h, w, 2, 2, K)
             return z.permute(0, 5, 1, 3, 2, 4).reshape(n, K, 2 * h, 2 * w)
-        y = ops.conv2d(x, w1, b1, relu=True)                 # [n, 4*Cout, h, w], channels ordered (a, b, co)
+        y = ops.conv2d(x, w1, b1, relu=True, **bound)        # [n, 4*Cout, h, w], channels ordered (a, b, co)
         n, _, h, w = y.shape
         if y.is_contiguous(memory_format=torch.channels_last) and y.dim() == 4:
             # The pixel shuffle only permutes pixels and mask_score is a 1x1 conv, so they commute: score the four
@@ -378,12 +386,12 @@ class MaskBranch(nn.Module):
             # 256-channel feature map (two 50 MB permute copies per call in the first version).
             yv = y.permute(0, 2, 3, 1).reshape(n, h, w * 4, cout).permute(0, 3, 1, 2)
             z = ops.conv2d(yv, self.mask_score.weight, self.mask_score.bias, out_format="nhwc",
-                           out_dtype=torch.float32)                                               # [n, K, h, 4w]
+                           out_dtype=torch.float32, **bound)                                      # [n, K, h, 4w]
             K = z.shape[1]
             z = z.permute(0, 2, 3, 1).reshape(n, h, w, 2, 2, K)                                    # (i, j, a, b, k)
             return z.permute(0, 5, 1, 3, 2, 4).reshape(n, K, 2 * h, 2 * w)
         y = y.reshape(n, 2, 2, cout, h, w).permute(0, 3, 4, 1, 5, 2).reshape(n, cout, 2 * h, 2 * w)
-        return ops.conv2d(y, self.mask_score.weight, self.mask_score.bias, out_format="nchw")
+        return ops.conv2d(y, self.mask_score.weight, self.mask_score.bias, out_format="nchw", **bound)
 
 
 class FCNSubNet(nn.Module):
@@ -534,6 +542,7 @@ class resnet_upsnet(nn.Module):
         self.static_engine = True     # fixed shapes + device-side counts: no host sync inside the forward
         self.use_cuda_graph = True    # capture the static forward once per (shape, precision) and replay it
         self.overlap_heads = True     # semantic head on a side stream, concurrent with the detection chain
+        self.dedup_mask_rows = True   # mask branch on the distinct boxes only (ops.mask_rows), not on both padded buffers
         self._side = {}
         self._graphs = {}
         self.max_graphs = 6           # captured graphs kept (LRU): one activation pool each (~2 GB at 1024x2048)
@@ -686,10 +695,20 @@ class resnet_upsnet(nn.Module):
             s2, b2, c2, n2 = self.mask_roi_panoptic_static(rois, roi_valid, bbox_pred, cls_prob, im_info)
         # models/resnet_upsnet.py:203-222 runs the mask branch twice (detections, panoptic candidates).  Every roi is
         # processed independently, so both sets go through it as ONE batch: half the launches, fuller tile waves.
-        logits = self.mask_branch(feats, torch.cat([b1, b2], 0)).float()
-        mask_prob = torch.sigmoid(logits[:b1.shape[0]])
+        # A roi's logits depend on its box alone, and a candidate that also survives as a detection has the detection's
+        # box bit for bit (same maskroi_prepare decode), so the batch is the u distinct live boxes: the detections, then
+        # the candidates that match none (ops.mask_rows).  The branch skips rows >= u, so mask_probs rows >= n1 are
+        # unspecified.
         ms = self.cfg.mask_size
-        mask_score = logits[b1.shape[0]:].gather(1, c2.view(-1, 1, 1, 1).expand(-1, -1, ms, ms))
+        if self.dedup_mask_rows and x.is_cuda:
+            rows, u, pan_row = ops.mask_rows(b1, n1, b2, n2)
+            logits = self.mask_branch(feats, rows, n_dev=u).float()
+            K = logits.shape[1]
+            mask_score = logits.view(-1, ms, ms).index_select(0, pan_row.long() * K + c2).view(-1, 1, ms, ms)
+        else:
+            logits = self.mask_branch(feats, torch.cat([b1, b2], 0)).float()
+            mask_score = logits[b1.shape[0]:].gather(1, c2.view(-1, 1, 1, 1).expand(-1, -1, ms, ms))
+        mask_prob = torch.sigmoid(logits[:b1.shape[0]])
         if fork:
             cur.wait_event(done)
         # fused x4 up-sampling: the fusion kernel reads the quarter-resolution score map (fcn_output, when the parity tests ask
@@ -745,7 +764,7 @@ class resnet_upsnet(nn.Module):
         if not (self.use_cuda_graph and x.is_cuda):
             return self._forward_static(x, im_info), None
         key = (tuple(x.shape), str(x.device), ops._PRECISION["conv"], bool(getattr(self, "keep_intermediates", False)),
-               tuple(float(v) for v in im_info), lane)
+               bool(self.dedup_mask_rows), tuple(float(v) for v in im_info), lane)
         ent = self._graphs.get(key)
         if ent is None:
             static_x = torch.empty(x.shape, dtype=torch.float32, device=x.device)

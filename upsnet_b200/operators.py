@@ -289,14 +289,22 @@ def _tc_ok(Cin, kh, kw, dg, deform=False):
     return (Cin % 64 == 0 or (Cin <= 8 and not deform)) and dg == 1 and kh * kw <= 49
 
 
+def _count(n_dev):
+    """A device-side count argument: None, or an int32 CUDA scalar (read by the kernels, never by the host)."""
+    if n_dev is not None:
+        assert n_dev.dtype == torch.int32 and n_dev.is_cuda and n_dev.numel() == 1
+    return n_dev
+
+
 def _igemm_tc(kind, x, offset, mask, weight, bias, residual, stride, padding, dilation, relu, prec, out_format,
-              out_dtype=None, residual_up2=False, pair_group=0, sigmoid_from=None):
+              out_dtype=None, residual_up2=False, pair_group=0, sigmoid_from=None, n_dev=None):
     """upsnet_igemm_forward: x logical NCHW (any memory format; fp32 or bf16) or a Pair; result logical NCHW whose
     storage is NHWC (channels_last view, the engine layout) unless out_format == 'nchw'.
     Output: bf16 / a Pair when the engine's activation stream (_stream()) is bf16 / pairs and the
     result stays in that NHWC stream; fp32 for plane-wise (NCHW) head outputs or when asked via out_dtype.
     pair_group=G (Pair output only): channels are written as [hi G][lo G] groups and the result is returned as the Pair
-    of logical shape [N, G, Ho, Wo*Cout/G] that this storage also is (see MaskBranch)."""
+    of logical shape [N, G, Ho, Wo*Cout/G] that this storage also is (see MaskBranch).
+    n_dev: optional int32 device scalar; images >= n_dev are not computed by the TMA-fed path (their output is unspecified)."""
     sh, sw = stride; ph, pw = padding; dh, dw = dilation
     N, Cin, H, W = x.shape
     Cout, _, kh, kw = weight.shape
@@ -364,7 +372,7 @@ def _igemm_tc(kind, x, offset, mask, weight, bias, residual, stride, padding, di
         check(lib().upsnet_igemm_forward(ptr(xs), ptr(offset), ptr(mask), ptr(packed), ptr(bias), ptr(res),
                                          ptr(store), N, H, W, Cin, Cout, kh, kw, sh, sw, ph, pw, dh, dw,
                                          _lib.LAYOUT_NHWC if nhwc_out else _lib.LAYOUT_NCHW, x_dt, y_dt, flags,
-                                         prec, stream_ptr(dev)), kind)
+                                         prec, ptr(_count(n_dev)), stream_ptr(dev)), kind)
     if pair_out:
         if pair_group:
             return Pair(store.view(N, Ho, Wo * (Cout // pair_group), 2 * pair_group))
@@ -376,9 +384,10 @@ def _igemm_tc(kind, x, offset, mask, weight, bias, residual, stride, padding, di
 # functional layer
 # ------------------------------------------------------------------------------------------------
 def conv2d(x, weight, bias=None, stride=1, padding=0, dilation=1, residual=None, relu=False, precision=None,
-           out_format=None, out_dtype=None, residual_up2=False, pair_group=0, sigmoid_from=None):
+           out_format=None, out_dtype=None, residual_up2=False, pair_group=0, sigmoid_from=None, n_dev=None):
     """Dense conv + fused bias / residual / ReLU epilogue.  fp32 precision -> upsnet_conv2d_forward
-    (NCHW CUDA-core tiles); bf16x3 / bf16 -> upsnet_igemm_forward (wgmma tiles, NHWC storage)."""
+    (NCHW CUDA-core tiles); bf16x3 / bf16 -> upsnet_igemm_forward (wgmma tiles, NHWC storage).
+    n_dev: optional int32 device scalar -- only images < n_dev are needed; the output of the others is unspecified."""
     require_cuda(x, weight, bias, residual)
     prec = _PRECISION["conv"] if precision is None else precision
     if prec != _lib.PREC_FP32_SIMT and _tc_ok(weight.shape[1], weight.shape[2], weight.shape[3], 1):
@@ -386,7 +395,7 @@ def conv2d(x, weight, bias=None, stride=1, padding=0, dilation=1, residual=None,
             residual, residual_up2 = torch.nn.functional.interpolate(as_float(residual), scale_factor=2, mode="nearest"), False
         return _igemm_tc("conv2d", x, None, None, weight, None if bias is None else f32c(bias), residual,
                          _pair(stride), _pair(padding), _pair(dilation), relu, prec, out_format, out_dtype,
-                         residual_up2, pair_group, sigmoid_from)
+                         residual_up2, pair_group, sigmoid_from, n_dev)
     if sigmoid_from is not None:      # CUDA-core path: the conv entry has no sigmoid epilogue
         y = conv2d(x, weight, bias, stride, padding, dilation, residual, relu, precision, out_format, out_dtype, residual_up2)
         y[:, sigmoid_from:] = torch.sigmoid(y[:, sigmoid_from:])
@@ -556,8 +565,9 @@ def fcn_score_fuse(s2, s3, s4, s5):
 
 
 def fpn_roi_align(feats, rois, pooled_height, pooled_width, spatial_scales, sampling_ratio=2, layout="nchw",
-                  return_levels=False):
-    """FPNRoIAlign.forward in one launch (level assignment on device, output already in roi order)."""
+                  return_levels=False, n_dev=None):
+    """FPNRoIAlign.forward in one launch (level assignment on device, output already in roi order).
+    n_dev: optional int32 device scalar (pair features only) -- rois >= n_dev are skipped, their output is unspecified."""
     assert len(feats) == 4 and len(spatial_scales) == 4
     require_cuda(rois, *feats)
     rois = f32c(rois)
@@ -579,7 +589,8 @@ def fpn_roi_align(feats, rois, pooled_height, pooled_width, spatial_scales, samp
             with torch.cuda.device(rois.device), _Timed("roi_align_fpn", 1, {"bytes": 2.0 * out.numel()}, rois.device):
                 check(lib().upsnet_roi_align_fpn_forward(fp, hs, ws, sc, B, Cc, _lib.LAYOUT_FLAT_PAIR if flat else _lib.LAYOUT_NHWC,
                                                          _lib.DTYPE_PAIR, ptr(rois), R, pooled_height, pooled_width,
-                                                         sampling_ratio, ptr(out), ptr(None), stream_ptr(rois.device)),
+                                                         sampling_ratio, ptr(out), ptr(None), ptr(_count(n_dev)),
+                                                         stream_ptr(rois.device)),
                       "fpn_roi_align")
         return Pair(out)
     if layout == "auto":
@@ -604,13 +615,14 @@ def fpn_roi_align(feats, rois, pooled_height, pooled_width, spatial_scales, samp
         Hs = [f.shape[1] for f in feats]; Ws = [f.shape[2] for f in feats]
         out = torch.empty((R, pooled_height, pooled_width, Cc), device=rois.device, dtype=odt)
         lay = _lib.LAYOUT_NHWC
+    assert n_dev is None, "fpn_roi_align: the roi count bound is implemented for pair features"
     levels = torch.empty((R,), device=rois.device, dtype=torch.int32) if return_levels else None
     fp = (C.c_void_p * 4)(*[f.data_ptr() for f in feats])
     hs = (C.c_int * 4)(*Hs); ws = (C.c_int * 4)(*Ws)
     sc = (C.c_float * 4)(*[float(s) for s in spatial_scales])
     with torch.cuda.device(rois.device), _Timed("roi_align_fpn", 1, {"bytes": 4.0 * out.numel()}, rois.device):
         check(lib().upsnet_roi_align_fpn_forward(fp, hs, ws, sc, B, Cc, lay, 1 if bf16 else 0, ptr(rois), R, pooled_height,
-                                                 pooled_width, sampling_ratio, ptr(out), ptr(levels),
+                                                 pooled_width, sampling_ratio, ptr(out), ptr(levels), ptr(None),
                                                  stream_ptr(rois.device)), "fpn_roi_align")
     return (out, levels) if return_levels else out
 
@@ -788,6 +800,24 @@ def maskroi_finish(keep, cnt, offs, sc, cls, bx, top_n, cap):
                                           int(cap), ptr(out_sc), ptr(out_bx), ptr(out_cls), ptr(n_out), stream_ptr(dev)),
               "maskroi_finish")
     return out_sc, out_bx, out_cls, n_out[0], n_out[1]
+
+
+def mask_rows(b1, n1, b2, n2):
+    """Rows of the mask branch for one image (upsnet_mask_rows): b1 [cap1,5] / n1 detections, b2 [cap2,5] / n2 panoptic
+    candidates (counts: int32 device scalars) -> (rows [cap1+cap2,5], u int32 device scalar, pan_row int32 [cap2]).  rows
+    holds the detections, then the candidates whose box matches no detection bit for bit; candidate j's logits are row
+    pan_row[j] of the branch's output."""
+    require_cuda(b1, n1, b2, n2)
+    dev = b1.device
+    cap1, cap2 = b1.shape[0], b2.shape[0]
+    b1, b2 = f32c(b1), f32c(b2)
+    rows = torch.empty((cap1 + cap2, 5), dtype=torch.float32, device=dev)
+    u = torch.empty((), dtype=torch.int32, device=dev)
+    pan_row = torch.empty((cap2,), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev), _Timed("maskroi", 1, {"bytes": 40.0 * (cap1 + cap2)}, dev):
+        check(lib().upsnet_mask_rows(ptr(b1), ptr(_count(n1)), cap1, ptr(b2), ptr(_count(n2)), cap2, ptr(rows), ptr(u),
+                                     ptr(pan_row), stream_ptr(dev)), "mask_rows")
+    return rows, u, pan_row
 
 
 def nms(boxes, scores, thresh):
