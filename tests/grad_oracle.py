@@ -16,6 +16,8 @@ the device, and the error bounds the GPU backward tests measure against.
 The *_bounds functions give, per output element, the sum of the absolute values of the terms that make it up (fp64).
 A kernel that computes the same sums in fp32 is within a small multiple of fp32 epsilon of that bound; see `check`.
 The keyword arguments `right_guard` and `shift` build deliberately wrong variants for the sensitivity test.
+* dcn_columns / dcn_gemm: the arithmetic of the inference DCN kernels per precision mode (bf16x3 on fp32 or pair
+  activations, bf16), with planted faults; special_offsets(window=...) / window_origins: the window kernel's geometry.
 """
 import math
 
@@ -24,7 +26,10 @@ import torch
 
 # Largest observed |kernel - fp64| / bound on an H100 is a few times below these (tests/test_gpu_backward.py prints it).
 TOL = {"dcn_y": 8e-7, "dcn_dx": 8e-7, "dcn_doffset": 8e-7, "dcn_dmask": 6e-7, "dcn_dweight": 8e-7, "dcn_dbias": 2e-7,
-       "roi_y": 2e-6, "roi_dfeat": 2e-6}
+       "roi_y": 2e-6, "roi_dfeat": 2e-6,
+       # inference (tensor-core) DCN forward per precision mode: about 4x the worst ratio measured on an H100, far below
+       # the a-priori 2.1e-4, 1.35e-4 and 3.5e-5 derived in tests/test_gpu_forward_fp64.py
+       "dcn_x3_pair": 2e-5, "dcn_x3_f32": 1.2e-5, "dcn_bf16": 2.6e-6}
 ATOL = 1e-6
 
 
@@ -132,6 +137,108 @@ def deform_conv_bounds(x, offset, weight, bias, mask, dy, stride=1, padding=0, d
 
 
 # ------------------------------------------------------------------------------------------------
+# the arithmetic of the inference (tensor-core) DCN kernels, restated for the reference of the bf16 path and for the
+# sensitivity test of the forward tolerances
+# ------------------------------------------------------------------------------------------------
+def bf16_round(v, trunc=False):
+    """v (float64) rounded to bf16 (8 significant bits), ties to even, or towards zero (trunc); float64 result."""
+    m, e = torch.frexp(v)
+    m = m * 256
+    return torch.ldexp(torch.trunc(m) if trunc else torch.round(m), e - 8)
+
+
+def half_ulp_bf16(v):
+    """Half a bf16 ulp of |v| (0 where v == 0), float64."""
+    _, e = torch.frexp(v.abs())
+    return torch.where(v == 0, 0.0, torch.ldexp(torch.ones_like(v), e - 9))
+
+
+def split_bf16(v):
+    """(hi, lo) = (bf16(v), bf16(v - hi)) of fp32 values v, as float64."""
+    hi = bf16_round(v)
+    return hi, bf16_round(v - hi)
+
+
+def _fl32(v):
+    return v.float().double()
+
+
+def dcn_columns(x, offset, kh, kw, stride, padding, dilation, mask=None, mode="x3_f32", fault=None, window=None):
+    """The blended samples [N, C, K, Ho, Wo] (float64 tensors holding the kernel's values) as the tensor-core gathers
+    form them (csrc/igemm_tc.cu, csrc/dcn_win.cu).  Corner weights: the fp32 bilinear weight of each corner times the
+    mask, in fp32, 0 for corners outside the image.
+      'x3_f32'  fp32 activations x: fp32 FMA chain over the four corners, split into bf16 (hi, lo) -> (hi, lo)
+      'x3_pair' pair activations x = (hi, lo): hi plane in an fp32 FMA chain, lo plane in a bf16 FMA chain
+                (HMUL2 + 3 HFMA2) with bf16-rounded weights, the two added in fp32 and split -> (hi, lo)
+      'bf16'    bf16 activations x: the weights rounded to bf16, then a bf16 FMA chain -> s
+    Faults for the sensitivity test: 'right_guard', 'shift' (as in deform_conv), 'mask_hi_only' (x3: the lo plane of
+    x, or of the split sample, without the mask), 'truncate' (bf16: the chain truncates instead of rounding),
+    'window_edge' (window=(TW, TH): dcn_win.cu's in-window test one px too wide, reading the corner one past the window
+    as 0)."""
+    planes = x if mode == "x3_pair" else (x,)
+    C = planes[0].shape[1]
+    xs = torch.cat([p.float() for p in planes], 1)
+    corners, _, _ = _corners(xs, offset, kh, kw, stride, padding, dilation, None, 1 if fault == "right_guard" else 0,
+                             1 / 64 if fault == "shift" else 0.0)
+    wts = [wt for _, wt, _ in corners]
+    if fault == "window_edge":
+        N, Ho, Wo = offset.shape[0], offset.shape[2], offset.shape[3]
+        (sh, sw), (ph, pw), (dh, dw) = _pair(stride), _pair(padding), _pair(dilation)
+        K = kh * kw
+        base_h = (np.arange(Ho)[None, :, None] * sh - ph + (np.arange(K) // kw)[:, None, None] * dh) * np.ones((1, 1, Wo))
+        base_w = (np.arange(Wo)[None, None, :] * sw - pw + (np.arange(K) % kw)[:, None, None] * dw) * np.ones((1, Ho, 1))
+        o = offset.detach().float().double().cpu().numpy().reshape(N, K, 2, Ho, Wo)
+        ox, oy, hl, wl, valid = window_origins(base_h + o[:, :, 0], base_w + o[:, :, 1], xs.shape[2], xs.shape[3], window)
+        dx, dy = wl - ox, hl - oy
+        inside = (dx >= 0) & (dx + 1 < WIN_W) & (dy >= 0) & (dy + 1 < WIN_H)
+        wide = valid & ~inside & (dx >= 0) & (dx < WIN_W) & (dy >= 0) & (dy < WIN_H)      # the one-px-too-wide test
+        drop_r = torch.from_numpy(wide & (dx + 1 == WIN_W)).to(xs.device)
+        drop_b = torch.from_numpy(wide & (dy + 1 == WIN_H)).to(xs.device)
+        wts = [wts[0], wts[1] * ~drop_r, wts[2] * ~drop_b, wts[3] * ~(drop_r | drop_b)]
+    m32 = None if mask is None else mask.float()
+    wm = [w if m32 is None else w * m32 for w in wts]                    # fp32, as the kernels' sample tables
+    wm, wts = [w.double()[:, None] for w in wm], [w.double()[:, None] for w in wts]
+    vals = [v.double() for v, _, _ in corners]
+    if mode == "bf16":
+        s = None
+        for v, w in zip(vals, wm):
+            s = bf16_round(bf16_round(w) * v + (0 if s is None else s), trunc=fault == "truncate")
+        return s
+    if mode == "x3_f32":
+        w_hi = wts if fault == "mask_hi_only" else wm
+        s = None
+        for v, w in zip(vals, w_hi):
+            s = _fl32(w * v + (0 if s is None else s))
+        hi, lo = split_bf16(s)
+        return (hi * mask.double()[:, None], lo) if fault == "mask_hi_only" and mask is not None else (hi, lo)
+    assert mode == "x3_pair"
+    acc, lacc = None, None
+    for v, w, w_nm in zip(vals, wm, wts):
+        acc = _fl32(w * v[:, :C] + (0 if acc is None else acc))
+        lacc = bf16_round(bf16_round(w_nm if fault == "mask_hi_only" else w) * v[:, C:] + (0 if lacc is None else lacc))
+    return split_bf16(_fl32(acc + lacc))
+
+
+def dcn_gemm(col, weight, bias=None, mode="x3_f32", fault=None, dtype=torch.float32):
+    """y [N, Cout, Ho, Wo] from the columns of dcn_columns: bf16 x bf16 products (exact) summed in `dtype`.
+    x3: s_hi w_hi + s_lo w_hi + s_hi w_lo (fault 'drop_lohi': without s_lo w_hi); bf16: s w (weights bf16-exact)."""
+    Cout = weight.shape[0]
+    w2 = weight.double().reshape(Cout, -1)
+
+    def mm(a, b):
+        N, Ho, Wo = a.shape[0], a.shape[3], a.shape[4]
+        return torch.einsum("ok,nkp->nop", b.to(dtype), a.reshape(N, -1, Ho * Wo).to(dtype)).view(N, Cout, Ho, Wo)
+    if mode == "bf16":
+        y = mm(col, w2)
+    else:
+        (s_hi, s_lo), (w_hi, w_lo) = col, split_bf16(w2)
+        y = mm(s_hi, w_hi) + mm(s_hi, w_lo)
+        if fault != "drop_lohi":
+            y = y + mm(s_lo, w_hi)
+    return y if bias is None else y + bias.to(dtype).view(1, Cout, 1, 1)
+
+
+# ------------------------------------------------------------------------------------------------
 # ROIAlign (Caffe2, aligned=False) and the FPN level rule
 # ------------------------------------------------------------------------------------------------
 def _axis_weights(start, size, n_bins, grid, extent, dtype, dev, shift, f):
@@ -211,6 +318,23 @@ def roi_align_bounds(feat, rois, PH, PW, scale, sr, dout):
             "feat": bf, "feat_slack": sf}
 
 
+def hand_rois(H, W, scale, n_random, seed):
+    """Hand-placed rois (image coordinates) on a [*, *, H, W] map at `scale`, then random ones on both images."""
+    iw, ih = W / scale, H / scale
+    hand = [[0, 4, 4, 60, 50], [1, 10, 20, 100, 90],              # plain, batch index 1
+            [0, -20, -10, 30, 25], [1, iw - 30, ih - 40, iw + 30, ih + 10],   # partly outside
+            [1, -100, -100, -60, -50], [0, iw + 8, 4, iw + 60, 40],           # entirely outside
+            [0, iw - 1 / scale, 0, iw - 1 / scale, ih - 1 / scale],           # on the last column (zero width)
+            [1, 0, ih - 1 / scale, iw - 1 / scale, ih - 1 / scale],           # on the last row
+            [0, 0, 0, iw - 1 / scale, ih - 1 / scale],                         # the whole map
+            [0, 10.25, 10.5, 10.75, 10.875], [1, 33.5, 7.25, 34.0, 7.5]]       # smaller than one pixel
+    rng = np.random.default_rng(seed)
+    cxy = rng.uniform(0, 1, (n_random, 2)) * np.array([iw, ih])
+    sz = np.exp(rng.uniform(np.log(2), np.log(max(iw, ih)), (n_random, 2)))
+    rnd = np.concatenate([rng.integers(0, 2, (n_random, 1)), cxy - sz / 2, cxy + sz / 2], 1)
+    return torch.tensor(np.concatenate([np.array(hand, np.float64), rnd]), dtype=torch.float32)
+
+
 def fpn_levels(rois):
     """Index into [P2..P5] of every roi (fpn_roi_align.py's rule in float32)."""
     r = rois.detach().float().cpu().numpy()
@@ -247,10 +371,12 @@ def fpn_roi_align_bounds(feats, rois, PH, PW, scales, sr, dout):
     return out
 
 
-def special_offsets(N, kh, kw, Ho, Wo, H, W, stride, padding, dilation, seed, frac=0.5, scale=1.5):
+def special_offsets(N, kh, kw, Ho, Wo, H, W, stride, padding, dilation, seed, frac=0.5, scale=1.5, window=None):
     """fp32 offsets [N, 2*kh*kw, Ho, Wo]: a share `frac` of the sample coordinates is placed exactly on the values where
     floor and the corner guards decide (integers, -1, H, (-1, 0), (H-1, H), beyond the image), the rest are random.  All
-    values are dyadic, so the fp32 positions are exact."""
+    values are dyadic, so the fp32 positions are exact.
+    window=(TW, TH), stride 1 only: then the samples of every TW x TH tile of output pixels are rearranged for the window
+    kernel (csrc/dcn_win.cu), see _place_window."""
     (sh, sw), (ph, pw), (dh, dw) = _pair(stride), _pair(padding), _pair(dilation)
     rng = np.random.default_rng(seed)
     K = kh * kw
@@ -263,7 +389,97 @@ def special_offsets(N, kh, kw, Ho, Wo, H, W, stride, padding, dilation, seed, fr
                        -1.5, -3, E + 2, E + 0.25, E // 2, E // 2 + 0.75])
         tgt = sp[rng.integers(0, len(sp), (N,) + base.shape)]
         rnd = base + np.round(rng.standard_normal((N,) + base.shape) * scale * 256) / 256
-        return np.where(rng.uniform(size=(N,) + base.shape) < frac, tgt, rnd) - base
+        return np.where(rng.uniform(size=(N,) + base.shape) < frac, tgt, rnd)
 
-    off = np.stack([coord(base_h, H), coord(base_w, W)], 2).reshape(N, 2 * K, Ho, Wo)
+    h, w = coord(base_h, H), coord(base_w, W)
+    if window is not None:
+        assert (sh, sw) == (1, 1), "the window kernel runs stride-1 layers only"
+        _place_window(h, w, base_h, base_w, H, W, window, rng)
+    off = np.stack([h - base_h, w - base_w], 2).reshape(N, 2 * K, Ho, Wo)
     return torch.from_numpy(off.astype(np.float32))
+
+
+# ------------------------------------------------------------------------------------------------
+# the window of csrc/dcn_win.cu: per tile of output pixels one WIN_W x WIN_H-pixel window of the input is staged in
+# shared memory; samples with both corner columns and both corner rows inside it read it, the others (outliers) read
+# global memory.
+# ------------------------------------------------------------------------------------------------
+WIN_W, WIN_H = 32, 20          # DW_WW, DW_WH
+
+
+def _origin(hl, wl, cnt):
+    """dcn_win.cu's window origin of one tile from the floors of its valid samples (int arrays) and their count: the
+    corner bounding box if it fits, else centred on the mean floor (fp32 arithmetic, as the kernel)."""
+    if cnt == 0:
+        return 0, 0
+
+    def axis(fl, size):
+        lo, hi = int(fl.min()), int(fl.max()) + 1
+        if hi - lo + 1 <= size:
+            return lo
+        return int(np.floor(np.float32(int(fl.sum())) / np.float32(cnt) + np.float32(1))) - size // 2
+    return axis(wl, WIN_W), axis(hl, WIN_H)
+
+
+def _tiles(N, Ho, Wo, tile):
+    TW, TH = tile
+    for n in range(N):
+        for y0 in range(0, Ho, TH):
+            for x0 in range(0, Wo, TW):
+                yield n, slice(y0, min(y0 + TH, Ho)), slice(x0, min(x0 + TW, Wo))
+
+
+def window_origins(h, w, H, W, tile):
+    """Window origin (ox, oy) of every sample of h, w (float64 [N, K, Ho, Wo], exact fp32 sample coordinates) for the
+    kernel's TW x TH tiles of output pixels, with the floors and the validity (-1 < h < H, -1 < w < W) of the samples."""
+    valid = (h > -1) & (h < H) & (w > -1) & (w < W)
+    hl, wl = np.floor(h).astype(np.int64), np.floor(w).astype(np.int64)
+    ox, oy = np.zeros(h.shape, np.int64), np.zeros(h.shape, np.int64)
+    for n, ys, xs in _tiles(h.shape[0], h.shape[2], h.shape[3], tile):
+        v = valid[n, :, ys, xs]
+        ox[n, :, ys, xs], oy[n, :, ys, xs] = _origin(hl[n, :, ys, xs][v], wl[n, :, ys, xs][v], int(v.sum()))
+    return ox, oy, hl, wl, valid
+
+
+def _place_window(h, w, base_h, base_w, H, W, tile, rng):
+    """Rearrange the sample coordinates h, w ([N, K, Ho, Wo], in place) tile by tile, cycling through three modes:
+    0 / 1  every sample inside the image, the corner bounding box exactly WIN_W - 1, WIN_W or WIN_W + 1 px wide (mode 0)
+           or WIN_H - 1, WIN_H, WIN_H + 1 px tall (mode 1): both sides of the kernel's `box fits -> window at the box`
+           test, and with a fitting box, samples whose high corner is the window's last column / row.
+    2      one far outlier (at the far image corner) makes the box too large, so the window is centred on the mean
+           sample; then samples are placed on the window's last column and row -- integer ones, whose zero-weight high
+           corner lies one past the window, and fractional ones, which leave it -- one px before them, and one px before
+           the window's first column and row: both sides of the per-sample `both corners inside -> window, else
+           global-memory outlier` test."""
+    N, K, Ho, Wo = h.shape
+    for t, (n, ys, xs) in enumerate(_tiles(N, Ho, Wo, tile)):
+        th, tw = h[n, :, ys, xs], w[n, :, ys, xs]                # views
+        bh, bw = base_h[:, ys, xs], base_w[:, ys, xs]
+        mode, d = t % 3, (t // 3) % 3 - 1
+        # the bulk: inside the tile's own base footprint and inside the image (all valid, the box fits)
+        np.clip(th, max(bh.min(), 0), min(bh.max(), H - 1), out=th)
+        np.clip(tw, max(bw.min(), 0), min(bw.max(), W - 1), out=tw)
+        if mode < 2:
+            a, E, size = (tw, W, WIN_W) if mode == 0 else (th, H, WIN_H)
+            span = size + d                                      # corner box = max floor + 1 - min floor + 1
+            lo = min(max(a.min(), 0), E - span)
+            if lo < 0:
+                continue                                         # the image is narrower than the span
+            top = lo + span - 2 + (0.5 if t % 2 else 0.0)        # the largest floor is lo + span - 2
+            np.clip(a, lo, top, out=a)
+            a.flat[0], a.flat[-1] = lo, top
+            continue
+        far = (0 if xs.start > W / 2 else W - 1, 0 if ys.start > H / 2 else H - 1)
+        tw.flat[K // 2 * tw.shape[1] * tw.shape[2]], th.flat[K // 2 * th.shape[1] * th.shape[2]] = far
+        slots = rng.choice(np.arange(1, th.size), size=8, replace=False)
+        for _ in range(4):                                       # the placed samples move the mean a little
+            ox, oy = _origin(np.floor(th).astype(np.int64).ravel(), np.floor(tw).astype(np.int64).ravel(), th.size)
+            xm, ym = ox + WIN_W // 2, oy + WIN_H // 2
+            # (row, column): last column integer / fractional, the column before it, before the first column; same for rows
+            edge = [(ym, ox + WIN_W - 1), (ym, ox + WIN_W - 0.5), (ym, ox + WIN_W - 1.75), (ym, ox - 0.5),
+                    (oy + WIN_H - 1, xm), (oy + WIN_H - 0.5, xm), (oy + WIN_H - 1.25, xm), (oy - 0.5, xm + 0.25)]
+            for s, (yy, xx) in zip(slots, edge):
+                if -1 < yy < H and -1 < xx < W:
+                    th.flat[s], tw.flat[s] = yy, xx
+            if _origin(np.floor(th).astype(np.int64).ravel(), np.floor(tw).astype(np.int64).ravel(), th.size) == (ox, oy):
+                break

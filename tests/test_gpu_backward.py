@@ -107,23 +107,6 @@ def test_deform_conv_function_vs_fp64(dev, name, modulated):
 # ------------------------------------------------------------------------------------------------
 # RoIAlignFunction
 # ------------------------------------------------------------------------------------------------
-def _rois(H, W, scale, n_random, seed):
-    """Hand-placed rois (image coordinates) on a [*, *, H, W] map at `scale`, then random ones on both images."""
-    iw, ih = W / scale, H / scale
-    hand = [[0, 4, 4, 60, 50], [1, 10, 20, 100, 90],              # plain, batch index 1
-            [0, -20, -10, 30, 25], [1, iw - 30, ih - 40, iw + 30, ih + 10],   # partly outside
-            [1, -100, -100, -60, -50], [0, iw + 8, 4, iw + 60, 40],           # entirely outside
-            [0, iw - 1 / scale, 0, iw - 1 / scale, ih - 1 / scale],           # on the last column (zero width)
-            [1, 0, ih - 1 / scale, iw - 1 / scale, ih - 1 / scale],           # on the last row
-            [0, 0, 0, iw - 1 / scale, ih - 1 / scale],                         # the whole map
-            [0, 10.25, 10.5, 10.75, 10.875], [1, 33.5, 7.25, 34.0, 7.5]]       # smaller than one pixel
-    rng = np.random.default_rng(seed)
-    cxy = rng.uniform(0, 1, (n_random, 2)) * np.array([iw, ih])
-    sz = np.exp(rng.uniform(np.log(2), np.log(max(iw, ih)), (n_random, 2)))
-    rnd = np.concatenate([rng.integers(0, 2, (n_random, 1)), cxy - sz / 2, cxy + sz / 2], 1)
-    return torch.tensor(np.concatenate([np.array(hand, np.float64), rnd]), dtype=torch.float32)
-
-
 def _roi_case(dev, B, C, H, W, rois, PH, PW, scale, sr, seed, forward=None):
     """forward(features, rois): the call under test, RoIAlignFunction by default."""
     from upsnet_b200.training import RoIAlignFunction
@@ -156,7 +139,7 @@ def test_roi_align_backward_vs_fp64(dev):
 @pytest.mark.parametrize("sr", [0, 1, 2, 4])
 @pytest.mark.parametrize("pooled", [(7, 7), (14, 14), (3, 5)])
 def test_roi_align_function_vs_fp64(dev, pooled, sr):
-    _roi_case(dev, 2, 16, 30, 44, _rois(30, 44, 0.25, 25, sr), *pooled, 0.25, sr, 4)
+    _roi_case(dev, 2, 16, 30, 44, G.hand_rois(30, 44, 0.25, 25, sr), *pooled, 0.25, sr, 4)
 
 
 def test_roi_align_many_overlapping_rois(dev):
@@ -174,7 +157,7 @@ def test_roi_align_no_rois_zero_gradient(dev):
 
 def test_roi_align_grid_stride(dev):
     """R * C * 14 * 14 = 1.6 M output elements, above the 1.08 M threads of the capped grid."""
-    _roi_case(dev, 2, 64, 40, 56, _rois(40, 56, 0.25, 117, 12), 14, 14, 0.25, 2, 12)
+    _roi_case(dev, 2, 64, 40, 56, G.hand_rois(40, 56, 0.25, 117, 12), 14, 14, 0.25, 2, 12)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -2,11 +2,17 @@
 every layer shape class of the engine against the CPU oracle at the "fp32 logits within 1e-3" contract -- in practice
 held to ~1e-5 relative, which is what makes the pair stream an fp32-grade format.  Own file = own process (a trap in a
 tensor-core kernel poisons the CUDA context)."""
+import os
+import sys
+
 import numpy as np
 import pytest
 import torch
 
 from oracle import oracle as O
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from kernel_trace import launched_kernels  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 X3 = 1
@@ -52,12 +58,9 @@ def test_pair_roundtrip(dev, pair_mode):
 
 
 def _conv_kernels(fn):
-    """fn() under torch.profiler: its result and the names of the implicit-GEMM conv kernels it launched."""
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        out = fn()
-        torch.cuda.synchronize()
-    return out, {e.key for e in prof.key_averages() if "igemm_" in e.key}
+    """fn() under torch.profiler: its result and the names of the implicit-GEMM conv kernels it launched
+    (tests/kernel_trace.py: sessions that lost their records are repeated)."""
+    return launched_kernels(fn, lambda n: "igemm_" in n)
 
 
 def _assert_kernel(names, tma):

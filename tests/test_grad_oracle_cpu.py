@@ -139,6 +139,100 @@ def test_dcn_tolerance_accepts_fp32_rejects_near_miss(case, modulated):
     assert not passes(_dcn_families(case, modulated, x, off, w, b, m, dy, shift=1 / 64))
 
 
+FWD_CASES = [  # (N, Cin, Cout, H, W, padding / dilation, special_offsets frac, window tile)
+    (1, 8, 4, 40, 72, 1, 0.3, (16, 8)),        # window-mode offsets on 16 x 8 tiles (3 x 9 tiles of the three modes)
+    (2, 4, 3, 11, 13, 1, 1.0, None),
+    (1, 6, 5, 24, 20, 2, 0.3, (8, 4)),         # dilation 2, window mode on the small-map 8 x 4 tiles
+]
+FWD_FAULTS = {  # every fault each family's constant must reject
+    "x3_pair": ["right_guard", "shift", "drop_lohi", "mask_hi_only", "window_edge"],
+    "x3_f32": ["right_guard", "shift", "drop_lohi", "mask_hi_only"],
+    "bf16": ["right_guard", "shift", "truncate"],       # one bf16 plane: no hi / lo to mask apart
+}
+
+
+def _fwd_inputs(case, modulated, seed):
+    N, Cin, Cout, H, W, pd, frac, tile = case
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(N, Cin, H, W, generator=g)
+    off = G.special_offsets(N, 3, 3, H, W, H, W, 1, pd, pd, seed, frac, window=tile)
+    w = torch.randn(Cout, Cin, 3, 3, generator=g) / (Cin * 9) ** 0.5
+    b = torch.randn(Cout, generator=g)
+    m = torch.rand(N, 9, H, W, generator=g) * 2 if modulated else None
+    return x, off, w, b, m
+
+
+@pytest.mark.parametrize("modulated", [False, True])
+@pytest.mark.parametrize("case", FWD_CASES)
+@pytest.mark.parametrize("family", list(FWD_FAULTS))
+def test_forward_tolerance_accepts_kernel_arithmetic_rejects_faults(family, case, modulated):
+    """Each inference DCN precision mode (tests/test_gpu_forward_fp64.py) emulated in torch -- the gather's blend, the
+    bf16 hi/lo split of sample and weights, three products (bf16x3) or one (bf16), fp32 accumulation -- passes its
+    family's constant against the float64 reference, and each planted fault fails it.  Cases are narrowed to a few input
+    channels: the faults that change a sample by 2^-9 of itself (drop_lohi, mask_hi_only) are diluted by averaging over
+    the 9 Cin terms of an output, so with hundreds of channels their per-element ratio drops towards the constants.
+    The window-edge fault changes only samples one px past the window, which window-mode offsets place; without them
+    (case 2) it cannot be seen and is not asserted."""
+    x, off, w, b, m = _fwd_inputs(case, modulated, 17)
+    pd, tile = case[5], case[7]
+    cfg = (3, 3, 1, pd, pd)
+    if family == "x3_pair":
+        hi = x.bfloat16().float()
+        xin = (hi, (x - hi).bfloat16().float())
+        xexact = xin[0].double() + xin[1].double()
+    else:
+        xin = x.bfloat16().float() if family == "bf16" else x
+        xexact = xin.double()
+    if family == "bf16":
+        w = w.bfloat16().float()
+        col = G.dcn_columns(xin, off, *cfg, mask=m, mode="bf16")
+        want = G.dcn_gemm(col, w, b, "bf16", dtype=torch.float64)
+        bound = G.dcn_gemm(col.abs(), w.abs(), b.abs(), "bf16", dtype=torch.float64)
+    else:
+        want = G.deform_conv(xexact, off.double(), w.double(), b.double(), None if m is None else m.double(), 1, pd, pd,
+                             offset32=off)
+        bound = G.deform_conv(xexact.abs(), off.double(), w.double().abs(), b.double().abs(),
+                              None if m is None else m.double(), 1, pd, pd, offset32=off)
+    c = G.TOL["dcn_" + family]
+
+    def run(fault=None):
+        col = G.dcn_columns(xin, off, *cfg, mask=m, mode=family, fault=fault, window=tile)
+        return G.dcn_gemm(col, w, b, family, fault=fault)
+
+    ok, ratio = G.check(run(), want, bound, c)
+    assert ok, (family, "emulation rejected", ratio, c)
+    for fault in FWD_FAULTS[family]:
+        if (fault == "mask_hi_only" and m is None) or (fault == "window_edge" and tile is None):
+            continue
+        ok, ratio = G.check(run(fault), want, bound, c)
+        assert not ok, (family, fault, "accepted", ratio, c)
+
+
+def test_window_offsets_hit_the_window_geometry():
+    """special_offsets(window=tile) produces, for dcn_win.cu's window placement: corner boxes 1 px narrower than,
+    exactly as wide as and 1 px wider than the window in both axes; integer and fractional samples on the last column
+    and row of a mean-centred window, and samples just before its first column and row."""
+    H, W, Ho, Wo, K = 40, 72, 40, 72, 9
+    off = G.special_offsets(1, 3, 3, Ho, Wo, H, W, 1, 1, 1, 4, 0.3, window=(16, 8))
+    assert torch.equal(off, G.special_offsets(1, 3, 3, Ho, Wo, H, W, 1, 1, 1, 4, 0.3, window=(16, 8)))
+    o = off.double().numpy().reshape(1, K, 2, Ho, Wo)
+    bh = (np.arange(Ho)[None, :, None] - 1 + (np.arange(K) // 3)[:, None, None]) * np.ones((1, 1, Wo))
+    bw = (np.arange(Wo)[None, None, :] - 1 + (np.arange(K) % 3)[:, None, None]) * np.ones((1, Ho, 1))
+    h, w = bh + o[:, :, 0], bw + o[:, :, 1]
+    ox, oy, hl, wl, valid = G.window_origins(h, w, H, W, (16, 8))
+    spans_w, spans_h = set(), set()
+    for n, ys, xs in G._tiles(1, Ho, Wo, (16, 8)):
+        v = valid[n, :, ys, xs]
+        spans_w.add(int(wl[n, :, ys, xs][v].max()) + 2 - int(wl[n, :, ys, xs][v].min()))
+        spans_h.add(int(hl[n, :, ys, xs][v].max()) + 2 - int(hl[n, :, ys, xs][v].min()))
+    assert {G.WIN_W - 1, G.WIN_W, G.WIN_W + 1} <= spans_w and {G.WIN_H - 1, G.WIN_H, G.WIN_H + 1} <= spans_h
+    dx, dy = wl - ox, hl - oy
+    integer_w, integer_h = w == np.floor(w), h == np.floor(h)
+    for sel in (dx == G.WIN_W - 1) & integer_w, (dx == G.WIN_W - 1) & ~integer_w, (dy == G.WIN_H - 1) & integer_h, \
+            (dy == G.WIN_H - 1) & ~integer_h, dx == -1, dy == -1:
+        assert int((sel & valid).sum()) >= 3
+
+
 @pytest.mark.parametrize("sr", [0, 2])
 def test_roi_tolerance_accepts_fp32_rejects_near_miss(sr):
     g = torch.Generator().manual_seed(8)
