@@ -540,6 +540,38 @@ int upsnet_dcn_col2im_coord(const float *dcol, const float *x, const float *offs
 int upsnet_roi_align_backward(const float *dout, const float *rois, int R, int B, int C, int H, int W, int PH, int PW,
                               int sampling_ratio, float spatial_scale, float *dfeat, void *stream);
 
+/* ---------------------------------------------------------------------------------------
+ * upsnet_rpn_targets: the RPN training targets of one image (training configuration, BASELINE config #4).
+ * replaces: rpn/assign_anchor.py:447-595 _get_rpn_blobs, called per image by add_rpn_blobs (:370-445) from the data loaders
+ *           (dataset/coco.py:129, cityscapes.py:122, ade20k.py:116): the float32 IoU matrix of the inside anchors against
+ *           every box (the Cython bbox/bbox.pyx:21-65), its argmaxes and tie sets, two np.random.choice draws and four dense
+ *           arrays per level, on the host.
+ * Anchors: level l has field_sizes[l]^2 cells of A anchors, anchor (l, y, x, a) = float32(cell_anchors[l][a] (float64
+ *   [L,A,4], generate_anchors.py:50-76) + (x, y, x, y) * strides[l]), ordered level, cell (y, x), a (generate_anchors.py:
+ *   79-130).  Inside: in float64, x1 >= -straddle, y1 >= -straddle, x2 < im_width + straddle, y2 < im_height + straddle;
+ *   every anchor when straddle_thresh < 0.
+ * gt_boxes float32 [G,4], 1 <= G <= UPSNET_RPN_TARGETS_MAX_G (more: UPSNET_E_UNSUPPORTED).  IoU bit-exact to bbox.pyx as
+ *   Cython compiles it (double `+ 1.0`, double `ua`).  fg = an inside anchor whose IoU equals some box's maximum over the
+ *   inside anchors (a maximum of 0 included) or whose own maximum is >= positive_overlap; bg candidates = maximum <
+ *   negative_overlap (float32 compares).  More than num_fg fg anchors: the ones drawn are disabled; then num_bg =
+ *   batch_size - #fg anchors are drawn from the bg candidates (an fg anchor drawn becomes 0), and none is labelled 0 when
+ *   there are no more than num_bg candidates.  A draw of `size` among n candidates takes the positions p (in anchor order)
+ *   with the `size` smallest keys splitmix64(s ^ p * 0x9E3779B97F4A7C15), s = seed for the fg draw and splitmix64(seed)
+ *   for the bg draw.
+ * Outputs, the per-level blobs of the reference concatenated over levels: labels int64 [1,A,F,F] (-1 / 0 / 1),
+ *   bbox_targets (bbox_transform_inv of the anchors with label 1 after the fg draw, against their first-argmax box),
+ *   inside_weights (1 where the final label is 1) and outside_weights (float32(1.0 / #labels >= 0) where the label is
+ *   >= 0), each float32 [1,4A,F,F] with channel a*4 + c; counts int32 [4] = inside anchors, fg candidates, final fg,
+ *   final bg.  All device memory; the call never synchronises.
+ * Workspace: upsnet_rpn_targets_workspace_bytes(total anchors, batch_size). */
+#define UPSNET_RPN_TARGETS_MAX_G 4096
+int upsnet_rpn_targets_workspace_bytes(long long num_anchors, int batch_size, size_t *bytes);
+int upsnet_rpn_targets(const float *gt_boxes, int G, const double *cell_anchors, const int *strides,
+                       const int *field_sizes, int L, int A, double im_height, double im_width, double straddle_thresh,
+                       float positive_overlap, float negative_overlap, int batch_size, int num_fg, unsigned long long seed,
+                       int64_t *labels, float *bbox_targets, float *inside_weights, float *outside_weights, int *counts,
+                       void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -98,6 +98,9 @@ def lib():
         L.upsnet_cocoeval_accumulate.argtypes = [vp, i, vp, vp, i, vp, vp, vp, vp, sz, vp]
         L.upsnet_combined_pan_workspace_bytes.argtypes = [i, i, i, C.POINTER(sz)]
         L.upsnet_combined_pan_result.argtypes = [vp, i, i, i, vp, vp, i, vp, vp, i, vp, i, i, f, f, i, vp, vp, vp, sz, vp]
+        L.upsnet_rpn_targets_workspace_bytes.argtypes = [C.c_longlong, i, C.POINTER(sz)]
+        L.upsnet_rpn_targets.argtypes = [vp, i, vp, C.POINTER(i), C.POINTER(i), i, i, d, d, d, f, f, i, i, C.c_ulonglong,
+                                         vp, vp, vp, vp, vp, vp, sz, vp]
         _lib = L
     return _lib
 
@@ -116,6 +119,7 @@ EXPORTED_SYMBOLS = [
     "upsnet_sseg_update", "upsnet_cocoeval_workspace_bytes", "upsnet_cocoeval_image",
     "upsnet_cocoeval_accumulate_workspace_bytes", "upsnet_cocoeval_accumulate",
     "upsnet_combined_pan_workspace_bytes", "upsnet_combined_pan_result",
+    "upsnet_rpn_targets_workspace_bytes", "upsnet_rpn_targets",
 ]
 
 

@@ -11,6 +11,7 @@
 // test oracle for these kernels) produces.
 #include <cfloat>
 
+#include "anchors.cuh"
 #include "common.cuh"
 
 namespace ups {
@@ -60,14 +61,11 @@ __global__ void rpn_decode_kernel(const RpnDecodeParams p) {
   const int a = (int)(i % p.A);
   const long long pix = i / p.A;
   const int x = (int)(pix % p.w[l]), y = (int)(pix / p.w[l]);
-  // anchors = float32(base(float64) + shift) (pyramid_proposal.py:83-100, bbox_transform.py:298)
-  const double sx = (double)(x * p.stride[l]), sy = (double)(y * p.stride[l]);
-  const double* b = p.base + ((size_t)l * p.A + a) * 4;
-  const float x1 = (float)(b[0] + sx), y1 = (float)(b[1] + sy), x2 = (float)(b[2] + sx), y2 = (float)(b[3] + sy);
+  const float4 an = shifted_anchor(p.base + ((size_t)l * p.A + a) * 4, x, y, p.stride[l]);
   const size_t hw = (size_t)p.h[l] * p.w[l];
   const float* d = p.deltas[l] + (size_t)a * 4 * hw + (size_t)y * p.w[l] + x;
-  const float4 o = decode_clip(x1, y1, x2, y2, __ldg(d), __ldg(d + hw), __ldg(d + 2 * hw), __ldg(d + 3 * hw), p.xform_clip,
-                               p.im_h, p.im_w);
+  const float4 o = decode_clip(an.x, an.y, an.z, an.w, __ldg(d), __ldg(d + hw), __ldg(d + 2 * hw), __ldg(d + 3 * hw),
+                               p.xform_clip, p.im_h, p.im_w);
   reinterpret_cast<float4*>(p.out)[t] = o;
 }
 

@@ -1,0 +1,518 @@
+// rpn_target.cu -- RPN training targets of one image (rpn/assign_anchor.py:447-595 _get_rpn_blobs, called by
+// add_rpn_blobs from the training data loaders), replacing the host's float32 IoU matrix of every inside anchor against
+// every ground-truth box, its argmaxes and tie sets, the two np.random.choice draws and the dense per-level arrays.
+//
+// Launches (none synchronises the host; every count stays on the device):
+//   1. rt_max:     per anchor: inside test, IoU against every box (boxes staged through shared memory in chunks),
+//                  max and first argmax; per box: max over the inside anchors (atomicMax on the bit pattern, IoU >= 0)
+//   2. rt_label:   per anchor: fg candidate (IoU == some box's max, or max >= pos), bg candidate (max < neg); per-CTA counts
+//   3. rt_scan:    CTA offsets, totals, and what each draw has to do
+//   4. rt_compact: candidate lists in anchor order with the 64-bit key of each position (the seeded rule of np.random.choice)
+//   5. rt_select:  8 radix passes: the exact k-th smallest key of each draw
+//   6. rt_mark:    the drawn anchors (<= batch of them) into two short lists
+//   7. rt_write:   one CTA writes labels, box targets and weights of those anchors over the constant fill
+#include "anchors.cuh"
+#include "common.cuh"
+
+namespace ups {
+
+constexpr int kRtThreads = 256;     // anchors per CTA in the per-anchor passes
+constexpr int kRtChunk = 1024;      // boxes staged in shared memory at a time
+constexpr int kRtMaxG = UPSNET_RPN_TARGETS_MAX_G;
+constexpr int kRtLevels = 8;
+constexpr int kRtSelBlocks = 264;   // grid-stride CTAs of the select / mark passes, per draw
+
+enum { kFlagInside = 1, kFlagFg = 2, kFlagBg = 4, kFlagBgDrawn = 8 };
+enum { kDrawAll = 0, kDrawNone = 1, kDrawSelect = 2 };
+
+struct RtState {
+  unsigned int hist[2][256];
+  unsigned long long prefix[2];     // after the 8 passes: the k-th smallest key of the draw
+  int n[2], k[2], need[2], mode[2];
+  unsigned int ticket[2];
+  int list_cnt[2];
+};
+
+struct RtParams {
+  const float* gt;                  // [G,4]
+  const double* cell;               // [L,A,4]
+  long long off[kRtLevels + 1];     // first anchor of each level
+  int F[kRtLevels], stride[kRtLevels];
+  int L, A, N, G, nblk, batch, num_fg;
+  double im_h, im_w, straddle;
+  float pos, neg;
+  unsigned long long seed;
+  // workspace
+  RtState* st;
+  unsigned int* gtmax;              // [G] float bits
+  float* amax;                      // [N]
+  int* aarg;                        // [N]
+  unsigned char* flags;             // [N]
+  int* blk;                         // [nblk][3] fg, bg, inside counts; then [nblk][2] fg, bg offsets
+  unsigned long long* keys[2];      // [N] per draw, in candidate order
+  int* idx[2];                      // [N] anchor of each candidate
+  int* list[2];                     // [batch] drawn anchors
+  // outputs
+  int64_t* labels;
+  float *targets, *inside_w, *outside_w;
+  int* counts;
+};
+
+__device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
+  unsigned long long z = x + 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+__device__ __forceinline__ int anchor_level(const RtParams& p, int n) {
+  int l = 0;
+  while (l + 1 < p.L && n >= p.off[l + 1]) ++l;
+  return l;
+}
+
+// where anchor n (the reference's order: level, then cell (y, x), then a) lives in the per-level blobs
+struct AnchorPos {
+  int l, a, yx, FF;
+  float4 box;
+};
+
+__device__ __forceinline__ AnchorPos anchor_of(const RtParams& p, int n) {
+  AnchorPos o;
+  o.l = anchor_level(p, n);
+  const int r = n - (int)p.off[o.l];
+  const int cell = r / p.A;
+  o.a = r - cell * p.A;
+  const int F = p.F[o.l], y = cell / F, x = cell - y * F;
+  o.yx = y * F + x;
+  o.FF = F * F;
+  o.box = shifted_anchor(p.cell + ((size_t)o.l * p.A + o.a) * 4, x, y, p.stride[o.l]);
+  return o;
+}
+
+// element of the labels blob [1,A,F,F] and first element of the [1,4A,F,F] blobs (channel a*4 + c), levels concatenated
+__device__ __forceinline__ size_t label_at(const RtParams& p, const AnchorPos& q) {
+  return (size_t)p.off[q.l] + (size_t)q.a * q.FF + q.yx;
+}
+__device__ __forceinline__ size_t coord_at(const RtParams& p, const AnchorPos& q) {
+  return 4 * (size_t)p.off[q.l] + (size_t)(4 * q.a) * q.FF + q.yx;
+}
+
+__device__ __forceinline__ bool is_inside(const RtParams& p, float4 an) {
+  if (p.straddle < 0.0) return true;
+  return (double)an.x >= -p.straddle && (double)an.y >= -p.straddle && (double)an.z < p.im_w + p.straddle &&
+         (double)an.w < p.im_h + p.straddle;
+}
+
+// (f64(f32(x2 - x1)) + 1.0) * (f64(f32(y2 - y1)) + 1.0): bbox.pyx's box area as Cython compiles it (the `+ 1` is a
+// double literal)
+__device__ __forceinline__ double area64(float4 b) {
+  return __dmul_rn(__dadd_rn((double)__fsub_rn(b.z, b.x), 1.0), __dadd_rn((double)__fsub_rn(b.w, b.y), 1.0));
+}
+
+// bbox.pyx bbox_overlaps for one (anchor, box) pair, bit-exact to the compiled extension.  iw and ih are
+// f32(f64(f32(min - max)) + 1.0) there; that double rounding is innocuous for a sum of two float32 values (53 >= 2*24 + 1
+// bits), so they are the float32 sum computed here.
+__device__ __forceinline__ float pair_iou(float4 a, double a_area, float4 q, float q_area) {
+  const float iw = __fadd_rn(__fsub_rn(fminf(a.z, q.z), fmaxf(a.x, q.x)), 1.0f);
+  if (!(iw > 0.f)) return 0.f;
+  const float ih = __fadd_rn(__fsub_rn(fminf(a.w, q.w), fmaxf(a.y, q.y)), 1.0f);
+  if (!(ih > 0.f)) return 0.f;
+  const float inter = __fmul_rn(iw, ih);
+  const float ua = (float)__dsub_rn(__dadd_rn(a_area, (double)q_area), (double)inter);
+  return __fdiv_rn(inter, ua);
+}
+
+__device__ __forceinline__ float4 load_box(const float* gt, int k) {
+  return make_float4(__ldg(gt + 4 * k), __ldg(gt + 4 * k + 1), __ldg(gt + 4 * k + 2), __ldg(gt + 4 * k + 3));
+}
+
+// 1. per-anchor max / first argmax and per-box max
+__global__ void __launch_bounds__(kRtThreads) rt_max_kernel(const RtParams p) {
+  __shared__ float4 sbox[kRtChunk];
+  __shared__ float sarea[kRtChunk];
+  __shared__ unsigned int smax[kRtChunk];
+  const int n = blockIdx.x * kRtThreads + threadIdx.x;
+  bool inside = false;
+  float4 an = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (n < p.N) {
+    an = anchor_of(p, n).box;
+    inside = is_inside(p, an);
+  }
+  const double a_area = area64(an);
+  float best = -1.f;
+  int arg = 0;
+  for (int c0 = 0; c0 < p.G; c0 += kRtChunk) {
+    const int cn = min(kRtChunk, p.G - c0);
+    __syncthreads();
+    for (int k = threadIdx.x; k < cn; k += kRtThreads) {
+      const float4 q = load_box(p.gt, c0 + k);
+      sbox[k] = q;
+      sarea[k] = (float)area64(q);
+      smax[k] = 0u;
+    }
+    __syncthreads();
+    if (inside) {
+      for (int k = 0; k < cn; ++k) {
+        const float o = pair_iou(an, a_area, sbox[k], sarea[k]);
+        if (o > best) { best = o; arg = c0 + k; }     // strict: the first argmax, as numpy's
+        const unsigned int b = __float_as_uint(o);
+        if (b > smax[k]) atomicMax(&smax[k], b);
+      }
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < cn; k += kRtThreads)
+      if (smax[k]) atomicMax(&p.gtmax[c0 + k], smax[k]);
+  }
+  if (n < p.N) {
+    p.amax[n] = best;
+    p.aarg[n] = arg;
+    p.flags[n] = inside ? kFlagInside : 0;
+  }
+}
+
+// 2. candidate flags; an anchor is fg when one of its IoUs equals that box's max (boxes whose max is 0 included)
+__global__ void __launch_bounds__(kRtThreads) rt_label_kernel(const RtParams p) {
+  __shared__ float4 sbox[kRtChunk];
+  __shared__ float sarea[kRtChunk];
+  __shared__ float smax[kRtChunk];
+  const int n = blockIdx.x * kRtThreads + threadIdx.x;
+  bool inside = false, fg = false, bg = false;
+  float4 an = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (n < p.N) {
+    inside = (p.flags[n] & kFlagInside) != 0;
+    if (inside) {
+      const float m = p.amax[n];
+      fg = m >= p.pos;
+      bg = m < p.neg;
+      an = anchor_of(p, n).box;
+    }
+  }
+  const double a_area = area64(an);
+  bool look = inside && !fg;
+  for (int c0 = 0; c0 < p.G; c0 += kRtChunk) {
+    const int cn = min(kRtChunk, p.G - c0);
+    __syncthreads();
+    for (int k = threadIdx.x; k < cn; k += kRtThreads) {
+      const float4 q = load_box(p.gt, c0 + k);
+      sbox[k] = q;
+      sarea[k] = (float)area64(q);
+      smax[k] = __uint_as_float(__ldcg(p.gtmax + c0 + k));
+    }
+    __syncthreads();
+    if (look) {
+      for (int k = 0; k < cn; ++k)
+        if (pair_iou(an, a_area, sbox[k], sarea[k]) == smax[k]) { fg = true; look = false; break; }
+    }
+  }
+  if (n < p.N) p.flags[n] = (inside ? kFlagInside : 0) | (fg ? kFlagFg : 0) | (bg ? kFlagBg : 0);
+  const int cf = __syncthreads_count(fg), cb = __syncthreads_count(bg), ci = __syncthreads_count(inside);
+  if (threadIdx.x == 0) {
+    p.blk[3 * blockIdx.x] = cf;
+    p.blk[3 * blockIdx.x + 1] = cb;
+    p.blk[3 * blockIdx.x + 2] = ci;
+  }
+}
+
+// exclusive scan of one int per thread over a 1024-thread CTA; *total gets the sum
+__device__ __forceinline__ int cta_scan_excl(int v, int* warp_sums, int* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warp_sums[wid] = x;
+  __syncthreads();
+  if (wid == 0) {
+    int w = warp_sums[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += y;
+    }
+    warp_sums[lane] = w;
+  }
+  __syncthreads();
+  const int base = wid ? warp_sums[wid - 1] : 0;
+  *total = warp_sums[31];
+  __syncthreads();
+  return base + x - v;
+}
+
+// 3. CTA offsets of both candidate lists and the plan of both draws (one CTA of 1024 threads)
+__global__ void __launch_bounds__(1024) rt_scan_kernel(const RtParams p) {
+  __shared__ int warp_sums[32];
+  int carry_f = 0, carry_b = 0, carry_i = 0;
+  int* off = p.blk + 3 * p.nblk;
+  for (int b0 = 0; b0 < p.nblk; b0 += 1024) {
+    const int b = b0 + threadIdx.x;
+    const bool ok = b < p.nblk;
+    int tf, tb, ti;
+    const int ef = cta_scan_excl(ok ? p.blk[3 * b] : 0, warp_sums, &tf);
+    const int eb = cta_scan_excl(ok ? p.blk[3 * b + 1] : 0, warp_sums, &tb);
+    cta_scan_excl(ok ? p.blk[3 * b + 2] : 0, warp_sums, &ti);
+    if (ok) { off[2 * b] = carry_f + ef; off[2 * b + 1] = carry_b + eb; }
+    carry_f += tf; carry_b += tb; carry_i += ti;
+  }
+  if (threadIdx.x == 0) {
+    RtState* st = p.st;
+    const int nf = carry_f, nb = carry_b;
+    p.counts[0] = carry_i;
+    p.counts[1] = nf;
+    // fg: when nf > num_fg, np.random.choice disables the nf - num_fg smallest keys, i.e. keeps the num_fg largest
+    st->n[0] = nf;
+    st->mode[0] = nf > p.num_fg ? kDrawSelect : kDrawAll;
+    st->k[0] = st->need[0] = p.num_fg;
+    // bg: num_bg = batch - #(label 1); with no more candidates than that, no anchor is labelled 0
+    const int num_bg = p.batch - min(nf, p.num_fg);
+    st->n[1] = nb;
+    st->mode[1] = (nb > num_bg && num_bg > 0) ? kDrawSelect : kDrawNone;
+    st->k[1] = st->need[1] = num_bg;
+  }
+}
+
+// 4. candidate lists in anchor order (= the reference's index lists) with the key of each position:
+//    key(s, pos) = splitmix64(s ^ pos * golden gamma), s = seed (fg) or splitmix64(seed) (bg); fg keys are stored inverted so
+//    that both draws select the k smallest
+__global__ void __launch_bounds__(kRtThreads) rt_compact_kernel(const RtParams p) {
+  __shared__ int wf[kRtThreads / 32], wb[kRtThreads / 32];
+  const int n = blockIdx.x * kRtThreads + threadIdx.x;
+  const int fl = n < p.N ? p.flags[n] : 0;
+  const bool fg = fl & kFlagFg, bg = fl & kFlagBg;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const unsigned bf = __ballot_sync(0xffffffffu, fg), bb = __ballot_sync(0xffffffffu, bg);
+  if (lane == 0) { wf[wid] = __popc(bf); wb[wid] = __popc(bb); }
+  __syncthreads();
+  const unsigned lt = (1u << lane) - 1u;
+  int rf = __popc(bf & lt), rb = __popc(bb & lt);
+  for (int w = 0; w < wid; ++w) { rf += wf[w]; rb += wb[w]; }
+  const int* off = p.blk + 3 * p.nblk + 2 * blockIdx.x;
+  const unsigned long long gamma = 0x9E3779B97F4A7C15ull;
+  if (fg) {
+    const int pos = off[0] + rf;
+    p.keys[0][pos] = ~splitmix64(p.seed ^ ((unsigned long long)pos * gamma));
+    p.idx[0][pos] = n;
+  }
+  if (bg) {
+    const int pos = off[1] + rb;
+    p.keys[1][pos] = splitmix64(splitmix64(p.seed) ^ ((unsigned long long)pos * gamma));
+    p.idx[1][pos] = n;
+  }
+}
+
+// 5. one 8-bit digit of the radix select of both draws (blockIdx.y); the last CTA of a draw fixes the digit
+__global__ void __launch_bounds__(kRtThreads) rt_select_kernel(const RtParams p, int shift) {
+  const int s = blockIdx.y;
+  RtState* st = p.st;
+  if (st->mode[s] != kDrawSelect) return;
+  __shared__ unsigned int sh[256];
+  __shared__ int s_last;
+  sh[threadIdx.x] = 0u;
+  __syncthreads();
+  const int n = st->n[s];
+  const unsigned long long prefix = st->prefix[s];
+  const unsigned long long mask_hi = shift >= 56 ? 0ull : (~0ull << (shift + 8));
+  const unsigned long long* keys = p.keys[s];
+  for (int i = blockIdx.x * kRtThreads + threadIdx.x; i < n; i += gridDim.x * kRtThreads) {
+    const unsigned long long key = keys[i];
+    if ((key & mask_hi) == prefix) atomicAdd(&sh[(unsigned)(key >> shift) & 255u], 1u);
+  }
+  __syncthreads();
+  if (sh[threadIdx.x]) atomicAdd(&st->hist[s][threadIdx.x], sh[threadIdx.x]);
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = atomicAdd(&st->ticket[s], 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  sh[threadIdx.x] = __ldcg(&st->hist[s][threadIdx.x]);
+  st->hist[s][threadIdx.x] = 0u;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned int need = (unsigned int)st->need[s];
+    unsigned int acc = 0;
+    int d = 0;
+    for (; d < 255; ++d) {
+      if (acc + sh[d] >= need) break;
+      acc += sh[d];
+    }
+    st->need[s] = (int)(need - acc);
+    st->prefix[s] = prefix | ((unsigned long long)d << shift);
+    st->ticket[s] = 0u;
+  }
+}
+
+// 6. the drawn anchors: fg keeps (keys <= the k-th), bg labels them 0 and flags them for rt_write
+__global__ void __launch_bounds__(kRtThreads) rt_mark_kernel(const RtParams p) {
+  const int s = blockIdx.y;
+  RtState* st = p.st;
+  const int mode = st->mode[s];
+  if (mode == kDrawNone) return;
+  const int n = st->n[s];
+  const unsigned long long kth = st->prefix[s];
+  for (int i = blockIdx.x * kRtThreads + threadIdx.x; i < n; i += gridDim.x * kRtThreads) {
+    if (mode == kDrawAll || p.keys[s][i] <= kth) {
+      const int a = p.idx[s][i];
+      p.list[s][atomicAdd(&st->list_cnt[s], 1)] = a;
+      if (s == 1) p.flags[a] |= kFlagBgDrawn;
+    }
+  }
+}
+
+// bbox_transform.py:332-363 bbox_transform_inv with weights 1, float32
+__device__ __forceinline__ float4 box_target(float4 e, float4 g) {
+  const float ew = __fadd_rn(__fsub_rn(e.z, e.x), 1.0f), eh = __fadd_rn(__fsub_rn(e.w, e.y), 1.0f);
+  const float ecx = __fadd_rn(e.x, __fmul_rn(0.5f, ew)), ecy = __fadd_rn(e.y, __fmul_rn(0.5f, eh));
+  const float gw = __fadd_rn(__fsub_rn(g.z, g.x), 1.0f), gh = __fadd_rn(__fsub_rn(g.w, g.y), 1.0f);
+  const float gcx = __fadd_rn(g.x, __fmul_rn(0.5f, gw)), gcy = __fadd_rn(g.y, __fmul_rn(0.5f, gh));
+  return make_float4(__fdiv_rn(__fsub_rn(gcx, ecx), ew), __fdiv_rn(__fsub_rn(gcy, ecy), eh), logf(__fdiv_rn(gw, ew)),
+                     logf(__fdiv_rn(gh, eh)));
+}
+
+// 7. the drawn anchors over the constant fill (labels -1, everything else 0); one CTA
+__global__ void __launch_bounds__(kRtThreads) rt_write_kernel(const RtParams p) {
+  RtState* st = p.st;
+  const int nfs = st->list_cnt[0], nbs = st->list_cnt[1];
+  int overlap = 0;     // fg-stage anchors relabelled 0 by the bg draw
+  for (int i0 = 0; i0 < nfs; i0 += kRtThreads) {
+    const int i = i0 + threadIdx.x;
+    overlap += __syncthreads_count(i < nfs && (p.flags[p.list[0][i]] & kFlagBgDrawn));
+  }
+  const int num_examples = nfs + nbs - overlap;
+  const float w = num_examples > 0 ? (float)__ddiv_rn(1.0, (double)num_examples) : 0.f;
+  for (int i = threadIdx.x; i < nbs; i += kRtThreads) {
+    const AnchorPos q = anchor_of(p, p.list[1][i]);
+    p.labels[label_at(p, q)] = 0;
+    float* ow = p.outside_w + coord_at(p, q);
+    for (int c = 0; c < 4; ++c) ow[(size_t)c * q.FF] = w;
+  }
+  for (int i = threadIdx.x; i < nfs; i += kRtThreads) {
+    const int n = p.list[0][i];
+    const AnchorPos q = anchor_of(p, n);
+    const size_t base = coord_at(p, q);
+    const float4 t = box_target(q.box, load_box(p.gt, p.aarg[n]));
+    p.targets[base] = t.x;
+    p.targets[base + q.FF] = t.y;
+    p.targets[base + 2 * (size_t)q.FF] = t.z;
+    p.targets[base + 3 * (size_t)q.FF] = t.w;
+    if (!(p.flags[n] & kFlagBgDrawn)) {
+      p.labels[label_at(p, q)] = 1;
+      for (int c = 0; c < 4; ++c) {
+        p.inside_w[base + (size_t)c * q.FF] = 1.f;
+        p.outside_w[base + (size_t)c * q.FF] = w;
+      }
+    }
+  }
+  if (threadIdx.x == 0) {
+    p.counts[2] = nfs - overlap;
+    p.counts[3] = nbs;
+  }
+}
+
+struct RtLayout {
+  size_t state, gtmax, amax, aarg, flags, blk, keys0, keys1, idx0, idx1, list0, list1, total;
+};
+
+inline RtLayout rt_layout(long long N, int batch) {
+  RtLayout o;
+  const long long nblk = (N + kRtThreads - 1) / kRtThreads;
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t r = at; at = align_up(at + bytes, 256); return r; };
+  o.state = take(sizeof(RtState));
+  o.gtmax = take((size_t)kRtMaxG * 4);
+  o.amax = take((size_t)N * 4);
+  o.aarg = take((size_t)N * 4);
+  o.flags = take((size_t)N);
+  o.blk = take((size_t)nblk * 5 * 4);
+  o.keys0 = take((size_t)N * 8);
+  o.keys1 = take((size_t)N * 8);
+  o.idx0 = take((size_t)N * 4);
+  o.idx1 = take((size_t)N * 4);
+  o.list0 = take((size_t)batch * 4);
+  o.list1 = take((size_t)batch * 4);
+  o.total = at;
+  return o;
+}
+
+}  // namespace ups
+
+extern "C" int upsnet_rpn_targets_workspace_bytes(long long num_anchors, int batch_size, size_t* bytes) {
+  if (!bytes || num_anchors <= 0 || num_anchors >= (1ll << 31) || batch_size <= 0) return UPSNET_E_BADARG;
+  *bytes = ups::rt_layout(num_anchors, batch_size).total;
+  return 0;
+}
+
+extern "C" int upsnet_rpn_targets(const float* gt_boxes, int G, const double* cell_anchors, const int* strides,
+                                  const int* field_sizes, int L, int A, double im_height, double im_width,
+                                  double straddle_thresh, float positive_overlap, float negative_overlap, int batch_size,
+                                  int num_fg, unsigned long long seed, int64_t* labels, float* bbox_targets,
+                                  float* inside_weights, float* outside_weights, int* counts, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  using namespace ups;
+  if (!gt_boxes || !cell_anchors || !strides || !field_sizes || !labels || !bbox_targets || !inside_weights ||
+      !outside_weights || !counts || !workspace)
+    return UPSNET_E_BADARG;
+  if (G <= 0 || L <= 0 || L > kRtLevels || A <= 0 || batch_size <= 0 || num_fg <= 0 || num_fg > batch_size)
+    return UPSNET_E_BADARG;
+  if (G > kRtMaxG) return UPSNET_E_UNSUPPORTED;
+  RtParams p{};
+  long long N = 0;
+  for (int l = 0; l < L; ++l) {
+    if (field_sizes[l] <= 0 || strides[l] <= 0) return UPSNET_E_BADARG;
+    p.off[l] = N;
+    p.F[l] = field_sizes[l];
+    p.stride[l] = strides[l];
+    N += (long long)A * field_sizes[l] * field_sizes[l];
+  }
+  p.off[L] = N;
+  if (N >= (1ll << 31)) return UPSNET_E_UNSUPPORTED;
+  const RtLayout lo = rt_layout(N, batch_size);
+  if (workspace_bytes < lo.total) return UPSNET_E_WORKSPACE;
+  char* ws = (char*)workspace;
+  p.gt = gt_boxes; p.cell = cell_anchors;
+  p.L = L; p.A = A; p.N = (int)N; p.G = G; p.nblk = (int)((N + kRtThreads - 1) / kRtThreads);
+  p.batch = batch_size; p.num_fg = num_fg;
+  p.im_h = im_height; p.im_w = im_width; p.straddle = straddle_thresh;
+  p.pos = positive_overlap; p.neg = negative_overlap; p.seed = seed;
+  p.st = (RtState*)(ws + lo.state);
+  p.gtmax = (unsigned int*)(ws + lo.gtmax);
+  p.amax = (float*)(ws + lo.amax);
+  p.aarg = (int*)(ws + lo.aarg);
+  p.flags = (unsigned char*)(ws + lo.flags);
+  p.blk = (int*)(ws + lo.blk);
+  p.keys[0] = (unsigned long long*)(ws + lo.keys0);
+  p.keys[1] = (unsigned long long*)(ws + lo.keys1);
+  p.idx[0] = (int*)(ws + lo.idx0);
+  p.idx[1] = (int*)(ws + lo.idx1);
+  p.list[0] = (int*)(ws + lo.list0);
+  p.list[1] = (int*)(ws + lo.list1);
+  p.labels = labels; p.targets = bbox_targets; p.inside_w = inside_weights; p.outside_w = outside_weights;
+  p.counts = counts;
+  cudaStream_t st = (cudaStream_t)stream;
+  UPS_CUDA(cudaMemsetAsync(p.st, 0, sizeof(RtState), st));
+  UPS_CUDA(cudaMemsetAsync(p.gtmax, 0, (size_t)G * 4, st));
+  // the constant fill of the outputs: label -1 (all bytes 0xff), targets and weights 0
+  UPS_CUDA(cudaMemsetAsync(labels, 0xff, (size_t)N * 8, st));
+  UPS_CUDA(cudaMemsetAsync(bbox_targets, 0, (size_t)N * 16, st));
+  UPS_CUDA(cudaMemsetAsync(inside_weights, 0, (size_t)N * 16, st));
+  UPS_CUDA(cudaMemsetAsync(outside_weights, 0, (size_t)N * 16, st));
+  rt_max_kernel<<<p.nblk, kRtThreads, 0, st>>>(p);
+  UPS_CHECK_LAUNCH();
+  rt_label_kernel<<<p.nblk, kRtThreads, 0, st>>>(p);
+  UPS_CHECK_LAUNCH();
+  rt_scan_kernel<<<1, 1024, 0, st>>>(p);
+  UPS_CHECK_LAUNCH();
+  rt_compact_kernel<<<p.nblk, kRtThreads, 0, st>>>(p);
+  UPS_CHECK_LAUNCH();
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    rt_select_kernel<<<dim3(kRtSelBlocks, 2), kRtThreads, 0, st>>>(p, shift);
+    UPS_CHECK_LAUNCH();
+  }
+  rt_mark_kernel<<<dim3(kRtSelBlocks, 2), kRtThreads, 0, st>>>(p);
+  UPS_CHECK_LAUNCH();
+  rt_write_kernel<<<1, kRtThreads, 0, st>>>(p);
+  UPS_CHECK_LAUNCH();
+  return 0;
+}

@@ -10,12 +10,16 @@
 * FlatBucketAllReduce: the gradient all-reduce of `upsnet_end2end_train.py:121` (hvd.DistributedOptimizer) as flat bf16
   buckets over torch.distributed (NCCL between the GPUs, gloo in the CPU tests): gradients are packed per bucket,
   reduced asynchronously while the rest of backward runs, averaged and unpacked before the optimiser step.
+* RPNTargets: the RPN training targets of one image (rpn/assign_anchor.py:370-595 add_rpn_blobs / _get_rpn_blobs, run by
+  the reference's data loaders on the host) on the device (csrc/rpn_target.cu), as the label dict coco.py:133-142 builds.
 
-Scope note: this is the operator / communication layer of the training configuration.  Losses, target assignment and the
-optimiser are plain torch in the reference and stay that way; the dense backward convolutions are library calls.
+Scope note: this is the operator / communication layer of the training configuration plus the RPN targets.  Losses, the
+RCNN / mask targets and the optimiser are plain torch or numpy in the reference and stay that way; the dense backward
+convolutions are library calls.
 """
 import ctypes as C
 
+import numpy as np
 import torch
 import torch.distributed as dist
 from torch.nn.modules.utils import _pair
@@ -248,3 +252,95 @@ class FlatBucketAllReduce:
 
     def __call__(self):
         return self.start().finish()
+
+
+# ------------------------------------------------------------------------------------------------
+# RPN training targets
+# ------------------------------------------------------------------------------------------------
+class RPNTargets:
+    """add_rpn_blobs for one image on the device.
+
+    Built from the reference's `config` (network.rpn_feat_stride, anchor_scales[0], anchor_ratios, rcnn_feat_stride;
+    train.max_size, rpn_batch_size, rpn_fg_fraction, rpn_positive_overlap, rpn_negative_overlap, rpn_straddle_thresh) or
+    from the same values as keywords.  Labels, weights and the dx / dy targets are bit-exact to the reference; dw / dh go
+    through a float32 log (numpy's is not correctly rounded either).  The two np.random.choice draws are replaced by a
+    seeded rule (include/upsnet_b200.h, upsnet_rpn_targets): the same seed gives the same targets."""
+
+    def __init__(self, config=None, *, feat_strides=(4, 8, 16, 32, 64), anchor_scale=8, anchor_ratios=(0.5, 1, 2),
+                 rcnn_feat_stride=32, max_size=1333, batch_size=256, fg_fraction=0.5, positive_overlap=0.7,
+                 negative_overlap=0.3, straddle_thresh=0):
+        from .detection import generate_anchors
+        if config is not None:
+            net, tr = config.network, config.train
+            feat_strides, anchor_scale, anchor_ratios = net.rpn_feat_stride, net.anchor_scales[0], net.anchor_ratios
+            rcnn_feat_stride, max_size, batch_size = net.rcnn_feat_stride, tr.max_size, tr.rpn_batch_size
+            fg_fraction, positive_overlap = tr.rpn_fg_fraction, tr.rpn_positive_overlap
+            negative_overlap, straddle_thresh = tr.rpn_negative_overlap, tr.rpn_straddle_thresh
+        self.strides = [int(s) for s in feat_strides]
+        fpn_max = rcnn_feat_stride * np.ceil(max_size / float(rcnn_feat_stride))          # generate_anchors.py:98-101
+        self.field_sizes = [int(np.ceil(fpn_max / float(s))) for s in self.strides]
+        self.cell = np.stack([generate_anchors(s, (anchor_scale * s,), anchor_ratios) for s in self.strides])
+        self.A = self.cell.shape[1]
+        self.num_anchors = sum(self.A * F * F for F in self.field_sizes)
+        self.batch_size, self.num_fg = int(batch_size), int(fg_fraction * batch_size)   # assign_anchor.py:502
+        self.pos, self.neg, self.straddle = float(positive_overlap), float(negative_overlap), float(straddle_thresh)
+        self._dev = {}
+        self.counts = None
+
+    def _buffers(self, dev):
+        if dev not in self._dev:
+            sz = C.c_size_t()
+            check(lib().upsnet_rpn_targets_workspace_bytes(self.num_anchors, self.batch_size, C.byref(sz)),
+                  "rpn_targets_workspace_bytes")
+            self._dev[dev] = (torch.from_numpy(np.ascontiguousarray(self.cell, np.float64)).to(dev),
+                              torch.empty(sz.value, dtype=torch.uint8, device=dev))
+        return self._dev[dev]
+
+    def __call__(self, gt_boxes, im_height, im_width, seed=None):
+        """gt_boxes: CUDA float32 [G,4] (already scaled); -> {'rpn_labels_fpn{s}': int64 [1,A,F,F],
+        'rpn_bbox_targets_fpn{s}' / 'rpn_bbox_inside_weights_fpn{s}' / 'rpn_bbox_outside_weights_fpn{s}': float32
+        [1,4A,F,F]} as views of four flat device tensors.  self.counts: int32 [4] on the device (inside anchors, fg
+        candidates, final fg, final bg).  seed=None draws one from np.random, so np.random.seed governs it."""
+        require_cuda(gt_boxes)
+        gt = f32c(gt_boxes).reshape(-1, 4)
+        if gt.shape[0] == 0:
+            # the reference raises NameError here (anchor_to_gt_max is unbound without boxes)
+            raise _lib.UpsnetError("rpn_targets: no ground-truth boxes")
+        if seed is None:
+            seed = int(np.random.randint(np.iinfo(np.int64).max, dtype=np.int64))
+        dev = gt.device
+        cell, ws = self._buffers(dev)
+        N = self.num_anchors
+        labels = torch.empty(N, dtype=torch.int64, device=dev)
+        targets, inside, outside = (torch.empty(4 * N, dtype=torch.float32, device=dev) for _ in range(3))
+        counts = torch.empty(4, dtype=torch.int32, device=dev)
+        L = len(self.strides)
+        with torch.cuda.device(dev):
+            check(lib().upsnet_rpn_targets(ptr(gt), gt.shape[0], ptr(cell), (C.c_int * L)(*self.strides),
+                                           (C.c_int * L)(*self.field_sizes), L, self.A, float(im_height),
+                                           float(im_width), self.straddle, self.pos, self.neg, self.batch_size,
+                                           self.num_fg, int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(labels), ptr(targets),
+                                           ptr(inside), ptr(outside), ptr(counts), ptr(ws), ws.numel(),
+                                           stream_ptr(dev)), "rpn_targets")
+        self.counts = counts
+        out, off = {}, 0
+        for s, F in zip(self.strides, self.field_sizes):
+            n = self.A * F * F
+            out["rpn_labels_fpn%d" % s] = labels[off:off + n].view(1, self.A, F, F)
+            for name, t in (("rpn_bbox_targets_fpn%d", targets), ("rpn_bbox_inside_weights_fpn%d", inside),
+                            ("rpn_bbox_outside_weights_fpn%d", outside)):
+                out[name % s] = t[4 * off:4 * (off + n)].view(1, 4 * self.A, F, F)
+            off += n
+        return out
+
+    def from_roidb(self, entry, im_scale, device, seed=None):
+        """Drop-in for add_rpn_blobs on one roidb entry: boxes of a class > 0 that are not crowd, times the Python float
+        im_scale (im_scales[0] of get_image_blob, assign_anchor.py:399); image size np.round(h * scale) (:391-392)."""
+        keep = np.where((entry["gt_classes"] > 0) & (entry["is_crowd"] == 0))[0]
+        boxes = (entry["boxes"][keep, :] * float(im_scale)).astype(np.float32)
+        if boxes.shape[0] == 0:
+            raise _lib.UpsnetError("rpn_targets: no ground-truth boxes")
+        im_height = np.round(entry["height"] * im_scale)
+        im_width = np.round(entry["width"] * im_scale)
+        gt = torch.from_numpy(np.ascontiguousarray(boxes)).to(device)
+        return self(gt, im_height, im_width, seed)
