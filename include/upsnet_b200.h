@@ -572,6 +572,50 @@ int upsnet_rpn_targets(const float *gt_boxes, int G, const double *cell_anchors,
                        int64_t *labels, float *bbox_targets, float *inside_weights, float *outside_weights, int *counts,
                        void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---------------------------------------------------------------------------------------
+ * upsnet_proposal_targets: the Mask R-CNN proposal targets of one image (training configuration).
+ * replaces: operators/modules/proposal_mask_target.py:37-62 ProposalMaskTarget.forward, run in the middle of the model's
+ *           forward (models/resnet_upsnet.py:105-110): rois.cpu(), add_proposals (dataset/json_dataset.py:335-348,
+ *           454-516, 538-556), sample_rois (bbox/sample_rois.py:51-176), add_mask_rcnn_blobs with pycocotools' polygon
+ *           rasteriser (mask/mask_transform.py:195-323) and nine host-to-device copies.
+ * Rows: the G gt rows of the roidb entry, then rois[r, 1:] * float32(1 / im_scale) for the rows r with rois[r, 0] == 0
+ *   (float32, as numpy >= 2 computes it).  A gt row takes max overlap / class / gt row from gt_max_overlaps,
+ *   gt_max_classes (max / argmax of the entry's gt_overlaps; -1 / 0 for crowd) and gt_box_to_gt_ind; a proposal takes
+ *   the IoU (bit-exact to the compiled bbox.pyx) against every gt row of class > 0, crowd included: with a first-argmax
+ *   max > 0, (max, gt_classes of that row, that row), else (0, 0, -1).  Every gt row must have gt_classes > 0.
+ * Sampling: fg = max >= fg_thresh (> 0), bg = bg_thresh_lo <= max < bg_thresh_hi (float32 compares); fg_per_image is
+ *   int(np.round(fg_fraction * batch_rois)), computed by the caller; min(fg_per_image, #fg) fg rows and
+ *   min(batch_rois - that, #bg) bg rows are drawn: a draw of `size` among n candidates takes the positions p (in row
+ *   order) with the `size` smallest keys splitmix64(s ^ p * 0x9E3779B97F4A7C15), s = seed for the fg draw and
+ *   splitmix64(seed) for the bg draw (the rule of upsnet_rpn_targets), and keeps them in row order.
+ * Outputs (batch_rois rows; rows past the fg + bg rows are 0, nongt_inds past its count -1):
+ *   rois_out float32 [batch_rois,5] = (0, box * im_scale); labels int64 [batch_rois] = class of the fg rows, 0 for bg;
+ *   bbox_targets / bbox_inside_weights / bbox_outside_weights float32 [batch_rois, 4K]: at columns 4*label..4*label+3
+ *   of an fg row, bbox_transform_inv(box, gt box of gt_inds[box_to_gt_ind]) with weights (wx, wy, ww, wh) multiplied
+ *   first, and weights 1 (an fg proposal on a crowd box regresses to the crowd box); nongt_inds int64 [batch_rois] = the
+ *   output rows that are proposals; roi_has_mask uint8 [batch_rois] = label > 0.
+ *   Mask rows (capacity max(fg_per_image, 1)): mask_rois float32 [.,5] = the fg rows of rois_out; mask_int32 float32
+ *   [., K * M * M], -1 outside the label's M x M block, which holds (row-major [y][x]) the union of the polygons of the
+ *   non-crowd object whose box (obj_boxes: float32 min / max of its polygon coordinates) has the largest IoU with the
+ *   row's box (first argmax), rasterised as maskApi.c rleFrPoly does at M x M after ((p - x1) * M) / max(x2 - x1, 1) in
+ *   float32.  Without fg rows: one mask row, the first bg row, all -1, and roi_has_mask[0] = 1.
+ *   Objects: obj_poly_off [num_objects + 1] indexes polygons, poly_vert_off [P + 1] indexes verts float32 [V,2].
+ *   counts int32 [5] = fg rows, bg rows, mask rows, error (1 when there is neither fg nor bg: the reference raises
+ *   IndexError), nongt_inds count.  All device memory; the call never synchronises.
+ * Limits: 1 <= G <= UPSNET_RPN_TARGETS_MAX_G, mask_size <= 32, batch_rois <= 4096, cls_agnostic_bbox_reg = 0; otherwise
+ *   UPSNET_E_UNSUPPORTED.  Workspace: upsnet_proposal_targets_workspace_bytes(R, G, batch_rois). */
+int upsnet_proposal_targets_workspace_bytes(int num_rois, int num_gt, int batch_rois, size_t *bytes);
+int upsnet_proposal_targets(const float *rois, int R, const float *gt_boxes, const float *gt_max_overlaps,
+                            const int *gt_max_classes, const int *gt_classes, const int *gt_box_to_gt_ind, int G,
+                            const float *obj_boxes, const int *obj_poly_off, const int *poly_vert_off, const float *verts,
+                            int num_objects, float im_scale, int num_classes, int batch_rois, int fg_per_image,
+                            float fg_thresh, float bg_thresh_hi, float bg_thresh_lo, float wx, float wy, float ww,
+                            float wh, int cls_agnostic_bbox_reg, int mask_size, unsigned long long seed, float *rois_out,
+                            int64_t *labels, float *bbox_targets, float *bbox_inside_weights,
+                            float *bbox_outside_weights, int64_t *nongt_inds, float *mask_rois, float *mask_int32,
+                            unsigned char *roi_has_mask, int *counts, void *workspace, size_t workspace_bytes,
+                            void *stream);
+
 #ifdef __cplusplus
 }
 #endif

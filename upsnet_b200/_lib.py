@@ -101,6 +101,9 @@ def lib():
         L.upsnet_rpn_targets_workspace_bytes.argtypes = [C.c_longlong, i, C.POINTER(sz)]
         L.upsnet_rpn_targets.argtypes = [vp, i, vp, C.POINTER(i), C.POINTER(i), i, i, d, d, d, f, f, i, i, C.c_ulonglong,
                                          vp, vp, vp, vp, vp, vp, sz, vp]
+        L.upsnet_proposal_targets_workspace_bytes.argtypes = [i, i, i, C.POINTER(sz)]
+        L.upsnet_proposal_targets.argtypes = [vp, i] + [vp] * 5 + [i] + [vp] * 4 + [i, f, i, i, i] + [f] * 7 + \
+            [i, i, C.c_ulonglong] + [vp] * 11 + [sz, vp]
         _lib = L
     return _lib
 
@@ -120,6 +123,7 @@ EXPORTED_SYMBOLS = [
     "upsnet_cocoeval_accumulate_workspace_bytes", "upsnet_cocoeval_accumulate",
     "upsnet_combined_pan_workspace_bytes", "upsnet_combined_pan_result",
     "upsnet_rpn_targets_workspace_bytes", "upsnet_rpn_targets",
+    "upsnet_proposal_targets_workspace_bytes", "upsnet_proposal_targets",
 ]
 
 

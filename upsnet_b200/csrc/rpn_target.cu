@@ -13,6 +13,7 @@
 //   7. rt_write:   one CTA writes labels, box targets and weights of those anchors over the constant fill
 #include "anchors.cuh"
 #include "common.cuh"
+#include "targets.cuh"
 
 namespace ups {
 
@@ -58,13 +59,6 @@ struct RtParams {
   int* counts;
 };
 
-__device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
-  unsigned long long z = x + 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
 __device__ __forceinline__ int anchor_level(const RtParams& p, int n) {
   int l = 0;
   while (l + 1 < p.L && n >= p.off[l + 1]) ++l;
@@ -102,25 +96,6 @@ __device__ __forceinline__ bool is_inside(const RtParams& p, float4 an) {
   if (p.straddle < 0.0) return true;
   return (double)an.x >= -p.straddle && (double)an.y >= -p.straddle && (double)an.z < p.im_w + p.straddle &&
          (double)an.w < p.im_h + p.straddle;
-}
-
-// (f64(f32(x2 - x1)) + 1.0) * (f64(f32(y2 - y1)) + 1.0): bbox.pyx's box area as Cython compiles it (the `+ 1` is a
-// double literal)
-__device__ __forceinline__ double area64(float4 b) {
-  return __dmul_rn(__dadd_rn((double)__fsub_rn(b.z, b.x), 1.0), __dadd_rn((double)__fsub_rn(b.w, b.y), 1.0));
-}
-
-// bbox.pyx bbox_overlaps for one (anchor, box) pair, bit-exact to the compiled extension.  iw and ih are
-// f32(f64(f32(min - max)) + 1.0) there; that double rounding is innocuous for a sum of two float32 values (53 >= 2*24 + 1
-// bits), so they are the float32 sum computed here.
-__device__ __forceinline__ float pair_iou(float4 a, double a_area, float4 q, float q_area) {
-  const float iw = __fadd_rn(__fsub_rn(fminf(a.z, q.z), fmaxf(a.x, q.x)), 1.0f);
-  if (!(iw > 0.f)) return 0.f;
-  const float ih = __fadd_rn(__fsub_rn(fminf(a.w, q.w), fmaxf(a.y, q.y)), 1.0f);
-  if (!(ih > 0.f)) return 0.f;
-  const float inter = __fmul_rn(iw, ih);
-  const float ua = (float)__dsub_rn(__dadd_rn(a_area, (double)q_area), (double)inter);
-  return __fdiv_rn(inter, ua);
 }
 
 __device__ __forceinline__ float4 load_box(const float* gt, int k) {
@@ -214,33 +189,6 @@ __global__ void __launch_bounds__(kRtThreads) rt_label_kernel(const RtParams p) 
   }
 }
 
-// exclusive scan of one int per thread over a 1024-thread CTA; *total gets the sum
-__device__ __forceinline__ int cta_scan_excl(int v, int* warp_sums, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp_sums[wid] = x;
-  __syncthreads();
-  if (wid == 0) {
-    int w = warp_sums[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += y;
-    }
-    warp_sums[lane] = w;
-  }
-  __syncthreads();
-  const int base = wid ? warp_sums[wid - 1] : 0;
-  *total = warp_sums[31];
-  __syncthreads();
-  return base + x - v;
-}
-
 // 3. CTA offsets of both candidate lists and the plan of both draws (one CTA of 1024 threads)
 __global__ void __launch_bounds__(1024) rt_scan_kernel(const RtParams p) {
   __shared__ int warp_sums[32];
@@ -289,15 +237,14 @@ __global__ void __launch_bounds__(kRtThreads) rt_compact_kernel(const RtParams p
   int rf = __popc(bf & lt), rb = __popc(bb & lt);
   for (int w = 0; w < wid; ++w) { rf += wf[w]; rb += wb[w]; }
   const int* off = p.blk + 3 * p.nblk + 2 * blockIdx.x;
-  const unsigned long long gamma = 0x9E3779B97F4A7C15ull;
   if (fg) {
     const int pos = off[0] + rf;
-    p.keys[0][pos] = ~splitmix64(p.seed ^ ((unsigned long long)pos * gamma));
+    p.keys[0][pos] = ~draw_key(p.seed, 0, (unsigned long long)pos);
     p.idx[0][pos] = n;
   }
   if (bg) {
     const int pos = off[1] + rb;
-    p.keys[1][pos] = splitmix64(splitmix64(p.seed) ^ ((unsigned long long)pos * gamma));
+    p.keys[1][pos] = draw_key(p.seed, 1, (unsigned long long)pos);
     p.idx[1][pos] = n;
   }
 }
@@ -361,16 +308,6 @@ __global__ void __launch_bounds__(kRtThreads) rt_mark_kernel(const RtParams p) {
   }
 }
 
-// bbox_transform.py:332-363 bbox_transform_inv with weights 1, float32
-__device__ __forceinline__ float4 box_target(float4 e, float4 g) {
-  const float ew = __fadd_rn(__fsub_rn(e.z, e.x), 1.0f), eh = __fadd_rn(__fsub_rn(e.w, e.y), 1.0f);
-  const float ecx = __fadd_rn(e.x, __fmul_rn(0.5f, ew)), ecy = __fadd_rn(e.y, __fmul_rn(0.5f, eh));
-  const float gw = __fadd_rn(__fsub_rn(g.z, g.x), 1.0f), gh = __fadd_rn(__fsub_rn(g.w, g.y), 1.0f);
-  const float gcx = __fadd_rn(g.x, __fmul_rn(0.5f, gw)), gcy = __fadd_rn(g.y, __fmul_rn(0.5f, gh));
-  return make_float4(__fdiv_rn(__fsub_rn(gcx, ecx), ew), __fdiv_rn(__fsub_rn(gcy, ecy), eh), logf(__fdiv_rn(gw, ew)),
-                     logf(__fdiv_rn(gh, eh)));
-}
-
 // 7. the drawn anchors over the constant fill (labels -1, everything else 0); one CTA
 __global__ void __launch_bounds__(kRtThreads) rt_write_kernel(const RtParams p) {
   RtState* st = p.st;
@@ -392,7 +329,7 @@ __global__ void __launch_bounds__(kRtThreads) rt_write_kernel(const RtParams p) 
     const int n = p.list[0][i];
     const AnchorPos q = anchor_of(p, n);
     const size_t base = coord_at(p, q);
-    const float4 t = box_target(q.box, load_box(p.gt, p.aarg[n]));
+    const float4 t = box_target(q.box, load_box(p.gt, p.aarg[n]), make_float4(1.f, 1.f, 1.f, 1.f));
     p.targets[base] = t.x;
     p.targets[base + q.FF] = t.y;
     p.targets[base + 2 * (size_t)q.FF] = t.z;

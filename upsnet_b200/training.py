@@ -12,10 +12,13 @@
   reduced asynchronously while the rest of backward runs, averaged and unpacked before the optimiser step.
 * RPNTargets: the RPN training targets of one image (rpn/assign_anchor.py:370-595 add_rpn_blobs / _get_rpn_blobs, run by
   the reference's data loaders on the host) on the device (csrc/rpn_target.cu), as the label dict coco.py:133-142 builds.
+* ProposalTargets: the Mask R-CNN proposal targets of one image (operators/modules/proposal_mask_target.py, run by the
+  reference on the host in the middle of the forward) on the device (csrc/proposal_target.cu): roi sampling, box
+  targets and the class-specific polygon mask targets.
 
-Scope note: this is the operator / communication layer of the training configuration plus the RPN targets.  Losses, the
-RCNN / mask targets and the optimiser are plain torch or numpy in the reference and stay that way; the dense backward
-convolutions are library calls.
+Scope note: this is the operator / communication layer of the training configuration plus the RPN and proposal targets.
+Losses and the optimiser are plain torch in the reference and stay that way; the dense backward convolutions are
+library calls.
 """
 import ctypes as C
 
@@ -344,3 +347,153 @@ class RPNTargets:
         im_width = np.round(entry["width"] * im_scale)
         gt = torch.from_numpy(np.ascontiguousarray(boxes)).to(device)
         return self(gt, im_height, im_width, seed)
+
+
+# ------------------------------------------------------------------------------------------------
+# Mask R-CNN proposal targets
+# ------------------------------------------------------------------------------------------------
+class PackedGT:
+    """The ground truth of one roidb entry on the device (ProposalTargets.pack_roidb): views of one int32 upload."""
+
+    def __init__(self, buf, parts, G, O):
+        self.buf, self.G, self.O = buf, G, O
+        for name, (off, n, dtype) in parts.items():
+            v = buf[off:off + n]
+            setattr(self, name, v.view(torch.float32) if dtype == np.float32 else v)
+
+
+class ProposalTargets:
+    """ProposalMaskTarget.forward for one image on the device.
+
+    Built from the reference's `config` (dataset.num_classes, train.batch_rois / fg_fraction / fg_thresh / bg_thresh_hi
+    / bg_thresh_lo, network.bbox_reg_weights / mask_size / cls_agnostic_bbox_reg) or from the same values as keywords.
+    Every output is bit-exact to the reference except the dw / dh targets, which go through a float32 log (numpy's is
+    not correctly rounded either).  The two np.random.choice draws of sample_rois are replaced by the seeded rule of
+    RPNTargets (include/upsnet_b200.h, upsnet_proposal_targets): the same seed gives the same targets.
+
+    Unlike the reference, the proposals are not appended to the roidb entry: nothing downstream reads them
+    (get_gt_rois keeps the rows of class > 0 only)."""
+
+    def __init__(self, config=None, *, num_classes=81, batch_rois=512, fg_fraction=0.25, fg_thresh=0.5, bg_thresh_hi=0.5,
+                 bg_thresh_lo=0.0, bbox_reg_weights=(10., 10., 5., 5.), mask_size=28, cls_agnostic_bbox_reg=False):
+        if config is not None:
+            net, tr = config.network, config.train
+            num_classes, batch_rois, fg_fraction = config.dataset.num_classes, tr.batch_rois, tr.fg_fraction
+            fg_thresh, bg_thresh_hi, bg_thresh_lo = tr.fg_thresh, tr.bg_thresh_hi, tr.bg_thresh_lo
+            bbox_reg_weights, mask_size = net.bbox_reg_weights, net.mask_size
+            cls_agnostic_bbox_reg = net.cls_agnostic_bbox_reg
+        self.K, self.batch_rois, self.M = int(num_classes), int(batch_rois), int(mask_size)
+        self.fg_per_image = int(np.round(fg_fraction * self.batch_rois))           # sample_rois.py:56 (half to even)
+        self.fg_thresh, self.bg_hi, self.bg_lo = float(fg_thresh), float(bg_thresh_hi), float(bg_thresh_lo)
+        self.weights = tuple(float(w) for w in bbox_reg_weights)
+        self.cls_agnostic = bool(cls_agnostic_bbox_reg)
+        self.mask_capacity = max(self.fg_per_image, 1)
+        self.counts = None
+
+    def pack_roidb(self, entry, device):
+        """One host-to-device upload of the entry's ground truth: boxes, gt_classes, gt_overlaps' max / argmax,
+        box_to_gt_ind_map and the float32 polygons of the non-crowd objects of class > 0."""
+        boxes = np.ascontiguousarray(entry["boxes"], np.float32).reshape(-1, 4)
+        G = boxes.shape[0]
+        cls = np.asarray(entry["gt_classes"]).astype(np.int64)
+        crowd = np.asarray(entry["is_crowd"]).astype(bool)
+        if G == 0 or (cls <= 0).any():
+            raise _lib.UpsnetError("proposal_targets: every gt row needs a class > 0 (json_dataset writes no other)")
+        if (cls >= self.K).any():
+            raise _lib.UpsnetError("proposal_targets: a gt class is not below num_classes")
+        ov = entry["gt_overlaps"]
+        ov = ov.toarray() if hasattr(ov, "toarray") else np.asarray(ov)
+        b2g = np.asarray(entry["box_to_gt_ind_map"]).astype(np.int64)
+        if ((b2g < -G) | (b2g >= G)).any():
+            raise _lib.UpsnetError("proposal_targets: box_to_gt_ind_map out of range")
+        obj = np.flatnonzero((cls > 0) & ~crowd)
+        if obj.size == 0:
+            # add_rpn_blobs fails on such an image in the reference, and RPNTargets.from_roidb raises there too
+            raise _lib.UpsnetError("proposal_targets: no non-crowd ground truth")
+        obj_boxes, obj_off, poly_off, verts = [], [0], [0], []
+        for i in obj:
+            segm = entry["segms"][i]
+            if not isinstance(segm, list) or not segm:
+                raise _lib.UpsnetError("proposal_targets: segmentation %d is not a polygon list" % i)
+            ps = [np.asarray(p, np.float32) for p in segm]
+            if any(p.ndim != 1 or p.size < 6 or p.size % 2 for p in ps):
+                raise _lib.UpsnetError("proposal_targets: polygon of segmentation %d has an odd or < 6 coordinates" % i)
+            allp = np.concatenate(ps)
+            obj_boxes.append([allp[0::2].min(), allp[1::2].min(), allp[0::2].max(), allp[1::2].max()])
+            for p in ps:
+                verts.append(p)
+                poly_off.append(poly_off[-1] + p.size // 2)
+            obj_off.append(obj_off[-1] + len(ps))
+        f32 = np.float32
+        arrays = [("boxes", boxes.ravel(), f32), ("gt_max", ov.max(1).astype(f32), f32),
+                  ("gt_maxcls", ov.argmax(1).astype(np.int32), np.int32), ("gt_classes", cls.astype(np.int32), np.int32),
+                  ("gt_map", b2g.astype(np.int32), np.int32),
+                  ("obj_boxes", np.asarray(obj_boxes, f32).ravel(), f32),
+                  ("obj_poly", np.asarray(obj_off, np.int32), np.int32),
+                  ("poly_vert", np.asarray(poly_off, np.int32), np.int32),
+                  ("verts", np.concatenate(verts).astype(f32), f32)]
+        parts, chunks, off = {}, [], 0
+        for name, a, dt in arrays:
+            a = np.ascontiguousarray(a, dt)
+            parts[name] = (off, a.size, dt)
+            chunks.append(a.view(np.int32))
+            pad = (-a.size) % 4                     # 16-byte aligned parts
+            chunks.append(np.zeros(pad, np.int32))
+            off += a.size + pad
+        buf = torch.from_numpy(np.concatenate(chunks)).to(device)
+        return PackedGT(buf, parts, G, len(obj))
+
+    def __call__(self, rois, packed, im_scale, seed=None):
+        """rois: CUDA float32 [R,5]; packed: pack_roidb's; im_scale: the image's scale (float32).  -> dict of padded
+        device buffers: rois [B,5], labels int64 [B], bbox_targets / bbox_inside_weights / bbox_outside_weights [B,4K],
+        nongt_inds int64 [B] (-1 past its count), roi_has_mask uint8 [B], mask_rois [C,5], mask_int32 float32
+        [C, K*M*M], with B = batch_rois and C = max(round(fg_fraction * B), 1).  self.counts: int32 [5] on the device
+        (fg rows, bg rows, mask rows, error, nongt_inds count).  seed=None draws one from np.random."""
+        require_cuda(rois)
+        rois = f32c(rois).reshape(-1, 5)
+        if seed is None:
+            seed = int(np.random.randint(np.iinfo(np.int64).max, dtype=np.int64))
+        dev = rois.device
+        R, B, K, M, C_ = rois.shape[0], self.batch_rois, self.K, self.M, self.mask_capacity
+        sz = C.c_size_t()
+        check(lib().upsnet_proposal_targets_workspace_bytes(R, packed.G, B, C.byref(sz)),
+              "proposal_targets_workspace_bytes")
+        ws = torch.empty(sz.value, dtype=torch.uint8, device=dev)
+        f = dict(device=dev, dtype=torch.float32)
+        out = dict(rois=torch.empty((B, 5), **f), labels=torch.empty(B, dtype=torch.int64, device=dev),
+                   bbox_targets=torch.empty((B, 4 * K), **f), bbox_inside_weights=torch.empty((B, 4 * K), **f),
+                   bbox_outside_weights=torch.empty((B, 4 * K), **f), mask_rois=torch.empty((C_, 5), **f),
+                   mask_int32=torch.empty((C_, K * M * M), **f),
+                   roi_has_mask=torch.empty(B, dtype=torch.uint8, device=dev),
+                   nongt_inds=torch.empty(B, dtype=torch.int64, device=dev))
+        counts = torch.empty(5, dtype=torch.int32, device=dev)
+        pk = packed
+        with torch.cuda.device(dev):
+            check(lib().upsnet_proposal_targets(
+                ptr(rois) if R else None, R, ptr(pk.boxes), ptr(pk.gt_max), ptr(pk.gt_maxcls), ptr(pk.gt_classes),
+                ptr(pk.gt_map), pk.G, ptr(pk.obj_boxes), ptr(pk.obj_poly), ptr(pk.poly_vert), ptr(pk.verts), pk.O,
+                float(np.float32(im_scale)), K, B, self.fg_per_image, self.fg_thresh, self.bg_hi, self.bg_lo,
+                *self.weights, int(self.cls_agnostic), M, int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(out["rois"]),
+                ptr(out["labels"]), ptr(out["bbox_targets"]), ptr(out["bbox_inside_weights"]),
+                ptr(out["bbox_outside_weights"]), ptr(out["nongt_inds"]), ptr(out["mask_rois"]),
+                ptr(out["mask_int32"]), ptr(out["roi_has_mask"]), ptr(counts), ptr(ws), ws.numel(),
+                stream_ptr(dev)), "proposal_targets")
+        self.counts = counts
+        return out
+
+    NAMES = ("rois", "labels", "bbox_targets", "bbox_inside_weights", "bbox_outside_weights", "mask_rois", "mask_int32",
+             "roi_has_mask", "nongt_inds")
+
+    def from_roidb(self, rois, entry, im_info, seed=None):
+        """Drop-in for ProposalMaskTarget.forward(rois, roidb, im_info) on one image: its nine tensors (rois, labels
+        int64, bbox_targets, the inside / outside weights, mask_rois, mask_int32 float32 [n_mask, K*M*M], roi_has_mask
+        uint8, nongt_inds int64) as views of the device buffers.  One synchronisation, to read the counts."""
+        im_scale = np.float32(np.asarray(im_info.cpu() if torch.is_tensor(im_info) else im_info).reshape(-1, 3)[0, 2])
+        out = self(rois, self.pack_roidb(entry, rois.device), im_scale, seed)
+        nf, nb, nm, err, nn = (int(v) for v in self.counts.cpu())
+        if err:
+            raise _lib.UpsnetError("proposal_targets: no fg and no bg rois (the reference raises IndexError)")
+        n = nf + nb
+        sl = dict(rois=n, labels=n, bbox_targets=n, bbox_inside_weights=n, bbox_outside_weights=n, mask_rois=nm,
+                  mask_int32=nm, roi_has_mask=n, nongt_inds=nn)
+        return tuple(out[k][:sl[k]] for k in self.NAMES)
