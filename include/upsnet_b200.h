@@ -616,6 +616,66 @@ int upsnet_proposal_targets(const float *rois, int R, const float *gt_boxes, con
                             unsigned char *roi_has_mask, int *counts, void *workspace, size_t workspace_bytes,
                             void *stream);
 
+/* ---------------------------------------------------------------------------------------
+ * upsnet_panoptic_loss_forward / _backward: the panoptic head of the training forward of one image, fused.
+ * replaces: models/resnet_upsnet.py:156-179 and 250-257: the class gather of mask_score, SegTerm and MaskTerm
+ *           (operators/modules/unary_logits.py:24-105), the void logits, torch.cat, MaskMatching
+ *           (operators/modules/mask_matching.py:37-58), calc_panoptic_acc and
+ *           CrossEntropyLoss(ignore_index=255, reduce=False)(...).mean(), with autograd's backward of that composition.
+ *           No [1,k,h,w] plane is built; backward keeps 8 bytes per pixel.
+ * Inputs (device): fcn_score float32 [S,h,w]; mask_score float32 [k,C,M,M], C == num_classes or C == 1 (already
+ *   gathered); gt_rois float32 [k,5] = (0,x1,y1,x2,y2); cls_idx int64 [k] (a value outside 0..num_classes-1 is treated
+ *   as 0); seg_gt int64 [h,w]; mask_gt [G,h,w], uint8 or int64 (mask_gt_is_int64); keep_inds int64 [k] or NULL (then
+ *   G == k; an index outside 0..G-1 paints nothing).  num_stuff = S - num_classes + 1; thing class c is seg channel
+ *   T(c) = num_stuff + c - 1.
+ * Channels at a pixel: 0..num_stuff-1 = fcn_score; num_stuff + i = seg_i + mask_i; with enable_void a last channel
+ *   max over t >= num_stuff of fcn_score[t], minus max over i of seg_i (the zeros outside the windows take part).
+ *   seg_i = fcn_score[T(cls_i)] inside SegTerm's window, else 0: with b = float32(roi) * box_scale,
+ *     [int(b.y1), int(rint(b.y2) + 1)) x [int(b.x1), int(rint(b.x2) + 1)), rint = half to even, bounds clamped to the
+ *     image (a negative bound is clamped to 0, where the reference's slice would wrap around); empty for class 0.
+ *   mask_i = mask_score[i, cls_i] (channel 0 when C == 1) resized to (bh,bw) = (max(r.y2-r.y1+1,1), max(r.x2-r.x1+1,1)),
+ *     r = trunc(b), by ATen's bilinear rule (align_corners = False: src = max(scale * (dst + 0.5) - 0.5, 0) with
+ *     scale = M / bw in float32, second tap min(i0 + 1, M - 1)), pasted at (r.y1, r.x1), cropped to the image, else 0.
+ * Ground truth at a pixel: seg_gt where it is <= S - num_classes or >= 255, else -1; then num_stuff + j for the last j
+ *   with mask_gt[keep_inds[j]] (mask_gt[j] without keep_inds) neither 0 nor 255; what is still -1 becomes num_stuff + k
+ *   with keep_inds, 255 without.  A value that is neither a channel nor 255 (the reference's cross-entropy raises on
+ *   it) gives no loss and no gradient and is never counted correct.
+ * Outputs (device): loss[1] = sum of (log-sum-exp - logit of the ground-truth channel) over the pixels whose ground
+ *   truth is not 255, divided by h*w; accuracy[1] = counts[0] / (h*w - counts[1]); counts int32 [2] = pixels whose
+ *   arg-max channel (ties: the lowest) equals the ground truth, pixels whose ground truth is 255; lse float32 [h*w] and
+ *   gt_channel int32 [h*w] are what backward reads.  When every pixel is 255 the accuracy is 0 / 0 (the reference
+ *   asserts there).
+ * Backward: grad_out float32 [1] on the device; d_fcn_score float32 [S,h,w] (every element written) and d_mask_score
+ *   float32 [k,C,M,M] (zero outside the selected channel); either may be NULL.  With p = softmax and
+ *   g_c = (p_c - [c == gt]) * grad_out / (h*w) on the pixels with a loss: stuff channels get g_c; T(c) gets the g of
+ *   the instances of class c whose SegTerm window covers the pixel, + g_void on the arg-max thing channel, - g_void on
+ *   the channel of the instance that wins max_i seg_i (nothing when a zero wins); d_mask_score is the transpose of the
+ *   resize-and-paste applied to g_{num_stuff+i}, computed as a gather.
+ * Same inputs give the same bytes (no atomics); no call synchronises or reads the device; both are capturable.
+ * Limits: M <= 32, S*h*w < 2^31, k*C*M*M < 2^31 (else UPSNET_E_UNSUPPORTED); k >= 1.
+ * Workspace: upsnet_panoptic_loss_workspace_bytes(k, h, w), for either call; nothing in it outlives the call. */
+int upsnet_panoptic_loss_workspace_bytes(int k, int h, int w, size_t *bytes);
+int upsnet_panoptic_loss_forward(const float *fcn_score, int S, int h, int w, const float *mask_score, int k, int C,
+                                 int mask_size, const float *gt_rois, const int64_t *cls_idx, const int64_t *seg_gt,
+                                 const void *mask_gt, int mask_gt_is_int64, int G, const int64_t *keep_inds,
+                                 int num_classes, int enable_void, float box_scale, float *loss, float *accuracy,
+                                 int *counts, float *lse, int *gt_channel, void *workspace, size_t workspace_bytes,
+                                 void *stream);
+int upsnet_panoptic_loss_backward(const float *fcn_score, int S, int h, int w, const float *mask_score, int k, int C,
+                                  int mask_size, const float *gt_rois, const int64_t *cls_idx, int num_classes,
+                                  int enable_void, float box_scale, const float *lse, const int *gt_channel,
+                                  const float *grad_out, float *d_fcn_score, float *d_mask_score, void *workspace,
+                                  size_t workspace_bytes, void *stream);
+
+/* upsnet_panoptic_gt: the ground-truth rule above alone (MaskMatching.forward), as the int64 [h,w] map the reference
+ * returns; k counts keep_inds and is ignored without them. */
+int upsnet_panoptic_gt(const int64_t *seg_gt, const void *mask_gt, int mask_gt_is_int64, int G, const int64_t *keep_inds,
+                       int k, int h, int w, int num_seg_classes, int num_classes, int64_t *panoptic_gt, void *stream);
+
+/* upsnet_draw_keys: keys[p] = the draw key of candidate position p = 0..n-1 (the rule of upsnet_rpn_targets: stream_id
+ * 0 is its fg draw, 1 its bg draw), so that a host restatement of the rule can be compared with the device's. */
+int upsnet_draw_keys(unsigned long long seed, int stream_id, int n, unsigned long long *keys, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

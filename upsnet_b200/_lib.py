@@ -104,6 +104,12 @@ def lib():
         L.upsnet_proposal_targets_workspace_bytes.argtypes = [i, i, i, C.POINTER(sz)]
         L.upsnet_proposal_targets.argtypes = [vp, i] + [vp] * 5 + [i] + [vp] * 4 + [i, f, i, i, i] + [f] * 7 + \
             [i, i, C.c_ulonglong] + [vp] * 11 + [sz, vp]
+        L.upsnet_panoptic_loss_workspace_bytes.argtypes = [i, i, i, C.POINTER(sz)]
+        L.upsnet_panoptic_loss_forward.argtypes = [vp, i, i, i, vp, i, i, i, vp, vp, vp, vp, i, i, vp, i, i, f] + \
+            [vp] * 6 + [sz, vp]
+        L.upsnet_panoptic_loss_backward.argtypes = [vp, i, i, i, vp, i, i, i, vp, vp, i, i, f] + [vp] * 6 + [sz, vp]
+        L.upsnet_panoptic_gt.argtypes = [vp, vp, i, i, vp, i, i, i, i, i, vp, vp]
+        L.upsnet_draw_keys.argtypes = [C.c_ulonglong, i, i, vp, vp]
         _lib = L
     return _lib
 
@@ -124,6 +130,8 @@ EXPORTED_SYMBOLS = [
     "upsnet_combined_pan_workspace_bytes", "upsnet_combined_pan_result",
     "upsnet_rpn_targets_workspace_bytes", "upsnet_rpn_targets",
     "upsnet_proposal_targets_workspace_bytes", "upsnet_proposal_targets",
+    "upsnet_panoptic_loss_workspace_bytes", "upsnet_panoptic_loss_forward", "upsnet_panoptic_loss_backward",
+    "upsnet_panoptic_gt", "upsnet_draw_keys",
 ]
 
 

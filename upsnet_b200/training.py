@@ -15,10 +15,13 @@
 * ProposalTargets: the Mask R-CNN proposal targets of one image (operators/modules/proposal_mask_target.py, run by the
   reference on the host in the middle of the forward) on the device (csrc/proposal_target.cu): roi sampling, box
   targets and the class-specific polygon mask targets.
+* PanopticLoss: the panoptic head of the training forward (models/resnet_upsnet.py:144-179: SegTerm, MaskTerm, the void
+  logits, MaskMatching, calc_panoptic_acc and the cross-entropy) as one fused loss with hand-written forward and
+  backward kernels (csrc/panoptic_loss.cu), plus the two host helpers for the lines before it (gt_rois, draw_keep).
 
-Scope note: this is the operator / communication layer of the training configuration plus the RPN and proposal targets.
-Losses and the optimiser are plain torch in the reference and stay that way; the dense backward convolutions are
-library calls.
+Scope note: this is the operator / communication layer of the training configuration plus the RPN and proposal targets
+and the panoptic loss.  The other losses (RPN, RCNN, mask, semantic) and the optimiser are library calls on dense
+tensors in the reference and stay that way; the dense backward convolutions are library calls.
 """
 import ctypes as C
 
@@ -497,3 +500,185 @@ class ProposalTargets:
         sl = dict(rois=n, labels=n, bbox_targets=n, bbox_inside_weights=n, bbox_outside_weights=n, mask_rois=nm,
                   mask_int32=nm, roi_has_mask=n, nongt_inds=nn)
         return tuple(out[k][:sl[k]] for k in self.NAMES)
+
+
+# ------------------------------------------------------------------------------------------------
+# panoptic head loss
+# ------------------------------------------------------------------------------------------------
+_GAMMA = np.uint64(0x9E3779B97F4A7C15)
+
+
+def _splitmix64(x):
+    with np.errstate(over="ignore"):
+        z = x + _GAMMA
+        z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        return z ^ (z >> np.uint64(31))
+
+
+def draw_keys(seed, n):
+    """uint64 [n]: the key of every candidate position of a draw, csrc/targets.cuh draw_key on stream 0."""
+    with np.errstate(over="ignore"):
+        return _splitmix64(np.uint64(int(seed) & 0xFFFFFFFFFFFFFFFF) ^ (np.arange(n, dtype=np.uint64) * _GAMMA))
+
+
+def draw_keep(G, fraction, seed=None):
+    """The keep_inds draw of models/resnet_upsnet.py:149, np.random.choice(G, max(int(G * fraction), 1), replace=False),
+    by the seeded rule of the target classes: the positions with the smallest draw_keys(seed, G), in ascending key
+    order (int64).  seed=None draws one from np.random, so np.random.seed governs it."""
+    if G <= 0:
+        raise _lib.UpsnetError("draw_keep: no ground-truth boxes")
+    if seed is None:
+        seed = int(np.random.randint(np.iinfo(np.int64).max, dtype=np.int64))
+    size = max(int(G * fraction), 1)
+    return np.argsort(draw_keys(seed, G), kind="stable")[:size].astype(np.int64)
+
+
+def gt_rois(entry, im_scale, device):
+    """get_gt_rois (models/resnet_upsnet.py:287-291) of one roidb entry: the non-crowd boxes of a class > 0 times the
+    float32 im_scale (im_info[0, 2]) as float32 [n,5] rows (0, x1, y1, x2, y2), and their classes (int64 [n]), on
+    `device`."""
+    inds = np.where((entry["gt_classes"] > 0) & (entry["is_crowd"] == 0))[0]
+    boxes = (np.asarray(entry["boxes"], np.float32)[inds] * np.float32(im_scale)).astype(np.float32)
+    rois = np.hstack((np.zeros((boxes.shape[0], 1), np.float32), boxes.reshape(-1, 4)))
+    cls = np.asarray(entry["gt_classes"])[inds].astype(np.int64)
+    return torch.from_numpy(rois).to(device), torch.from_numpy(cls).to(device)
+
+
+def _pl_workspace(k, h, w, dev):
+    sz = C.c_size_t()
+    check(lib().upsnet_panoptic_loss_workspace_bytes(k, h, w, C.byref(sz)), "panoptic_loss_workspace_bytes")
+    return torch.empty(sz.value, dtype=torch.uint8, device=dev)
+
+
+class PanopticLossFunction(torch.autograd.Function):
+    """(loss, accuracy, counts) = the fused panoptic loss (include/upsnet_b200.h, upsnet_panoptic_loss_forward);
+    differentiable in fcn_score and mask_score.  Inputs are validated by PanopticLoss.forward."""
+
+    @staticmethod
+    def forward(ctx, fcn_score, mask_score, gt_rois, cls_idx, seg_gt, mask_gt, keep_inds, num_classes, enable_void,
+                box_scale, mask_size):
+        dev = fcn_score.device
+        _, S, h, w = fcn_score.shape
+        k, Cm = mask_score.shape[0], mask_score.shape[1]
+        fcn, msk = f32c(fcn_score.detach()), f32c(mask_score.detach())
+        loss, acc = (torch.empty((), dtype=torch.float32, device=dev) for _ in range(2))
+        counts = torch.empty(2, dtype=torch.int32, device=dev)
+        lse = torch.empty(h * w, dtype=torch.float32, device=dev)
+        gtc = torch.empty(h * w, dtype=torch.int32, device=dev)
+        ws = _pl_workspace(k, h, w, dev)
+        with torch.cuda.device(dev):
+            check(lib().upsnet_panoptic_loss_forward(
+                ptr(fcn), S, h, w, ptr(msk), k, Cm, mask_size, ptr(gt_rois), ptr(cls_idx), ptr(seg_gt), ptr(mask_gt),
+                int(mask_gt.dtype == torch.int64), mask_gt.shape[0], ptr(keep_inds), num_classes, int(enable_void),
+                box_scale, ptr(loss), ptr(acc), ptr(counts), ptr(lse), ptr(gtc), ptr(ws), ws.numel(),
+                stream_ptr(dev)), "panoptic_loss_forward")
+        ctx.save_for_backward(fcn, msk, gt_rois, cls_idx, lse, gtc)
+        ctx.cfg = (num_classes, int(enable_void), box_scale, mask_size)
+        ctx.mark_non_differentiable(acc, counts)
+        return loss, acc, counts
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_acc, _grad_counts):
+        fcn, msk, rois, cls, lse, gtc = ctx.saved_tensors
+        num_classes, enable_void, box_scale, mask_size = ctx.cfg
+        dev = fcn.device
+        _, S, h, w = fcn.shape
+        k, Cm = msk.shape[0], msk.shape[1]
+        go = f32c(grad_loss).reshape(1)
+        dfcn = torch.empty_like(fcn) if ctx.needs_input_grad[0] else None
+        dmsk = torch.empty_like(msk) if ctx.needs_input_grad[1] else None
+        if dfcn is not None or dmsk is not None:
+            ws = _pl_workspace(k, h, w, dev)
+            with torch.cuda.device(dev):
+                check(lib().upsnet_panoptic_loss_backward(
+                    ptr(fcn), S, h, w, ptr(msk), k, Cm, mask_size, ptr(rois), ptr(cls), num_classes, enable_void,
+                    box_scale, ptr(lse), ptr(gtc), ptr(go), ptr(dfcn), ptr(dmsk), ptr(ws), ws.numel(),
+                    stream_ptr(dev)), "panoptic_loss_backward")
+        return (dfcn, dmsk) + (None,) * 9
+
+
+class PanopticLoss(torch.nn.Module):
+    """The panoptic head of the training forward of one image (models/resnet_upsnet.py:156-179, 250-257) as one fused,
+    parameter-free loss: the class gather of mask_score, SegTerm, MaskTerm, the void logits, MaskMatching, the
+    cross-entropy (ignore 255, mean over all pixels) and calc_panoptic_acc, without building a [1,k,h,w] plane and
+    without a host read.  Built from the reference's `config` (dataset.num_seg_classes / num_classes,
+    network.mask_size, enable_void = train.panoptic_box_keep_fraction < 1) or from the same values as keywords.
+
+    Ground-truth boxes are never negative; a negative SegTerm bound is clamped to 0 here, where the reference's Python
+    slice would wrap around, so no parity is claimed for such boxes.  The same inputs give the same bytes."""
+
+    def __init__(self, config=None, *, num_seg_classes=None, num_classes=None, enable_void=True, box_scale=1 / 4.0,
+                 mask_size=28):
+        super().__init__()
+        if config is not None:
+            num_seg_classes, num_classes = config.dataset.num_seg_classes, config.dataset.num_classes
+            mask_size = config.network.mask_size
+            enable_void = config.train.panoptic_box_keep_fraction < 1
+        if num_seg_classes is None or num_classes is None:
+            raise _lib.UpsnetError("panoptic_loss: num_seg_classes and num_classes are required")
+        self.num_seg_classes, self.num_classes = int(num_seg_classes), int(num_classes)
+        self.enable_void, self.box_scale, self.mask_size = bool(enable_void), float(box_scale), int(mask_size)
+        self.counts = None
+
+    @staticmethod
+    def _labels(seg_gt_4x, mask_gt, keep_inds):
+        """-> (seg int64 [1,h,w], mask_gt uint8 / int64 [G,h,w], keep_inds int64 on the device or None), checked."""
+        require_cuda(seg_gt_4x, mask_gt)
+        if seg_gt_4x.dim() != 3 or seg_gt_4x.shape[0] != 1:
+            raise _lib.UpsnetError("panoptic_loss: seg_gt_4x must be [1,h,w] (one image)")
+        if mask_gt.dim() != 3 or mask_gt.shape[0] == 0 or mask_gt.shape[1:] != seg_gt_4x.shape[1:]:
+            raise _lib.UpsnetError("panoptic_loss: mask_gt must be [G,h,w] with G >= 1 and the size of seg_gt_4x")
+        if mask_gt.dtype not in (torch.uint8, torch.int64):
+            raise _lib.UpsnetError("panoptic_loss: mask_gt must be uint8 or int64")
+        if keep_inds is not None:
+            if not torch.is_tensor(keep_inds) or not keep_inds.is_cuda:
+                host = np.asarray(keep_inds.cpu() if torch.is_tensor(keep_inds) else keep_inds).astype(np.int64).reshape(-1)
+                if host.size == 0 or host.min() < 0 or host.max() >= mask_gt.shape[0]:
+                    raise _lib.UpsnetError("panoptic_loss: keep_inds must index mask_gt")
+                keep_inds = torch.from_numpy(host).to(mask_gt.device)
+            keep_inds = keep_inds.to(torch.int64).reshape(-1).contiguous()
+        return seg_gt_4x.to(torch.int64).contiguous(), mask_gt.contiguous(), keep_inds
+
+    def panoptic_gt(self, seg_gt_4x, mask_gt, keep_inds=None):
+        """MaskMatching.forward: the int64 [1,h,w] ground truth of the panoptic logits."""
+        seg, mgt, keep = self._labels(seg_gt_4x, mask_gt, keep_inds)
+        out = torch.empty_like(seg)
+        _, h, w = seg.shape
+        with torch.cuda.device(seg.device):
+            check(lib().upsnet_panoptic_gt(ptr(seg), ptr(mgt), int(mgt.dtype == torch.int64), mgt.shape[0], ptr(keep),
+                                           0 if keep is None else keep.numel(), h, w, self.num_seg_classes,
+                                           self.num_classes, ptr(out), stream_ptr(seg.device)), "panoptic_gt")
+        return out
+
+    def forward(self, fcn_score, mask_score, gt_rois, cls_idx, seg_gt_4x, mask_gt, keep_inds=None):
+        """fcn_score [1,S,h,w]; mask_score [k,C,M,M] with C = num_classes (the mask branch's output on gt_rois) or 1
+        (already gathered); gt_rois [k,5] and cls_idx [k], after keep_inds when there is a draw; seg_gt_4x [1,h,w];
+        mask_gt [G,h,w] uint8 or int64; keep_inds [k] (tensor or numpy) or None.  -> (loss, accuracy), 0-dim device
+        tensors; self.counts: int32 [2] on the device (correct pixels, ignored pixels)."""
+        E = _lib.UpsnetError
+        require_cuda(fcn_score, mask_score, gt_rois, cls_idx)
+        if self.enable_void != (keep_inds is not None):
+            raise E("panoptic_loss: enable_void goes with keep_inds (the reference sets the two together)")
+        if fcn_score.dim() != 4 or fcn_score.shape[0] != 1:
+            raise E("panoptic_loss: only batch size 1 (fcn_score [1,S,h,w])")
+        if fcn_score.shape[1] != self.num_seg_classes:
+            raise E("panoptic_loss: fcn_score has %d channels, not num_seg_classes" % fcn_score.shape[1])
+        k = mask_score.shape[0]
+        if k == 0:
+            raise E("panoptic_loss: no ground-truth boxes")
+        M = self.mask_size
+        if mask_score.dim() != 4 or mask_score.shape[1] not in (1, self.num_classes) or tuple(mask_score.shape[2:]) != (M, M):
+            raise E("panoptic_loss: mask_score must be [k,num_classes,%d,%d] or [k,1,%d,%d]" % (M, M, M, M))
+        if tuple(gt_rois.shape) != (k, 5) or cls_idx.numel() != k:
+            raise E("panoptic_loss: gt_rois must be [k,5] and cls_idx [k], k = mask_score.shape[0]")
+        seg, mgt, keep = self._labels(seg_gt_4x, mask_gt, keep_inds)
+        if seg.shape[1:] != fcn_score.shape[2:]:
+            raise E("panoptic_loss: seg_gt_4x and fcn_score differ in size")
+        if (keep.numel() if keep is not None else mgt.shape[0]) != k:
+            raise E("panoptic_loss: one ground-truth mask per box (keep_inds, or all of mask_gt, must have k entries)")
+        loss, acc, counts = PanopticLossFunction.apply(
+            fcn_score, mask_score, f32c(gt_rois), cls_idx.to(torch.int64).reshape(-1).contiguous(), seg, mgt, keep,
+            self.num_classes, self.enable_void, self.box_scale, M)
+        self.counts = counts
+        return loss, acc
