@@ -676,6 +676,31 @@ int upsnet_panoptic_gt(const int64_t *seg_gt, const void *mask_gt, int mask_gt_i
  * 0 is its fg draw, 1 its bg draw), so that a host restatement of the rule can be compared with the device's. */
 int upsnet_draw_keys(unsigned long long seed, int stream_id, int n, unsigned long long *keys, void *stream);
 
+/* ---- panoptic training labels (labels.cu) ----
+ * upsnet_training_labels: the label maps of one training image (the label block of the reference's Cityscapes / COCO
+ * loaders and collate / gt_list_to_blob) from its uint8 label map [h0,w0]:
+ *   seg_gt     int64 [Hs,Ws]     = label[seg_rows[y], seg_cols[x]]
+ *   seg_gt_4x  int64 [Hq,Wq]     = label[q_rows[y], q_cols[x]]
+ *   seg_roi_gt int64 [n_roi,M,M] = label[roi_rows[i*M + y], roi_cols[i*M + x]]
+ *   mask_gt    uint8 or int64 [G,Hm,Wm] = 1 where canvas pixel (m_rows[y], m_cols[x]) is set by Pillow's polygon fill
+ *              (ImageDraw.polygon(outline=1, fill=1)) of any polygon of instance g, else 0
+ * Every table is int32 and host-built (cv2 INTER_NEAREST composed through each resize, the flip folded into the
+ * label-map columns); -1 marks padding, written as 255.  m_cols is non-decreasing on its non-negative entries.
+ * Polygons: instance g owns polygons [obj_poly[g], obj_poly[g+1]), polygon p the int32 (x, y) vertex pairs
+ * [poly_vert[p], poly_vert[p+1]) of verts, already truncated toward zero as Pillow does; obj_yrange[2g..2g+1] is the
+ * instance's lowest and highest vertex y.  max_poly_verts / max_obj_verts are the largest vertex counts of one polygon
+ * and of one instance: above the limits below, or G above UPSNET_LABELS_MAX_G, the call returns UPSNET_E_UNSUPPORTED
+ * before any launch.  One owner thread per output element, no atomics: the same inputs give the same bytes. */
+#define UPSNET_LABELS_MAX_POLY_VERTS 1024
+#define UPSNET_LABELS_MAX_OBJ_VERTS 1536
+#define UPSNET_LABELS_MAX_G 65535
+int upsnet_training_labels(const unsigned char* label, int h0, int w0, const int* seg_rows, int Hs, const int* seg_cols,
+                           int Ws, int64_t* seg_gt, const int* q_rows, int Hq, const int* q_cols, int Wq,
+                           int64_t* seg_gt_4x, const int* m_rows, int Hm, const int* m_cols, int Wm, const int* obj_poly,
+                           const int* poly_vert, const int* verts, const int* obj_yrange, int G, int max_poly_verts,
+                           int max_obj_verts, void* mask_gt, int mask_gt_is_int64, const int* roi_rows,
+                           const int* roi_cols, int n_roi, int M, int64_t* seg_roi_gt, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -110,6 +110,8 @@ def lib():
         L.upsnet_panoptic_loss_backward.argtypes = [vp, i, i, i, vp, i, i, i, vp, vp, i, i, f] + [vp] * 6 + [sz, vp]
         L.upsnet_panoptic_gt.argtypes = [vp, vp, i, i, vp, i, i, i, i, i, vp, vp]
         L.upsnet_draw_keys.argtypes = [C.c_ulonglong, i, i, vp, vp]
+        L.upsnet_training_labels.argtypes = [vp, i, i, vp, i, vp, i, vp, vp, i, vp, i, vp, vp, i, vp, i] + [vp] * 4 + \
+            [i, i, i, vp, i, vp, vp, i, i, vp, vp]
         _lib = L
     return _lib
 
@@ -131,7 +133,7 @@ EXPORTED_SYMBOLS = [
     "upsnet_rpn_targets_workspace_bytes", "upsnet_rpn_targets",
     "upsnet_proposal_targets_workspace_bytes", "upsnet_proposal_targets",
     "upsnet_panoptic_loss_workspace_bytes", "upsnet_panoptic_loss_forward", "upsnet_panoptic_loss_backward",
-    "upsnet_panoptic_gt", "upsnet_draw_keys",
+    "upsnet_panoptic_gt", "upsnet_draw_keys", "upsnet_training_labels",
 ]
 
 

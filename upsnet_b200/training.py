@@ -15,6 +15,8 @@
 * ProposalTargets: the Mask R-CNN proposal targets of one image (operators/modules/proposal_mask_target.py, run by the
   reference on the host in the middle of the forward) on the device (csrc/proposal_target.cu): roi sampling, box
   targets and the class-specific polygon mask targets.
+* PanopticLabels: the label maps of the semantic and panoptic heads (seg_gt, seg_gt_4x, mask_gt, seg_roi_gt), built by
+  the reference's data loaders on the host, on the device (csrc/labels.cu), with Pillow's polygon fill restated.
 * PanopticLoss: the panoptic head of the training forward (models/resnet_upsnet.py:144-179: SegTerm, MaskTerm, the void
   logits, MaskMatching, calc_panoptic_acc and the cross-entropy) as one fused loss with hand-written forward and
   backward kernels (csrc/panoptic_loss.cu), plus the two host helpers for the lines before it (gt_rois, draw_keep).
@@ -355,6 +357,40 @@ class RPNTargets:
 # ------------------------------------------------------------------------------------------------
 # Mask R-CNN proposal targets
 # ------------------------------------------------------------------------------------------------
+def pack_polygons(segms, rows, what):
+    """The polygon layout shared by ProposalTargets.pack_roidb and PanopticLabels.pack_roidb: segms[i] for i in rows,
+    each a non-empty list of flat [x0, y0, x1, y1, ...] polygons of >= 6 coordinates (dict / RLE segmentations are
+    rejected).  -> (obj_poly int32 [n+1]: first polygon of each object, poly_vert int32 [P+1]: first vertex of each
+    polygon, per object the list of its float64 polygons)."""
+    obj_off, poly_off, polys = [0], [0], []
+    for i in rows:
+        segm = segms[i]
+        if not isinstance(segm, list) or not segm:
+            raise _lib.UpsnetError("%s: segmentation %d is not a polygon list" % (what, i))
+        ps = [np.asarray(p, np.float64) for p in segm]
+        if any(p.ndim != 1 or p.size < 6 or p.size % 2 for p in ps):
+            raise _lib.UpsnetError("%s: polygon of segmentation %d has an odd or < 6 coordinates" % (what, i))
+        for p in ps:
+            poly_off.append(poly_off[-1] + p.size // 2)
+        obj_off.append(obj_off[-1] + len(ps))
+        polys.append(ps)
+    return np.asarray(obj_off, np.int32), np.asarray(poly_off, np.int32), polys
+
+
+def _upload_parts(arrays, device):
+    """[(name, array, dtype)] -> (one int32 device buffer with every part 16-byte aligned, {name: (offset, size,
+    dtype)})."""
+    parts, chunks, off = {}, [], 0
+    for name, a, dt in arrays:
+        a = np.ascontiguousarray(a, dt)
+        parts[name] = (off, a.size, dt)
+        chunks.append(a.view(np.int32))
+        pad = (-a.size) % 4
+        chunks.append(np.zeros(pad, np.int32))
+        off += a.size + pad
+    return torch.from_numpy(np.concatenate(chunks)).to(device), parts
+
+
 class PackedGT:
     """The ground truth of one roidb entry on the device (ProposalTargets.pack_roidb): views of one int32 upload."""
 
@@ -413,37 +449,21 @@ class ProposalTargets:
         if obj.size == 0:
             # add_rpn_blobs fails on such an image in the reference, and RPNTargets.from_roidb raises there too
             raise _lib.UpsnetError("proposal_targets: no non-crowd ground truth")
-        obj_boxes, obj_off, poly_off, verts = [], [0], [0], []
-        for i in obj:
-            segm = entry["segms"][i]
-            if not isinstance(segm, list) or not segm:
-                raise _lib.UpsnetError("proposal_targets: segmentation %d is not a polygon list" % i)
-            ps = [np.asarray(p, np.float32) for p in segm]
-            if any(p.ndim != 1 or p.size < 6 or p.size % 2 for p in ps):
-                raise _lib.UpsnetError("proposal_targets: polygon of segmentation %d has an odd or < 6 coordinates" % i)
+        obj_off, poly_off, polys = pack_polygons(entry["segms"], obj, "proposal_targets")
+        obj_boxes, verts = [], []
+        for ps in polys:
+            ps = [p.astype(np.float32) for p in ps]
             allp = np.concatenate(ps)
             obj_boxes.append([allp[0::2].min(), allp[1::2].min(), allp[0::2].max(), allp[1::2].max()])
-            for p in ps:
-                verts.append(p)
-                poly_off.append(poly_off[-1] + p.size // 2)
-            obj_off.append(obj_off[-1] + len(ps))
+            verts.extend(ps)
         f32 = np.float32
         arrays = [("boxes", boxes.ravel(), f32), ("gt_max", ov.max(1).astype(f32), f32),
                   ("gt_maxcls", ov.argmax(1).astype(np.int32), np.int32), ("gt_classes", cls.astype(np.int32), np.int32),
                   ("gt_map", b2g.astype(np.int32), np.int32),
                   ("obj_boxes", np.asarray(obj_boxes, f32).ravel(), f32),
-                  ("obj_poly", np.asarray(obj_off, np.int32), np.int32),
-                  ("poly_vert", np.asarray(poly_off, np.int32), np.int32),
+                  ("obj_poly", obj_off, np.int32), ("poly_vert", poly_off, np.int32),
                   ("verts", np.concatenate(verts).astype(f32), f32)]
-        parts, chunks, off = {}, [], 0
-        for name, a, dt in arrays:
-            a = np.ascontiguousarray(a, dt)
-            parts[name] = (off, a.size, dt)
-            chunks.append(a.view(np.int32))
-            pad = (-a.size) % 4                     # 16-byte aligned parts
-            chunks.append(np.zeros(pad, np.int32))
-            off += a.size + pad
-        buf = torch.from_numpy(np.concatenate(chunks)).to(device)
+        buf, parts = _upload_parts(arrays, device)
         return PackedGT(buf, parts, G, len(obj))
 
     def __call__(self, rois, packed, im_scale, seed=None):
@@ -682,3 +702,192 @@ class PanopticLoss(torch.nn.Module):
             self.num_classes, self.enable_void, self.box_scale, M)
         self.counts = counts
         return loss, acc
+
+
+# ------------------------------------------------------------------------------------------------
+# panoptic training labels
+# ------------------------------------------------------------------------------------------------
+def _nearest(n, fx, n_out=None):
+    """cv2.resize(INTER_NEAREST) source indices along an axis of length n: by a scale fx (output cvRound(n * fx)), or
+    to a size n_out (cv2's scale is then n_out / n in double)."""
+    from .operators import label_restore_index
+    if n_out is None:
+        n_out = int(np.rint(n * fx))
+    else:
+        fx = n_out / float(n)
+    if n_out == n:                      # cv2.resize copies when the size does not change, whatever fx is
+        return np.arange(n, dtype=np.int32)
+    return label_restore_index(n_out, fx, n).astype(np.int32)
+
+
+def _pad_table(t, n):
+    out = np.full(n, -1, np.int32)
+    out[:len(t)] = t
+    return out
+
+
+class PackedLabels:
+    """One roidb entry's instance polygons on the device (PanopticLabels.pack_roidb): views of one int32 upload, plus
+    the host-side boxes of seg_roi_gt and the vertex counts the limits are checked against."""
+
+    def __init__(self, buf, parts, G, roi_boxes, max_poly_verts, max_obj_verts):
+        self.buf, self.G, self.roi_boxes = buf, G, roi_boxes
+        self.max_poly_verts, self.max_obj_verts = max_poly_verts, max_obj_verts
+        for name, (off, n, _) in parts.items():
+            setattr(self, name, buf[off:off + n])
+
+
+class PanopticLabels:
+    """The label maps of the semantic and panoptic heads of one training image on the device: the label block of the
+    reference's loaders (dataset/cityscapes.py:166-189, dataset/coco.py:151-187) and collate / gt_list_to_blob
+    (dataset/base_dataset.py:925-976), bit-exact to them with Pillow 12.2 and cv2 4.13.
+
+    seg_gt / seg_gt_4x / seg_roi_gt are gathers from the uint8 label map through cv2 INTER_NEAREST index tables built
+    on the host (the flip folded into the columns); mask_gt evaluates Pillow's polygon fill only at the canvas pixels
+    the two nearest resizes sample (csrc/labels.cu).  Built from the reference's `config` (network.mask_size,
+    network.rpn_feat_stride[-2], train.fcn_with_roi_loss) or from the same values as keywords.  `dataset` selects the
+    loader: "cityscapes" draws every roidb row and sizes the canvas int(blob / scale); "coco" draws the non-crowd
+    rows, sizes it np.round(blob / scale), and keeps only non-crowd boxes for seg_roi_gt."""
+
+    def __init__(self, config=None, *, dataset="cityscapes", mask_size=28, with_roi=None, stride=32):
+        if dataset not in ("cityscapes", "coco"):
+            raise _lib.UpsnetError("panoptic_labels: dataset must be 'cityscapes' or 'coco'")
+        if config is not None:
+            mask_size, stride = config.network.mask_size, config.network.rpn_feat_stride[-2]
+            if with_roi is None:
+                with_roi = config.train.fcn_with_roi_loss
+        self.dataset, self.M, self.stride = dataset, int(mask_size), int(stride)
+        self.with_roi = bool(with_roi)
+
+    def _rows(self, entry):
+        cls = np.asarray(entry["gt_classes"])
+        crowd = np.asarray(entry["is_crowd"])
+        if self.dataset == "cityscapes":
+            return np.arange(len(cls)), np.where(cls > 0)[0]
+        return np.where(crowd == 0)[0], np.where((cls > 0) & (crowd == 0))[0]
+
+    def pack_roidb(self, entry, im_scale, device):
+        """One upload of the polygons drawn into mask_gt (ProposalTargets' layout, vertices truncated toward zero to
+        int32 as Pillow does), and the seg_roi_gt boxes np.around(boxes * im_scale).astype(int32) with the reference's
+        +1 for a degenerate side (host-side)."""
+        draw, roi_rows = self._rows(entry)
+        obj_off, poly_off, polys = pack_polygons(entry["segms"], draw, "panoptic_labels")
+        verts = [np.trunc(p).astype(np.int32) for ps in polys for p in ps]
+        yr = np.zeros((len(polys), 2), np.int32)
+        for g, ps in enumerate(polys):
+            ys = np.concatenate([np.trunc(p[1::2]) for p in ps])
+            yr[g] = (ys.min(), ys.max())
+        sizes = np.diff(poly_off)
+        per_obj = [int(sizes[obj_off[g]:obj_off[g + 1]].sum()) for g in range(len(polys))]
+        boxes = None
+        if self.with_roi:
+            boxes = np.around(np.asarray(entry["boxes"])[roi_rows] * float(im_scale)).astype(np.int32).reshape(-1, 4)
+            for b in boxes:
+                if b[3] == b[1]:
+                    b[3] += 1
+                if b[2] == b[0]:
+                    b[2] += 1
+        arrays = [("obj_poly", obj_off, np.int32), ("poly_vert", poly_off, np.int32),
+                  ("verts", np.concatenate(verts) if verts else np.zeros(2, np.int32), np.int32),
+                  ("obj_yrange", yr.ravel(), np.int32)]
+        buf, parts = _upload_parts(arrays, device)
+        return PackedLabels(buf, parts, len(polys), boxes, int(sizes.max()) if sizes.size else 0,
+                            max(per_obj) if per_obj else 0)
+
+    def tables(self, label_shape, packed, im_shape, im_scale, flipped):
+        """The int32 index tables of one call (host): {name: array} in label-map coordinates, -1 = padding, and the
+        output shapes.  Raises where the reference fails: a canvas whose resize is not the blob's size, an empty
+        seg_roi_gt crop."""
+        s, st = float(im_scale), self.stride
+        h0, w0 = label_shape
+        rows, cols = _nearest(h0, s), _nearest(w0, s)
+        if flipped:
+            cols = (w0 - 1 - cols).astype(np.int32)
+        h, w = len(rows), len(cols)
+        Hp, Wp = int(np.ceil(h / float(st)) * st), int(np.ceil(w / float(st)) * st)
+        qr, qc = _nearest(h, 0.25), _nearest(w, 0.25)
+        t = {"seg_rows": _pad_table(rows, Hp), "seg_cols": _pad_table(cols, Wp),
+             "q_rows": _pad_table(rows[qr], int(Hp * 0.25)), "q_cols": _pad_table(cols[qc], int(Wp * 0.25))}
+        Hb, Wb = (int(v) for v in im_shape)
+        if self.dataset == "cityscapes":
+            Hc, Wc = int(Hb / s), int(Wb / s)
+        else:
+            Hc, Wc = int(np.round(Hb / s)), int(np.round(Wb / s))
+        cr, cc = _nearest(Hc, s), _nearest(Wc, s)
+        if (len(cr), len(cc)) != (Hb, Wb):
+            raise _lib.UpsnetError("panoptic_labels: the %dx%d canvas resized by %r is %dx%d, not the blob's %dx%d"
+                                   % (Hc, Wc, s, len(cr), len(cc), Hb, Wb))
+        Hbp, Wbp = int(np.ceil(Hb / float(st)) * st), int(np.ceil(Wb / float(st)) * st)
+        t["m_rows"] = _pad_table(cr[_nearest(Hb, 0.25)], int(Hbp * 0.25))
+        t["m_cols"] = _pad_table(cc[_nearest(Wb, 0.25)], int(Wbp * 0.25))
+        n = 0
+        if self.with_roi:
+            b = packed.roi_boxes
+            n = len(b)
+            rr, rc = np.zeros((n, self.M), np.int32), np.zeros((n, self.M), np.int32)
+            ar, ac = np.arange(h), np.arange(w)
+            for i in range(n):
+                ys, xs = ar[b[i][1]:b[i][3]], ac[b[i][0]:b[i][2]]
+                if ys.size == 0 or xs.size == 0:
+                    raise _lib.UpsnetError("panoptic_labels: seg_roi_gt box %d crops nothing (cv2.resize raises)" % i)
+                rr[i] = rows[ys[_nearest(ys.size, None, self.M)]]
+                rc[i] = cols[xs[_nearest(xs.size, None, self.M)]]
+            t["roi_rows"], t["roi_cols"] = rr.ravel(), rc.ravel()
+        return t, n
+
+    def prepare(self, label_shape, packed, im_shape, im_scale, flipped, device):
+        """tables() uploaded in one copy: the device half of a call, so that `launch` issues kernels only (and can be
+        captured in a CUDA graph)."""
+        t, n = self.tables(label_shape, packed, im_shape, im_scale, flipped)
+        buf, parts = _upload_parts([(k, v, np.int32) for k, v in t.items()], device)
+        tab = {k: buf[off:off + m] for k, (off, m, _) in parts.items()}
+        tab["n_roi"], tab["label_shape"] = n, tuple(label_shape)
+        return tab
+
+    def launch(self, label_map, packed, tab, mask_dtype=torch.uint8):
+        """The kernels of one call on prepared tables; -> the dict of __call__."""
+        require_cuda(label_map)
+        if label_map.dim() != 2 or label_map.dtype != torch.uint8:
+            raise _lib.UpsnetError("panoptic_labels: label_map must be uint8 [h0,w0]")
+        if tuple(label_map.shape) != tab["label_shape"]:
+            raise _lib.UpsnetError("panoptic_labels: the tables were prepared for another label map size")
+        if mask_dtype not in (torch.uint8, torch.int64):
+            raise _lib.UpsnetError("panoptic_labels: mask_dtype must be uint8 or int64")
+        lab = label_map.contiguous()
+        dev = lab.device
+        n = tab["n_roi"]
+        Hs, Ws, Hq, Wq = (tab[k].numel() for k in ("seg_rows", "seg_cols", "q_rows", "q_cols"))
+        Hm, Wm, G = tab["m_rows"].numel(), tab["m_cols"].numel(), packed.G
+        out = {"seg_gt": torch.empty((1, Hs, Ws), dtype=torch.int64, device=dev),
+               "seg_gt_4x": torch.empty((1, Hq, Wq), dtype=torch.int64, device=dev),
+               "mask_gt": torch.empty((G, Hm, Wm), dtype=mask_dtype, device=dev)}
+        if self.with_roi:
+            out["seg_roi_gt"] = torch.empty((n, self.M, self.M), dtype=torch.int64, device=dev)
+        pk = packed
+        with torch.cuda.device(dev):
+            check(lib().upsnet_training_labels(
+                ptr(lab), lab.shape[0], lab.shape[1], ptr(tab["seg_rows"]), Hs, ptr(tab["seg_cols"]), Ws,
+                ptr(out["seg_gt"]), ptr(tab["q_rows"]), Hq, ptr(tab["q_cols"]), Wq, ptr(out["seg_gt_4x"]),
+                ptr(tab["m_rows"]), Hm, ptr(tab["m_cols"]), Wm, ptr(pk.obj_poly), ptr(pk.poly_vert), ptr(pk.verts),
+                ptr(pk.obj_yrange), G, pk.max_poly_verts, pk.max_obj_verts,
+                ptr(out["mask_gt"]) if G else None, int(mask_dtype == torch.int64),
+                ptr(tab["roi_rows"]) if n else None, ptr(tab["roi_cols"]) if n else None, n, self.M,
+                ptr(out["seg_roi_gt"]) if n else None, stream_ptr(dev)), "training_labels")
+        return out
+
+    def __call__(self, label_map, packed, im_shape, im_scale, flipped, mask_dtype=torch.uint8):
+        """label_map: CUDA uint8 [h0,w0] (the decoded label PNG, not flipped); packed: pack_roidb's; im_shape: the
+        resized image's (h, w) (get_image_blob); im_scale: im_scales[0], a Python float; flipped: the entry's flag.
+        -> dict of device tensors: seg_gt int64 [1,Hp,Wp], seg_gt_4x int64 [1,Hp/4,Wp/4], mask_gt mask_dtype (uint8
+        or int64; 0 / 1, 255 in the padding) [G,Hb_p/4,Wb_p/4], and seg_roi_gt int64 [n,M,M] when with_roi."""
+        require_cuda(label_map)
+        tab = self.prepare(tuple(label_map.shape), packed, im_shape, im_scale, flipped, label_map.device)
+        return self.launch(label_map, packed, tab, mask_dtype)
+
+    def from_roidb(self, entry, label_map, im_shape, im_scale, device):
+        """Drop-in for the loader's label block and collate: {'seg_gt', 'seg_gt_4x', 'mask_gt' (int64), and
+        'seg_roi_gt' when with_roi} with the reference's shapes and dtypes.  label_map: the decoded label PNG (uint8
+        numpy array or tensor), not flipped; the flip is entry['flipped']."""
+        lab = label_map if torch.is_tensor(label_map) else torch.from_numpy(np.ascontiguousarray(label_map, np.uint8))
+        packed = self.pack_roidb(entry, im_scale, device)
+        return self(lab.to(device), packed, im_shape, im_scale, bool(entry["flipped"]), mask_dtype=torch.int64)
