@@ -161,17 +161,33 @@ def test_fpn_level_thresholds_match_numpy():
     assert np.array_equal(O.fpn_level(rois), O.fpn_level_numpy(rois))
 
 
-def test_cabi_library_exports_every_declared_symbol():
+def test_cabi_bindings_cover_every_declared_symbol(tmp_path):
     from upsnet_b200 import _lib, build
     header = open(os.path.join(ROOT, "include", "upsnet_b200.h")).read()
     declared = sorted(set(re.findall(r"\bint\s+(upsnet_\w+)\s*\(", header)))
     assert declared, "no declarations parsed"
-    assert sorted(_lib.EXPORTED_SYMBOLS) == declared
+    decls = dict(_lib.declarations())
+    assert sorted(decls) == declared
     so = build.build()  # nvcc cross-compiles for sm_90a without a GPU
     L = ctypes.CDLL(so)
     for name in declared:
         assert hasattr(L, name), name
     assert L.upsnet_version(None) == 90
+    # lib() binds every declaration, one argtype per parameter (counted here from the raw declaration)
+    bound = _lib.lib()
+    for name, params in re.findall(r"\bint\s+(upsnet_\w+)\s*\(([^)]*)\)\s*;", re.sub(r"/\*.*?\*/", "", header, flags=re.S)):
+        assert len(getattr(bound, name).argtypes) == params.count(",") + 1, name
+        assert getattr(bound, name).argtypes == decls[name], name
+    vp, i, f, d, sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_double, ctypes.c_size_t
+    assert decls["upsnet_version"] == [vp]
+    assert decls["upsnet_rpn_targets"] == [vp, i, vp, vp, vp, i, i, d, d, d, f, f, i, i, ctypes.c_ulonglong,
+                                           vp, vp, vp, vp, vp, vp, sz, vp]
+    assert decls["upsnet_roi_align_fpn_forward"] == [vp] * 4 + [i] * 4 + [vp] + [i] * 4 + [vp] * 4
+    assert decls["upsnet_cocoeval_workspace_bytes"] == [i, i, ctypes.c_longlong, vp]
+    odd = tmp_path / "odd.h"
+    odd.write_text("int upsnet_odd(const float *x, short n, void *stream);\n")
+    with pytest.raises(_lib.UpsnetError, match="short n"):
+        _lib.declarations(str(odd))
 
 
 def test_ops_fail_loudly_without_cuda_tensors():

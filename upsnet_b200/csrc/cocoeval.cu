@@ -424,11 +424,40 @@ coco_accumulate_kernel(const upsnet_coco_record* __restrict__ rec, const unsigne
   }
 }
 
+// segm only: the detections' and the ground truths' run boundaries
+inline size_t coco_image_layout(int n, int cap, long long gt_counts_total, void* base, CocoImageArgs& p) {
+  WsCarve c(base);
+  p.det_bnd = c.take<unsigned>((size_t)n * cap);
+  p.gt_bnd = c.take<unsigned>((size_t)gt_counts_total);
+  return c.bytes();
+}
+
+struct CocoAccWs {
+  unsigned long long *keys_in, *keys_out;
+  int *vals_in, *vals_out;
+  void* cub;                 // the tail of the workspace: CUB's radix-sort temporary storage
+  size_t cub_bytes;
+};
+
+inline int coco_acc_layout(int n_records, void* base, CocoAccWs& w, size_t* bytes) {
+  UPS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, w.cub_bytes, (const unsigned long long*)nullptr,
+                                           (unsigned long long*)nullptr, (const int*)nullptr, (int*)nullptr, n_records));
+  WsCarve c(base);
+  w.keys_in = c.take<unsigned long long>(n_records);
+  w.keys_out = c.take<unsigned long long>(n_records);
+  w.vals_in = c.take<int>(n_records);
+  w.vals_out = c.take<int>(n_records);
+  w.cub = c.take<char>(w.cub_bytes);
+  *bytes = c.bytes();
+  return 0;
+}
+
 }  // namespace ups
 
 extern "C" int upsnet_cocoeval_workspace_bytes(int n, int cap, long long gt_counts_total, size_t* bytes) {
   if (!bytes || n < 0 || cap < 0 || gt_counts_total < 0) return UPSNET_E_BADARG;
-  *bytes = ups::align_up(sizeof(unsigned) * (size_t)n * cap, 256) + sizeof(unsigned) * (size_t)gt_counts_total;
+  ups::CocoImageArgs p{};
+  *bytes = ups::coco_image_layout(n, cap, gt_counts_total, nullptr, p);
   return 0;
 }
 
@@ -451,11 +480,9 @@ extern "C" int upsnet_cocoeval_image(int segm, const float* boxes, const float* 
                   gt_table, num_gt, gt_counts, (const long long*)gt_offsets, num_categories, class_to_k, image_slot,
                   records, record_cap, n_records, npig, err, nullptr, nullptr, segm ? 1 : 0};
   if (segm) {
-    // gt_offsets lives on the device: the caller sizes the workspace with the total it staged from the host
-    const size_t need = align_up(sizeof(unsigned) * (size_t)n * cap, 256);
-    if (!workspace || workspace_bytes < need) return UPSNET_E_WORKSPACE;
-    p.det_bnd = (unsigned*)workspace;
-    p.gt_bnd = (unsigned*)((char*)workspace + need);
+    // gt_offsets lives on the device: the caller sizes the workspace with the total it staged from the host, and the
+    // ground truths' region, the last one, is checked here with a total of 0
+    if (!workspace || workspace_bytes < coco_image_layout(n, cap, 0, workspace, p)) return UPSNET_E_WORKSPACE;
   }
   static PerDeviceOnce configured;
   if (configured.need())
@@ -467,12 +494,8 @@ extern "C" int upsnet_cocoeval_image(int segm, const float* boxes, const float* 
 
 extern "C" int upsnet_cocoeval_accumulate_workspace_bytes(int n_records, size_t* bytes) {
   if (!bytes || n_records < 0) return UPSNET_E_BADARG;
-  size_t cub_bytes = 0;
-  UPS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                           (const int*)nullptr, (int*)nullptr, n_records));
-  const size_t n = (size_t)n_records;
-  *bytes = 2 * ups::align_up(8 * n, 256) + 2 * ups::align_up(4 * n, 256) + cub_bytes;
-  return 0;
+  ups::CocoAccWs w;
+  return ups::coco_acc_layout(n_records, nullptr, w, bytes);
 }
 
 extern "C" int upsnet_cocoeval_accumulate(const upsnet_coco_record* records, int n_records, const int* image_rank,
@@ -481,25 +504,20 @@ extern "C" int upsnet_cocoeval_accumulate(const upsnet_coco_record* records, int
   using namespace ups;
   if (n_records < 0 || num_categories < 1 || num_categories > UPSNET_COCOEVAL_MAX_CATEGORIES) return UPSNET_E_BADARG;
   if (!npig || !precision || !recall || !scores || (n_records > 0 && (!records || !image_rank))) return UPSNET_E_BADARG;
+  CocoAccWs w;
   size_t need = 0;
-  const int rc = upsnet_cocoeval_accumulate_workspace_bytes(n_records, &need);
+  const int rc = coco_acc_layout(n_records, workspace, w, &need);
   if (rc) return rc;
   if (!workspace || workspace_bytes < need) return UPSNET_E_WORKSPACE;
-  const size_t n = (size_t)n_records;
-  char* w = (char*)workspace;
-  unsigned long long* keys_in = (unsigned long long*)w;       w += align_up(8 * n, 256);
-  unsigned long long* keys_out = (unsigned long long*)w;      w += align_up(8 * n, 256);
-  int* vals_in = (int*)w;                                     w += align_up(4 * n, 256);
-  int* vals_out = (int*)w;                                    w += align_up(4 * n, 256);
-  size_t cub_bytes = need - (size_t)(w - (char*)workspace);
   cudaStream_t st = (cudaStream_t)stream;
   if (n_records > 0) {
-    coco_keys_kernel<<<ceil_div(n_records, 256), 256, 0, st>>>(records, n_records, image_rank, keys_in, vals_in);
+    coco_keys_kernel<<<ceil_div(n_records, 256), 256, 0, st>>>(records, n_records, image_rank, w.keys_in, w.vals_in);
     UPS_CHECK_LAUNCH();
-    UPS_CUDA(cub::DeviceRadixSort::SortPairs(w, cub_bytes, keys_in, keys_out, vals_in, vals_out, n_records, 0, 64, st));
+    UPS_CUDA(cub::DeviceRadixSort::SortPairs(w.cub, w.cub_bytes, w.keys_in, w.keys_out, w.vals_in, w.vals_out, n_records, 0,
+                                             64, st));
   }
   coco_accumulate_kernel<<<dim3(num_categories, kCocoA, kCocoM), 32 * kCocoT, 0, st>>>(
-      records, keys_out, vals_out, n_records, npig, num_categories, precision, recall, scores);
+      records, w.keys_out, w.vals_out, n_records, npig, num_categories, precision, recall, scores);
   UPS_CHECK_LAUNCH();
   return 0;
 }

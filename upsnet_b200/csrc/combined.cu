@@ -230,23 +230,21 @@ combined_merge_kernel(const __grid_constant__ CombinedArgs p, unsigned char* __r
   }
 }
 
-struct CbLayout { size_t hist, bits, owner, total; };
-
-inline CbLayout cb_layout(int H, int W) {
+inline size_t cb_layout(int H, int W, void* base, CombinedArgs& p) {
   const size_t HW = (size_t)H * W;
-  CbLayout l;
-  l.hist = 0;
-  l.bits = align_up(256 * sizeof(int), 256);
-  l.owner = l.bits + align_up((HW + 31) / 32 * sizeof(unsigned), 256);
-  l.total = l.owner + align_up(HW * sizeof(unsigned short), 256);
-  return l;
+  WsCarve c(base);
+  p.hist = c.take<int>(256);
+  p.bits = c.take<unsigned>((HW + 31) / 32);
+  p.owner = c.take<unsigned short>(HW);
+  return c.bytes();
 }
 
 }  // namespace ups
 
 extern "C" int upsnet_combined_pan_workspace_bytes(int n, int H, int W, size_t* bytes) {
   if (!bytes || n < 0 || H < 1 || W < 1 || (long long)H * W > (1ll << 24)) return UPSNET_E_BADARG;
-  *bytes = ups::cb_layout(H, W).total;
+  ups::CombinedArgs p{};
+  *bytes = ups::cb_layout(H, W, nullptr, p);
   return 0;
 }
 
@@ -261,16 +259,15 @@ extern "C" int upsnet_combined_pan_result(const void* sem, int sem_elem_size, in
   if (num_classes < 1 || num_classes > 256 || num_seg_classes < num_classes || num_seg_classes - num_classes > 255)
     return UPSNET_E_BADARG;
   if (n > 0 && (!scores || !cls_inds || !counts || !run_len || cap < 1)) return UPSNET_E_BADARG;
-  const CbLayout l = cb_layout(H, W);
-  if (!workspace || workspace_bytes < l.total) return UPSNET_E_WORKSPACE;
-  char* ws = (char*)workspace;
   CombinedArgs p{sem_elem_size == 1 ? (const unsigned char*)sem : nullptr,
                  sem_elem_size == 8 ? (const long long*)sem : nullptr, H, W,
                  scores, (const long long*)cls_inds, n, n_dev, counts, cap, run_len,
                  num_seg_classes - num_classes, num_classes, score_threshold, fraction_threshold, stuff_area_limit,
-                 err, (unsigned*)(ws + l.bits), (unsigned short*)(ws + l.owner), (int*)(ws + l.hist)};
+                 err};
+  if (!workspace || workspace_bytes < cb_layout(H, W, workspace, p)) return UPSNET_E_WORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
-  UPS_CUDA(cudaMemsetAsync(ws, 0, l.owner, st));        // histogram + occupancy bitmap (the owner map is read under it)
+  // histogram + occupancy bitmap (the owner map is read under it)
+  UPS_CUDA(cudaMemsetAsync(p.hist, 0, (char*)p.owner - (char*)p.hist, st));
   const int hist_blocks = max(1, min(2 * num_sms(), ceil_div(H * W, kCbThreads * 16)));
   combined_decide_kernel<<<1 + hist_blocks, kCbThreads, 0, st>>>(p);
   UPS_CHECK_LAUNCH();

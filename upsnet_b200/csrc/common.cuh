@@ -52,4 +52,23 @@ __host__ __device__ inline int conv_out_size(int in, int pad, int dil, int k, in
   return (in + 2 * pad - (dil * (k - 1) + 1)) / stride + 1;
 }
 
+// Lays out a caller-owned workspace as consecutive 256-byte-aligned regions, in the order of the take() calls.  On a
+// null base it only adds up the size; on the caller's buffer take() also returns each region's address.  So one
+// function per entry point both sizes its workspace (for *_workspace_bytes) and carves it.
+class WsCarve {
+ public:
+  explicit WsCarve(void* base) : base_((char*)base) {}
+  template <typename T>
+  T* take(size_t count) {
+    T* p = base_ ? (T*)(base_ + off_) : nullptr;
+    off_ = align_up(off_ + count * sizeof(T), 256);
+    return p;
+  }
+  size_t bytes() const { return off_; }
+
+ private:
+  char* base_;
+  size_t off_ = 0;
+};
+
 }  // namespace ups

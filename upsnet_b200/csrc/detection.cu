@@ -507,11 +507,25 @@ topk_sort_kernel(const TopkParams p) {
   }
 }
 
+inline size_t topk_layout(int L, void* base, TopkParams& p) {
+  WsCarve c(base);
+  p.hist = c.take<unsigned int>((size_t)L * kTkBins);
+  p.keys = c.take<unsigned long long>((size_t)L * kTkMaxK);
+  p.prefix = c.take<unsigned long long>(L);
+  // ticket, need, fill and done share one region, so that one memset clears them
+  unsigned int* ctr = c.take<unsigned int>((size_t)L * 4);
+  if (ctr) {
+    p.ticket = ctr; p.need = (int*)(ctr + L); p.fill = ctr + 2 * L; p.done = (int*)(ctr + 3 * L);
+  }
+  return c.bytes();
+}
+
 }  // namespace ups
 
 extern "C" int upsnet_rpn_topk_workspace_bytes(int L, size_t* bytes) {
   if (!bytes || L <= 0 || L > ups::kMaxLevels) return UPSNET_E_BADARG;
-  *bytes = (size_t)L * (ups::kTkBins * 4 + 4 + 8 + 4 + 4 + 4 + 4 + (size_t)ups::kTkMaxK * 8) + 256;
+  ups::TopkParams p{};
+  *bytes = ups::topk_layout(L, nullptr, p);
   return 0;
 }
 
@@ -522,18 +536,8 @@ extern "C" int upsnet_rpn_topk(const float* const* probs, const int* hs, const i
   if (!probs || !hs || !ws || !out_scores || !out_idx || !workspace) return UPSNET_E_BADARG;
   if (L <= 0 || L > kMaxLevels || A <= 0 || pre_nms_top_n <= 0) return UPSNET_E_BADARG;
   if (pre_nms_top_n > kTkMaxK) return UPSNET_E_UNSUPPORTED;
-  size_t need_bytes = 0;
-  upsnet_rpn_topk_workspace_bytes(L, &need_bytes);
-  if (workspace_bytes < need_bytes) return UPSNET_E_WORKSPACE;
   TopkParams p{};
-  char* base = (char*)workspace;
-  p.hist = (unsigned int*)base; base += (size_t)L * kTkBins * 4;
-  p.keys = (unsigned long long*)base; base += (size_t)L * kTkMaxK * 8;
-  p.prefix = (unsigned long long*)base; base += (size_t)L * 8;
-  p.ticket = (unsigned int*)base; base += (size_t)L * 4;
-  p.need = (int*)base; base += (size_t)L * 4;
-  p.fill = (unsigned int*)base; base += (size_t)L * 4;
-  p.done = (int*)base; base += (size_t)L * 4;
+  if (workspace_bytes < topk_layout(L, workspace, p)) return UPSNET_E_WORKSPACE;
   p.nlev = L; p.A = A; p.out_scores = out_scores; p.out_idx = out_idx;
   int acc = 0, max_blocks = 0;
   for (int l = 0; l < L; ++l) {
@@ -550,7 +554,7 @@ extern "C" int upsnet_rpn_topk(const float* const* probs, const int* hs, const i
   cudaStream_t st = (cudaStream_t)stream;
   // histograms + tickets start at zero (every pass re-arms them for the next one)
   UPS_CUDA(cudaMemsetAsync(p.hist, 0, (size_t)L * kTkBins * 4, st));
-  UPS_CUDA(cudaMemsetAsync(p.ticket, 0, (size_t)L * 4 * 4, st));    // ticket, need, fill, done are contiguous
+  UPS_CUDA(cudaMemsetAsync(p.ticket, 0, (size_t)L * 4 * 4, st));    // ticket, need, fill, done
   const dim3 grid((unsigned)max_blocks, (unsigned)L);
   const int shifts[5] = {43, 32, 22, 11, 0}, nbits[5] = {11, 11, 10, 11, 11};
   for (int ps = 0; ps < 5; ++ps) {

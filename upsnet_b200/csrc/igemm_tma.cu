@@ -737,6 +737,15 @@ static void stem_geometry(int H, int W, int kh, int kw, int pad, int* Ho, int* W
   *Wp = 2 * *Wo + 8;
 }
 
+// the zero-padded bf16 NHWC8 image (16 bytes per pixel): the hi plane, then the lo plane, which only the pair stem has
+inline size_t stem_layout(int N, int Hp, int Wp, bool pair, void* base, uint4** hi, uint4** lo) {
+  WsCarve c(base);
+  const size_t pixels = (size_t)N * Hp * Wp;
+  *hi = c.take<uint4>(pixels);
+  *lo = pair ? c.take<uint4>(pixels) : nullptr;
+  return c.bytes();
+}
+
 }  // namespace ups
 
 extern "C" int upsnet_tma_set_tile_n(int bn) {
@@ -750,7 +759,8 @@ extern "C" int upsnet_stem_workspace_bytes(int N, int H, int W, int kh, int kw, 
   int Ho, Wo, Hp, Wp;
   ups::stem_geometry(H, W, kh, kw, pad, &Ho, &Wo, &Hp, &Wp);
   if (Ho <= 0 || Wo <= 0) return UPSNET_E_BADARG;
-  *bytes = (size_t)N * Hp * Wp * 16 * 2;     // hi plane + lo plane (the lo plane is only written / read by the pair stem)
+  uint4 *hi, *lo;
+  *bytes = ups::stem_layout(N, Hp, Wp, true, nullptr, &hi, &lo);
   return 0;
 }
 
@@ -782,8 +792,8 @@ extern "C" int upsnet_stem_forward(const float* x, const void* packed_w, const f
   stem_geometry(H, W, kh, kw, pad, &Ho, &Wo, &Hp, &Wp);
   if (Ho <= 0 || Wo <= 0) return UPSNET_E_BADARG;
   const bool pair = (epi_flags & UPSNET_EPI_STEM_PAIR) != 0;
-  const size_t plane_bytes = (size_t)N * Hp * Wp * 16;
-  if (workspace_bytes < plane_bytes * (pair ? 2 : 1)) return UPSNET_E_WORKSPACE;
+  uint4 *x_hi, *x_lo;
+  if (workspace_bytes < stem_layout(N, Hp, Wp, pair, workspace, &x_hi, &x_lo)) return UPSNET_E_WORKSPACE;
   EncodeTiledFn enc = tma_encoder();
   if (!enc) return UPSNET_E_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
@@ -814,9 +824,9 @@ extern "C" int upsnet_stem_forward(const float* x, const void* packed_w, const f
     const cuuint32_t bw2[2] = {64, (cuuint32_t)g.BN};
     const cuuint64_t dy[4] = {(cuuint64_t)Cout * (pair ? 2 : 1), (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)N};
     const cuuint32_t by[4] = {64, (cuuint32_t)g.bw, (cuuint32_t)g.bh, (cuuint32_t)g.bn};
-    if (!encode_bf16(enc, &tm_x, workspace, 5, dx, bx, sx)) return UPSNET_E_UNSUPPORTED;
+    if (!encode_bf16(enc, &tm_x, x_hi, 5, dx, bx, sx)) return UPSNET_E_UNSUPPORTED;
     tm_lo = tm_x;
-    if (pair && !encode_bf16(enc, &tm_lo, (char*)workspace + plane_bytes, 5, dx, bx, sx)) return UPSNET_E_UNSUPPORTED;
+    if (pair && !encode_bf16(enc, &tm_lo, x_lo, 5, dx, bx, sx)) return UPSNET_E_UNSUPPORTED;
     if (!encode_bf16(enc, &tm_w, packed_w, 2, dwt, bw2)) return UPSNET_E_UNSUPPORTED;
     if (!encode_bf16(enc, &tm_y, y, 4, dy, by)) return UPSNET_E_UNSUPPORTED;
   }
@@ -824,8 +834,7 @@ extern "C" int upsnet_stem_forward(const float* x, const void* packed_w, const f
     const long long total = (long long)N * Hp * Wp;
     long long blocks = (total + 255) / 256;
     if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
-    stem_pack_image_kernel<<<(unsigned)blocks, 256, 0, st>>>(x, (uint4*)workspace, pair ? (uint4*)((char*)workspace + plane_bytes) : nullptr,
-                                                             N, Cin, H, W, pad, Hp, Wp);
+    stem_pack_image_kernel<<<(unsigned)blocks, 256, 0, st>>>(x, x_hi, x_lo, N, Cin, H, W, pad, Hp, Wp);
     UPS_CHECK_LAUNCH();
   }
   const int sms = num_sms();

@@ -195,11 +195,19 @@ im_post_rle_kernel(const float* __restrict__ mask_probs, int C, int M, const flo
   }
 }
 
+// the run boundaries of every detection, [n][cap]
+inline size_t im_post_layout(int n, int cap, void* base, long long** pos) {
+  WsCarve c(base);
+  *pos = c.take<long long>((size_t)(n > 0 ? n : 1) * cap);
+  return c.bytes();
+}
+
 }  // namespace ups
 
 extern "C" int upsnet_im_post_workspace_bytes(int n, int cap, size_t* bytes) {
   if (!bytes || n < 0 || cap < 2) return UPSNET_E_BADARG;
-  *bytes = (size_t)(n > 0 ? n : 1) * cap * sizeof(long long) + 256;
+  long long* pos;
+  *bytes = ups::im_post_layout(n, cap, nullptr, &pos);
   return 0;
 }
 
@@ -210,13 +218,11 @@ extern "C" int upsnet_im_post_rle(const float* mask_probs, int C, int M, const f
   if (!mask_probs || !boxes || !cls_inds || !counts || !run_len || !overflow || !workspace) return UPSNET_E_BADARG;
   if (n < 0 || C < 1 || M < 1 || H <= 0 || W <= 0 || cap < 2) return UPSNET_E_BADARG;
   if (M + 2 > kPostMaxM || W > kPostMaxCols || H > kPostMaxRows) return UPSNET_E_UNSUPPORTED;
-  size_t need = 0;
-  upsnet_im_post_workspace_bytes(n, cap, &need);
-  if (workspace_bytes < need) return UPSNET_E_WORKSPACE;
+  long long* pos;
+  if (workspace_bytes < im_post_layout(n, cap, workspace, &pos)) return UPSNET_E_WORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   UPS_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), st));
   if (n == 0) return 0;
-  long long* pos = reinterpret_cast<long long*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
   im_post_rle_kernel<<<n, kPostThreads, 0, st>>>(mask_probs, C, M, boxes, cls_inds, n, n_dev, H, W, counts, pos, cap, run_len,
                                                  overflow);
   UPS_CHECK_LAUNCH();

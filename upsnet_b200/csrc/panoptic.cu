@@ -58,45 +58,41 @@ struct PanWorkspace {
 // avail = 0: the preferred layout (all bit windows resident, up to kBitsBudget).  avail > 0: the caller's workspace size
 // -- the bit-window budget shrinks to what fits (more rounds of consecutive ranks), so the round structure is a RUNTIME
 // property of the call; returns 0 when not even the minimum (one window, or all / kMaxRounds words) fits.
-static inline size_t pan_ws_layout(int n, int H, int W, int num_thing, PanWorkspace* ws,
-                                                char* base, size_t avail = 0) {
+static inline size_t pan_ws_layout(int n, int H, int W, int num_thing, PanWorkspace& ws,
+                                                void* base, size_t avail = 0) {
   const int nn = n > 0 ? n : 1;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-  const size_t o_order = take(sizeof(int) * nn), o_flag = take(sizeof(int) * nn);
-  const size_t o_list = take(sizeof(int) * nn), o_meta = take(sizeof(int) * 4);
-  const size_t o_geom = take(sizeof(int) * nn * 13);
+  WsCarve c(base);
+  ws.order = c.take<int>(nn);
+  ws.kept_flag = c.take<int>(nn);
+  ws.kept_list = c.take<int>(nn);
+  ws.meta = c.take<int>(4);
+  int* g = c.take<int>((size_t)nn * 13);
+  if (g) {
+    ws.g.bx0 = g; ws.g.by0 = g + nn; ws.g.w = g + 2 * nn; ws.g.h = g + 3 * nn;
+    ws.g.gx0 = g + 4 * nn; ws.g.gy0 = g + 5 * nn; ws.g.gx1 = g + 6 * nn; ws.g.gy1 = g + 7 * nn;
+    ws.g.sx0 = g + 8 * nn; ws.g.sy0 = g + 9 * nn; ws.g.sx1 = g + 10 * nn; ws.g.sy1 = g + 11 * nn;
+    ws.g.cls = g + 12 * nn;
+  }
   const int Ww = ceil_div(W, 32);
-  const size_t plane = (size_t)num_thing * H * Ww * sizeof(unsigned int);
-  const size_t o_occ = take(plane);
-  const size_t o_off = take(sizeof(long long) * nn), o_msum = take(sizeof(int) * nn);
-  const size_t o_round = take(sizeof(int) * (kMaxRounds + 1));
+  ws.occ = c.take<unsigned int>((size_t)num_thing * H * Ww);
+  ws.off = c.take<long long>(nn);
+  ws.msum = c.take<int>(nn);
+  ws.round_lo = c.take<int>(kMaxRounds + 1);
   // bit windows: every instance needs at most one full plane (H*Ww words).  All of them are resident when they
   // fit the budget, otherwise the instances are processed in rounds of consecutive ranks.
   const long long win = (long long)H * Ww, all = win * nn;
   long long budget = all < kBitsBudget ? all : kBitsBudget;
   if (avail) {
-    const long long fit = ((long long)avail - (long long)off) / (long long)sizeof(unsigned int) - win - 64;
+    const long long fit = ((long long)avail - (long long)c.bytes()) / (long long)sizeof(unsigned int) - win - 64;
     if (fit < budget) budget = fit;
     if (budget < win || (all + budget - 1) / budget > kMaxRounds) return 0;
   }
   if ((all + budget - 1) / budget > kMaxRounds) budget = (all + kMaxRounds - 1) / kMaxRounds;
   if (budget < win) budget = win;
-  const int rounds = (int)((all + budget - 1) / budget);
-  const size_t o_bits = take(sizeof(unsigned int) * (size_t)(budget + win));
-  if (ws) {
-    ws->order = (int*)(base + o_order); ws->kept_flag = (int*)(base + o_flag);
-    ws->kept_list = (int*)(base + o_list); ws->meta = (int*)(base + o_meta);
-    int* g = (int*)(base + o_geom);
-    ws->g.bx0 = g; ws->g.by0 = g + nn; ws->g.w = g + 2 * nn; ws->g.h = g + 3 * nn;
-    ws->g.gx0 = g + 4 * nn; ws->g.gy0 = g + 5 * nn; ws->g.gx1 = g + 6 * nn; ws->g.gy1 = g + 7 * nn;
-    ws->g.sx0 = g + 8 * nn; ws->g.sy0 = g + 9 * nn; ws->g.sx1 = g + 10 * nn; ws->g.sy1 = g + 11 * nn;
-    ws->g.cls = g + 12 * nn;
-    ws->occ = (unsigned int*)(base + o_occ);
-    ws->off = (long long*)(base + o_off); ws->msum = (int*)(base + o_msum); ws->round_lo = (int*)(base + o_round);
-    ws->bits = (unsigned int*)(base + o_bits); ws->budget = budget; ws->rounds = rounds;
-  }
-  return off;
+  ws.rounds = (int)((all + budget - 1) / budget);
+  ws.budget = budget;
+  ws.bits = c.take<unsigned int>((size_t)(budget + win));
+  return c.bytes();
 }
 
 // ---- resize coefficients: oracle resize_coef_x / resize_coef_y, un-fused ----
@@ -656,7 +652,7 @@ extern "C" int upsnet_mask_removal(const float* boxes, const float* cls_prob, co
   if (n < 1 || H <= 0 || W <= 0 || num_thing <= 0) return UPSNET_E_BADARG;
   if (n > kMaxList) return UPSNET_E_UNSUPPORTED;
   PanWorkspace ws;
-  const size_t need = pan_ws_layout(n, H, W, num_thing, &ws, (char*)workspace, workspace_bytes);
+  const size_t need = pan_ws_layout(n, H, W, num_thing, ws, workspace, workspace_bytes);
   if (need == 0 || workspace_bytes < need) return UPSNET_E_WORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const int Ww = ceil_div(W, 32);
@@ -688,14 +684,16 @@ extern "C" int upsnet_mask_removal(const float* boxes, const float* cls_prob, co
 
 extern "C" int upsnet_panoptic_workspace_bytes(int n, int H, int W, int num_thing, size_t* bytes) {
   if (!bytes || n < 0 || H <= 0 || W <= 0 || num_thing <= 0) return UPSNET_E_BADARG;
-  *bytes = ups::pan_ws_layout(n, H, W, num_thing, nullptr, nullptr);
+  ups::PanWorkspace ws;
+  *bytes = ups::pan_ws_layout(n, H, W, num_thing, ws, nullptr);
   return 0;
 }
 
 extern "C" int upsnet_panoptic_workspace_min_bytes(int n, int H, int W, int num_thing, size_t* bytes) {
   if (!bytes || n < 0 || H <= 0 || W <= 0 || num_thing <= 0) return UPSNET_E_BADARG;
   // fixed part + the smallest bit-window budget: max(one window, all windows / kMaxRounds), plus the spill window
-  const size_t full = ups::pan_ws_layout(n, H, W, num_thing, nullptr, nullptr);
+  ups::PanWorkspace ws;
+  const size_t full = ups::pan_ws_layout(n, H, W, num_thing, ws, nullptr);
   const long long win = (long long)H * ups::ceil_div(W, 32), all = win * (n > 0 ? n : 1);
   long long budget = all < ups::kBitsBudget ? all : ups::kBitsBudget;
   long long minb = (all + ups::kMaxRounds - 1) / ups::kMaxRounds;
@@ -719,7 +717,7 @@ static int panoptic_head_impl(const float* fcn, bool up4, int S, int H, int W, c
   if (((uintptr_t)fcn & 15) || ((uintptr_t)labels & 15) || (sem_labels && ((uintptr_t)sem_labels & 15)))
     return UPSNET_E_BADARG;
   PanWorkspace ws;
-  const size_t need = pan_ws_layout(n, H, W, num_thing, &ws, (char*)workspace, workspace_bytes);
+  const size_t need = pan_ws_layout(n, H, W, num_thing, ws, workspace, workspace_bytes);
   if (need == 0 || workspace_bytes < need) return UPSNET_E_WORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const int Ww = ceil_div(W, 32);

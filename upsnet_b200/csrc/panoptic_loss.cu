@@ -314,31 +314,27 @@ __global__ void pl_draw_keys_kernel(unsigned long long seed, int stream_id, int 
   if (p < n) keys[p] = draw_key(seed, stream_id, (unsigned long long)p);
 }
 
-struct PlLayout { size_t tab, part_loss, part_cnt, total; int nblocks; };
+inline int pl_blocks(int h, int w) { return (int)(((size_t)h * w + kPlThreads - 1) / kPlThreads); }
 
-inline PlLayout pl_layout(int k, int h, int w) {
-  PlLayout o;
-  size_t at = 0;
-  auto take = [&](size_t bytes) { const size_t r = at; at = align_up(at + bytes, 256); return r; };
-  o.nblocks = (int)(((size_t)h * w + kPlThreads - 1) / kPlThreads);
-  o.tab = take((size_t)k * sizeof(PlInst));
-  o.part_loss = take((size_t)o.nblocks * sizeof(double));
-  o.part_cnt = take((size_t)o.nblocks * 2 * sizeof(int));
-  o.total = at;
-  return o;
+inline size_t pl_layout(int k, int h, int w, void* base, PlArgs& a) {
+  const int nblocks = pl_blocks(h, w);
+  WsCarve c(base);
+  a.tab = c.take<PlInst>(k);
+  a.part_loss = c.take<double>(nblocks);
+  a.part_cnt = c.take<int>((size_t)nblocks * 2);
+  return c.bytes();
 }
 
-// argument checks and the instance table shared by forward and backward
-int pl_prepare(PlArgs& a, const PlLayout& lo, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+// argument checks, the workspace carve and the instance table shared by forward and backward
+int pl_prepare(PlArgs& a, void* workspace, size_t workspace_bytes, cudaStream_t st) {
   if (!a.fcn || !a.mask || !a.rois || !a.cls || !workspace) return UPSNET_E_BADARG;
   if (a.S <= 0 || a.h <= 0 || a.w <= 0 || a.k <= 0 || a.M <= 0 || a.num_classes <= 0 || a.num_classes > a.S ||
       (a.C != 1 && a.C != a.num_classes) || !(a.box_scale > 0.f))
     return UPSNET_E_BADARG;
   if (a.M > kPlMaxM || (size_t)a.S * a.h * a.w >= (1ull << 31) || (size_t)a.k * a.C * a.M * a.M >= (1ull << 31))
     return UPSNET_E_UNSUPPORTED;
-  if (workspace_bytes < lo.total) return UPSNET_E_WORKSPACE;
+  if (workspace_bytes < pl_layout(a.k, a.h, a.w, workspace, a)) return UPSNET_E_WORKSPACE;
   a.num_stuff = a.S - a.num_classes + 1;
-  a.tab = (PlInst*)((char*)workspace + lo.tab);
   a.tab_smem = (size_t)a.k * sizeof(PlInst) <= kPlSmemTable;
   pl_table_kernel<<<ceil_div(a.k, 128), 128, 0, st>>>(a);
   UPS_CHECK_LAUNCH();
@@ -350,7 +346,8 @@ int pl_prepare(PlArgs& a, const PlLayout& lo, void* workspace, size_t workspace_
 
 extern "C" int upsnet_panoptic_loss_workspace_bytes(int k, int h, int w, size_t* bytes) {
   if (!bytes || k <= 0 || h <= 0 || w <= 0) return UPSNET_E_BADARG;
-  *bytes = ups::pl_layout(k, h, w).total;
+  ups::PlArgs a{};
+  *bytes = ups::pl_layout(k, h, w, nullptr, a);
   return 0;
 }
 
@@ -370,18 +367,16 @@ extern "C" int upsnet_panoptic_loss_forward(const float* fcn_score, int S, int h
   a.enable_void = enable_void ? 1 : 0; a.box_scale = box_scale;
   a.lse = lse; a.gtc = gt_channel;
   cudaStream_t st = (cudaStream_t)stream;
-  const PlLayout lo = pl_layout(k, h, w);
-  const int rc = pl_prepare(a, lo, workspace, workspace_bytes, st);
+  const int rc = pl_prepare(a, workspace, workspace_bytes, st);
   if (rc) return rc;
-  a.part_loss = (double*)((char*)workspace + lo.part_loss);
-  a.part_cnt = (int*)((char*)workspace + lo.part_cnt);
+  const int nblocks = pl_blocks(h, w);
   const size_t smem = a.tab_smem ? (size_t)k * sizeof(PlInst) : 0;
   if (mask_gt_is_int64)
-    pl_forward_kernel<int64_t><<<lo.nblocks, kPlThreads, smem, st>>>(a);
+    pl_forward_kernel<int64_t><<<nblocks, kPlThreads, smem, st>>>(a);
   else
-    pl_forward_kernel<unsigned char><<<lo.nblocks, kPlThreads, smem, st>>>(a);
+    pl_forward_kernel<unsigned char><<<nblocks, kPlThreads, smem, st>>>(a);
   UPS_CHECK_LAUNCH();
-  pl_finish_kernel<<<1, kPlThreads, 0, st>>>(a.part_loss, a.part_cnt, lo.nblocks, h * w, loss, accuracy, counts);
+  pl_finish_kernel<<<1, kPlThreads, 0, st>>>(a.part_loss, a.part_cnt, nblocks, h * w, loss, accuracy, counts);
   UPS_CHECK_LAUNCH();
   return 0;
 }
@@ -400,12 +395,11 @@ extern "C" int upsnet_panoptic_loss_backward(const float* fcn_score, int S, int 
   a.lse = const_cast<float*>(lse); a.gtc = const_cast<int*>(gt_channel);
   a.grad_out = grad_out; a.dfcn = d_fcn_score; a.dmask = d_mask_score;
   cudaStream_t st = (cudaStream_t)stream;
-  const PlLayout lo = pl_layout(k, h, w);
-  const int rc = pl_prepare(a, lo, workspace, workspace_bytes, st);
+  const int rc = pl_prepare(a, workspace, workspace_bytes, st);
   if (rc) return rc;
   if (d_fcn_score) {
     const size_t smem = a.tab_smem ? (size_t)k * sizeof(PlInst) : 0;
-    pl_map_grad_kernel<<<lo.nblocks, kPlThreads, smem, st>>>(a);
+    pl_map_grad_kernel<<<pl_blocks(h, w), kPlThreads, smem, st>>>(a);
     UPS_CHECK_LAUNCH();
   }
   if (d_mask_score) {

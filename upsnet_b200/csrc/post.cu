@@ -26,17 +26,15 @@ struct UniWs {
   unsigned char* ins_of; // [kUniMaxInst]
 };
 
-static size_t uni_ws_layout(int S, UniWs* ws, char* base) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-  const size_t o_hist = take(sizeof(int) * (size_t)kUniMaxInst * S), o_pres = take(sizeof(int) * kUniMaxInst);
-  const size_t o_area = take(sizeof(int) * kUniMaxCls), o_err = take(sizeof(int));
-  const size_t o_seg = take(kUniMaxInst), o_ins = take(kUniMaxInst);
-  if (ws) {
-    ws->hist = (int*)(base + o_hist); ws->present = (int*)(base + o_pres); ws->area = (int*)(base + o_area);
-    ws->err = (int*)(base + o_err); ws->seg_of = (unsigned char*)(base + o_seg); ws->ins_of = (unsigned char*)(base + o_ins);
-  }
-  return off;
+static size_t uni_ws_layout(int S, UniWs& ws, void* base) {
+  WsCarve c(base);
+  ws.hist = c.take<int>((size_t)kUniMaxInst * S);
+  ws.present = c.take<int>(kUniMaxInst);
+  ws.area = c.take<int>(kUniMaxCls);
+  ws.err = c.take<int>(1);
+  ws.seg_of = c.take<unsigned char>(kUniMaxInst);
+  ws.ins_of = c.take<unsigned char>(kUniMaxInst);
+  return c.bytes();
 }
 
 // (instance, semantic class) histogram.  Neighbouring pixels mostly share both keys, so the lanes of a warp that hold the
@@ -191,7 +189,8 @@ label_restore_kernel(const long long* __restrict__ src0, const long long* __rest
 
 extern "C" int upsnet_unified_pan_workspace_bytes(int num_seg_classes, size_t* bytes) {
   if (!bytes || num_seg_classes <= 0 || num_seg_classes > ups::kUniMaxCls) return UPSNET_E_BADARG;
-  *bytes = ups::uni_ws_layout(num_seg_classes, nullptr, nullptr);
+  ups::UniWs ws;
+  *bytes = ups::uni_ws_layout(num_seg_classes, ws, nullptr);
   return 0;
 }
 
@@ -204,11 +203,12 @@ extern "C" int upsnet_unified_pan_result(const long long* seg, const long long* 
   if (H <= 0 || W <= 0 || k < 0 || num_classes < 1 || num_seg_classes < num_classes || num_seg_classes > kUniMaxCls)
     return UPSNET_E_BADARG;
   UniWs ws;
-  if (workspace_bytes < uni_ws_layout(num_seg_classes, &ws, (char*)workspace)) return UPSNET_E_WORKSPACE;
+  const size_t need = uni_ws_layout(num_seg_classes, ws, workspace);
+  if (workspace_bytes < need) return UPSNET_E_WORKSPACE;
   const int id_last = num_seg_classes - num_classes;
   const size_t HW = (size_t)H * W;
   cudaStream_t st = (cudaStream_t)stream;
-  UPS_CUDA(cudaMemsetAsync(workspace, 0, uni_ws_layout(num_seg_classes, nullptr, nullptr), st));
+  UPS_CUDA(cudaMemsetAsync(workspace, 0, need, st));
   size_t blocks = (HW + 255) / 256;
   if (blocks > (size_t)kNumSMs * 16) blocks = (size_t)kNumSMs * 16;
   uni_hist_kernel<<<(unsigned)blocks, 256, 0, st>>>(seg, pan, HW, id_last, num_seg_classes, ws);

@@ -34,16 +34,13 @@ struct PqWs {
   unsigned* list;   // [kPqMaxPairs] hash slot of the i-th inserted pair
 };
 
-static size_t pq_ws_layout(PqWs* ws, char* base) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-  const size_t o_keys = take(sizeof(unsigned) * kPqHash), o_cnt = take(sizeof(unsigned) * kPqHash);
-  const size_t o_n = take(sizeof(int)), o_list = take(sizeof(unsigned) * kPqMaxPairs);
-  if (ws) {
-    ws->keys = (unsigned*)(base + o_keys); ws->cnt = (unsigned*)(base + o_cnt);
-    ws->n_pairs = (int*)(base + o_n); ws->list = (unsigned*)(base + o_list);
-  }
-  return off;
+static size_t pq_ws_layout(PqWs& ws, void* base) {
+  WsCarve c(base);
+  ws.keys = c.take<unsigned>(kPqHash);
+  ws.cnt = c.take<unsigned>(kPqHash);
+  ws.n_pairs = c.take<int>(1);
+  ws.list = c.take<unsigned>(kPqMaxPairs);
+  return c.bytes();
 }
 
 __device__ __forceinline__ unsigned pq_hash(unsigned key, int bits) { return (key * 2654435761u) >> (32 - bits); }
@@ -292,7 +289,8 @@ pq_finalize_kernel(const long long* __restrict__ table, int G, PqWs ws, long lon
 
 extern "C" int upsnet_pq_workspace_bytes(size_t* bytes) {
   if (!bytes) return UPSNET_E_BADARG;
-  *bytes = ups::pq_ws_layout(nullptr, nullptr);
+  ups::PqWs ws;
+  *bytes = ups::pq_ws_layout(ws, nullptr);
   return 0;
 }
 
@@ -304,7 +302,7 @@ extern "C" int upsnet_pq_update(const unsigned char* pan_2ch, const unsigned cha
     return UPSNET_E_BADARG;
   if (H <= 0 || W <= 0 || num_gt < 0) return UPSNET_E_BADARG;
   PqWs ws;
-  if (workspace_bytes < pq_ws_layout(&ws, (char*)workspace)) return UPSNET_E_WORKSPACE;
+  if (workspace_bytes < pq_ws_layout(ws, workspace)) return UPSNET_E_WORKSPACE;
   static bool attr_set[64] = {};                  // the shared-memory opt-in is per device
   int dev = 0;
   UPS_CUDA(cudaGetDevice(&dev));

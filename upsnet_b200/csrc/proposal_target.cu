@@ -394,30 +394,24 @@ __global__ void __launch_bounds__(kPtThreads) pt_mask_kernel(const PtParams p) {
   }
 }
 
-struct PtLayout {
-  size_t ovl, cls, map, flags, list0, list1, rowbox, total;
-};
-
-inline PtLayout pt_layout(int S, int batch) {
-  PtLayout o;
-  size_t at = 0;
-  auto take = [&](size_t bytes) { const size_t r = at; at = align_up(at + bytes, 256); return r; };
-  o.ovl = take((size_t)S * 4);
-  o.cls = take((size_t)S * 4);
-  o.map = take((size_t)S * 4);
-  o.flags = take((size_t)S);
-  o.list0 = take((size_t)S * 4);
-  o.list1 = take((size_t)S * 4);
-  o.rowbox = take((size_t)batch * 16);
-  o.total = at;
-  return o;
+inline size_t pt_layout(int S, int batch, void* base, PtParams& p) {
+  WsCarve c(base);
+  p.ovl = c.take<float>(S);
+  p.cls = c.take<int>(S);
+  p.map = c.take<int>(S);
+  p.flags = c.take<unsigned char>(S);
+  p.list[0] = c.take<int>(S);
+  p.list[1] = c.take<int>(S);
+  p.rowbox = c.take<float4>(batch);
+  return c.bytes();
 }
 
 }  // namespace ups
 
 extern "C" int upsnet_proposal_targets_workspace_bytes(int num_rois, int num_gt, int batch_rois, size_t* bytes) {
   if (!bytes || num_rois < 0 || num_gt <= 0 || batch_rois <= 0) return UPSNET_E_BADARG;
-  *bytes = ups::pt_layout(num_rois + num_gt, batch_rois).total;
+  ups::PtParams p{};
+  *bytes = ups::pt_layout(num_rois + num_gt, batch_rois, nullptr, p);
   return 0;
 }
 
@@ -441,10 +435,8 @@ extern "C" int upsnet_proposal_targets(
     return UPSNET_E_BADARG;
   if (cls_agnostic_bbox_reg || G > kPtMaxG || mask_size > kPtMaxM || batch_rois > kPtMaxBatch) return UPSNET_E_UNSUPPORTED;
   const int S = R + G;
-  const PtLayout lo = pt_layout(S, batch_rois);
-  if (workspace_bytes < lo.total) return UPSNET_E_WORKSPACE;
-  char* ws = (char*)workspace;
   PtParams p{};
+  if (workspace_bytes < pt_layout(S, batch_rois, workspace, p)) return UPSNET_E_WORKSPACE;
   p.rois = rois; p.gt = gt_boxes; p.gt_ovl = gt_max_overlaps; p.gt_maxcls = gt_max_classes; p.gt_cls = gt_classes;
   p.gt_map = gt_box_to_gt_ind; p.obj_box = obj_boxes; p.obj_poly = obj_poly_off; p.poly_vert = poly_vert_off;
   p.verts = verts;
@@ -455,13 +447,6 @@ extern "C" int upsnet_proposal_targets(
   p.fg_thresh = fg_thresh; p.bg_hi = bg_thresh_hi; p.bg_lo = bg_thresh_lo;
   p.weights = make_float4(wx, wy, ww, wh);
   p.seed = seed;
-  p.ovl = (float*)(ws + lo.ovl);
-  p.cls = (int*)(ws + lo.cls);
-  p.map = (int*)(ws + lo.map);
-  p.flags = (unsigned char*)(ws + lo.flags);
-  p.list[0] = (int*)(ws + lo.list0);
-  p.list[1] = (int*)(ws + lo.list1);
-  p.rowbox = (float4*)(ws + lo.rowbox);
   p.rois_out = rois_out; p.labels = labels; p.targets = bbox_targets; p.inside = bbox_inside_weights;
   p.outside = bbox_outside_weights; p.nongt = nongt_inds; p.mask_rois = mask_rois; p.mask = mask_int32;
   p.has_mask = roi_has_mask; p.counts = counts;

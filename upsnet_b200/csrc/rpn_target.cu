@@ -348,36 +348,30 @@ __global__ void __launch_bounds__(kRtThreads) rt_write_kernel(const RtParams p) 
   }
 }
 
-struct RtLayout {
-  size_t state, gtmax, amax, aarg, flags, blk, keys0, keys1, idx0, idx1, list0, list1, total;
-};
-
-inline RtLayout rt_layout(long long N, int batch) {
-  RtLayout o;
+inline size_t rt_layout(long long N, int batch, void* base, RtParams& p) {
   const long long nblk = (N + kRtThreads - 1) / kRtThreads;
-  size_t at = 0;
-  auto take = [&](size_t bytes) { const size_t r = at; at = align_up(at + bytes, 256); return r; };
-  o.state = take(sizeof(RtState));
-  o.gtmax = take((size_t)kRtMaxG * 4);
-  o.amax = take((size_t)N * 4);
-  o.aarg = take((size_t)N * 4);
-  o.flags = take((size_t)N);
-  o.blk = take((size_t)nblk * 5 * 4);
-  o.keys0 = take((size_t)N * 8);
-  o.keys1 = take((size_t)N * 8);
-  o.idx0 = take((size_t)N * 4);
-  o.idx1 = take((size_t)N * 4);
-  o.list0 = take((size_t)batch * 4);
-  o.list1 = take((size_t)batch * 4);
-  o.total = at;
-  return o;
+  WsCarve c(base);
+  p.st = c.take<RtState>(1);
+  p.gtmax = c.take<unsigned int>(kRtMaxG);
+  p.amax = c.take<float>(N);
+  p.aarg = c.take<int>(N);
+  p.flags = c.take<unsigned char>(N);
+  p.blk = c.take<int>(nblk * 5);
+  p.keys[0] = c.take<unsigned long long>(N);
+  p.keys[1] = c.take<unsigned long long>(N);
+  p.idx[0] = c.take<int>(N);
+  p.idx[1] = c.take<int>(N);
+  p.list[0] = c.take<int>(batch);
+  p.list[1] = c.take<int>(batch);
+  return c.bytes();
 }
 
 }  // namespace ups
 
 extern "C" int upsnet_rpn_targets_workspace_bytes(long long num_anchors, int batch_size, size_t* bytes) {
   if (!bytes || num_anchors <= 0 || num_anchors >= (1ll << 31) || batch_size <= 0) return UPSNET_E_BADARG;
-  *bytes = ups::rt_layout(num_anchors, batch_size).total;
+  ups::RtParams p{};
+  *bytes = ups::rt_layout(num_anchors, batch_size, nullptr, p);
   return 0;
 }
 
@@ -405,26 +399,12 @@ extern "C" int upsnet_rpn_targets(const float* gt_boxes, int G, const double* ce
   }
   p.off[L] = N;
   if (N >= (1ll << 31)) return UPSNET_E_UNSUPPORTED;
-  const RtLayout lo = rt_layout(N, batch_size);
-  if (workspace_bytes < lo.total) return UPSNET_E_WORKSPACE;
-  char* ws = (char*)workspace;
+  if (workspace_bytes < rt_layout(N, batch_size, workspace, p)) return UPSNET_E_WORKSPACE;
   p.gt = gt_boxes; p.cell = cell_anchors;
   p.L = L; p.A = A; p.N = (int)N; p.G = G; p.nblk = (int)((N + kRtThreads - 1) / kRtThreads);
   p.batch = batch_size; p.num_fg = num_fg;
   p.im_h = im_height; p.im_w = im_width; p.straddle = straddle_thresh;
   p.pos = positive_overlap; p.neg = negative_overlap; p.seed = seed;
-  p.st = (RtState*)(ws + lo.state);
-  p.gtmax = (unsigned int*)(ws + lo.gtmax);
-  p.amax = (float*)(ws + lo.amax);
-  p.aarg = (int*)(ws + lo.aarg);
-  p.flags = (unsigned char*)(ws + lo.flags);
-  p.blk = (int*)(ws + lo.blk);
-  p.keys[0] = (unsigned long long*)(ws + lo.keys0);
-  p.keys[1] = (unsigned long long*)(ws + lo.keys1);
-  p.idx[0] = (int*)(ws + lo.idx0);
-  p.idx[1] = (int*)(ws + lo.idx1);
-  p.list[0] = (int*)(ws + lo.list0);
-  p.list[1] = (int*)(ws + lo.list1);
   p.labels = labels; p.targets = bbox_targets; p.inside_w = inside_weights; p.outside_w = outside_weights;
   p.counts = counts;
   cudaStream_t st = (cudaStream_t)stream;

@@ -40,7 +40,7 @@ import ctypes as C
 import numpy as np
 import torch
 
-from ._lib import UpsnetError, check, lib, ptr, stream_ptr
+from ._lib import UpsnetError, call, query_bytes
 from .operators import label_restore_geometry, label_restore_index
 
 MAX_GT = 4096          # UPSNET_PQ_MAX_GT: ground-truth segments per image
@@ -111,9 +111,8 @@ class PanopticQuality:
         self._counts = torch.zeros((3, 256), dtype=torch.int64, device=self.device)    # tp, fp, fn
         self._iou = torch.zeros((256,), dtype=torch.float64, device=self.device)
         self._err = torch.zeros((1,), dtype=torch.int32, device=self.device)
-        nb = C.c_size_t(0)
-        check(lib().upsnet_pq_workspace_bytes(C.byref(nb)), "pq_workspace_bytes")
-        self._ws = torch.empty((nb.value,), dtype=torch.uint8, device=self.device)
+        nb = query_bytes("pq_workspace_bytes")
+        self._ws = torch.empty((nb,), dtype=torch.uint8, device=self.device)
         # segment-table staging: a ring of pinned host / device buffer pairs, each guarded by the event of its last
         # H2D copy.  A slot used inside a CUDA-graph capture is taken out of the ring: the graph reads it at replay.
         self._stage = [(torch.empty((5 * MAX_GT,), dtype=torch.int64, pin_memory=True),
@@ -158,10 +157,8 @@ class PanopticQuality:
                 ev.record(torch.cuda.current_stream(self.device))
                 self._stage[k] = (host, tdev, ev)
             self._next += 1
-        with torch.cuda.device(self.device):
-            check(lib().upsnet_pq_update(ptr(pan), ptr(gt), H, W, ptr(tdev), G, ptr(self._flags), ptr(self._counts),
-                                         ptr(self._iou), ptr(self._err), ptr(self._ws), self._ws.numel(),
-                                         stream_ptr(self.device)), "pq_update")
+        call("pq_update", self.device, pan, gt, H, W, tdev, G, self._flags, self._counts,
+             self._iou, self._err, self._ws, self._ws.numel())
         if check_errors:
             self.check_errors()
 
@@ -291,10 +288,8 @@ class SegmentationIoU:
         if torch.cuda.is_current_stream_capturing():
             self._captured.append(tab)
         H, W = gt_hw
-        with torch.cuda.device(self.device):
-            check(lib().upsnet_sseg_update(ptr(p), p.element_size(), pred_hw[1], ptr(tab), C.c_void_p(tab.data_ptr() + 4 * H),
-                                           ptr(g), H, W, self.num_classes, ptr(self._acc), stream_ptr(self.device)),
-                  "sseg_update")
+        call("sseg_update", self.device, p, p.element_size(), pred_hw[1], tab, C.c_void_p(tab.data_ptr() + 4 * H),
+             g, H, W, self.num_classes, self._acc)
 
     def confusion_matrix(self):
         """float64 [C, C] (row = ground truth, column = prediction): the matrix the reference accumulates."""
@@ -546,10 +541,9 @@ class DetectionAP:
                 H, W = (int(v) for v in im_size)
             elif G:
                 H, W = int(table[7, 0]), int(table[8, 0])
-            nb = C.c_size_t(0)
-            check(lib().upsnet_cocoeval_workspace_bytes(n, cap, int(counts.size), C.byref(nb)), "cocoeval_workspace_bytes")
-            if self._ws.numel() < nb.value:
-                self._ws = torch.empty((nb.value,), dtype=torch.uint8, device=self.device)
+            nb = query_bytes("cocoeval_workspace_bytes", n, cap, int(counts.size))
+            if self._ws.numel() < nb:
+                self._ws = torch.empty((nb,), dtype=torch.uint8, device=self.device)
         if n_dev is not None and (not n_dev.is_cuda or n_dev.dtype != torch.int32):
             raise ValueError("n_dev must be a device int32 tensor")
         if G <= MAX_AP_GT:
@@ -557,12 +551,10 @@ class DetectionAP:
         else:                          # only counted: the device raises the error flag without reading the table
             t_ptr = o_ptr = c_ptr = None
         slot = len(self._image_ids)
-        with torch.cuda.device(self.device):
-            check(lib().upsnet_cocoeval_image(int(segm), ptr(b), ptr(s), ptr(c), n, ptr(n_dev), ptr(cnt), cap, ptr(rl), H, W,
-                                              t_ptr, G, c_ptr, o_ptr, len(self.cat_ids), ptr(self._cls_to_k), slot,
-                                              ptr(self._records), self.record_capacity, ptr(self._n_rec), ptr(self._npig),
-                                              ptr(self._err), ptr(self._ws), self._ws.numel(), stream_ptr(self.device)),
-                  "cocoeval_image")
+        call("cocoeval_image", self.device, int(segm), b, s, c, n, n_dev, cnt, cap, rl, H, W,
+             t_ptr, G, c_ptr, o_ptr, len(self.cat_ids), self._cls_to_k, slot,
+             self._records, self.record_capacity, self._n_rec, self._npig,
+             self._err, self._ws, self._ws.numel())
         self._image_ids.append(image_id)
         self._seen.add(image_id)
 
@@ -581,18 +573,15 @@ class DetectionAP:
         rank = np.empty(len(self._image_ids), np.int32)
         rank[np.argsort(np.asarray(self._image_ids), kind="stable")] = np.arange(len(self._image_ids), dtype=np.int32)
         rank_d = torch.from_numpy(rank).to(self.device)
-        nb = C.c_size_t(0)
-        check(lib().upsnet_cocoeval_accumulate_workspace_bytes(N, C.byref(nb)), "cocoeval_accumulate_workspace_bytes")
-        ws = torch.empty((max(nb.value, 1),), dtype=torch.uint8, device=self.device)
+        nb = query_bytes("cocoeval_accumulate_workspace_bytes", N)
+        ws = torch.empty((max(nb, 1),), dtype=torch.uint8, device=self.device)
         f64 = dict(dtype=torch.float64, device=self.device)
         out = torch.empty((2 * 10 * 101 * K * 12 + 10 * K * 12,), **f64)
         precision = out[:10 * 101 * K * 12].view(10, 101, K, 4, 3)
         scores = out[10 * 101 * K * 12:2 * 10 * 101 * K * 12].view(10, 101, K, 4, 3)
         recall = out[2 * 10 * 101 * K * 12:].view(10, K, 4, 3)
-        with torch.cuda.device(self.device):
-            check(lib().upsnet_cocoeval_accumulate(ptr(self._records), N, ptr(rank_d), ptr(self._npig), K, ptr(precision),
-                                                   ptr(recall), ptr(scores), ptr(ws), ws.numel(), stream_ptr(self.device)),
-                  "cocoeval_accumulate")
+        call("cocoeval_accumulate", self.device, self._records, N, rank_d, self._npig, K, precision,
+             recall, scores, ws, ws.numel())
         host = out.cpu().numpy()                                         # the one copy back
         n1 = 10 * 101 * K * 12
         return {"precision": host[:n1].reshape(10, 101, K, 4, 3), "scores": host[n1:2 * n1].reshape(10, 101, K, 4, 3),

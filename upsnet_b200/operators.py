@@ -25,7 +25,7 @@ from torch.nn.modules.utils import _pair
 from torch.nn.parameter import Parameter
 
 from . import _lib
-from ._lib import check, f32c, lib, ptr, require_cuda, stream_ptr
+from ._lib import call, f32c, query_bytes, require_cuda, try_call
 
 # default arithmetic of the convolution tiles; switched by upsnet_b200.set_precision()
 _PRECISION = {"conv": _lib.PREC_FP32_SIMT}
@@ -179,13 +179,10 @@ def _packed_weight(weight):
 
 def _pack_igemm(weight):
     Cout, Cin, kh, kw = weight.shape
-    nbytes = C.c_size_t(0)
-    check(lib().upsnet_igemm_packed_weight_bytes(Cout, Cin, kh, kw, C.byref(nbytes)), "igemm_packed_weight_bytes")
-    buf = torch.empty(nbytes.value, dtype=torch.uint8, device=weight.device)
+    nbytes = query_bytes("igemm_packed_weight_bytes", Cout, Cin, kh, kw)
+    buf = torch.empty(nbytes, dtype=torch.uint8, device=weight.device)
     w = f32c(weight.detach())
-    with torch.cuda.device(weight.device):
-        check(lib().upsnet_igemm_pack_weight(ptr(w), Cout, Cin, kh, kw, ptr(buf), stream_ptr(weight.device)),
-              "igemm_pack_weight")
+    call("igemm_pack_weight", weight.device, w, Cout, Cin, kh, kw, buf)
     STATS["launches"] += 1
     return buf
 
@@ -201,17 +198,13 @@ def _packed_weight_dcn(weight):
 
 def _pack_dcn(weight):
     Cout, Cin, kh, kw = weight.shape
-    nbytes = C.c_size_t(0)
-    rc = lib().upsnet_dcn_packed_weight_bytes(Cout, Cin, kh, kw, C.byref(nbytes))
-    buf = None
-    if rc == 0:
-        buf = torch.empty(nbytes.value, dtype=torch.uint8, device=weight.device)
-        w = f32c(weight.detach())
-        with torch.cuda.device(weight.device):
-            check(lib().upsnet_dcn_pack_weight(ptr(w), Cout, Cin, kh, kw, ptr(buf), stream_ptr(weight.device)), "dcn_pack_weight")
-        STATS["launches"] += 1
-    elif rc != -2:
-        check(rc, "dcn_packed_weight_bytes")
+    nbytes = query_bytes("dcn_packed_weight_bytes", Cout, Cin, kh, kw, unsupported=True)
+    if nbytes is None:
+        return None
+    buf = torch.empty(nbytes, dtype=torch.uint8, device=weight.device)
+    w = f32c(weight.detach())
+    call("dcn_pack_weight", weight.device, w, Cout, Cin, kh, kw, buf)
+    STATS["launches"] += 1
     return buf
 
 
@@ -231,13 +224,10 @@ def _dcn_window(x, offset, mask, weight, bias, padding, dilation, relu):
     work = {"flops": 2.0 * N * Ho * Wo * Cout * Cin * kh * kw * 3, "algo_flops": 2.0 * N * Ho * Wo * Cout * Cin * kh * kw,
             "shape": "N%d %dx%d Cin%d->Cout%d k%d s1 pair->pair (window)" % (N, H, W, Cin, Cout, kh),
             "bytes": float(x.store.numel() * 2 + 4 * weight.numel() + store.numel() * 2 + offset.numel() * 4)}
-    with torch.cuda.device(x.device), _Timed("dcn", 1, work, x.device):
-        rc = lib().upsnet_dcn_pair_forward(ptr(x.store), ptr(offset), ptr(mask), ptr(packed), ptr(bias), ptr(store), N, H, W,
-                                           Cin, Cout, kh, kw, ph, pw, dh, dw, _lib.EPI_RELU if relu else 0, stream_ptr(x.device))
-    if rc == -2:
-        return None
-    check(rc, "dcn_pair_forward")
-    return Pair(store)
+    with _Timed("dcn", 1, work, x.device):
+        rc = try_call("dcn_pair_forward", x.device, x.store, offset, mask, packed, bias, store, N, H, W, Cin, Cout, kh, kw,
+                      ph, pw, dh, dw, _lib.EPI_RELU if relu else 0)
+    return None if rc == _lib.E_UNSUPPORTED else Pair(store)
 
 
 _stem_cache = {}   # packed bf16 [Cout][kh][8][8] per weight
@@ -257,31 +247,27 @@ def stem_conv(x, weight, bias, padding, relu=True, pair=False):
     dev = x.device
 
     def pack():
-        nb = C.c_size_t(0)
-        check(lib().upsnet_stem_packed_weight_bytes(Cout, kh, C.byref(nb)), "stem_packed_weight_bytes")
-        packed = torch.empty(nb.value, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            check(lib().upsnet_stem_pack_weight(ptr(f32c(weight.detach())), Cout, Cin, kh, kw, ptr(packed), stream_ptr(dev)),
-                  "stem_pack_weight")
+        nb = query_bytes("stem_packed_weight_bytes", Cout, kh)
+        packed = torch.empty(nb, dtype=torch.uint8, device=dev)
+        call("stem_pack_weight", dev, f32c(weight.detach()), Cout, Cin, kh, kw, packed)
         STATS["launches"] += 1
         return packed
 
     packed = _per_weight(_stem_cache, weight, pack, device=dev)
-    nb = C.c_size_t(0)
-    check(lib().upsnet_stem_workspace_bytes(N, H, W, kh, kw, int(padding), C.byref(nb)), "stem_workspace_bytes")
+    nb = query_bytes("stem_workspace_bytes", N, H, W, kh, kw, int(padding))
     if _stem_ws is None:
         _stem_ws = _Workspace()
-    ws = _stem_ws.get(dev, nb.value)
+    ws = _stem_ws.get(dev, nb)
     Ho, Wo = (H + 2 * padding - kh) // 2 + 1, (W + 2 * padding - kw) // 2 + 1
     store = torch.empty((N, Ho, Wo, Cout * (2 if pair else 1)), dtype=torch.bfloat16, device=dev)
     fl = 2.0 * N * Ho * Wo * Cout * Cin * kh * kw
     work = {"flops": fl * (3 if pair else 1), "algo_flops": fl,
             "shape": "N%d %dx%d Cin%d->Cout%d k%d s2 float32->%s (stem, TMA)" % (N, H, W, Cin, Cout, kh, "pair" if pair else "bfloat16"),
             "bytes": float(4 * x.numel() + 2 * store.numel())}
-    with torch.cuda.device(dev), _Timed("conv2d", 2, work, dev):
-        check(lib().upsnet_stem_forward(ptr(x), ptr(packed), ptr(None if bias is None else f32c(bias)), ptr(store), N, Cin, H, W,
-                                        Cout, kh, kw, int(padding), (_lib.EPI_RELU if relu else 0) | (_lib.EPI_STEM_PAIR if pair else 0),
-                                        ptr(ws), ws.numel(), stream_ptr(dev)), "stem_forward")
+    with _Timed("conv2d", 2, work, dev):
+        call("stem_forward", dev, x, packed, None if bias is None else f32c(bias), store, N, Cin, H, W,
+             Cout, kh, kw, int(padding), (_lib.EPI_RELU if relu else 0) | (_lib.EPI_STEM_PAIR if pair else 0),
+             ws, ws.numel())
     return Pair(store) if pair else store.permute(0, 3, 1, 2)
 
 
@@ -368,11 +354,11 @@ def _igemm_tc(kind, x, offset, mask, weight, bias, residual, stride, padding, di
     if sigmoid_from is not None:
         assert not pair_out and not nhwc_out and residual is None, "sigmoid epilogue: fp32 NCHW head outputs"
         flags |= _lib.EPI_SIGMOID_FROM(sigmoid_from)
-    with torch.cuda.device(dev), _Timed(kind, 1, work, dev):
-        check(lib().upsnet_igemm_forward(ptr(xs), ptr(offset), ptr(mask), ptr(packed), ptr(bias), ptr(res),
-                                         ptr(store), N, H, W, Cin, Cout, kh, kw, sh, sw, ph, pw, dh, dw,
-                                         _lib.LAYOUT_NHWC if nhwc_out else _lib.LAYOUT_NCHW, x_dt, y_dt, flags,
-                                         prec, ptr(_count(n_dev)), stream_ptr(dev)), kind)
+    with _Timed(kind, 1, work, dev):
+        call("igemm_forward", dev, xs, offset, mask, packed, bias, res,
+             store, N, H, W, Cin, Cout, kh, kw, sh, sw, ph, pw, dh, dw,
+             _lib.LAYOUT_NHWC if nhwc_out else _lib.LAYOUT_NCHW, x_dt, y_dt, flags,
+             prec, _count(n_dev))
     if pair_out:
         if pair_group:
             return Pair(store.view(N, Ho, Wo * (Cout // pair_group), 2 * pair_group))
@@ -420,10 +406,9 @@ def conv2d(x, weight, bias=None, stride=1, padding=0, dilation=1, residual=None,
     prec = _lib.PREC_FP32_SIMT
     work = {"flops": 2.0 * N * Ho * Wo * Cout * Cin * kh * kw, "algo_flops": 2.0 * N * Ho * Wo * Cout * Cin * kh * kw,
             "bytes": 4.0 * (x.numel() + weight.numel() + y.numel() * (2 if residual is not None else 1))}
-    with torch.cuda.device(x.device), _Timed("conv2d_simt", 1, work, x.device):
-        check(lib().upsnet_conv2d_forward(ptr(x), ptr(weight), ptr(bias), ptr(residual), ptr(y), N, Cin, H, W,
-                                          Cout, kh, kw, sh, sw, ph, pw, dh, dw, _lib.EPI_RELU if relu else 0,
-                                          prec, stream_ptr(x.device)), "conv2d")
+    with _Timed("conv2d_simt", 1, work, x.device):
+        call("conv2d_forward", x.device, x, weight, bias, residual, y, N, Cin, H, W,
+             Cout, kh, kw, sh, sw, ph, pw, dh, dw, _lib.EPI_RELU if relu else 0, prec)
     return y
 
 
@@ -485,11 +470,10 @@ def deform_conv(data, offset, weight, bias=None, stride=1, padding=0, dilation=1
     work = {"flops": 2.0 * N * Ho * Wo * Cout * Cin * kh * kw, "algo_flops": 2.0 * N * Ho * Wo * Cout * Cin * kh * kw,
             "bytes": 4.0 * (data.numel() + offset.numel() + weight.numel() + y.numel() +
                             (mask.numel() if mask is not None else 0))}
-    with torch.cuda.device(data.device), _Timed("dcn_simt", 1, work, data.device):
-        check(lib().upsnet_dcn_forward(ptr(data), ptr(offset), ptr(mask), ptr(weight), ptr(bias), ptr(y), N, Cin,
-                                       H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, deformable_groups,
-                                       _lib.EPI_RELU if relu else 0, prec, stream_ptr(data.device)),
-              "deform_conv")
+    with _Timed("dcn_simt", 1, work, data.device):
+        call("dcn_forward", data.device, data, offset, mask, weight, bias, y, N, Cin,
+             H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, deformable_groups,
+             _lib.EPI_RELU if relu else 0, prec)
     return y
 
 
@@ -508,10 +492,9 @@ def roi_align(features, rois, pooled_height, pooled_width, spatial_scale, sampli
         lay = _lib.LAYOUT_NHWC
     if R == 0:
         return out
-    with torch.cuda.device(features.device), _Timed("roi_align", 1, {"bytes": 4.0 * out.numel()}, features.device):
-        check(lib().upsnet_roi_align_forward(ptr(features), B, Cc, H, W, lay, 0, ptr(rois), R, pooled_height,
-                                             pooled_width, sampling_ratio, float(spatial_scale), ptr(out),
-                                             stream_ptr(features.device)), "roi_align")
+    with _Timed("roi_align", 1, {"bytes": 4.0 * out.numel()}, features.device):
+        call("roi_align_forward", features.device, features, B, Cc, H, W, lay, 0, rois, R, pooled_height,
+             pooled_width, sampling_ratio, float(spatial_scale), out)
     return out
 
 
@@ -524,17 +507,16 @@ def max_pool2d(x, kernel_size, stride, padding):
     Wo = (W + 2 * padding - kernel_size) // stride + 1
     if isinstance(x, Pair):
         store = torch.empty((N, Ho, Wo, 2 * Cc), device=x.device, dtype=torch.bfloat16)
-        with torch.cuda.device(x.device), _Timed("maxpool", 1, {"bytes": float((x.store.numel() + store.numel()) * 2)}, x.device):
-            check(lib().upsnet_maxpool2d_nhwc(ptr(x.store), ptr(store), N, H, W, Cc, kernel_size, stride, padding,
-                                              _lib.DTYPE_PAIR, stream_ptr(x.device)), "maxpool2d")
+        with _Timed("maxpool", 1, {"bytes": float((x.store.numel() + store.numel()) * 2)}, x.device):
+            call("maxpool2d_nhwc", x.device, x.store, store, N, H, W, Cc, kernel_size, stride, padding, _lib.DTYPE_PAIR)
         return Pair(store)
     if x.dtype not in (torch.float32, torch.bfloat16):
         x = x.float()
     xs = _nhwc(x)
     store = torch.empty((N, Ho, Wo, Cc), device=x.device, dtype=x.dtype)
-    with torch.cuda.device(x.device), _Timed("maxpool", 1, {"bytes": float((xs.numel() + store.numel()) * x.element_size())}, x.device):
-        check(lib().upsnet_maxpool2d_nhwc(ptr(xs), ptr(store), N, H, W, Cc, kernel_size, stride, padding,
-                                          1 if x.dtype == torch.bfloat16 else 0, stream_ptr(x.device)), "maxpool2d")
+    with _Timed("maxpool", 1, {"bytes": float((xs.numel() + store.numel()) * x.element_size())}, x.device):
+        call("maxpool2d_nhwc", x.device, xs, store, N, H, W, Cc, kernel_size, stride, padding,
+             1 if x.dtype == torch.bfloat16 else 0)
     return store.permute(0, 3, 1, 2)
 
 
@@ -545,8 +527,8 @@ def upsample_bilinear(x, factor):
     x = f32c(x)
     N, Cc, H, W = x.shape
     y = torch.empty((N, Cc, H * factor, W * factor), dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device), _Timed("upsample", 1, {"bytes": 4.0 * (x.numel() + y.numel())}, x.device):
-        check(lib().upsnet_upsample_bilinear_nchw(ptr(x), ptr(y), N * Cc, H, W, int(factor), stream_ptr(x.device)), "upsample")
+    with _Timed("upsample", 1, {"bytes": 4.0 * (x.numel() + y.numel())}, x.device):
+        call("upsample_bilinear_nchw", x.device, x, y, N * Cc, H, W, int(factor))
     return y
 
 
@@ -558,9 +540,8 @@ def fcn_score_fuse(s2, s3, s4, s5):
     N, Cc, H, W = s2.shape
     assert s3.shape == (N, Cc, H // 2, W // 2) and s4.shape == (N, Cc, H // 4, W // 4) and s5.shape == (N, Cc, H // 8, W // 8)
     out = torch.empty_like(s2)
-    with torch.cuda.device(s2.device), _Timed("upsample", 1, {"bytes": 4.0 * (2 * s2.numel() + s3.numel() + s4.numel() + s5.numel())}, s2.device):
-        check(lib().upsnet_fcn_score_fuse(ptr(s2), ptr(s3), ptr(s4), ptr(s5), ptr(out), N * Cc, H, W, stream_ptr(s2.device)),
-              "fcn_score_fuse")
+    with _Timed("upsample", 1, {"bytes": 4.0 * (2 * s2.numel() + s3.numel() + s4.numel() + s5.numel())}, s2.device):
+        call("fcn_score_fuse", s2.device, s2, s3, s4, s5, out, N * Cc, H, W)
     return out
 
 
@@ -586,12 +567,10 @@ def fpn_roi_align(feats, rois, pooled_height, pooled_width, spatial_scales, samp
             fp = (C.c_void_p * 4)(*[f.store.data_ptr() for f in feats])
             hs = (C.c_int * 4)(*[f.shape[2] for f in feats]); ws = (C.c_int * 4)(*[f.shape[3] for f in feats])
             sc = (C.c_float * 4)(*[float(s_) for s_ in spatial_scales])
-            with torch.cuda.device(rois.device), _Timed("roi_align_fpn", 1, {"bytes": 2.0 * out.numel()}, rois.device):
-                check(lib().upsnet_roi_align_fpn_forward(fp, hs, ws, sc, B, Cc, _lib.LAYOUT_FLAT_PAIR if flat else _lib.LAYOUT_NHWC,
-                                                         _lib.DTYPE_PAIR, ptr(rois), R, pooled_height, pooled_width,
-                                                         sampling_ratio, ptr(out), ptr(None), ptr(_count(n_dev)),
-                                                         stream_ptr(rois.device)),
-                      "fpn_roi_align")
+            with _Timed("roi_align_fpn", 1, {"bytes": 2.0 * out.numel()}, rois.device):
+                call("roi_align_fpn_forward", rois.device, fp, hs, ws, sc, B, Cc,
+                     _lib.LAYOUT_FLAT_PAIR if flat else _lib.LAYOUT_NHWC, _lib.DTYPE_PAIR, rois, R, pooled_height,
+                     pooled_width, sampling_ratio, out, None, _count(n_dev))
         return Pair(out)
     if layout == "auto":
         # engine tensors: logical NCHW; if every level is stored channels_last use the NHWC kernel
@@ -620,10 +599,9 @@ def fpn_roi_align(feats, rois, pooled_height, pooled_width, spatial_scales, samp
     fp = (C.c_void_p * 4)(*[f.data_ptr() for f in feats])
     hs = (C.c_int * 4)(*Hs); ws = (C.c_int * 4)(*Ws)
     sc = (C.c_float * 4)(*[float(s) for s in spatial_scales])
-    with torch.cuda.device(rois.device), _Timed("roi_align_fpn", 1, {"bytes": 4.0 * out.numel()}, rois.device):
-        check(lib().upsnet_roi_align_fpn_forward(fp, hs, ws, sc, B, Cc, lay, 1 if bf16 else 0, ptr(rois), R, pooled_height,
-                                                 pooled_width, sampling_ratio, ptr(out), ptr(levels), ptr(None),
-                                                 stream_ptr(rois.device)), "fpn_roi_align")
+    with _Timed("roi_align_fpn", 1, {"bytes": 4.0 * out.numel()}, rois.device):
+        call("roi_align_fpn_forward", rois.device, fp, hs, ws, sc, B, Cc, lay, 1 if bf16 else 0, rois, R, pooled_height,
+             pooled_width, sampling_ratio, out, levels, None)
     return (out, levels) if return_levels else out
 
 
@@ -687,14 +665,12 @@ def nms_segmented(boxes_sorted, seg_offsets, max_seg_len, thresh, side=False):
     assert seg_offsets.dtype == torch.int32
     S = seg_offsets.numel() - 1
     dev = boxes_sorted.device
-    nbytes = C.c_size_t(0)
-    check(lib().upsnet_nms_workspace_bytes(S, max_seg_len, C.byref(nbytes)), "nms_workspace_bytes")
-    ws = (_nms_ws_side if side else _nms_ws).get(dev, nbytes.value)
+    nbytes = query_bytes("nms_workspace_bytes", S, max_seg_len)
+    ws = (_nms_ws_side if side else _nms_ws).get(dev, nbytes)
     keep = torch.empty((S, max_seg_len), dtype=torch.int32, device=dev)
     cnt = torch.empty((S,), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev), _Timed("nms", 2, {"bytes": 20.0 * boxes_sorted.shape[0]}, dev):
-        check(lib().upsnet_nms_segmented(ptr(boxes_sorted), ptr(seg_offsets), S, max_seg_len, float(thresh),
-                                         ptr(keep), ptr(cnt), ptr(ws), ws.numel(), stream_ptr(dev)), "nms")
+    with _Timed("nms", 2, {"bytes": 20.0 * boxes_sorted.shape[0]}, dev):
+        call("nms_segmented", dev, boxes_sorted, seg_offsets, S, max_seg_len, float(thresh), keep, cnt, ws, ws.numel())
     return keep, cnt
 
 
@@ -712,11 +688,10 @@ def rpn_decode(bbox_preds, top_idx, shapes, strides, base_anchors, A, im_h, im_w
     ks = [int(t.numel()) for t in top_idx]
     out = torch.empty((sum(ks), 4), dtype=torch.float32, device=dev)
     vp, ci = C.c_void_p, C.c_int
-    with torch.cuda.device(dev), _Timed("rpn_decode", 1, {"bytes": 56.0 * sum(ks)}, dev):
-        check(lib().upsnet_rpn_decode((vp * L)(*[b.data_ptr() for b in bbox_preds]), (vp * L)(*[t.data_ptr() for t in top_idx]),
-                                      (ci * L)(*ks), (ci * L)(*[int(s[0]) for s in shapes]), (ci * L)(*[int(s[1]) for s in shapes]),
-                                      (ci * L)(*[int(s) for s in strides]), ptr(base_anchors), L, int(A), float(im_h), float(im_w),
-                                      ptr(out), stream_ptr(dev)), "rpn_decode")
+    with _Timed("rpn_decode", 1, {"bytes": 56.0 * sum(ks)}, dev):
+        call("rpn_decode", dev, (vp * L)(*[b.data_ptr() for b in bbox_preds]), (vp * L)(*[t.data_ptr() for t in top_idx]),
+             (ci * L)(*ks), (ci * L)(*[int(s[0]) for s in shapes]), (ci * L)(*[int(s[1]) for s in shapes]),
+             (ci * L)(*[int(s) for s in strides]), base_anchors, L, int(A), float(im_h), float(im_w), out)
     return out
 
 
@@ -736,14 +711,13 @@ def rpn_topk(probs, A, pre_nms_top_n):
     out_i = torch.empty((sum(ks),), dtype=torch.int64, device=dev)
     if _topk_ws is None:
         _topk_ws = _Workspace()
-    nbytes = C.c_size_t(0)
-    check(lib().upsnet_rpn_topk_workspace_bytes(L, C.byref(nbytes)), "rpn_topk_workspace_bytes")
-    ws = _topk_ws.get(dev, nbytes.value)
+    nbytes = query_bytes("rpn_topk_workspace_bytes", L)
+    ws = _topk_ws.get(dev, nbytes)
     vp, ci = C.c_void_p, C.c_int
-    with torch.cuda.device(dev), _Timed("rpn_topk", 7, {"bytes": 4.0 * 6 * sum(pr.numel() for pr in probs)}, dev):
-        check(lib().upsnet_rpn_topk((vp * L)(*[pr.data_ptr() for pr in probs]), (ci * L)(*[int(pr.shape[-2]) for pr in probs]),
-                                    (ci * L)(*[int(pr.shape[-1]) for pr in probs]), L, int(A), int(pre_nms_top_n),
-                                    ptr(out_s), ptr(out_i), ptr(ws), ws.numel(), stream_ptr(dev)), "rpn_topk")
+    with _Timed("rpn_topk", 7, {"bytes": 4.0 * 6 * sum(pr.numel() for pr in probs)}, dev):
+        call("rpn_topk", dev, (vp * L)(*[pr.data_ptr() for pr in probs]), (ci * L)(*[int(pr.shape[-2]) for pr in probs]),
+             (ci * L)(*[int(pr.shape[-1]) for pr in probs]), L, int(A), int(pre_nms_top_n),
+             out_s, out_i, ws, ws.numel())
     return out_s, out_i, ks
 
 
@@ -756,9 +730,8 @@ def rpn_collect(keep, cnt, offs, boxes, scores, post_nms_top_n):
     rois = torch.empty((post, 5), dtype=torch.float32, device=dev)
     out_s = torch.empty((post,), dtype=torch.float32, device=dev)
     ok = torch.empty((post,), dtype=torch.bool, device=dev)
-    with torch.cuda.device(dev), _Timed("rpn_collect", 1, {"bytes": 28.0 * post}, dev):
-        check(lib().upsnet_rpn_collect(ptr(keep), ptr(cnt), ptr(offs), ptr(f32c(boxes)), ptr(f32c(scores)), S, M, post,
-                                       ptr(rois), ptr(out_s), ptr(ok), stream_ptr(dev)), "rpn_collect")
+    with _Timed("rpn_collect", 1, {"bytes": 28.0 * post}, dev):
+        call("rpn_collect", dev, keep, cnt, offs, f32c(boxes), f32c(scores), S, M, post, rois, out_s, ok)
     return rois, out_s, ok
 
 
@@ -777,10 +750,10 @@ def maskroi_prepare(rois, roi_valid, bbox_delta, cls_prob, class_agnostic, score
     bx = torch.empty((n, 4), dtype=torch.float32, device=dev)
     offs = torch.empty((nseg + 1,), dtype=torch.int32, device=dev)
     w4 = (C.c_float * 4)(*[float(w) for w in weights])
-    with torch.cuda.device(dev), _Timed("maskroi", 1, {"bytes": 4.0 * (rois.numel() + bbox_delta.numel() + cls_prob.numel())}, dev):
-        check(lib().upsnet_maskroi_prepare(ptr(rois), ptr(roi_valid), ptr(bbox_delta), ptr(cls_prob), R, Cn,
-                                           1 if class_agnostic else 0, float(score_thresh), w4, float(im_h), float(im_w),
-                                           ptr(sc), ptr(cls), ptr(bx), ptr(offs), stream_ptr(dev)), "maskroi_prepare")
+    with _Timed("maskroi", 1, {"bytes": 4.0 * (rois.numel() + bbox_delta.numel() + cls_prob.numel())}, dev):
+        call("maskroi_prepare", dev, rois, roi_valid, bbox_delta, cls_prob, R, Cn,
+             1 if class_agnostic else 0, float(score_thresh), w4, float(im_h), float(im_w),
+             sc, cls, bx, offs)
     return sc, cls, bx, offs
 
 
@@ -795,10 +768,9 @@ def maskroi_finish(keep, cnt, offs, sc, cls, bx, top_n, cap):
     out_bx = torch.empty((cap, 5), dtype=torch.float32, device=dev)
     out_cls = torch.empty((cap,), dtype=torch.int64, device=dev)
     n_out = torch.empty((2,), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev), _Timed("maskroi", 1, {"bytes": 32.0 * cap}, dev):
-        check(lib().upsnet_maskroi_finish(ptr(keep), ptr(cnt), ptr(offs), ptr(sc), ptr(cls), ptr(bx), nseg, M, int(top_n),
-                                          int(cap), ptr(out_sc), ptr(out_bx), ptr(out_cls), ptr(n_out), stream_ptr(dev)),
-              "maskroi_finish")
+    with _Timed("maskroi", 1, {"bytes": 32.0 * cap}, dev):
+        call("maskroi_finish", dev, keep, cnt, offs, sc, cls, bx, nseg, M, int(top_n),
+             int(cap), out_sc, out_bx, out_cls, n_out)
     return out_sc, out_bx, out_cls, n_out[0], n_out[1]
 
 
@@ -814,9 +786,8 @@ def mask_rows(b1, n1, b2, n2):
     rows = torch.empty((cap1 + cap2, 5), dtype=torch.float32, device=dev)
     u = torch.empty((), dtype=torch.int32, device=dev)
     pan_row = torch.empty((cap2,), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev), _Timed("maskroi", 1, {"bytes": 40.0 * (cap1 + cap2)}, dev):
-        check(lib().upsnet_mask_rows(ptr(b1), ptr(_count(n1)), cap1, ptr(b2), ptr(_count(n2)), cap2, ptr(rows), ptr(u),
-                                     ptr(pan_row), stream_ptr(dev)), "mask_rows")
+    with _Timed("maskroi", 1, {"bytes": 40.0 * (cap1 + cap2)}, dev):
+        call("mask_rows", dev, b1, _count(n1), cap1, b2, _count(n2), cap2, rows, u, pan_row)
     return rows, u, pan_row
 
 
@@ -1044,10 +1015,9 @@ def panoptic_fuse(fcn_output, mask_rois, cls_prob, mask_logit, cls_idx, num_stuf
     assert boxes.shape == (n, 4) and prob.numel() == n and ml.numel() == n * 784 and cls.numel() == n
     dev = fcn.device
     num_thing = S - num_stuff
-    nbytes = C.c_size_t(0)
-    check(lib().upsnet_panoptic_workspace_bytes(n, H, W, num_thing, C.byref(nbytes)), "panoptic_workspace_bytes")
+    nbytes = query_bytes("panoptic_workspace_bytes", n, H, W, num_thing)
     if workspace_bytes is None:
-        ws = _pan_ws.get(dev, nbytes.value)
+        ws = _pan_ws.get(dev, nbytes)
     else:
         # caller-chosen (smaller) workspace: the instances' bit windows are then processed in several rounds of
         # consecutive score ranks -- same results (upsnet_panoptic_workspace_min_bytes is the floor)
@@ -1059,15 +1029,15 @@ def panoptic_fuse(fcn_output, mask_rois, cls_prob, mask_logit, cls_idx, num_stuf
     labels = torch.empty((1, H, W), dtype=torch.int64, device=dev)
     sem = torch.empty((1, H, W), dtype=torch.int64, device=dev) if want_sem else None
     work = {"bytes": 4.0 * S * H * W / (16 if up4 else 1) + 8.0 * H * W * (2 if want_sem else 1) + n * (4.0 * 784 + 24)}
-    with torch.cuda.device(dev), _Timed("panoptic_head", 5, work, dev):
+    with _Timed("panoptic_head", 5, work, dev):
         if up4:
-            check(lib().upsnet_panoptic_head_up4(ptr(fcn), S, Hs, Ws, ptr(boxes), ptr(prob), ptr(ml), ptr(cls), n, ptr(n_dev),
-                                                 num_stuff, float(fraction_threshold), ptr(keep), ptr(k), ptr(labels),
-                                                 ptr(sem), ptr(ws), ws.numel(), stream_ptr(dev)), "panoptic_head_up4")
+            call("panoptic_head_up4", dev, fcn, S, Hs, Ws, boxes, prob, ml, cls, n, n_dev,
+                 num_stuff, float(fraction_threshold), keep, k, labels,
+                 sem, ws, ws.numel())
         else:
-            check(lib().upsnet_panoptic_head(ptr(fcn), S, H, W, ptr(boxes), ptr(prob), ptr(ml), ptr(cls), n, ptr(n_dev),
-                                             num_stuff, float(fraction_threshold), ptr(keep), ptr(k), ptr(labels),
-                                             ptr(sem), ptr(ws), ws.numel(), stream_ptr(dev)), "panoptic_head")
+            call("panoptic_head", dev, fcn, S, H, W, boxes, prob, ml, cls, n, n_dev,
+                 num_stuff, float(fraction_threshold), keep, k, labels,
+                 sem, ws, ws.numel())
     if n_dev is not None:
         return (keep, labels, sem, k) if want_sem else (keep, labels, k)
     keep = keep[:int(k.item())]
@@ -1091,16 +1061,14 @@ class MaskRemoval(nn.Module):
         n, (H, W) = boxes.shape[0], (int(im_shape[0]), int(im_shape[1]))
         dev = boxes.device
         num_thing = max(int(cls.max().item()), 1)          # mask_image planes: np.max(cls_idx) (host read, as the reference)
-        nbytes = C.c_size_t(0)
-        check(lib().upsnet_panoptic_workspace_bytes(n, H, W, num_thing, C.byref(nbytes)), "panoptic_workspace_bytes")
-        ws = _pan_ws.get(dev, nbytes.value)
+        nbytes = query_bytes("panoptic_workspace_bytes", n, H, W, num_thing)
+        ws = _pan_ws.get(dev, nbytes)
         keep = torch.zeros((max(n, 1),), dtype=torch.int64, device=dev)
         k = torch.empty((1,), dtype=torch.int32, device=dev)
         energy = torch.empty((n, H, W), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev), _Timed("mask_removal", 5, {"bytes": 4.0 * n * H * W}, dev):
-            check(lib().upsnet_mask_removal(ptr(boxes), ptr(prob), ptr(ml), ptr(cls), n, None, H, W, num_thing,
-                                            float(self.fraction_threshold), ptr(keep), ptr(k), ptr(energy), ptr(ws),
-                                            ws.numel(), stream_ptr(dev)), "mask_removal")
+        with _Timed("mask_removal", 5, {"bytes": 4.0 * n * H * W}, dev):
+            call("mask_removal", dev, boxes, prob, ml, cls, n, None, H, W, num_thing,
+                 float(self.fraction_threshold), keep, k, energy, ws, ws.numel())
         kk = int(k.item())
         return keep[:kk], energy[:kk].unsqueeze(0)
 
@@ -1226,15 +1194,14 @@ def unified_pan_result(seg, pan, cls_inds, num_seg_classes, num_classes, stuff_a
     cls = cls_inds.to(torch.int64).contiguous()
     H, W = pan.shape
     dev = pan.device
-    nb = C.c_size_t(0)
-    check(lib().upsnet_unified_pan_workspace_bytes(int(num_seg_classes), C.byref(nb)), "unified_pan_workspace_bytes")
-    ws = _uni_ws.get(dev, nb.value)
+    nb = query_bytes("unified_pan_workspace_bytes", int(num_seg_classes))
+    ws = _uni_ws.get(dev, nb)
     out = torch.empty((H, W, 3), dtype=torch.uint8, device=dev)
     err = torch.zeros((1,), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev), _Timed("unified_pan", 5, {"bytes": 19.0 * H * W}, dev):
-        check(lib().upsnet_unified_pan_result(ptr(seg), ptr(pan), ptr(cls), int(cls.numel()), ptr(k_dev), H, W,
-                                              int(num_seg_classes), int(num_classes), int(stuff_area_limit), ptr(out), ptr(err),
-                                              ptr(ws), ws.numel(), stream_ptr(dev)), "unified_pan_result")
+    with _Timed("unified_pan", 5, {"bytes": 19.0 * H * W}, dev):
+        call("unified_pan_result", dev, seg, pan, cls, int(cls.numel()), k_dev, H, W,
+             int(num_seg_classes), int(num_classes), int(stuff_area_limit), out, err,
+             ws, ws.numel())
     if check_errors:
         e = int(err.item())
         if e & 2:
@@ -1256,8 +1223,8 @@ def prep_image(image_hwc_u8, pixel_means, scale=1.0, stride=32):
     Hp, Wp = int(math.ceil(ho / float(stride)) * stride), int(math.ceil(wo / float(stride)) * stride)
     blob = torch.empty((1, 3, Hp, Wp), dtype=torch.float32, device=im.device)
     pm = (C.c_double * 3)(*[float(v) for v in pixel_means])
-    with torch.cuda.device(im.device), _Timed("prep_image", 1, {"bytes": 3.0 * h * w + 12.0 * Hp * Wp}, im.device):
-        check(lib().upsnet_prep_image(ptr(im), h, w, float(scale), ho, wo, Hp, Wp, pm, ptr(blob), stream_ptr(im.device)), "prep_image")
+    with _Timed("prep_image", 1, {"bytes": 3.0 * h * w + 12.0 * Hp * Wp}, im.device):
+        call("prep_image", im.device, im, h, w, float(scale), ho, wo, Hp, Wp, pm, blob)
     return blob, (ho, wo)
 
 
@@ -1297,9 +1264,9 @@ def label_restore(label_map, im_info, *more_maps):
     dev = srcs[0].device
     outs = [torch.empty(lead + (oh, ow), dtype=torch.int64, device=dev) for _ in srcs]
     two = len(srcs) == 2
-    with torch.cuda.device(dev), _Timed("label_restore", 1, {"bytes": 16.0 * oh * ow * len(srcs)}, dev):
-        check(lib().upsnet_label_restore(ptr(srcs[0]), ptr(srcs[1] if two else None), Hp, Wp, h, w, fx, oh, ow,
-                                         ptr(outs[0]), ptr(outs[1] if two else None), stream_ptr(dev)), "label_restore")
+    with _Timed("label_restore", 1, {"bytes": 16.0 * oh * ow * len(srcs)}, dev):
+        call("label_restore", dev, srcs[0], srcs[1] if two else None, Hp, Wp, h, w, fx, oh, ow,
+             outs[0], outs[1] if two else None)
     return tuple(outs) if two else outs[0]
 
 
@@ -1363,15 +1330,14 @@ def im_post_rle(pred_boxes, pred_masks, cls_inds, im_h, im_w, n_dev=None, cap=No
     cls = cls_inds.to(torch.int64).contiguous()
     dev = masks.device
     cap = int(cap) if cap else 16 * int(im_w) + 64
-    nb = C.c_size_t(0)
-    check(lib().upsnet_im_post_workspace_bytes(n, cap, C.byref(nb)), "im_post_workspace_bytes")
-    ws = _impost_ws.get(dev, nb.value)
+    nb = query_bytes("im_post_workspace_bytes", n, cap)
+    ws = _impost_ws.get(dev, nb)
     counts = torch.empty((max(n, 1), cap), dtype=torch.int32, device=dev)      # uint32 payload
     run_len = torch.zeros((max(n, 1),), dtype=torch.int32, device=dev)
     ovf = torch.zeros((1,), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev), _Timed("im_post", 1, {"bytes": 4.0 * masks.numel()}, dev):
-        check(lib().upsnet_im_post_rle(ptr(masks), Cc, M, ptr(boxes), ptr(cls), n, ptr(n_dev), int(im_h), int(im_w), ptr(counts),
-                                       cap, ptr(run_len), ptr(ovf), ptr(ws), ws.numel(), stream_ptr(dev)), "im_post_rle")
+    with _Timed("im_post", 1, {"bytes": 4.0 * masks.numel()}, dev):
+        call("im_post_rle", dev, masks, Cc, M, boxes, cls, n, n_dev, int(im_h), int(im_w), counts,
+             cap, run_len, ovf, ws, ws.numel())
     return counts[:n], run_len[:n], ovf
 
 
@@ -1430,17 +1396,15 @@ def combined_pan_result(sem, scores, cls_inds, rle, num_seg_classes, num_classes
     cap = int(counts.shape[1]) if counts.dim() == 2 else 1
     cn, rl = counts.contiguous(), run_len.to(torch.int32).contiguous()
     dev = sem.device
-    nb = C.c_size_t(0)
-    check(lib().upsnet_combined_pan_workspace_bytes(n, H, W, C.byref(nb)), "combined_pan_workspace_bytes")
-    ws = _comb_ws.get(dev, nb.value)
+    nb = query_bytes("combined_pan_workspace_bytes", n, H, W)
+    ws = _comb_ws.get(dev, nb)
     out = torch.empty((H, W, 3), dtype=torch.uint8, device=dev)
     err = torch.zeros((1,), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev), _Timed("combined_pan", 3, {"bytes": (sem.element_size() * 2 + 3.25) * H * W}, dev):
-        check(lib().upsnet_combined_pan_result(ptr(sem), sem.element_size(), H, W, ptr(sc), ptr(cls), n, ptr(n_dev),
-                                               ptr(cn), cap, ptr(rl), int(num_seg_classes), int(num_classes),
-                                               float(score_threshold), float(fraction_threshold), int(stuff_area_limit),
-                                               ptr(out), ptr(err), ptr(ws), ws.numel(), stream_ptr(dev)),
-              "combined_pan_result")
+    with _Timed("combined_pan", 3, {"bytes": (sem.element_size() * 2 + 3.25) * H * W}, dev):
+        call("combined_pan_result", dev, sem, sem.element_size(), H, W, sc, cls, n, n_dev,
+             cn, cap, rl, int(num_seg_classes), int(num_classes),
+             float(score_threshold), float(fraction_threshold), int(stuff_area_limit),
+             out, err, ws, ws.numel())
     if check_errors:
         e = int(err.item())
         if e & 2:

@@ -33,7 +33,7 @@ import torch.distributed as dist
 from torch.nn.modules.utils import _pair
 
 from . import _lib
-from ._lib import check, f32c, lib, ptr, require_cuda, stream_ptr
+from ._lib import call, f32c, query_bytes, require_cuda
 
 
 def _conv_out(n, pad, dil, k, stride):
@@ -75,17 +75,14 @@ class _DeformConvBase(torch.autograd.Function):
         dw_ = torch.zeros((Cout, K), dtype=torch.float32, device=dev)
         col = torch.empty((K, P), dtype=torch.float32, device=dev)
         g = (Cin, H, W, kh, kw, sh, sw, ph, pw, dh, dw)
-        st = stream_ptr(dev)
-        with torch.cuda.device(dev):
-            for n in range(N):          # the reference loops over the batch as well (functions/deform_conv.py:84-104)
-                m_n = None if mask is None else mask[n]
-                go = grad_out[n].reshape(Cout, P)
-                check(lib().upsnet_dcn_im2col(ptr(x[n]), ptr(offset[n]), ptr(m_n), *g, ptr(col), st), "dcn_im2col")
-                dw_.addmm_(go, col.t())                                         # d(weight) += dY col^T
-                dcol = torch.mm(w2.t(), go)                                     # d(col) = W^T dY
-                check(lib().upsnet_dcn_col2im(ptr(dcol), ptr(offset[n]), ptr(m_n), *g, ptr(dx[n]), st), "dcn_col2im")
-                check(lib().upsnet_dcn_col2im_coord(ptr(dcol), ptr(x[n]), ptr(offset[n]), ptr(m_n), *g, ptr(doff[n]),
-                                                    ptr(None if dmask is None else dmask[n]), st), "dcn_col2im_coord")
+        for n in range(N):          # the reference loops over the batch as well (functions/deform_conv.py:84-104)
+            m_n = None if mask is None else mask[n]
+            go = grad_out[n].reshape(Cout, P)
+            call("dcn_im2col", dev, x[n], offset[n], m_n, *g, col)
+            dw_.addmm_(go, col.t())                                         # d(weight) += dY col^T
+            dcol = torch.mm(w2.t(), go)                                     # d(col) = W^T dY
+            call("dcn_col2im", dev, dcol, offset[n], m_n, *g, dx[n])
+            call("dcn_col2im_coord", dev, dcol, x[n], offset[n], m_n, *g, doff[n], None if dmask is None else dmask[n])
         dbias = grad_out.sum(dim=(0, 2, 3)) if ctx.has_bias else None
         return dx, doff, dmask, dw_.view_as(weight), dbias
 
@@ -134,9 +131,7 @@ class RoIAlignFunction(torch.autograd.Function):
             return torch.zeros((B, Cc, H, W), dtype=torch.float32, device=grad_out.device), None, None, None, None, None
         grad_out, rois = f32c(grad_out), f32c(rois)
         dfeat = torch.empty((B, Cc, H, W), dtype=torch.float32, device=grad_out.device)
-        with torch.cuda.device(grad_out.device):
-            check(lib().upsnet_roi_align_backward(ptr(grad_out), ptr(rois), rois.shape[0], B, Cc, H, W, ph, pw, sr, scale,
-                                                  ptr(dfeat), stream_ptr(grad_out.device)), "roi_align_backward")
+        call("roi_align_backward", grad_out.device, grad_out, rois, rois.shape[0], B, Cc, H, W, ph, pw, sr, scale, dfeat)
         return dfeat, None, None, None, None, None
 
 
@@ -190,19 +185,17 @@ class FPNRoIAlignFunction(torch.autograd.Function):
         grad_out, rois = f32c(grad_out), f32c(rois)
         R = rois.shape[0]
         dfeats = []
-        with torch.cuda.device(grad_out.device):
-            for lv, (B, Cc, H, W) in enumerate(shapes):
-                if not ctx.needs_input_grad[5 + lv]:
-                    dfeats.append(None)
-                    continue
-                if R == 0:
-                    dfeats.append(torch.zeros((B, Cc, H, W), dtype=torch.float32, device=grad_out.device))
-                    continue
-                g = torch.where((levels == lv).view(R, 1, 1, 1), grad_out, 0.0).contiguous()
-                dfeat = torch.empty((B, Cc, H, W), dtype=torch.float32, device=grad_out.device)
-                check(lib().upsnet_roi_align_backward(ptr(g), ptr(rois), R, B, Cc, H, W, ph, pw, sr, scales[lv],
-                                                      ptr(dfeat), stream_ptr(grad_out.device)), "roi_align_backward")
-                dfeats.append(dfeat)
+        for lv, (B, Cc, H, W) in enumerate(shapes):
+            if not ctx.needs_input_grad[5 + lv]:
+                dfeats.append(None)
+                continue
+            if R == 0:
+                dfeats.append(torch.zeros((B, Cc, H, W), dtype=torch.float32, device=grad_out.device))
+                continue
+            g = torch.where((levels == lv).view(R, 1, 1, 1), grad_out, 0.0).contiguous()
+            dfeat = torch.empty((B, Cc, H, W), dtype=torch.float32, device=grad_out.device)
+            call("roi_align_backward", grad_out.device, g, rois, R, B, Cc, H, W, ph, pw, sr, scales[lv], dfeat)
+            dfeats.append(dfeat)
         return (None, None, None, None, None) + tuple(dfeats)
 
 
@@ -297,11 +290,9 @@ class RPNTargets:
 
     def _buffers(self, dev):
         if dev not in self._dev:
-            sz = C.c_size_t()
-            check(lib().upsnet_rpn_targets_workspace_bytes(self.num_anchors, self.batch_size, C.byref(sz)),
-                  "rpn_targets_workspace_bytes")
+            sz = query_bytes("rpn_targets_workspace_bytes", self.num_anchors, self.batch_size)
             self._dev[dev] = (torch.from_numpy(np.ascontiguousarray(self.cell, np.float64)).to(dev),
-                              torch.empty(sz.value, dtype=torch.uint8, device=dev))
+                              torch.empty(sz, dtype=torch.uint8, device=dev))
         return self._dev[dev]
 
     def __call__(self, gt_boxes, im_height, im_width, seed=None):
@@ -323,13 +314,11 @@ class RPNTargets:
         targets, inside, outside = (torch.empty(4 * N, dtype=torch.float32, device=dev) for _ in range(3))
         counts = torch.empty(4, dtype=torch.int32, device=dev)
         L = len(self.strides)
-        with torch.cuda.device(dev):
-            check(lib().upsnet_rpn_targets(ptr(gt), gt.shape[0], ptr(cell), (C.c_int * L)(*self.strides),
-                                           (C.c_int * L)(*self.field_sizes), L, self.A, float(im_height),
-                                           float(im_width), self.straddle, self.pos, self.neg, self.batch_size,
-                                           self.num_fg, int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(labels), ptr(targets),
-                                           ptr(inside), ptr(outside), ptr(counts), ptr(ws), ws.numel(),
-                                           stream_ptr(dev)), "rpn_targets")
+        call("rpn_targets", dev, gt, gt.shape[0], cell, (C.c_int * L)(*self.strides),
+             (C.c_int * L)(*self.field_sizes), L, self.A, float(im_height),
+             float(im_width), self.straddle, self.pos, self.neg, self.batch_size,
+             self.num_fg, int(seed) & 0xFFFFFFFFFFFFFFFF, labels, targets,
+             inside, outside, counts, ws, ws.numel())
         self.counts = counts
         out, off = {}, 0
         for s, F in zip(self.strides, self.field_sizes):
@@ -478,10 +467,8 @@ class ProposalTargets:
             seed = int(np.random.randint(np.iinfo(np.int64).max, dtype=np.int64))
         dev = rois.device
         R, B, K, M, C_ = rois.shape[0], self.batch_rois, self.K, self.M, self.mask_capacity
-        sz = C.c_size_t()
-        check(lib().upsnet_proposal_targets_workspace_bytes(R, packed.G, B, C.byref(sz)),
-              "proposal_targets_workspace_bytes")
-        ws = torch.empty(sz.value, dtype=torch.uint8, device=dev)
+        sz = query_bytes("proposal_targets_workspace_bytes", R, packed.G, B)
+        ws = torch.empty(sz, dtype=torch.uint8, device=dev)
         f = dict(device=dev, dtype=torch.float32)
         out = dict(rois=torch.empty((B, 5), **f), labels=torch.empty(B, dtype=torch.int64, device=dev),
                    bbox_targets=torch.empty((B, 4 * K), **f), bbox_inside_weights=torch.empty((B, 4 * K), **f),
@@ -491,16 +478,13 @@ class ProposalTargets:
                    nongt_inds=torch.empty(B, dtype=torch.int64, device=dev))
         counts = torch.empty(5, dtype=torch.int32, device=dev)
         pk = packed
-        with torch.cuda.device(dev):
-            check(lib().upsnet_proposal_targets(
-                ptr(rois) if R else None, R, ptr(pk.boxes), ptr(pk.gt_max), ptr(pk.gt_maxcls), ptr(pk.gt_classes),
-                ptr(pk.gt_map), pk.G, ptr(pk.obj_boxes), ptr(pk.obj_poly), ptr(pk.poly_vert), ptr(pk.verts), pk.O,
-                float(np.float32(im_scale)), K, B, self.fg_per_image, self.fg_thresh, self.bg_hi, self.bg_lo,
-                *self.weights, int(self.cls_agnostic), M, int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(out["rois"]),
-                ptr(out["labels"]), ptr(out["bbox_targets"]), ptr(out["bbox_inside_weights"]),
-                ptr(out["bbox_outside_weights"]), ptr(out["nongt_inds"]), ptr(out["mask_rois"]),
-                ptr(out["mask_int32"]), ptr(out["roi_has_mask"]), ptr(counts), ptr(ws), ws.numel(),
-                stream_ptr(dev)), "proposal_targets")
+        call("proposal_targets", dev, rois if R else None, R, pk.boxes, pk.gt_max, pk.gt_maxcls, pk.gt_classes,
+             pk.gt_map, pk.G, pk.obj_boxes, pk.obj_poly, pk.poly_vert, pk.verts, pk.O,
+             float(np.float32(im_scale)), K, B, self.fg_per_image, self.fg_thresh, self.bg_hi, self.bg_lo,
+             *self.weights, int(self.cls_agnostic), M, int(seed) & 0xFFFFFFFFFFFFFFFF, out["rois"],
+             out["labels"], out["bbox_targets"], out["bbox_inside_weights"],
+             out["bbox_outside_weights"], out["nongt_inds"], out["mask_rois"],
+             out["mask_int32"], out["roi_has_mask"], counts, ws, ws.numel())
         self.counts = counts
         return out
 
@@ -566,9 +550,8 @@ def gt_rois(entry, im_scale, device):
 
 
 def _pl_workspace(k, h, w, dev):
-    sz = C.c_size_t()
-    check(lib().upsnet_panoptic_loss_workspace_bytes(k, h, w, C.byref(sz)), "panoptic_loss_workspace_bytes")
-    return torch.empty(sz.value, dtype=torch.uint8, device=dev)
+    sz = query_bytes("panoptic_loss_workspace_bytes", k, h, w)
+    return torch.empty(sz, dtype=torch.uint8, device=dev)
 
 
 class PanopticLossFunction(torch.autograd.Function):
@@ -587,12 +570,9 @@ class PanopticLossFunction(torch.autograd.Function):
         lse = torch.empty(h * w, dtype=torch.float32, device=dev)
         gtc = torch.empty(h * w, dtype=torch.int32, device=dev)
         ws = _pl_workspace(k, h, w, dev)
-        with torch.cuda.device(dev):
-            check(lib().upsnet_panoptic_loss_forward(
-                ptr(fcn), S, h, w, ptr(msk), k, Cm, mask_size, ptr(gt_rois), ptr(cls_idx), ptr(seg_gt), ptr(mask_gt),
-                int(mask_gt.dtype == torch.int64), mask_gt.shape[0], ptr(keep_inds), num_classes, int(enable_void),
-                box_scale, ptr(loss), ptr(acc), ptr(counts), ptr(lse), ptr(gtc), ptr(ws), ws.numel(),
-                stream_ptr(dev)), "panoptic_loss_forward")
+        call("panoptic_loss_forward", dev, fcn, S, h, w, msk, k, Cm, mask_size, gt_rois, cls_idx, seg_gt, mask_gt,
+             int(mask_gt.dtype == torch.int64), mask_gt.shape[0], keep_inds, num_classes, int(enable_void),
+             box_scale, loss, acc, counts, lse, gtc, ws, ws.numel())
         ctx.save_for_backward(fcn, msk, gt_rois, cls_idx, lse, gtc)
         ctx.cfg = (num_classes, int(enable_void), box_scale, mask_size)
         ctx.mark_non_differentiable(acc, counts)
@@ -610,11 +590,8 @@ class PanopticLossFunction(torch.autograd.Function):
         dmsk = torch.empty_like(msk) if ctx.needs_input_grad[1] else None
         if dfcn is not None or dmsk is not None:
             ws = _pl_workspace(k, h, w, dev)
-            with torch.cuda.device(dev):
-                check(lib().upsnet_panoptic_loss_backward(
-                    ptr(fcn), S, h, w, ptr(msk), k, Cm, mask_size, ptr(rois), ptr(cls), num_classes, enable_void,
-                    box_scale, ptr(lse), ptr(gtc), ptr(go), ptr(dfcn), ptr(dmsk), ptr(ws), ws.numel(),
-                    stream_ptr(dev)), "panoptic_loss_backward")
+            call("panoptic_loss_backward", dev, fcn, S, h, w, msk, k, Cm, mask_size, rois, cls, num_classes, enable_void,
+                 box_scale, lse, gtc, go, dfcn, dmsk, ws, ws.numel())
         return (dfcn, dmsk) + (None,) * 9
 
 
@@ -665,10 +642,9 @@ class PanopticLoss(torch.nn.Module):
         seg, mgt, keep = self._labels(seg_gt_4x, mask_gt, keep_inds)
         out = torch.empty_like(seg)
         _, h, w = seg.shape
-        with torch.cuda.device(seg.device):
-            check(lib().upsnet_panoptic_gt(ptr(seg), ptr(mgt), int(mgt.dtype == torch.int64), mgt.shape[0], ptr(keep),
-                                           0 if keep is None else keep.numel(), h, w, self.num_seg_classes,
-                                           self.num_classes, ptr(out), stream_ptr(seg.device)), "panoptic_gt")
+        call("panoptic_gt", seg.device, seg, mgt, int(mgt.dtype == torch.int64), mgt.shape[0], keep,
+             0 if keep is None else keep.numel(), h, w, self.num_seg_classes,
+             self.num_classes, out)
         return out
 
     def forward(self, fcn_score, mask_score, gt_rois, cls_idx, seg_gt_4x, mask_gt, keep_inds=None):
@@ -864,15 +840,13 @@ class PanopticLabels:
         if self.with_roi:
             out["seg_roi_gt"] = torch.empty((n, self.M, self.M), dtype=torch.int64, device=dev)
         pk = packed
-        with torch.cuda.device(dev):
-            check(lib().upsnet_training_labels(
-                ptr(lab), lab.shape[0], lab.shape[1], ptr(tab["seg_rows"]), Hs, ptr(tab["seg_cols"]), Ws,
-                ptr(out["seg_gt"]), ptr(tab["q_rows"]), Hq, ptr(tab["q_cols"]), Wq, ptr(out["seg_gt_4x"]),
-                ptr(tab["m_rows"]), Hm, ptr(tab["m_cols"]), Wm, ptr(pk.obj_poly), ptr(pk.poly_vert), ptr(pk.verts),
-                ptr(pk.obj_yrange), G, pk.max_poly_verts, pk.max_obj_verts,
-                ptr(out["mask_gt"]) if G else None, int(mask_dtype == torch.int64),
-                ptr(tab["roi_rows"]) if n else None, ptr(tab["roi_cols"]) if n else None, n, self.M,
-                ptr(out["seg_roi_gt"]) if n else None, stream_ptr(dev)), "training_labels")
+        call("training_labels", dev, lab, lab.shape[0], lab.shape[1], tab["seg_rows"], Hs, tab["seg_cols"], Ws,
+             out["seg_gt"], tab["q_rows"], Hq, tab["q_cols"], Wq, out["seg_gt_4x"],
+             tab["m_rows"], Hm, tab["m_cols"], Wm, pk.obj_poly, pk.poly_vert, pk.verts,
+             pk.obj_yrange, G, pk.max_poly_verts, pk.max_obj_verts,
+             out["mask_gt"] if G else None, int(mask_dtype == torch.int64),
+             tab["roi_rows"] if n else None, tab["roi_cols"] if n else None, n, self.M,
+             out["seg_roi_gt"] if n else None)
         return out
 
     def __call__(self, label_map, packed, im_shape, im_scale, flipped, mask_dtype=torch.uint8):
