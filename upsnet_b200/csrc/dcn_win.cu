@@ -330,42 +330,11 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
             hc[2] = __ldg(reinterpret_cast<const uint4*>(b10)); lc[2] = __ldg(reinterpret_cast<const uint4*>(b10 + p.Cin));
             hc[3] = __ldg(reinterpret_cast<const uint4*>(b11)); lc[3] = __ldg(reinterpret_cast<const uint4*>(b11 + p.Cin));
           }
-          // blend: hi plane in fp32 on channel pairs (exact products of bf16 values), lo plane in packed bf16x2 (2^-9 of the
-          // value: its blend needs 2^-9 relative accuracy only), summed in fp32 and split again
-          const float wf4[4] = {wv.x, wv.y, wv.z, wv.w};
-          unsigned long long acc[4] = {0ull, 0ull, 0ull, 0ull};
-          __nv_bfloat162 lacc[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const uint32_t hw_[4] = {hc[i].x, hc[i].y, hc[i].z, hc[i].w};
-            const uint32_t lw_[4] = {lc[i].x, lc[i].y, lc[i].z, lc[i].w};
-            const __nv_bfloat162 wb = __float2bfloat162_rn(wf4[i]);
-            unsigned long long wp;
-            asm("mov.b64 %0, {%1, %1};" : "=l"(wp) : "r"(__float_as_uint(wf4[i])));
-#pragma unroll
-            for (int qq = 0; qq < 4; ++qq) {
-              unsigned long long hp;
-              asm("mov.b64 %0, {%1, %2};" : "=l"(hp) : "r"(hw_[qq] << 16), "r"(hw_[qq] & 0xffff0000u));
-              acc[qq] = f32x2_fma(wp, hp, acc[qq]);
-              const __nv_bfloat162 lv = *reinterpret_cast<const __nv_bfloat162*>(&lw_[qq]);
-              lacc[qq] = i == 0 ? __hmul2(wb, lv) : __hfma2(wb, lv, lacc[qq]);
-            }
-          }
-          uint32_t ohi[4], olo[4];
-#pragma unroll
-          for (int qq = 0; qq < 4; ++qq) {
-            const uint32_t lw = *reinterpret_cast<const uint32_t*>(&lacc[qq]);
-            unsigned long long lp;
-            asm("mov.b64 %0, {%1, %2};" : "=l"(lp) : "r"(lw << 16), "r"(lw & 0xffff0000u));
-            acc[qq] = f32x2_add(acc[qq], lp);
-            uint32_t a0, a1;
-            asm("mov.b64 {%0, %1}, %2;" : "=r"(a0), "=r"(a1) : "l"(acc[qq]));
-            const float v0 = __uint_as_float(a0), v1 = __uint_as_float(a1);
-            ohi[qq] = pack_bf16x2(v0, v1);
-            olo[qq] = pack_bf16x2(v0 - __uint_as_float(ohi[qq] << 16), v1 - __uint_as_float(ohi[qq] & 0xffff0000u));
-          }
-          sts128(a_row + a_off, make_uint4(ohi[0], ohi[1], ohi[2], ohi[3]));
-          sts128(a_row + DW_BM * ROWB + a_off, make_uint4(olo[0], olo[1], olo[2], olo[3]));
+          // blend and split again: the arithmetic of the gather kernel's pair path (igemm_tc.cu), shared through pair.cuh
+          uint4 ohi, olo;
+          pair_blend8(wv, hc, lc, ohi, olo);
+          sts128(a_row + a_off, ohi);
+          sts128(a_row + DW_BM * ROWB + a_off, olo);
         }
         fence_proxy_async();    // generic-proxy stores -> visible to wgmma (async proxy)
         __syncwarp();
@@ -520,10 +489,7 @@ dcn_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
           }
           uint32_t hw[8], lw[8];
 #pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            hw[e] = pack_bf16x2(o[2 * e], o[2 * e + 1]);
-            lw[e] = pack_bf16x2(o[2 * e] - __uint_as_float(hw[e] << 16), o[2 * e + 1] - __uint_as_float(hw[e] & 0xffff0000u));
-          }
+          for (int e = 0; e < 8; ++e) split_pair2(o[2 * e], o[2 * e + 1], hw[e], lw[e]);
           uint4* dh_ = reinterpret_cast<uint4*>(yp + co);
           uint4* dl_ = reinterpret_cast<uint4*>(yp + p.Cout + co);
           dh_[0] = make_uint4(hw[0], hw[1], hw[2], hw[3]); dh_[1] = make_uint4(hw[4], hw[5], hw[6], hw[7]);
@@ -544,8 +510,8 @@ __global__ void dcn_win_pack_kernel(const float* __restrict__ w, int Cout, int C
     const int kk = (int)(i % (size_t)K), co = (int)(i / (size_t)K);
     const int sc = kk / (16 * DW_KHW), rem = kk - sc * 16 * DW_KHW, tap = rem >> 4, c = sc * 16 + (rem & 15);
     const float v = co < Cout ? w[((size_t)co * Cin + c) * DW_KHW + tap] : 0.f;
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    const __nv_bfloat16 l = __float2bfloat16_rn(v - __bfloat162float(h));
+    __nv_bfloat16 h, l;
+    split_bf16(v, h, l);
     hi[i] = *reinterpret_cast<const uint16_t*>(&h);
     lo[i] = *reinterpret_cast<const uint16_t*>(&l);
   }

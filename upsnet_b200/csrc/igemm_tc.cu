@@ -285,18 +285,9 @@ igemm_tc_kernel(const TcParams p) {
               }
             }
             const uint32_t soff = (uint32_t)r * 128u + (uint32_t)((j ^ (r & 7)) << 4);
-            uint4 hi4;
-            hi4.x = pack_bf16x2(v[0], v[1]); hi4.y = pack_bf16x2(v[2], v[3]);
-            hi4.z = pack_bf16x2(v[4], v[5]); hi4.w = pack_bf16x2(v[6], v[7]);
+            const uint4 hi4 = pack_bf16x8(v);
             *reinterpret_cast<uint4*>(a_hi + soff) = hi4;
-            if (x3) {
-              uint4 lo;
-              lo.x = pack_bf16x2(v[0] - bf16_round(v[0]), v[1] - bf16_round(v[1]));
-              lo.y = pack_bf16x2(v[2] - bf16_round(v[2]), v[3] - bf16_round(v[3]));
-              lo.z = pack_bf16x2(v[4] - bf16_round(v[4]), v[5] - bf16_round(v[5]));
-              lo.w = pack_bf16x2(v[6] - bf16_round(v[6]), v[7] - bf16_round(v[7]));
-              *reinterpret_cast<uint4*>(a_lo + soff) = lo;
-            }
+            if (x3) *reinterpret_cast<uint4*>(a_lo + soff) = pair_lo8(v, hi4);
           }
         } else if (!DEFORM && XPAIR) {
           // dense, hi/lo pair activations: the hi and lo 128-byte rows ARE the smem rows of the two A tiles -> two cp.async
@@ -315,16 +306,13 @@ igemm_tc_kernel(const TcParams p) {
           }
         } else if (DEFORM && XPAIR) {
           // deformable, hi/lo pair activations: 8 lanes x 16 B cover a row's 64 channels of one plane; per corner one hi and
-          // one lo load.  The gather is issue-bound, so the blend is written for instruction count: hi plane = fp32 FMAs on
-          // channel pairs (exact fp32 products of the bf16 values),
-          // lo plane = packed bf16x2 HFMA2 with bf16-rounded weights (the lo plane is 2^-9 of the value, its blend only needs
-          // 2^-9 relative accuracy -> 2^-18 overall); the two sums are added in fp32 and the result is split again.
+          // one lo load, blended and split again by pair_blend8 (pair.cuh), the blend of the window kernel (dcn_win.cu).
           const __nv_bfloat16* xh = reinterpret_cast<const __nv_bfloat16*>(p.x);
 #pragma unroll 1
           for (int pass = 0; pass < TC_BM / 32; ++pass) {
             const int r = r_first + pass * 32;
             const long long rb = rowinfo[r];
-            unsigned long long acc[4] = {0ull, 0ull, 0ull, 0ull};      // fp32x2: channels (2q, 2q+1)
+            uint4 hi = make_uint4(0u, 0u, 0u, 0u), lo = hi;
             if (rb >= 0) {
               const __nv_bfloat16* xb = xh + rb + c0;
               const float4 wv = tw[tap * TC_BM + r];
@@ -333,44 +321,12 @@ igemm_tc_kernel(const TcParams p) {
               const uint4 hb = __ldg(reinterpret_cast<const uint4*>(xb + ov.y)), lb = __ldg(reinterpret_cast<const uint4*>(xb + ov.y + p.Cin));
               const uint4 hd = __ldg(reinterpret_cast<const uint4*>(xb + ov.z)), ld = __ldg(reinterpret_cast<const uint4*>(xb + ov.z + p.Cin));
               const uint4 he = __ldg(reinterpret_cast<const uint4*>(xb + ov.w)), le = __ldg(reinterpret_cast<const uint4*>(xb + ov.w + p.Cin));
-              const uint32_t H[4][4] = {{ha.x, ha.y, ha.z, ha.w}, {hb.x, hb.y, hb.z, hb.w}, {hd.x, hd.y, hd.z, hd.w}, {he.x, he.y, he.z, he.w}};
-              const uint32_t Lo[4][4] = {{la.x, la.y, la.z, la.w}, {lb.x, lb.y, lb.z, lb.w}, {ld.x, ld.y, ld.z, ld.w}, {le.x, le.y, le.z, le.w}};
-              const float wf[4] = {wv.x, wv.y, wv.z, wv.w};
-              __nv_bfloat162 lacc[4];
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const __nv_bfloat162 wb = __float2bfloat162_rn(wf[i]);
-                unsigned long long wp;
-                asm("mov.b64 %0, {%1, %1};" : "=l"(wp) : "r"(__float_as_uint(wf[i])));
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  unsigned long long hp;
-                  asm("mov.b64 %0, {%1, %2};" : "=l"(hp) : "r"(H[i][q] << 16), "r"(H[i][q] & 0xffff0000u));
-                  acc[q] = f32x2_fma(wp, hp, acc[q]);
-                  const __nv_bfloat162 lv = *reinterpret_cast<const __nv_bfloat162*>(&Lo[i][q]);
-                  lacc[q] = i == 0 ? __hmul2(wb, lv) : __hfma2(wb, lv, lacc[q]);
-                }
-              }
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const uint32_t lw = *reinterpret_cast<const uint32_t*>(&lacc[q]);
-                unsigned long long lp;
-                asm("mov.b64 %0, {%1, %2};" : "=l"(lp) : "r"(lw << 16), "r"(lw & 0xffff0000u));
-                acc[q] = f32x2_add(acc[q], lp);
-              }
+              const uint4 hc[4] = {ha, hb, hd, he}, lc[4] = {la, lb, ld, le};
+              pair_blend8(wv, hc, lc, hi, lo);
             }
             const uint32_t soff = (uint32_t)r * 128u + (uint32_t)((j ^ (r & 7)) << 4);
-            uint32_t hw[4], lw4[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              uint32_t a0, a1;
-              asm("mov.b64 {%0, %1}, %2;" : "=r"(a0), "=r"(a1) : "l"(acc[q]));
-              const float v0 = __uint_as_float(a0), v1 = __uint_as_float(a1);
-              hw[q] = pack_bf16x2(v0, v1);
-              lw4[q] = pack_bf16x2(v0 - __uint_as_float(hw[q] << 16), v1 - __uint_as_float(hw[q] & 0xffff0000u));
-            }
-            *reinterpret_cast<uint4*>(a_hi + soff) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-            *reinterpret_cast<uint4*>(a_lo + soff) = make_uint4(lw4[0], lw4[1], lw4[2], lw4[3]);
+            *reinterpret_cast<uint4*>(a_hi + soff) = hi;
+            *reinterpret_cast<uint4*>(a_lo + soff) = lo;
           }
         } else if (!DEFORM && XBF16) {
           // dense, bf16 activations: the 128-byte row IS the smem row -> cp.async 16 B per (row, chunk)
@@ -409,15 +365,10 @@ igemm_tc_kernel(const TcParams p) {
           for (int pass = 0; pass < TC_BM / 16; ++pass) {
             const int r = rr0 + pass * 16;
             const uint32_t soff = (uint32_t)r * 128u + (uint32_t)(((l16 >> 1) ^ (r & 7)) << 4) + (uint32_t)((l16 & 1) << 3);
-            uint2 hi;
-            hi.x = pack_bf16x2(qv[pass].x, qv[pass].y); hi.y = pack_bf16x2(qv[pass].z, qv[pass].w);
+            const float4 v = qv[pass];
+            const uint2 hi = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
             *reinterpret_cast<uint2*>(a_hi + soff) = hi;
-            if (x3) {
-              uint2 lo;
-              lo.x = pack_bf16x2(qv[pass].x - bf16_round(qv[pass].x), qv[pass].y - bf16_round(qv[pass].y));
-              lo.y = pack_bf16x2(qv[pass].z - bf16_round(qv[pass].z), qv[pass].w - bf16_round(qv[pass].w));
-              *reinterpret_cast<uint2*>(a_lo + soff) = lo;
-            }
+            if (x3) *reinterpret_cast<uint2*>(a_lo + soff) = make_uint2(pair_lo2(v.x, v.y, hi.x), pair_lo2(v.z, v.w, hi.y));
           }
         } else if (XBF16) {
           // deformable, bf16 activations: 4 lanes x 32 B cover a row's 64 channels (two 16-byte loads per corner,
@@ -480,15 +431,9 @@ igemm_tc_kernel(const TcParams p) {
               v.w = wv.x * a0.w + wv.y * b0.w + wv.z * d0.w + wv.w * e0.w;
             }
             const uint32_t soff = (uint32_t)r * 128u + (uint32_t)(((l16 >> 1) ^ (r & 7)) << 4) + (uint32_t)((l16 & 1) << 3);
-            uint2 hi;
-            hi.x = pack_bf16x2(v.x, v.y); hi.y = pack_bf16x2(v.z, v.w);
+            const uint2 hi = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
             *reinterpret_cast<uint2*>(a_hi + soff) = hi;
-            if (x3) {
-              uint2 lo;
-              lo.x = pack_bf16x2(v.x - bf16_round(v.x), v.y - bf16_round(v.y));
-              lo.y = pack_bf16x2(v.z - bf16_round(v.z), v.w - bf16_round(v.w));
-              *reinterpret_cast<uint2*>(a_lo + soff) = lo;
-            }
+            if (x3) *reinterpret_cast<uint2*>(a_lo + soff) = make_uint2(pair_lo2(v.x, v.y, hi.x), pair_lo2(v.z, v.w, hi.y));
           }
         }
         cp_async_commit();
@@ -633,23 +578,19 @@ igemm_tc_kernel(const TcParams p) {
                   const uint32_t hw[4] = {rh.x, rh.y, rh.z, rh.w}, lw[4] = {rl.x, rl.y, rl.z, rl.w};
 #pragma unroll
                   for (int e = 0; e < 4; ++e) {
-                    o[2 * e] += __uint_as_float(hw[e] << 16) + __uint_as_float(lw[e] << 16);
-                    o[2 * e + 1] += __uint_as_float(hw[e] & 0xffff0000u) + __uint_as_float(lw[e] & 0xffff0000u);
+                    o[2 * e] += pair_x(hw[e], lw[e]);
+                    o[2 * e + 1] += pair_y(hw[e], lw[e]);
                   }
                 }
                 if (p.relu) {
 #pragma unroll
                   for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], 0.f);
                 }
-                uint32_t hw[4], lw[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  hw[e] = pack_bf16x2(o[2 * e], o[2 * e + 1]);
-                  lw[e] = pack_bf16x2(o[2 * e] - __uint_as_float(hw[e] << 16), o[2 * e + 1] - __uint_as_float(hw[e] & 0xffff0000u));
-                }
+                uint4 hi, lo;
+                split_pair8(o, hi, lo);
                 __nv_bfloat16* yp = reinterpret_cast<__nv_bfloat16*>(p.y) + (size_t)pgr * ypitch + co;
-                *reinterpret_cast<uint4*>(yp) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                *reinterpret_cast<uint4*>(yp + p.Cout) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+                *reinterpret_cast<uint4*>(yp) = hi;
+                *reinterpret_cast<uint4*>(yp + p.Cout) = lo;
               } else if (p.y_bf16) {
                 const float4 a = *reinterpret_cast<const float4*>(src), b = *reinterpret_cast<const float4*>(src + 4);
                 float o[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
@@ -658,18 +599,15 @@ igemm_tc_kernel(const TcParams p) {
                   const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
 #pragma unroll
                   for (int e = 0; e < 4; ++e) {
-                    o[2 * e] += __uint_as_float(rw[e] << 16);
-                    o[2 * e + 1] += __uint_as_float(rw[e] & 0xffff0000u);
+                    o[2 * e] += bf16x2_x(rw[e]);
+                    o[2 * e + 1] += bf16x2_y(rw[e]);
                   }
                 }
                 if (p.relu) {
 #pragma unroll
                   for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], 0.f);
                 }
-                uint4 w;
-                w.x = pack_bf16x2(o[0], o[1]); w.y = pack_bf16x2(o[2], o[3]);
-                w.z = pack_bf16x2(o[4], o[5]); w.w = pack_bf16x2(o[6], o[7]);
-                *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.y) + (size_t)pgr * p.Cout + co) = w;
+                *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.y) + (size_t)pgr * p.Cout + co) = pack_bf16x8(o);
               } else {
                 float4 o = *reinterpret_cast<const float4*>(src);
                 if (p.residual) {
@@ -716,21 +654,16 @@ igemm_tc_kernel(const TcParams p) {
                   const uint32_t rw[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
 #pragma unroll
                   for (int q = 0; q < 8; ++q) {
-                    o16[2 * q] += __uint_as_float(rw[q] << 16);
-                    o16[2 * q + 1] += __uint_as_float(rw[q] & 0xffff0000u);
+                    o16[2 * q] += bf16x2_x(rw[q]);
+                    o16[2 * q + 1] += bf16x2_y(rw[q]);
                   }
                 }
                 if (p.relu) {
 #pragma unroll
                   for (int e = 0; e < 16; ++e) o16[e] = fmaxf(o16[e], 0.f);
                 }
-                uint4 w0, w1;
-                w0.x = pack_bf16x2(o16[0], o16[1]); w0.y = pack_bf16x2(o16[2], o16[3]);
-                w0.z = pack_bf16x2(o16[4], o16[5]); w0.w = pack_bf16x2(o16[6], o16[7]);
-                w1.x = pack_bf16x2(o16[8], o16[9]); w1.y = pack_bf16x2(o16[10], o16[11]);
-                w1.z = pack_bf16x2(o16[12], o16[13]); w1.w = pack_bf16x2(o16[14], o16[15]);
-                reinterpret_cast<uint4*>(yo)[0] = w0;
-                reinterpret_cast<uint4*>(yo)[1] = w1;
+                reinterpret_cast<uint4*>(yo)[0] = pack_bf16x8(o16);
+                reinterpret_cast<uint4*>(yo)[1] = pack_bf16x8(o16 + 8);
               } else {
 #pragma unroll
                 for (int e = 0; e < 16; ++e) {
@@ -802,8 +735,8 @@ __global__ void pack_weight_kernel(const float* __restrict__ w, int Cout, int Ci
     const int co = (int)(i / (size_t)Kp);
     const int tap = kk / Cin, c = kk - tap * Cin;
     const float v = (co < Cout && kk < KHW * Cin) ? w[((size_t)co * Cin + c) * KHW + tap] : 0.f;
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    const __nv_bfloat16 l = __float2bfloat16_rn(v - __bfloat162float(h));
+    __nv_bfloat16 h, l;
+    split_bf16(v, h, l);
     hi[i] = *reinterpret_cast<const uint16_t*>(&h);
     lo[i] = *reinterpret_cast<const uint16_t*>(&l);
   }

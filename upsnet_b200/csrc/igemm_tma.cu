@@ -411,13 +411,14 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
                   hw = lds32(ra + (((uint32_t)j ^ fr_rx[h]) << 4) + cq4);
                   lw = lds32(ra + L.res_slab + (((uint32_t)j ^ fr_rx[h]) << 4) + cq4);
                 }
-                a += __uint_as_float(hw << 16) + __uint_as_float(lw << 16);
-                b += __uint_as_float(hw & 0xffff0000u) + __uint_as_float(lw & 0xffff0000u);
+                a += pair_x(hw, lw);
+                b += pair_y(hw, lw);
               }
               if (g.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
-              const uint32_t hw = pack_bf16x2(a, b);
+              uint32_t hw, lw;
+              split_pair2(a, b, hw, lw);
               sts32(oa, hw);
-              sts32(oa + TM_SLAB_BYTES, pack_bf16x2(a - __uint_as_float(hw << 16), b - __uint_as_float(hw & 0xffff0000u)));
+              sts32(oa + TM_SLAB_BYTES, lw);
             }
           }
           fence_proxy_async();
@@ -467,8 +468,8 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
               const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
   #pragma unroll
               for (int e = 0; e < 4; ++e) {
-                o[c * 8 + 2 * e] += __uint_as_float(rw[e] << 16);
-                o[c * 8 + 2 * e + 1] += __uint_as_float(rw[e] & 0xffff0000u);
+                o[c * 8 + 2 * e] += bf16x2_x(rw[e]);
+                o[c * 8 + 2 * e + 1] += bf16x2_y(rw[e]);
               }
             }
           }
@@ -477,12 +478,7 @@ igemm_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
             for (int e = 0; e < 32; ++e) o[e] = fmaxf(o[e], 0.f);
           }
   #pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint4 w;
-            w.x = pack_bf16x2(o[c * 8], o[c * 8 + 1]); w.y = pack_bf16x2(o[c * 8 + 2], o[c * 8 + 3]);
-            w.z = pack_bf16x2(o[c * 8 + 4], o[c * 8 + 5]); w.w = pack_bf16x2(o[c * 8 + 6], o[c * 8 + 7]);
-            sts128(out_slab + sw_row + (((jb + c) ^ rx) << 4), w);
-          }
+          for (int c = 0; c < 4; ++c) sts128(out_slab + sw_row + (((jb + c) ^ rx) << 4), pack_bf16x8(o + c * 8));
           if ((u & 1) == 1 || g.BN == 64) {
             fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA store
             named_bar(bar_id, bar_cnt);
@@ -704,17 +700,9 @@ __global__ void stem_pack_image_kernel(const float* __restrict__ x, uint4* __res
     float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (hi >= 0 && hi < H && wi >= 0 && wi < W)
       for (int ch = 0; ch < C; ++ch) v[ch] = __ldg(x + (((size_t)n * C + ch) * H + hi) * W + wi);
-    uint4 o;
-    o.x = pack_bf16x2(v[0], v[1]); o.y = pack_bf16x2(v[2], v[3]); o.z = pack_bf16x2(v[4], v[5]); o.w = pack_bf16x2(v[6], v[7]);
+    const uint4 o = pack_bf16x8(v);
     xp[t] = o;
-    if (xp_lo) {     // pair stem: second plane = bf16(v - hi)
-      uint4 l;
-      l.x = pack_bf16x2(v[0] - __uint_as_float(o.x << 16), v[1] - __uint_as_float(o.x & 0xffff0000u));
-      l.y = pack_bf16x2(v[2] - __uint_as_float(o.y << 16), v[3] - __uint_as_float(o.y & 0xffff0000u));
-      l.z = pack_bf16x2(v[4] - __uint_as_float(o.z << 16), v[5] - __uint_as_float(o.z & 0xffff0000u));
-      l.w = pack_bf16x2(v[6] - __uint_as_float(o.w << 16), v[7] - __uint_as_float(o.w & 0xffff0000u));
-      xp_lo[t] = l;
-    }
+    if (xp_lo) xp_lo[t] = pair_lo8(v, o);     // pair stem: second plane = bf16(v - hi)
   }
 }
 
@@ -724,9 +712,10 @@ __global__ void stem_pack_weight_kernel(const float* __restrict__ w, int Cout, i
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int c = i & 7, kx = (i >> 3) & 7, ky = (i >> 6) % kh, co = i / (64 * kh);
     const float v = (c < Cin && kx < kw) ? w[(((size_t)co * Cin + c) * kh + ky) * kw + kx] : 0.f;
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
+    __nv_bfloat16 h, l;
+    split_bf16(v, h, l);
     packed[i] = h;
-    packed[total + i] = __float2bfloat16_rn(v - __bfloat162float(h));      // lo plane (pair stem)
+    packed[total + i] = l;      // lo plane (pair stem)
   }
 }
 

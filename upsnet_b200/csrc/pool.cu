@@ -6,6 +6,7 @@
 #include <cfloat>
 
 #include "common.cuh"
+#include "pair.cuh"
 #include "up4.cuh"
 
 namespace ups {
@@ -77,8 +78,7 @@ __global__ void maxpool_nhwc_pair_kernel(const uint4* __restrict__ x, uint4* __r
         const uint32_t hw[4] = {vh.x, vh.y, vh.z, vh.w}, lw[4] = {vl.x, vl.y, vl.z, vl.w};
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          const float a = __uint_as_float(hw[e] << 16) + __uint_as_float(lw[e] << 16);
-          const float b = __uint_as_float(hw[e] & 0xffff0000u) + __uint_as_float(lw[e] & 0xffff0000u);
+          const float a = pair_x(hw[e], lw[e]), b = pair_y(hw[e], lw[e]);
           if (a > best[2 * e]) { best[2 * e] = a; bh[e] = (bh[e] & 0xffff0000u) | (hw[e] & 0xffffu); bl[e] = (bl[e] & 0xffff0000u) | (lw[e] & 0xffffu); }
           if (b > best[2 * e + 1]) { best[2 * e + 1] = b; bh[e] = (bh[e] & 0xffffu) | (hw[e] & 0xffff0000u); bl[e] = (bl[e] & 0xffffu) | (lw[e] & 0xffff0000u); }
         }

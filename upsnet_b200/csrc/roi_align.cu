@@ -13,6 +13,7 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "pair.cuh"
 
 namespace ups {
 
@@ -195,16 +196,12 @@ roi_align_nhwc_bf16_kernel(FpnFeats f, int C, const float* __restrict__ rois, in
           const uint32_t a[2] = {v00.x, v00.y}, bq[2] = {v01.x, v01.y}, d[2] = {v10.x, v10.y}, e[2] = {v11.x, v11.y};
 #pragma unroll
           for (int q = 0; q < 2; ++q) {
-            acc[2 * q] += (s.w00 * __uint_as_float(a[q] << 16) + s.w01 * __uint_as_float(bq[q] << 16) +
-                           s.w10 * __uint_as_float(d[q] << 16) + s.w11 * __uint_as_float(e[q] << 16));
-            acc[2 * q + 1] += (s.w00 * __uint_as_float(a[q] & 0xffff0000u) + s.w01 * __uint_as_float(bq[q] & 0xffff0000u) +
-                               s.w10 * __uint_as_float(d[q] & 0xffff0000u) + s.w11 * __uint_as_float(e[q] & 0xffff0000u));
+            acc[2 * q] += (s.w00 * bf16x2_x(a[q]) + s.w01 * bf16x2_x(bq[q]) + s.w10 * bf16x2_x(d[q]) + s.w11 * bf16x2_x(e[q]));
+            acc[2 * q + 1] += (s.w00 * bf16x2_y(a[q]) + s.w01 * bf16x2_y(bq[q]) + s.w10 * bf16x2_y(d[q]) + s.w11 * bf16x2_y(e[q]));
           }
         }
       }
-      __nv_bfloat162 o0 = __floats2bfloat162_rn(acc[0] / cnt, acc[1] / cnt), o1 = __floats2bfloat162_rn(acc[2] / cnt, acc[3] / cnt);
-      uint2 w;
-      w.x = *reinterpret_cast<uint32_t*>(&o0); w.y = *reinterpret_cast<uint32_t*>(&o1);
+      const uint2 w = make_uint2(pack_bf16x2(acc[0] / cnt, acc[1] / cnt), pack_bf16x2(acc[2] / cnt, acc[3] / cnt));
       *reinterpret_cast<uint2*>(out + (((size_t)n * PH + ph) * PW + pw) * C + c) = w;
     }
   }
@@ -260,17 +257,12 @@ roi_align_nhwc_bf16_roi_kernel(FpnFeats f, int C, const float* __restrict__ rois
         const uint32_t d[4] = {v10.x, v10.y, v10.z, v10.w}, e[4] = {v11.x, v11.y, v11.z, v11.w};
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          acc[2 * k] += (w.x * __uint_as_float(a[k] << 16) + w.y * __uint_as_float(bq[k] << 16) +
-                         w.z * __uint_as_float(d[k] << 16) + w.w * __uint_as_float(e[k] << 16));
-          acc[2 * k + 1] += (w.x * __uint_as_float(a[k] & 0xffff0000u) + w.y * __uint_as_float(bq[k] & 0xffff0000u) +
-                             w.z * __uint_as_float(d[k] & 0xffff0000u) + w.w * __uint_as_float(e[k] & 0xffff0000u));
+          acc[2 * k] += (w.x * bf16x2_x(a[k]) + w.y * bf16x2_x(bq[k]) + w.z * bf16x2_x(d[k]) + w.w * bf16x2_x(e[k]));
+          acc[2 * k + 1] += (w.x * bf16x2_y(a[k]) + w.y * bf16x2_y(bq[k]) + w.z * bf16x2_y(d[k]) + w.w * bf16x2_y(e[k]));
         }
       }
-      uint4 wv;
-      __nv_bfloat162 o0 = __floats2bfloat162_rn(acc[0] / cnt, acc[1] / cnt), o1 = __floats2bfloat162_rn(acc[2] / cnt, acc[3] / cnt);
-      __nv_bfloat162 o2 = __floats2bfloat162_rn(acc[4] / cnt, acc[5] / cnt), o3 = __floats2bfloat162_rn(acc[6] / cnt, acc[7] / cnt);
-      wv.x = *reinterpret_cast<uint32_t*>(&o0); wv.y = *reinterpret_cast<uint32_t*>(&o1);
-      wv.z = *reinterpret_cast<uint32_t*>(&o2); wv.w = *reinterpret_cast<uint32_t*>(&o3);
+      const uint4 wv = make_uint4(pack_bf16x2(acc[0] / cnt, acc[1] / cnt), pack_bf16x2(acc[2] / cnt, acc[3] / cnt),
+                                  pack_bf16x2(acc[4] / cnt, acc[5] / cnt), pack_bf16x2(acc[6] / cnt, acc[7] / cnt));
       *reinterpret_cast<uint4*>(out + ((size_t)n * PH * PW + bin) * C + c) = wv;
     }
   }
@@ -332,25 +324,13 @@ roi_align_nhwc_pair_roi_kernel(FpnFeats f, int C, const float* __restrict__ rois
         const uint32_t E[4] = {h3.x, h3.y, h3.z, h3.w}, e[4] = {l3.x, l3.y, l3.z, l3.w};
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          acc[2 * k] += (w.x * (__uint_as_float(A[k] << 16) + __uint_as_float(a[k] << 16)) +
-                         w.y * (__uint_as_float(B[k] << 16) + __uint_as_float(bq[k] << 16)) +
-                         w.z * (__uint_as_float(D[k] << 16) + __uint_as_float(d[k] << 16)) +
-                         w.w * (__uint_as_float(E[k] << 16) + __uint_as_float(e[k] << 16)));
-          acc[2 * k + 1] += (w.x * (__uint_as_float(A[k] & 0xffff0000u) + __uint_as_float(a[k] & 0xffff0000u)) +
-                             w.y * (__uint_as_float(B[k] & 0xffff0000u) + __uint_as_float(bq[k] & 0xffff0000u)) +
-                             w.z * (__uint_as_float(D[k] & 0xffff0000u) + __uint_as_float(d[k] & 0xffff0000u)) +
-                             w.w * (__uint_as_float(E[k] & 0xffff0000u) + __uint_as_float(e[k] & 0xffff0000u)));
+          acc[2 * k] += (w.x * pair_x(A[k], a[k]) + w.y * pair_x(B[k], bq[k]) + w.z * pair_x(D[k], d[k]) + w.w * pair_x(E[k], e[k]));
+          acc[2 * k + 1] += (w.x * pair_y(A[k], a[k]) + w.y * pair_y(B[k], bq[k]) + w.z * pair_y(D[k], d[k]) + w.w * pair_y(E[k], e[k]));
         }
       }
       uint32_t hw[4], lw[4];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float u = acc[2 * k] / cnt, v = acc[2 * k + 1] / cnt;
-        __nv_bfloat162 hh = __floats2bfloat162_rn(u, v);
-        hw[k] = *reinterpret_cast<uint32_t*>(&hh);
-        __nv_bfloat162 ll = __floats2bfloat162_rn(u - __uint_as_float(hw[k] << 16), v - __uint_as_float(hw[k] & 0xffff0000u));
-        lw[k] = *reinterpret_cast<uint32_t*>(&ll);
-      }
+      for (int k = 0; k < 4; ++k) split_pair2(acc[2 * k] / cnt, acc[2 * k + 1] / cnt, hw[k], lw[k]);
       __nv_bfloat16* op = out + (size_t)n * roi_stride + (size_t)bin * pix_stride + c;
       *reinterpret_cast<uint4*>(op) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
       *reinterpret_cast<uint4*>(op + lo_off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);

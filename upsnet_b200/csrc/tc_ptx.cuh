@@ -1,11 +1,14 @@
 // tc_ptx.cuh -- PTX wrappers shared by the Hopper tensor-core kernels (igemm_tc.cu, igemm_tma.cu, dcn_win.cu): mbarriers,
 // TMA (bulk tensor) copies, wgmma (bf16 in, fp32 accumulators in registers) + its shared-memory descriptors, accumulator
-// staging through shared memory for the row-per-thread epilogues, named barriers, setmaxnreg, cp.async.
+// staging through shared memory for the row-per-thread epilogues, named barriers, setmaxnreg, cp.async.  The bf16 word and
+// hi/lo pair format these kernels read and write is in pair.cuh.
 #pragma once
 #include <cuda.h>   // CUtensorMap only
 #include <cuda_bf16.h>
 #include <cstdint>
 #include <cstdio>
+
+#include "pair.cuh"
 
 namespace ups {
 
@@ -203,25 +206,10 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_but2() { asm volatile("cp.async.wait_group 2;" ::: "memory"); }
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
 // 32-byte read-only global load (two 16-byte vectors); p must be 32-byte aligned
 __device__ __forceinline__ void ldg256(const void* p, uint4& lo, uint4& hi) {
   lo = __ldg(reinterpret_cast<const uint4*>(p));
   hi = __ldg(reinterpret_cast<const uint4*>(p) + 1);
-}
-// packed fp32 pairs (low word = first value): element-wise fma / add
-__device__ __forceinline__ unsigned long long f32x2_fma(unsigned long long a, unsigned long long b, unsigned long long c) {
-  const float r0 = fmaf(__uint_as_float((uint32_t)a), __uint_as_float((uint32_t)b), __uint_as_float((uint32_t)c));
-  const float r1 = fmaf(__uint_as_float((uint32_t)(a >> 32)), __uint_as_float((uint32_t)(b >> 32)), __uint_as_float((uint32_t)(c >> 32)));
-  return ((unsigned long long)__float_as_uint(r1) << 32) | __float_as_uint(r0);
-}
-__device__ __forceinline__ unsigned long long f32x2_add(unsigned long long a, unsigned long long b) {
-  const float r0 = __uint_as_float((uint32_t)a) + __uint_as_float((uint32_t)b);
-  const float r1 = __uint_as_float((uint32_t)(a >> 32)) + __uint_as_float((uint32_t)(b >> 32));
-  return ((unsigned long long)__float_as_uint(r1) << 32) | __float_as_uint(r0);
 }
 // w.x*a + w.y*b + w.z*d + w.w*e on packed bf16 pairs (weights replicated into both halves)
 __device__ __forceinline__ uint32_t bf2_blend(const uint4& w, uint32_t a, uint32_t b, uint32_t d, uint32_t e) {
@@ -233,6 +221,5 @@ __device__ __forceinline__ uint32_t bf2_blend(const uint4& w, uint32_t a, uint32
   acc = __hfma2(we, *reinterpret_cast<const __nv_bfloat162*>(&e), acc);
   return *reinterpret_cast<const uint32_t*>(&acc);
 }
-__device__ __forceinline__ float bf16_round(float a) { return __bfloat162float(__float2bfloat16_rn(a)); }
 
 }  // namespace ups

@@ -169,22 +169,27 @@ def _per_weight(cache, weight, make, device=None, versioned=True):
     return value
 
 
+def _packed(cache, weight, pack, nbytes, nbytes_args, unsupported=False):
+    """upsnet_<pack> of the fp32 weight [Cout,Cin,kh,kw] into a uint8 buffer of upsnet_<nbytes>(*nbytes_args) bytes, made
+    once per weight tensor and kept in `cache` (_per_weight).  With `unsupported`, None (cached too) when the size query
+    answers UPSNET_E_UNSUPPORTED."""
+    def make():
+        n = query_bytes(nbytes, *nbytes_args, unsupported=unsupported)
+        if n is None:
+            return None
+        buf = torch.empty(n, dtype=torch.uint8, device=weight.device)
+        call(pack, weight.device, f32c(weight.detach()), *weight.shape, buf)
+        STATS["launches"] += 1
+        return buf
+    return _per_weight(cache, weight, make, device=weight.device)
+
+
 _packed_cache = {}
 
 
 def _packed_weight(weight):
     """bf16 hi/lo planes [Cout_pad][kh*kw][Cin] (upsnet_igemm_pack_weight), cached per weight tensor+version."""
-    return _per_weight(_packed_cache, weight, lambda: _pack_igemm(weight), device=weight.device)
-
-
-def _pack_igemm(weight):
-    Cout, Cin, kh, kw = weight.shape
-    nbytes = query_bytes("igemm_packed_weight_bytes", Cout, Cin, kh, kw)
-    buf = torch.empty(nbytes, dtype=torch.uint8, device=weight.device)
-    w = f32c(weight.detach())
-    call("igemm_pack_weight", weight.device, w, Cout, Cin, kh, kw, buf)
-    STATS["launches"] += 1
-    return buf
+    return _packed(_packed_cache, weight, "igemm_pack_weight", "igemm_packed_weight_bytes", weight.shape)
 
 
 _dcn_packed_cache = {}
@@ -193,19 +198,7 @@ _dcn_packed_cache = {}
 def _packed_weight_dcn(weight):
     """upsnet_dcn_pack_weight: bf16 hi/lo planes in the window kernel's K order (16-channel sub-chunk, tap, channel);
     None when the layer shape is not supported by that kernel (cached too).  Cached like _packed_weight."""
-    return _per_weight(_dcn_packed_cache, weight, lambda: _pack_dcn(weight), device=weight.device)
-
-
-def _pack_dcn(weight):
-    Cout, Cin, kh, kw = weight.shape
-    nbytes = query_bytes("dcn_packed_weight_bytes", Cout, Cin, kh, kw, unsupported=True)
-    if nbytes is None:
-        return None
-    buf = torch.empty(nbytes, dtype=torch.uint8, device=weight.device)
-    w = f32c(weight.detach())
-    call("dcn_pack_weight", weight.device, w, Cout, Cin, kh, kw, buf)
-    STATS["launches"] += 1
-    return buf
+    return _packed(_dcn_packed_cache, weight, "dcn_pack_weight", "dcn_packed_weight_bytes", weight.shape, unsupported=True)
 
 
 def _dcn_window(x, offset, mask, weight, bias, padding, dilation, relu):
@@ -246,14 +239,7 @@ def stem_conv(x, weight, bias, padding, relu=True, pair=False):
     Cout, _, kh, kw = weight.shape
     dev = x.device
 
-    def pack():
-        nb = query_bytes("stem_packed_weight_bytes", Cout, kh)
-        packed = torch.empty(nb, dtype=torch.uint8, device=dev)
-        call("stem_pack_weight", dev, f32c(weight.detach()), Cout, Cin, kh, kw, packed)
-        STATS["launches"] += 1
-        return packed
-
-    packed = _per_weight(_stem_cache, weight, pack, device=dev)
+    packed = _packed(_stem_cache, weight, "stem_pack_weight", "stem_packed_weight_bytes", (Cout, kh))
     nb = query_bytes("stem_workspace_bytes", N, H, W, kh, kw, int(padding))
     if _stem_ws is None:
         _stem_ws = _Workspace()
