@@ -676,6 +676,97 @@ int upsnet_panoptic_gt(const int64_t *seg_gt, const void *mask_gt, int mask_gt_i
  * 0 is its fg draw, 1 its bg draw), so that a host restatement of the rule can be compared with the device's. */
 int upsnet_draw_keys(unsigned long long seed, int stream_id, int n, unsigned long long *keys, void *stream);
 
+/* ---- training losses (train_loss.cu) ----------------------------------------------------
+ * upsnet_semantic_loss_forward / _backward: the semantic head's loss of one image, with the x4 up-sampling fused in.
+ * replaces: models/fcn.py:101 F.interpolate(fcn_score, None, 4, mode='bilinear', align_corners=False) and
+ *           models/resnet_upsnet.py:79,131 CrossEntropyLoss(ignore_index=255)(fcn_output, seg_gt), with autograd's
+ *           backward of that composition.  No [S,4h,4w] tensor is built; backward keeps 4 bytes per output pixel.
+ * Inputs (device): fcn_score float32 [S,h,w]; seg_gt [4h,4w], uint8 or int64 (seg_gt_is_int64).  The logits of output
+ *   pixel o are those upsnet_upsample_bilinear_nchw (factor 4) writes, bit for bit (up4.cuh).  t(o) = seg_gt[o].
+ * Outputs (device): loss[1] = sum over pixels with t in 0..S-1 of (log-sum-exp - logit of t), divided by their count N
+ *   (NaN when N = 0, as torch's mean); counts int32 [2] = (N, pixels whose label is neither 255 nor in 0..S-1: torch
+ *   would assert on them; here they give no loss and no gradient and are not in N); lse float32 [4h*4w], 16-byte
+ *   aligned, is what backward reads (written everywhere, meaningful where t is a channel).
+ * Backward: grad_out float32 [1] and counts (forward's) on the device; d_fcn_score float32 [S,h,w], every element
+ *   written: grad_out / N * sum over o of w(o -> source) * (softmax_c(o) - [c = t(o)]), w the up-sampling's tap
+ *   weights, as a gather (no atomics); all zeros when N = 0.
+ * Same inputs give the same bytes; no call synchronises or reads the device; both are capturable.
+ * Limits: S*h*w < 2^31, 16*h*w < 2^31, S <= 32767 (else UPSNET_E_UNSUPPORTED).
+ * Workspace: upsnet_semantic_loss_workspace_bytes(h, w), forward only; nothing in it outlives the call. */
+int upsnet_semantic_loss_workspace_bytes(int h, int w, size_t *bytes);
+int upsnet_semantic_loss_forward(const float *fcn_score, int S, int h, int w, const void *seg_gt, int seg_gt_is_int64,
+                                 float *loss, int *counts, float *lse, void *workspace, size_t workspace_bytes,
+                                 void *stream);
+int upsnet_semantic_loss_backward(const float *fcn_score, int S, int h, int w, const void *seg_gt, int seg_gt_is_int64,
+                                  const float *lse, const int *counts, const float *grad_out, float *d_fcn_score,
+                                  void *stream);
+
+/* upsnet_rpn_loss_forward / _backward: the RPN loss of one image over all FPN levels in one launch.
+ * replaces: models/rpn.py:60-92 RPNLoss.forward (with_fpn): per level, the [:, :, :h, :w] slices of the label maps,
+ *           F.binary_cross_entropy_with_logits(score, label, weight = label != -1, reduction='sum') / rpn_batch_size
+ *           and smooth_l1_loss(sigma = 3) / batch (= 1), summed over the levels; with autograd's backward.
+ * Inputs: host arrays of num_levels entries (num_levels <= 8): h[l], w[l] = the score map's size; device pointers
+ *   cls_score[l] float32 [A,h,w], bbox_pred[l] float32 [4A,h,w] (contiguous); labels[l] int64 and bbox_targets[l],
+ *   bbox_inside_weights[l], bbox_outside_weights[l] float32, read in place from fields at least as large as the map:
+ *   element (c, y, x) of level l is at c * strides[2l] + y * strides[2l+1] + x (label_strides for the labels,
+ *   bbox_strides for the three box fields), no slice copies.
+ * Outputs (device): cls_loss[1] = sum over anchors with label != -1 of (1 - t) x + m + log(exp(-m) + exp(-x - m)),
+ *   m = max(-x, 0), divided by rpn_batch_size; bbox_loss[1] = sum of ow * (|d| < 1/9 ? 4.5 d^2 : |d| - 0.5/9),
+ *   d = iw * (pred - target).
+ * Backward: grad_cls, grad_bbox float32 [1] on the device; d_cls_score[l] = (label != -1) (sigmoid(x) - t) grad_cls /
+ *   rpn_batch_size, d_bbox_pred[l] = ow iw (|d| < 1/9 ? 9 d : sign d) grad_bbox, every element written; either host
+ *   array may be NULL.
+ * Same inputs give the same bytes; no call synchronises or reads the device; both are capturable.  Batch size 1.
+ * Limits: num_levels <= 8, 4A*h*w < 2^31 per level and A * sum h*w < 2^31 (else UPSNET_E_UNSUPPORTED).
+ * Workspace: upsnet_rpn_loss_workspace_bytes(A * sum of h[l]*w[l]), forward only. */
+int upsnet_rpn_loss_workspace_bytes(int num_anchors, size_t *bytes);
+int upsnet_rpn_loss_forward(int num_levels, int A, const int *h, const int *w, const float *const *cls_score,
+                            const float *const *bbox_pred, const int64_t *const *labels, const long long *label_strides,
+                            const float *const *bbox_targets, const float *const *bbox_inside_weights,
+                            const float *const *bbox_outside_weights, const long long *bbox_strides,
+                            float rpn_batch_size, float *cls_loss, float *bbox_loss, void *workspace,
+                            size_t workspace_bytes, void *stream);
+int upsnet_rpn_loss_backward(int num_levels, int A, const int *h, const int *w, const float *const *cls_score,
+                             const float *const *bbox_pred, const int64_t *const *labels, const long long *label_strides,
+                             const float *const *bbox_targets, const float *const *bbox_inside_weights,
+                             const float *const *bbox_outside_weights, const long long *bbox_strides,
+                             float rpn_batch_size, const float *grad_cls, const float *grad_bbox,
+                             float *const *d_cls_score, float *const *d_bbox_pred, void *stream);
+
+/* upsnet_mask_rcnn_loss_forward / _backward: the Mask R-CNN loss and accuracy of one image.
+ * replaces: models/rcnn.py:159-197 MaskRCNNLoss.forward: CrossEntropyLoss(ignore_index=-1), smooth_l1_loss(sigma = 1)
+ *           / R, rcnn_accuracy and mask_loss / (mask_weight.sum() + 1e-10); with autograd's backward.
+ * Inputs (device, contiguous): cls_score float32 [R,K]; cls_label int64 [R]; bbox_pred, bbox_target,
+ *   bbox_inside_weight, bbox_outside_weight float32 [R,B]; mask_score, mask_target float32 of mask_numel elements
+ *   each ([n,K,M,M] and [n,K*M*M]; both may be NULL when mask_numel = 0).  Forward reads each once.
+ * Outputs (device): cls_loss[1] = mean over rows with a label in 0..K-1 of (log-sum-exp - logit of the label) (NaN
+ *   without such rows); bbox_loss[1] = sum of ow * (|d| < 1 ? d^2 / 2 : |d| - 1/2), d = iw * (pred - target), / R;
+ *   mask_loss[1] = sum over t != -1 of -x (t - b) + log(1 + exp(-|x|)), b = (x >= 0), divided by float32(W) + 1e-10
+ *   in float32, W the number of such elements (0 when W = 0); accuracy[1] = (counts[2] - counts[1]) / (R - counts[1])
+ *   (rcnn_accuracy as written: the rows labelled -1 are subtracted from the correct ones too); counts int32 [4] =
+ *   (rows with a label in 0..K-1, rows labelled -1, rows whose arg-max (ties: the lowest class) equals the label, W).
+ *   A label outside -1..K-1 (torch asserts on it) gives no loss and no gradient.
+ * Backward: counts (forward's) and grad_cls, grad_bbox, grad_mask float32 [1] on the device; d_cls_score =
+ *   (softmax - onehot) grad_cls / counts[0] on rows with a label, else 0; d_bbox_pred = ow iw (|d| < 1 ? d : sign d)
+ *   grad_bbox / R; d_mask_score = (t != -1) (sigmoid(x) - t) grad_mask / (float32(W) + 1e-10).  Every element is
+ *   written; any of the three may be NULL.
+ * Same inputs give the same bytes; no call synchronises or reads the device; both are capturable.
+ * Limits: R*K, R*B and mask_numel < 2^31 (else UPSNET_E_UNSUPPORTED); R >= 1.
+ * Workspace: upsnet_mask_rcnn_loss_workspace_bytes(R, B, mask_numel), forward only. */
+int upsnet_mask_rcnn_loss_workspace_bytes(int R, int B, long long mask_numel, size_t *bytes);
+int upsnet_mask_rcnn_loss_forward(const float *cls_score, const int64_t *cls_label, int R, int K, const float *bbox_pred,
+                                  const float *bbox_target, const float *bbox_inside_weight,
+                                  const float *bbox_outside_weight, int B, const float *mask_score,
+                                  const float *mask_target, long long mask_numel, float *cls_loss, float *bbox_loss,
+                                  float *mask_loss, float *accuracy, int *counts, void *workspace,
+                                  size_t workspace_bytes, void *stream);
+int upsnet_mask_rcnn_loss_backward(const float *cls_score, const int64_t *cls_label, int R, int K, const float *bbox_pred,
+                                   const float *bbox_target, const float *bbox_inside_weight,
+                                   const float *bbox_outside_weight, int B, const float *mask_score,
+                                   const float *mask_target, long long mask_numel, const int *counts,
+                                   const float *grad_cls, const float *grad_bbox, const float *grad_mask,
+                                   float *d_cls_score, float *d_bbox_pred, float *d_mask_score, void *stream);
+
 /* ---- panoptic training labels (labels.cu) ----
  * upsnet_training_labels: the label maps of one training image (the label block of the reference's Cityscapes / COCO
  * loaders and collate / gt_list_to_blob) from its uint8 label map [h0,w0]:

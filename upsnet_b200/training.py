@@ -20,10 +20,15 @@
 * PanopticLoss: the panoptic head of the training forward (models/resnet_upsnet.py:144-179: SegTerm, MaskTerm, the void
   logits, MaskMatching, calc_panoptic_acc and the cross-entropy) as one fused loss with hand-written forward and
   backward kernels (csrc/panoptic_loss.cu), plus the two host helpers for the lines before it (gt_rois, draw_keep).
+* SemanticLoss, RPNLoss, MaskRCNNLoss: the other losses of the training forward (models/resnet_upsnet.py:127-142) with
+  hand-written forward and backward kernels (csrc/train_loss.cu).  SemanticLoss evaluates the x4 up-sampling of
+  fcn_score inside the cross-entropy, so the [1,S,4h,4w] fcn_output (159 MB at 1024x2048, S 19), its log-softmax and
+  its gradient are never built; RPNLoss covers the five FPN levels in one launch and reads the label fields in place;
+  MaskRCNNLoss reads mask_score and mask_target once.
 
-Scope note: this is the operator / communication layer of the training configuration plus the RPN and proposal targets
-and the panoptic loss.  The other losses (RPN, RCNN, mask, semantic) and the optimiser are library calls on dense
-tensors in the reference and stay that way; the dense backward convolutions are library calls.
+Scope note: this is the operator / communication layer of the training configuration, the RPN and proposal targets,
+the label maps and every loss of the training forward.  fcn_roi_loss (train.fcn_with_roi_loss is off in every shipped
+configuration) and the optimiser are not built; the dense backward convolutions are library calls.
 """
 import ctypes as C
 
@@ -678,6 +683,257 @@ class PanopticLoss(torch.nn.Module):
             self.num_classes, self.enable_void, self.box_scale, M)
         self.counts = counts
         return loss, acc
+
+
+# ------------------------------------------------------------------------------------------------
+# semantic, RPN and Mask R-CNN losses
+# ------------------------------------------------------------------------------------------------
+def _scalars(dev, n):
+    return [torch.empty((), dtype=torch.float32, device=dev) for _ in range(n)]
+
+
+def _grad(g, dev):
+    """A loss's incoming gradient as a float32 [1] device tensor (zero when autograd passes None)."""
+    return torch.zeros(1, dtype=torch.float32, device=dev) if g is None else f32c(g).reshape(1)
+
+
+class SemanticLossFunction(torch.autograd.Function):
+    """(loss, counts) = the fused semantic loss (include/upsnet_b200.h, upsnet_semantic_loss_forward); differentiable in
+    fcn_score.  Inputs are validated by SemanticLoss.forward."""
+
+    @staticmethod
+    def forward(ctx, fcn_score, seg_gt):
+        dev = fcn_score.device
+        _, S, h, w = fcn_score.shape
+        fcn = f32c(fcn_score.detach())
+        (loss,) = _scalars(dev, 1)
+        counts = torch.empty(2, dtype=torch.int32, device=dev)
+        lse = torch.empty(16 * h * w, dtype=torch.float32, device=dev)
+        ws = torch.empty(query_bytes("semantic_loss_workspace_bytes", h, w), dtype=torch.uint8, device=dev)
+        is64 = int(seg_gt.dtype == torch.int64)
+        call("semantic_loss_forward", dev, fcn, S, h, w, seg_gt, is64, loss, counts, lse, ws, ws.numel())
+        ctx.save_for_backward(fcn, seg_gt, lse, counts)
+        ctx.mark_non_differentiable(counts)
+        return loss, counts
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_counts):
+        fcn, seg, lse, counts = ctx.saved_tensors
+        _, S, h, w = fcn.shape
+        dfcn = torch.empty_like(fcn)
+        call("semantic_loss_backward", fcn.device, fcn, S, h, w, seg, int(seg.dtype == torch.int64), lse, counts,
+             _grad(grad_loss, fcn.device), dfcn)
+        return dfcn, None
+
+
+class SemanticLoss(torch.nn.Module):
+    """The semantic head's loss of one training image (models/fcn.py:101 + models/resnet_upsnet.py:79,131):
+    CrossEntropyLoss(ignore_index=255)(F.interpolate(fcn_score, scale_factor=4, mode='bilinear', align_corners=False),
+    seg_gt), with the x4 up-sampling evaluated inside the loss (the logits are ops.upsample_bilinear's, bit for bit), so
+    the [1,S,4h,4w] tensor, its log-softmax and its gradient are never built.  Backward keeps 4 bytes per output pixel.
+
+    A label that is neither 255 nor a channel (torch asserts on it) gives no loss and no gradient; self.counts, int32 [2]
+    on the device, is (pixels in the mean, such invalid pixels).  When every pixel is ignored the loss is NaN and the
+    gradient zero, as torch's.  The same inputs give the same bytes."""
+
+    def forward(self, fcn_score, seg_gt):
+        """fcn_score [1,S,h,w] (float32; other float dtypes are cast); seg_gt [1,4h,4w] int64 or uint8.  -> loss, a
+        0-dim device tensor."""
+        E = _lib.UpsnetError
+        require_cuda(fcn_score, seg_gt)
+        if fcn_score.dim() != 4 or fcn_score.shape[0] != 1:
+            raise E("semantic_loss: only batch size 1 (fcn_score [1,S,h,w])")
+        _, S, h, w = fcn_score.shape
+        if seg_gt.dim() != 3 or tuple(seg_gt.shape) != (1, 4 * h, 4 * w):
+            raise E("semantic_loss: seg_gt must be [1,%d,%d] (four times fcn_score's size), not %s"
+                    % (4 * h, 4 * w, tuple(seg_gt.shape)))
+        if seg_gt.dtype not in (torch.int64, torch.uint8):
+            raise E("semantic_loss: seg_gt must be int64 or uint8")
+        loss, counts = SemanticLossFunction.apply(fcn_score, seg_gt.contiguous())
+        self.counts = counts
+        return loss
+
+
+def _carray(ctype, values):
+    return (ctype * len(values))(*values)
+
+
+class RPNLossFunction(torch.autograd.Function):
+    """(cls_loss, bbox_loss) = the fused RPN loss (include/upsnet_b200.h, upsnet_rpn_loss_forward), differentiable in
+    every level's score and box prediction.  `fields` holds the per-level label maps and their strides; inputs are
+    validated by RPNLoss.forward."""
+
+    @staticmethod
+    def forward(ctx, fields, batch, *maps):
+        L = len(maps) // 2
+        scores, preds = [f32c(m.detach()) for m in maps[:L]], [f32c(m.detach()) for m in maps[L:]]
+        dev = scores[0].device
+        A = scores[0].shape[1]
+        args = RPNLossFunction._args(scores, preds, fields)
+        total = A * sum(s.shape[2] * s.shape[3] for s in scores)
+        cls_loss, bbox_loss = _scalars(dev, 2)
+        ws = torch.empty(query_bytes("rpn_loss_workspace_bytes", total), dtype=torch.uint8, device=dev)
+        call("rpn_loss_forward", dev, L, A, *args, float(batch), cls_loss, bbox_loss, ws, ws.numel())
+        ctx.save_for_backward(*scores, *preds)
+        ctx.fields, ctx.batch = fields, batch
+        return cls_loss, bbox_loss
+
+    @staticmethod
+    def _args(scores, preds, fields):
+        """The per-level host arrays of the C call, from h / w through bbox_strides."""
+        ptrs = lambda ts: _carray(C.c_void_p, [t.data_ptr() for t in ts])  # noqa: E731
+        lab, tgt, iw, ow, lst, bst = fields
+        return (_carray(C.c_int, [s.shape[2] for s in scores]), _carray(C.c_int, [s.shape[3] for s in scores]),
+                ptrs(scores), ptrs(preds), ptrs(lab), _carray(C.c_longlong, lst), ptrs(tgt), ptrs(iw), ptrs(ow),
+                _carray(C.c_longlong, bst))
+
+    @staticmethod
+    def backward(ctx, grad_cls, grad_bbox):
+        t = ctx.saved_tensors
+        L = len(t) // 2
+        scores, preds = list(t[:L]), list(t[L:])
+        dev = scores[0].device
+        want_s = any(ctx.needs_input_grad[2:2 + L])
+        want_p = any(ctx.needs_input_grad[2 + L:])
+        ds = [torch.empty_like(s) for s in scores] if want_s else None
+        dp = [torch.empty_like(p) for p in preds] if want_p else None
+        if want_s or want_p:
+            ptrs = lambda ts: _carray(C.c_void_p, [x.data_ptr() for x in ts]) if ts is not None else None  # noqa: E731
+            call("rpn_loss_backward", dev, L, scores[0].shape[1], *RPNLossFunction._args(scores, preds, ctx.fields),
+                 float(ctx.batch), _grad(grad_cls, dev), _grad(grad_bbox, dev), ptrs(ds), ptrs(dp))
+        return (None, None) + tuple(ds if want_s else [None] * L) + tuple(dp if want_p else [None] * L)
+
+
+class RPNLoss(torch.nn.Module):
+    """RPNLoss.forward of models/rpn.py:60-92 (with_fpn) for one image, all FPN levels in one launch forward and one
+    backward: BCE-with-logits of the scores against the labels (weight label != -1, sum / rpn_batch_size) and the
+    smooth-L1 (sigma 3) of the box predictions with inside / outside weights (sum / batch, batch 1), each summed over the
+    levels.  The label dict is RPNTargets' (or the reference loader's, on the device); its F x F field maps are read in
+    place through their strides where the reference slices [:, :, :h, :w].  Built from the reference's `config`
+    (train.rpn_batch_size * train.batch_size, as models/resnet_upsnet.py:79 does) or `rpn_batch_size`.  The same inputs
+    give the same bytes."""
+
+    STRIDES = (4, 8, 16, 32, 64)
+
+    def __init__(self, config=None, *, rpn_batch_size=256):
+        super().__init__()
+        if config is not None:
+            rpn_batch_size = config.train.rpn_batch_size * config.train.batch_size
+        self.rpn_batch_size = int(rpn_batch_size)
+
+    def forward(self, rpn_cls_score, rpn_bbox_pred, label):
+        """rpn_cls_score / rpn_bbox_pred: the per-level lists [1,A,h,w] / [1,4A,h,w], strides 4, 8, ... in order;
+        label: dict with 'rpn_labels_fpn{s}' [1,A,F,F] and 'rpn_bbox_{targets,inside_weights,outside_weights}_fpn{s}'
+        [1,4A,F,F], F >= h, w.  -> (cls_loss, bbox_loss), 0-dim device tensors."""
+        E = _lib.UpsnetError
+        scores, preds = list(rpn_cls_score), list(rpn_bbox_pred)
+        if not scores or len(scores) != len(preds) or len(scores) > len(self.STRIDES):
+            raise E("rpn_loss: one score and one box map per level, at most %d levels" % len(self.STRIDES))
+        require_cuda(*scores, *preds)
+        A = scores[0].shape[1]
+        lab, tgt, iw, ow, lst, bst = [], [], [], [], [], []
+        for s, p, st in zip(scores, preds, self.STRIDES):
+            if s.dim() != 4 or s.shape[0] != 1 or p.dim() != 4 or p.shape[0] != 1:
+                raise E("rpn_loss: only batch size 1 (score [1,A,h,w], box prediction [1,4A,h,w])")
+            h, w = s.shape[2:]
+            if s.shape[1] != A or tuple(p.shape[1:]) != (4 * A, h, w):
+                raise E("rpn_loss: stride %d: score %s and box prediction %s do not match" % (st, tuple(s.shape),
+                                                                                            tuple(p.shape)))
+            try:
+                lv = [label[k % st] for k in ("rpn_labels_fpn%d", "rpn_bbox_targets_fpn%d",
+                                               "rpn_bbox_inside_weights_fpn%d", "rpn_bbox_outside_weights_fpn%d")]
+            except KeyError as e:
+                raise E("rpn_loss: label has no %s" % e) from None
+            require_cuda(*lv)
+            for f, ch in zip(lv, (A, 4 * A, 4 * A, 4 * A)):
+                if f.dim() != 4 or f.shape[0] != 1 or f.shape[1] != ch:
+                    raise E("rpn_loss: stride %d: label field %s is not [1,%d,F,F]" % (st, tuple(f.shape), ch))
+                if f.shape[2] < h or f.shape[3] < w:
+                    raise E("rpn_loss: stride %d: label field %s is smaller than the %dx%d map" % (st, tuple(f.shape), h, w))
+            l0 = lv[0] if lv[0].dtype == torch.int64 else lv[0].to(torch.int64)
+            box = [f if f.dtype == torch.float32 else f.float() for f in lv[1:]]
+            if l0.stride(3) != 1:
+                l0 = l0.contiguous()
+            if any(b.stride() != box[0].stride() or b.shape != box[0].shape or b.stride(3) != 1 for b in box):
+                box = [b.contiguous() for b in box]
+            lab.append(l0); tgt.append(box[0]); iw.append(box[1]); ow.append(box[2])
+            lst += [l0.stride(1), l0.stride(2)]
+            bst += [box[0].stride(1), box[0].stride(2)]
+        return RPNLossFunction.apply((lab, tgt, iw, ow, lst, bst), self.rpn_batch_size, *scores, *preds)
+
+
+class MaskRCNNLossFunction(torch.autograd.Function):
+    """(cls_loss, bbox_loss, mask_loss, accuracy, counts) = the fused Mask R-CNN loss (include/upsnet_b200.h,
+    upsnet_mask_rcnn_loss_forward), differentiable in cls_score, bbox_pred and mask_score.  Inputs are validated by
+    MaskRCNNLoss.forward."""
+
+    @staticmethod
+    def forward(ctx, cls_score, bbox_pred, mask_score, cls_label, bbox_target, iw, ow, mask_target):
+        cls, pred, msk = f32c(cls_score.detach()), f32c(bbox_pred.detach()), f32c(mask_score.detach())
+        dev = cls.device
+        R, K = cls.shape
+        B, n = pred.shape[1], msk.numel()
+        outs = _scalars(dev, 4)
+        counts = torch.empty(4, dtype=torch.int32, device=dev)
+        ws = torch.empty(query_bytes("mask_rcnn_loss_workspace_bytes", R, B, n), dtype=torch.uint8, device=dev)
+        args = (cls, cls_label, R, K, pred, bbox_target, iw, ow, B, msk if n else None, mask_target if n else None, n)
+        call("mask_rcnn_loss_forward", dev, *args, *outs, counts, ws, ws.numel())
+        ctx.save_for_backward(cls, cls_label, pred, bbox_target, iw, ow, msk, mask_target, counts)
+        ctx.mark_non_differentiable(outs[3], counts)
+        return (*outs, counts)
+
+    @staticmethod
+    def backward(ctx, grad_cls, grad_bbox, grad_mask, _grad_acc, _grad_counts):
+        cls, lab, pred, tgt, iw, ow, msk, mtgt, counts = ctx.saved_tensors
+        dev = cls.device
+        R, K = cls.shape
+        B, n = pred.shape[1], msk.numel()
+        need = ctx.needs_input_grad
+        dcls = torch.empty_like(cls) if need[0] else None
+        dpred = torch.empty_like(pred) if need[1] else None
+        dmsk = torch.empty_like(msk) if need[2] else None
+        if need[0] or need[1] or (need[2] and n):
+            call("mask_rcnn_loss_backward", dev, cls, lab, R, K, pred, tgt, iw, ow, B, msk if n else None,
+                 mtgt if n else None, n, counts, _grad(grad_cls, dev), _grad(grad_bbox, dev), _grad(grad_mask, dev),
+                 dcls, dpred, dmsk if n else None)
+        return (dcls, dpred, dmsk) + (None,) * 5
+
+
+class MaskRCNNLoss(torch.nn.Module):
+    """MaskRCNNLoss.forward of models/rcnn.py:159-197 for one image, one fused launch forward and one backward:
+    cross-entropy with ignore_index -1 (mean over the other rows), smooth-L1 (sigma 1, sum / R), rcnn_accuracy exactly as
+    written ((correct - ignored) / (R - ignored), the ignored rows subtracted from the correct ones too) and the mask loss
+    sum(w (-x (t - b) + log(1 + exp(x - 2 x b)))) / (sum(w) + 1e-10), w = (t != -1), b = (x >= 0).  Takes the outputs of
+    ProposalTargets.from_roidb unchanged.  self.counts, int32 [4] on the device: (rows in the mean, rows labelled -1, rows
+    whose arg-max equals the label, mask elements with a target).  `batch_size` is accepted for the reference's
+    signature and, as there, unused.  The same inputs give the same bytes."""
+
+    def __init__(self, batch_size=None):
+        super().__init__()
+        self.counts = None
+
+    def forward(self, cls_score, bbox_pred, mask_score, cls_label, bbox_target, bbox_inside_weight, bbox_outside_weight,
+                mask_target):
+        """cls_score [R,K]; bbox_pred and the three box tensors [R,B]; mask_score [n,K,M,M]; cls_label [R] (int64;
+        -1 ignored); mask_target [n,K*M*M] (or any shape of as many elements; -1 ignored).  -> (cls_loss, bbox_loss,
+        mask_loss, accuracy), 0-dim device tensors."""
+        E = _lib.UpsnetError
+        box = (bbox_target, bbox_inside_weight, bbox_outside_weight)
+        require_cuda(cls_score, bbox_pred, mask_score, cls_label, mask_target, *box)
+        if cls_score.dim() != 2 or cls_score.shape[0] == 0:
+            raise E("mask_rcnn_loss: cls_score must be [R,K] with R >= 1")
+        R = cls_score.shape[0]
+        if cls_label.numel() != R:
+            raise E("mask_rcnn_loss: cls_label must have one entry per cls_score row")
+        if bbox_pred.dim() != 2 or bbox_pred.shape[0] != R or any(tuple(b.shape) != tuple(bbox_pred.shape) for b in box):
+            raise E("mask_rcnn_loss: bbox_pred and the box targets / weights must all be [R,B]")
+        if mask_score.dim() != 4 or mask_target.numel() != mask_score.numel() or (
+                mask_target.dim() and mask_target.shape[0] != mask_score.shape[0]):
+            raise E("mask_rcnn_loss: mask_target must have mask_score's rows and elements ([n,K*M*M] for [n,K,M,M])")
+        loss = MaskRCNNLossFunction.apply(cls_score, bbox_pred, mask_score, cls_label.to(torch.int64).reshape(-1).contiguous(),
+                                          *[f32c(b) for b in box], f32c(mask_target))
+        self.counts = loss[4]
+        return loss[:4]
 
 
 # ------------------------------------------------------------------------------------------------
