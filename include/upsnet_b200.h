@@ -792,6 +792,64 @@ int upsnet_training_labels(const unsigned char* label, int h0, int w0, const int
                            int max_obj_verts, void* mask_gt, int mask_gt_is_int64, const int* roi_rows,
                            const int* roi_cols, int n_roi, int M, int64_t* seg_roi_gt, void* stream);
 
+/* ---- optimiser step (sgd.cu) ----------------------------------------------------------------
+ * upsnet_sgd_apply: one momentum-SGD step over every parameter listed in a chunk table, in one launch.
+ * replaces: lib/nn/optimizer.py:80-104 SGD.step(lr) (four element-wise ops per parameter, issued from Python), the
+ *           '/ world' and copy into p.grad of an all-reduced bf16 bucket before it, and the momentum decay of
+ *           upsnet_end2end_train.py:235-240 (every momentum buffer .div_(10) after a decay iteration).
+ * Chunk table (device, 8-byte aligned, num_chunks entries of upsnet_sgd_chunk): one CTA per entry.  param / buf / grad
+ *   point at the entry's first element; n >= 0 elements; group indexes the three host arrays of num_groups entries
+ *   (1 <= num_groups <= UPSNET_SGD_MAX_GROUPS, else UPSNET_E_UNSUPPORTED).  kind UPSNET_SGD_GRAD_F32: grad is float32
+ *   (a p.grad); UPSNET_SGD_GRAD_BF16: grad is a bf16 bucket segment, read as float32 and multiplied by inv_world
+ *   (= 1.0f / world, what torch's CUDA true division by a host scalar does); UPSNET_SGD_GRAD_NONE: a parameter with a
+ *   momentum buffer but no gradient this step, whose buffer only the decay touches (grad unused).  buf may be NULL in a
+ *   group whose momentum is 0.  Any addresses are accepted: 16-byte accesses are used where param, buf and grad allow
+ *   them (grad: 16 bytes for float32, 8 for bf16), element accesses otherwise.  Entries of at most UPSNET_SGD_CHUNK
+ *   elements keep the grid balanced; the ranges of different entries must not overlap.
+ * Learning rate: lr_table == NULL: `lr`, no decay (the drop-in step(lr)).  Otherwise the scheduled step: k =
+ *   *iteration - table_begin (device int), lr = lr_table[k] (device float64 [table_len]) and decay = decay_table[k]
+ *   (device uint8); when k is outside [0, table_len) the launch changes nothing.
+ * Rounding, per element, with glr = group_lr[group], wd = group_weight_decay[group], m = group_momentum[group]; each line
+ *   rounds once to float32 (fma: one fused rounding; torch's CUDA add_(x, alpha=) is self + alpha * x, one FMA):
+ *     d = g                              (bf16: float(g) * inv_world)
+ *     d = fma(wd, p, d)                  only if wd != 0 (skipped, not multiplied by 0)
+ *     a = (float)(glr * lr)              the double product rounded once, as torch converts the Python scalar
+ *     b = fma(a, d, b * m); p = p - b    if m != 0 (a new buffer is +0, so its first value is +0 * m + a d)
+ *     p = p - d                          if m == 0: lr does not enter, as in the reference
+ *     b = b * 0.1f                       after the update, on a decay step (div_(10) on CUDA multiplies by 1.0f / 10)
+ *   p.grad is not written (the reference leaves g + wd p in it; nothing reads that).  No atomics: same inputs, same bytes.
+ * upsnet_sgd_pack: the bf16 bucket of FlatBucketAllReduce.start() from the parameters' float32 gradients, one launch per
+ *   bucket: out[i] = bf16 round-to-nearest-even of grad[i] (torch's .to(torch.bfloat16)), zeros where grad is NULL (a
+ *   None gradient).  Table (device, 8-byte aligned) of upsnet_sgd_pack_chunk, one CTA per entry, any alignment.
+ * upsnet_sgd_advance: *iteration += 1 in a one-thread launch; the scheduled step issues it after its apply launches.
+ * None of the three synchronises or reads the device; all are capturable in a CUDA graph. */
+#define UPSNET_SGD_MAX_GROUPS 16
+#define UPSNET_SGD_CHUNK 8192
+#define UPSNET_SGD_GRAD_F32 0
+#define UPSNET_SGD_GRAD_BF16 1
+#define UPSNET_SGD_GRAD_NONE 2
+typedef struct {
+  float *param;
+  float *buf;
+  const void *grad;
+  int n;
+  int group;
+  int kind;
+  float inv_world;
+} upsnet_sgd_chunk; /* 40 bytes */
+typedef struct {
+  const float *grad;
+  void *out;
+  int n;
+  int reserved;
+} upsnet_sgd_pack_chunk; /* 24 bytes */
+int upsnet_sgd_apply(const upsnet_sgd_chunk *chunks, int num_chunks, int num_groups, const double *group_lr,
+                     const float *group_weight_decay, const float *group_momentum, double lr, const double *lr_table,
+                     const unsigned char *decay_table, const int *iteration, int table_begin, int table_len,
+                     void *stream);
+int upsnet_sgd_pack(const upsnet_sgd_pack_chunk *chunks, int num_chunks, void *stream);
+int upsnet_sgd_advance(int *iteration, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,7 +9,8 @@
   the *WithOffset* modules differentiable; its backward convs are library calls too.
 * FlatBucketAllReduce: the gradient all-reduce of `upsnet_end2end_train.py:121` (hvd.DistributedOptimizer) as flat bf16
   buckets over torch.distributed (NCCL between the GPUs, gloo in the CPU tests): gradients are packed per bucket,
-  reduced asynchronously while the rest of backward runs, averaged and unpacked before the optimiser step.
+  reduced asynchronously while the rest of backward runs, averaged and unpacked before the optimiser step (or, with
+  step(optimizer), packed on the device and applied by the optimiser straight from the reduced buckets).
 * RPNTargets: the RPN training targets of one image (rpn/assign_anchor.py:370-595 add_rpn_blobs / _get_rpn_blobs, run by
   the reference's data loaders on the host) on the device (csrc/rpn_target.cu), as the label dict coco.py:133-142 builds.
 * ProposalTargets: the Mask R-CNN proposal targets of one image (operators/modules/proposal_mask_target.py, run by the
@@ -25,10 +26,15 @@
   fcn_score inside the cross-entropy, so the [1,S,4h,4w] fcn_output (159 MB at 1024x2048, S 19), its log-softmax and
   its gradient are never built; RPNLoss covers the five FPN levels in one launch and reads the label fields in place;
   MaskRCNNLoss reads mask_score and mask_target once.
+* SGD, LRSchedule: the optimiser (lib/nn/optimizer.py:19-106) with the learning-rate schedule and momentum decay of
+  upsnet_end2end_train.py:76-103, 235-240, every parameter updated in one launch (csrc/sgd.cu), from p.grad or, through
+  FlatBucketAllReduce.step, straight from the all-reduced bf16 buckets; with a schedule attached the step issues kernels
+  only and can be replayed from a CUDA graph.  Unlike the reference, the step does not write g + wd p back into p.grad.
 
 Scope note: this is the operator / communication layer of the training configuration, the RPN and proposal targets,
-the label maps and every loss of the training forward.  fcn_roi_loss (train.fcn_with_roi_loss is off in every shipped
-configuration) and the optimiser are not built; the dense backward convolutions are library calls.
+the label maps, every loss of the training forward and the optimiser.  fcn_roi_loss (train.fcn_with_roi_loss is off in
+every shipped configuration), Adam and clip_grad (imported by the training script, never called) are not built; the
+dense backward convolutions are library calls.
 """
 import ctypes as C
 
@@ -36,6 +42,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 from torch.nn.modules.utils import _pair
+from torch.optim.optimizer import required
 
 from . import _lib
 from ._lib import call, f32c, query_bytes, require_cuda
@@ -229,6 +236,7 @@ class FlatBucketAllReduce:
         if cur:
             self.buckets.append(cur)
         self._flat, self._work = [None] * len(self.buckets), []
+        self._fused = None      # step(): (optimizer, world, bf16 buffers, apply tables, pack tables)
 
     def start(self):
         assert dist.is_available() and dist.is_initialized()
@@ -258,6 +266,294 @@ class FlatBucketAllReduce:
 
     def __call__(self):
         return self.start().finish()
+
+    def step(self, optimizer, lr=None):
+        """start(); finish(); optimizer.step(lr) without the passes in between: every bucket is packed on the device
+        (upsnet_sgd_pack) into a persistent bf16 buffer, its all_reduce starts asynchronously, and as each completes the
+        optimiser is applied straight from the reduced bucket (upsnet_sgd_apply, 1/world folded in).  The same bytes as
+        the three calls, except that p.grad is not written.  As after finish(), every parameter takes part (a None
+        gradient packs as zeros).  `lr` as optimizer.step takes it: a value, or None with a schedule attached.  The
+        bucket parameters must be exactly the optimiser's; bf16 buckets only."""
+        assert dist.is_available() and dist.is_initialized()
+        if not isinstance(optimizer, SGD):
+            raise _lib.UpsnetError("FlatBucketAllReduce.step: the optimiser must be upsnet_b200.SGD")
+        if self.dtype != torch.bfloat16:
+            raise _lib.UpsnetError("FlatBucketAllReduce.step: reduce_dtype must be torch.bfloat16")
+        if {id(p) for p in self.params} != {id(p) for p in optimizer._params} or len(self.params) != len(optimizer._params):
+            raise _lib.UpsnetError("FlatBucketAllReduce.step: the buckets' parameters are not the optimiser's")
+        lr = optimizer._check_lr(lr)
+        dev = optimizer._dev
+        for p in self.params:               # every parameter is updated, so every buffer exists after this step
+            optimizer._buffer(p, optimizer._group_of[p])
+        world = dist.get_world_size(self.group)
+        if self._fused is None or self._fused[0] is not optimizer or self._fused[1] != world:
+            flats = [torch.empty(sum(p.numel() for p in b), dtype=torch.bfloat16, device=dev) for b in self.buckets]
+            tables = [optimizer._bucket_table(b, f, world) for b, f in zip(self.buckets, flats)]
+            self._fused = (optimizer, world, flats, tables, [None] * len(self.buckets))
+        _, _, flats, tables, packs = self._fused
+        work = []
+        for bi, bucket in enumerate(self.buckets):
+            key = tuple(p.grad.data_ptr() if p.grad is not None else 0 for p in bucket)
+            if packs[bi] is None or packs[bi][0] != key:
+                packs[bi] = (key,) + _pack_table(bucket, flats[bi], dev)
+            call("sgd_pack", dev, packs[bi][1], packs[bi][2])
+            work.append(dist.all_reduce(flats[bi], op=dist.ReduceOp.SUM, group=self.group, async_op=True))
+        for bi in range(len(self.buckets)):
+            work[bi].wait()
+            optimizer._apply(tables[bi][0], tables[bi][1], lr)
+        optimizer._advance()
+        return self
+
+
+# ------------------------------------------------------------------------------------------------
+# optimiser (lib/nn/optimizer.py SGD + the learning-rate schedule and momentum decay of upsnet_end2end_train.py)
+# ------------------------------------------------------------------------------------------------
+_CHUNK = 8192       # UPSNET_SGD_CHUNK
+_MAX_GROUPS = 16    # UPSNET_SGD_MAX_GROUPS
+_GRAD_F32, _GRAD_BF16, _GRAD_NONE = 0, 1, 2
+_CHUNK_DT = np.dtype([("param", "<u8"), ("buf", "<u8"), ("grad", "<u8"), ("n", "<i4"), ("group", "<i4"),
+                      ("kind", "<i4"), ("inv_world", "<f4")])        # upsnet_sgd_chunk
+_PACK_DT = np.dtype([("grad", "<u8"), ("out", "<u8"), ("n", "<i4"), ("reserved", "<i4")])    # upsnet_sgd_pack_chunk
+
+
+def _upload_table(rows, dtype, dev):
+    a = np.zeros(len(rows), dtype)
+    for i, r in enumerate(rows):
+        a[i] = r
+    return torch.from_numpy(a.view(np.uint8)).to(dev), len(rows)
+
+
+def _pack_table(bucket, flat, dev):
+    """(device table, entries) of upsnet_sgd_pack for one bucket: each gradient's chunks at its offset in `flat`."""
+    rows, off = [], 0
+    for p in bucket:
+        g = p.grad
+        if g is not None:
+            if g.dtype != torch.float32 or g.device != flat.device or not g.is_contiguous():
+                raise _lib.UpsnetError("FlatBucketAllReduce.step: gradients must be contiguous float32 on the device")
+        for s in range(0, p.numel(), _CHUNK):
+            n = min(_CHUNK, p.numel() - s)
+            rows.append((0 if g is None else g.data_ptr() + 4 * s, flat.data_ptr() + 2 * (off + s), n, 0))
+        off += p.numel()
+    return _upload_table(rows, _PACK_DT, dev)
+
+
+class LRSchedule:
+    """The learning rate of iteration `it`, adjust_learning_rate / lr_factor / lr_poly of upsnet_end2end_train.py:76-103
+    restated with the same Python float operations (bit-identical values):
+      'step': base_lr * (0.1 ** number of decay iterations <= it), after a warm-up from base_lr / 10 that is linear in
+              it / warmup_iteration;
+      'poly': base_lr * (1 - it / max_iteration) ** 0.9, during warm-up the smaller of that and the linear warm-up.
+    Built from the reference's `config` (train.lr_schedule, lr, max_iteration, decay_iteration, warmup_iteration,
+    begin_iteration) or from the same values as keywords.  table() is the float64 table of [begin_iteration,
+    max_iteration) and decay_flags() marks the iterations i after which the training loop decays the momentum buffers
+    (i + 1 in decay_iteration, whatever the schedule); SGD.attach_schedule uploads both."""
+
+    def __init__(self, config=None, *, lr_schedule="step", base_lr=None, max_iteration=None, decay_iteration=(),
+                 warmup_iteration=0, begin_iteration=0):
+        if config is not None:
+            tr = config.train
+            lr_schedule, base_lr, max_iteration = tr.lr_schedule, tr.lr, tr.max_iteration
+            decay_iteration, warmup_iteration = tr.decay_iteration, tr.warmup_iteration
+            begin_iteration = getattr(tr, "begin_iteration", 0)
+        if lr_schedule not in ("step", "poly"):
+            raise _lib.UpsnetError("LRSchedule: lr_schedule must be 'step' or 'poly', not %r" % (lr_schedule,))
+        if base_lr is None or max_iteration is None:
+            raise _lib.UpsnetError("LRSchedule: base_lr and max_iteration are required")
+        self.lr_schedule, self.base_lr, self.max_iteration = lr_schedule, base_lr, int(max_iteration)
+        self.decay_iteration = list(decay_iteration)
+        self.warmup_iteration, self.begin_iteration = warmup_iteration, int(begin_iteration)
+        if not 0 <= self.begin_iteration < self.max_iteration:
+            raise _lib.UpsnetError("LRSchedule: begin_iteration must be in [0, max_iteration)")
+
+    def _warmup(self, it):
+        alpha = it / self.warmup_iteration
+        return self.base_lr * (1 / 10.0 * (1 - alpha) + alpha)
+
+    def __call__(self, it):
+        if self.lr_schedule == "step":
+            if it < self.warmup_iteration:
+                return self._warmup(it)
+            idx = len(self.decay_iteration)
+            for i, d in enumerate(self.decay_iteration):
+                if it < d:
+                    idx = i
+                    break
+            return self.base_lr * (0.1 ** idx)
+        poly = self.base_lr * ((1 - float(it) / self.max_iteration) ** (0.9))
+        if it < self.warmup_iteration:
+            return min(self._warmup(it), poly)
+        return poly
+
+    def table(self):
+        return np.array([self(i) for i in range(self.begin_iteration, self.max_iteration)], np.float64)
+
+    def decay_flags(self):
+        decay = set(self.decay_iteration)
+        return np.array([(i + 1) in decay for i in range(self.begin_iteration, self.max_iteration)], np.uint8)
+
+
+class SGD(torch.optim.Optimizer):
+    """Drop-in for lib.nn.optimizer.SGD (momentum SGD with per-group learning-rate multipliers: the reference passes
+    lr=1 and get_params_lr()'s groups, 'lr' 1 or 2 and an optional 'weight_decay'), every parameter updated in one
+    launch (upsnet_sgd_apply; the rounding of each element is in include/upsnet_b200.h).
+
+    * step(lr) has the reference's signature.  A parameter whose p.grad is None is skipped entirely.  With momentum 0
+      the reference applies p -= g + wd p and ignores lr; so does this.
+    * The momentum buffers live in one flat float32 allocation (each segment 16-byte aligned); state[p]['momentum_buffer']
+      is a view of it, created the first time p has a gradient, so state_dict() aliases the buffers and the reference's
+      decay loop (optimizer.state_dict()['state'][k]['momentum_buffer'].div_(10)) acts on them.  state_dict() /
+      load_state_dict() use the reference's format; load_state_dict copies into the flat buffer.
+    * attach_schedule(LRSchedule) and step() with no argument: the learning rate and the momentum decay come from device
+      tables at a device iteration counter, which the step advances; such a step issues kernels only and can be captured
+      in a CUDA graph (after one eager step, which uploads the chunk table).
+    * Unlike the reference, p.grad is not written: the reference leaves g + wd p in it, which nothing reads.
+    * zero_grad() zeroes gradients in place (set_to_none=False, the reference's torch behaviour), so their pointers and
+      the cached chunk table stay valid.  dampening != 0 raises, as the reference asserts; nesterov is not built.
+    float32 CUDA parameters on one device only."""
+
+    def __init__(self, params, lr=required, momentum=0, dampening=0, weight_decay=0,
+                 nesterov=False):
+        if nesterov:
+            raise _lib.UpsnetError("SGD: nesterov momentum is not built")
+        if dampening != 0:
+            raise _lib.UpsnetError("SGD: dampening is not implemented (the reference asserts dampening == 0)")
+        super().__init__(params, dict(lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay,
+                                      nesterov=nesterov))
+        if any(g["nesterov"] for g in self.param_groups):
+            raise _lib.UpsnetError("SGD: nesterov momentum is not built")
+        if any(g["dampening"] != 0 for g in self.param_groups):
+            raise _lib.UpsnetError("SGD: dampening is not implemented (the reference asserts dampening == 0)")
+        if len(self.param_groups) > _MAX_GROUPS:
+            raise _lib.UpsnetError("SGD: at most %d parameter groups" % _MAX_GROUPS)
+        self._params = [p for g in self.param_groups for p in g["params"]]
+        if not self._params:
+            raise _lib.UpsnetError("SGD: no parameters")
+        for p in self._params:
+            if not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous():
+                raise _lib.UpsnetError("SGD: parameters must be contiguous float32 CUDA tensors, not %s %s"
+                                       % (p.dtype, p.device))
+        self._dev = self._params[0].device
+        if any(p.device != self._dev for p in self._params):
+            raise _lib.UpsnetError("SGD: every parameter must be on one device")
+        offs, n = [], 0
+        for p in self._params:
+            offs.append(n)
+            n += (p.numel() + 3) // 4 * 4
+        self._flat = torch.zeros(max(n, 4), dtype=torch.float32, device=self._dev)
+        self._views = {p: self._flat[o:o + p.numel()].view_as(p) for p, o in zip(self._params, offs)}
+        self._group_of = {p: gi for gi, g in enumerate(self.param_groups) for p in g["params"]}
+        self._table_key, self._table = None, None
+        self._sched = None
+
+    # -- the reference's interface --------------------------------------------------------------
+    def zero_grad(self, set_to_none=False):
+        super().zero_grad(set_to_none=set_to_none)
+
+    def step(self, lr=None, closure=None):
+        loss = closure() if closure is not None else None
+        lr = self._check_lr(lr)
+        key = tuple(p.grad.data_ptr() if p.grad is not None else 0 for p in self._params)
+        if key != self._table_key:
+            self._table, self._table_key = self._grad_table(), key
+        self._apply(self._table[0], self._table[1], lr)
+        self._advance()
+        return loss
+
+    def load_state_dict(self, state_dict):
+        super().load_state_dict(state_dict)
+        loaded = {p: s["momentum_buffer"] for p, s in self.state.items() if "momentum_buffer" in s}
+        self._flat.zero_()
+        for p, v in self._views.items():
+            if p in loaded:
+                v.copy_(loaded[p])
+                self.state[p]["momentum_buffer"] = v
+        self._table_key = None
+
+    # -- schedule ----------------------------------------------------------------------------------
+    def attach_schedule(self, schedule):
+        """Learning rate and momentum decay from `schedule` (an LRSchedule) on the device; the device iteration counter
+        starts at schedule.begin_iteration.  step() then takes no argument."""
+        if not isinstance(schedule, LRSchedule):
+            raise _lib.UpsnetError("SGD.attach_schedule: an LRSchedule is required")
+        self._sched = (schedule, torch.from_numpy(schedule.table()).to(self._dev),
+                       torch.from_numpy(schedule.decay_flags()).to(self._dev),
+                       torch.full((1,), schedule.begin_iteration, dtype=torch.int32, device=self._dev))
+
+    @property
+    def iteration(self):
+        """The device iteration counter of the attached schedule (reads the device)."""
+        return None if self._sched is None else int(self._sched[3].item())
+
+    # -- internals ---------------------------------------------------------------------------------
+    def _check_lr(self, lr):
+        if self._sched is not None and lr is not None:
+            raise _lib.UpsnetError("SGD.step: a schedule is attached; call step() without a learning rate")
+        if self._sched is None and lr is None:
+            raise _lib.UpsnetError("SGD.step: a learning rate is required (or attach_schedule first)")
+        return None if lr is None else float(lr)
+
+    def _buffer(self, p, gi):
+        """The flat-buffer address of p's momentum buffer, created (as +0) on its first use; 0 without momentum."""
+        if self.param_groups[gi]["momentum"] == 0:
+            return 0
+        st = self.state[p]
+        if "momentum_buffer" not in st:
+            self._views[p].zero_()
+            st["momentum_buffer"] = self._views[p]
+        return self._views[p].data_ptr()
+
+    def _grad_table(self):
+        rows = []
+        for p in self._params:
+            gi = self._group_of[p]
+            g = p.grad
+            if g is None:
+                if p in self.state and "momentum_buffer" in self.state[p]:
+                    kind, gp = _GRAD_NONE, 0
+                else:
+                    continue
+            else:
+                if g.dtype != torch.float32 or g.device != self._dev or not g.is_contiguous():
+                    raise _lib.UpsnetError("SGD.step: gradients must be contiguous float32 on the parameters' device")
+                kind, gp = _GRAD_F32, g.data_ptr()
+            bp = self._buffer(p, gi)
+            rows += self._rows(p, bp, gp, 4, gi, kind, 1.0)
+        return _upload_table(rows, _CHUNK_DT, self._dev)
+
+    def _bucket_table(self, bucket, flat, world):
+        """The chunk table of one bf16 bucket (FlatBucketAllReduce.step): every parameter, gradient = its segment."""
+        rows, off = [], 0
+        inv = float(np.float32(1.0) / np.float32(world))
+        for p in bucket:
+            gi = self._group_of[p]
+            rows += self._rows(p, self._buffer(p, gi), flat.data_ptr() + 2 * off, 2, gi, _GRAD_BF16, inv)
+            off += p.numel()
+        return _upload_table(rows, _CHUNK_DT, self._dev)
+
+    @staticmethod
+    def _rows(p, bp, gp, gsize, gi, kind, inv):
+        rows = []
+        for s in range(0, p.numel(), _CHUNK):
+            rows.append((p.data_ptr() + 4 * s, bp + 4 * s if bp else 0, gp + gsize * s if gp else 0,
+                         min(_CHUNK, p.numel() - s), gi, kind, inv))
+        return rows
+
+    def _apply(self, table, n, lr):
+        groups = self.param_groups
+        glr = (C.c_double * len(groups))(*[float(g["lr"]) for g in groups])
+        wd = (C.c_float * len(groups))(*[float(g["weight_decay"]) for g in groups])
+        mom = (C.c_float * len(groups))(*[float(g["momentum"]) for g in groups])
+        if self._sched is None:
+            call("sgd_apply", self._dev, table, n, len(groups), glr, wd, mom, lr, None, None, None, 0, 0)
+        else:
+            sch, lrt, dec, it = self._sched
+            call("sgd_apply", self._dev, table, n, len(groups), glr, wd, mom, 0.0, lrt, dec, it, sch.begin_iteration,
+                 lrt.numel())
+
+    def _advance(self):
+        if self._sched is not None:
+            call("sgd_advance", self._dev, self._sched[3])
 
 
 # ------------------------------------------------------------------------------------------------
