@@ -17,6 +17,7 @@
 #include <cub/device/device_radix_sort.cuh>
 
 #include "common.cuh"
+#include "cta.cuh"
 
 namespace ups {
 
@@ -60,27 +61,20 @@ struct CocoSmem {
 };
 static_assert(sizeof(CocoSmem) <= 227 * 1024, "one category's state fits in shared memory");
 
-// Appends the indices i < n with pred(i) to out[] in ascending order (a block-wide ballot scan); returns the count
-// (every thread gets it).  `cap` bounds the writes; the returned count is not clamped.
+// Appends the indices i < n with pred(i) to out[] in ascending order; returns the count (every thread gets it), with
+// out[] complete for every thread.  `cap` bounds the writes; the returned count is not clamped.
 template <typename Pred>
 __device__ int block_compact(int n, int* out, int cap, int* warp_n, Pred pred) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int total = 0;
   for (int base = 0; base < n; base += kCocoThreads) {
     const int i = base + threadIdx.x;
     const bool f = i < n && pred(i);
-    const unsigned bal = __ballot_sync(0xffffffffu, f);
-    if (lane == 0) warp_n[warp] = __popc(bal);
-    __syncthreads();
-    int off = total;
-    for (int w = 0; w < warp; ++w) off += warp_n[w];
-    off += __popc(bal & ((1u << lane) - 1u));
+    int chunk;
+    const int off = total + cta_ballot_rank<kCocoThreads>(f, warp_n, &chunk);
     if (f && off < cap) out[off] = i;
-    int sum = 0;
-    for (int w = 0; w < kCocoThreads / 32; ++w) sum += warp_n[w];
-    total += sum;
-    __syncthreads();
+    total += chunk;
   }
+  __syncthreads();   // out[] is complete
   return total;
 }
 
@@ -329,8 +323,7 @@ coco_image_kernel(const __grid_constant__ CocoImageArgs p) {
 // ---- accumulate ----
 
 __device__ __forceinline__ unsigned long long coco_sort_key(const upsnet_coco_record& r, const int* image_rank) {
-  unsigned u = __float_as_uint(r.score + 0.0f);                 // -0 -> +0: the two compare equal in numpy
-  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);               // ascending float order as unsigned
+  const unsigned u = orderable(r.score + 0.0f);                 // -0 -> +0: the two compare equal in numpy
   return ((unsigned long long)(unsigned)r.category << 56) | ((unsigned long long)(~u) << 24) |
          ((unsigned long long)(unsigned)image_rank[r.image] << 7) | (unsigned long long)(unsigned)r.rank;
 }

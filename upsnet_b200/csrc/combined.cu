@@ -17,6 +17,7 @@
 #include <cub/block/block_scan.cuh>
 
 #include "common.cuh"
+#include "cta.cuh"
 
 namespace ups {
 
@@ -103,9 +104,8 @@ __device__ void combined_decide(const CombinedArgs& p, CbSmem& s) {
     const long long c = p.cls[d];
     const float sc = p.scores[d];
     if (c < 1 || c >= p.num_classes || sc < p.score_thr) continue;
-    unsigned u = __float_as_uint(sc + 0.0f);              // -0 -> +0; one NaN (numpy sorts every NaN last)
-    if (sc != sc) u = 0x7fc00000u;
-    u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);      // ascending float order as unsigned
+    // -0 -> +0; one NaN (numpy sorts every NaN last)
+    const unsigned u = orderable(sc != sc ? __uint_as_float(0x7fc00000u) : sc + 0.0f);
     s.key[atomicAdd(&s.nv, 1)] = ((unsigned long long)u << 32) | ((unsigned long long)c << 11) | (unsigned long long)d;
   }
   __syncthreads();

@@ -13,6 +13,7 @@
 
 #include "anchors.cuh"
 #include "common.cuh"
+#include "cta.cuh"
 
 namespace ups {
 
@@ -107,18 +108,7 @@ maskroi_prepare_kernel(const float* __restrict__ rois, const uint8_t* __restrict
   while (sortN < s_ncand) sortN <<= 1;
   for (int i = s_ncand + tid; i < sortN; i += kMrThreads) keys[i] = ~0ull;
   __syncthreads();
-  // bitonic sort, ascending, over the next power of two >= the candidate count
-  for (int k = 2; k <= sortN; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int t = tid; t < sortN / 2; t += kMrThreads) {
-        const int lo = ((t / j) * (j << 1)) + (t % j), hi = lo + j;
-        const unsigned long long a = keys[lo], b = keys[hi];
-        const bool up = (lo & k) == 0;
-        if ((a > b) == up) { keys[lo] = b; keys[hi] = a; }
-      }
-      __syncthreads();
-    }
-  }
+  cta_bitonic_sort<kMrThreads, false>(keys, sortN);   // ascending, over the next power of two >= the candidate count
   if (tid == 0) {
     int acc = 0;
     for (int s = 0; s < nseg; ++s) { offs_out[s] = acc; acc += seg_cnt[s]; }
@@ -152,38 +142,6 @@ maskroi_prepare_kernel(const float* __restrict__ rois, const uint8_t* __restrict
 // ----------------------------------------------------------------------------------------------
 constexpr int kAllCap = 4096;
 
-__device__ __forceinline__ unsigned orderable(float f) {
-  const unsigned u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
-// exclusive block scan of one int per thread (1024 threads); returns the prefix, total in *total
-__device__ __forceinline__ int block_scan_excl(int v, int* warp_sums, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp_sums[wid] = x;
-  __syncthreads();
-  if (wid == 0) {
-    int w = warp_sums[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += y;
-    }
-    warp_sums[lane] = w;   // inclusive
-  }
-  __syncthreads();
-  const int base = wid ? warp_sums[wid - 1] : 0;
-  *total = warp_sums[31];
-  __syncthreads();
-  return base + x - v;
-}
-
 __global__ void __launch_bounds__(kMrThreads, 1)
 maskroi_finish_kernel(const int* __restrict__ keep, const int* __restrict__ cnt, const int* __restrict__ offs,
                       const float* __restrict__ sc, const int* __restrict__ cls, const float* __restrict__ bx, int nseg,
@@ -192,10 +150,7 @@ maskroi_finish_kernel(const int* __restrict__ keep, const int* __restrict__ cnt,
   __shared__ int gidx[kAllCap];
   __shared__ unsigned key[kAllCap];
   __shared__ int seg_base[130];
-  __shared__ int hist[256];
-  __shared__ int warp_sums[32];
-  __shared__ unsigned sel_prefix;
-  __shared__ int sel_k;
+  __shared__ int warp_sums[kMrThreads / 32];
   const int tid = threadIdx.x;
   const int all_cap = min(nseg * M, kAllCap);
   if (tid == 0) {
@@ -218,32 +173,9 @@ maskroi_finish_kernel(const int* __restrict__ keep, const int* __restrict__ cnt,
   __syncthreads();
   // k-th largest score (mask_roi.py:106-121): 4-pass radix select over the order-preserving keys
   const int K = min(top_n, all_cap);
-  unsigned kth = 0u;            // keep everything
-  if (top_n > 0 && nk >= K) {
-    if (tid == 0) { sel_prefix = 0u; sel_k = K; }
-    __syncthreads();
-    for (int pass = 0; pass < 4; ++pass) {
-      const int shift = 24 - 8 * pass;
-      const unsigned pmask = pass == 0 ? 0u : (0xffffffffu << (shift + 8));
-      for (int b = tid; b < 256; b += kMrThreads) hist[b] = 0;
-      __syncthreads();
-      const unsigned pref = sel_prefix;
-      for (int i = tid; i < nk; i += kMrThreads)
-        if ((key[i] & pmask) == pref) atomicAdd(&hist[(key[i] >> shift) & 255u], 1);
-      __syncthreads();
-      if (tid == 0) {
-        int need = sel_k, b = 255;
-        for (; b > 0; --b) {
-          if (hist[b] >= need) break;
-          need -= hist[b];
-        }
-        sel_k = need;
-        sel_prefix = pref | ((unsigned)b << shift);
-      }
-      __syncthreads();
-    }
-    kth = sel_prefix;
-  }
+  const unsigned kth = (top_n > 0 && nk >= K)
+                           ? cta_radix_select<kMrThreads, unsigned, 32, 8, true>([&](int i) { return key[i]; }, nk, K)
+                           : 0u;      // keep everything
   // ordered compaction of {score >= kth} into the output slots
   constexpr int PER = kAllCap / kMrThreads;
   int flags[PER], mine = 0;
@@ -253,8 +185,8 @@ maskroi_finish_kernel(const int* __restrict__ keep, const int* __restrict__ cnt,
     flags[e] = (i < nk && key[i] >= kth) ? 1 : 0;
     mine += flags[e];
   }
-  int total = 0;
-  int dst = block_scan_excl(mine, warp_sums, &total);
+  int total;
+  int dst = cta_scan_excl<kMrThreads>(mine, warp_sums, &total);
   const int n_sel = min(total, cap);
 #pragma unroll
   for (int e = 0; e < PER; ++e) {
@@ -393,7 +325,6 @@ topk_pass_kernel(const TopkParams p, int shift, int bits, int first) {
   if ((int)blockIdx.x >= lv.blocks) return;
   if (!first && p.done[l]) return;      // an earlier pass already narrowed the candidates to what the sort kernel can take
   __shared__ unsigned int sh[kTkBins];
-  __shared__ int s_last;
   for (int b = threadIdx.x; b < kTkBins; b += kTkThreads) sh[b] = 0;
   __syncthreads();
   const unsigned long long fixed = first ? 0ull : p.prefix[l];
@@ -419,45 +350,19 @@ topk_pass_kernel(const TopkParams p, int shift, int bits, int first) {
   unsigned int* gh = p.hist + (size_t)l * kTkBins;
   for (int b = threadIdx.x; b < kTkBins; b += kTkThreads)
     if (sh[b]) atomicAdd(&gh[b], sh[b]);
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(&p.ticket[l], 1u) == (unsigned int)(lv.blocks - 1)) ? 1 : 0;
-  __syncthreads();
-  if (!s_last) return;
+  if (!last_cta(&p.ticket[l], (unsigned)lv.blocks)) return;
   // ---- last CTA of this level: find the digit that contains the need-th largest key ----
-  __threadfence();
   for (int b = threadIdx.x; b < kTkBins; b += kTkThreads) { sh[b] = __ldcg(&gh[b]); gh[b] = 0; }
   __syncthreads();
-  if (threadIdx.x < 32) {
-    // warp scan from the top bin downwards, 64 bins per lane
-    const int lane = threadIdx.x;
-    const int need = first ? lv.k : p.need[l];
-    const int per = kTkBins / 32;
-    unsigned int mine = 0;
-    for (int b = 0; b < per; ++b) mine += sh[kTkBins - 1 - (lane * per + b)];
-    unsigned int incl = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned int y = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += y;
-    }
-    const unsigned int excl = incl - mine;
-    const bool here = excl < (unsigned int)need && incl >= (unsigned int)need;
-    if (here) {
-      unsigned int acc = excl;
-      int d = 0;
-      for (int b = 0; b < per; ++b) {
-        const int bin = kTkBins - 1 - (lane * per + b);
-        if (acc + sh[bin] >= (unsigned int)need) { d = bin; break; }
-        acc += sh[bin];
-      }
-      p.need[l] = need - (int)acc;
-      p.prefix[l] = fixed | ((unsigned long long)d << shift);
-      // early exit: everything above the bucket (k - need') plus the WHOLE bucket fits the sort buffer -> no need to
-      // resolve the remaining digits, the sort orders the bucket and the first k are taken
-      if ((long long)(lv.k - (need - (int)acc)) + (long long)sh[d] <= (long long)kTkMaxK) p.done[l] = 1;
-    }
-    if (lane == 0) { p.ticket[l] = 0; p.fill[l] = 0; }
+  RadixDigit d;
+  if (threadIdx.x < 32 && warp_radix_digit<kTkBins, true>(sh, first ? lv.k : p.need[l], &d)) {
+    p.need[l] = d.need;
+    p.prefix[l] = fixed | ((unsigned long long)d.digit << shift);
+    // early exit: everything above the bucket (k - need') plus the WHOLE bucket fits the sort buffer -> no need to
+    // resolve the remaining digits, the sort orders the bucket and the first k are taken
+    if ((long long)(lv.k - d.need) + (long long)sh[d.digit] <= (long long)kTkMaxK) p.done[l] = 1;
+    p.ticket[l] = 0;
+    p.fill[l] = 0;
   }
 }
 
@@ -489,20 +394,10 @@ topk_sort_kernel(const TopkParams p) {
   const int nk = min((int)p.fill[l], kTkMaxK);       // == k unless a pass exited early with a whole bucket
   for (int i = tid; i < kTkMaxK; i += 1024) sk[i] = i < nk ? p.keys[(size_t)l * kTkMaxK + i] : 0ull;
   __syncthreads();
-  for (int k = 2; k <= kTkMaxK; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      const int t = tid;   // kTkMaxK / 2 == 1024 pairs
-      const int lo = ((t / j) * (j << 1)) + (t % j), hi = lo + j;
-      const unsigned long long a = sk[lo], b = sk[hi];
-      const bool desc = (lo & k) == 0;
-      if ((a < b) == desc) { sk[lo] = b; sk[hi] = a; }
-      __syncthreads();
-    }
+  cta_bitonic_sort<1024, true>(sk, kTkMaxK);
   for (int i = tid; i < lv.k; i += 1024) {
     const unsigned long long key = sk[i];
-    const unsigned int o = (unsigned int)(key >> kTkIdxBits);
-    const unsigned int u = (o & 0x80000000u) ? (o & 0x7fffffffu) : ~o;   // inverse of orderable()
-    p.out_scores[lv.out_start + i] = __uint_as_float(u);
+    p.out_scores[lv.out_start + i] = from_orderable((unsigned int)(key >> kTkIdxBits));
     p.out_idx[lv.out_start + i] = (long long)((1u << kTkIdxBits) - 1u - (unsigned int)(key & ((1u << kTkIdxBits) - 1u)));
   }
 }
@@ -577,7 +472,7 @@ extern "C" int upsnet_rpn_topk(const float* const* probs, const int* hs, const i
 // ----------------------------------------------------------------------------------------------
 namespace ups {
 
-constexpr int kColMaxCand = 8192, kColMaxPost = 2048, kColBins = 4096;
+constexpr int kColMaxCand = 8192, kColMaxPost = 2048;
 
 __global__ void __launch_bounds__(1024, 1)
 rpn_collect_kernel(const int* __restrict__ keep, const int* __restrict__ cnt, const int* __restrict__ offs,
@@ -585,10 +480,8 @@ rpn_collect_kernel(const int* __restrict__ keep, const int* __restrict__ cnt, co
                    float* __restrict__ rois, float* __restrict__ out_scores, unsigned char* __restrict__ ok) {
   extern __shared__ unsigned long long ck[];            // [kColMaxCand] candidate keys, then [kColMaxPost] selected
   unsigned long long* sel = ck + kColMaxCand;
-  __shared__ unsigned int hist[kColBins];
   __shared__ int seg_base[kMaxLevels + 1];
-  __shared__ unsigned long long s_prefix;
-  __shared__ int s_need, s_nsel;
+  __shared__ int s_nsel;
   const int tid = threadIdx.x;
   if (tid == 0) {
     int acc = 0;
@@ -606,46 +499,8 @@ rpn_collect_kernel(const int* __restrict__ keep, const int* __restrict__ cnt, co
     }
   }
   __syncthreads();
-  unsigned long long kth = 0ull;
-  if (C > post) {
-    if (tid == 0) { s_prefix = 0ull; s_need = post; }
-    __syncthreads();
-    for (int pass = 0; pass < 4; ++pass) {
-      const int shift = 36 - 12 * pass;       // digits [36,48) [24,36) [12,24) [0,12) of the 45-bit key
-      const unsigned long long mask_hi = pass == 0 ? 0ull : (~0ull << (shift + 12));
-      for (int b = tid; b < kColBins; b += 1024) hist[b] = 0;
-      __syncthreads();
-      const unsigned long long pref = s_prefix;
-      for (int i = tid; i < C; i += 1024)
-        if ((ck[i] & mask_hi) == pref) atomicAdd(&hist[(unsigned int)(ck[i] >> shift) & (kColBins - 1)], 1u);
-      __syncthreads();
-      if (tid < 32) {
-        const int need = s_need, per = kColBins / 32;
-        unsigned int mine = 0;
-        for (int b = 0; b < per; ++b) mine += hist[kColBins - 1 - (tid * per + b)];
-        unsigned int incl = mine;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const unsigned int y = __shfl_up_sync(0xffffffffu, incl, o);
-          if (tid >= o) incl += y;
-        }
-        const unsigned int excl = incl - mine;
-        if (excl < (unsigned int)need && incl >= (unsigned int)need) {
-          unsigned int acc = excl;
-          int d = 0;
-          for (int b = 0; b < per; ++b) {
-            const int bin = kColBins - 1 - (tid * per + b);
-            if (acc + hist[bin] >= (unsigned int)need) { d = bin; break; }
-            acc += hist[bin];
-          }
-          s_need = need - (int)acc;
-          s_prefix = pref | ((unsigned long long)d << shift);
-        }
-      }
-      __syncthreads();
-    }
-    kth = s_prefix;
-  }
+  const unsigned long long kth =
+      C > post ? cta_radix_select<1024, unsigned long long, 45, 12, true>([&](int i) { return ck[i]; }, C, post) : 0ull;
   // selected keys (all distinct): exactly min(C, post) of them; order fixed by the sort below
   for (int i = tid; i < C; i += 1024)
     if (ck[i] >= kth) {
@@ -658,16 +513,7 @@ rpn_collect_kernel(const int* __restrict__ keep, const int* __restrict__ cnt, co
   while (sortN < nsel) sortN <<= 1;
   for (int i = nsel + tid; i < sortN; i += 1024) sel[i] = 0ull;
   __syncthreads();
-  for (int k = 2; k <= sortN; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int t = tid; t < sortN / 2; t += 1024) {
-        const int lo = ((t / j) * (j << 1)) + (t % j), hi = lo + j;
-        const unsigned long long a = sel[lo], b = sel[hi];
-        const bool desc = (lo & k) == 0;
-        if ((a < b) == desc) { sel[lo] = b; sel[hi] = a; }
-      }
-      __syncthreads();
-    }
+  cta_bitonic_sort<1024, true>(sel, sortN);
   for (int i = tid; i < post; i += 1024) {
     float4 bx = make_float4(0.f, 0.f, 0.f, 0.f);
     float sc = 0.f;
@@ -728,7 +574,7 @@ mask_rows_kernel(const float* __restrict__ b1, const int* __restrict__ n1p, int 
                  int* __restrict__ pan_row) {
   __shared__ int s_cnt[kRowThreads / 32];
   const int n1 = min(max(*n1p, 0), cap1), n2 = min(max(*n2p, 0), cap2);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const uint32_t* d = reinterpret_cast<const uint32_t*>(b1);
   for (int k = tid; k < n1 * 5; k += kRowThreads) rows[k] = b1[k];
   int base = n1;
@@ -746,22 +592,14 @@ mask_rows_kernel(const float* __restrict__ b1, const int* __restrict__ n1p, int 
       }
       fresh = src < 0;
     }
-    const unsigned bal = __ballot_sync(0xffffffffu, fresh);
-    if (lane == 0) s_cnt[warp] = __popc(bal);
-    __syncthreads();
-    int off = base, tot = 0;
-#pragma unroll
-    for (int w = 0; w < kRowThreads / 32; ++w) {
-      if (w < warp) off += s_cnt[w];
-      tot += s_cnt[w];
-    }
+    int tot;
+    const int rank = cta_ballot_rank<kRowThreads>(fresh, s_cnt, &tot);
     if (fresh) {
-      src = off + __popc(bal & ((1u << lane) - 1u));
+      src = base + rank;
       for (int k = 0; k < 5; ++k) rows[(size_t)src * 5 + k] = b2[(size_t)j * 5 + k];
     }
     if (j < cap2) pan_row[j] = src;
     base += tot;
-    __syncthreads();      // s_cnt is rewritten by the next chunk
   }
   for (int k = base * 5 + tid; k < (cap1 + cap2) * 5; k += kRowThreads) rows[k] = 0.f;
   if (tid == 0) *u_out = base;

@@ -22,6 +22,7 @@
 // oracle-of-record formula (oracle/upsnet_oracle.c resized_logit) in un-fused fp32 (_rn
 // intrinsics) so label maps are bit-exact.
 #include "common.cuh"
+#include "cta.cuh"
 #include "up4.cuh"
 
 namespace ups {
@@ -121,16 +122,18 @@ __device__ __forceinline__ float blend(const float* __restrict__ S, int sx, floa
 }
 
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024)
+constexpr int kPrepThreads = 1024;
+
+__global__ void __launch_bounds__(kPrepThreads)
 pan_prep_kernel(const float* __restrict__ boxes, const float* __restrict__ prob,
                 const int64_t* __restrict__ cls_idx, int n_max, const int* __restrict__ n_dev, int H, int W,
                 PanWorkspace ws) {
   const int n = n_dev ? max(min(*n_dev, n_max), 1) : n_max;   // device-side instance count (static-shape engine)
   if (threadIdx.x == 0) ws.meta[2] = n;
   __shared__ float s_prob[kMaxList];            // n <= kMaxList (checked by the entry point): the rank loop reads shared memory
-  for (int i = threadIdx.x; i < n; i += blockDim.x) s_prob[i] = prob[i];
+  for (int i = threadIdx.x; i < n; i += kPrepThreads) s_prob[i] = prob[i];
   __syncthreads();
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+  for (int i = threadIdx.x; i < n; i += kPrepThreads) {
     const float p = s_prob[i];
     int rank = 0;
     for (int j = 0; j < n; ++j) {
@@ -156,13 +159,11 @@ pan_prep_kernel(const float* __restrict__ boxes, const float* __restrict__ prob,
     ws.g.cls[i] = c;
   }
   // ---- bit-window sizes by rank -> exclusive scan -> word offsets and round boundaries ----
-  __shared__ long long s_warp[32];
-  __shared__ long long s_carry;
-  if (threadIdx.x == 0) s_carry = 0;
-  for (int q = threadIdx.x; q <= kMaxRounds; q += blockDim.x) ws.round_lo[q] = n;
+  __shared__ long long warp_sums[kPrepThreads / 32];
+  long long carry = 0;
+  for (int q = threadIdx.x; q <= kMaxRounds; q += kPrepThreads) ws.round_lo[q] = n;
   __syncthreads();   // order[] and the geometry are complete
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int base = 0; base < n; base += blockDim.x) {
+  for (int base = 0; base < n; base += kPrepThreads) {
     const int r = base + threadIdx.x;
     long long sz = 0;
     if (r < n) {
@@ -170,35 +171,17 @@ pan_prep_kernel(const float* __restrict__ boxes, const float* __restrict__ prob,
       const int x0 = ws.g.gx0[i], x1 = ws.g.gx1[i], y0 = ws.g.gy0[i], y1 = ws.g.gy1[i];
       sz = (long long)max(((x1 + 31) >> 5) - (x0 >> 5), 0) * max(y1 - y0, 0);
     }
-    long long x = sz;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const long long y = __shfl_up_sync(0xffffffffu, x, o);
-      if (lane >= o) x += y;
-    }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-      long long w = s_warp[lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const long long y = __shfl_up_sync(0xffffffffu, w, o);
-        if (lane >= o) w += y;
-      }
-      s_warp[lane] = w;
-    }
-    __syncthreads();
-    const long long start = s_carry + (warp ? s_warp[warp - 1] : 0) + x - sz;
+    long long tot;
+    const long long excl = cta_scan_excl<kPrepThreads>(sz, warp_sums, &tot);
     if (r < n) {
-      ws.off[r] = start;
+      ws.off[r] = carry + excl;
       ws.msum[r] = 0;
     }
-    __syncthreads();
-    if (threadIdx.x == blockDim.x - 1) s_carry += s_warp[31];
-    __syncthreads();
+    carry += tot;
   }
+  __syncthreads();   // off[] is complete
   // round boundaries: rank r opens round q when it is the first rank whose start offset falls in [q*budget, ...)
-  for (int r = threadIdx.x; r < n; r += blockDim.x) {
+  for (int r = threadIdx.x; r < n; r += kPrepThreads) {
     const int rq = (int)(ws.off[r] / ws.budget);
     if (r == 0 || (int)(ws.off[r - 1] / ws.budget) != rq) ws.round_lo[rq] = r;
   }
@@ -275,42 +258,33 @@ pan_bits_kernel(const float* __restrict__ mask_logit, int n_max, const int* __re
 // kept instances of the SAME class, so classes run concurrently and each CTA walks its class's instances of the
 // round in score order: |mask & occupied| by popc over the precomputed window words, the float64 ratio test
 // (mask_removal.py:82), occupied |= mask for the kept ones.
-__global__ void __launch_bounds__(1024)
+constexpr int kDecideThreads = 1024;
+
+__global__ void __launch_bounds__(kDecideThreads)
 pan_decide_kernel(int n_max, const int* __restrict__ n_dev, int H, int W, double fraction_threshold, int rq,
                   PanWorkspace ws) {
   const int n = n_dev ? max(min(*n_dev, n_max), 1) : n_max;
   __shared__ unsigned short list[kMaxList];   // ranks (score order) of this class's instances in this round
-  __shared__ int s_cnt;
   __shared__ int s_warp_cnt[32];
   const int c = blockIdx.x;  // 0-based class
   const int Ww = ceil_div(W, 32);
   unsigned int* occ = ws.occ + (size_t)c * H * Ww;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
   if (n == 1 && ws.g.cls[0] == 0) return;  // MaskROI's dummy detection: mask_removal.py:55-57
   const int r_lo = ws.round_lo[rq], r_hi = min(ws.round_lo[rq + 1], n);
   if (r_lo >= r_hi) return;
 
   // ---- ordered list of the ranks that belong to this class ----
-  if (threadIdx.x == 0) s_cnt = 0;
-  __syncthreads();
-  for (int base = r_lo; base < r_hi; base += blockDim.x) {
+  int cnt = 0;
+  for (int base = r_lo; base < r_hi; base += kDecideThreads) {
     const int r = base + threadIdx.x;
     const bool mine = r < r_hi && ws.g.cls[ws.order[r]] - 1 == c;
-    const unsigned int m = __ballot_sync(0xffffffffu, mine);
-    if (lane == 0) s_warp_cnt[warp] = __popc(m);
-    __syncthreads();
-    int off = s_cnt;
-    for (int w2 = 0; w2 < warp; ++w2) off += s_warp_cnt[w2];
-    if (mine) list[off + __popc(m & ((1u << lane) - 1u))] = (unsigned short)r;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int tot = 0;
-      for (int w2 = 0; w2 < (int)(blockDim.x >> 5); ++w2) tot += s_warp_cnt[w2];
-      s_cnt += tot;
-    }
-    __syncthreads();
+    int tot;
+    const int rank = cta_ballot_rank<kDecideThreads>(mine, s_warp_cnt, &tot);
+    if (mine) list[cnt + rank] = (unsigned short)r;
+    cnt += tot;
   }
-  const int cnt = s_cnt;
+  __syncthreads();   // list is complete
   // per-instance metadata of the whole class list staged in (dynamic) shared memory: inside the decision loops nothing but
   // the window words and the occupancy words comes from L2
   extern __shared__ __align__(16) unsigned char s_dyn[];
@@ -318,7 +292,7 @@ pan_decide_kernel(int n_max, const int* __restrict__ n_dev, int H, int W, double
   long long* s_off = reinterpret_cast<long long*>(s_win + n_max);      // word offset in ws.bits  [n_max]
   int* s_msum = reinterpret_cast<int*>(s_off + n_max);                 // |mask|                  [n_max]
   volatile int* s_state = reinterpret_cast<volatile int*>(s_msum + n_max);   // 0 undecided, 1 dropped, 2 kept   [n_max]
-  for (int li = threadIdx.x; li < cnt; li += blockDim.x) {
+  for (int li = threadIdx.x; li < cnt; li += kDecideThreads) {
     const int r = list[li];
     const int i = ws.order[r];
     const int x0 = ws.g.gx0[i], x1 = ws.g.gx1[i], y0 = ws.g.gy0[i], y1 = ws.g.gy1[i];
@@ -397,39 +371,28 @@ pan_decide_kernel(int n_max, const int* __restrict__ n_dev, int H, int W, double
   }
 }
 
-__global__ void __launch_bounds__(1024)
+constexpr int kCompactThreads = 1024;
+
+__global__ void __launch_bounds__(kCompactThreads)
 pan_compact_kernel(int n_max, const int* __restrict__ n_dev, PanWorkspace ws, int64_t* __restrict__ keep_out,
                    int* __restrict__ k_out) {
-  __shared__ int s_wcnt[32];
-  __shared__ int s_base;
+  __shared__ int s_wcnt[kCompactThreads / 32];
   const int n = n_dev ? max(min(*n_dev, n_max), 1) : n_max;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) s_base = 0;
-  __syncthreads();
-  for (int base = 0; base < n; base += 1024) {          // ordered (rank order) compaction, 1024 ranks per step
+  int k = 0;
+  for (int base = 0; base < n; base += kCompactThreads) {   // ordered (rank order) compaction
     const int r = base + threadIdx.x;
     const bool kept = r < n && ws.kept_flag[r] != 0;
-    const unsigned int m = __ballot_sync(0xffffffffu, kept);
-    if (lane == 0) s_wcnt[warp] = __popc(m);
-    __syncthreads();
-    int off = s_base;
-    for (int w2 = 0; w2 < warp; ++w2) off += s_wcnt[w2];
+    int tot;
+    const int rank = cta_ballot_rank<kCompactThreads>(kept, s_wcnt, &tot);
     if (kept) {
-      const int pos = off + __popc(m & ((1u << lane) - 1u));
       const int i = ws.order[r];
-      ws.kept_list[pos] = i;
-      keep_out[pos] = i;
+      ws.kept_list[k + rank] = i;
+      keep_out[k + rank] = i;
     }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int tot = 0;
-      for (int w2 = 0; w2 < 32; ++w2) tot += s_wcnt[w2];
-      s_base += tot;
-    }
-    __syncthreads();
+    k += tot;
   }
   if (threadIdx.x == 0) {
-    int k = s_base, zero_mask = 0;
+    int zero_mask = 0;
     if (k == 0) {  // mask_removal.py:89-92 (and :55-57): keep=[0] with an all-zero mask plane
       ws.kept_list[0] = 0; keep_out[0] = 0; k = 1; zero_mask = 1;
     }
@@ -453,14 +416,14 @@ pan_fuse_kernel(const float* __restrict__ fcn, int S, int H, int W, int num_stuf
                 const float* __restrict__ mask_logit, PanWorkspace ws,
                 int64_t* __restrict__ labels, int64_t* __restrict__ sem_labels) {
   __shared__ unsigned short list[kMaxList];
-  __shared__ int s_cnt, s_first_unlisted;
+  __shared__ int s_first_unlisted;
   __shared__ int s_warp_cnt[kFuseThreads / 32];
   const int k = ws.meta[0], zero_mask = ws.meta[1];
   const int tx0 = blockIdx.x * kTileW, ty0 = blockIdx.y * kTileH;
   const int tx1 = min(tx0 + kTileW, W), ty1 = min(ty0 + kTileH, H);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) { s_cnt = 0; s_first_unlisted = k; }
+  if (threadIdx.x == 0) s_first_unlisted = k;
   __syncthreads();
+  int n_hit = 0;
   // ---- bin kept instances against this tile (ascending j preserved) ----
   for (int base = 0; base < k; base += kFuseThreads) {
     const int j = base + threadIdx.x;
@@ -473,24 +436,13 @@ pan_fuse_kernel(const float* __restrict__ fcn, int S, int H, int W, int num_stuf
       hit = hit_seg || hit_msk;
       if (!hit) atomicMin(&s_first_unlisted, j);
     }
-    const unsigned int m = __ballot_sync(0xffffffffu, hit);
-    if (lane == 0) s_warp_cnt[warp] = __popc(m);
-    __syncthreads();
-    int off = s_cnt;
-    for (int w2 = 0; w2 < warp; ++w2) off += s_warp_cnt[w2];
-    if (hit) {
-      const int pos = off + __popc(m & ((1u << lane) - 1u));
-      if (pos < kMaxList) list[pos] = (unsigned short)j;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int tot = 0;
-      for (int w2 = 0; w2 < kFuseThreads / 32; ++w2) tot += s_warp_cnt[w2];
-      s_cnt += tot;
-    }
-    __syncthreads();
+    int tot;
+    const int pos = n_hit + cta_ballot_rank<kFuseThreads>(hit, s_warp_cnt, &tot);
+    if (hit && pos < kMaxList) list[pos] = (unsigned short)j;
+    n_hit += tot;
   }
-  const int cnt = min(s_cnt, kMaxList);
+  __syncthreads();   // list and s_first_unlisted are complete
+  const int cnt = min(n_hit, kMaxList);
   const int u0 = s_first_unlisted;  // smallest kept index whose windows miss the tile (value 0)
   const bool any_unlisted = u0 < k;
 
@@ -658,7 +610,7 @@ extern "C" int upsnet_mask_removal(const float* boxes, const float* cls_prob, co
   const int Ww = ceil_div(W, 32);
   UPS_CUDA(cudaMemsetAsync(ws.occ, 0, (size_t)num_thing * H * Ww * sizeof(unsigned int), st));
   UPS_CUDA(cudaMemsetAsync(ws.kept_flag, 0, sizeof(int) * n, st));
-  pan_prep_kernel<<<1, 1024, 0, st>>>(boxes, cls_prob, cls_idx, n, n_dev, H, W, ws);
+  pan_prep_kernel<<<1, kPrepThreads, 0, st>>>(boxes, cls_prob, cls_idx, n, n_dev, H, W, ws);
   UPS_CHECK_LAUNCH();
   {
     static ups::PerDeviceOnce configured;
@@ -669,10 +621,10 @@ extern "C" int upsnet_mask_removal(const float* boxes, const float* cls_prob, co
   for (int rq = 0; rq < ws.rounds; ++rq) {   // one round unless n * H * W/32 words exceed the bit-window budget
     pan_bits_kernel<<<dim3(kBitsChunks, n), kBitsThreads, 0, st>>>(mask_logit, n, n_dev, rq, ws);
     UPS_CHECK_LAUNCH();
-    pan_decide_kernel<<<num_thing, 1024, (size_t)n * 32, st>>>(n, n_dev, H, W, fraction_threshold, rq, ws);
+    pan_decide_kernel<<<num_thing, kDecideThreads, (size_t)n * 32, st>>>(n, n_dev, H, W, fraction_threshold, rq, ws);
     UPS_CHECK_LAUNCH();
   }
-  pan_compact_kernel<<<1, 1024, 0, st>>>(n, n_dev, ws, keep_out, k_out);
+  pan_compact_kernel<<<1, kCompactThreads, 0, st>>>(n, n_dev, ws, keep_out, k_out);
   UPS_CHECK_LAUNCH();
   if (mask_energy) {
     dim3 grid((unsigned)min((size_t)kNumSMs * 8, ((size_t)H * W + 255) / 256), (unsigned)n);
@@ -723,7 +675,7 @@ static int panoptic_head_impl(const float* fcn, bool up4, int S, int H, int W, c
   const int Ww = ceil_div(W, 32);
   UPS_CUDA(cudaMemsetAsync(ws.occ, 0, (size_t)num_thing * H * Ww * sizeof(unsigned int), st));
   UPS_CUDA(cudaMemsetAsync(ws.kept_flag, 0, sizeof(int) * n, st));
-  pan_prep_kernel<<<1, 1024, 0, st>>>(boxes, cls_prob, cls_idx, n, n_dev, H, W, ws);
+  pan_prep_kernel<<<1, kPrepThreads, 0, st>>>(boxes, cls_prob, cls_idx, n, n_dev, H, W, ws);
   UPS_CHECK_LAUNCH();
   {
     static ups::PerDeviceOnce configured;
@@ -734,10 +686,10 @@ static int panoptic_head_impl(const float* fcn, bool up4, int S, int H, int W, c
   for (int rq = 0; rq < ws.rounds; ++rq) {   // one round unless n * H * W/32 words exceed the bit-window budget
     pan_bits_kernel<<<dim3(kBitsChunks, n), kBitsThreads, 0, st>>>(mask_logit, n, n_dev, rq, ws);
     UPS_CHECK_LAUNCH();
-    pan_decide_kernel<<<num_thing, 1024, (size_t)n * 32, st>>>(n, n_dev, H, W, fraction_threshold, rq, ws);
+    pan_decide_kernel<<<num_thing, kDecideThreads, (size_t)n * 32, st>>>(n, n_dev, H, W, fraction_threshold, rq, ws);
     UPS_CHECK_LAUNCH();
   }
-  pan_compact_kernel<<<1, 1024, 0, st>>>(n, n_dev, ws, keep_out, k_out);
+  pan_compact_kernel<<<1, kCompactThreads, 0, st>>>(n, n_dev, ws, keep_out, k_out);
   UPS_CHECK_LAUNCH();
   dim3 grid(ceil_div(W, kTileW), ceil_div(H, kTileH));
   if (up4) pan_fuse_kernel<true><<<grid, kFuseThreads, 0, st>>>(fcn, S, H, W, num_stuff, mask_logit, ws, labels, sem_labels);

@@ -6,6 +6,7 @@
 // Determinism: every output element has one owner thread that sums in a fixed order, the loss and the counts go through
 // per-block partials and a fixed-order second stage; there is no atomic in this file.
 #include "common.cuh"
+#include "cta.cuh"
 #include "targets.cuh"
 
 namespace ups {
@@ -127,13 +128,11 @@ __device__ __forceinline__ const PlInst* pl_stage_table(const PlArgs& a, PlInst*
 template <typename MT>
 __global__ void __launch_bounds__(kPlThreads) pl_forward_kernel(PlArgs a) {
   extern __shared__ PlInst s_tab[];
-  __shared__ double s_loss[kPlThreads / 32];
-  __shared__ int s_cnt[2][kPlThreads / 32];
   const PlInst* tab = pl_stage_table(a, s_tab);
   const int hw = a.h * a.w, p = blockIdx.x * kPlThreads + threadIdx.x;
   const int nch = a.num_stuff + a.k + (a.enable_void ? 1 : 0);
-  double loss = 0.0;
-  int correct = 0, ignored = 0;
+  double loss[1] = {0.0};
+  int cnt[2] = {0, 0};              // correct, ignored
   if (p < hw) {
     const int y = p / a.w, x = p - y * a.w;
     const long long g = pl_gt_value<MT>(a.seg_gt, (const MT*)a.mask_gt, a.keep, a.keep ? a.k : a.G, a.G, hw, p, a.num_stuff);
@@ -162,50 +161,24 @@ __global__ void __launch_bounds__(kPlThreads) pl_forward_kernel(PlArgs a) {
     const bool valid = g >= 0 && g < nch && g != 255;
     a.lse[p] = lse;
     a.gtc[p] = g == 255 ? 255 : (valid ? (int)g : kPlInvalid);
-    if (valid) loss = (double)(lse - lg);
-    correct = am == g;
-    ignored = g == 255;
+    if (valid) loss[0] = (double)(lse - lg);
+    cnt[0] = am == g;
+    cnt[1] = g == 255;
   }
-  // block partials in a fixed order: lanes by shuffle, warps by thread 0
-  for (int o = 16; o; o >>= 1) {
-    loss += __shfl_down_sync(0xffffffffu, loss, o);
-    correct += __shfl_down_sync(0xffffffffu, correct, o);
-    ignored += __shfl_down_sync(0xffffffffu, ignored, o);
-  }
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) { s_loss[wid] = loss; s_cnt[0][wid] = correct; s_cnt[1][wid] = ignored; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int j = 1; j < kPlThreads / 32; ++j) { loss += s_loss[j]; correct += s_cnt[0][j]; ignored += s_cnt[1][j]; }
-    a.part_loss[blockIdx.x] = loss;
-    a.part_cnt[2 * blockIdx.x] = correct;
-    a.part_cnt[2 * blockIdx.x + 1] = ignored;
-  }
+  cta_partials<kPlThreads, 1, 2>(loss, cnt, a.part_loss, a.part_cnt);
 }
 
 // second stage: one CTA sums the block partials in a fixed order
 __global__ void __launch_bounds__(kPlThreads) pl_finish_kernel(const double* part_loss, const int* part_cnt, int nblocks, int hw,
                                                                float* loss, float* accuracy, int* counts) {
-  __shared__ double s_loss[kPlThreads];
-  __shared__ int s_cnt[2][kPlThreads];
-  double l = 0.0;
-  int c = 0, g = 0;
-  for (int j = threadIdx.x; j < nblocks; j += kPlThreads) { l += part_loss[j]; c += part_cnt[2 * j]; g += part_cnt[2 * j + 1]; }
-  s_loss[threadIdx.x] = l; s_cnt[0][threadIdx.x] = c; s_cnt[1][threadIdx.x] = g;
-  __syncthreads();
-  for (int o = kPlThreads / 2; o; o >>= 1) {
-    if (threadIdx.x < o) {
-      s_loss[threadIdx.x] += s_loss[threadIdx.x + o];
-      s_cnt[0][threadIdx.x] += s_cnt[0][threadIdx.x + o];
-      s_cnt[1][threadIdx.x] += s_cnt[1][threadIdx.x + o];
-    }
-    __syncthreads();
-  }
+  double l[1];
+  int c[2];
+  cta_sum_partials<kPlThreads, 1, 2>(part_loss, part_cnt, nblocks, l, c);
   if (threadIdx.x == 0) {
-    *loss = (float)(s_loss[0] / (double)hw);                                   // .mean() over all pixels, ignored included
-    *accuracy = __fdiv_rn((float)s_cnt[0][0], (float)(hw - s_cnt[1][0]));      // correct.float() / total.float()
-    counts[0] = s_cnt[0][0];
-    counts[1] = s_cnt[1][0];
+    *loss = (float)(l[0] / (double)hw);                                   // .mean() over all pixels, ignored included
+    *accuracy = __fdiv_rn((float)c[0], (float)(hw - c[1]));               // correct.float() / total.float()
+    counts[0] = c[0];
+    counts[1] = c[1];
   }
 }
 

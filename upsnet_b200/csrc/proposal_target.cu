@@ -26,6 +26,7 @@
 // formulation to the literal rleFrPoly on random polygons).  Every rounding step is an explicit _rn intrinsic: gcc's
 // x86-64 build of maskApi.c and numpy do not contract into FMA.
 #include "common.cuh"
+#include "cta.cuh"
 #include "targets.cuh"
 
 namespace ups {
@@ -136,50 +137,6 @@ __global__ void __launch_bounds__(kPtThreads) pt_assign_kernel(const PtParams p)
   }
 }
 
-// the k-th smallest key (k >= 1) of positions 0..n-1 of a draw, by eight 8-bit radix passes in one CTA
-__device__ unsigned long long cta_kth_key(unsigned long long seed, int stream, int n, int k, unsigned int* hist,
-                                          unsigned long long* s_prefix, int* s_need) {
-  __syncthreads();
-  if (threadIdx.x == 0) { *s_prefix = 0ull; *s_need = k; }
-  for (int shift = 56; shift >= 0; shift -= 8) {
-    if (threadIdx.x < 256) hist[threadIdx.x] = 0u;
-    __syncthreads();
-    const unsigned long long prefix = *s_prefix;
-    const unsigned long long mask_hi = shift >= 56 ? 0ull : (~0ull << (shift + 8));
-    for (int i = threadIdx.x; i < n; i += kPtSample) {
-      const unsigned long long key = draw_key(seed, stream, (unsigned long long)i);
-      if ((key & mask_hi) == prefix) atomicAdd(&hist[(unsigned)(key >> shift) & 255u], 1u);
-    }
-    __syncthreads();
-    if (threadIdx.x < 32) {                 // warp 0: lane l owns bins 8l..8l+7
-      const int lane = threadIdx.x;
-      unsigned int c[8], sum = 0;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { c[j] = hist[8 * lane + j]; sum += c[j]; }
-      unsigned int incl = sum;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const unsigned int y = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += y;
-      }
-      const unsigned int need = (unsigned int)*s_need, excl = incl - sum;
-      const unsigned int hit = __ballot_sync(0xffffffffu, incl >= need);
-      if (lane == __ffs(hit) - 1) {
-        unsigned int acc = excl;
-        int d = 0;
-        for (; d < 7; ++d) {
-          if (acc + c[d] >= need) break;
-          acc += c[d];
-        }
-        *s_need = (int)(need - acc);
-        *s_prefix = prefix | ((unsigned long long)(8 * lane + d) << shift);
-      }
-    }
-    __syncthreads();
-  }
-  return *s_prefix;
-}
-
 // one output row: the roidb row `slot`, fg (label = its class) or bg (label 0)
 __device__ void pt_write_row(const PtParams& p, int o, int slot, bool fg, unsigned char* s_nongt) {
   const float4 b = slot_box(p, slot);
@@ -204,10 +161,7 @@ __device__ void pt_write_row(const PtParams& p, int o, int slot, bool fg, unsign
 
 // 2. candidates, draws and the output rows (one CTA)
 __global__ void __launch_bounds__(kPtSample) pt_sample_kernel(const PtParams p) {
-  __shared__ int warp_sums[32];
-  __shared__ unsigned int hist[256];
-  __shared__ unsigned long long s_prefix;
-  __shared__ int s_need;
+  __shared__ int warp_sums[kPtSample / 32];
   __shared__ unsigned char s_nongt[kPtMaxBatch];
   int n[2] = {0, 0};
   for (int c0 = 0; c0 < p.S; c0 += kPtSample) {
@@ -219,8 +173,8 @@ __global__ void __launch_bounds__(kPtSample) pt_sample_kernel(const PtParams p) 
       bg = m < p.bg_hi && m >= p.bg_lo;
     }
     int tf, tb;
-    const int ef = cta_scan_excl(fg, warp_sums, &tf);
-    const int eb = cta_scan_excl(bg, warp_sums, &tb);
+    const int ef = cta_scan_excl<kPtSample>((int)fg, warp_sums, &tf);
+    const int eb = cta_scan_excl<kPtSample>((int)bg, warp_sums, &tb);
     if (fg) p.list[0][n[0] + ef] = slot;
     if (bg) p.list[1][n[1] + eb] = slot;
     n[0] += tf; n[1] += tb;
@@ -231,13 +185,16 @@ __global__ void __launch_bounds__(kPtSample) pt_sample_kernel(const PtParams p) 
 #pragma unroll
   for (int s = 0; s < 2; ++s) {
     const int k = take[s], cnt = n[s];
-    const unsigned long long kth = (k > 0 && k < cnt) ? cta_kth_key(p.seed, s, cnt, k, hist, &s_prefix, &s_need) : 0ull;
+    // the k-th smallest key of the draw, the keys recomputed from the positions
+    auto key_at = [&](int i) { return draw_key(p.seed, s, (unsigned long long)i); };
+    const unsigned long long kth =
+        (k > 0 && k < cnt) ? cta_radix_select<kPtSample, unsigned long long, 64, 8, false>(key_at, cnt, k) : 0ull;
     int base = s ? take[0] : 0;
     for (int c0 = 0; c0 < cnt && k > 0; c0 += kPtSample) {
       const int i = c0 + threadIdx.x;
-      const bool sel = i < cnt && (k == cnt || draw_key(p.seed, s, (unsigned long long)i) <= kth);
+      const bool sel = i < cnt && (k == cnt || key_at(i) <= kth);
       int tot;
-      const int e = cta_scan_excl(sel, warp_sums, &tot);
+      const int e = cta_scan_excl<kPtSample>((int)sel, warp_sums, &tot);
       if (sel) pt_write_row(p, base + e, p.list[s][i], s == 0, s_nongt);
       base += tot;
     }
@@ -250,7 +207,7 @@ __global__ void __launch_bounds__(kPtSample) pt_sample_kernel(const PtParams p) 
     const int o = c0 + threadIdx.x;
     const bool f = o < rows && s_nongt[o];
     int tot;
-    const int e = cta_scan_excl(f, warp_sums, &tot);
+    const int e = cta_scan_excl<kPtSample>((int)f, warp_sums, &tot);
     if (f) p.nongt[nn + e] = o;
     nn += tot;
   }

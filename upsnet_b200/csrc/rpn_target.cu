@@ -13,6 +13,7 @@
 //   7. rt_write:   one CTA writes labels, box targets and weights of those anchors over the constant fill
 #include "anchors.cuh"
 #include "common.cuh"
+#include "cta.cuh"
 #include "targets.cuh"
 
 namespace ups {
@@ -189,18 +190,20 @@ __global__ void __launch_bounds__(kRtThreads) rt_label_kernel(const RtParams p) 
   }
 }
 
-// 3. CTA offsets of both candidate lists and the plan of both draws (one CTA of 1024 threads)
-__global__ void __launch_bounds__(1024) rt_scan_kernel(const RtParams p) {
-  __shared__ int warp_sums[32];
+// 3. CTA offsets of both candidate lists and the plan of both draws (one CTA)
+constexpr int kRtScanThreads = 1024;
+
+__global__ void __launch_bounds__(kRtScanThreads) rt_scan_kernel(const RtParams p) {
+  __shared__ int warp_sums[kRtScanThreads / 32];
   int carry_f = 0, carry_b = 0, carry_i = 0;
   int* off = p.blk + 3 * p.nblk;
-  for (int b0 = 0; b0 < p.nblk; b0 += 1024) {
+  for (int b0 = 0; b0 < p.nblk; b0 += kRtScanThreads) {
     const int b = b0 + threadIdx.x;
     const bool ok = b < p.nblk;
     int tf, tb, ti;
-    const int ef = cta_scan_excl(ok ? p.blk[3 * b] : 0, warp_sums, &tf);
-    const int eb = cta_scan_excl(ok ? p.blk[3 * b + 1] : 0, warp_sums, &tb);
-    cta_scan_excl(ok ? p.blk[3 * b + 2] : 0, warp_sums, &ti);
+    const int ef = cta_scan_excl<kRtScanThreads>(ok ? p.blk[3 * b] : 0, warp_sums, &tf);
+    const int eb = cta_scan_excl<kRtScanThreads>(ok ? p.blk[3 * b + 1] : 0, warp_sums, &tb);
+    cta_scan_excl<kRtScanThreads>(ok ? p.blk[3 * b + 2] : 0, warp_sums, &ti);
     if (ok) { off[2 * b] = carry_f + ef; off[2 * b + 1] = carry_b + eb; }
     carry_f += tf; carry_b += tb; carry_i += ti;
   }
@@ -225,17 +228,12 @@ __global__ void __launch_bounds__(1024) rt_scan_kernel(const RtParams p) {
 //    key(s, pos) = splitmix64(s ^ pos * golden gamma), s = seed (fg) or splitmix64(seed) (bg); fg keys are stored inverted so
 //    that both draws select the k smallest
 __global__ void __launch_bounds__(kRtThreads) rt_compact_kernel(const RtParams p) {
-  __shared__ int wf[kRtThreads / 32], wb[kRtThreads / 32];
+  __shared__ int warp_n[kRtThreads / 32];
   const int n = blockIdx.x * kRtThreads + threadIdx.x;
   const int fl = n < p.N ? p.flags[n] : 0;
   const bool fg = fl & kFlagFg, bg = fl & kFlagBg;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const unsigned bf = __ballot_sync(0xffffffffu, fg), bb = __ballot_sync(0xffffffffu, bg);
-  if (lane == 0) { wf[wid] = __popc(bf); wb[wid] = __popc(bb); }
-  __syncthreads();
-  const unsigned lt = (1u << lane) - 1u;
-  int rf = __popc(bf & lt), rb = __popc(bb & lt);
-  for (int w = 0; w < wid; ++w) { rf += wf[w]; rb += wb[w]; }
+  int tot;
+  const int rf = cta_ballot_rank<kRtThreads>(fg, warp_n, &tot), rb = cta_ballot_rank<kRtThreads>(bg, warp_n, &tot);
   const int* off = p.blk + 3 * p.nblk + 2 * blockIdx.x;
   if (fg) {
     const int pos = off[0] + rf;
@@ -255,7 +253,6 @@ __global__ void __launch_bounds__(kRtThreads) rt_select_kernel(const RtParams p,
   RtState* st = p.st;
   if (st->mode[s] != kDrawSelect) return;
   __shared__ unsigned int sh[256];
-  __shared__ int s_last;
   sh[threadIdx.x] = 0u;
   __syncthreads();
   const int n = st->n[s];
@@ -268,25 +265,14 @@ __global__ void __launch_bounds__(kRtThreads) rt_select_kernel(const RtParams p,
   }
   __syncthreads();
   if (sh[threadIdx.x]) atomicAdd(&st->hist[s][threadIdx.x], sh[threadIdx.x]);
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = atomicAdd(&st->ticket[s], 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
+  if (!last_cta(&st->ticket[s], gridDim.x)) return;
   sh[threadIdx.x] = __ldcg(&st->hist[s][threadIdx.x]);
   st->hist[s][threadIdx.x] = 0u;
   __syncthreads();
-  if (threadIdx.x == 0) {
-    const unsigned int need = (unsigned int)st->need[s];
-    unsigned int acc = 0;
-    int d = 0;
-    for (; d < 255; ++d) {
-      if (acc + sh[d] >= need) break;
-      acc += sh[d];
-    }
-    st->need[s] = (int)(need - acc);
-    st->prefix[s] = prefix | ((unsigned long long)d << shift);
+  RadixDigit d;
+  if (threadIdx.x < 32 && warp_radix_digit<256, false>(sh, st->need[s], &d)) {
+    st->need[s] = d.need;
+    st->prefix[s] = prefix | ((unsigned long long)d.digit << shift);
     st->ticket[s] = 0u;
   }
 }
@@ -419,7 +405,7 @@ extern "C" int upsnet_rpn_targets(const float* gt_boxes, int G, const double* ce
   UPS_CHECK_LAUNCH();
   rt_label_kernel<<<p.nblk, kRtThreads, 0, st>>>(p);
   UPS_CHECK_LAUNCH();
-  rt_scan_kernel<<<1, 1024, 0, st>>>(p);
+  rt_scan_kernel<<<1, kRtScanThreads, 0, st>>>(p);
   UPS_CHECK_LAUNCH();
   rt_compact_kernel<<<p.nblk, kRtThreads, 0, st>>>(p);
   UPS_CHECK_LAUNCH();

@@ -1,5 +1,5 @@
 // targets.cuh -- arithmetic shared by the training-target kernels (rpn_target.cu, proposal_target.cu): bbox.pyx's IoU,
-// the seeded draw keys that replace np.random.choice, bbox_transform_inv and a CTA-wide exclusive scan
+// the seeded draw keys that replace np.random.choice and bbox_transform_inv
 #pragma once
 #include <cuda_runtime.h>
 
@@ -48,33 +48,6 @@ __device__ __forceinline__ float4 box_target(float4 e, float4 g, float4 w) {
   return make_float4(__fdiv_rn(__fmul_rn(w.x, __fsub_rn(gcx, ecx)), ew),
                      __fdiv_rn(__fmul_rn(w.y, __fsub_rn(gcy, ecy)), eh), __fmul_rn(w.z, logf(__fdiv_rn(gw, ew))),
                      __fmul_rn(w.w, logf(__fdiv_rn(gh, eh))));
-}
-
-// exclusive scan of one int per thread over a 1024-thread CTA; *total gets the sum
-__device__ __forceinline__ int cta_scan_excl(int v, int* warp_sums, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp_sums[wid] = x;
-  __syncthreads();
-  if (wid == 0) {
-    int w = warp_sums[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += y;
-    }
-    warp_sums[lane] = w;
-  }
-  __syncthreads();
-  const int base = wid ? warp_sums[wid - 1] : 0;
-  *total = warp_sums[31];
-  __syncthreads();
-  return base + x - v;
 }
 
 }  // namespace ups

@@ -9,78 +9,13 @@
 // Determinism: every output element has one owner thread that sums in a fixed order; the scalar losses go through
 // per-block partials and a fixed-order second stage.  There is no atomic in this file.
 #include "common.cuh"
+#include "cta.cuh"
 #include "up4.cuh"
 
 namespace ups {
 namespace {
 
 constexpr int kTlThreads = 256;
-
-// per-block sums of ND doubles and NI ints, in a fixed order (lanes by shuffle, warps by thread 0), written to slot
-// blockIdx.x of pd [nblocks, ND] and pi [nblocks, NI].  Every thread of the block (kTlThreads) must call it.
-template <int ND, int NI>
-__device__ __forceinline__ void tl_block_partials(double (&d)[ND], int (&n)[NI], double* pd, int* pi) {
-  __shared__ double s_d[kTlThreads / 32][ND];
-  __shared__ int s_i[kTlThreads / 32][NI];
-  for (int o = 16; o; o >>= 1) {
-#pragma unroll
-    for (int j = 0; j < ND; ++j) d[j] += __shfl_down_sync(0xffffffffu, d[j], o);
-#pragma unroll
-    for (int j = 0; j < NI; ++j) n[j] += __shfl_down_sync(0xffffffffu, n[j], o);
-  }
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) {
-#pragma unroll
-    for (int j = 0; j < ND; ++j) s_d[wid][j] = d[j];
-#pragma unroll
-    for (int j = 0; j < NI; ++j) s_i[wid][j] = n[j];
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int k = 1; k < kTlThreads / 32; ++k) {
-#pragma unroll
-      for (int j = 0; j < ND; ++j) d[j] += s_d[k][j];
-#pragma unroll
-      for (int j = 0; j < NI; ++j) n[j] += s_i[k][j];
-    }
-#pragma unroll
-    for (int j = 0; j < ND; ++j) pd[(size_t)blockIdx.x * ND + j] = d[j];
-#pragma unroll
-    for (int j = 0; j < NI; ++j) pi[(size_t)blockIdx.x * NI + j] = n[j];
-  }
-}
-
-// second stage, one CTA of kTlThreads: the sums of all block partials, in a fixed order; valid in every thread on return
-template <int ND, int NI>
-__device__ __forceinline__ void tl_finish(const double* pd, const int* pi, int nblocks, double (&d)[ND], int (&n)[NI]) {
-  __shared__ double s_d[kTlThreads][ND];
-  __shared__ int s_i[kTlThreads][NI];
-  const int t = threadIdx.x;
-#pragma unroll
-  for (int j = 0; j < ND; ++j) s_d[t][j] = 0.0;
-#pragma unroll
-  for (int j = 0; j < NI; ++j) s_i[t][j] = 0;
-  for (int b = t; b < nblocks; b += kTlThreads) {
-#pragma unroll
-    for (int j = 0; j < ND; ++j) s_d[t][j] += pd[(size_t)b * ND + j];
-#pragma unroll
-    for (int j = 0; j < NI; ++j) s_i[t][j] += pi[(size_t)b * NI + j];
-  }
-  __syncthreads();
-  for (int o = kTlThreads / 2; o; o >>= 1) {
-    if (t < o) {
-#pragma unroll
-      for (int j = 0; j < ND; ++j) s_d[t][j] += s_d[t + o][j];
-#pragma unroll
-      for (int j = 0; j < NI; ++j) s_i[t][j] += s_i[t + o][j];
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int j = 0; j < ND; ++j) d[j] = s_d[0][j];
-#pragma unroll
-  for (int j = 0; j < NI; ++j) n[j] = s_i[0][j];
-}
 
 inline int tl_blocks(long long n) { return (int)((n + kTlThreads - 1) / kTlThreads); }
 
@@ -146,14 +81,14 @@ __global__ void __launch_bounds__(kTlThreads) sem_forward_kernel(const float* __
     }
     *reinterpret_cast<float4*>(lse + o) = out;
   }
-  tl_block_partials<1, 2>(d, n, part_d, part_i);
+  cta_partials<kTlThreads, 1, 2>(d, n, part_d, part_i);
 }
 
 __global__ void __launch_bounds__(kTlThreads) sem_finish_kernel(const double* part_d, const int* part_i, int nblocks,
                                                                 float* loss, int* counts) {
   double d[1];
   int n[2];
-  tl_finish<1, 2>(part_d, part_i, nblocks, d, n);
+  cta_sum_partials<kTlThreads, 1, 2>(part_d, part_i, nblocks, d, n);
   if (threadIdx.x == 0) {
     *loss = (float)(d[0] / (double)n[0]);          // 0 / 0 = NaN when every pixel is ignored, as torch's mean
     counts[0] = n[0];
@@ -332,14 +267,14 @@ __global__ void __launch_bounds__(kTlThreads) rpn_forward_kernel(RpnArgs a, doub
     }
     d[1] = (double)bl;
   }
-  tl_block_partials<2, 1>(d, n, part_d, part_i);
+  cta_partials<kTlThreads, 2, 1>(d, n, part_d, part_i);
 }
 
 __global__ void __launch_bounds__(kTlThreads) rpn_finish_kernel(const double* part_d, const int* part_i, int nblocks,
                                                                 float batch, float* cls_loss, float* bbox_loss) {
   double d[2];
   int n[1];
-  tl_finish<2, 1>(part_d, part_i, nblocks, d, n);
+  cta_sum_partials<kTlThreads, 2, 1>(part_d, part_i, nblocks, d, n);
   if (threadIdx.x == 0) {
     *cls_loss = (float)(d[0] / (double)batch);
     *bbox_loss = (float)d[1];
@@ -500,7 +435,7 @@ __global__ void __launch_bounds__(kTlThreads) mr_forward_kernel(MrArgs a, double
       }
     }
   }
-  tl_block_partials<3, 4>(d, n, part_d, part_i);
+  cta_partials<kTlThreads, 3, 4>(d, n, part_d, part_i);
 }
 
 __global__ void __launch_bounds__(kTlThreads) mr_finish_kernel(const double* part_d, const int* part_i, int nblocks, int R,
@@ -508,7 +443,7 @@ __global__ void __launch_bounds__(kTlThreads) mr_finish_kernel(const double* par
                                                                float* accuracy, int* counts) {
   double d[3];
   int n[4];
-  tl_finish<3, 4>(part_d, part_i, nblocks, d, n);
+  cta_sum_partials<kTlThreads, 3, 4>(part_d, part_i, nblocks, d, n);
   if (threadIdx.x == 0) {
     *cls_loss = (float)(d[0] / (double)n[0]);                               // mean over rows with a target
     *bbox_loss = (float)(d[1] / (double)R);                                 // loss_box.sum() / loss_box.shape[0]
