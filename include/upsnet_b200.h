@@ -850,6 +850,53 @@ int upsnet_sgd_apply(const upsnet_sgd_chunk *chunks, int num_chunks, int num_gro
 int upsnet_sgd_pack(const upsnet_sgd_pack_chunk *chunks, int num_chunks, void *stream);
 int upsnet_sgd_advance(int *iteration, void *stream);
 
+/* ---- dense convolution / FC backward (conv_backward.cu) ------------------------------------------
+ * For a layer y = act(conv(x, W) + b [+ residual]) run by upsnet_igemm_forward, the gradients of x, W, b and the
+ * residual from dY.  replaces: autograd's conv backward (cuDNN dgrad / wgrad and the bias / residual reductions) of the
+ * trainable nn.Conv2d, nn.Linear and nn.ConvTranspose2d layers of models/resnet.py, models/fpn.py, models/rpn.py and
+ * models/rcnn.py.  None of these synchronises or reads the device; all are capturable in a CUDA graph.  No atomics: the
+ * same inputs give the same bytes.  precision is UPSNET_PREC_BF16X3 (g and x stored as hi/lo pairs) or UPSNET_PREC_BF16.
+ *
+ * upsnet_conv_grad_prepare: dy float32 logical [N,C,H,W], stored NCHW, or NHWC with UPSNET_GRAD_DY_NHWC (contiguous
+ *   either way).  g = dy * [y > 0] with UPSNET_GRAD_RELU (y float32 NHWC [N,H,W,Cg], the forward's output), else dy,
+ *   written NHWC [N,H,W,Cp] with Cp = Cg rounded up to a multiple of 64 and zeros in the padding: bf16 (PREC_BF16) or a
+ *   pair [N,H,W,2 Cp] (PREC_BF16X3, UPSNET_DTYPE_PAIR layout).  Cg = C, or 4 C with UPSNET_GRAD_UNSHUFFLE2: then dy is
+ *   [N,C,2H,2W] (the output of a ConvTranspose2d(k = 2, s = 2)) and g[n,h,w,(2a + b) C + c] = dy[n,c,2h + a,2w + b], the
+ *   gradient of the 1x1 conv to 4 C channels that the engine makes of it.  dbias (may be NULL): float32 [C], the sum of g
+ *   over the pixels (and the four (a, b) groups), accumulated in fp64 in a fixed order and rounded once; needs a
+ *   workspace of upsnet_conv_grad_prepare_workspace_bytes.  dres (may be NULL; not with UNSHUFFLE2): float32 NHWC
+ *   [N,H,W,C] = g, or with UPSNET_GRAD_RES_UP2 (H, W even) [N,H/2,W/2,C] = the sum of g over each 2x2 block,
+ *   ((g00 + g01) + g10) + g11, the gradient of the nearest-neighbour up-sampled residual of the FPN top-down path.
+ * upsnet_igemm_pack_weight_dgrad: the weights of the data gradient, for upsnet_igemm_forward run on g: W'[ci][tap][co] =
+ *   W[co][ci][kh*kw - 1 - tap] as bf16 hi / lo planes [cout_pad(Cin)][kh*kw][Cp] (upsnet_igemm_pack_weight's format for
+ *   a layer Cp -> Cin).  dX of a stride-1 layer is then upsnet_igemm_forward(g, ..., Cin = Cp, Cout = Cin, the same k and
+ *   dilation, padding d (k - 1) - p) with a float32 NHWC output.
+ * upsnet_conv_dgrad_scatter2: dX float32 NHWC [N,H,W,C] of a stride-2 1x1 layer (pad 0) from dxc = W^T g [N,(H+1)/2,
+ *   (W+1)/2,C] (upsnet_igemm_forward of g with the 1x1 dgrad weights): dxc at the even pixels, 0 elsewhere.  C % 4 == 0.
+ * upsnet_conv_wgrad: dw float32 [Cout][Cin][kh][kw] (torch's layout) = sum over the output pixels p and images of
+ *   g[p][co] * x[p * stride + tap * dil - pad][ci] with x outside the image 0; x NHWC bf16 [N,H,W,Cin] or pair
+ *   [N,H,W,2 Cin], g as upsnet_conv_grad_prepare writes it.  bf16x3: lo*hi + hi*lo + hi*hi products per pixel, bf16:
+ *   hi*hi; fp32 accumulation in wgmma, K split over CTAs into fp32 partial tiles added in a fixed order.  With
+ *   UPSNET_GRAD_UNSHUFFLE2 (1x1, Cout = 4 C) dw is written as the ConvTranspose2d weight [Cin][C][2][2] instead.
+ *   Workspace: upsnet_conv_wgrad_workspace_bytes.  UPSNET_E_UNSUPPORTED before any launch for stride > 1 with k > 1
+ *   or padding, Cin % 64 != 0, or kh * kw > 49 (groups != 1 has no parameter: it is not supported).
+ */
+#define UPSNET_GRAD_RELU 1
+#define UPSNET_GRAD_RES_UP2 2
+#define UPSNET_GRAD_UNSHUFFLE2 4
+#define UPSNET_GRAD_DY_NHWC 8
+int upsnet_conv_grad_prepare_workspace_bytes(int N, int C, int H, int W, int flags, size_t *bytes);
+int upsnet_conv_grad_prepare(const float *dy, const float *y, void *g, float *dbias, float *dres, int N, int C, int H,
+                             int W, int flags, int precision, void *workspace, size_t workspace_bytes, void *stream);
+int upsnet_igemm_packed_weight_dgrad_bytes(int Cout, int Cin, int kh, int kw, size_t *bytes);
+int upsnet_igemm_pack_weight_dgrad(const float *weight, int Cout, int Cin, int kh, int kw, void *packed, void *stream);
+int upsnet_conv_dgrad_scatter2(const float *dxc, float *dx, int N, int H, int W, int C, void *stream);
+int upsnet_conv_wgrad_workspace_bytes(int N, int H, int W, int Cin, int Cout, int kh, int kw, int stride_h, int stride_w,
+                                      int pad_h, int pad_w, int dil_h, int dil_w, int precision, size_t *bytes);
+int upsnet_conv_wgrad(const void *x_nhwc, const void *g, float *dw, int N, int H, int W, int Cin, int Cout, int kh, int kw,
+                      int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int flags, int precision,
+                      void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,8 +10,8 @@ from .operators import (DeformConv, DeformConvWithOffset, ModDeformConv, ModDefo
 
 from .pipeline import PipelinedEngine  # noqa: F401,E402
 from .evaluation import PanopticQuality, SegmentationIoU, DetectionAP  # noqa: F401,E402
-from .training import (FlatBucketAllReduce, LRSchedule, MaskRCNNLoss, PanopticLabels, PanopticLoss, RPNLoss,  # noqa: F401,E402
-                       SemanticLoss, SGD)
+from .training import (Conv2dFunction, ConvTranspose2x2Function, FlatBucketAllReduce, LRSchedule,  # noqa: F401,E402
+                       MaskRCNNLoss, PanopticLabels, PanopticLoss, RPNLoss, SemanticLoss, SGD)
 
 __all__ = ["PipelinedEngine", "DeformConv", "DeformConvWithOffset", "ModDeformConv", "ModDeformConvWithOffsetMask",
            "ModulatedDeformConv", "RoIAlign", "ROIAlign", "RoIAlignFunction", "FPNRoIAlign", "PanopticHead",
@@ -20,4 +20,4 @@ __all__ = ["PipelinedEngine", "DeformConv", "DeformConvWithOffset", "ModDeformCo
            "gpu_nms_wrapper", "panoptic_fuse", "set_precision", "unified_pan_result", "prep_image", "im_post", "im_post_rle",
            "label_restore", "combined_pan_result", "get_combined_pan_result", "PanopticQuality", "SegmentationIoU", "DetectionAP",
            "PanopticLoss", "PanopticLabels", "SemanticLoss", "RPNLoss", "MaskRCNNLoss", "SGD", "LRSchedule",
-           "FlatBucketAllReduce"]
+           "FlatBucketAllReduce", "Conv2dFunction", "ConvTranspose2x2Function"]

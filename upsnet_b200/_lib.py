@@ -27,6 +27,7 @@ def EPI_SIGMOID_FROM(c):
 PREC_FP32_SIMT, PREC_BF16X3, PREC_BF16 = 0, 1, 2
 DTYPE_F32, DTYPE_BF16, DTYPE_PAIR = 0, 1, 2
 LAYOUT_FLAT_PAIR = 2
+GRAD_RELU, GRAD_RES_UP2, GRAD_UNSHUFFLE2, GRAD_DY_NHWC = 1, 2, 4, 8
 
 E_UNSUPPORTED = -2
 _ERR = {-1: "bad argument", E_UNSUPPORTED: "unsupported configuration", -3: "workspace too small"}

@@ -134,6 +134,20 @@ template <> struct Wgmma<256> {
   }
 };
 
+// The same with both operands MN-major in shared memory (transpose bits tnspA = tnspB = 1): A is stored [16 k][64 m] and
+// B [16 k][N n], M / N contiguous.  The weight gradient reads its operands this way: the pixel boxes that TMA loads have
+// the channels (M = Cout, N = Cin) contiguous and the pixels (K) as rows.
+template <int N> struct WgmmaT;
+template <> struct WgmmaT<128> {
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
+  }
+};
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int PENDING> __device__ __forceinline__ void wgmma_wait() {
@@ -153,6 +167,12 @@ __device__ __forceinline__ uint32_t wg_desc_hi(uint32_t sbo_bytes) { return (sbo
 // the same for K-major SWIZZLE_64B tiles (64-byte rows, layout type 2): K advances by 16 bf16 with the same add of 2
 __device__ __forceinline__ uint32_t wg_desc_hi_sw64(uint32_t sbo_bytes) { return (sbo_bytes >> 4) | (2u << 30); }
 __device__ __forceinline__ uint64_t wg_desc(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
+// MN-major SWIZZLE_128B (WgmmaT): each 128-byte row holds 64 M (or N) elements of one k, 8 rows form a 1 KB atom.  The
+// leading byte offset is the stride between 64-element column blocks along M / N, the stride byte offset (wg_desc_hi)
+// the stride between 8-row groups along K; K advances by 16 rows = 2 KB (a descriptor add of 128).
+__device__ __forceinline__ uint32_t wg_desc_mn_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
+  return ((smem_addr >> 4) & 0x3fffu) | ((lbo_bytes >> 4) << 16);
+}
 
 // Accumulator staging: the warpgroup's 64 x N fragment (rows [row0, row0 + 64) of the tile) is written to a row-major fp32
 // buffer, `pitch` floats per row, columns [c0, c0 + NC) only, at buffer column (col - c0).  The epilogues then read whole

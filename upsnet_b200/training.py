@@ -7,6 +7,12 @@
   The dense GEMMs of the deformable backward (d(weight) = dY col^T, d(col) = W^T dY) are library calls (torch.mm), like the
   reference's; the gather / scatter / coordinate-gradient kernels are ours.  OffsetConvFunction makes the offset conv of
   the *WithOffset* modules differentiable; its backward convs are library calls too.
+* conv2d / linear / conv_transpose2x2 (Conv2dFunction, ConvTranspose2x2Function): the trainable dense convolutions and
+  FC layers of models/{resnet,fpn,rpn,rcnn}.py with device gradients (csrc/conv_backward.cu).  Forward is ops.conv2d with
+  the fused bias / residual / ReLU epilogue on the stored copy of x (hi/lo pair for bf16x3, bf16 NHWC for bf16), which
+  is also all backward keeps of x; backward prepares g (ReLU mask, padded NHWC pair / bf16, d bias, d residual) in one
+  pass, runs dX on the forward kernel with tap-flipped weights and dW on a split-K wgmma kernel, and launches only what
+  needs_input_grad asks for.
 * FlatBucketAllReduce: the gradient all-reduce of `upsnet_end2end_train.py:121` (hvd.DistributedOptimizer) as flat bf16
   buckets over torch.distributed (NCCL between the GPUs, gloo in the CPU tests): gradients are packed per bucket,
   reduced asynchronously while the rest of backward runs, averaged and unpacked before the optimiser step (or, with
@@ -32,9 +38,11 @@
   only and can be replayed from a CUDA graph.  Unlike the reference, the step does not write g + wd p back into p.grad.
 
 Scope note: this is the operator / communication layer of the training configuration, the RPN and proposal targets,
-the label maps, every loss of the training forward and the optimiser.  fcn_roi_loss (train.fcn_with_roi_loss is off in
-every shipped configuration), Adam and clip_grad (imported by the training script, never called) are not built; the
-dense backward convolutions are library calls.
+the label maps, every loss of the training forward, the dense convolutions and FC layers with their gradients, and the
+optimiser.  fcn_roi_loss (train.fcn_with_roi_loss is off in every shipped configuration), Adam and clip_grad (imported
+by the training script, never called) are not built; the model's training forward that composes these pieces is not
+built yet.  The offset convs of the *WithOffset* modules (OffsetConvFunction) and the GEMMs of the deformable backward
+stay library calls.
 """
 import ctypes as C
 
@@ -209,6 +217,201 @@ class FPNRoIAlignFunction(torch.autograd.Function):
             call("roi_align_backward", grad_out.device, g, rois, R, B, Cc, H, W, ph, pw, sr, scales[lv], dfeat)
             dfeats.append(dfeat)
         return (None, None, None, None, None) + tuple(dfeats)
+
+
+# ------------------------------------------------------------------------------------------------
+# dense convolutions and FC layers with device gradients (csrc/conv_backward.cu)
+# ------------------------------------------------------------------------------------------------
+_CONV_PREC = {"bf16x3": _lib.PREC_BF16X3, "bf16": _lib.PREC_BF16}
+_dgrad_cache = {}
+
+
+def _conv_prec(precision):
+    if precision not in _CONV_PREC:
+        raise ValueError("precision must be 'bf16x3' or 'bf16', got %r" % (precision,))
+    return _CONV_PREC[precision]
+
+
+def _stored_input(x, prec):
+    """The copy of x the forward kernel reads, and the weight gradient reads again: the hi/lo pair store [N,H,W,2C]
+    (bf16x3; the same bytes as the fp32 x) or bf16 NHWC [N,H,W,C] (bf16)."""
+    from . import operators as ops
+    x = x.detach()
+    if prec == _lib.PREC_BF16X3:
+        return ops.Pair.from_float(x).store
+    return ops._nhwc(x.to(torch.bfloat16))
+
+
+def _kernel_input(store, prec):
+    """The stored copy as ops.conv2d takes it: a Pair, or the logical [N,C,H,W] bf16 view of the NHWC store."""
+    from . import operators as ops
+    return ops.Pair(store) if prec == _lib.PREC_BF16X3 else store.permute(0, 3, 1, 2)
+
+
+def _check_conv_grad(N, Cin, H, W, weight, stride, padding, dilation, prec):
+    """Raises UpsnetError, before any launch, for a layer whose backward the kernels do not cover: groups != 1, Cin % 64,
+    stride > 1 with k > 1 or padding, a padding above d (k - 1) (no stride-1 data gradient as a convolution)."""
+    Cout, Cin_w, kh, kw = weight.shape
+    (sh, sw), (ph, pw), (dh, dw) = stride, padding, dilation
+    if Cin_w != Cin:
+        raise _lib.UpsnetError("conv2d backward: groups != 1 is not supported (weight %s, input channels %d)"
+                               % (tuple(weight.shape), Cin))
+    if (sh, sw) == (1, 1) and (ph > dh * (kh - 1) or pw > dw * (kw - 1)):
+        raise _lib.UpsnetError("conv2d backward: padding %s above dilation * (k - 1)" % ((ph, pw),))
+    query_bytes("conv_wgrad_workspace_bytes", N, H, W, Cin, Cout, kh, kw, sh, sw, ph, pw, dh, dw, prec)
+
+
+def conv2d_backward(dy, x_store, y_store, weight, geom, prec, relu=False, has_bias=False, residual_up2=False,
+                    need=(True, True, True, False), deconv=False):
+    """Gradients of y = act(conv(x, W) + b [+ residual]) from dy (float32 logical [N,Cout,Ho,Wo], or [N,C,2Ho,2Wo] for
+    the 2x2 deconv): (dx, dw, db, dres) for the four flags of `need`, None where not needed.  x_store: _stored_input(x);
+    y_store: the forward's float32 NHWC output (read for the ReLU mask); geom: (N, Cin, H, W, stride, padding, dilation)
+    of the forward.  dx and dres are float32 logical NCHW with channels_last storage.  Kernels only, no host sync:
+    capturable in a CUDA graph."""
+    from . import operators as ops
+    need_x, need_w, need_b, need_r = need
+    N, Cin, H, W, (sh, sw), (ph, pw), (dh, dw) = geom
+    Cw, _, kh, kw = weight.shape           # deconv: the 1x1 weight [4 C, Cin, 1, 1]
+    C = Cw // 4 if deconv else Cw
+    dev = dy.device
+    if dy.dtype != torch.float32:
+        dy = dy.float()
+    if dy.is_contiguous():
+        nhwc = False
+    elif dy.is_contiguous(memory_format=torch.channels_last):
+        nhwc = True
+    else:
+        dy, nhwc = dy.contiguous(), False
+    Ho, Wo = _conv_out(H, ph, dh, kh, sh), _conv_out(W, pw, dw, kw, sw)
+    Cp = (Cw + 63) // 64 * 64
+    pair = prec == _lib.PREC_BF16X3
+    flags = ((_lib.GRAD_RELU if relu else 0) | (_lib.GRAD_RES_UP2 if residual_up2 and need_r else 0) |
+             (_lib.GRAD_UNSHUFFLE2 if deconv else 0) | (_lib.GRAD_DY_NHWC if nhwc else 0))
+    g = torch.empty((N, Ho, Wo, Cp * (2 if pair else 1)), dtype=torch.bfloat16, device=dev)
+    db = torch.empty(C, dtype=torch.float32, device=dev) if (need_b and has_bias) else None
+    dres = None
+    if need_r:
+        Hr, Wr = (Ho // 2, Wo // 2) if residual_up2 else (Ho, Wo)
+        dres = torch.empty((N, Hr, Wr, C), dtype=torch.float32, device=dev)
+    ws = None
+    if db is not None:
+        ws = torch.empty(query_bytes("conv_grad_prepare_workspace_bytes", N, C, Ho, Wo, flags), dtype=torch.uint8, device=dev)
+    call("conv_grad_prepare", dev, dy, y_store if relu else None, g, db, dres, N, C, Ho, Wo, flags, prec,
+         ws, 0 if ws is None else ws.numel())
+    g_dt = _lib.DTYPE_PAIR if pair else _lib.DTYPE_BF16
+    dx = dw_ = None
+    if need_x:
+        packed = ops._packed(_dgrad_cache, weight, "igemm_pack_weight_dgrad", "igemm_packed_weight_dgrad_bytes",
+                             weight.shape)
+        strided = (sh, sw) != (1, 1)
+        qh, qw = (0, 0) if strided else (dh * (kh - 1) - ph, dw * (kw - 1) - pw)
+        out = torch.empty((N, Ho, Wo, Cin) if strided else (N, H, W, Cin), dtype=torch.float32, device=dev)
+        call("igemm_forward", dev, g, None, None, packed, None, None, out, N, Ho, Wo, Cp, Cin, kh, kw, 1, 1, qh, qw,
+             dh, dw, _lib.LAYOUT_NHWC, g_dt, _lib.DTYPE_F32, 0, prec, None)
+        if strided:
+            full = torch.empty((N, H, W, Cin), dtype=torch.float32, device=dev)
+            call("conv_dgrad_scatter2", dev, out, full, N, H, W, Cin)
+            out = full
+        dx = out.permute(0, 3, 1, 2)
+    if need_w:
+        nb = query_bytes("conv_wgrad_workspace_bytes", N, H, W, Cin, Cw, kh, kw, sh, sw, ph, pw, dh, dw, prec)
+        wws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        dw_ = torch.empty((Cin, C, 2, 2) if deconv else tuple(weight.shape), dtype=torch.float32, device=dev)
+        call("conv_wgrad", dev, x_store, g, dw_, N, H, W, Cin, Cw, kh, kw, sh, sw, ph, pw, dh, dw,
+             _lib.GRAD_UNSHUFFLE2 if deconv else 0, prec, wws, nb)
+    return dx, dw_, db, (None if dres is None else dres.permute(0, 3, 1, 2))
+
+
+class Conv2dFunction(torch.autograd.Function):
+    """y = act(conv(x, W) + b [+ residual]) with device gradients.  Forward: ops.conv2d on the stored copy of x (hi/lo pair
+    for bf16x3, bf16 NHWC for bf16) with the fused epilogue and a float32 output, the same bytes as ops.conv2d of that
+    copy; the copy is what backward keeps of x.  Backward (conv2d_backward): only what needs_input_grad asks for."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, residual, stride, padding, dilation, residual_up2, relu, precision):
+        from . import operators as ops
+        require_cuda(x, weight, bias, residual)
+        prec = _conv_prec(precision)
+        stride, padding, dilation = _pair(stride), _pair(padding), _pair(dilation)
+        N, Cin, H, W = x.shape
+        _check_conv_grad(N, Cin, H, W, weight, stride, padding, dilation, prec)
+        xs = _stored_input(x, prec)
+        y = ops.conv2d(_kernel_input(xs, prec), weight.detach(), None if bias is None else bias.detach(),
+                       stride, padding, dilation, None if residual is None else residual.detach(), relu, prec,
+                       out_dtype=torch.float32, residual_up2=residual_up2)
+        ctx.save_for_backward(xs, y if relu else None, weight)
+        ctx.cfg = ((N, Cin, H, W, stride, padding, dilation), prec, relu, bias is not None, residual_up2)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        xs, y, weight = ctx.saved_tensors
+        geom, prec, relu, has_bias, residual_up2 = ctx.cfg
+        ni = ctx.needs_input_grad
+        y_store = None if y is None else y.permute(0, 2, 3, 1)
+        dx, dw_, db, dres = conv2d_backward(grad_out, xs, y_store, weight, geom, prec, relu, has_bias, residual_up2,
+                                            (ni[0], ni[1], ni[2], ni[3]))
+        return dx, dw_, db, dres, None, None, None, None, None, None
+
+
+def conv2d(x, weight, bias=None, stride=1, padding=0, dilation=1, residual=None, residual_up2=False, relu=False,
+           precision="bf16x3"):
+    """Differentiable dense conv (groups 1) with the fused bias / residual / ReLU epilogue of ops.conv2d and device
+    gradients (Conv2dFunction).  x float32 [N,Cin,H,W] (Cin % 64 == 0); weight [Cout,Cin,kh,kw]; stride 2 only for 1x1
+    / pad 0; residual [N,Cout,Ho,Wo], or [N,Cout,Ho/2,Wo/2] with residual_up2 (nearest 2x up-sampling).
+    -> float32 [N,Cout,Ho,Wo], channels_last storage."""
+    return Conv2dFunction.apply(x, weight, bias, residual, stride, padding, dilation, residual_up2, relu, precision)
+
+
+def linear(x, weight, bias=None, relu=False, precision="bf16x3"):
+    """Differentiable y = x @ weight.T + bias (+ ReLU) as ops.linear computes it: a 1x1 conv over R one-pixel images.
+    x float32 [R, K] (K % 64 == 0), weight [Cout, K] -> float32 [R, Cout]."""
+    R, K = x.shape
+    y = conv2d(x.reshape(R, K, 1, 1), weight.reshape(weight.shape[0], K, 1, 1), bias, relu=relu, precision=precision)
+    return y.reshape(R, weight.shape[0])
+
+
+class ConvTranspose2x2Function(torch.autograd.Function):
+    """ConvTranspose2d(k = 2, s = 2) (+ ReLU) as the 1x1 conv to 4 C channels ordered (a, b, c) that the engine runs
+    (MaskBranch.prepare), followed by the pixel shuffle.  Backward reads dY through the 2x2 pixel-unshuffle of
+    upsnet_conv_grad_prepare and writes d weight straight in the [Cin, C, 2, 2] layout."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, relu, precision):
+        from . import operators as ops
+        require_cuda(x, weight, bias)
+        prec = _conv_prec(precision)
+        N, Cin, H, W = x.shape
+        C = weight.shape[1]
+        w1 = weight.detach().permute(2, 3, 1, 0).reshape(4 * C, Cin, 1, 1).contiguous()
+        b1 = None if bias is None else bias.detach().repeat(4).contiguous()
+        _check_conv_grad(N, Cin, H, W, w1, (1, 1), (0, 0), (1, 1), prec)
+        xs = _stored_input(x, prec)
+        y1 = ops.conv2d(_kernel_input(xs, prec), w1, b1, relu=relu, precision=prec, out_dtype=torch.float32)
+        store = y1.permute(0, 2, 3, 1)                                   # NHWC [N, H, W, (a, b, c)]
+        y = store.reshape(N, H, W, 2, 2, C).permute(0, 5, 1, 3, 2, 4).reshape(N, C, 2 * H, 2 * W)
+        ctx.save_for_backward(xs, store if relu else None, w1)
+        ctx.cfg = ((N, Cin, H, W, (1, 1), (0, 0), (1, 1)), prec, relu, bias is not None)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        xs, store, w1 = ctx.saved_tensors
+        geom, prec, relu, has_bias = ctx.cfg
+        ni = ctx.needs_input_grad
+        dx, dw_, db, _ = conv2d_backward(grad_out, xs, store, w1, geom, prec, relu, has_bias, False,
+                                         (ni[0], ni[1], ni[2], False), deconv=True)
+        return dx, dw_, db, None, None
+
+
+def conv_transpose2x2(x, weight, bias=None, stride=2, relu=False, precision="bf16x3"):
+    """Differentiable ConvTranspose2d with kernel = stride = 2, padding 0 (models/rcnn.py's mask deconv), with the ReLU
+    that follows it fused when relu=True.  x float32 [N,Cin,H,W] (Cin % 64 == 0), weight [Cin,C,2,2] ->
+    float32 [N,C,2H,2W].  Any other kernel size or stride raises."""
+    k = tuple(weight.shape[2:])
+    if k != (2, 2) or _pair(stride) != (2, 2):
+        raise _lib.UpsnetError("conv_transpose2x2: kernel %s / stride %s; only kernel = stride = 2" % (k, _pair(stride)))
+    return ConvTranspose2x2Function.apply(x, weight, bias, relu, precision)
 
 
 # ------------------------------------------------------------------------------------------------
