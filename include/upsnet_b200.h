@@ -265,6 +265,16 @@ int upsnet_upsample_bilinear_nchw(const float *x, float *y, int planes, int H, i
 int upsnet_fcn_score_fuse(const float *s2, const float *s3, const float *s4, const float *s5, float *out,
                           int planes, int H, int W, void *stream);
 
+/* The adjoint of upsnet_fcn_score_fuse (the semantic head's backward through the level sum):
+ * ds3 = up2^T(dscore), ds4 = up4^T(dscore), ds5 = up8^T(dscore) with the forward's bilinear weights (align_corners =
+ * False, clamped at 0, the last row / column repeated); d s2 is dscore itself, so nothing is written for it.
+ * replaces: autograd of the three F.interpolate of models/fcn.py:94-96 behind the score conv.
+ * dscore [planes,H,W] -> ds3 [planes,H/2,W/2], ds4 [planes,H/4,W/4], ds5 [planes,H/8,W/8] fp32, every element written.
+ * One launch.  A gather in a fixed order, no atomics: the same inputs give the same bytes; capturable.
+ * H % 8 == W % 8 == 0 and planes <= 65535, else UPSNET_E_UNSUPPORTED. */
+int upsnet_fcn_score_fuse_backward(const float *dscore, float *ds3, float *ds4, float *ds5, int planes, int H,
+                                   int W, void *stream);
+
 /* ---------------------------------------------------------------------------------------
  * Detection glue, fused (device-resident; nothing returns to the host).
  *

@@ -204,6 +204,82 @@ extern "C" int upsnet_fcn_score_fuse(const float* s2, const float* s3, const flo
   return 0;
 }
 
+// The adjoint of fcn_score_fuse: ds_l = up_f^T(dscore) for f = 2, 4, 8 (ds2 is dscore itself).  A gather: every source
+// pixel sums its own output footprint, so there are no atomics.  Source index s along an axis receives from the 2f
+// output coordinates f s - f/2 .. f s + 3f/2 - 1 (the forward's rule: clamped at 0 below, the last sample repeated
+// above), with the weights bilin_at gives it.  One CTA = a kFbTy x kFbTx source tile of one level and one plane:
+// A sums along x for every output row of the tile's footprint into shared memory, B sums those rows along y, each in a
+// fixed tap order.
+namespace ups {
+constexpr int kFbTx = 32, kFbTy = 8, kFbThreads = kFbTx * kFbTy;
+constexpr int kFbRows = 8 * kFbTy + 8;       // output rows of the x8 footprint of one tile, the largest
+
+// weight of source sample s in output coordinate o (n source samples, factor f), exactly as bilin_at forms it
+__device__ __forceinline__ float bilin_tap(int o, int s, int n, int f) {
+  const float src = fmaxf((1.0f / (float)f) * ((float)o + 0.5f) - 0.5f, 0.f);
+  const int i0 = (int)src, i1 = i0 + (i0 < n - 1 ? 1 : 0);
+  const float l = src - (float)i0;
+  return (i0 == s ? 1.f - l : 0.f) + (i1 == s ? l : 0.f);
+}
+
+__global__ void __launch_bounds__(kFbThreads)
+fcn_score_fuse_backward_kernel(const float* __restrict__ g, float* __restrict__ d3, float* __restrict__ d4,
+                               float* __restrict__ d5, int H, int W, int tiles3, int tiles4) {
+  __shared__ float s_xr[kFbRows * kFbTx];
+  int tile = blockIdx.x, lv = 1;
+  if (tile >= tiles3 + tiles4) { lv = 3; tile -= tiles3 + tiles4; }
+  else if (tile >= tiles3) { lv = 2; tile -= tiles3; }
+  const int f = 1 << lv, half = f >> 1, h = H >> lv, w = W >> lv;
+  const int tx = (w + kFbTx - 1) / kFbTx;
+  const int x0 = (tile % tx) * kFbTx, y0 = (tile / tx) * kFbTy;
+  const float* gp = g + (size_t)blockIdx.y * H * W;
+  float* dp = (lv == 1 ? d3 : lv == 2 ? d4 : d5) + (size_t)blockIdx.y * h * w;
+  const int rows = f * kFbTy + f, oy0 = f * y0 - half;
+  // A: output row oy0 + r, source column x0 + bx
+  for (int e = threadIdx.x; e < rows * kFbTx; e += kFbThreads) {
+    const int r = e / kFbTx, bx = e - r * kFbTx, xs = x0 + bx, oy = oy0 + r;
+    float acc = 0.f;
+    if (xs < w && oy >= 0 && oy < H) {
+      const float* row = gp + (size_t)oy * W;
+      for (int k = 0; k < 2 * f; ++k) {
+        const int ox = f * xs - half + k;
+        if (ox < 0 || ox >= W) continue;
+        acc = __fmaf_rn(bilin_tap(ox, xs, w, f), __ldg(row + ox), acc);
+      }
+    }
+    s_xr[e] = acc;
+  }
+  __syncthreads();
+  // B: one source pixel per thread; its output rows are halo rows f * sy .. f * sy + 2f - 1
+  const int sx = threadIdx.x % kFbTx, sy = threadIdx.x / kFbTx;
+  const int x = x0 + sx, y = y0 + sy;
+  if (x < w && y < h) {
+    float acc = 0.f;
+    for (int k = 0; k < 2 * f; ++k) {
+      const int oy = f * y - half + k;
+      if (oy < 0 || oy >= H) continue;
+      acc = __fmaf_rn(bilin_tap(oy, y, h, f), s_xr[(f * sy + k) * kFbTx + sx], acc);
+    }
+    dp[(size_t)y * w + x] = acc;
+  }
+}
+}  // namespace ups
+
+extern "C" int upsnet_fcn_score_fuse_backward(const float* dscore, float* ds3, float* ds4, float* ds5, int planes, int H,
+                                              int W, void* stream) {
+  if (!dscore || !ds3 || !ds4 || !ds5 || planes <= 0 || H <= 0 || W <= 0) return UPSNET_E_BADARG;
+  if ((H & 7) || (W & 7) || planes > 65535) return UPSNET_E_UNSUPPORTED;
+  long long tiles[3];
+  for (int lv = 1; lv <= 3; ++lv)
+    tiles[lv - 1] = (long long)ups::ceil_div(W >> lv, ups::kFbTx) * ups::ceil_div(H >> lv, ups::kFbTy);
+  const long long total = tiles[0] + tiles[1] + tiles[2];
+  if (total > 0x7fffffffLL) return UPSNET_E_UNSUPPORTED;
+  ups::fcn_score_fuse_backward_kernel<<<dim3((unsigned)total, (unsigned)planes), ups::kFbThreads, 0, (cudaStream_t)stream>>>(
+      dscore, ds3, ds4, ds5, H, W, (int)tiles[0], (int)tiles[1]);
+  UPS_CHECK_LAUNCH();
+  return 0;
+}
+
 extern "C" int upsnet_upsample_bilinear_nchw(const float* x, float* y, int planes, int H, int W, int factor, void* stream) {
   if (!x || !y || planes <= 0 || H <= 0 || W <= 0 || factor <= 0) return UPSNET_E_BADARG;
   if (((W * factor) & 3) || (((uintptr_t)y) & 15)) return UPSNET_E_UNSUPPORTED;

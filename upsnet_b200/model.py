@@ -9,7 +9,12 @@ resnet_upsnet}.py running on the sm_90a C ABI.
   panoptic_cls_probs, panoptic_outputs.
 * Frozen BatchNorm (models/resnet.py:69-78: always eval, requires_grad False) is folded into the
   preceding convolution once (prepare()); bias/ReLU/residual live in the conv epilogue.
-* Inference only (label must be None): training is BASELINE config #4, outside this round.
+* forward(data, label) -> the reference's nine training outputs (models/resnet_upsnet.py:88-195; Cityscapes configuration,
+  fcn_with_roi_loss off, one image): rpn_cls_loss, rpn_bbox_loss, cls_loss, bbox_loss, mask_loss, fcn_loss,
+  panoptic_loss, rcnn_accuracy, panoptic_accuracy, each float32 [1] on the device.  An eager autograd path separate from
+  the static engine: training.conv2d / linear / conv_transpose2x2 with BN folded per call, the DCN / ROIAlign backward
+  Functions, the semantic head's level sum through FcnScoreFuseFunction, and the device losses (_forward_train).
+  get_params_lr() gives the reference's 13 parameter groups for upsnet_b200.SGD.
 """
 import math
 
@@ -32,6 +37,8 @@ class UPSNetConfig:
         self.backbone_with_dconv = 100    # network.backbone_with_dconv (3 => DCN in res3..res5)
         self.backbone_with_dilation = False
         self.backbone_with_dpyramid = False
+        self.backbone_freeze_at = 2       # network.backbone_freeze_at: conv1 and res2..res<freeze_at> get no gradient
+        self.backbone_fix_bn = True       # network.backbone_fix_bn: BatchNorm frozen (eval statistics, no gradient)
         self.fpn_feature_dim = 256
         self.fpn_with_gap = False
         self.fcn_num_layers = 2
@@ -50,6 +57,15 @@ class UPSNetConfig:
         self.score_thresh = 0.05
         self.panoptic_score_thresh = 0.6
         self.panoptic_box_keep_fraction = 0.7   # < 1 => enable_void (resnet_upsnet.py:66-67)
+        # training forward (config.train.*): proposals, sampling, loss normalisers
+        self.train_rpn_pre_nms_top_n = 2000
+        self.train_rpn_post_nms_top_n = 2000
+        self.train_rpn_nms_thresh = 0.7
+        self.train_rpn_min_size = 0
+        self.batch_rois = 512
+        self.rpn_batch_size = 256
+        self.fg_fraction = 0.25
+        self.fcn_with_roi_loss = False
         for k, v in kw.items():
             if not hasattr(self, k):
                 raise AttributeError(k)
@@ -69,6 +85,8 @@ class UPSNetConfig:
                    backbone_with_dconv=int(get("network", "backbone_with_dconv", 100)),
                    backbone_with_dilation=bool(get("network", "backbone_with_dilation", False)),
                    backbone_with_dpyramid=bool(get("network", "backbone_with_dpyramid", False)),
+                   backbone_freeze_at=int(get("network", "backbone_freeze_at", 2)),
+                   backbone_fix_bn=bool(get("network", "backbone_fix_bn", True)),
                    fpn_feature_dim=int(get("network", "fpn_feature_dim", 256)), fpn_with_gap=bool(get("network", "fpn_with_gap", False)),
                    fcn_num_layers=int(get("network", "fcn_num_layers", 3)), num_anchors=int(get("network", "num_anchors", 3)),
                    anchor_scales=tuple(get("network", "anchor_scales", (8,))), anchor_ratios=tuple(get("network", "anchor_ratios", (0.5, 1, 2))),
@@ -78,7 +96,14 @@ class UPSNetConfig:
                    rpn_nms_thresh=float(get("test", "rpn_nms_thresh", 0.7)), rpn_min_size=int(get("test", "rpn_min_size", 0)),
                    nms_thresh=float(get("test", "nms_thresh", 0.5)), max_det=int(get("test", "max_det", 100)),
                    score_thresh=float(get("test", "score_thresh", 0.05)), panoptic_score_thresh=float(get("test", "panoptic_score_thresh", 0.6)),
-                   panoptic_box_keep_fraction=float(get("train", "panoptic_box_keep_fraction", 0.7)))
+                   panoptic_box_keep_fraction=float(get("train", "panoptic_box_keep_fraction", 0.7)),
+                   train_rpn_pre_nms_top_n=int(get("train", "rpn_pre_nms_top_n", 2000)),
+                   train_rpn_post_nms_top_n=int(get("train", "rpn_post_nms_top_n", 2000)),
+                   train_rpn_nms_thresh=float(get("train", "rpn_nms_thresh", 0.7)),
+                   train_rpn_min_size=int(get("train", "rpn_min_size", 0)),
+                   batch_rois=int(get("train", "batch_rois", 512)), rpn_batch_size=int(get("train", "rpn_batch_size", 256)),
+                   fg_fraction=float(get("train", "fg_fraction", 0.25)),
+                   fcn_with_roi_loss=bool(get("train", "fcn_with_roi_loss", False)))
 
     @classmethod
     def cityscapes_r50(cls):      # experiments/upsnet_resnet50_cityscapes_16gpu.yaml
@@ -87,7 +112,7 @@ class UPSNetConfig:
     @classmethod
     def coco_r101_dcn(cls):       # experiments/upsnet_resnet101_dcn_coco_3x_16gpu.yaml
         return cls(num_classes=81, num_seg_classes=133, backbone_with_dconv=3, fpn_with_gap=True,
-                   fcn_num_layers=3)
+                   fcn_num_layers=3, fcn_with_roi_loss=True)
 
 
 def _fold_bn(conv_w, bn):
@@ -525,6 +550,9 @@ class resnet_upsnet(nn.Module):
         self.pyramid_proposal = ProposalGenerator(cfg.rpn_feat_stride, cfg.anchor_scales, cfg.anchor_ratios,
                                                   cfg.rpn_pre_nms_top_n, cfg.rpn_post_nms_top_n,
                                                   cfg.rpn_nms_thresh, cfg.rpn_min_size)
+        self.pyramid_proposal_train = ProposalGenerator(cfg.rpn_feat_stride, cfg.anchor_scales, cfg.anchor_ratios,
+                                                        cfg.train_rpn_pre_nms_top_n, cfg.train_rpn_post_nms_top_n,
+                                                        cfg.train_rpn_nms_thresh, cfg.train_rpn_min_size)
         self.mask_roi = MaskROI(cfg.max_det, self.num_classes, cfg.nms_thresh, False, cfg.score_thresh,
                                 cfg.bbox_reg_weights)
         self.mask_roi_panoptic = MaskROI(cfg.max_det, self.num_classes, 0.5, True, cfg.panoptic_score_thresh,
@@ -548,14 +576,34 @@ class resnet_upsnet(nn.Module):
         self.max_graphs = 6           # captured graphs kept (LRU): one activation pool each (~2 GB at 1024x2048)
         self._prepared = False
         self.eval()
+        # backbone_freeze_at and backbone_fix_bn (models/resnet.py:69-78, 338-345): the stem, res2..res<freeze_at> and,
+        # with fix_bn, every BatchNorm are frozen, so they get no gradient and get_params_lr() does not list them
+        bb = self.resnet_backbone
+        frozen = [bb.conv1] + [getattr(bb, "res%d" % i) for i in range(2, cfg.backbone_freeze_at + 1)]
+        if cfg.backbone_fix_bn:
+            frozen += [m for m in self.modules() if isinstance(m, nn.BatchNorm2d)]
+        for m in frozen:
+            for p in m.parameters():
+                p.requires_grad_(False)
 
     def prepare(self):
         """Fold frozen BN, fuse sibling 1x1 heads, reshape the deconv: call after loading weights."""
+        self._drop_packed_weights()
         for m in self.modules():
             if m is not self and hasattr(m, "prepare"):
                 m.prepare()
         self._prepared = True
         return self
+
+    def _drop_packed_weights(self):
+        """Forget the packed copies ops keeps of the parameters themselves (keyed on the tensor and its version).
+        upsnet_b200.SGD bumps the version of what it updates, but a step replayed from a CUDA graph writes the parameters
+        without running any Python, so the model drops them wherever the parameters may have changed: in prepare() and at
+        the start of every training forward.  They are packed again, once, on their next use."""
+        from .training import _dgrad_cache
+        for cache in (ops._packed_cache, ops._dcn_packed_cache, ops._stem_cache, ops._view_cache, _dgrad_cache):
+            for p in self.parameters():
+                cache.pop(id(p), None)
 
     def _apply(self, fn, *a, **kw):
         """.to() / .cuda() / .float(): the folded / fused weights made by prepare() and the captured graphs refer to the
@@ -793,10 +841,34 @@ class resnet_upsnet(nn.Module):
         ops.STATS["launches"] += n_launch
         return out, graph
 
-    @torch.no_grad()
+    def get_params_lr(self):
+        """The reference's 13 parameter groups (models/resnet_upsnet.py:260-285, get_params of models/resnet.py:31-51):
+        the (empty) norm group, then for res3-res5, fpn, rcnn, mask_branch, rpn and fcn_head the weights at lr 1 and the
+        biases at lr 2 without weight decay, selected by the same name rule.  Only parameters with requires_grad."""
+        def params(prefixes, suffix):
+            for name, module in self.named_modules():
+                if name in prefixes:
+                    for n, p in module.named_parameters():
+                        n = name + "." + n
+                        if (n.split(".")[-1].startswith(suffix) or n.endswith(suffix)) and p.requires_grad:
+                            yield p
+        groups = [{"params": [], "lr": 1, "weight_decay": 0}]
+        for prefixes in (["resnet_backbone.res3", "resnet_backbone.res4", "resnet_backbone.res5"], ["fpn"], ["rcnn"],
+                         ["mask_branch"], ["rpn"], ["fcn_head"]):
+            groups.append({"params": list(params(prefixes, "weight")), "lr": 1})
+            groups.append({"params": list(params(prefixes, "bias")), "lr": 2, "weight_decay": 0})
+        return groups
+
     def forward(self, data, label=None):
+        """Inference (label None): the reference's result dict.  Training (label = the reference loader's dict): the
+        nine losses and accuracies of models/resnet_upsnet.py:180-193, each float32 [1] on the device, differentiable in
+        every parameter get_params_lr() lists (see _forward_train)."""
         if label is not None:
-            raise NotImplementedError("training forward (BASELINE config #4) is outside this round's scope")
+            return self._forward_train(data, label)
+        with torch.no_grad():
+            return self._forward_infer(data)
+
+    def _forward_infer(self, data):
         if not self._prepared:
             self.prepare()
         x = data["data"]
@@ -851,6 +923,172 @@ class resnet_upsnet(nn.Module):
                                          "bbox_pred": bbox_pred, "pmask_rois": pmask_rois, "pcls_prob": pcls_prob,
                                          "pmask_score": mask_score, "pcls_idx": pcls_idx, "keep_inds": keep}
         return results
+
+    # ------------------------------------------------------------------------------------------
+    # training forward: eager autograd, separate from the static engine
+    # ------------------------------------------------------------------------------------------
+    def _forward_train(self, data, label):
+        """models/resnet_upsnet.py:88-195 with label (Cityscapes configuration, fcn_with_roi_loss off, one image).
+
+        conv1 and res2 run under no_grad on the inference path (backbone_freeze_at = 2).  Every other dense conv and FC
+        layer is training.conv2d / linear / conv_transpose2x2, the frozen BatchNorm folded per call as w * scale plus a
+        constant shift, so autograd carries d weight back to the unfolded weight; DCN bottlenecks and the semantic head's
+        DeformConvWithOffset layers go through OffsetConvFunction / DeformConvFunction.  The semantic head scores every
+        level at its own resolution and sums the maps with FcnScoreFuseFunction: the 512-channel concat, the up-sampled
+        maps and fcn_output are never built (SemanticLoss up-samples inside the loss).  Proposals, proposal targets and
+        the panoptic keep draw run without gradients; np.random governs their draws, as in the reference.
+
+        Precision follows set_precision: 'bf16' runs the training convs in bf16; 'bf16x3' and 'fp32' run them in bf16x3
+        (there is no fp32 tensor-core backward).  A training forward drops the folded weights and captured graphs of the
+        inference engine, so the next inference forward folds the updated parameters again."""
+        from . import _lib, training as T
+        cfg = self.cfg
+        if cfg.fcn_with_roi_loss:
+            raise _lib.UpsnetError("training forward: train.fcn_with_roi_loss (fcn_roi_loss) is not built")
+        if cfg.fpn_with_gap:
+            raise _lib.UpsnetError("training forward: network.fpn_with_gap is not built")
+        if cfg.backbone_freeze_at != 2 or not cfg.backbone_fix_bn:
+            raise _lib.UpsnetError("training forward: only backbone_freeze_at = 2 with backbone_fix_bn (every shipped "
+                                   "configuration) is built, not freeze_at = %d, fix_bn = %s"
+                                   % (cfg.backbone_freeze_at, cfg.backbone_fix_bn))
+        x = data["data"]
+        _lib.require_cuda(x)
+        im_info = np.asarray(data["im_info"].cpu() if torch.is_tensor(data["im_info"]) else data["im_info"],
+                             dtype=np.float32).reshape(-1, 3)
+        if x.shape[0] != 1 or im_info.shape[0] != 1:
+            raise _lib.UpsnetError("training forward: one image per device")
+        self._prepared = False          # the optimiser updates the parameters in place after this step
+        self._graphs = {}
+        self._drop_packed_weights()
+        dev = x.device
+        prec = "bf16" if ops._PRECISION["conv"] == _lib.PREC_BF16 else "bf16x3"
+        lab = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in label.items()}
+        conv = lambda m, t, **kw: T.conv2d(t, m.weight, m.bias, precision=prec, **kw)     # noqa: E731
+
+        # backbone: frozen stem and res2 on the inference path, res3-res5 differentiable
+        bb = self.resnet_backbone
+        with torch.no_grad():
+            for m in [bb.conv1] + list(bb.res2.layers):
+                m.prepare()
+            r2 = ops.as_float(bb.res2(bb.conv1(x))).float()
+        r, stages = r2, []
+        for stage in (bb.res3, bb.res4, bb.res5):
+            for blk in stage.layers:
+                r = _train_bottleneck(blk, r, prec)
+            stages.append(r)
+        r3, r4, r5 = stages
+
+        # FPN (nearest 2x top-down add fused into the lateral conv), P6 = stride-2 subsample of P5
+        fp = self.fpn
+        p5_1x1 = conv(fp.fpn_p5_1x1, r5)
+        p4_plus = conv(fp.fpn_p4_1x1, r4, residual=p5_1x1, residual_up2=True)
+        p3_plus = conv(fp.fpn_p3_1x1, r3, residual=p4_plus, residual_up2=True)
+        p2_plus = conv(fp.fpn_p2_1x1, r2, residual=p3_plus, residual_up2=True)
+        p2, p3, p4, p5 = (conv(m, t, padding=1) for m, t in ((fp.fpn_p2, p2_plus), (fp.fpn_p3, p3_plus),
+                                                               (fp.fpn_p4, p4_plus), (fp.fpn_p5, p5_1x1)))
+        p6 = p5[:, :, ::2, ::2]
+
+        # RPN: shared 3x3 + ReLU, separate 1x1 heads (the logits feed the loss)
+        rp = self.rpn
+        rpn_score, rpn_bbox = [], []
+        for feat in (p2, p3, p4, p5, p6):
+            t = conv(rp.conv_proposal[0], feat, padding=1, relu=True)
+            rpn_score.append(conv(rp.cls_score, t))
+            rpn_bbox.append(conv(rp.bbox_pred, t))
+        with torch.no_grad():
+            rois, _ = self.pyramid_proposal_train([torch.sigmoid(s.detach()) for s in rpn_score], [b.detach() for b in rpn_bbox], im_info[0])
+            targets = T.ProposalTargets(num_classes=self.num_reg_classes, batch_rois=cfg.batch_rois,
+                                        fg_fraction=cfg.fg_fraction, bbox_reg_weights=cfg.bbox_reg_weights,
+                                        mask_size=cfg.mask_size).from_roidb(rois, lab["roidb"], im_info)
+        (s_rois, cls_label, bbox_target, bbox_iw, bbox_ow, mask_rois, mask_target, _, _) = targets
+
+        # semantic head: per-level subnet and 1x1 score slice, summed at P2 resolution
+        head = self.fcn_head
+        w = head.score.weight
+        scores = []
+        for l, feat in enumerate((p2, p3, p4, p5)):
+            for i in range(head.fcn_subnet.num_layers):
+                feat = F.relu(head.fcn_subnet.conv[i][0](feat))
+            scores.append(T.conv2d(feat, w[:, 128 * l:128 * (l + 1)], head.score.bias if l == 0 else None,
+                                   precision=prec))
+        fcn_score = T.FcnScoreFuseFunction.apply(*scores)
+
+        # instance head
+        levels = [p2, p3, p4, p5]
+        rc = self.rcnn
+        pool = T.FPNRoIAlignFunction.apply(s_rois, rc.pool_size, rc.pool_size, rc.roi_pooling.spatial_scale, 2, *levels)
+        fc6 = T.linear(pool.reshape(pool.shape[0], -1), rc.fc6[0].weight, rc.fc6[0].bias, relu=True, precision=prec)
+        fc7 = T.linear(fc6, rc.fc7[0].weight, rc.fc7[0].bias, relu=True, precision=prec)
+        cls_score = T.linear(fc7, rc.cls_score.weight, rc.cls_score.bias, precision=prec)
+        bbox_pred = T.linear(fc7, rc.bbox_pred.weight, rc.bbox_pred.bias, precision=prec)
+        mask_score = _train_mask_branch(self.mask_branch, levels, mask_rois, prec)
+        cls_loss, bbox_loss, mask_loss, rcnn_acc = T.MaskRCNNLoss(cfg.batch_rois)(
+            cls_score, bbox_pred, mask_score, cls_label, bbox_target, bbox_iw, bbox_ow, mask_target)
+        rpn_cls_loss, rpn_bbox_loss = T.RPNLoss(rpn_batch_size=cfg.rpn_batch_size)(rpn_score, rpn_bbox, lab)
+        fcn_loss = T.SemanticLoss()(fcn_score, lab["seg_gt"])
+
+        # panoptic head on the ground-truth boxes
+        gt_rois, cls_idx = T.gt_rois(lab["roidb"], im_info[0, 2], dev)
+        keep = T.draw_keep(gt_rois.shape[0], cfg.panoptic_box_keep_fraction) if self.enable_void else None
+        if keep is not None:
+            kd = torch.from_numpy(keep).to(dev)
+            gt_rois, cls_idx = gt_rois[kd], cls_idx[kd]
+        pan_mask = _train_mask_branch(self.mask_branch, levels, gt_rois, prec)
+        pan = T.PanopticLoss(num_seg_classes=self.num_seg_classes, num_classes=self.num_classes,
+                             enable_void=self.enable_void, mask_size=cfg.mask_size)
+        panoptic_loss, panoptic_acc = pan(fcn_score, pan_mask, gt_rois, cls_idx, lab["seg_gt_4x"], lab["mask_gt"], keep)
+
+        out = {"rpn_cls_loss": rpn_cls_loss, "rpn_bbox_loss": rpn_bbox_loss, "cls_loss": cls_loss, "bbox_loss": bbox_loss,
+               "mask_loss": mask_loss, "fcn_loss": fcn_loss, "panoptic_loss": panoptic_loss, "rcnn_accuracy": rcnn_acc,
+               "panoptic_accuracy": panoptic_acc}
+        out = {k: v.reshape(1) for k, v in out.items()}
+        if getattr(self, "keep_intermediates", False):   # the discrete decisions of the step, for an oracle replay
+            out["_intermediates"] = {
+                "rois": rois, "proposal_targets": dict(zip(T.ProposalTargets.NAMES, targets)), "gt_rois": gt_rois,
+                "cls_idx": cls_idx, "keep_inds": keep, "fpn": [f.detach() for f in (p2, p3, p4, p5, p6)]}
+        return out
+
+
+def _fold_bn_train(conv_w, bn):
+    """Frozen BatchNorm folded for a training conv: (conv_w * scale, shift), differentiable in conv_w only."""
+    with torch.no_grad():
+        scale = bn.weight / torch.sqrt(bn.running_var + bn.eps)
+        shift = (bn.bias - bn.running_mean * scale).contiguous()
+    return conv_w * scale.view(-1, 1, 1, 1), shift
+
+
+def _train_bottleneck(b, x, prec):
+    """Bottleneck.forward with device gradients (training.conv2d; DCN through Offset/DeformConvFunction)."""
+    from . import training as T
+    w1, b1 = _fold_bn_train(b.conv1.weight, b.bn1)
+    out = T.conv2d(x, w1, b1, stride=b.stride, relu=True, precision=prec)
+    w2, b2 = _fold_bn_train(b.conv2.weight, b.bn2)
+    if b.deformable:
+        offset = T.OffsetConvFunction.apply(out, b.conv2_offset.weight, b.conv2_offset.bias)
+        out = F.relu(T.DeformConvFunction.apply(out, offset, w2, b2, 1, b.dilation, b.dilation))
+    else:
+        out = T.conv2d(out, w2, b2, 1, b.dilation, b.dilation, relu=True, precision=prec)
+    residual = x
+    if b.downsample is not None:
+        wd, bd = _fold_bn_train(b.downsample[0].weight, b.downsample[1])
+        residual = T.conv2d(x, wd, bd, stride=b.stride, precision=prec)
+    w3, b3 = _fold_bn_train(b.conv3.weight, b.bn3)
+    return T.conv2d(out, w3, b3, residual=residual, relu=True, precision=prec)
+
+
+def _train_mask_branch(mb, levels, rois, prec):
+    """MaskBranch.forward with device gradients: ROIAlign 14x14, 4 x (3x3 + ReLU), 2x2 deconv + ReLU, 1x1 score."""
+    from . import training as T
+    M = mb.roi_pooling.pooled_height
+    if rois.shape[0] == 0:
+        return levels[0].new_zeros((0, mb.mask_score.weight.shape[0], 2 * M, 2 * M))
+    x = T.FPNRoIAlignFunction.apply(rois, M, M, mb.roi_pooling.spatial_scale, 2, *levels)
+    for i in range(1, 5):
+        c = getattr(mb, "mask_conv%d" % i)[0]
+        x = T.conv2d(x, c.weight, c.bias, padding=1, relu=True, precision=prec)
+    d = mb.mask_deconv1[0]
+    x = T.conv_transpose2x2(x, d.weight, d.bias, relu=True, precision=prec)
+    return T.conv2d(x, mb.mask_score.weight, mb.mask_score.bias, precision=prec)
 
 
 def resnet_50_upsnet(cfg=None):

@@ -36,12 +36,15 @@
   upsnet_end2end_train.py:76-103, 235-240, every parameter updated in one launch (csrc/sgd.cu), from p.grad or, through
   FlatBucketAllReduce.step, straight from the all-reduced bf16 buckets; with a schedule attached the step issues kernels
   only and can be replayed from a CUDA graph.  Unlike the reference, the step does not write g + wd p back into p.grad.
+* FcnScoreFuseFunction / fcn_score_fuse_backward: the semantic head's level sum s2 + up2(s3) + up4(s4) + up8(s5) with
+  its adjoint on the device (csrc/pool.cu upsnet_fcn_score_fuse_backward), used by the model's training forward.
 
 Scope note: this is the operator / communication layer of the training configuration, the RPN and proposal targets,
 the label maps, every loss of the training forward, the dense convolutions and FC layers with their gradients, and the
-optimiser.  fcn_roi_loss (train.fcn_with_roi_loss is off in every shipped configuration), Adam and clip_grad (imported
-by the training script, never called) are not built; the model's training forward that composes these pieces is not
-built yet.  The offset convs of the *WithOffset* modules (OffsetConvFunction) and the GEMMs of the deformable backward
+optimiser; resnet_upsnet.forward(data, label) (model.py) composes them into the training step of the Cityscapes
+configuration.  fcn_roi_loss (train.fcn_with_roi_loss, set by the COCO configurations upsnet_resnet50_coco_*.yaml and
+upsnet_resnet101_dcn_coco_3x_16gpu.yaml; the training forward raises there), Adam and clip_grad (imported by the
+training script, never called) are not built.  The offset convs of the *WithOffset* modules (OffsetConvFunction) and the GEMMs of the deformable backward
 stay library calls.
 """
 import ctypes as C
@@ -336,7 +339,9 @@ class Conv2dFunction(torch.autograd.Function):
         N, Cin, H, W = x.shape
         _check_conv_grad(N, Cin, H, W, weight, stride, padding, dilation, prec)
         xs = _stored_input(x, prec)
-        y = ops.conv2d(_kernel_input(xs, prec), weight.detach(), None if bias is None else bias.detach(),
+        # the weight itself, not a detached copy: its packed form is cached on the tensor and its version, so a
+        # parameter used several times in a step (the RPN head on five levels) is packed once
+        y = ops.conv2d(_kernel_input(xs, prec), weight, None if bias is None else bias.detach(),
                        stride, padding, dilation, None if residual is None else residual.detach(), relu, prec,
                        out_dtype=torch.float32, residual_up2=residual_up2)
         ctx.save_for_backward(xs, y if relu else None, weight)
@@ -412,6 +417,32 @@ def conv_transpose2x2(x, weight, bias=None, stride=2, relu=False, precision="bf1
     if k != (2, 2) or _pair(stride) != (2, 2):
         raise _lib.UpsnetError("conv_transpose2x2: kernel %s / stride %s; only kernel = stride = 2" % (k, _pair(stride)))
     return ConvTranspose2x2Function.apply(x, weight, bias, relu, precision)
+
+
+def fcn_score_fuse_backward(dscore):
+    """(ds3, ds4, ds5) = (up2^T, up4^T, up8^T)(dscore) for dscore float32 [N,C,H,W], H % 8 == W % 8 == 0: the adjoint of
+    ops.fcn_score_fuse in one launch (upsnet_fcn_score_fuse_backward)."""
+    require_cuda(dscore)
+    g = f32c(dscore)
+    N, Cc, H, W = g.shape
+    outs = [torch.empty((N, Cc, H >> l, W >> l), dtype=torch.float32, device=g.device) for l in (1, 2, 3)]
+    call("fcn_score_fuse_backward", g.device, g, *outs, N * Cc, H, W)
+    return tuple(outs)
+
+
+class FcnScoreFuseFunction(torch.autograd.Function):
+    """score = s2 + up2(s3) + up4(s4) + up8(s5) (bilinear, align_corners=False): forward ops.fcn_score_fuse, backward
+    its adjoint (fcn_score_fuse_backward); d s2 is the incoming gradient itself."""
+
+    @staticmethod
+    def forward(ctx, s2, s3, s4, s5):
+        from . import operators as ops
+        return ops.fcn_score_fuse(s2.detach(), s3.detach(), s4.detach(), s5.detach())
+
+    @staticmethod
+    def backward(ctx, grad):
+        g = f32c(grad)
+        return (g,) + fcn_score_fuse_backward(g)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -504,6 +535,7 @@ class FlatBucketAllReduce:
         for bi in range(len(self.buckets)):
             work[bi].wait()
             optimizer._apply(tables[bi][0], tables[bi][1], lr)
+            _bump_versions(self.buckets[bi])
         optimizer._advance()
         return self
 
@@ -539,6 +571,14 @@ def _pack_table(bucket, flat, dev):
             rows.append((0 if g is None else g.data_ptr() + 4 * s, flat.data_ptr() + 2 * (off + s), n, 0))
         off += p.numel()
     return _upload_table(rows, _PACK_DT, dev)
+
+
+def _bump_versions(params):
+    """The kernels write the parameters in place through raw pointers; advance their version counters as an in-place torch
+    op would, so that what is keyed on (tensor, version) -- the packed weights of ops, autograd's saved-tensor check --
+    sees the update.  Host only; a step replayed from a CUDA graph does not run it."""
+    for p in params:
+        torch.autograd.graph.increment_version(p)
 
 
 class LRSchedule:
@@ -611,6 +651,8 @@ class SGD(torch.optim.Optimizer):
       tables at a device iteration counter, which the step advances; such a step issues kernels only and can be captured
       in a CUDA graph (after one eager step, which uploads the chunk table).
     * Unlike the reference, p.grad is not written: the reference leaves g + wd p in it, which nothing reads.
+    * An eager step advances the version counter of every parameter, as an in-place torch op would; a step replayed
+      from a CUDA graph cannot, so code that caches per (tensor, version) must be told (resnet_upsnet does this itself).
     * zero_grad() zeroes gradients in place (set_to_none=False, the reference's torch behaviour), so their pointers and
       the cached chunk table stay valid.  dampening != 0 raises, as the reference asserts; nesterov is not built.
     float32 CUDA parameters on one device only."""
@@ -660,6 +702,7 @@ class SGD(torch.optim.Optimizer):
         if key != self._table_key:
             self._table, self._table_key = self._grad_table(), key
         self._apply(self._table[0], self._table[1], lr)
+        _bump_versions(self._params)
         self._advance()
         return loss
 
