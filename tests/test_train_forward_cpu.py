@@ -150,3 +150,18 @@ def test_freeze_config_sets_requires_grad_and_training_needs_freeze_at_2():
     assert all(p.requires_grad for n, p in m.named_parameters() if ".bn" in n and ".res3." in n)
     with pytest.raises(UpsnetError, match="fix_bn"):
         m(data, {"roidb": {}})
+
+
+def test_prepare_forgets_the_parameters_in_every_weight_cache():
+    """An optimiser step replayed from a CUDA graph leaves the parameters' versions as they were, so the model forgets
+    what every per-weight cache, the training dgrad packs included, holds for its parameters; other entries stay."""
+    from upsnet_b200 import operators as ops, training
+    from upsnet_b200.model import resnet_upsnet
+    m = resnet_upsnet([2, 2, 2, 2])
+    w, other = m.rpn.cls_score.weight, torch.zeros(2, 3)
+    assert training._dgrad_cache in ops._weight_caches
+    for cache in ops._weight_caches:
+        for t in (w, other):
+            ops._per_weight(cache, t, lambda: "packed")
+    m.prepare()
+    assert all(id(w) not in c and id(other) in c for c in ops._weight_caches)

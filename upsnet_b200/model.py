@@ -12,8 +12,9 @@ resnet_upsnet}.py running on the sm_90a C ABI.
 * forward(data, label) -> the reference's nine training outputs (models/resnet_upsnet.py:88-195; Cityscapes configuration,
   fcn_with_roi_loss off, one image): rpn_cls_loss, rpn_bbox_loss, cls_loss, bbox_loss, mask_loss, fcn_loss,
   panoptic_loss, rcnn_accuracy, panoptic_accuracy, each float32 [1] on the device.  An eager autograd path separate from
-  the static engine: training.conv2d / linear / conv_transpose2x2 with BN folded per call, the DCN / ROIAlign backward
-  Functions, the semantic head's level sum through FcnScoreFuseFunction, and the device losses (_forward_train).
+  the static engine: every module has forward_train(..., prec) next to its forward, built from training.conv2d / linear
+  / conv_transpose2x2 with BN folded per call, the DCN / ROIAlign backward Functions and, in the semantic head, the
+  level sum through FcnScoreFuseFunction; _forward_train composes them with the targets and the device losses.
   get_params_lr() gives the reference's 13 parameter groups for upsnet_b200.SGD.
 """
 import math
@@ -23,6 +24,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from . import _lib, training
 from . import operators as ops
 from .detection import MaskROI, ProposalGenerator, StaticMaskROI, StaticProposalGenerator
 from .operators import DeformConv, DeformConvWithOffset
@@ -116,8 +118,12 @@ class UPSNetConfig:
 
 
 def _fold_bn(conv_w, bn):
-    scale = bn.weight / torch.sqrt(bn.running_var + bn.eps)
-    return (conv_w * scale.view(-1, 1, 1, 1)).contiguous(), (bn.bias - bn.running_mean * scale).contiguous()
+    """Frozen BatchNorm folded into the preceding conv: (conv_w * scale, shift), differentiable in conv_w only.
+    prepare() detaches the result; forward_train keeps it, so autograd carries d weight back to the unfolded weight."""
+    with torch.no_grad():
+        scale = bn.weight / torch.sqrt(bn.running_var + bn.eps)
+        shift = (bn.bias - bn.running_mean * scale).contiguous()
+    return (conv_w * scale.view(-1, 1, 1, 1)).contiguous(), shift
 
 
 # ---------------------------------------------------------------------------------------------
@@ -164,6 +170,24 @@ class Bottleneck(nn.Module):
             out = ops.conv2d(out, f["w2"], f["b2"], 1, self.dilation, self.dilation, relu=True)
         residual = x if self.downsample is None else ops.conv2d(x, f["wd"], f["bd"], stride=self.stride)
         return ops.conv2d(out, f["w3"], f["b3"], residual=residual, relu=True)
+
+    def forward_train(self, x, prec):
+        """forward with device gradients: the dense convs through training.conv2d with BN folded per call, the
+        deformable 3x3 through OffsetConvFunction / DeformConvFunction."""
+        w1, b1 = _fold_bn(self.conv1.weight, self.bn1)
+        out = training.conv2d(x, w1, b1, stride=self.stride, relu=True, precision=prec)
+        w2, b2 = _fold_bn(self.conv2.weight, self.bn2)
+        if self.deformable:
+            offset = training.OffsetConvFunction.apply(out, self.conv2_offset.weight, self.conv2_offset.bias)
+            out = F.relu(training.DeformConvFunction.apply(out, offset, w2, b2, 1, self.dilation, self.dilation))
+        else:
+            out = training.conv2d(out, w2, b2, 1, self.dilation, self.dilation, relu=True, precision=prec)
+        residual = x
+        if self.downsample is not None:
+            wd, bd = _fold_bn(self.downsample[0].weight, self.downsample[1])
+            residual = training.conv2d(x, wd, bd, stride=self.stride, precision=prec)
+        w3, b3 = _fold_bn(self.conv3.weight, self.bn3)
+        return training.conv2d(out, w3, b3, residual=residual, relu=True, precision=prec)
 
 
 class Stem(nn.Module):
@@ -228,6 +252,20 @@ class ResNetBackbone(nn.Module):
         r4 = self.res4(r3)
         return r2, r3, r4, self.res5(r4)
 
+    def forward_train(self, x, prec):
+        """r2 .. r5 of the training forward: the frozen stem and res2 (backbone_freeze_at = 2) on the inference path
+        under no_grad, folded afresh, then res3 - res5 with device gradients."""
+        with torch.no_grad():
+            for m in [self.conv1] + list(self.res2.layers):
+                m.prepare()
+            r = ops.as_float(self.res2(self.conv1(x))).float()
+        out = [r]
+        for stage in (self.res3, self.res4, self.res5):
+            for blk in stage.layers:
+                r = blk.forward_train(r, prec)
+            out.append(r)
+        return tuple(out)
+
 
 # ---------------------------------------------------------------------------------------------
 # FPN / RPN / heads (models/fpn.py, rpn.py, rcnn.py, fcn.py)
@@ -272,6 +310,20 @@ class FPN(nn.Module):
         p6 = ops.subsample2(p5)                                         # MaxPool2d(kernel 1, stride 2)
         return p2, p3, p4, p5, p6
 
+    def forward_train(self, res2, res3, res4, res5, prec):
+        """forward with device gradients (training.conv2d, the same fused top-down add); without fpn_gap."""
+        def c(m, x, **kw):
+            return training.conv2d(x, m.weight, m.bias, precision=prec, **kw)
+        p5_1x1 = c(self.fpn_p5_1x1, res5)
+        p4_plus = c(self.fpn_p4_1x1, res4, residual=p5_1x1, residual_up2=True)
+        p3_plus = c(self.fpn_p3_1x1, res3, residual=p4_plus, residual_up2=True)
+        p2_plus = c(self.fpn_p2_1x1, res2, residual=p3_plus, residual_up2=True)
+        p2 = c(self.fpn_p2, p2_plus, padding=1)
+        p3 = c(self.fpn_p3, p3_plus, padding=1)
+        p4 = c(self.fpn_p4, p4_plus, padding=1)
+        p5 = c(self.fpn_p5, p5_1x1, padding=1)
+        return p2, p3, p4, p5, p5[:, :, ::2, ::2]
+
 
 class RPN(nn.Module):
     """models/rpn.py:26-57."""
@@ -299,6 +351,14 @@ class RPN(nn.Module):
         A = self.num_anchors
         both = ops.conv2d(t, self._f[0], self._f[1], out_format="nchw", sigmoid_from=5 * A).float()
         return both[:, :A], both[:, A:5 * A], both[:, 5 * A:]
+
+    def forward_train(self, x, prec):
+        """(cls_score, bbox_pred) logits of one level with device gradients: the shared 3x3 + ReLU, then the two 1x1
+        heads as separate convs."""
+        c = self.conv_proposal[0]
+        t = training.conv2d(x, c.weight, c.bias, padding=1, relu=True, precision=prec)
+        return (training.conv2d(t, self.cls_score.weight, self.cls_score.bias, precision=prec),
+                training.conv2d(t, self.bbox_pred.weight, self.bbox_pred.bias, precision=prec))
 
 
 class RCNN(nn.Module):
@@ -335,22 +395,31 @@ class RCNN(nn.Module):
         if isinstance(feat[0], ops.Pair):
             # hi/lo pair stream: ROIAlign writes the flattened (ph, pw, c) feature as one pair 'pixel' per roi
             ps = self.pool_size
-            pool = ops.fpn_roi_align(list(feat), rois, ps, ps, self.roi_pooling.spatial_scale, layout="flat_pair")
-            fc6 = ops.linear(pool, self._w6_nhwc, self.fc6[0].bias, relu=True)
-            fc7 = ops.linear(fc6, self.fc7[0].weight, self.fc7[0].bias, relu=True)
-            both = ops.linear(fc7, self._f[0], self._f[1], out_dtype=torch.float32).float()
-            return {"cls_score": both[:, :self.num_classes].contiguous(),
-                    "bbox_pred": both[:, self.num_classes:].contiguous(), "fc_feat": fc7}
-        pool = self.roi_pooling(feat, rois)
-        nhwc = pool.permute(0, 2, 3, 1)
-        if self._f is not None and nhwc.is_contiguous() and not pool.is_contiguous():
-            fc6 = ops.linear(nhwc.reshape(pool.size(0), -1), self._w6_nhwc, self.fc6[0].bias, relu=True)
+            x = ops.fpn_roi_align(list(feat), rois, ps, ps, self.roi_pooling.spatial_scale, layout="flat_pair")
+            w6 = self._w6_nhwc
         else:
-            fc6 = ops.linear(pool.reshape(pool.size(0), -1), self.fc6[0].weight, self.fc6[0].bias, relu=True)
+            pool = self.roi_pooling(feat, rois)
+            nhwc = pool.permute(0, 2, 3, 1)
+            if self._f is not None and nhwc.is_contiguous() and not pool.is_contiguous():
+                x, w6 = nhwc.reshape(pool.size(0), -1), self._w6_nhwc
+            else:
+                x, w6 = pool.reshape(pool.size(0), -1), self.fc6[0].weight
+        fc6 = ops.linear(x, w6, self.fc6[0].bias, relu=True)
         fc7 = ops.linear(fc6, self.fc7[0].weight, self.fc7[0].bias, relu=True)
         both = ops.linear(fc7, self._f[0], self._f[1], out_dtype=torch.float32).float()
         return {"cls_score": both[:, :self.num_classes].contiguous(),
                 "bbox_pred": both[:, self.num_classes:].contiguous(), "fc_feat": fc7}
+
+    def forward_train(self, feat, rois, prec):
+        """(cls_score, bbox_pred) with device gradients: FPNRoIAlignFunction on the fp32 levels, then fc6, fc7 and the
+        two heads as separate training.linear calls."""
+        ps = self.pool_size
+        pool = training.FPNRoIAlignFunction.apply(rois, ps, ps, self.roi_pooling.spatial_scale, 2, *feat)
+        fc6 = training.linear(pool.reshape(pool.shape[0], -1), self.fc6[0].weight, self.fc6[0].bias, relu=True,
+                              precision=prec)
+        fc7 = training.linear(fc6, self.fc7[0].weight, self.fc7[0].bias, relu=True, precision=prec)
+        return (training.linear(fc7, self.cls_score.weight, self.cls_score.bias, precision=prec),
+                training.linear(fc7, self.bbox_pred.weight, self.bbox_pred.bias, precision=prec))
 
 
 class MaskBranch(nn.Module):
@@ -397,26 +466,36 @@ class MaskBranch(nn.Module):
             yv = ops.conv2d(x, w1, b1, relu=True, pair_group=cout, **bound)                     # Pair [n, Cout, h, 4w]
             n, _, h, w4 = yv.shape
             w = w4 // 4
-            z = ops.conv2d(yv, self.mask_score.weight, self.mask_score.bias, out_format="nhwc", out_dtype=torch.float32,
-                           **bound)
-            K = z.shape[1]
-            z = z.permute(0, 2, 3, 1).reshape(n, h, w, 2, 2, K)
-            return z.permute(0, 5, 1, 3, 2, 4).reshape(n, K, 2 * h, 2 * w)
-        y = ops.conv2d(x, w1, b1, relu=True, **bound)        # [n, 4*Cout, h, w], channels ordered (a, b, co)
-        n, _, h, w = y.shape
-        if y.is_contiguous(memory_format=torch.channels_last) and y.dim() == 4:
+        else:
+            y = ops.conv2d(x, w1, b1, relu=True, **bound)        # [n, 4*Cout, h, w], channels ordered (a, b, co)
+            n, _, h, w = y.shape
+            if not (y.is_contiguous(memory_format=torch.channels_last) and y.dim() == 4):
+                y = y.reshape(n, 2, 2, cout, h, w).permute(0, 3, 4, 1, 5, 2).reshape(n, cout, 2 * h, 2 * w)
+                return ops.conv2d(y, self.mask_score.weight, self.mask_score.bias, out_format="nchw", **bound)
             # The pixel shuffle only permutes pixels and mask_score is a 1x1 conv, so they commute: score the four
             # (a, b) channel groups in place -- the NHWC storage [n,h,w,(a,b,co)] IS an NHWC tensor of 4w "pixels" per
             # row with Cout channels (a free view) -- and shuffle the num_classes-channel logits instead of the
             # 256-channel feature map (two 50 MB permute copies per call in the first version).
             yv = y.permute(0, 2, 3, 1).reshape(n, h, w * 4, cout).permute(0, 3, 1, 2)
-            z = ops.conv2d(yv, self.mask_score.weight, self.mask_score.bias, out_format="nhwc",
-                           out_dtype=torch.float32, **bound)                                      # [n, K, h, 4w]
-            K = z.shape[1]
-            z = z.permute(0, 2, 3, 1).reshape(n, h, w, 2, 2, K)                                    # (i, j, a, b, k)
-            return z.permute(0, 5, 1, 3, 2, 4).reshape(n, K, 2 * h, 2 * w)
-        y = y.reshape(n, 2, 2, cout, h, w).permute(0, 3, 4, 1, 5, 2).reshape(n, cout, 2 * h, 2 * w)
-        return ops.conv2d(y, self.mask_score.weight, self.mask_score.bias, out_format="nchw", **bound)
+        z = ops.conv2d(yv, self.mask_score.weight, self.mask_score.bias, out_format="nhwc", out_dtype=torch.float32,
+                       **bound)                                                                   # [n, K, h, 4w]
+        K = z.shape[1]
+        z = z.permute(0, 2, 3, 1).reshape(n, h, w, 2, 2, K)                                        # (i, j, a, b, k)
+        return z.permute(0, 5, 1, 3, 2, 4).reshape(n, K, 2 * h, 2 * w)
+
+    def forward_train(self, feat, rois, prec):
+        """Mask logits with device gradients: FPNRoIAlignFunction 14x14 on the fp32 levels, 4 x (3x3 + ReLU), the 2x2
+        deconv + ReLU (training.conv_transpose2x2) and the 1x1 score."""
+        M = self.roi_pooling.pooled_height
+        if rois.shape[0] == 0:
+            return feat[0].new_zeros((0, self.mask_score.weight.shape[0], 2 * M, 2 * M))
+        x = training.FPNRoIAlignFunction.apply(rois, M, M, self.roi_pooling.spatial_scale, 2, *feat)
+        for i in range(1, 5):
+            c = getattr(self, "mask_conv%d" % i)[0]
+            x = training.conv2d(x, c.weight, c.bias, padding=1, relu=True, precision=prec)
+        d = self.mask_deconv1[0]
+        x = training.conv_transpose2x2(x, d.weight, d.bias, relu=True, precision=prec)
+        return training.conv2d(x, self.mask_score.weight, self.mask_score.bias, precision=prec)
 
 
 class FCNSubNet(nn.Module):
@@ -528,6 +607,19 @@ class FCNHead(nn.Module):
             ret["fcn_output"] = F.interpolate(score, None, self.upsample_rate, mode="bilinear", align_corners=False)
         return ret
 
+    def forward_train(self, p2, p3, p4, p5, prec):
+        """fcn_score with device gradients, by the prepared forward's commutation: each level through the subnet's
+        DeformConvWithOffset layers and its 128-channel slice of the 1x1 score conv, the four maps summed at P2
+        resolution by FcnScoreFuseFunction.  The concat and fcn_output are never built (SemanticLoss up-samples)."""
+        w = self.score.weight
+        scores = []
+        for l, feat in enumerate((p2, p3, p4, p5)):
+            for i in range(self.fcn_subnet.num_layers):
+                feat = F.relu(self.fcn_subnet.conv[i][0](feat))
+            scores.append(training.conv2d(feat, w[:, 128 * l:128 * (l + 1)], self.score.bias if l == 0 else None,
+                                          precision=prec))
+        return training.FcnScoreFuseFunction.apply(*scores)
+
 
 # ---------------------------------------------------------------------------------------------
 class resnet_upsnet(nn.Module):
@@ -588,22 +680,12 @@ class resnet_upsnet(nn.Module):
 
     def prepare(self):
         """Fold frozen BN, fuse sibling 1x1 heads, reshape the deconv: call after loading weights."""
-        self._drop_packed_weights()
+        ops.forget_packed(self.parameters())
         for m in self.modules():
             if m is not self and hasattr(m, "prepare"):
                 m.prepare()
         self._prepared = True
         return self
-
-    def _drop_packed_weights(self):
-        """Forget the packed copies ops keeps of the parameters themselves (keyed on the tensor and its version).
-        upsnet_b200.SGD bumps the version of what it updates, but a step replayed from a CUDA graph writes the parameters
-        without running any Python, so the model drops them wherever the parameters may have changed: in prepare() and at
-        the start of every training forward.  They are packed again, once, on their next use."""
-        from .training import _dgrad_cache
-        for cache in (ops._packed_cache, ops._dcn_packed_cache, ops._stem_cache, ops._view_cache, _dgrad_cache):
-            for p in self.parameters():
-                cache.pop(id(p), None)
 
     def _apply(self, fn, *a, **kw):
         """.to() / .cuda() / .float(): the folded / fused weights made by prepare() and the captured graphs refer to the
@@ -930,18 +1012,14 @@ class resnet_upsnet(nn.Module):
     def _forward_train(self, data, label):
         """models/resnet_upsnet.py:88-195 with label (Cityscapes configuration, fcn_with_roi_loss off, one image).
 
-        conv1 and res2 run under no_grad on the inference path (backbone_freeze_at = 2).  Every other dense conv and FC
-        layer is training.conv2d / linear / conv_transpose2x2, the frozen BatchNorm folded per call as w * scale plus a
-        constant shift, so autograd carries d weight back to the unfolded weight; DCN bottlenecks and the semantic head's
-        DeformConvWithOffset layers go through OffsetConvFunction / DeformConvFunction.  The semantic head scores every
-        level at its own resolution and sums the maps with FcnScoreFuseFunction: the 512-channel concat, the up-sampled
-        maps and fcn_output are never built (SemanticLoss up-samples inside the loss).  Proposals, proposal targets and
-        the panoptic keep draw run without gradients; np.random governs their draws, as in the reference.
+        Each module runs its forward_train: the backbone with conv1 and res2 frozen on the inference path
+        (backbone_freeze_at = 2), then the FPN, the RPN per level, the semantic head, the RCNN and the mask branch, with
+        device gradients.  Proposals, proposal targets and the panoptic keep draw run without gradients; np.random
+        governs their draws, as in the reference, so the modules run in the order below.
 
         Precision follows set_precision: 'bf16' runs the training convs in bf16; 'bf16x3' and 'fp32' run them in bf16x3
         (there is no fp32 tensor-core backward).  A training forward drops the folded weights and captured graphs of the
         inference engine, so the next inference forward folds the updated parameters again."""
-        from . import _lib, training as T
         cfg = self.cfg
         if cfg.fcn_with_roi_loss:
             raise _lib.UpsnetError("training forward: train.fcn_with_roi_loss (fcn_roi_loss) is not built")
@@ -957,85 +1035,47 @@ class resnet_upsnet(nn.Module):
                              dtype=np.float32).reshape(-1, 3)
         if x.shape[0] != 1 or im_info.shape[0] != 1:
             raise _lib.UpsnetError("training forward: one image per device")
-        self._prepared = False          # the optimiser updates the parameters in place after this step
+        # the optimiser updates the parameters in place after this step, possibly from a replayed CUDA graph
+        self._prepared = False
         self._graphs = {}
-        self._drop_packed_weights()
+        ops.forget_packed(self.parameters())
         dev = x.device
         prec = "bf16" if ops._PRECISION["conv"] == _lib.PREC_BF16 else "bf16x3"
         lab = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in label.items()}
-        conv = lambda m, t, **kw: T.conv2d(t, m.weight, m.bias, precision=prec, **kw)     # noqa: E731
 
-        # backbone: frozen stem and res2 on the inference path, res3-res5 differentiable
-        bb = self.resnet_backbone
-        with torch.no_grad():
-            for m in [bb.conv1] + list(bb.res2.layers):
-                m.prepare()
-            r2 = ops.as_float(bb.res2(bb.conv1(x))).float()
-        r, stages = r2, []
-        for stage in (bb.res3, bb.res4, bb.res5):
-            for blk in stage.layers:
-                r = _train_bottleneck(blk, r, prec)
-            stages.append(r)
-        r3, r4, r5 = stages
-
-        # FPN (nearest 2x top-down add fused into the lateral conv), P6 = stride-2 subsample of P5
-        fp = self.fpn
-        p5_1x1 = conv(fp.fpn_p5_1x1, r5)
-        p4_plus = conv(fp.fpn_p4_1x1, r4, residual=p5_1x1, residual_up2=True)
-        p3_plus = conv(fp.fpn_p3_1x1, r3, residual=p4_plus, residual_up2=True)
-        p2_plus = conv(fp.fpn_p2_1x1, r2, residual=p3_plus, residual_up2=True)
-        p2, p3, p4, p5 = (conv(m, t, padding=1) for m, t in ((fp.fpn_p2, p2_plus), (fp.fpn_p3, p3_plus),
-                                                               (fp.fpn_p4, p4_plus), (fp.fpn_p5, p5_1x1)))
-        p6 = p5[:, :, ::2, ::2]
-
-        # RPN: shared 3x3 + ReLU, separate 1x1 heads (the logits feed the loss)
-        rp = self.rpn
+        r2, r3, r4, r5 = self.resnet_backbone.forward_train(x, prec)
+        p2, p3, p4, p5, p6 = self.fpn.forward_train(r2, r3, r4, r5, prec)
         rpn_score, rpn_bbox = [], []
         for feat in (p2, p3, p4, p5, p6):
-            t = conv(rp.conv_proposal[0], feat, padding=1, relu=True)
-            rpn_score.append(conv(rp.cls_score, t))
-            rpn_bbox.append(conv(rp.bbox_pred, t))
+            score, bbox = self.rpn.forward_train(feat, prec)
+            rpn_score.append(score)
+            rpn_bbox.append(bbox)
         with torch.no_grad():
             rois, _ = self.pyramid_proposal_train([torch.sigmoid(s.detach()) for s in rpn_score], [b.detach() for b in rpn_bbox], im_info[0])
-            targets = T.ProposalTargets(num_classes=self.num_reg_classes, batch_rois=cfg.batch_rois,
-                                        fg_fraction=cfg.fg_fraction, bbox_reg_weights=cfg.bbox_reg_weights,
-                                        mask_size=cfg.mask_size).from_roidb(rois, lab["roidb"], im_info)
+            targets = training.ProposalTargets(num_classes=self.num_reg_classes, batch_rois=cfg.batch_rois,
+                                               fg_fraction=cfg.fg_fraction, bbox_reg_weights=cfg.bbox_reg_weights,
+                                               mask_size=cfg.mask_size).from_roidb(rois, lab["roidb"], im_info)
         (s_rois, cls_label, bbox_target, bbox_iw, bbox_ow, mask_rois, mask_target, _, _) = targets
-
-        # semantic head: per-level subnet and 1x1 score slice, summed at P2 resolution
-        head = self.fcn_head
-        w = head.score.weight
-        scores = []
-        for l, feat in enumerate((p2, p3, p4, p5)):
-            for i in range(head.fcn_subnet.num_layers):
-                feat = F.relu(head.fcn_subnet.conv[i][0](feat))
-            scores.append(T.conv2d(feat, w[:, 128 * l:128 * (l + 1)], head.score.bias if l == 0 else None,
-                                   precision=prec))
-        fcn_score = T.FcnScoreFuseFunction.apply(*scores)
+        fcn_score = self.fcn_head.forward_train(p2, p3, p4, p5, prec)
 
         # instance head
         levels = [p2, p3, p4, p5]
-        rc = self.rcnn
-        pool = T.FPNRoIAlignFunction.apply(s_rois, rc.pool_size, rc.pool_size, rc.roi_pooling.spatial_scale, 2, *levels)
-        fc6 = T.linear(pool.reshape(pool.shape[0], -1), rc.fc6[0].weight, rc.fc6[0].bias, relu=True, precision=prec)
-        fc7 = T.linear(fc6, rc.fc7[0].weight, rc.fc7[0].bias, relu=True, precision=prec)
-        cls_score = T.linear(fc7, rc.cls_score.weight, rc.cls_score.bias, precision=prec)
-        bbox_pred = T.linear(fc7, rc.bbox_pred.weight, rc.bbox_pred.bias, precision=prec)
-        mask_score = _train_mask_branch(self.mask_branch, levels, mask_rois, prec)
-        cls_loss, bbox_loss, mask_loss, rcnn_acc = T.MaskRCNNLoss(cfg.batch_rois)(
+        cls_score, bbox_pred = self.rcnn.forward_train(levels, s_rois, prec)
+        mask_score = self.mask_branch.forward_train(levels, mask_rois, prec)
+        cls_loss, bbox_loss, mask_loss, rcnn_acc = training.MaskRCNNLoss(cfg.batch_rois)(
             cls_score, bbox_pred, mask_score, cls_label, bbox_target, bbox_iw, bbox_ow, mask_target)
-        rpn_cls_loss, rpn_bbox_loss = T.RPNLoss(rpn_batch_size=cfg.rpn_batch_size)(rpn_score, rpn_bbox, lab)
-        fcn_loss = T.SemanticLoss()(fcn_score, lab["seg_gt"])
+        rpn_cls_loss, rpn_bbox_loss = training.RPNLoss(rpn_batch_size=cfg.rpn_batch_size)(rpn_score, rpn_bbox, lab)
+        fcn_loss = training.SemanticLoss()(fcn_score, lab["seg_gt"])
 
         # panoptic head on the ground-truth boxes
-        gt_rois, cls_idx = T.gt_rois(lab["roidb"], im_info[0, 2], dev)
-        keep = T.draw_keep(gt_rois.shape[0], cfg.panoptic_box_keep_fraction) if self.enable_void else None
+        gt_rois, cls_idx = training.gt_rois(lab["roidb"], im_info[0, 2], dev)
+        keep = training.draw_keep(gt_rois.shape[0], cfg.panoptic_box_keep_fraction) if self.enable_void else None
         if keep is not None:
             kd = torch.from_numpy(keep).to(dev)
             gt_rois, cls_idx = gt_rois[kd], cls_idx[kd]
-        pan_mask = _train_mask_branch(self.mask_branch, levels, gt_rois, prec)
-        pan = T.PanopticLoss(num_seg_classes=self.num_seg_classes, num_classes=self.num_classes,
-                             enable_void=self.enable_void, mask_size=cfg.mask_size)
+        pan_mask = self.mask_branch.forward_train(levels, gt_rois, prec)
+        pan = training.PanopticLoss(num_seg_classes=self.num_seg_classes, num_classes=self.num_classes,
+                                    enable_void=self.enable_void, mask_size=cfg.mask_size)
         panoptic_loss, panoptic_acc = pan(fcn_score, pan_mask, gt_rois, cls_idx, lab["seg_gt_4x"], lab["mask_gt"], keep)
 
         out = {"rpn_cls_loss": rpn_cls_loss, "rpn_bbox_loss": rpn_bbox_loss, "cls_loss": cls_loss, "bbox_loss": bbox_loss,
@@ -1044,51 +1084,9 @@ class resnet_upsnet(nn.Module):
         out = {k: v.reshape(1) for k, v in out.items()}
         if getattr(self, "keep_intermediates", False):   # the discrete decisions of the step, for an oracle replay
             out["_intermediates"] = {
-                "rois": rois, "proposal_targets": dict(zip(T.ProposalTargets.NAMES, targets)), "gt_rois": gt_rois,
+                "rois": rois, "proposal_targets": dict(zip(training.ProposalTargets.NAMES, targets)), "gt_rois": gt_rois,
                 "cls_idx": cls_idx, "keep_inds": keep, "fpn": [f.detach() for f in (p2, p3, p4, p5, p6)]}
         return out
-
-
-def _fold_bn_train(conv_w, bn):
-    """Frozen BatchNorm folded for a training conv: (conv_w * scale, shift), differentiable in conv_w only."""
-    with torch.no_grad():
-        scale = bn.weight / torch.sqrt(bn.running_var + bn.eps)
-        shift = (bn.bias - bn.running_mean * scale).contiguous()
-    return conv_w * scale.view(-1, 1, 1, 1), shift
-
-
-def _train_bottleneck(b, x, prec):
-    """Bottleneck.forward with device gradients (training.conv2d; DCN through Offset/DeformConvFunction)."""
-    from . import training as T
-    w1, b1 = _fold_bn_train(b.conv1.weight, b.bn1)
-    out = T.conv2d(x, w1, b1, stride=b.stride, relu=True, precision=prec)
-    w2, b2 = _fold_bn_train(b.conv2.weight, b.bn2)
-    if b.deformable:
-        offset = T.OffsetConvFunction.apply(out, b.conv2_offset.weight, b.conv2_offset.bias)
-        out = F.relu(T.DeformConvFunction.apply(out, offset, w2, b2, 1, b.dilation, b.dilation))
-    else:
-        out = T.conv2d(out, w2, b2, 1, b.dilation, b.dilation, relu=True, precision=prec)
-    residual = x
-    if b.downsample is not None:
-        wd, bd = _fold_bn_train(b.downsample[0].weight, b.downsample[1])
-        residual = T.conv2d(x, wd, bd, stride=b.stride, precision=prec)
-    w3, b3 = _fold_bn_train(b.conv3.weight, b.bn3)
-    return T.conv2d(out, w3, b3, residual=residual, relu=True, precision=prec)
-
-
-def _train_mask_branch(mb, levels, rois, prec):
-    """MaskBranch.forward with device gradients: ROIAlign 14x14, 4 x (3x3 + ReLU), 2x2 deconv + ReLU, 1x1 score."""
-    from . import training as T
-    M = mb.roi_pooling.pooled_height
-    if rois.shape[0] == 0:
-        return levels[0].new_zeros((0, mb.mask_score.weight.shape[0], 2 * M, 2 * M))
-    x = T.FPNRoIAlignFunction.apply(rois, M, M, mb.roi_pooling.spatial_scale, 2, *levels)
-    for i in range(1, 5):
-        c = getattr(mb, "mask_conv%d" % i)[0]
-        x = T.conv2d(x, c.weight, c.bias, padding=1, relu=True, precision=prec)
-    d = mb.mask_deconv1[0]
-    x = T.conv_transpose2x2(x, d.weight, d.bias, relu=True, precision=prec)
-    return T.conv2d(x, mb.mask_score.weight, mb.mask_score.bias, precision=prec)
 
 
 def resnet_50_upsnet(cfg=None):

@@ -155,10 +155,10 @@ import weakref
 
 
 def _per_weight(cache, weight, make, device=None, versioned=True):
-    """make() once per weight tensor, kept in `cache`: id(tensor) -> (weakref to the tensor, version, value).
-    Keyed on the weight TENSOR OBJECT (weak): a data_ptr key would alias a freed weight whose storage the caching
-    allocator handed to a new tensor.  Entries die with their tensor; with `versioned`, _version catches in-place
-    updates; with `device`, a value (None allowed) made for another device is made again."""
+    """make() once per weight tensor, kept in `cache` (made by _weight_cache): id(tensor) -> (weakref to the tensor,
+    version, value).  Keyed on the weight TENSOR OBJECT (weak): a data_ptr key would alias a freed weight whose storage
+    the caching allocator handed to a new tensor.  Entries die with their tensor; with `versioned`, _version catches
+    in-place updates; with `device`, a value (None allowed) made for another device is made again."""
     hit = cache.get(id(weight))
     if (hit is not None and hit[0]() is weight and (not versioned or hit[1] == weight._version) and
             (device is None or hit[2] is None or hit[2].device == device)):
@@ -167,6 +167,26 @@ def _per_weight(cache, weight, make, device=None, versioned=True):
     wid = id(weight)
     cache[wid] = (weakref.ref(weight, lambda _r, _k=wid: cache.pop(_k, None)), weight._version, value)
     return value
+
+
+_weight_caches = []
+
+
+def _weight_cache():
+    """A new cache for _per_weight, recorded so that forget_packed reaches it."""
+    cache = {}
+    _weight_caches.append(cache)
+    return cache
+
+
+def forget_packed(tensors):
+    """Drop what every per-weight cache holds for `tensors`; it is made again, once, on next use.  The version check
+    misses writes that bypass the tensor's version counter, such as an optimiser step replayed from a CUDA graph, so
+    a model forgets its parameters wherever they may have changed that way."""
+    ids = [id(t) for t in tensors]
+    for cache in _weight_caches:
+        for i in ids:
+            cache.pop(i, None)
 
 
 def _packed(cache, weight, pack, nbytes, nbytes_args, unsupported=False):
@@ -184,7 +204,7 @@ def _packed(cache, weight, pack, nbytes, nbytes_args, unsupported=False):
     return _per_weight(cache, weight, make, device=weight.device)
 
 
-_packed_cache = {}
+_packed_cache = _weight_cache()
 
 
 def _packed_weight(weight):
@@ -192,7 +212,7 @@ def _packed_weight(weight):
     return _packed(_packed_cache, weight, "igemm_pack_weight", "igemm_packed_weight_bytes", weight.shape)
 
 
-_dcn_packed_cache = {}
+_dcn_packed_cache = _weight_cache()
 
 
 def _packed_weight_dcn(weight):
@@ -223,7 +243,7 @@ def _dcn_window(x, offset, mask, weight, bias, padding, dilation, relu):
     return None if rc == _lib.E_UNSUPPORTED else Pair(store)
 
 
-_stem_cache = {}   # packed bf16 [Cout][kh][8][8] per weight
+_stem_cache = _weight_cache()   # packed bf16 [Cout][kh][8][8] per weight
 _stem_ws = None
 
 
@@ -409,7 +429,7 @@ def linear(x, weight, bias=None, relu=False, precision=None, out_dtype=None):
     return y if isinstance(y, Pair) else y.reshape(N, weight.shape[0])
 
 
-_view_cache = {}
+_view_cache = _weight_cache()
 
 
 def _as_1x1(weight):

@@ -57,6 +57,7 @@ from torch.optim.optimizer import required
 
 from . import _lib
 from ._lib import call, f32c, query_bytes, require_cuda
+from .operators import _weight_cache
 
 
 def _conv_out(n, pad, dil, k, stride):
@@ -226,7 +227,7 @@ class FPNRoIAlignFunction(torch.autograd.Function):
 # dense convolutions and FC layers with device gradients (csrc/conv_backward.cu)
 # ------------------------------------------------------------------------------------------------
 _CONV_PREC = {"bf16x3": _lib.PREC_BF16X3, "bf16": _lib.PREC_BF16}
-_dgrad_cache = {}
+_dgrad_cache = _weight_cache()
 
 
 def _conv_prec(precision):
