@@ -711,6 +711,41 @@ int upsnet_semantic_loss_backward(const float *fcn_score, int S, int h, int w, c
                                   const float *lse, const int *counts, const float *grad_out, float *d_fcn_score,
                                   void *stream);
 
+/* upsnet_fcn_roi_loss_forward / _backward: the semantic head's ROI loss of one image (train.fcn_with_roi_loss).
+ * replaces: models/fcn.py:102-106 roi_score = score(RoIAlign(M, M, spatial_scale)(feat, rois)), feat the 512-channel
+ *           concat of the four up-sampled levels, and models/resnet_upsnet.py:132-134
+ *           CrossEntropyLoss(ignore_index=255, reduce=False)(roi_score, seg_roi_gt).mean(), with autograd's backward.
+ *           The score conv and ROIAlign commute, so the loss samples the S-plane fcn_score (the score conv's output,
+ *           bias included) instead: neither feat, the [R,512,M,M] roi features nor their gradients are built.
+ * Inputs (device): fcn_score float32 [S,h,w]; bias float32 [S] (the score conv's); rois float32 [R,5] in image
+ *   coordinates (column 0, the batch index, is not read: one image); seg_roi_gt [R,M,M], uint8 or int64
+ *   (seg_roi_gt_is_int64).  The roi score of cell (r, ph, pw), channel c, is ROIAlign of plane c by the forward rule of
+ *   upsnet_roi_align_forward (roi_sample.cuh, aligned=False, sampling_ratio x sampling_ratio samples) plus
+ *   bias[c] * (1 - n_inside / count): ROIAlign gives a sample outside the map 0, so sampling fcn_score carries only
+ *   n_inside / count of the bias that the reference adds once per cell.  The term is 0 for every cell whose samples are
+ *   inside the map.
+ * Outputs (device): loss[1] = sum over cells whose target t is in 0..S-1 of (log-sum-exp - roi score of t), divided by
+ *   R*M*M (reduce=False then mean: ignored cells count in the denominator); counts int32 [2] = (cells with a target,
+ *   cells whose target is neither 255 nor in 0..S-1: no loss and no gradient); lse float32 [R*M*M], what backward reads.
+ * Backward: lse (forward's) and grad_out float32 [1] on the device; d_fcn_score float32 [S,h,w], every element written
+ *   (0 where no roi samples): the transpose of the sampling applied to (softmax - onehot) * grad_out / (R*M*M), as a
+ *   gather over the rois in order with the forward's tap weights; d_bias float32 [S], the gradient of the correction
+ *   term alone (the caller adds it to what the bias receives through fcn_score).  No atomics.
+ * Same inputs give the same bytes; no call synchronises or reads the device; both are capturable.
+ * Limits: 1 <= R <= 1024, M <= 64, sampling_ratio = 2, S*h*w < 2^31, S*R*M*M < 2^31, S <= 32767 (else
+ *   UPSNET_E_UNSUPPORTED, before any launch).
+ * Workspace: upsnet_fcn_roi_loss_workspace_bytes(S, R, M, backward) (UPSNET_E_UNSUPPORTED for R or M beyond the
+ *   limits): backward = 0 for the forward's (block partials), 1 for the backward's (4*S*R*M*M bytes of roi-score gradient plus 4*R*M*M); nothing in it outlives the call. */
+int upsnet_fcn_roi_loss_workspace_bytes(int S, int R, int M, int backward, size_t *bytes);
+int upsnet_fcn_roi_loss_forward(const float *fcn_score, const float *bias, int S, int h, int w, const float *rois, int R,
+                                const void *seg_roi_gt, int seg_roi_gt_is_int64, int M, int sampling_ratio,
+                                float spatial_scale, float *loss, int *counts, float *lse, void *workspace,
+                                size_t workspace_bytes, void *stream);
+int upsnet_fcn_roi_loss_backward(const float *fcn_score, const float *bias, int S, int h, int w, const float *rois, int R,
+                                 const void *seg_roi_gt, int seg_roi_gt_is_int64, int M, int sampling_ratio,
+                                 float spatial_scale, const float *lse, const float *grad_out, float *d_fcn_score,
+                                 float *d_bias, void *workspace, size_t workspace_bytes, void *stream);
+
 /* upsnet_rpn_loss_forward / _backward: the RPN loss of one image over all FPN levels in one launch.
  * replaces: models/rpn.py:60-92 RPNLoss.forward (with_fpn): per level, the [:, :, :h, :w] slices of the label maps,
  *           F.binary_cross_entropy_with_logits(score, label, weight = label != -1, reduction='sum') / rpn_batch_size

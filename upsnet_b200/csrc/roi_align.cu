@@ -14,6 +14,7 @@
 
 #include "common.cuh"
 #include "pair.cuh"
+#include "roi_sample.cuh"
 
 namespace ups {
 
@@ -37,31 +38,6 @@ __device__ __forceinline__ int fpn_level_of(float x1, float y1, float x2, float 
   return (x >= t1) + (x >= t2) + (x >= t3);
 }
 
-struct SamplePos {
-  int o00, o01, o10, o11;  // element offsets (in pixels) of the four taps
-  float w00, w01, w10, w11;
-};
-
-// roi_align_kernel.cu:43-95 -- returns weights/offsets instead of the value so that the NHWC
-// kernel can reuse them across channels.  An out-of-range sample has all weights 0.
-__device__ __forceinline__ SamplePos roi_sample(int H, int W, float y, float x) {
-  SamplePos s;
-  if (y < -1.0f || y > (float)H || x < -1.0f || x > (float)W) {
-    s.o00 = s.o01 = s.o10 = s.o11 = 0;
-    s.w00 = s.w01 = s.w10 = s.w11 = 0.f;
-    return s;
-  }
-  if (y <= 0) y = 0;
-  if (x <= 0) x = 0;
-  int yl = (int)y, xl = (int)x, yh, xh;
-  if (yl >= H - 1) { yh = yl = H - 1; y = (float)yl; } else yh = yl + 1;
-  if (xl >= W - 1) { xh = xl = W - 1; x = (float)xl; } else xh = xl + 1;
-  const float ly = y - yl, lx = x - xl, hy = 1.f - ly, hx = 1.f - lx;
-  s.o00 = yl * W + xl; s.o01 = yl * W + xh; s.o10 = yh * W + xl; s.o11 = yh * W + xh;
-  s.w00 = hy * hx; s.w01 = hy * lx; s.w10 = ly * hx; s.w11 = ly * lx;
-  return s;
-}
-
 // ------------------------------------------------------------------------------------------
 // NCHW: thread per output element (n, c, ph, pw)
 // ------------------------------------------------------------------------------------------
@@ -82,16 +58,14 @@ roi_align_nchw_kernel(FpnFeats f, int C, const float* __restrict__ rois, int R, 
     if (levels_out && c == 0 && ph == 0 && pw == 0) levels_out[n] = lv;
     const int H = f.H[lv], W = f.W[lv];
     const float sc = f.scale[lv];
-    const float rsw = rx1 * sc, rsh = ry1 * sc, rew = rx2 * sc, reh = ry2 * sc;
-    const float rw = fmaxf(rew - rsw, 1.f), rh = fmaxf(reh - rsh, 1.f);
-    const float bsh = rh / (float)PH, bsw = rw / (float)PW;
-    const int gh = sr > 0 ? sr : (int)ceilf(rh / PH), gw = sr > 0 ? sr : (int)ceilf(rw / PW);
+    const RoiBins g = roi_bins(rx1, ry1, rx2, ry2, sc, PH, PW);
+    const int gh = sr > 0 ? sr : (int)ceilf(g.bsh), gw = sr > 0 ? sr : (int)ceilf(g.bsw);
     const float* d = reinterpret_cast<const float*>(f.p[lv]) + ((size_t)b * C + c) * H * W;
     float acc = 0.f;
     for (int iy = 0; iy < gh; ++iy) {
-      const float y = rsh + ph * bsh + (float)(iy + .5f) * bsh / (float)gh;
+      const float y = roi_sample_coord(g.rsh, ph, g.bsh, iy, gh);
       for (int ix = 0; ix < gw; ++ix) {
-        const float x = rsw + pw * bsw + (float)(ix + .5f) * bsw / (float)gw;
+        const float x = roi_sample_coord(g.rsw, pw, g.bsw, ix, gw);
         const SamplePos s = roi_sample(H, W, y, x);
         acc += (s.w00 * __ldg(d + s.o00) + s.w01 * __ldg(d + s.o01) + s.w10 * __ldg(d + s.o10) +
                 s.w11 * __ldg(d + s.o11));
@@ -116,10 +90,8 @@ roi_align_nhwc_kernel(FpnFeats f, int C, const float* __restrict__ rois, int R, 
   if (levels_out && ph == 0 && threadIdx.x == 0) levels_out[n] = lv;
   const int H = f.H[lv], W = f.W[lv];
   const float sc = f.scale[lv];
-  const float rsw = rx1 * sc, rsh = ry1 * sc, rew = rx2 * sc, reh = ry2 * sc;
-  const float rw = fmaxf(rew - rsw, 1.f), rh = fmaxf(reh - rsh, 1.f);
-  const float bsh = rh / (float)PH, bsw = rw / (float)PW;
-  const int gh = sr > 0 ? sr : (int)ceilf(rh / PH), gw = sr > 0 ? sr : (int)ceilf(rw / PW);
+  const RoiBins g = roi_bins(rx1, ry1, rx2, ry2, sc, PH, PW);
+  const int gh = sr > 0 ? sr : (int)ceilf(g.bsh), gw = sr > 0 ? sr : (int)ceilf(g.bsw);
   const float inv_count_div = (float)(gh * gw);
   const float* base = reinterpret_cast<const float*>(f.p[lv]) + (size_t)b * H * W * C;
   for (int c = threadIdx.x * VEC; c < C; c += blockDim.x * VEC) {
@@ -128,9 +100,9 @@ roi_align_nhwc_kernel(FpnFeats f, int C, const float* __restrict__ rois, int R, 
 #pragma unroll
       for (int v = 0; v < VEC; ++v) acc[v] = 0.f;
       for (int iy = 0; iy < gh; ++iy) {
-        const float y = rsh + ph * bsh + (float)(iy + .5f) * bsh / (float)gh;
+        const float y = roi_sample_coord(g.rsh, ph, g.bsh, iy, gh);
         for (int ix = 0; ix < gw; ++ix) {
-          const float x = rsw + pw * bsw + (float)(ix + .5f) * bsw / (float)gw;
+          const float x = roi_sample_coord(g.rsw, pw, g.bsw, ix, gw);
           const SamplePos s = roi_sample(H, W, y, x);
           if (VEC == 4) {
             const float4 v00 = __ldg((const float4*)(base + (size_t)s.o00 * C + c));
@@ -175,19 +147,17 @@ roi_align_nhwc_bf16_kernel(FpnFeats f, int C, const float* __restrict__ rois, in
   if (levels_out && ph == 0 && threadIdx.x == 0) levels_out[n] = lv;
   const int H = f.H[lv], W = f.W[lv];
   const float sc = f.scale[lv];
-  const float rsw = rx1 * sc, rsh = ry1 * sc, rew = rx2 * sc, reh = ry2 * sc;
-  const float rw = fmaxf(rew - rsw, 1.f), rh = fmaxf(reh - rsh, 1.f);
-  const float bsh = rh / (float)PH, bsw = rw / (float)PW;
-  const int gh = sr > 0 ? sr : (int)ceilf(rh / PH), gw = sr > 0 ? sr : (int)ceilf(rw / PW);
+  const RoiBins g = roi_bins(rx1, ry1, rx2, ry2, sc, PH, PW);
+  const int gh = sr > 0 ? sr : (int)ceilf(g.bsh), gw = sr > 0 ? sr : (int)ceilf(g.bsw);
   const float cnt = (float)(gh * gw);
   const __nv_bfloat16* base = reinterpret_cast<const __nv_bfloat16*>(f.p[lv]) + (size_t)b * H * W * C;
   for (int c = threadIdx.x * 4; c < C; c += blockDim.x * 4) {
     for (int pw = 0; pw < PW; ++pw) {
       float acc[4] = {0.f, 0.f, 0.f, 0.f};
       for (int iy = 0; iy < gh; ++iy) {
-        const float y = rsh + ph * bsh + (float)(iy + .5f) * bsh / (float)gh;
+        const float y = roi_sample_coord(g.rsh, ph, g.bsh, iy, gh);
         for (int ix = 0; ix < gw; ++ix) {
-          const float x = rsw + pw * bsw + (float)(ix + .5f) * bsw / (float)gw;
+          const float x = roi_sample_coord(g.rsw, pw, g.bsw, ix, gw);
           const SamplePos s = roi_sample(H, W, y, x);
           const uint2 v00 = __ldg(reinterpret_cast<const uint2*>(base + (size_t)s.o00 * C + c));
           const uint2 v01 = __ldg(reinterpret_cast<const uint2*>(base + (size_t)s.o01 * C + c));
@@ -225,17 +195,15 @@ roi_align_nhwc_bf16_roi_kernel(FpnFeats f, int C, const float* __restrict__ rois
   if (levels_out && threadIdx.x == 0) levels_out[n] = lv;
   const int H = f.H[lv], W = f.W[lv];
   const float sc = f.scale[lv];
-  const float rsw = rx1 * sc, rsh = ry1 * sc, rew = rx2 * sc, reh = ry2 * sc;
-  const float rw = fmaxf(rew - rsw, 1.f), rh = fmaxf(reh - rsh, 1.f);
-  const float bsh = rh / (float)PH, bsw = rw / (float)PW;
+  const RoiBins g = roi_bins(rx1, ry1, rx2, ry2, sc, PH, PW);
   const int gh = sr, gw = sr;                 // launcher guarantees sr > 0 and PH*PW*sr*sr <= kRoiMaxSamples
   const float cnt = (float)(gh * gw);
   const int per_bin = gh * gw, nsamp = PH * PW * per_bin;
   for (int t = threadIdx.x; t < nsamp; t += blockDim.x) {
     const int bin = t / per_bin, q = t - bin * per_bin;
     const int ph = bin / PW, pw = bin - ph * PW, iy = q / gw, ix = q - iy * gw;
-    const float y = rsh + ph * bsh + (float)(iy + .5f) * bsh / (float)gh;
-    const float x = rsw + pw * bsw + (float)(ix + .5f) * bsw / (float)gw;
+    const float y = roi_sample_coord(g.rsh, ph, g.bsh, iy, gh);
+    const float x = roi_sample_coord(g.rsw, pw, g.bsw, ix, gw);
     const SamplePos sp = roi_sample(H, W, y, x);
     s_off[t] = make_int4(sp.o00 * C, sp.o01 * C, sp.o10 * C, sp.o11 * C);
     s_w[t] = make_float4(sp.w00, sp.w01, sp.w10, sp.w11);
@@ -288,17 +256,15 @@ roi_align_nhwc_pair_roi_kernel(FpnFeats f, int C, const float* __restrict__ rois
   if (levels_out && threadIdx.x == 0) levels_out[n] = lv;
   const int H = f.H[lv], W = f.W[lv];
   const float sc = f.scale[lv];
-  const float rsw = rx1 * sc, rsh = ry1 * sc, rew = rx2 * sc, reh = ry2 * sc;
-  const float rw = fmaxf(rew - rsw, 1.f), rh = fmaxf(reh - rsh, 1.f);
-  const float bsh = rh / (float)PH, bsw = rw / (float)PW;
+  const RoiBins g = roi_bins(rx1, ry1, rx2, ry2, sc, PH, PW);
   const int gh = sr, gw = sr;
   const float cnt = (float)(gh * gw);
   const int per_bin = gh * gw, nsamp = PH * PW * per_bin;
   for (int t = threadIdx.x; t < nsamp; t += blockDim.x) {
     const int bin = t / per_bin, q = t - bin * per_bin;
     const int ph = bin / PW, pw = bin - ph * PW, iy = q / gw, ix = q - iy * gw;
-    const float y = rsh + ph * bsh + (float)(iy + .5f) * bsh / (float)gh;
-    const float x = rsw + pw * bsw + (float)(ix + .5f) * bsw / (float)gw;
+    const float y = roi_sample_coord(g.rsh, ph, g.bsh, iy, gh);
+    const float x = roi_sample_coord(g.rsw, pw, g.bsw, ix, gw);
     const SamplePos sp = roi_sample(H, W, y, x);
     s_off[t] = make_int4(sp.o00 * 2 * C, sp.o01 * 2 * C, sp.o10 * 2 * C, sp.o11 * 2 * C);
     s_w[t] = make_float4(sp.w00, sp.w01, sp.w10, sp.w11);

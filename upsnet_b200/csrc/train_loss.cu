@@ -6,10 +6,17 @@
 // log-sum-exp of every output pixel (4 bytes) for backward; backward is the transpose of the up-sampling applied to the
 // per-pixel softmax gradient, computed as a gather over a source tile and its output halo in shared memory.
 //
+// FCN ROI loss (train.fcn_with_roi_loss, models/fcn.py:102-106 + models/resnet_upsnet.py:132-134): the cross-entropy of
+// the score conv applied to RoIAlign(28x28, 1/4) of the 512-channel concat of the semantic head.  The score conv and
+// ROIAlign are both linear and act on different axes, so the loss samples the S-plane fcn_score instead (plus the share
+// of the score bias that ROIAlign's out-of-map zeros remove); backward is a gather over the ROI samples that reach each
+// fcn_score pixel, the taps re-derived with the forward's rule (roi_sample.cuh).
+//
 // Determinism: every output element has one owner thread that sums in a fixed order; the scalar losses go through
 // per-block partials and a fixed-order second stage.  There is no atomic in this file.
 #include "common.cuh"
 #include "cta.cuh"
+#include "roi_sample.cuh"
 #include "up4.cuh"
 
 namespace ups {
@@ -533,6 +540,226 @@ int mr_args(MrArgs& a, const float* cls_score, const int64_t* cls_label, int R, 
   return 0;
 }
 
+
+// ================================================================================================
+// FCN ROI loss
+// ================================================================================================
+constexpr int kFrSr = 2;            // sampling ratio: the four samples of a cell stay in registers
+constexpr int kFrSamples = kFrSr * kFrSr;
+constexpr int kFrMaxR = 1024;       // rois; their bin geometry fits the gather's shared memory
+constexpr int kFrMaxM = 64;
+constexpr int kFrCh = 8;            // channels per thread of the backward gather
+
+struct FrCell {
+  SamplePos s[kFrSamples];
+  float corr;                       // 1 - n_inside / count: the share of the score bias that sampling fcn_score misses
+};
+
+__device__ __forceinline__ RoiBins fr_bins(const float* rois, int r, int M, float sc) {
+  const float* q = rois + (size_t)r * 5;
+  return roi_bins(__ldg(q + 1), __ldg(q + 2), __ldg(q + 3), __ldg(q + 4), sc, M, M);
+}
+
+// the samples of cell (ph, pw) of a roi, by roi_align_nchw_kernel's rule
+__device__ __forceinline__ FrCell fr_cell(const RoiBins& g, int ph, int pw, int h, int w) {
+  FrCell c;
+  int inside = 0;
+#pragma unroll
+  for (int iy = 0; iy < kFrSr; ++iy) {
+    const float y = roi_sample_coord(g.rsh, ph, g.bsh, iy, kFrSr);
+#pragma unroll
+    for (int ix = 0; ix < kFrSr; ++ix) {
+      const float x = roi_sample_coord(g.rsw, pw, g.bsw, ix, kFrSr);
+      c.s[iy * kFrSr + ix] = roi_sample(h, w, y, x);
+      inside += roi_sample_inside(h, w, y, x);
+    }
+  }
+  c.corr = 1.f - (float)inside / (float)kFrSamples;
+  return c;
+}
+
+// the reference's roi score of one channel: RoIAlign of the plane pl, plus bias * corr (exactly 0 inside the map)
+__device__ __forceinline__ float fr_value(const FrCell& c, const float* __restrict__ pl, float bias) {
+  float acc = 0.f;
+#pragma unroll
+  for (int q = 0; q < kFrSamples; ++q) {
+    const SamplePos& s = c.s[q];
+    acc += (s.w00 * __ldg(pl + s.o00) + s.w01 * __ldg(pl + s.o01) + s.w10 * __ldg(pl + s.o10) + s.w11 * __ldg(pl + s.o11));
+  }
+  return acc / (float)kFrSamples + bias * c.corr;
+}
+
+// one thread per roi cell: streaming log-sum-exp over the S roi scores, the loss of a cell with a target
+template <typename LT>
+__global__ void __launch_bounds__(kTlThreads) fr_forward_kernel(const float* __restrict__ fcn, const float* __restrict__ bias,
+                                                               int S, int h, int w, const float* __restrict__ rois, int R,
+                                                               int M, float sc, const LT* __restrict__ gt,
+                                                               float* __restrict__ lse, double* part_d, int* part_i) {
+  const int i = blockIdx.x * kTlThreads + threadIdx.x, mm = M * M;
+  double d[1] = {0.0};
+  int n[2] = {0, 0};
+  if (i < R * mm) {
+    const int t = sem_target<LT>(gt, i, S);
+    n[0] = t >= 0;
+    n[1] = t == kSemInvalid;
+    float l = 0.f;
+    if (t >= 0) {
+      const int r = i / mm, p = i - r * mm, ph = p / M, pw = p - ph * M;
+      const FrCell c = fr_cell(fr_bins(rois, r, M, sc), ph, pw, h, w);
+      const size_t hw = (size_t)h * w;
+      float m = -INFINITY, s = 0.f, lt = 0.f;
+      for (int ch = 0; ch < S; ++ch) {
+        const float v = fr_value(c, fcn + ch * hw, __ldg(bias + ch));
+        if (v > m) { s = __fmaf_rn(s, expf(m - v), 1.f); m = v; }
+        else s += expf(v - m);
+        if (ch == t) lt = v;
+      }
+      l = m + logf(s);
+      d[0] = (double)(l - lt);
+    }
+    lse[i] = l;
+  }
+  cta_partials<kTlThreads, 1, 2>(d, n, part_d, part_i);
+}
+
+__global__ void __launch_bounds__(kTlThreads) fr_finish_kernel(const double* part_d, const int* part_i, int nblocks, int cells,
+                                                               float* loss, int* counts) {
+  double d[1];
+  int n[2];
+  cta_sum_partials<kTlThreads, 1, 2>(part_d, part_i, nblocks, d, n);
+  if (threadIdx.x == 0) {
+    *loss = (float)(d[0] / (double)cells);      // reduce=False + .mean(): ignored cells count in the denominator
+    counts[0] = n[0];
+    counts[1] = n[1];
+  }
+}
+
+// backward, pass 1: gc[ch][cell] = (softmax_ch - [ch = t]) * grad_out / cells, channel-major; corr[cell] for d bias
+template <typename LT>
+__global__ void __launch_bounds__(kTlThreads) fr_grad_kernel(const float* __restrict__ fcn, const float* __restrict__ bias,
+                                                            int S, int h, int w, const float* __restrict__ rois, int R, int M,
+                                                            float sc, const LT* __restrict__ gt, const float* __restrict__ lse,
+                                                            const float* __restrict__ grad_out, float* __restrict__ gc,
+                                                            float* __restrict__ corr) {
+  const int i = blockIdx.x * kTlThreads + threadIdx.x, mm = M * M, cells = R * mm;
+  if (i >= cells) return;
+  const int t = sem_target<LT>(gt, i, S);
+  if (t < 0) {
+    for (int ch = 0; ch < S; ++ch) gc[(size_t)ch * cells + i] = 0.f;
+    corr[i] = 0.f;
+    return;
+  }
+  const int r = i / mm, p = i - r * mm, ph = p / M, pw = p - ph * M;
+  const FrCell c = fr_cell(fr_bins(rois, r, M, sc), ph, pw, h, w);
+  const size_t hw = (size_t)h * w;
+  const float l = lse[i], scale = __fdiv_rn(*grad_out, (float)cells);
+  for (int ch = 0; ch < S; ++ch) {
+    const float v = fr_value(c, fcn + ch * hw, __ldg(bias + ch));
+    gc[(size_t)ch * cells + i] = __fmul_rn(expf(v - l) - (ch == t ? 1.f : 0.f), scale);
+  }
+  corr[i] = c.corr;
+}
+
+// a candidate sample index, kept in [-2, K] before the conversion to int (far rois give huge quotients)
+__device__ __forceinline__ float fr_clampk(float k, int K) { return fminf(fmaxf(k, -2.f), (float)K); }
+
+// backward, pass 2: d fcn_score[c][y][x] = sum over rois in order, then over the samples whose taps can reach (y, x), of
+// tap weight * gc[c][cell] / count.  A sample reaches row y only if max(sample y, 0) lies in [y-1, y+1) (below 0 it is
+// clamped to 0; at or above h-1 it reads row h-1 alone), so each roi contributes a short range of sample rows and
+// columns; every candidate's taps are re-derived with roi_sample, so the weights are the forward's, bit for bit.
+__global__ void __launch_bounds__(kTlThreads) fr_gather_kernel(const float* __restrict__ gc, const float* __restrict__ rois,
+                                                              int R, int M, float sc, int S, int h, int w,
+                                                              float* __restrict__ dfcn) {
+  __shared__ float4 s_geo[kFrMaxR];
+  __shared__ float2 s_inv[kFrMaxR];     // 1 / sample step along x and y: the candidate ranges need no division
+  for (int r = threadIdx.x; r < R; r += kTlThreads) {
+    const RoiBins g = fr_bins(rois, r, M, sc);
+    s_geo[r] = make_float4(g.rsw, g.rsh, g.bsw, g.bsh);
+    s_inv[r] = make_float2(kFrSr / g.bsw, kFrSr / g.bsh);
+  }
+  __syncthreads();
+  const int pix = blockIdx.x * kTlThreads + threadIdx.x;
+  if (pix >= h * w) return;
+  const int y = pix / w, x = pix - y * w, c0 = blockIdx.y * kFrCh, K = M * kFrSr, cells = R * M * M;
+  const float ylo = y <= 1 ? -1.f : (float)(y - 1), yhi = y == h - 1 ? (float)h : (float)(y + 1);
+  const float xlo = x <= 1 ? -1.f : (float)(x - 1), xhi = x == w - 1 ? (float)w : (float)(x + 1);
+  float acc[kFrCh];
+#pragma unroll
+  for (int j = 0; j < kFrCh; ++j) acc[j] = 0.f;
+  for (int r = 0; r < R; ++r) {
+    const float4 g = s_geo[r];
+    const float2 inv = s_inv[r];
+    // candidate sample indices k = p * kFrSr + i, coordinate ~ start + (k + 0.5) * bin / kFrSr, widened by one (which
+    // also covers the rounding of the reciprocal)
+    const int ky0 = max((int)floorf(fr_clampk((ylo - g.y) * inv.y - 0.5f, K)) - 1, 0);
+    const int ky1 = min((int)ceilf(fr_clampk((yhi - g.y) * inv.y - 0.5f, K)) + 1, K - 1);
+    const int kx0 = max((int)floorf(fr_clampk((xlo - g.x) * inv.x - 0.5f, K)) - 1, 0);
+    const int kx1 = min((int)ceilf(fr_clampk((xhi - g.x) * inv.x - 0.5f, K)) + 1, K - 1);
+    for (int ky = ky0; ky <= ky1; ++ky) {
+      const int ph = ky / kFrSr, iy = ky - ph * kFrSr;
+      const float ys = roi_sample_coord(g.y, ph, g.w, iy, kFrSr);
+      for (int kx = kx0; kx <= kx1; ++kx) {
+        const int pw = kx / kFrSr, ix = kx - pw * kFrSr;
+        const SamplePos s = roi_sample(h, w, ys, roi_sample_coord(g.x, pw, g.z, ix, kFrSr));
+        const float wt = (s.o00 == pix ? s.w00 : 0.f) + (s.o01 == pix ? s.w01 : 0.f) + (s.o10 == pix ? s.w10 : 0.f) +
+                         (s.o11 == pix ? s.w11 : 0.f);
+        if (wt == 0.f) continue;
+        const float* gp = gc + (size_t)c0 * cells + ((size_t)r * M + ph) * M + pw;
+#pragma unroll
+        for (int j = 0; j < kFrCh; ++j)
+          if (c0 + j < S) acc[j] = __fmaf_rn(wt, __ldg(gp + (size_t)j * cells), acc[j]);
+      }
+    }
+  }
+  const size_t hw = (size_t)h * w;
+#pragma unroll
+  for (int j = 0; j < kFrCh; ++j)
+    if (c0 + j < S) dfcn[(c0 + j) * hw + pix] = acc[j] * (1.f / kFrSamples);   // count is a power of two: exact
+}
+
+// backward, pass 3: d bias[c] = sum over cells of gc[c][cell] * corr[cell] (a fixed-order tree per channel)
+__global__ void __launch_bounds__(kTlThreads) fr_dbias_kernel(const float* __restrict__ gc, const float* __restrict__ corr,
+                                                             int cells, float* __restrict__ dbias) {
+  __shared__ float s_a[kTlThreads];
+  const int c = blockIdx.x;
+  float a = 0.f;
+  for (int i = threadIdx.x; i < cells; i += kTlThreads) {
+    const float k = __ldg(corr + i);
+    if (k != 0.f) a = __fmaf_rn(__ldg(gc + (size_t)c * cells + i), k, a);
+  }
+  s_a[threadIdx.x] = a;
+  __syncthreads();
+  for (int o = kTlThreads / 2; o; o >>= 1) {
+    if (threadIdx.x < o) s_a[threadIdx.x] += s_a[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) dbias[c] = s_a[0];
+}
+
+inline size_t fr_layout(int S, int R, int M, int backward, void* base, double** pd, int** pi, float** gc, float** corr) {
+  const long long cells = (long long)R * M * M;
+  WsCarve c(base);
+  if (backward) {
+    *gc = c.take<float>((size_t)S * cells);
+    *corr = c.take<float>((size_t)cells);
+  } else {
+    const int nblocks = tl_blocks(cells);
+    *pd = c.take<double>(nblocks);
+    *pi = c.take<int>((size_t)nblocks * 2);
+  }
+  return c.bytes();
+}
+
+int fr_check(const float* fcn, const float* bias, int S, int h, int w, const float* rois, int R, const void* gt, int M,
+             int sampling_ratio, float spatial_scale) {
+  if (!fcn || !bias || !rois || !gt || S <= 0 || h <= 0 || w <= 0 || R < 0 || M <= 0 || !(spatial_scale > 0.f))
+    return UPSNET_E_BADARG;
+  if (R == 0 || R > kFrMaxR || M > kFrMaxM || sampling_ratio != kFrSr || (size_t)S * h * w >= (1ull << 31) ||
+      (size_t)S * R * M * M >= (1ull << 31) || S > 32767)
+    return UPSNET_E_UNSUPPORTED;
+  return 0;
+}
+
 }  // namespace
 }  // namespace ups
 
@@ -694,6 +921,69 @@ extern "C" int upsnet_mask_rcnn_loss_backward(const float* cls_score, const int6
   a.dcls = d_cls_score; a.dpred = d_bbox_pred; a.dmask = mask_numel > 0 ? d_mask_score : nullptr;
   mr_backward_kernel<<<a.nb_mask + a.nb_bbox + a.nb_cls, kTlThreads, 0, (cudaStream_t)stream>>>(a, counts, grad_cls,
                                                                                                grad_bbox, grad_mask);
+  UPS_CHECK_LAUNCH();
+  return 0;
+}
+
+// ---- FCN ROI loss -------------------------------------------------------------------------------
+extern "C" int upsnet_fcn_roi_loss_workspace_bytes(int S, int R, int M, int backward, size_t* bytes) {
+  if (!bytes || S <= 0 || R < 0 || M <= 0) return UPSNET_E_BADARG;
+  if (R == 0 || R > ups::kFrMaxR || M > ups::kFrMaxM) return UPSNET_E_UNSUPPORTED;
+  double* pd; int* pi; float* gc; float* corr;
+  *bytes = ups::fr_layout(S, R, M, backward, nullptr, &pd, &pi, &gc, &corr);
+  return 0;
+}
+
+extern "C" int upsnet_fcn_roi_loss_forward(const float* fcn_score, const float* bias, int S, int h, int w, const float* rois,
+                                           int R, const void* seg_roi_gt, int seg_roi_gt_is_int64, int M,
+                                           int sampling_ratio, float spatial_scale, float* loss, int* counts, float* lse,
+                                           void* workspace, size_t workspace_bytes, void* stream) {
+  using namespace ups;
+  int rc = fr_check(fcn_score, bias, S, h, w, rois, R, seg_roi_gt, M, sampling_ratio, spatial_scale);
+  if (rc) return rc;
+  if (!loss || !counts || !lse || !workspace) return UPSNET_E_BADARG;
+  double* pd; int* pi; float* gc; float* corr;
+  if (workspace_bytes < fr_layout(S, R, M, 0, workspace, &pd, &pi, &gc, &corr)) return UPSNET_E_WORKSPACE;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int cells = R * M * M, nblocks = tl_blocks(cells);
+  if (seg_roi_gt_is_int64)
+    fr_forward_kernel<int64_t><<<nblocks, kTlThreads, 0, st>>>(fcn_score, bias, S, h, w, rois, R, M, spatial_scale,
+                                                               (const int64_t*)seg_roi_gt, lse, pd, pi);
+  else
+    fr_forward_kernel<unsigned char><<<nblocks, kTlThreads, 0, st>>>(fcn_score, bias, S, h, w, rois, R, M, spatial_scale,
+                                                                     (const unsigned char*)seg_roi_gt, lse, pd, pi);
+  UPS_CHECK_LAUNCH();
+  fr_finish_kernel<<<1, kTlThreads, 0, st>>>(pd, pi, nblocks, cells, loss, counts);
+  UPS_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int upsnet_fcn_roi_loss_backward(const float* fcn_score, const float* bias, int S, int h, int w, const float* rois,
+                                            int R, const void* seg_roi_gt, int seg_roi_gt_is_int64, int M,
+                                            int sampling_ratio, float spatial_scale, const float* lse,
+                                            const float* grad_out, float* d_fcn_score, float* d_bias, void* workspace,
+                                            size_t workspace_bytes, void* stream) {
+  using namespace ups;
+  int rc = fr_check(fcn_score, bias, S, h, w, rois, R, seg_roi_gt, M, sampling_ratio, spatial_scale);
+  if (rc) return rc;
+  if (!lse || !grad_out || !d_fcn_score || !d_bias || !workspace) return UPSNET_E_BADARG;
+  double* pd; int* pi; float* gc; float* corr;
+  if (workspace_bytes < fr_layout(S, R, M, 1, workspace, &pd, &pi, &gc, &corr)) return UPSNET_E_WORKSPACE;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int cells = R * M * M;
+  if (seg_roi_gt_is_int64)
+    fr_grad_kernel<int64_t><<<tl_blocks(cells), kTlThreads, 0, st>>>(fcn_score, bias, S, h, w, rois, R, M, spatial_scale,
+                                                                     (const int64_t*)seg_roi_gt, lse, grad_out, gc, corr);
+  else
+    fr_grad_kernel<unsigned char><<<tl_blocks(cells), kTlThreads, 0, st>>>(fcn_score, bias, S, h, w, rois, R, M,
+                                                                           spatial_scale, (const unsigned char*)seg_roi_gt,
+                                                                           lse, grad_out, gc, corr);
+  UPS_CHECK_LAUNCH();
+  fr_gather_kernel<<<dim3(tl_blocks((long long)h * w), ceil_div(S, kFrCh)), kTlThreads, 0, st>>>(gc, rois, R, M,
+                                                                                                  spatial_scale, S, h, w,
+                                                                                                  d_fcn_score);
+  UPS_CHECK_LAUNCH();
+  fr_dbias_kernel<<<S, kTlThreads, 0, st>>>(gc, corr, cells, d_bias);
   UPS_CHECK_LAUNCH();
   return 0;
 }

@@ -9,12 +9,15 @@ resnet_upsnet}.py running on the sm_90a C ABI.
   panoptic_cls_probs, panoptic_outputs.
 * Frozen BatchNorm (models/resnet.py:69-78: always eval, requires_grad False) is folded into the
   preceding convolution once (prepare()); bias/ReLU/residual live in the conv epilogue.
-* forward(data, label) -> the reference's nine training outputs (models/resnet_upsnet.py:88-195; Cityscapes configuration,
-  fcn_with_roi_loss off, one image): rpn_cls_loss, rpn_bbox_loss, cls_loss, bbox_loss, mask_loss, fcn_loss,
-  panoptic_loss, rcnn_accuracy, panoptic_accuracy, each float32 [1] on the device.  An eager autograd path separate from
-  the static engine: every module has forward_train(..., prec) next to its forward, built from training.conv2d / linear
-  / conv_transpose2x2 with BN folded per call, the DCN / ROIAlign backward Functions and, in the semantic head, the
-  level sum through FcnScoreFuseFunction; _forward_train composes them with the targets and the device losses.
+* forward(data, label) -> the reference's training outputs (models/resnet_upsnet.py:88-195; one image): rpn_cls_loss,
+  rpn_bbox_loss, cls_loss, bbox_loss, mask_loss, fcn_loss, panoptic_loss, rcnn_accuracy, panoptic_accuracy, each
+  float32 [1] on the device, plus fcn_roi_loss (float32 [], as the reference returns it) when train.fcn_with_roi_loss
+  is set (every COCO configuration, which also sets network.fpn_with_gap: FPN's context vector folded into the P5
+  lateral conv's bias).
+  An eager autograd path separate from the static engine: every module has forward_train(..., prec) next to its
+  forward, built from training.conv2d / linear / conv_transpose2x2 with BN folded per call, the DCN / ROIAlign backward Functions and, in the semantic head, the level sum through
+  FcnScoreFuseFunction; _forward_train composes them with the targets and the device losses (FcnRoiLoss for the
+  semantic head's ROI loss, which samples fcn_score instead of the 512-channel concat).
   get_params_lr() gives the reference's 13 parameter groups for upsnet_b200.SGD.
 """
 import math
@@ -110,6 +113,10 @@ class UPSNetConfig:
     @classmethod
     def cityscapes_r50(cls):      # experiments/upsnet_resnet50_cityscapes_16gpu.yaml
         return cls()
+
+    @classmethod
+    def coco_r50(cls):            # experiments/upsnet_resnet50_coco_{4,8,16}gpu.yaml
+        return cls(num_classes=81, num_seg_classes=133, fpn_with_gap=True, fcn_num_layers=3, fcn_with_roi_loss=True)
 
     @classmethod
     def coco_r101_dcn(cls):       # experiments/upsnet_resnet101_dcn_coco_3x_16gpu.yaml
@@ -311,10 +318,16 @@ class FPN(nn.Module):
         return p2, p3, p4, p5, p6
 
     def forward_train(self, res2, res3, res4, res5, prec):
-        """forward with device gradients (training.conv2d, the same fused top-down add); without fpn_gap."""
-        def c(m, x, **kw):
-            return training.conv2d(x, m.weight, m.bias, precision=prec, **kw)
-        p5_1x1 = c(self.fpn_p5_1x1, res5)
+        """forward with device gradients (training.conv2d, the same fused top-down add).  With fpn_gap, the context
+        vector fpn_gap(GAP(res5)) (models/fpn.py:84-86, added to every P5 lateral pixel) is folded into the bias of the
+        P5 lateral conv, so that conv's d bias carries the gradient to both biases, fpn_gap and res5."""
+        def c(m, x, bias=None, **kw):
+            return training.conv2d(x, m.weight, m.bias if bias is None else bias, precision=prec, **kw)
+        p5_bias = None
+        if hasattr(self, "fpn_gap"):        # one image: the context vector is one row
+            gap = training.linear(res5.mean((2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, precision=prec)
+            p5_bias = self.fpn_p5_1x1.bias + gap.reshape(self.feature_dim)
+        p5_1x1 = c(self.fpn_p5_1x1, res5, p5_bias)
         p4_plus = c(self.fpn_p4_1x1, res4, residual=p5_1x1, residual_up2=True)
         p3_plus = c(self.fpn_p3_1x1, res3, residual=p4_plus, residual_up2=True)
         p2_plus = c(self.fpn_p2_1x1, res2, residual=p3_plus, residual_up2=True)
@@ -1010,21 +1023,22 @@ class resnet_upsnet(nn.Module):
     # training forward: eager autograd, separate from the static engine
     # ------------------------------------------------------------------------------------------
     def _forward_train(self, data, label):
-        """models/resnet_upsnet.py:88-195 with label (Cityscapes configuration, fcn_with_roi_loss off, one image).
+        """models/resnet_upsnet.py:88-195 with label (one image).
 
         Each module runs its forward_train: the backbone with conv1 and res2 frozen on the inference path
-        (backbone_freeze_at = 2), then the FPN, the RPN per level, the semantic head, the RCNN and the mask branch, with
-        device gradients.  Proposals, proposal targets and the panoptic keep draw run without gradients; np.random
-        governs their draws, as in the reference, so the modules run in the order below.
+        (backbone_freeze_at = 2), then the FPN (with its global-context branch under fpn_with_gap), the RPN per level, the semantic head, the RCNN and the mask branch, with device gradients.  Proposals, proposal targets and the
+        panoptic keep draw run without gradients; np.random governs their draws, as in the reference, so the modules
+        run in the order below.  With train.fcn_with_roi_loss, the semantic head's ROI loss (FcnRoiLoss) runs on every
+        ground-truth box, taken before the keep draw as the reference takes them; the label must then carry
+        seg_roi_gt with one row per such box, which is checked before anything is launched.  With keep_intermediates the
+        output also carries those boxes ('fcn_rois').
 
         Precision follows set_precision: 'bf16' runs the training convs in bf16; 'bf16x3' and 'fp32' run them in bf16x3
         (there is no fp32 tensor-core backward).  A training forward drops the folded weights and captured graphs of the
         inference engine, so the next inference forward folds the updated parameters again."""
         cfg = self.cfg
         if cfg.fcn_with_roi_loss:
-            raise _lib.UpsnetError("training forward: train.fcn_with_roi_loss (fcn_roi_loss) is not built")
-        if cfg.fpn_with_gap:
-            raise _lib.UpsnetError("training forward: network.fpn_with_gap is not built")
+            self._check_seg_roi_gt(label)
         if cfg.backbone_freeze_at != 2 or not cfg.backbone_fix_bn:
             raise _lib.UpsnetError("training forward: only backbone_freeze_at = 2 with backbone_fix_bn (every shipped "
                                    "configuration) is built, not freeze_at = %d, fix_bn = %s"
@@ -1067,8 +1081,12 @@ class resnet_upsnet(nn.Module):
         rpn_cls_loss, rpn_bbox_loss = training.RPNLoss(rpn_batch_size=cfg.rpn_batch_size)(rpn_score, rpn_bbox, lab)
         fcn_loss = training.SemanticLoss()(fcn_score, lab["seg_gt"])
 
-        # panoptic head on the ground-truth boxes
+        # panoptic head on the ground-truth boxes; the ROI loss takes all of them, before the keep draw
         gt_rois, cls_idx = training.gt_rois(lab["roidb"], im_info[0, 2], dev)
+        fcn_rois = gt_rois
+        if cfg.fcn_with_roi_loss:
+            fcn_roi_loss = training.FcnRoiLoss(cfg.mask_size)(fcn_score, self.fcn_head.score.bias, fcn_rois,
+                                                              lab["seg_roi_gt"])
         keep = training.draw_keep(gt_rois.shape[0], cfg.panoptic_box_keep_fraction) if self.enable_void else None
         if keep is not None:
             kd = torch.from_numpy(keep).to(dev)
@@ -1082,11 +1100,29 @@ class resnet_upsnet(nn.Module):
                "mask_loss": mask_loss, "fcn_loss": fcn_loss, "panoptic_loss": panoptic_loss, "rcnn_accuracy": rcnn_acc,
                "panoptic_accuracy": panoptic_acc}
         out = {k: v.reshape(1) for k, v in out.items()}
+        if cfg.fcn_with_roi_loss:
+            out["fcn_roi_loss"] = fcn_roi_loss
         if getattr(self, "keep_intermediates", False):   # the discrete decisions of the step, for an oracle replay
             out["_intermediates"] = {
                 "rois": rois, "proposal_targets": dict(zip(training.ProposalTargets.NAMES, targets)), "gt_rois": gt_rois,
                 "cls_idx": cls_idx, "keep_inds": keep, "fpn": [f.detach() for f in (p2, p3, p4, p5, p6)]}
+            if cfg.fcn_with_roi_loss:
+                out["_intermediates"]["fcn_rois"] = fcn_rois
         return out
+
+    @staticmethod
+    def _check_seg_roi_gt(label):
+        """fcn_with_roi_loss needs label['seg_roi_gt'] with one [M,M] row per ground-truth box of get_gt_rois
+        (non-crowd, class > 0)."""
+        roidb = label.get("roidb", {})
+        seg = label.get("seg_roi_gt")
+        if seg is None or "gt_classes" not in roidb or "is_crowd" not in roidb:
+            raise _lib.UpsnetError("training forward: train.fcn_with_roi_loss needs label['seg_roi_gt'] and the roidb's "
+                                   "gt_classes / is_crowd")
+        n = int(((np.asarray(roidb["gt_classes"]) > 0) & (np.asarray(roidb["is_crowd"]) == 0)).sum())
+        if seg.dim() != 3 or seg.shape[0] != n:
+            raise _lib.UpsnetError("training forward: train.fcn_with_roi_loss: label['seg_roi_gt'] has %s rows, the "
+                                   "roidb %d ground-truth boxes" % (tuple(seg.shape), n))
 
 
 def resnet_50_upsnet(cfg=None):

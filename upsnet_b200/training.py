@@ -27,11 +27,12 @@
 * PanopticLoss: the panoptic head of the training forward (models/resnet_upsnet.py:144-179: SegTerm, MaskTerm, the void
   logits, MaskMatching, calc_panoptic_acc and the cross-entropy) as one fused loss with hand-written forward and
   backward kernels (csrc/panoptic_loss.cu), plus the two host helpers for the lines before it (gt_rois, draw_keep).
-* SemanticLoss, RPNLoss, MaskRCNNLoss: the other losses of the training forward (models/resnet_upsnet.py:127-142) with
-  hand-written forward and backward kernels (csrc/train_loss.cu).  SemanticLoss evaluates the x4 up-sampling of
+* SemanticLoss, FcnRoiLoss, RPNLoss, MaskRCNNLoss: the other losses of the training forward
+  (models/resnet_upsnet.py:127-142) with hand-written forward and backward kernels (csrc/train_loss.cu).  SemanticLoss evaluates the x4 up-sampling of
   fcn_score inside the cross-entropy, so the [1,S,4h,4w] fcn_output (159 MB at 1024x2048, S 19), its log-softmax and
   its gradient are never built; RPNLoss covers the five FPN levels in one launch and reads the label fields in place;
-  MaskRCNNLoss reads mask_score and mask_target once.
+  MaskRCNNLoss reads mask_score and mask_target once.  FcnRoiLoss samples fcn_score where the reference samples the
+  512-channel concat of the semantic head, so neither that concat nor the [R,512,28,28] roi features are built.
 * SGD, LRSchedule: the optimiser (lib/nn/optimizer.py:19-106) with the learning-rate schedule and momentum decay of
   upsnet_end2end_train.py:76-103, 235-240, every parameter updated in one launch (csrc/sgd.cu), from p.grad or, through
   FlatBucketAllReduce.step, straight from the all-reduced bf16 buckets; with a schedule attached the step issues kernels
@@ -42,9 +43,8 @@
 Scope note: this is the operator / communication layer of the training configuration, the RPN and proposal targets,
 the label maps, every loss of the training forward, the dense convolutions and FC layers with their gradients, and the
 optimiser; resnet_upsnet.forward(data, label) (model.py) composes them into the training step of the Cityscapes
-configuration.  fcn_roi_loss (train.fcn_with_roi_loss, set by the COCO configurations upsnet_resnet50_coco_*.yaml and
-upsnet_resnet101_dcn_coco_3x_16gpu.yaml; the training forward raises there), Adam and clip_grad (imported by the
-training script, never called) are not built.  The offset convs of the *WithOffset* modules (OffsetConvFunction) and the GEMMs of the deformable backward
+configuration and of the COCO configurations (network.fpn_with_gap, train.fcn_with_roi_loss through FcnRoiLoss).  Adam
+and clip_grad (imported by the training script, never called) are not built.  The offset convs of the *WithOffset* modules (OffsetConvFunction) and the GEMMs of the deformable backward
 stay library calls.
 """
 import ctypes as C
@@ -1293,6 +1293,84 @@ class SemanticLoss(torch.nn.Module):
         if seg_gt.dtype not in (torch.int64, torch.uint8):
             raise E("semantic_loss: seg_gt must be int64 or uint8")
         loss, counts = SemanticLossFunction.apply(fcn_score, seg_gt.contiguous())
+        self.counts = counts
+        return loss
+
+
+class FcnRoiLossFunction(torch.autograd.Function):
+    """(loss, counts) = the fused FCN ROI loss (include/upsnet_b200.h, upsnet_fcn_roi_loss_forward); differentiable in
+    fcn_score and score_bias.  Inputs are validated by FcnRoiLoss.forward."""
+
+    @staticmethod
+    def forward(ctx, fcn_score, score_bias, rois, seg_roi_gt, mask_size, spatial_scale):
+        dev = fcn_score.device
+        _, S, h, w = fcn_score.shape
+        R = rois.shape[0]
+        fcn, bias = f32c(fcn_score.detach()), f32c(score_bias.detach())
+        (loss,) = _scalars(dev, 1)
+        counts = torch.empty(2, dtype=torch.int32, device=dev)
+        lse = torch.empty(R * mask_size * mask_size, dtype=torch.float32, device=dev)
+        ws = torch.empty(query_bytes("fcn_roi_loss_workspace_bytes", S, R, mask_size, 0), dtype=torch.uint8, device=dev)
+        is64 = int(seg_roi_gt.dtype == torch.int64)
+        call("fcn_roi_loss_forward", dev, fcn, bias, S, h, w, rois, R, seg_roi_gt, is64, mask_size, 2, spatial_scale,
+             loss, counts, lse, ws, ws.numel())
+        ctx.save_for_backward(fcn, bias, rois, seg_roi_gt, lse)
+        ctx.cfg = (mask_size, spatial_scale)
+        ctx.mark_non_differentiable(counts)
+        return loss, counts
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_counts):
+        fcn, bias, rois, seg, lse = ctx.saved_tensors
+        M, scale = ctx.cfg
+        dev = fcn.device
+        _, S, h, w = fcn.shape
+        R = rois.shape[0]
+        dfcn, dbias = torch.empty_like(fcn), torch.empty_like(bias)
+        ws = torch.empty(query_bytes("fcn_roi_loss_workspace_bytes", S, R, M, 1), dtype=torch.uint8, device=dev)
+        call("fcn_roi_loss_backward", dev, fcn, bias, S, h, w, rois, R, seg, int(seg.dtype == torch.int64), M, 2, scale,
+             lse, _grad(grad_loss, dev), dfcn, dbias, ws, ws.numel())
+        return dfcn, dbias, None, None, None, None
+
+
+class FcnRoiLoss(torch.nn.Module):
+    """The semantic head's ROI loss of one training image (train.fcn_with_roi_loss; models/fcn.py:102-106 +
+    models/resnet_upsnet.py:132-134): CrossEntropyLoss(ignore_index=255, reduce=False)(score(RoIAlign(M, M, 1/4)(feat,
+    rois)), seg_roi_gt).mean(), with feat the 512-channel concat of the head.  The 1x1 score conv and ROIAlign commute,
+    so the loss samples fcn_score (the score conv's output at quarter resolution) and adds the part of score_bias that
+    ROIAlign's out-of-map zeros remove; feat, the [R,512,M,M] roi features and their gradients are never built.
+
+    The mean runs over all R*M*M cells, ignored ones included, as the reference's.  A target that is neither 255 nor a
+    class gives no loss and no gradient; self.counts, int32 [2] on the device, is (cells with a target, such invalid
+    cells).  The loss is differentiable in fcn_score and score_bias; nothing synchronises with the host, so the call can
+    be captured.  The same inputs give the same bytes."""
+
+    def __init__(self, mask_size=28, spatial_scale=0.25):
+        super().__init__()
+        self.mask_size, self.spatial_scale = int(mask_size), float(spatial_scale)
+
+    def forward(self, fcn_score, score_bias, rois, seg_roi_gt):
+        """fcn_score [1,S,h,w] (float32; other float dtypes are cast); score_bias [S]; rois float32 [R,5] (batch index,
+        x1, y1, x2, y2 in image coordinates, as gt_rois gives them), 1 <= R <= 1024; seg_roi_gt [R,M,M] int64 or uint8.
+        -> loss, a 0-dim device tensor."""
+        E = _lib.UpsnetError
+        require_cuda(fcn_score, score_bias, rois, seg_roi_gt)
+        M = self.mask_size
+        if fcn_score.dim() != 4 or fcn_score.shape[0] != 1:
+            raise E("fcn_roi_loss: only batch size 1 (fcn_score [1,S,h,w])")
+        S = fcn_score.shape[1]
+        if tuple(score_bias.shape) != (S,):
+            raise E("fcn_roi_loss: score_bias must be [%d], not %s" % (S, tuple(score_bias.shape)))
+        if rois.dim() != 2 or rois.shape[1] != 5 or rois.dtype != torch.float32:
+            raise E("fcn_roi_loss: rois must be float32 [R,5], not %s %s" % (rois.dtype, tuple(rois.shape)))
+        R = rois.shape[0]
+        if tuple(seg_roi_gt.shape) != (R, M, M):
+            raise E("fcn_roi_loss: seg_roi_gt must be [%d,%d,%d] (one row per roi), not %s"
+                    % (R, M, M, tuple(seg_roi_gt.shape)))
+        if seg_roi_gt.dtype not in (torch.int64, torch.uint8):
+            raise E("fcn_roi_loss: seg_roi_gt must be int64 or uint8")
+        loss, counts = FcnRoiLossFunction.apply(fcn_score, score_bias, rois.contiguous(), seg_roi_gt.contiguous(), M,
+                                                self.spatial_scale)
         self.counts = counts
         return loss
 
