@@ -37,3 +37,39 @@ def launched_kernels(fn, keep, sessions=12, pad=0.05):
             return out, {e.key for e in events if keep(e.key) and MARKER not in e.key}
         DISCARDED[0] += 1
     raise AssertionError("torch.profiler lost the marker records of %d sessions in a row" % sessions)
+
+
+def launched_kernels_each(fns, keep, sessions=12, pad=0.05):
+    """[{names of the kernels fns[i]() launched for which keep(name) holds} for each i] from ONE profiler session: a
+    marker kernel before each call and after the last, the device records ordered by start time and cut at the markers.
+    A process that opens many sessions makes later sessions lose their records more often, so a test that needs the
+    kernels of many calls asks for them here, once.  Only a session with all len(fns) + 1 markers recorded is used;
+    otherwise every fn runs again in a new session with longer idle ends, so each fn must be callable repeatedly."""
+    from torch.profiler import ProfilerActivity, profile
+    for attempt in range(sessions):
+        idle = min(pad * 2 ** attempt, 0.4)
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            time.sleep(idle)
+            for fn in fns:
+                torch.cuda._sleep(1000)
+                torch.cuda.synchronize()
+                fn()
+                torch.cuda.synchronize()
+            torch.cuda._sleep(1000)
+            torch.cuda.synchronize()
+            time.sleep(idle)
+        events = sorted((e.start_ns(), e.name()) for e in prof.profiler.kineto_results.events()
+                        if e.device_type() == torch.autograd.DeviceType.CUDA)
+        if sum(MARKER in name for _, name in events) == len(fns) + 1:
+            out, cur = [], None
+            for _, name in events:
+                if MARKER in name:
+                    if cur is not None:
+                        out.append(cur)
+                    cur = set()
+                elif cur is not None and keep(name):
+                    cur.add(name)
+            return out
+        DISCARDED[0] += 1
+    raise AssertionError("torch.profiler lost the marker records of %d sessions in a row" % sessions)

@@ -1,7 +1,10 @@
 """CPU check that the bounds of tests/test_gpu_conv_backward.py have teeth: a torch restatement of the dense-conv
 backward arithmetic (tests/conv_grad_oracle.py: hi/lo pairs or bf16 operands, flipped-tap dgrad, per-tap wgrad over K
-splits) passes grad_oracle.check at the a-priori constants, and each planted fault fails it: a tap not flipped, x read
-one pixel off, one K split dropped, the ReLU mask missing."""
+splits, the stride-2 1x1 dX scattered from its compact result) passes grad_oracle.check at the a-priori constants, and
+each planted fault fails it: a tap not flipped, x read one pixel off, one K split dropped, the ReLU mask missing, and
+the errors a wide layer's dX route could make: one 64-channel tile of dX from the neighbouring tile's weight rows, a
+3x3 tap past the last row of one image reading the next image's first row (N = 2, as when a 128-pixel tile of the
+flattened pixels straddles two images), the compact stride-2 result scattered to the odd pixels or one pixel off."""
 import os
 import sys
 
@@ -66,3 +69,51 @@ def test_dropped_split_fails(prec):
 def test_missing_relu_mask_fails(prec):
     okx, okw, _, _ = _run(prec, 3, 1, 1, mask=False)
     assert not okx and not okw
+
+
+def _wide(prec, tile_from=None, stacked=False):
+    """dX of a 3x3 / pad 1 conv, 192 -> 24 channels (three 64-channel dX tiles), N = 2 images of 5 x 6."""
+    gen = torch.Generator().manual_seed(23)
+    x = torch.randn((2, 192, 5, 6), generator=gen)
+    w = torch.randn((24, 192, 3, 3), generator=gen) * (2.0 / (192 * 9)) ** 0.5
+    dy = torch.randn((2, 24, 5, 6), generator=gen)
+    g, dx, _, bx, _ = CG.reference(x, w, dy, 1, 1)
+    ex = CG.dgrad(dy, w, 1, 1, prec, tile_from=tile_from, stacked=stacked)
+    return G.check(ex, dx, bx, CG.apriori(prec, "dx", 64 * 9))
+
+
+@pytest.mark.parametrize("prec", ["bf16x3", "bf16"])
+def test_wide_restatement_passes(prec):
+    ok, r = _wide(prec)
+    assert ok, r
+
+
+@pytest.mark.parametrize("tile", [0, 1])
+@pytest.mark.parametrize("prec", ["bf16x3", "bf16"])
+def test_dx_tile_from_neighbour_fails(prec, tile):
+    assert not _wide(prec, tile_from=tile)[0]
+
+
+@pytest.mark.parametrize("prec", ["bf16x3", "bf16"])
+def test_tap_reads_next_image_fails(prec):
+    assert not _wide(prec, stacked=True)[0]
+
+
+def _stride2(prec, H, W, scatter):
+    gen = torch.Generator().manual_seed(H * W)
+    x = torch.randn((2, 64, H, W), generator=gen)
+    w = torch.randn((16, 64, 1, 1), generator=gen) * (2.0 / 64) ** 0.5
+    y = F.conv2d(x, w, None, 2)
+    dy = torch.randn(y.shape, generator=gen)
+    g, dx, _, bx, _ = CG.reference(x, w, dy, 0, 1, y, stride=2)
+    ex = CG.dgrad_stride2((dy * (y > 0).float()), w, H, W, prec, scatter)
+    return G.check(ex, dx, bx, CG.apriori(prec, "dx", 64))
+
+
+@pytest.mark.parametrize("hw", [(7, 9), (8, 6), (9, 10)])
+@pytest.mark.parametrize("prec", ["bf16x3", "bf16"])
+def test_stride2_scatter(prec, hw):
+    ok, r = _stride2(prec, *hw, "even")
+    assert ok, r
+    assert not _stride2(prec, *hw, "odd")[0]
+    assert not _stride2(prec, *hw, "shift")[0]

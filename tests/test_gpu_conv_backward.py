@@ -19,11 +19,12 @@ d bias: exact fp32 terms summed in fp64 in a fixed order, rounded once: 2^-24 (c
   ((g00 + g01) + g10) + g11 in fp32 for residual_up2: 3 * 2^-24 (c = 2^-22).
 
 Measured on an NVIDIA H100 80GB HBM3 (SXM, power limit 700 W), worst err / bound over all cases: bf16x3 dX 1.73e-5,
-dW 1.34e-5; bf16 dX 6.3e-3, dW 4.9e-3; d bias 3.4e-8, d residual 1.2e-7.  TOL below holds about 4x the bf16x3 values.
-The a-priori constants live in tests/conv_grad_oracle.py; tests/test_conv_grad_oracle_cpu.py shows they reject an
-unflipped tap, a one-pixel shift, a dropped K split and a missing ReLU mask.
+dW 1.34e-5; bf16 dX 6.3e-3, dW 4.9e-3; d bias 3.4e-8, d residual 1.2e-7.  conv_grad_cases.TOL holds about 4x the
+bf16x3 values.  The layer harness lives in tests/conv_grad_cases.py, the a-priori constants in
+tests/conv_grad_oracle.py; tests/test_conv_grad_oracle_cpu.py shows they reject an unflipped tap, a one-pixel shift, a
+dropped K split and a missing ReLU mask.  tests/test_gpu_conv_backward_wide.py runs the same harness at the channel
+widths of the training forward.
 """
-import math
 import os
 import sys
 
@@ -32,16 +33,9 @@ import torch
 import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import grad_oracle as G  # noqa: E402
-from conv_grad_oracle import apriori  # noqa: E402
+from conv_grad_cases import _check, _rand, _run_linear, _vjp, report, run_conv, run_deconv  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-WORST = {}
-# About 4x the worst err / bound measured on the H100 (bf16x3: dX 1.73e-5 at the RPN cls head, dW 1.34e-5 at fc6), used
-# where it is below the a-priori constant.  bf16: the operands' own rounding is the error (measured dX 6.3e-3, dW 4.9e-3
-# against 7.8e-3 a priori), so the a-priori constant is the tolerance.  d bias (3.4e-8) and d residual (1.2e-7) are
-# checked at their a-priori 1.2e-7 and 2.4e-7.
-TOL = {("bf16x3", "dx"): 7e-5, ("bf16x3", "dw"): 5.5e-5}
 
 
 @pytest.fixture(scope="module")
@@ -51,80 +45,9 @@ def dev():
 
 
 @pytest.fixture(scope="module", autouse=True)
-def report():
+def _report():
     yield
-    for k in sorted(WORST):
-        print("conv backward worst err/bound %-34s %.3e" % (k, WORST[k]))
-
-
-def _check(name, prec, grad, got, want, bound, K, splits=1):
-    c = apriori(prec, grad, K, splits)
-    tol = TOL.get((prec, grad))
-    c_use = min(c, tol) if tol is not None else c
-    ok, ratio = G.check(got, want, bound, c_use)
-    key = "%s %s %s" % (name, prec, grad)
-    WORST[key] = max(WORST.get(key, 0.0), ratio)
-    assert ok, "%s: worst err/bound %.3e > c %.3e" % (key, ratio, c_use)
-
-
-def _rand(shape, dev, scale=1.0, seed=0):
-    g = torch.Generator(device=dev).manual_seed(seed)
-    return torch.randn(shape, generator=g, device=dev) * scale
-
-
-def _vjp(f, inputs, cot):
-    """float64 autograd of f at `inputs` with cotangent cot, and of f at |inputs| with |cot| (the sums of |terms|)."""
-    xs = [t.double().detach().requires_grad_(True) for t in inputs]
-    out = f(*xs)
-    grads = torch.autograd.grad(out, xs, cot.double())
-    xa = [t.double().abs().detach().requires_grad_(True) for t in inputs]
-    outa = f(*xa)
-    bounds = torch.autograd.grad(outa, xa, cot.double().abs())
-    return grads, bounds
-
-
-def run_conv(dev, name, prec, N, Cin, H, W, Cout, k, stride=1, pad=0, dil=1, bias=True, relu=False, res=None,
-             seed=0, nhwc_dy=False, need_x=True):
-    """One layer: training.conv2d forward + backward vs float64 autograd.  res: None, 'same' or 'up2'."""
-    from upsnet_b200 import training
-    x = _rand((N, Cin, H, W), dev, 1.0, seed)
-    w = _rand((Cout, Cin, k, k), dev, (2.0 / (Cin * k * k)) ** 0.5, seed + 1).requires_grad_(True)
-    b = _rand((Cout,), dev, 0.1, seed + 2).requires_grad_(True) if bias else None
-    Ho = (H + 2 * pad - dil * (k - 1) - 1) // stride + 1
-    Wo = (W + 2 * pad - dil * (k - 1) - 1) // stride + 1
-    r = None
-    if res == "same":
-        r = _rand((N, Cout, Ho, Wo), dev, 1.0, seed + 3).requires_grad_(True)
-    elif res == "up2":
-        r = _rand((N, Cout, Ho // 2, Wo // 2), dev, 1.0, seed + 3).requires_grad_(True)
-    xg = x.clone().requires_grad_(need_x)
-    y = training.conv2d(xg, w, b, stride, pad, dil, residual=r, residual_up2=(res == "up2"), relu=relu, precision=prec)
-    assert y.shape == (N, Cout, Ho, Wo) and y.dtype == torch.float32
-    dy = _rand((N, Cout, Ho, Wo), dev, 1.0, seed + 4)
-    if nhwc_dy:
-        dy = dy.contiguous(memory_format=torch.channels_last)
-    y.backward(dy)
-    g = dy.double() * (y.detach() > 0).double() if relu else dy.double()
-    conv = lambda a, bw: F.conv2d(a, bw, None, stride, pad, dil)   # noqa: E731
-    (gx, gw), (bx, bw) = _vjp(conv, [x, w.detach()], g)
-    S = 1
-    if need_x:
-        assert xg.grad.shape == x.shape
-        _check(name, prec, "dx", xg.grad, gx, bx, ((Cout + 63) // 64 * 64) * k * k)
-    else:
-        assert xg.grad is None
-    from upsnet_b200 import _lib
-    nb = _lib.query_bytes("conv_wgrad_workspace_bytes", N, H, W, Cin, Cout, k, k, stride, stride, pad, pad, dil, dil,
-                          _lib.PREC_BF16X3 if prec == "bf16x3" else _lib.PREC_BF16)
-    S = max(1, nb // (4 * k * k * ((Cout + 127) // 128 * 128) * ((Cin + 127) // 128 * 128)))
-    _check(name, prec, "dw", w.grad, gw, bw, math.ceil(N * Ho * Wo / S / 64) * 64 + 64, S)
-    if bias:
-        _check(name, prec, "db", b.grad, g.sum((0, 2, 3)), g.abs().sum((0, 2, 3)), N * Ho * Wo)
-    if res == "same":
-        _check(name, prec, "dres", r.grad, g, g.abs(), 1)
-    elif res == "up2":
-        _check(name, prec, "dres", r.grad, F.avg_pool2d(g, 2) * 4, F.avg_pool2d(g.abs(), 2) * 4, 4)
-    return y
+    report()
 
 
 PRECS = ["bf16x3", "bf16"]
@@ -164,21 +87,6 @@ def test_dy_nhwc_and_no_dgrad(dev, prec):
     run_conv(dev, "lat2 no dx", prec, 1, 256, 12, 20, 128, 1, 1, 0, 1, True, False, None, seed=6, need_x=False)
 
 
-def _run_linear(dev, name, prec, R, K, Cout, relu, seed):
-    from upsnet_b200 import training
-    x = _rand((R, K), dev, 1.0, seed).requires_grad_(True)
-    w = _rand((Cout, K), dev, (2.0 / K) ** 0.5, seed + 1).requires_grad_(True)
-    b = _rand((Cout,), dev, 0.1, seed + 2).requires_grad_(True)
-    y = training.linear(x, w, b, relu=relu, precision=prec)
-    dy = _rand((R, Cout), dev, 1.0, seed + 3)
-    y.backward(dy)
-    g = dy.double() * (y.detach() > 0).double() if relu else dy.double()
-    (gx, gw), (bx, bw) = _vjp(lambda a, ww: F.linear(a, ww), [x.detach(), w.detach()], g)
-    _check(name, prec, "dx", x.grad, gx, bx, (Cout + 63) // 64 * 64)
-    _check(name, prec, "dw", w.grad, gw, bw, math.ceil(R / 64) * 64 + 64)
-    _check(name, prec, "db", b.grad, g.sum(0), g.abs().sum(0), R)
-
-
 @pytest.mark.parametrize("prec", PRECS)
 def test_linear_heads(dev, prec):
     """fc6 (K = 12544), fc7 and the cls / bbox heads on one-pixel images."""
@@ -193,22 +101,7 @@ def test_linear_heads(dev, prec):
 @pytest.mark.parametrize("prec", PRECS)
 def test_deconv_2x2(dev, prec):
     """The mask branch's ConvTranspose2d(256, 256, 2, 2) + ReLU on 163 rois of 14 x 14."""
-    from upsnet_b200 import training
-    R, Cin, C, H = 163, 256, 256, 14
-    x = _rand((R, Cin, H, H), dev, 1.0, 21).requires_grad_(True)
-    w = _rand((Cin, C, 2, 2), dev, (2.0 / Cin) ** 0.5, 22).requires_grad_(True)
-    b = _rand((C,), dev, 0.1, 23).requires_grad_(True)
-    y = training.conv_transpose2x2(x, w, b, relu=True, precision=prec)
-    assert y.shape == (R, C, 2 * H, 2 * H)
-    y64 = torch.relu(F.conv_transpose2d(x.detach().double(), w.detach().double(), b.detach().double(), stride=2))
-    assert float((y.detach().double() - y64).abs().max()) < 0.1
-    dy = _rand(y.shape, dev, 1.0, 24)
-    y.backward(dy)
-    g = dy.double() * (y.detach() > 0).double()
-    (gx, gw), (bx, bw) = _vjp(lambda a, ww: F.conv_transpose2d(a, ww, None, stride=2), [x.detach(), w.detach()], g)
-    _check("deconv 2x2", prec, "dx", x.grad, gx, bx, 4 * C)
-    _check("deconv 2x2", prec, "dw", w.grad, gw, bw, math.ceil(R * H * H / 64) * 64 + 64, 64)
-    _check("deconv 2x2", prec, "db", b.grad, g.sum((0, 2, 3)), g.abs().sum((0, 2, 3)), R * 4 * H * H)
+    run_deconv(dev, "deconv 2x2", prec, 163, 256, 256, 14, 21)
 
 
 def test_fullsize(dev):
