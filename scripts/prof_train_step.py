@@ -2,8 +2,8 @@
 warm-up, images/s and peak memory, in bf16 and bf16x3.  --config picks the configuration: cityscapes_r50 (UPSNet-50 at
 1024x2048, the default), coco_r50 (UPSNet-50 COCO at 800x1344: fpn_with_gap, fcn_with_roi_loss) or coco_r101_dcn
 (UPSNet-101 with DCN in res3-res5, COCO at 800x1344).  As a comparator, the same step composed from library ops
-(tests/train_forward_oracle.py, or tests/train_forward_coco_oracle.py for COCO, on cuDNN: fp32 with TF32 off, and bf16
-autocast) with the same discrete decisions.  Prints the card name and power limit of the run.
+(tests/train_forward_oracle.py, on cuDNN: fp32 with TF32 off, and bf16 autocast) with the same discrete decisions.
+Prints the card name and power limit of the run.
 
   python scripts/prof_train_step.py [--config cityscapes_r50] [--steps 5] [--warmup 2]
 """
@@ -34,15 +34,13 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("prof_train_step.py needs a CUDA device")
-    import train_forward_coco_oracle as CO
     import train_forward_oracle as TF
     import upsnet_b200 as U
     from upsnet_b200.model import UPSNetConfig
     from upsnet_b200.synthetic import synthetic_model
     make_cfg, depth, (H, W), dataset = CONFIGS[a.config]
     cfg = getattr(UPSNetConfig, make_cfg)()
-    coco = dataset == "coco"
-    losses = CO.LOSSES if cfg.fcn_with_roi_loss else TF.LOSSES
+    losses = TF.COCO_LOSSES if cfg.fcn_with_roi_loss else TF.LOSSES
     print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                          text=True).stdout.strip())
     dev = torch.device("cuda", 0)
@@ -84,9 +82,10 @@ def main():
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cudnn.benchmark = True
     for name, ac in (("library fp32 (TF32 off)", None), ("library bf16 autocast", torch.bfloat16)):
-        kw = dict(depth=depth, num_classes=cfg.num_classes, num_seg_classes=cfg.num_seg_classes,
-                  dconv_from=cfg.backbone_with_dconv, fcn_layers=cfg.fcn_num_layers, dtype=torch.float32, device=dev)
-        orc = (CO.CocoTrainOracle if coco else TF.TrainOracle)(sd, TF.trainable_names(m), **kw)
+        orc = TF.TrainOracle(sd, TF.trainable_names(m), depth=depth, num_classes=cfg.num_classes,
+                             num_seg_classes=cfg.num_seg_classes, dconv_from=cfg.backbone_with_dconv,
+                             fcn_layers=cfg.fcn_num_layers, with_gap=cfg.fpn_with_gap,
+                             fcn_with_roi_loss=cfg.fcn_with_roi_loss, dtype=torch.float32, device=dev)
         times = []
         torch.cuda.reset_peak_memory_stats(dev)
         for it in range(a.warmup + a.steps):

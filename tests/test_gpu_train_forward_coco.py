@@ -1,5 +1,5 @@
 """The training forward of the COCO configurations on the device (UPSNetConfig.coco_r50: fpn_with_gap,
-fcn_with_roi_loss, fcn_num_layers 3, 81 / 133 classes) against the float64 oracle of tests/train_forward_coco_oracle.py,
+fcn_with_roi_loss, fcn_num_layers 3, 81 / 133 classes) against the float64 oracle of tests/train_forward_oracle.py,
 with the criteria of tests/test_gpu_train_forward.py (train_forward_oracle.LOSS_TOL / grad_tol).
 
 The synthetic model calibrates the FPN laterals to RMS 1 but leaves fpn_gap at the reference's nn.Linear
@@ -15,7 +15,6 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-import train_forward_coco_oracle as CO  # noqa: E402
 import train_forward_oracle as TF  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -39,7 +38,7 @@ def precision():
 def _calibrate_gap(m, x):
     with torch.no_grad():
         r5 = m.resnet_backbone.forward_train(x, "bf16x3")[3]
-        g = CO.gap_vector(r5, m.fpn.fpn_gap.weight, m.fpn.fpn_gap.bias)
+        g = TF.gap_vector(r5, m.fpn.fpn_gap.weight, m.fpn.fpn_gap.bias)
         s = 1.0 / float(g.pow(2).mean().sqrt())
         m.fpn.fpn_gap.weight.mul_(s)
         m.fpn.fpn_gap.bias.mul_(s)
@@ -71,20 +70,20 @@ def _product_step(m, data, label, seed):
     m.zero_grad(set_to_none=True)
     np.random.seed(seed)
     out = m(data, label)
-    sum(out[k] for k in CO.LOSSES).backward()
+    sum(out[k] for k in TF.COCO_LOSSES).backward()
     return out
 
 
 def _oracle(m, depth, dconv, dev, dtype=torch.float64, **kw):
     sd = {k: v.detach() for k, v in m.state_dict().items()}
-    return CO.CocoTrainOracle(sd, TF.trainable_names(m), depth=depth, num_classes=81, num_seg_classes=133,
-                              dconv_from=dconv, fcn_layers=3, dtype=dtype, device=dev, **kw)
+    return TF.TrainOracle(sd, TF.trainable_names(m), depth=depth, num_classes=81, num_seg_classes=133, dconv_from=dconv,
+                          fcn_layers=3, with_gap=True, fcn_with_roi_loss=True, dtype=dtype, device=dev, **kw)
 
 
 def _errors(m, out, want, wgrads):
     named = dict(m.named_parameters())
     err = TF.grad_errors({k: named[k].grad for k in wgrads}, wgrads)
-    lerr = {k: abs(float(out[k]) - want[k]) / max(abs(want[k]), 1e-3) for k in CO.LOSSES}
+    lerr = {k: abs(float(out[k]) - want[k]) / max(abs(want[k]), 1e-3) for k in TF.COCO_LOSSES}
     return err, lerr
 
 
@@ -123,8 +122,8 @@ def test_reduced_coco_model_vs_oracle(dev, precision, prec, dconv):
     # the planted faults: the same criteria reject an oracle without the gap's gradient, or whose ROI loss takes the
     # kept boxes only
     if prec == "bf16x3" and dconv == 100:
-        for fault in CO.COCO_FAULTS:
-            fw, fg = _oracle(m, depth, dconv, dev, coco_fault=fault).step(data["data"], label, inter)
+        for fault in TF.COCO_FAULTS:
+            fw, fg = _oracle(m, depth, dconv, dev, fault=fault).step(data["data"], label, inter)
             assert _rejected(*_errors(m, out, fw, fg), prec), fault
 
 
@@ -172,7 +171,7 @@ def test_full_size_coco_step(dev, precision):
     with torch.backends.cudnn.flags(enabled=True, allow_tf32=False):
         torch.backends.cuda.matmul.allow_tf32 = False
         want = _oracle(m, depth, 100, dev, torch.float32).forward(data["data"], label, inter)
-    for k in CO.LOSSES:
+    for k in TF.COCO_LOSSES:
         rel = abs(float(out[k]) - float(want[k])) / max(abs(float(want[k])), 1e-3)
         print("full-size %s %.6g %.6g rel %.2e" % (k, float(out[k]), float(want[k]), rel))
         assert rel <= TF.LOSS_TOL["bf16x3"], (k, rel)

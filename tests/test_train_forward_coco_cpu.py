@@ -1,4 +1,4 @@
-"""The COCO pieces of the training oracle (tests/train_forward_coco_oracle.py) on CPU: its ROI loss reproduces the
+"""The COCO pieces of the training oracle (tests/train_forward_oracle.py) on CPU: its ROI loss reproduces the
 reference fixture (tests/golden/reference_fcn_roi_loss.npz), and the criteria of the GPU comparison reject its two
 planted faults, the ROI loss on the boxes kept by the panoptic draw and a context vector detached from fpn_gap."""
 import os
@@ -10,7 +10,6 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import fcn_roi_loss_oracle as FO  # noqa: E402
-import train_forward_coco_oracle as CO  # noqa: E402
 import train_forward_oracle as TF  # noqa: E402
 
 Z = np.load(os.path.join(HERE, "golden", "reference_fcn_roi_loss.npz"))
@@ -26,7 +25,7 @@ def test_roi_loss_matches_the_reference_and_rejects_the_kept_boxes():
     out = {}
     for k in (None, keep):
         w, b = c["weight"].double().requires_grad_(True), c["bias"].double().requires_grad_(True)
-        loss = CO.roi_loss(feat, w, b, c["rois"], c["seg"], keep=k)
+        loss = TF.roi_loss(feat, w, b, c["rois"], c["seg"], keep=k)
         loss.backward()
         out[k is None] = (float(loss), {"fcn_head.score.weight": w.grad, "fcn_head.score.bias": b.grad})
     want = float(Z["case/%s/loss" % name])
@@ -41,7 +40,7 @@ def test_detached_gap_is_rejected():
     for detached in (False, True):
         w = (torch.randn(256, 2048, generator=g, dtype=torch.float64) * 0.02).requires_grad_(True)
         bias = torch.randn(256, generator=g, dtype=torch.float64).requires_grad_(True)
-        v = CO.gap_vector(res5, w, bias, detached)
+        v = TF.gap_vector(res5, w, bias, detached)
         assert v.shape == (1, 256, 1, 1)
         if not detached:
             ref = torch.nn.functional.linear(res5.mean((2, 3)), w, bias)

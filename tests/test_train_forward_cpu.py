@@ -12,7 +12,7 @@ sys.path.insert(0, HERE)
 import train_forward_oracle as TF  # noqa: E402
 
 
-def _decisions(entry, H, W, seed, K=9, R=48, M=28):
+def _decisions(entry, H, W, seed, K=9, S=19, R=48, M=28):
     """Discrete decisions and loader labels of one step, drawn at random (the GPU tests take them from the product)."""
     rng = np.random.default_rng(seed)
     f32 = np.float32
@@ -47,34 +47,54 @@ def _decisions(entry, H, W, seed, K=9, R=48, M=28):
         w_ = (rng.random((1, 12, Fh, Fw)) < 0.1).astype(f32)
         label["rpn_bbox_inside_weights_fpn%d" % s] = torch.from_numpy(w_)
         label["rpn_bbox_outside_weights_fpn%d" % s] = torch.from_numpy(w_ / 64)
-    seg = rng.integers(0, 19, (1, H, W))
+    seg = rng.integers(0, S, (1, H, W))
     seg[rng.random((1, H, W)) < 0.1] = 255
     label["seg_gt"] = torch.from_numpy(seg)
     label["seg_gt_4x"] = torch.from_numpy(seg[:, ::4, ::4].copy())
     label["mask_gt"] = torch.from_numpy((rng.random((G, H // 4, W // 4)) < 0.2).astype(np.uint8))
+    inter["fcn_rois"] = gt                      # the ROI loss takes every ground-truth box, before the keep draw
+    seg_roi = rng.integers(0, S, (G, M, M))
+    seg_roi[rng.random((G, M, M)) < 0.2] = 255
+    label["seg_roi_gt"] = torch.from_numpy(seg_roi)
     return inter, label
 
 
-@pytest.fixture(scope="module")
-def tiny():
+def _tiny(cfg=None, K=9, S=19):
     from upsnet_b200.synthetic import synthetic_model
     with torch.random.fork_rng(devices=[]):
-        m = synthetic_model(depth=(2, 2, 2, 2), seed=3)
+        m = synthetic_model(cfg, depth=(2, 2, 2, 2), seed=3)
     H, W = 64, 96
-    entry, _ = TF.synthetic_entry(5, H, W, 5)
-    inter, label = _decisions(entry, H, W, 7)
+    entry, _ = TF.synthetic_entry(5, H, W, 5, num_classes=K)
+    inter, label = _decisions(entry, H, W, 7, K, S)
     sd = {k: v.detach().cpu() for k, v in m.state_dict().items()}
     return sd, TF.trainable_names(m), TF.image(11, H, W), inter, label
 
 
-def _run(tiny, dtype=torch.float64, fault=None):
+def _run(tiny, dtype=torch.float64, fault=None, **kw):
     sd, names, img, inter, label = tiny
-    return TF.TrainOracle(sd, names, dtype=dtype, fault=fault).step(img, label, inter)
+    return TF.TrainOracle(sd, names, dtype=dtype, fault=fault, **kw).step(img, label, inter)
+
+
+# the oracle of UPSNetConfig.coco_r50's structure: FPN's global context branch and the semantic head's ROI loss
+COCO = dict(num_classes=81, num_seg_classes=133, fcn_layers=3, with_gap=True, fcn_with_roi_loss=True)
+
+
+@pytest.fixture(scope="module")
+def tiny():
+    return _tiny()
 
 
 @pytest.fixture(scope="module")
 def clean(tiny):
     return _run(tiny)
+
+
+@pytest.fixture(scope="module")
+def coco():
+    """(the tiny step of a coco_r50-structured model, its clean oracle step)"""
+    from upsnet_b200.model import UPSNetConfig
+    tiny = _tiny(UPSNetConfig.coco_r50(), K=81, S=133)
+    return tiny, _run(tiny, **COCO)
 
 
 def test_fp32_oracle_passes_criterion(tiny, clean):
@@ -85,9 +105,13 @@ def test_fp32_oracle_passes_criterion(tiny, clean):
         assert abs(out[k] - clean[0][k]) <= TF.LOSS_TOL["bf16x3"] * max(abs(clean[0][k]), 1e-3), k
 
 
-@pytest.mark.parametrize("fault", TF.FAULTS)
-def test_planted_fault_rejected(tiny, clean, fault):
-    _, g = _run(tiny, fault=fault)
+@pytest.mark.parametrize("fault", TF.FAULTS + TF.COCO_FAULTS)
+def test_planted_fault_rejected(request, fault):
+    if fault in TF.COCO_FAULTS:
+        (tiny, clean), kw = request.getfixturevalue("coco"), COCO
+    else:
+        tiny, clean, kw = request.getfixturevalue("tiny"), request.getfixturevalue("clean"), {}
+    _, g = _run(tiny, fault=fault, **kw)
     err = TF.grad_errors(g, clean[1])
     assert any(e > TF.grad_tol(k, "bf16x3") for k, e in err.items()), fault
 

@@ -1,24 +1,32 @@
-"""Differentiable restatement of the training forward of models/resnet_upsnet.py:88-195 in plain torch -- TEST
-INFRASTRUCTURE ONLY, independent of the product as oracle/literal_model.py is.
+"""The training step of models/resnet_upsnet.py:88-195 in plain torch, differentiable -- TEST INFRASTRUCTURE ONLY,
+independent of the product.
 
-The graph is written the way the reference writes it: un-folded frozen BatchNorm, conv1 / res2 detached
-(backbone_freeze_at = 2), nearest-neighbour FPN up-sampling materialised, the semantic head as concat -> score -> x4
-up-sampling inside the cross-entropy, ConvTranspose2d for the mask deconv, torchvision's deform_conv2d and roi_align for
-the custom operators, and the existing loss oracles (train_loss_oracle, panoptic_loss_oracle).  The discrete decisions of
-a step (proposals, sampled targets, gt rois, keep_inds) are taken from the product's `_intermediates`, so the oracle
-replays the same step.  Parameters are leaf tensors in any float dtype, on the CPU or the GPU.
+The graph is oracle/literal_model.py's LiteralUPSNet, the reference's graph restated literally; this module adds what
+is about training: the trainable parameters and their gradients, conv1 / res2 frozen (backbone_freeze_at = 2), the
+losses, and the planted faults.  The losses are the existing loss oracles (train_loss_oracle, panoptic_loss_oracle),
+with the semantic head's cross-entropy taken on the x4 up-sampled score.  The discrete decisions of a step (proposals,
+sampled targets, gt rois, keep_inds) are taken from the product's `_intermediates`, so the oracle replays the same
+step.  Parameters are leaf tensors in any float dtype, on the CPU or the GPU.
 
-`fault` plants one of FAULTS, for the tests that show the gradient criterion rejects it.
+The COCO configurations build the same oracle with with_gap (FPN's global context branch, models/fpn.py:84-86) and
+fcn_with_roi_loss (the semantic head's ROI loss, models/fcn.py:102-106, models/resnet_upsnet.py:132-134, restated
+literally: RoIAlign of the 512-channel concat, the score conv, the cross-entropy with ignore_index 255 averaged over
+every cell, on the product's 'fcn_rois': every ground-truth box, before the keep draw).
+
+`fault` plants one of FAULTS or COCO_FAULTS, for the tests that show the gradient criterion rejects it: 'gap_detached'
+takes no gradient through fpn_gap, 'rois_after_keep' takes the ROI loss on the kept boxes and their seg_roi_gt rows.
 """
 import numpy as np
 import torch
 import torch.nn.functional as F
-import torchvision
 
+import fcn_roi_loss_oracle as FO
 import panoptic_loss_oracle as PO
 import train_loss_oracle as TO
+from oracle.literal_model import LiteralUPSNet
 
 FAULTS = ("bn_scale_dw", "p6_grad", "fcn_level_detached", "pan_mask_grad", "res2_trainable")
+COCO_FAULTS = ("gap_detached", "rois_after_keep")
 STRIDES = (4, 8, 16, 32, 64)
 
 
@@ -28,143 +36,78 @@ def trainable_names(model):
     return [n for n, p in model.named_parameters() if id(p) in ids]
 
 
-class TrainOracle:
-    def __init__(self, state_dict, trainable, depth=(2, 2, 2, 2), num_classes=9, num_seg_classes=19, dconv_from=100,
-                 fcn_layers=2, rpn_batch_size=256, dtype=torch.float64, device="cpu", fault=None):
-        assert fault is None or fault in FAULTS
+def gap_vector(res5, weight, bias, detached=False):
+    """models/fpn.py:85: fpn_gap(adaptive_avg_pool2d(res5, 1)) as [1, C, 1, 1]."""
+    if detached:
+        res5, weight, bias = res5.detach(), weight.detach(), bias.detach()
+    return F.linear(F.adaptive_avg_pool2d(res5, (1, 1)).flatten(1), weight, bias).view(1, -1, 1, 1)
+
+
+def roi_loss(feat, weight, bias, rois, seg, keep=None):
+    """The reference's fcn_roi_loss from the 512-channel concat feat [1,512,h,w]; with keep, the faulty variant that
+    takes only the kept boxes (and their rows)."""
+    if keep is not None:
+        keep = torch.as_tensor(keep, device=rois.device).long()
+        rois, seg = rois[keep], seg[keep]
+    f = feat[0]
+    By, Bx, _ = FO.roi_align_weights(rois, f.shape[1], f.shape[2], seg.shape[1])
+    rf = torch.einsum("rmy,cyx,rnx->rcmn", By.to(f.dtype), f, Bx.to(f.dtype))
+    return FO.ce_mean(F.conv2d(rf, weight, bias), seg.long())
+
+
+class TrainOracle(LiteralUPSNet):
+    def __init__(self, state_dict, trainable, depth=(2, 2, 2, 2), rpn_batch_size=256, fcn_with_roi_loss=False,
+                 dtype=torch.float64, fault=None, **kw):
+        assert fault is None or fault in FAULTS + COCO_FAULTS
         self.fault = fault
         train = set(trainable)
         if fault == "res2_trainable":
             train |= {k for k in state_dict if k.startswith("resnet_backbone.res2.") and ".bn" not in k and
                       "downsample.1" not in k and not k.endswith(("running_mean", "running_var", "num_batches_tracked"))}
-        self.p = {}
-        for k, v in state_dict.items():
-            if k.endswith("num_batches_tracked"):
-                continue
-            t = v.detach().to(device=device, dtype=dtype).clone()
-            self.p[k] = t.requires_grad_(k in train)
+        super().__init__(state_dict, depth=depth, dtype=dtype, trainable=train, **kw)
         self.trainable = sorted(train)
-        self.depth, self.num_classes, self.num_seg_classes = depth, num_classes, num_seg_classes
-        self.dconv_from, self.fcn_layers, self.rpn_batch_size = dconv_from, fcn_layers, rpn_batch_size
-        self.dtype, self.device = dtype, device
+        self.rpn_batch_size, self.fcn_with_roi_loss = rpn_batch_size, fcn_with_roi_loss
 
     def grads(self):
         return {k: (None if self.p[k].grad is None else self.p[k].grad.detach()) for k in self.trainable}
 
-    # ------------------------------------------------------------------ primitives
-    def conv(self, x, name, stride=1, padding=0, dilation=1):
-        return F.conv2d(x, self.p[name + ".weight"], self.p.get(name + ".bias"), stride, padding, dilation)
+    # ------------------------------------------------------------------ the frozen stem and the planted faults
+    def stem_res2(self, x):
+        if self.fault == "res2_trainable":
+            return super().stem_res2(x)
+        with torch.no_grad():
+            return super().stem_res2(x)
 
-    def bn(self, x, name):          # frozen BatchNorm, eval mode, NOT folded
-        s = self.p
-        y = F.batch_norm(x, s[name + ".running_mean"], s[name + ".running_var"], s[name + ".weight"], s[name + ".bias"],
-                         False, 0.0, 1e-5)
+    def bn(self, x, name):
+        y = super().bn(x, name)
         if self.fault == "bn_scale_dw":     # the value is right, the gradient skips the BN scale
             y = x + (y - x).detach()
         return y
 
-    def dcn(self, x, offset, name, padding=1, dilation=1):
-        return torchvision.ops.deform_conv2d(x, offset, self.p[name + ".weight"], self.p.get(name + ".bias"), stride=1,
-                                             padding=padding, dilation=dilation)
-
-    # ------------------------------------------------------------------ backbone / FPN / RPN
-    def bottleneck(self, x, p, stride, deformable, has_down):
-        out = F.relu(self.bn(self.conv(x, p + ".conv1", stride), p + ".bn1"))
-        if deformable:
-            out = self.dcn(out, self.conv(out, p + ".conv2_offset", 1, 1, 1), p + ".conv2")
-        else:
-            out = self.conv(out, p + ".conv2", 1, 1, 1)
-        out = F.relu(self.bn(out, p + ".bn2"))
-        out = self.bn(self.conv(out, p + ".conv3"), p + ".bn3")
-        residual = x
-        if has_down:
-            residual = self.bn(self.conv(x, p + ".downsample.0", stride), p + ".downsample.1")
-        return F.relu(out + residual)
-
-    def res_block(self, x, name, blocks, stride, deformable):
-        for i in range(max(blocks, 2)):
-            x = self.bottleneck(x, "resnet_backbone.%s.layers.%d" % (name, i), stride if i == 0 else 1, deformable, i == 0)
-        return x
-
-    def backbone(self, x):
-        with torch.set_grad_enabled(self.fault == "res2_trainable"):
-            c1 = F.relu(self.bn(self.conv(x, "resnet_backbone.conv1.conv1", 2, 3), "resnet_backbone.conv1.bn1"))
-            r2 = self.res_block(F.max_pool2d(c1, 3, 2, 1), "res2", self.depth[0], 1, False)
-        if self.fault != "res2_trainable":
-            r2 = r2.detach()
-        d = self.dconv_from
-        r3 = self.res_block(r2, "res3", self.depth[1], 2, d <= 3)
-        r4 = self.res_block(r3, "res4", self.depth[2], 2, d <= 4)
-        r5 = self.res_block(r4, "res5", self.depth[3], 2, d <= 5)
-        return r2, r3, r4, r5
+    def gap(self, res5):
+        return gap_vector(res5, self.p["fpn.fpn_gap.weight"], self.p["fpn.fpn_gap.bias"], self.fault == "gap_detached")
 
     def fpn(self, r2, r3, r4, r5):
-        up = lambda t: F.interpolate(t, scale_factor=2, mode="nearest")     # noqa: E731
-        p5_1x1 = self.conv(r5, "fpn.fpn_p5_1x1")
-        p4_plus = up(p5_1x1) + self.conv(r4, "fpn.fpn_p4_1x1")
-        p3_plus = up(p4_plus) + self.conv(r3, "fpn.fpn_p3_1x1")
-        p2_plus = up(p3_plus) + self.conv(r2, "fpn.fpn_p2_1x1")
-        p2, p3, p4, p5 = (self.conv(t, "fpn.fpn_p%d" % l, 1, 1) for l, t in ((2, p2_plus), (3, p3_plus), (4, p4_plus),
-                                                                             (5, p5_1x1)))
-        p6 = F.max_pool2d(p5.detach() if self.fault == "p6_grad" else p5, 1, 2)
-        return p2, p3, p4, p5, p6
+        p = super().fpn(r2, r3, r4, r5)
+        if self.fault == "p6_grad":
+            p = p[:4] + (F.max_pool2d(p[3].detach(), 1, 2),)
+        return p
 
-    def rpn(self, feat):
-        x = F.relu(self.conv(feat, "rpn.conv_proposal.0", 1, 1))
-        return self.conv(x, "rpn.cls_score"), self.conv(x, "rpn.bbox_pred")
-
-    # ------------------------------------------------------------------ heads
-    def fcn_head(self, p2, p3, p4, p5):
-        outs = []
-        for l, x in enumerate((p2, p3, p4, p5)):
-            for i in range(self.fcn_layers):
-                p = "fcn_head.fcn_subnet.conv.%d.0" % i
-                x = F.relu(self.dcn(x, self.conv(x, p + ".conv_offset", 1, 1, 1), p + ".conv"))
-            if self.fault == "fcn_level_detached" and l == 2:
-                x = x.detach()
-            outs.append(x if l == 0 else F.interpolate(x, None, 2 ** l, mode="bilinear", align_corners=False))
-        return self.conv(torch.cat(outs, 1), "fcn_head.score")
-
-    def fpn_roi_align(self, feats, rois, ps):
-        r = rois.detach().cpu().numpy().astype(np.float32)
-        w, h = r[:, 3] - r[:, 1] + 1, r[:, 4] - r[:, 2] + 1
-        lv = np.clip(np.floor(2 + np.log2(np.sqrt(w * h) / 224 + 1e-6)), 0, 3).astype(np.int64)    # fpn_roi_align.py:35-38
-        rr = rois.detach().to(feats[0].device, feats[0].dtype)
-        parts, order = [], []
-        for l in range(4):
-            idx = np.where(lv == l)[0]
-            if len(idx):
-                sel = torch.from_numpy(idx).to(rr.device)
-                parts.append(torchvision.ops.roi_align(feats[l], rr[sel], (ps, ps), 1.0 / 2 ** (l + 2), 2, False))
-                order.append(idx)
-        inv = np.argsort(np.concatenate(order))
-        return torch.cat(parts)[torch.from_numpy(inv).to(rr.device)]
-
-    def rcnn(self, feats, rois):
-        x = self.fpn_roi_align(feats, rois, 7).flatten(1)
-        x = F.relu(F.linear(x, self.p["rcnn.fc6.0.weight"], self.p["rcnn.fc6.0.bias"]))
-        x = F.relu(F.linear(x, self.p["rcnn.fc7.0.weight"], self.p["rcnn.fc7.0.bias"]))
-        return (F.linear(x, self.p["rcnn.cls_score.weight"], self.p["rcnn.cls_score.bias"]),
-                F.linear(x, self.p["rcnn.bbox_pred.weight"], self.p["rcnn.bbox_pred.bias"]))
-
-    def mask_branch(self, feats, rois):
-        x = self.fpn_roi_align(feats, rois, 14)
-        for i in range(1, 5):
-            x = F.relu(self.conv(x, "mask_branch.mask_conv%d.0" % i, 1, 1))
-        x = F.relu(F.conv_transpose2d(x, self.p["mask_branch.mask_deconv1.0.weight"],
-                                      self.p["mask_branch.mask_deconv1.0.bias"], 2))
-        return self.conv(x, "mask_branch.mask_score")
+    def fcn_level(self, x, level):
+        x = super().fcn_level(x, level)
+        return x.detach() if self.fault == "fcn_level_detached" and level == 2 else x
 
     # ------------------------------------------------------------------ the step
     def forward(self, image, label, inter):
-        """image [1,3,H,W]; label: the loader's dict (rpn fields, seg_gt, seg_gt_4x, mask_gt); inter: the product's
-        _intermediates.  -> dict of the nine outputs as 0-dim tensors (accuracies as floats)."""
+        """image [1,3,H,W]; label: the loader's dict (rpn fields, seg_gt, seg_gt_4x, mask_gt, and seg_roi_gt with the
+        ROI loss); inter: the product's _intermediates.  -> dict of the nine outputs, plus fcn_roi_loss with the ROI
+        loss, as 0-dim tensors (accuracies as floats)."""
         dev, dt = self.device, self.dtype
         r2, r3, r4, r5 = self.backbone(image.to(dev, dt))
         fpn = self.fpn(r2, r3, r4, r5)
         rpn = [self.rpn(f) for f in fpn]
         rpn_cls = rpn_box = 0
-        for (score, pred), s in zip(rpn, STRIDES):
+        for (score, pred, _), s in zip(rpn, STRIDES):
             h, w = score.shape[2:]
             sl = lambda k: label[k % s].to(dev)[:, :, :h, :w]             # noqa: E731
             lab = sl("rpn_labels_fpn%d")
@@ -173,13 +116,13 @@ class TrainOracle:
             rpn_box = rpn_box + TO._smooth_l1(pred, sl("rpn_bbox_targets_fpn%d").to(dt),
                                               sl("rpn_bbox_inside_weights_fpn%d").to(dt),
                                               sl("rpn_bbox_outside_weights_fpn%d").to(dt), 3.0).sum()
-        score = self.fcn_head(*fpn[:4])
-        up = F.interpolate(score, None, 4, mode="bilinear", align_corners=False)
-        fcn_loss = TO.semantic_from_logits(up, label["seg_gt"].to(dev))[0]
+        fcn = self.fcn_head(*fpn[:4])
+        fcn_loss = TO.semantic_from_logits(fcn["fcn_output"], label["seg_gt"].to(dev))[0]
 
         t = inter["proposal_targets"]
         feats = list(fpn[:4])
-        cls_score, bbox_pred = self.rcnn(feats, t["rois"])
+        rcnn = self.rcnn(feats, t["rois"])
+        cls_score, bbox_pred = rcnn["cls_score"], rcnn["bbox_pred"]
         lab = t["labels"].to(dev).long()
         cls_loss = F.cross_entropy(cls_score, lab, ignore_index=-1)
         box = TO._smooth_l1(bbox_pred, *(t[k].to(dev, dt) for k in ("bbox_targets", "bbox_inside_weights",
@@ -201,19 +144,24 @@ class TrainOracle:
         pm = self.mask_branch(feats, gt_rois)
         if self.fault == "pan_mask_grad":
             pm = pm.detach()
-        logits = PO.panoptic_logits(score.cpu().to(dt), pm.cpu().to(dt), gt_rois.detach().cpu().numpy(), cls_idx.cpu().numpy(),
-                                    self.num_classes, keep is not None)
+        logits = PO.panoptic_logits(fcn["fcn_score"].cpu().to(dt), pm.cpu().to(dt), gt_rois.detach().cpu().numpy(),
+                                    cls_idx.cpu().numpy(), self.num_classes, keep is not None)
         gt = PO.panoptic_gt(label["seg_gt_4x"].cpu().numpy(), label["mask_gt"].cpu().numpy(),
                             None if keep is None else np.asarray(keep), self.num_seg_classes, self.num_classes)
         panoptic_loss, correct, ignored = PO.loss_and_accuracy(logits, gt)
-        return {"rpn_cls_loss": rpn_cls, "rpn_bbox_loss": rpn_box, "cls_loss": cls_loss, "bbox_loss": bbox_loss,
-                "mask_loss": mask_loss, "fcn_loss": fcn_loss, "panoptic_loss": panoptic_loss.to(dev),
-                "rcnn_accuracy": rcnn_acc, "panoptic_accuracy": correct / float(gt.size - ignored)}
+        out = {"rpn_cls_loss": rpn_cls, "rpn_bbox_loss": rpn_box, "cls_loss": cls_loss, "bbox_loss": bbox_loss,
+               "mask_loss": mask_loss, "fcn_loss": fcn_loss, "panoptic_loss": panoptic_loss.to(dev),
+               "rcnn_accuracy": rcnn_acc, "panoptic_accuracy": correct / float(gt.size - ignored)}
+        if self.fcn_with_roi_loss:
+            rois, seg = inter["fcn_rois"].to(dev), label["seg_roi_gt"].to(dev)
+            out["fcn_roi_loss"] = roi_loss(fcn["fcn_feat"], self.p["fcn_head.score.weight"], self.p["fcn_head.score.bias"],
+                                           rois, seg, keep if self.fault == "rois_after_keep" else None)
+        return out
 
     def step(self, image, label, inter):
-        """forward + backward of the sum of the seven losses -> (outputs as floats, grads)."""
+        """forward + backward of the sum of the losses -> (outputs as floats, grads)."""
         out = self.forward(image, label, inter)
-        total = sum(out[k] for k in LOSSES)
+        total = sum(out[k] for k in COCO_LOSSES if k in out)
         total.backward()
         return {k: float(v.detach()) if torch.is_tensor(v) else float(v) for k, v in out.items()}, self.grads()
 
@@ -233,6 +181,7 @@ def grad_tol(name, prec):
     return (OFFSET_GRAD_TOL if "offset" in name else GRAD_TOL)[prec]
 
 LOSSES = ("rpn_cls_loss", "rpn_bbox_loss", "cls_loss", "bbox_loss", "mask_loss", "fcn_loss", "panoptic_loss")
+COCO_LOSSES = LOSSES + ("fcn_roi_loss",)
 OUTPUTS = LOSSES + ("rcnn_accuracy", "panoptic_accuracy")
 
 
