@@ -364,9 +364,12 @@ int upsnet_unified_pan_result(const long long *seg, const long long *pan, const 
  * as OpenCV does when factors are given); (out_h,out_w) = the resized size (cvRound(h*scale), cvRound(w*scale));
  * (pad_h,pad_w) >= it; blob fp32 [3,pad_h,pad_w]: resized (image - pixel_means), zeros in the padding.  The means are
  * float64 like config.network.pixel_means: numpy subtracts in double and stores float32 (base_dataset.py:154).
+ * flip != 0: the image is mirrored first, as get_image_blob does for a flipped roidb entry (base_dataset.py:128-129,
+ * im[:, ::-1, :]): source column x is read as w - 1 - x before the mean subtraction and the bilinear taps, so the blob
+ * equals, bit for bit, the one of a host-flipped copy with flip = 0.
  */
 int upsnet_prep_image(const unsigned char *image_hwc, int h, int w, double scale, int out_h, int out_w, int pad_h,
-                      int pad_w, const double pixel_means[3], float *blob, void *stream);
+                      int pad_w, const double pixel_means[3], float *blob, int flip, void *stream);
 
 /* upsnet_label_restore: a network-resolution label map back to the original image size.
  * replaces: upsnet_end2end_test.py:259-266 -- crop [:h,:w], astype(uint8) (values wrap mod 256), cv2.resize(fx = fy,

@@ -11,7 +11,8 @@ from .operators import (DeformConv, DeformConvWithOffset, ModDeformConv, ModDefo
 from .pipeline import PipelinedEngine  # noqa: F401,E402
 from .evaluation import PanopticQuality, SegmentationIoU, DetectionAP  # noqa: F401,E402
 from .training import (Conv2dFunction, ConvTranspose2x2Function, FlatBucketAllReduce, LRSchedule,  # noqa: F401,E402
-                       FcnRoiLoss, MaskRCNNLoss, PanopticLabels, PanopticLoss, RPNLoss, SemanticLoss, SGD)
+                       FcnRoiLoss, MaskRCNNLoss, PanopticLabels, PanopticLoss, RPNLoss, SemanticLoss, SGD,
+                       TrainingSample)
 
 __all__ = ["PipelinedEngine", "DeformConv", "DeformConvWithOffset", "ModDeformConv", "ModDeformConvWithOffsetMask",
            "ModulatedDeformConv", "RoIAlign", "ROIAlign", "RoIAlignFunction", "FPNRoIAlign", "PanopticHead",
@@ -19,5 +20,5 @@ __all__ = ["PipelinedEngine", "DeformConv", "DeformConvWithOffset", "ModDeformCo
            "conv2d", "linear", "deform_conv", "roi_align", "fpn_roi_align", "nms", "nms_segmented", "gpu_nms",
            "gpu_nms_wrapper", "panoptic_fuse", "set_precision", "unified_pan_result", "prep_image", "im_post", "im_post_rle",
            "label_restore", "combined_pan_result", "get_combined_pan_result", "PanopticQuality", "SegmentationIoU", "DetectionAP",
-           "PanopticLoss", "PanopticLabels", "SemanticLoss", "FcnRoiLoss", "RPNLoss", "MaskRCNNLoss", "SGD", "LRSchedule",
+           "PanopticLoss", "PanopticLabels", "TrainingSample", "SemanticLoss", "FcnRoiLoss", "RPNLoss", "MaskRCNNLoss", "SGD", "LRSchedule",
            "FlatBucketAllReduce", "Conv2dFunction", "ConvTranspose2x2Function"]

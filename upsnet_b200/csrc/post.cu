@@ -131,23 +131,27 @@ __device__ __forceinline__ void lin_coef(int d, int n_src, double scale, int& s,
 
 __global__ void __launch_bounds__(256)
 prep_image_kernel(const unsigned char* __restrict__ src, int h, int w, int ho, int wo, int Hp, int Wp, double inv_scale,
-                  double m0, double m1, double m2, float* __restrict__ out) {
+                  double m0, double m1, double m2, int flip, float* __restrict__ out) {
   const size_t plane = (size_t)Hp * Wp;
   // cv2.resize(im, None, None, fx, fy): the source step is 1 / fx -- the given factor, NOT the ratio of the rounded sizes
   const double sx = inv_scale, sy = inv_scale;
   const bool same = (h == ho && w == wo);
+  // flip: column x of the flipped image (get_image_blob's im[:, ::-1, :]) is source column w - 1 - x.  Every column index
+  // goes through it after the tap geometry, so the result is the kernel's output for a host-flipped copy, bit for bit.
+  const int xr = flip ? w - 1 : 0, xs = flip ? -1 : 1;
   for (size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x; p < plane; p += (size_t)gridDim.x * blockDim.x) {
     const int y = (int)(p / Wp), x = (int)(p - (size_t)y * Wp);
     float v0 = 0.f, v1 = 0.f, v2 = 0.f;
     if (y < ho && x < wo) {
       if (same) {
-        const unsigned char* q = src + ((size_t)y * w + x) * 3;
+        const unsigned char* q = src + ((size_t)y * w + (xr + xs * x)) * 3;
         v0 = (float)((double)q[0] - m0); v1 = (float)((double)q[1] - m1); v2 = (float)((double)q[2] - m2);   // numpy: float64 subtract, float32 store
       } else {
         int x0, y0; float fx, fy;
         lin_coef(x, w, sx, x0, fx);
         lin_coef(y, h, sy, y0, fy);
-        const int x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
+        const int x1 = xr + xs * min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
+        x0 = xr + xs * x0;
         const unsigned char* a = src + ((size_t)y0 * w + x0) * 3; const unsigned char* b = src + ((size_t)y0 * w + x1) * 3;
         const unsigned char* c = src + ((size_t)y1 * w + x0) * 3; const unsigned char* d = src + ((size_t)y1 * w + x1) * 3;
         const float gx = __fsub_rn(1.f, fx), gy = __fsub_rn(1.f, fy);
@@ -224,14 +228,15 @@ extern "C" int upsnet_unified_pan_result(const long long* seg, const long long* 
 }
 
 extern "C" int upsnet_prep_image(const unsigned char* image_hwc, int h, int w, double scale, int out_h, int out_w, int pad_h,
-                                 int pad_w, const double pixel_means[3], float* blob, void* stream) {
+                                 int pad_w, const double pixel_means[3], float* blob, int flip, void* stream) {
   if (!image_hwc || !blob || !pixel_means) return UPSNET_E_BADARG;
   if (h <= 0 || w <= 0 || out_h <= 0 || out_w <= 0 || pad_h < out_h || pad_w < out_w || !(scale > 0.0)) return UPSNET_E_BADARG;
   const size_t plane = (size_t)pad_h * pad_w;
   size_t blocks = (plane + 255) / 256;
   if (blocks > (size_t)ups::kNumSMs * 16) blocks = (size_t)ups::kNumSMs * 16;
   ups::prep_image_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(image_hwc, h, w, out_h, out_w, pad_h, pad_w, 1.0 / scale,
-                                                                              pixel_means[0], pixel_means[1], pixel_means[2], blob);
+                                                                              pixel_means[0], pixel_means[1], pixel_means[2],
+                                                                              flip ? 1 : 0, blob);
   UPS_CHECK_LAUNCH();
   return 0;
 }

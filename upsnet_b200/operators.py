@@ -1217,10 +1217,11 @@ def unified_pan_result(seg, pan, cls_inds, num_seg_classes, num_classes, stuff_a
     return out
 
 
-def prep_image(image_hwc_u8, pixel_means, scale=1.0, stride=32):
+def prep_image(image_hwc_u8, pixel_means, scale=1.0, stride=32, flip=False):
     """dataset/base_dataset.py:143-174 prep_im_for_blob + :898-923 im_list_to_blob on the device: uint8 [h,w,3] (BGR)
     -> fp32 blob [1,3,Hp,Wp] (mean-subtracted, bilinearly resized by `scale`, zero-padded to a multiple of `stride`)
-    and the resized (h, w)."""
+    and the resized (h, w).  flip=True mirrors the image first (get_image_blob's im[:, ::-1, :] for a flipped roidb
+    entry), bit-identical to passing a flipped copy."""
     require_cuda(image_hwc_u8)
     assert image_hwc_u8.dtype == torch.uint8 and image_hwc_u8.dim() == 3 and image_hwc_u8.shape[2] == 3
     im = image_hwc_u8.contiguous()
@@ -1230,7 +1231,7 @@ def prep_image(image_hwc_u8, pixel_means, scale=1.0, stride=32):
     blob = torch.empty((1, 3, Hp, Wp), dtype=torch.float32, device=im.device)
     pm = (C.c_double * 3)(*[float(v) for v in pixel_means])
     with _Timed("prep_image", 1, {"bytes": 3.0 * h * w + 12.0 * Hp * Wp}, im.device):
-        call("prep_image", im.device, im, h, w, float(scale), ho, wo, Hp, Wp, pm, blob)
+        call("prep_image", im.device, im, h, w, float(scale), ho, wo, Hp, Wp, pm, blob, int(bool(flip)))
     return blob, (ho, wo)
 
 

@@ -24,6 +24,8 @@
   targets and the class-specific polygon mask targets.
 * PanopticLabels: the label maps of the semantic and panoptic heads (seg_gt, seg_gt_4x, mask_gt, seg_roi_gt), built by
   the reference's data loaders on the host, on the device (csrc/labels.cu), with Pillow's polygon fill restated.
+* TrainingSample: the (data, label) pair of one roidb entry as the reference's loader and collate yield it (scale draw,
+  horizontal flip, image blob, im_info, RPN targets, label maps), from the decoded uint8 image and label map.
 * PanopticLoss: the panoptic head of the training forward (models/resnet_upsnet.py:144-179: SegTerm, MaskTerm, the void
   logits, MaskMatching, calc_panoptic_acc and the cross-entropy) as one fused loss with hand-written forward and
   backward kernels (csrc/panoptic_loss.cu), plus the two host helpers for the lines before it (gt_rois, draw_keep).
@@ -57,7 +59,7 @@ from torch.optim.optimizer import required
 
 from . import _lib
 from ._lib import call, f32c, query_bytes, require_cuda
-from .operators import _weight_cache
+from .operators import _weight_cache, prep_image
 
 
 def _conv_out(n, pad, dil, k, stride):
@@ -1742,3 +1744,92 @@ class PanopticLabels:
         lab = label_map if torch.is_tensor(label_map) else torch.from_numpy(np.ascontiguousarray(label_map, np.uint8))
         packed = self.pack_roidb(entry, im_scale, device)
         return self(lab.to(device), packed, im_shape, im_scale, bool(entry["flipped"]), mask_dtype=torch.int64)
+
+
+# ------------------------------------------------------------------------------------------------
+# one training sample: the loader's __getitem__ (phase train) + collate
+# ------------------------------------------------------------------------------------------------
+class TrainingSample:
+    """The (data, label) pair the reference's DataLoader yields for one roidb entry (dataset/cityscapes.py:117-193,
+    dataset/coco.py:124-191 with phase 'train', and collate, dataset/base_dataset.py:952-988), built on the device:
+
+      data  = {'data': float32 [1,3,Hp,Wp] (prep_image, flipped as the entry says), 'im_info': numpy float32 [1,3]}
+      label = {'roidb': the entry's minimal roidb (add_rpn_blobs' valid_keys), the RPN fields of RPNTargets,
+               'seg_gt', 'seg_gt_4x', 'mask_gt' (int64), 'seg_roi_gt' with train.fcn_with_roi_loss (PanopticLabels),
+               'gt_classes': every row (cityscapes) or the non-crowd rows (coco), in the entry's dtype}
+
+    The scale is drawn as get_image_blob draws it, np.random.randint(0, high=len(scales), size=1), and capped by
+    prep_im_for_blob's max_size rule in float64, so under the same np.random state the reference and this class train
+    at the same scale; the RPN subsampling seed is drawn after it (RPNTargets).  Built from the reference's `config`
+    (train.scales, train.max_size, network.pixel_means, network.rpn_feat_stride[-2], and what RPNTargets and
+    PanopticLabels read) or from the same values as keywords (the rest go to RPNTargets); `dataset` selects the loader,
+    "cityscapes" or "coco".
+
+    Not built here: data_4x (collate makes it, no module of the model reads it); the image and PNG decoding (host);
+    RLE segmentations (PanopticLabels rejects them); the flipped entries themselves (extend_with_flipped_entries: a
+    flipped entry carries flipped boxes and segms and flipped=True); any stream or prefetch machinery."""
+
+    ROIDB_KEYS = ("boxes", "segms", "seg_areas", "gt_classes", "gt_overlaps", "is_crowd", "box_to_gt_ind_map")
+
+    def __init__(self, config=None, *, dataset="cityscapes", scales=(800,), max_size=1333,
+                 pixel_means=(102.9801, 115.9465, 122.7717), stride=32, mask_size=28, with_roi=None, **rpn):
+        if config is not None:
+            if not config.network.use_caffe_model:
+                raise _lib.UpsnetError("training_sample: only network.use_caffe_model (mean subtraction) is built")
+            scales, max_size = config.train.scales, config.train.max_size
+            pixel_means, stride = config.network.pixel_means, config.network.rpn_feat_stride[-2]
+            self.rpn = RPNTargets(config)
+            self.labels = PanopticLabels(config, dataset=dataset, with_roi=with_roi)
+        else:
+            self.rpn = RPNTargets(max_size=max_size, **rpn)
+            self.labels = PanopticLabels(dataset=dataset, mask_size=mask_size, with_roi=with_roi, stride=stride)
+        if len(scales) == 0:
+            raise _lib.UpsnetError("training_sample: no train.scales")
+        self.scales, self.max_size = list(scales), max_size
+        self.pixel_means = [float(v) for v in pixel_means]
+        self.stride, self.dataset = int(stride), dataset
+
+    def im_scale(self, target_size, h, w):
+        """prep_im_for_blob's scale of an h x w image for one target size (base_dataset.py:158-168)."""
+        size_min, size_max = min(h, w), max(h, w)
+        s = float(target_size) / float(size_min)
+        if np.round(s * size_max) > self.max_size:
+            s = float(self.max_size) / float(size_max)
+        return s
+
+    def draw_scale(self, h, w):
+        """get_image_blob's draw (base_dataset.py:119-121) -> (scale index, im_scale)."""
+        ind = int(np.random.randint(0, high=len(self.scales), size=1)[0])
+        return ind, self.im_scale(self.scales[ind], h, w)
+
+    def sample(self, entry, image_bgr_u8, label_map_u8, device, seed=None):
+        """entry: a roidb entry; image_bgr_u8: the decoded image uint8 [h,w,3] and label_map_u8: the decoded label PNG
+        uint8 [h,w], both as read from disk (not flipped), numpy arrays or tensors; seed: RPNTargets' subsampling seed
+        (None draws it from np.random after the scale).  -> (data, label) as in the class docstring.  Bad input raises
+        UpsnetError before any kernel is launched."""
+        h, w = int(entry["height"]), int(entry["width"])
+        im, lab = (x if torch.is_tensor(x) else torch.from_numpy(np.ascontiguousarray(x))
+                   for x in (image_bgr_u8, label_map_u8))
+        if im.dtype != torch.uint8 or tuple(im.shape) != (h, w, 3):
+            raise _lib.UpsnetError("training_sample: the image is %s %s, the entry's is uint8 (%d, %d, 3)"
+                                   % (im.dtype, tuple(im.shape), h, w))
+        if lab.dtype != torch.uint8 or tuple(lab.shape) != (h, w):
+            raise _lib.UpsnetError("training_sample: the label map is %s %s, the entry's is uint8 (%d, %d)"
+                                   % (lab.dtype, tuple(lab.shape), h, w))
+        cls, crowd = np.asarray(entry["gt_classes"]), np.asarray(entry["is_crowd"])
+        if not ((cls > 0) & (crowd == 0)).any():
+            raise _lib.UpsnetError("training_sample: no ground-truth boxes (add_rpn_blobs fails on such an entry)")
+        _, s = self.draw_scale(h, w)
+        ho, wo = int(np.rint(h * s)), int(np.rint(w * s))
+        flipped = bool(entry["flipped"])
+        # the host half of the label maps first: a polygon or canvas they reject raises before any launch
+        packed = self.labels.pack_roidb(entry, s, device)
+        tab = self.labels.prepare((h, w), packed, (ho, wo), s, flipped, device)
+        blob, _ = prep_image(im.to(device, non_blocking=True), self.pixel_means, s, self.stride, flip=flipped)
+        data = {"data": blob, "im_info": np.array([[np.round(h * s), np.round(w * s), s]], np.float32)}
+        label = {"roidb": {k: entry[k] for k in self.ROIDB_KEYS if k in entry}}
+        label.update(self.rpn.from_roidb(entry, s, device, seed))
+        label.update(self.labels.launch(lab.to(device, non_blocking=True), packed, tab, mask_dtype=torch.int64))
+        rows = np.arange(len(cls)) if self.dataset == "cityscapes" else np.flatnonzero(crowd == 0)
+        label["gt_classes"] = torch.from_numpy(np.ascontiguousarray(cls[rows])).to(device)
+        return data, label
