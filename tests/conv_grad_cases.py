@@ -1,7 +1,8 @@
 """The layer harness of the dense-conv backward tests (tests/test_gpu_conv_backward.py, test_gpu_conv_backward_wide.py):
 one layer through upsnet_b200.training.conv2d / linear / conv_transpose2x2, forward and backward, against float64
 autograd of F.conv2d / F.linear / F.conv_transpose2d on the device, element by element through grad_oracle.check at the
-a-priori constants of conv_grad_oracle.apriori (or TOL where it is tighter).  The float64 reference takes the same
+a-priori constants of conv_grad_oracle.apriori (or TOL where it is tighter), and the forward output y against
+conv_grad_oracle.forward at conv_grad_oracle.forward_c.  The float64 reference takes the same
 float32 x, W, b, residual and dY, and the ReLU mask of the kernel's own forward output (so that an output at exactly 0
 cannot decide the mask differently).  WORST collects the worst err / bound per (case, precision, gradient)."""
 import math
@@ -13,7 +14,7 @@ import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import grad_oracle as G  # noqa: E402
-from conv_grad_oracle import apriori  # noqa: E402
+from conv_grad_oracle import apriori, forward, forward_c  # noqa: E402
 
 WORST = {}
 # About 4x the worst err / bound measured on the H100 (bf16x3: dX 1.73e-5 at the RPN cls head, dW 1.34e-5 at fc6), used
@@ -36,6 +37,25 @@ def _check(name, prec, grad, got, want, bound, K, splits=1):
     key = "%s %s %s" % (name, prec, grad)
     WORST[key] = max(WORST.get(key, 0.0), ratio)
     assert ok, "%s: worst err/bound %.3e > c %.3e" % (key, ratio, c_use)
+
+
+def _check_y(name, prec, y, x, w, b=None, stride=1, pad=0, dil=1, r=None, up2=False, relu=False):
+    """The forward output y (float32 [N, Cout, Ho, Wo]) element by element against conv_grad_oracle.forward on the copy
+    of x the kernel reads (the hi / lo pair of x for bf16x3, bf16(x) for bf16)."""
+    from upsnet_b200 import operators as ops
+    x = x.detach()
+    if prec == "bf16x3":
+        C, st = x.shape[1], ops.Pair.from_float(x).store
+        xr = tuple(st[..., i * C:(i + 1) * C].double().permute(0, 3, 1, 2) for i in (0, 1))
+    else:
+        xr = x.bfloat16().double()
+    want, bound, _ = forward(xr, w.detach(), None if b is None else b.detach(), stride, pad, dil,
+                             None if r is None else r.detach(), up2, relu, prec)
+    c = forward_c(prec, w.shape[1] * w.shape[2] * w.shape[3], int(b is not None) + int(r is not None))
+    ok, ratio = G.check(y.detach(), want, bound, c)
+    key = "%s %s y" % (name, prec)
+    WORST[key] = max(WORST.get(key, 0.0), ratio)
+    assert ok, "%s: worst err/bound %.3e > c %.3e" % (key, ratio, c)
 
 
 def _rand(shape, dev, scale=1.0, seed=0):
@@ -79,6 +99,7 @@ def run_conv(dev, name, prec, N, Cin, H, W, Cout, k, stride=1, pad=0, dil=1, bia
     xg = x.clone().requires_grad_(need_x)
     y = training.conv2d(xg, w, b, stride, pad, dil, residual=r, residual_up2=(res == "up2"), relu=relu, precision=prec)
     assert y.shape == (N, Cout, Ho, Wo) and y.dtype == torch.float32
+    _check_y(name, prec, y, x, w, b, stride, pad, dil, r, res == "up2", relu)
     dy = _rand((N, Cout, Ho, Wo), dev, 1.0, seed + 4)
     if nhwc_dy:
         dy = dy.contiguous(memory_format=torch.channels_last)
@@ -108,6 +129,7 @@ def _run_linear(dev, name, prec, R, K, Cout, relu, seed, bias=True):
     w = _rand((Cout, K), dev, (2.0 / K) ** 0.5, seed + 1).requires_grad_(True)
     b = _rand((Cout,), dev, 0.1, seed + 2).requires_grad_(True) if bias else None
     y = training.linear(x, w, b, relu=relu, precision=prec)
+    _check_y(name, prec, y.reshape(R, Cout, 1, 1), x.reshape(R, K, 1, 1), w.reshape(Cout, K, 1, 1), b, relu=relu)
     dy = _rand((R, Cout), dev, 1.0, seed + 3)
     y.backward(dy)
     g = dy.double() * (y.detach() > 0).double() if relu else dy.double()
@@ -126,8 +148,10 @@ def run_deconv(dev, name, prec, R, Cin, C, H, seed):
     b = _rand((C,), dev, 0.1, seed + 2).requires_grad_(True)
     y = training.conv_transpose2x2(x, w, b, relu=True, precision=prec)
     assert y.shape == (R, C, 2 * H, 2 * H)
-    y64 = torch.relu(F.conv_transpose2d(x.detach().double(), w.detach().double(), b.detach().double(), stride=2))
-    assert float((y.detach().double() - y64).abs().max()) < 0.1
+    # the 1x1 conv to 4 C channels ordered (a, b, c) the kernel runs, then the pixel shuffle
+    w1 = w.detach().permute(2, 3, 1, 0).reshape(4 * C, Cin, 1, 1)
+    y1 = y.detach().reshape(R, C, H, 2, H, 2).permute(0, 3, 5, 1, 2, 4).reshape(R, 4 * C, H, H)
+    _check_y(name, prec, y1, x, w1, b.detach().repeat(4), relu=True)
     dy = _rand(y.shape, dev, 1.0, seed + 3)
     y.backward(dy)
     g = dy.double() * (y.detach() > 0).double()

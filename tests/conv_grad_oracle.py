@@ -11,12 +11,24 @@
   image's first row), the compact stride-2 result scattered to the odd pixels or one pixel off.
 """
 import math
+import os
+import sys
 
 import torch
 import torch.nn.functional as F
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import grad_oracle as G  # noqa: E402
+
 
 def apriori(prec, grad, K, splits=1):
+    if grad == "y":
+        # forward accumulation of K exact products per output (tests/test_gpu_conv_forward_fp64.py): the tensor core adds
+        # the 16 products of one wgmma step to the fp32 accumulator with at most 2 * 2^-24 of the magnitudes, three MMAs
+        # per step in bf16x3; the CUDA-core kernel chains K fp32 FMAs
+        if prec == "fp32":
+            return K * 2.0 ** -24
+        return (3 if prec == "bf16x3" else 1) * math.ceil(K / 16) * 2.0 ** -23
     if grad == "db":
         return 2.0 ** -23
     if grad == "dres":
@@ -99,6 +111,142 @@ def wgrad(x, g, kh, kw, padding, dilation, prec, splits=1, drop=None, shift=0):
                 a, b = bounds[s], bounds[s + 1]
                 dw[:, :, ki, kj] += _products(gt[a:b], xt[a:b], prec, lambda u, v: u.t() @ v)
     return dw
+
+
+EPI = 2.0 ** -23               # one fp32 add of the epilogue (bias, residual), relative to the bound
+SIGMOID_SLACK = 2.0 ** -21     # expf (2 ulp), the add and the division of 1 / (1 + e^-o), relative to the result
+# About 4x the worst forward err / bound measured on an NVIDIA H100 80GB HBM3 (SXM, power limit 700 W), used where it is
+# below the a-priori constant: bf16x3 3.1e-6 (fc6, K = 12544: the gather kernel on the engine's rows and the training
+# forward), bf16 1.0e-6 (training forward; the engine's rows 5.4e-7), fp32 4.0e-7 (res4.0 downsample on the CUDA-core
+# kernel)
+FWD_TOL = {"bf16x3": 1.2e-5, "bf16": 4e-6, "fp32": 1.6e-6}
+
+
+def forward_c(prec, K, adds):
+    """The constant c of |kernel - forward| <= c * bound + slack + 1e-6 for an output made of K products and `adds`
+    epilogue additions: the a-priori accumulation and epilogue terms, or FWD_TOL[prec] where that is tighter."""
+    c = apriori(prec, "y", K) + adds * EPI
+    return min(c, FWD_TOL[prec]) if prec in FWD_TOL else c
+
+
+def store_slack(y, bound, c, out):
+    """The rounding of the stored result o, |o| <= |y| + c * bound: half a bf16 ulp of |o| (bf16 output), the hi / lo
+    split's 2^-17 |o| (pair output), nothing (fp32)."""
+    top = y.abs() + c * bound
+    if out == "bf16":
+        return G.half_ulp_bf16(top)
+    if out == "pair":
+        return 2.0 ** -17 * top
+    return torch.zeros_like(y)
+
+
+def _split_rne(v, trunc=False):
+    hi = G.bf16_round(v, trunc)
+    return hi, G.bf16_round(v - hi, trunc)
+
+
+def forward(x, weight, bias=None, stride=1, padding=0, dilation=1, residual=None, residual_up2=False, relu=False,
+            prec="bf16x3", sigmoid_from=None, fault=None, dtype=torch.float64):
+    """(y, bound, slack) in float64 of one dense conv as the forward kernels compute it (csrc/igemm_tma.cu,
+    csrc/igemm_tc.cu, csrc/igemm_simt.cu): the exact sum of the products the kernel issues, on the operands it sees,
+    then bias, residual (same size, or nearest x2 with residual_up2), ReLU and the sigmoid of the channels from
+    sigmoid_from on.  bound: the sum of |terms| (products, bias, residual), over 4 on the sigmoid channels; slack: the
+    sigmoid's own rounding (None without one).
+      x: the activation values the kernel reads, a float tensor [N,Cin,H,W], or the tuple (hi, lo) of a pair.
+      weight: fp32, split by upsnet_igemm_pack_weight into hi = bf16(w), lo = bf16(w - hi) (round to nearest even).
+      prec 'bf16x3': lo*hi + hi*lo + hi*hi, fp32 activations split the same way in the kernel; 'bf16': hi*hi, fp32
+      activations rounded to bf16; 'fp32': the plain products (CUDA-core kernel).  residual: the values the epilogue
+      adds (hi + lo of a pair residual).
+    Planted faults for tests/test_conv_grad_oracle_cpu.py: 'shift' (every tap reads one pixel to the right), 'stacked'
+    (the N images read as one tall image: a tap past the last row of one image reads the next one's first row),
+    'drop_kblock' (the last 64-channel k-block of the last tap left out), 'tile_from' (output channels 0..63 computed
+    from the weight rows 64..127), 'drop_lohi' (the lo*hi MMA left out), 'trunc' (the activation split, or the bf16
+    rounding, truncates), 'odd' (a stride-2 1x1 reads the odd pixels), 'up2_off' (the up2 residual read at column
+    (w + 1) / 2), 'bias_next' (channel co gets the bias of co + 1), 'sigmoid_early' (the sigmoid starts one channel
+    early), 'relu_first' (ReLU applied before the residual).
+    dtype=torch.float32 sums the products (exact in fp32 but for prec 'fp32') and runs the epilogue in fp32 instead: an
+    emulation of the kernels' accumulation that the bounds must accept."""
+    dt = torch.float64
+    Cout, _, kh, kw = weight.shape
+    trunc = fault == "trunc"
+    if isinstance(x, tuple):
+        assert prec == "bf16x3", "pair activations belong to precision bf16x3"
+        xh, xl = (t.to(dt) for t in x)
+    else:
+        xv = x.to(dt)
+        if prec == "bf16x3":
+            xh, xl = _split_rne(xv, trunc)
+        elif prec == "bf16":
+            xh = G.bf16_round(xv, trunc)
+    w = weight.to(dt)
+    if fault == "tile_from":
+        w = w.clone()
+        w[0:64] = w[64:128]
+    if fault == "drop_kblock":
+        w = w.clone()
+        w[:, -64:, -1, -1] = 0
+    # (activation, weight, |weight| of the products it stands for); hi*hi + hi*lo as one product with hi + lo (exact in
+    # float64: 8 by 17 bits), so that a large layer needs two float64 convolutions instead of three
+    if prec == "fp32":
+        terms = [(xv, w, w.abs())]
+    else:
+        wh, wl = _split_rne(w)
+        terms = [(xh, wh, wh.abs())] if prec == "bf16" else [(xh, wh + wl, wh.abs() + wl.abs())]
+        if prec == "bf16x3" and fault != "drop_lohi":
+            terms.append((xl, wh, wh.abs()))
+    s = stride if isinstance(stride, int) else stride[0]
+
+    def conv(a, b):
+        if s != 1 and kh == kw == 1:          # the strided view of a 1x1 / pad 0 layer: every s-th row and pixel
+            Ho, Wo = (a.shape[2] - 1) // s + 1, (a.shape[3] - 1) // s + 1
+            o = 1 if fault == "odd" else 0
+            v = torch.zeros(a.shape[:2] + (Ho, Wo), dtype=a.dtype, device=a.device)
+            part = a[:, :, o::s, o::s]
+            v[:, :, :part.shape[2], :part.shape[3]] = part
+            a = v
+        if fault == "shift":
+            a = F.pad(a, (0, 1))[..., 1:]
+        if fault == "stacked":
+            N, C, H, W = a.shape
+            tall = a.transpose(0, 1).reshape(1, C, N * H, W)
+            y = F.conv2d(tall, b, None, 1, padding, dilation)
+            return y.reshape(Cout, N, -1, y.shape[3]).transpose(0, 1)
+        return F.conv2d(a, b, None, 1 if kh == kw == 1 else s, padding, dilation)
+
+    def rnd(t):
+        return t.to(dtype).double()
+
+    y = rnd(sum(conv(a.to(dtype), b.to(dtype)).double() for a, b, _ in terms))
+    bound = sum(conv(a.abs(), ba) for a, _, ba in terms)
+    if bias is not None:
+        bv = bias.to(dt)
+        if fault == "bias_next":
+            bv = torch.cat([bv[1:], bv[:1]])
+        y = rnd(y + bv.view(1, -1, 1, 1))
+        bound = bound + bv.abs().view(1, -1, 1, 1)
+    if residual is not None:
+        r = residual.to(dt)
+        if residual_up2:
+            r = r.repeat_interleave(2, 2)
+            cols = torch.arange(y.shape[3], device=y.device) // 2
+            if fault == "up2_off":
+                cols = ((torch.arange(y.shape[3], device=y.device) + 1) // 2).clamp_max(r.shape[3] - 1)
+            r = r[..., cols]
+        if fault == "relu_first":
+            y = y.clamp_min(0)
+        y = rnd(y + r)
+        bound = bound + r.abs()
+    if relu and fault != "relu_first":
+        y = y.clamp_min(0)
+    slack = None
+    if sigmoid_from is not None:
+        s0 = sigmoid_from - 1 if fault == "sigmoid_early" else sigmoid_from
+        y, bound = y.clone(), bound.clone()
+        y[:, s0:] = rnd(torch.sigmoid(y[:, s0:]))
+        bound[:, s0:] = bound[:, s0:] / 4
+        slack = torch.zeros_like(y)
+        slack[:, s0:] = SIGMOID_SLACK * y[:, s0:]
+    return y, bound, slack
 
 
 def reference(x, weight, dy, padding, dilation, y=None, stride=1):

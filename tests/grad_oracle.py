@@ -153,6 +153,18 @@ def half_ulp_bf16(v):
     return torch.where(v == 0, 0.0, torch.ldexp(torch.ones_like(v), e - 9))
 
 
+def check_pair_split(store):
+    """A pair tensor [..., 2C] is normalised: hi == bf16(hi + lo) and |lo| <= half an ulp of hi.  When o - hi lies just
+    below half an ulp, lo = bf16(o - hi) rounds up to exactly half an ulp and hi + lo is a rounding midpoint (about 1 in
+    1000 elements of Pair.from_float); there either neighbour is a nearest bf16 value, so hi passes if it is one of them."""
+    c = store.shape[-1] // 2
+    hi, lo = store[..., :c].double(), store[..., c:].double()
+    v = hi + lo
+    r = bf16_round(v)
+    assert bool(((r == hi) | ((v - hi).abs() == (v - r).abs())).all()), "hi is not the bf16 rounding of hi + lo"
+    assert bool((lo.abs() <= half_ulp_bf16(hi)).all()), "|lo| exceeds half an ulp of hi"
+
+
 def split_bf16(v):
     """(hi, lo) = (bf16(v), bf16(v - hi)) of fp32 values v, as float64."""
     hi = bf16_round(v)

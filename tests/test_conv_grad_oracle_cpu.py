@@ -4,7 +4,14 @@ splits, the stride-2 1x1 dX scattered from its compact result) passes grad_oracl
 each planted fault fails it: a tap not flipped, x read one pixel off, one K split dropped, the ReLU mask missing, and
 the errors a wide layer's dX route could make: one 64-channel tile of dX from the neighbouring tile's weight rows, a
 3x3 tap past the last row of one image reading the next image's first row (N = 2, as when a 128-pixel tile of the
-flattened pixels straddles two images), the compact stride-2 result scattered to the odd pixels or one pixel off."""
+flattened pixels straddles two images), the compact stride-2 result scattered to the odd pixels or one pixel off.
+
+The forward (conv_grad_oracle.forward, the bounds of tests/test_gpu_conv_forward_fp64.py): its sums in fp32 pass
+forward_c in every precision, and each planted fault fails it.  Swept over K = Cin * k * k (powers of two, 1x1 layers, a
+3x3 for the stacked images), every fault is still rejected at K = 131072 (the largest K tried; the widest layer the engine
+runs is fc6, K = 12544) in every precision but one: a truncating hi / lo split of fp32 activations at bf16x3 changes
+each product by about 2^-17 of its size with a random sign, and is rejected only up to K = 128.  Pair activations, the
+engine's bf16x3 input, are split on the host by Pair.from_float and not in the kernel."""
 import os
 import sys
 
@@ -117,3 +124,72 @@ def test_stride2_scatter(prec, hw):
     assert ok, r
     assert not _stride2(prec, *hw, "odd")[0]
     assert not _stride2(prec, *hw, "shift")[0]
+
+
+# ------------------------------------------------------------------------------------------------
+# forward (tests/test_gpu_conv_forward_fp64.py): conv_grad_oracle.forward's sums in fp32 pass the constant the GPU test
+# uses, and each planted fault fails it
+# ------------------------------------------------------------------------------------------------
+def _fwd_layer(name):
+    """(x, weight, kwargs) of a small layer: '3x3' 128 -> 192, N = 2 images of 7 x 9; 's2' 1x1 / stride 2, 64 -> 64 on
+    9 x 11; 'up2' 1x1 64 -> 64 + a half-resolution residual on 8 x 10; 'res' 1x1 64 -> 64 + a residual + ReLU; 'head'
+    the RPN's 1x1 A + 4A + A head (A = 3) with the sigmoid from channel 5A."""
+    gen = torch.Generator().manual_seed(len(name))
+    cin, cout, k, (H, W) = {"3x3": (128, 192, 3, (7, 9)), "s2": (64, 64, 1, (9, 11)), "up2": (64, 64, 1, (8, 10)),
+                            "res": (64, 64, 1, (7, 9)), "head": (64, 18, 1, (7, 9))}[name]
+    x = torch.randn((2, cin, H, W), generator=gen)
+    w = torch.randn((cout, cin, k, k), generator=gen) * (2.0 / (cin * k * k)) ** 0.5
+    kw = dict(bias=torch.randn(cout, generator=gen) * 0.5, padding=k // 2, relu=name in ("3x3", "res"))
+    if name == "s2":
+        kw["stride"] = 2
+    if name == "up2":
+        kw.update(residual=torch.randn((2, cout, H // 2, W // 2), generator=gen), residual_up2=True)
+    if name == "res":
+        kw["residual"] = torch.randn((2, cout, H, W), generator=gen)
+    if name == "head":
+        kw["sigmoid_from"] = 15
+    return x, w, kw
+
+
+def _fwd_check(prec, name, fault=None, pair=False):
+    x, w, kw = _fwd_layer(name)
+    if pair:
+        x = CG.split(x)
+    want, bound, slack = CG.forward(x, w, prec=prec, **kw)
+    got, _, _ = CG.forward(x, w, prec=prec, fault=fault, dtype=torch.float32, **kw)
+    K = w.shape[1] * w.shape[2] * w.shape[3]
+    c = CG.forward_c(prec, K, int(kw.get("bias") is not None) + int(kw.get("residual") is not None))
+    return G.check(got, want, bound, c, slack=slack)
+
+
+FWD_LAYERS = ["3x3", "s2", "up2", "res", "head"]
+
+
+@pytest.mark.parametrize("name", FWD_LAYERS)
+@pytest.mark.parametrize("prec", ["bf16x3", "bf16", "fp32"])
+def test_forward_restatement_passes(prec, name):
+    ok, r = _fwd_check(prec, name)
+    assert ok, r
+    if prec == "bf16x3":
+        ok, r = _fwd_check(prec, name, pair=True)
+        assert ok, r
+
+
+FWD_FAULTS = [("shift", "3x3"), ("stacked", "3x3"), ("drop_kblock", "3x3"), ("tile_from", "3x3"), ("odd", "s2"),
+              ("up2_off", "up2"), ("bias_next", "res"), ("sigmoid_early", "head"), ("relu_first", "res")]
+
+
+@pytest.mark.parametrize("fault", FWD_FAULTS, ids=[f for f, _ in FWD_FAULTS])
+@pytest.mark.parametrize("prec", ["bf16x3", "bf16", "fp32"])
+def test_forward_fault_fails(prec, fault):
+    assert not _fwd_check(prec, fault[1], fault[0])[0]
+
+
+@pytest.mark.parametrize("name", ["3x3", "s2"])
+def test_forward_dropped_lohi_fails(name):
+    assert not _fwd_check("bf16x3", name, "drop_lohi")[0]
+
+
+@pytest.mark.parametrize("prec", ["bf16x3", "bf16"])
+def test_forward_truncated_split_fails(prec):
+    assert not _fwd_check(prec, "s2", "trunc")[0]

@@ -85,18 +85,6 @@ def _check(key, family, got, want, bound, slack=None):
     assert ok, (key, "worst err / bound %.3g > c = %g" % (ratio, c))
 
 
-def _check_pair_split(store):
-    """A pair tensor [..., 2C] is normalised: hi == bf16(hi + lo) and |lo| <= half an ulp of hi.  When o - hi lies just
-    below half an ulp, lo = bf16(o - hi) rounds up to exactly half an ulp and hi + lo is a rounding midpoint (about 1 in
-    1000 elements of Pair.from_float); there either neighbour is a nearest bf16 value, so hi passes if it is one of them."""
-    c = store.shape[-1] // 2
-    hi, lo = store[..., :c].double(), store[..., c:].double()
-    v = hi + lo
-    r = G.bf16_round(v)
-    assert bool(((r == hi) | ((v - hi).abs() == (v - r).abs())).all()), "hi is not the bf16 rounding of hi + lo"
-    assert bool((lo.abs() <= G.half_ulp_bf16(hi)).all()), "|lo| exceeds half an ulp of hi"
-
-
 # ------------------------------------------------------------------------------------------------
 # deformable convolution
 # ------------------------------------------------------------------------------------------------
@@ -215,7 +203,7 @@ def _dcn_paths(U, c, off, x, w, b, m, paths):
         assert got.shape == want.shape
         _check(path, family, got, want, bound, slack)
         if store is not None:
-            _check_pair_split(store)
+            G.check_pair_split(store)
 
 
 def _all_paths(c):
@@ -290,11 +278,11 @@ def test_roi_align_layouts_vs_fp64(dev, pooled, sr):
         return
     out = torch.empty(R, PH, PW, 2 * C, dtype=torch.bfloat16, device=dev)
     _roi_c_abi(feat.store, B, C, H, W, _lib.LAYOUT_NHWC, _lib.DTYPE_PAIR, rois, PH, PW, scale, sr, out)
-    _check_pair_split(out)
+    G.check_pair_split(out)
     _check("roi pair", "roi_y", ops.Pair(out).float().double(), y64, bound, slack + 2.0 ** -17 * top)
     out = torch.empty(R, 1, 1, 2 * PH * PW * C, dtype=torch.bfloat16, device=dev)
     _roi_c_abi(feat.store, B, C, H, W, _lib.LAYOUT_FLAT_PAIR, _lib.DTYPE_PAIR, rois, PH, PW, scale, sr, out)
-    _check_pair_split(out)
+    G.check_pair_split(out)
     flat = ops.Pair(out).float().double().reshape(R, PH, PW, C).permute(0, 3, 1, 2)
     _check("roi flat pair", "roi_y", flat, y64, bound, slack + 2.0 ** -17 * top)
 
@@ -340,7 +328,7 @@ def test_fpn_roi_align_pair_roi_count_vs_fp64(dev, sr, flat):
     y64 = G.fpn_roi_align(fx, rois[:n], PH, PW, SCALES, sr)
     bd = G.fpn_roi_align_bounds(fx, rois[:n], PH, PW, SCALES, sr, torch.zeros_like(y64))
     top = y64.abs() + G.TOL["roi_y"] * bd["y"]
-    _check_pair_split(out[:n])
+    G.check_pair_split(out[:n])
     got = ops.Pair(out[:n].contiguous()).float().double()
     got = got.reshape(n, PH, PW, Cc).permute(0, 3, 1, 2) if flat else got
     _check("roi fpn pair n_dev" + (" flat" if flat else ""), "roi_y", got, y64, bd["y"], bd["y_slack"] + 2.0 ** -17 * top)
