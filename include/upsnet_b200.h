@@ -283,10 +283,12 @@ int upsnet_fcn_score_fuse_backward(const float *dscore, float *ds3, float *ds4, 
  *           bbox/bbox_transform.py:290-330,45-60) for the selected indices.
  * deltas[l] fp32 [4A,h_l,w_l] (RPN head output, channel a*4+c); top_idx[l] int64 [k_l] flat (y,x,a) indices
  * (device); k/hs/ws/strides host arrays [L]; base_anchors float64 [L,A,4] on the device (generate_anchors);
+ * im_info fp32 [3] on the device: the reference's (h, w, scale) row; boxes are clipped to [0, w-1] x [0, h-1].  It is
+ * read when the kernel runs, so a captured graph takes a new image size by rewriting the row before each replay.
  * boxes_out fp32 [sum k_l, 4] in level order. */
 int upsnet_rpn_decode(const float *const *deltas, const long long *const *top_idx, const int *k,
                       const int *hs, const int *ws, const int *strides, const double *base_anchors,
-                      int L, int A, float im_h, float im_w, float *boxes_out, void *stream);
+                      int L, int A, const float *im_info, float *boxes_out, void *stream);
 
 /* upsnet_rpn_topk: the pre_nms_top_n best anchors of every pyramid level, sorted by descending score, one call.
  * replaces: operators/functions/pyramid_proposal.py:104-118 (per-level argsort(-scores)[:pre_nms_top_n]).
@@ -310,12 +312,13 @@ int upsnet_rpn_collect(const int *keep, const int *keep_cnt, const int *seg_offs
 /* upsnet_maskroi_prepare: candidate selection (prob > score_thresh, roi valid), ordering (class segment
  * ascending -- one segment when class_agnostic --, score descending, roi-major index ascending) and box decode
  * (weights, clip) in one launch.  replaces: operators/modules/mask_roi.py:36-95 up to the per-class NMS.
- * rois [R,5]; roi_valid uint8 [R]; bbox_delta [R,4C]; cls_prob [R,C]; R*(C-1) <= 8192.
+ * rois [R,5]; roi_valid uint8 [R]; bbox_delta [R,4C]; cls_prob [R,C]; R*(C-1) <= 8192; im_info fp32 [3] on the
+ * device, (h, w, scale), read when the kernel runs (as in upsnet_rpn_decode): boxes are clipped to [0, w-1] x [0, h-1].
  * sc_out/cls_out/bx_out [R*(C-1)] (/[.,4]): candidates first, in NMS input order (others: score -1);
  * offs_out int32 [nseg+1]: segment offsets for upsnet_nms_segmented. */
 int upsnet_maskroi_prepare(const float *rois, const unsigned char *roi_valid, const float *bbox_delta,
                            const float *cls_prob, int R, int C, int class_agnostic, float score_thresh,
-                           const float weights[4], float im_h, float im_w, float *sc_out, int *cls_out,
+                           const float weights[4], const float *im_info, float *sc_out, int *cls_out,
                            float *bx_out, int *offs_out, void *stream);
 
 /* upsnet_maskroi_finish: NMS survivors (class-major) -> keep scores >= the top_n-th largest -> `cap` output

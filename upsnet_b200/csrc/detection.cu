@@ -17,7 +17,8 @@
 
 namespace ups {
 
-// bbox/bbox_transform.py:290-330 for one (box, delta) pair; weights divide the deltas; clip to the image.
+// bbox/bbox_transform.py:290-330 for one (box, delta) pair; weights divide the deltas; clip to the image (im_h x im_w,
+// the first two entries of the device im_info row, so one captured graph serves every image of its padded shape).
 __device__ __forceinline__ float4 decode_clip(float x1, float y1, float x2, float y2, float dx, float dy, float dw, float dh,
                                               float xform_clip, float im_h, float im_w) {
   const float w = __fadd_rn(__fsub_rn(x2, x1), 1.0f), h = __fadd_rn(__fsub_rn(y2, y1), 1.0f);
@@ -49,7 +50,8 @@ struct RpnDecodeParams {
   int k[kMaxLevels], h[kMaxLevels], w[kMaxLevels], stride[kMaxLevels], start[kMaxLevels + 1];
   const double* base;                    // [L, A, 4] generate_anchors() of every level (float64, like the reference)
   int L, A;
-  float im_h, im_w, xform_clip;
+  const float* im_info;                  // [3] (h, w, scale) on the device
+  float xform_clip;
   float* out;                            // [sum k, 4]
 };
 
@@ -66,7 +68,7 @@ __global__ void rpn_decode_kernel(const RpnDecodeParams p) {
   const size_t hw = (size_t)p.h[l] * p.w[l];
   const float* d = p.deltas[l] + (size_t)a * 4 * hw + (size_t)y * p.w[l] + x;
   const float4 o = decode_clip(an.x, an.y, an.z, an.w, __ldg(d), __ldg(d + hw), __ldg(d + 2 * hw), __ldg(d + 3 * hw),
-                               p.xform_clip, p.im_h, p.im_w);
+                               p.xform_clip, __ldg(p.im_info), __ldg(p.im_info + 1));
   reinterpret_cast<float4*>(p.out)[t] = o;
 }
 
@@ -80,7 +82,7 @@ __global__ void __launch_bounds__(kMrThreads, 1)
 maskroi_prepare_kernel(const float* __restrict__ rois, const uint8_t* __restrict__ roi_valid,
                        const float* __restrict__ bbox_delta, const float* __restrict__ cls_prob, int R, int C,
                        int class_agnostic, float score_thresh, float wx, float wy, float ww, float wh, float xform_clip,
-                       float im_h, float im_w, float* __restrict__ sc_out, int* __restrict__ cls_out,
+                       const float* __restrict__ im_info, float* __restrict__ sc_out, int* __restrict__ cls_out,
                        float* __restrict__ bx_out, int* __restrict__ offs_out) {
   extern __shared__ unsigned long long keys[];   // kSortN
   __shared__ int seg_cnt[130];
@@ -117,6 +119,7 @@ maskroi_prepare_kernel(const float* __restrict__ rois, const uint8_t* __restrict
   }
   __syncthreads();
   const int n_cand = seg_cnt[nseg + 1];
+  const float im_h = __ldg(im_info), im_w = __ldg(im_info + 1);
   for (int pidx = tid; pidx < n; pidx += kMrThreads) {
     float sc = -1.0f;
     int cls = 0;
@@ -221,9 +224,10 @@ maskroi_finish_kernel(const int* __restrict__ keep, const int* __restrict__ cnt,
 }  // namespace ups
 
 extern "C" int upsnet_rpn_decode(const float* const* deltas, const long long* const* top_idx, const int* k, const int* hs,
-                                 const int* ws, const int* strides, const double* base_anchors, int L, int A, float im_h,
-                                 float im_w, float* boxes_out, void* stream) {
-  if (!deltas || !top_idx || !k || !hs || !ws || !strides || !base_anchors || !boxes_out) return UPSNET_E_BADARG;
+                                 const int* ws, const int* strides, const double* base_anchors, int L, int A,
+                                 const float* im_info, float* boxes_out, void* stream) {
+  if (!deltas || !top_idx || !k || !hs || !ws || !strides || !base_anchors || !im_info || !boxes_out)
+    return UPSNET_E_BADARG;
   if (L <= 0 || L > ups::kMaxLevels || A <= 0) return UPSNET_E_BADARG;
   ups::RpnDecodeParams p{};
   int acc = 0;
@@ -235,7 +239,7 @@ extern "C" int upsnet_rpn_decode(const float* const* deltas, const long long* co
     acc += k[l];
   }
   p.start[L] = acc;
-  p.base = base_anchors; p.L = L; p.A = A; p.im_h = im_h; p.im_w = im_w;
+  p.base = base_anchors; p.L = L; p.A = A; p.im_info = im_info;
   p.xform_clip = (float)4.135166556742356;   // log(1000 / 16), bbox_transform.py
   p.out = boxes_out;
   if (acc == 0) return 0;
@@ -246,9 +250,10 @@ extern "C" int upsnet_rpn_decode(const float* const* deltas, const long long* co
 
 extern "C" int upsnet_maskroi_prepare(const float* rois, const unsigned char* roi_valid, const float* bbox_delta,
                                       const float* cls_prob, int R, int C, int class_agnostic, float score_thresh,
-                                      const float weights[4], float im_h, float im_w, float* sc_out, int* cls_out,
+                                      const float weights[4], const float* im_info, float* sc_out, int* cls_out,
                                       float* bx_out, int* offs_out, void* stream) {
-  if (!rois || !roi_valid || !bbox_delta || !cls_prob || !weights || !sc_out || !cls_out || !bx_out || !offs_out)
+  if (!rois || !roi_valid || !bbox_delta || !cls_prob || !weights || !im_info || !sc_out || !cls_out || !bx_out ||
+      !offs_out)
     return UPSNET_E_BADARG;
   if (R <= 0 || C < 2) return UPSNET_E_BADARG;
   if ((long long)R * (C - 1) > ups::kSortN || C - 1 > 128 || score_thresh < 0.f) return UPSNET_E_UNSUPPORTED;
@@ -259,7 +264,7 @@ extern "C" int upsnet_maskroi_prepare(const float* rois, const unsigned char* ro
   }
   ups::maskroi_prepare_kernel<<<1, ups::kMrThreads, ups::kSortN * 8, (cudaStream_t)stream>>>(
       rois, roi_valid, bbox_delta, cls_prob, R, C, class_agnostic, score_thresh, weights[0], weights[1], weights[2],
-      weights[3], (float)4.135166556742356, im_h, im_w, sc_out, cls_out, bx_out, offs_out);
+      weights[3], (float)4.135166556742356, im_info, sc_out, cls_out, bx_out, offs_out);
   UPS_CHECK_LAUNCH();
   return 0;
 }

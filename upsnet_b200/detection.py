@@ -77,6 +77,13 @@ def bbox_transform(boxes, deltas, weights=(1., 1., 1., 1.)):
 
 
 def clip_boxes(boxes, im_h, im_w):
+    """im_h, im_w: Python floats, or 0-dim tensors on the boxes' device (the bounds are then read when the clamp runs, so
+    the clip is the same inside a captured graph for every image size written to the row they come from)."""
+    if torch.is_tensor(im_w):
+        # clamp_(min=0, max=tensor) would stage the scalar bound through host memory, which a capture does not allow
+        for c, lim in ((0, im_w), (1, im_h), (2, im_w), (3, im_h)):
+            boxes[:, c::4].clamp_min_(0).clamp_max_(lim - 1)
+        return boxes
     boxes[:, 0::4].clamp_(min=0, max=im_w - 1)
     boxes[:, 1::4].clamp_(min=0, max=im_h - 1)
     boxes[:, 2::4].clamp_(min=0, max=im_w - 1)
@@ -255,10 +262,12 @@ class StaticProposalGenerator(ProposalGenerator):
         return self._anchors[key]
 
     def __call__(self, cls_probs, bbox_preds, im_info):
-        """-> rois [post,5] (invalid rows are all-zero), scores [post], valid [post] bool."""
+        """im_info: the (h, w, scale) row, a float32 [3] tensor on the device of cls_probs or a host row (uploaded).
+        -> rois [post,5] (invalid rows are all-zero), scores [post], valid [post] bool."""
         assert self.min_size == 0, "static path assumes config.test.rpn_min_size == 0 (all shipped yamls)"
         dev = cls_probs[0].device
-        im_h, im_w = float(im_info[0]), float(im_info[1])
+        im_info = _ops.im_info_device(im_info, dev)
+        im_h, im_w = im_info[0], im_info[1]
         boxes_l, scores_l, lens, idx_l = [], [], [], []
         fused = FUSED["on"] and dev.type == "cuda"
         if fused and 0 < self.pre <= 2048 and all(c.shape[0] == 1 and c.numel() < (1 << 22) for c in cls_probs):
@@ -268,7 +277,7 @@ class StaticProposalGenerator(ProposalGenerator):
             starts = np.concatenate([[0], np.cumsum(lens)])
             idx_l = [top_i[starts[l]:starts[l + 1]] for l in range(len(lens))]
             boxes = _ops.rpn_decode([b[0] for b in bbox_preds], idx_l, [c.shape[-2:] for c in cls_probs],
-                                    self.feat_stride[:len(cls_probs)], self._base_anchors(len(cls_probs), dev), A, im_h, im_w)
+                                    self.feat_stride[:len(cls_probs)], self._base_anchors(len(cls_probs), dev), A, im_info)
             return self._after_topk(boxes, scores, lens, dev)
         for l in range(len(cls_probs)):
             A = cls_probs[l].shape[1]
@@ -283,7 +292,7 @@ class StaticProposalGenerator(ProposalGenerator):
         if fused:   # one launch: shifted anchors + bbox_transform + clip for the top-k of every level
             boxes = _ops.rpn_decode([b[0] for b in bbox_preds], idx_l, [c.shape[-2:] for c in cls_probs],
                                     self.feat_stride[:len(cls_probs)], self._base_anchors(len(cls_probs), dev),
-                                    cls_probs[0].shape[1], im_h, im_w)
+                                    cls_probs[0].shape[1], im_info)
         else:
             boxes = torch.cat(boxes_l)
         scores = torch.cat(scores_l)
@@ -345,8 +354,10 @@ class StaticMaskROI(MaskROI):
         return self._const[key]
 
     def __call__(self, rois, roi_valid, bbox_delta, cls_prob, im_info, side=False):
-        """side=True: this call runs on a side stream concurrently with another MaskROI (separate NMS scratch)."""
+        """im_info: the (h, w, scale) row, a float32 [3] tensor on the rois' device or a host row (uploaded).
+        side=True: this call runs on a side stream concurrently with another MaskROI (separate NMS scratch)."""
         dev = rois.device
+        im_info = _ops.im_info_device(im_info, dev)
         C, R = self.num_classes, rois.shape[0]
         Cm = C - 1
         nseg = 1 if self.class_agnostic else Cm
@@ -354,14 +365,14 @@ class StaticMaskROI(MaskROI):
         M = R if (not self.class_agnostic or self.score_thresh >= 0.5) else R * Cm
         if FUSED["on"] and dev.type == "cuda" and R * Cm <= 8192 and Cm <= 128:
             sc, cls, bx, offs = _ops.maskroi_prepare(rois, roi_valid, bbox_delta, cls_prob, self.class_agnostic,
-                                                     self.score_thresh, self.weights, float(im_info[0]), float(im_info[1]))
+                                                     self.score_thresh, self.weights, im_info)
             keep, cnt = (_ops.nms_segmented(bx, offs, M, self.nms_thresh, side=True) if side
                          else nms_segmented(bx, offs, M, self.nms_thresh))
             o_sc, o_bx, o_cls, n_out, self.last_flags = _ops.maskroi_finish(keep, cnt, offs, sc, cls, bx, self.top_n, self.cap)
             return o_sc, o_bx, o_cls, n_out
         cls_flat, ridx_flat = self._consts(R, dev)
-        proposal = clip_boxes(bbox_transform(rois[:, 1:], bbox_delta, self.weights), float(im_info[0]),
-                              float(im_info[1])).reshape(R, C, 4)
+        proposal = clip_boxes(bbox_transform(rois[:, 1:], bbox_delta, self.weights), im_info[0],
+                              im_info[1]).reshape(R, C, 4)
         prob = cls_prob[:, 1:]
         cand = ((prob > self.score_thresh) & roi_valid[:, None]).reshape(-1)
         sc_all = torch.where(cand, prob.reshape(-1), torch.full_like(prob.reshape(-1), -1.0))

@@ -678,7 +678,12 @@ class resnet_upsnet(nn.Module):
         self.dedup_mask_rows = True   # mask branch on the distinct boxes only (ops.mask_rows), not on both padded buffers
         self._side = {}
         self._graphs = {}
-        self.max_graphs = 6           # captured graphs kept (LRU): one activation pool each (~2 GB at 1024x2048)
+        self._pools = {}
+        # captured graphs kept (LRU), one per (padded input shape, precision, lane).  The graphs of a lane share one
+        # activation pool, so an entry costs its graph and static outputs plus what its shape adds to the pool: a median
+        # of 53 MB (bf16x3) / 64 MB (bf16), at most 432 MB, of memory_reserved for COCO R50 shapes up to 800x1344 on an
+        # H100 80GB HBM3 at 700 W (scripts/prof_mixed_sizes.py).  128 keeps a COCO-style mix (35 padded shapes in 120 images) resident on 2 lanes.
+        self.max_graphs = 128
         self._prepared = False
         self.eval()
         # backbone_freeze_at and backbone_fix_bn (models/resnet.py:69-78, 338-345): the stem, res2..res<freeze_at> and,
@@ -705,7 +710,7 @@ class resnet_upsnet(nn.Module):
         old parameter storage -- rebuild them lazily on the next forward."""
         r = super()._apply(fn, *a, **kw)
         self._prepared = False
-        self._graphs = {}
+        self._graphs, self._pools = {}, {}
         return r
 
     # COCO -> Cityscapes head remapping of models/resnet.py:223-273 (fine-tuning a COCO checkpoint on Cityscapes)
@@ -733,7 +738,7 @@ class resnet_upsnet(nn.Module):
         else:
             r = self._load_reference_style(dict(state_dict), bool(resume))
         self._prepared = False
-        self._graphs = {}
+        self._graphs, self._pools = {}, {}
         return r
 
     def _load_reference_style(self, state_dict, resume):
@@ -892,10 +897,11 @@ class resnet_upsnet(nn.Module):
         return self._side[key]
 
     def _run_static(self, x, im_info, lane=0):
-        """One image through the static engine on the CURRENT stream.  `lane` selects an independent engine instance (its own
-        captured graph, activation pool, output buffers and scratch workspaces): callers that keep several images in flight
-        run lane i on stream i (pipeline.PipelinedEngine, bench.py) -- the single-CTA detection kernels of one image then
-        hide under the machine-filling convolutions of the other."""
+        """One image through the static engine on the CURRENT stream.  im_info: the image's (h, w, scale) row, a host row
+        or a CUDA float32 [3] tensor.  `lane` selects an independent engine instance (its own captured graphs, activation
+        pool, output buffers and scratch workspaces): callers that keep several images in flight run lane i on stream i
+        (pipeline.PipelinedEngine, bench.py) -- the single-CTA detection kernels of one image then hide under the
+        machine-filling convolutions of the other."""
         prev_slot = ops.WS_SLOT["i"]
         ops.WS_SLOT["i"] = int(lane)
         try:
@@ -903,35 +909,61 @@ class resnet_upsnet(nn.Module):
         finally:
             ops.WS_SLOT["i"] = prev_slot
 
+    @staticmethod
+    def _write_im_info(ent, im_info):
+        """Enqueue the copy of im_info into the entry's device row on the current stream.  A host row is staged in pinned
+        memory (torch's pinned allocator holds the block until the copy has run), so the host never waits; it is not
+        copied again while it equals the row last written to this entry."""
+        if torch.is_tensor(im_info) and im_info.is_cuda:
+            ent[4].copy_(im_info.reshape(3), non_blocking=True)
+            ent[5] = None
+            return
+        row = tuple(np.asarray(im_info, dtype=np.float32).reshape(-1)[:3].tolist())
+        if row != ent[5]:
+            ent[4].copy_(torch.tensor(row, dtype=torch.float32).pin_memory(), non_blocking=True)
+            ent[5] = row
+
     def _run_static_lane(self, x, im_info, lane):
         if not (self.use_cuda_graph and x.is_cuda):
-            return self._forward_static(x, im_info), None
+            return self._forward_static(x, ops.im_info_device(im_info, x.device)), None
+        # the image geometry is a device input of the graph (the detection clips read it when they run), so one graph
+        # serves every image of a padded shape
         key = (tuple(x.shape), str(x.device), ops._PRECISION["conv"], bool(getattr(self, "keep_intermediates", False)),
-               bool(self.dedup_mask_rows), tuple(float(v) for v in im_info), lane)
+               bool(self.dedup_mask_rows), lane)
         ent = self._graphs.get(key)
         if ent is None:
             static_x = torch.empty(x.shape, dtype=torch.float32, device=x.device)
             static_x.copy_(x)
+            ent = [None, static_x, None, 0, torch.empty((3,), dtype=torch.float32, device=x.device), None]
+            self._write_im_info(ent, im_info)
             cur = torch.cuda.current_stream(x.device)
             side = torch.cuda.Stream(device=x.device)
             side.wait_stream(cur)
             with torch.cuda.stream(side):       # warm-up: workspaces, packed weights, anchor tables, cudnn/cub plans
                 for _ in range(2):
-                    self._forward_static(static_x, im_info)
+                    self._forward_static(static_x, ent[4])
             cur.wait_stream(side)
             torch.cuda.synchronize(x.device)
+            # Every graph of a lane is captured into the lane's one memory pool, so k captured shapes cost about one
+            # activation pool.  Their intermediates overlap, which is safe under one invariant: a lane's graphs never
+            # replay concurrently (a lane runs on one stream), and a graph's outputs are consumed -- copied or cloned,
+            # as _forward_infer and PipelinedEngine do -- before the lane replays any graph again.
+            pool = self._pools.get((str(x.device), lane))
+            if pool is None:
+                pool = self._pools[(str(x.device), lane)] = torch.cuda.graph_pool_handle()
             graph = torch.cuda.CUDAGraph()
             l0 = ops.STATS["launches"]
-            with torch.cuda.graph(graph):
-                out = self._forward_static(static_x, im_info)
-            ent = (graph, static_x, out, ops.STATS["launches"] - l0)
-            while len(self._graphs) >= self.max_graphs:      # LRU: every entry pins one full activation pool
+            with torch.cuda.graph(graph, pool=pool):
+                out = self._forward_static(static_x, ent[4])
+            ent[0], ent[2], ent[3] = graph, out, ops.STATS["launches"] - l0
+            while len(self._graphs) >= self.max_graphs:      # LRU
                 self._graphs.pop(next(iter(self._graphs)))
             self._graphs[key] = ent
         else:
             self._graphs[key] = self._graphs.pop(key)        # most recently used last
-        graph, static_x, out, n_launch = ent
-        static_x.copy_(x, non_blocking=True)
+            ent[1].copy_(x, non_blocking=True)
+            self._write_im_info(ent, im_info)
+        graph, _, out, n_launch = ent[:4]
         graph.replay()
         ops.STATS["launches"] += n_launch
         return out, graph

@@ -680,10 +680,26 @@ def nms_segmented(boxes_sorted, seg_offsets, max_seg_len, thresh, side=False):
     return keep, cnt
 
 
-def rpn_decode(bbox_preds, top_idx, shapes, strides, base_anchors, A, im_h, im_w):
+def im_info_device(im_info, dev):
+    """The image geometry row (h, w, scale) as a float32 [3] tensor on `dev`.  A float32 tensor already there is returned
+    as it is; a host row ([3] or [1,3], numpy or tensor) is uploaded through pinned memory without blocking the host
+    (torch's pinned allocator keeps the staging block until the copy has run).  The detection kernels read the row when
+    they run, so a captured graph that reads a device row takes a new image size by a copy into that row."""
+    if torch.is_tensor(im_info) and im_info.device == torch.device(dev) and im_info.dtype == torch.float32:
+        assert im_info.numel() == 3, "im_info: one (h, w, scale) row"
+        return im_info.reshape(3)
+    t = im_info.detach().cpu() if torch.is_tensor(im_info) else torch.from_numpy(np.asarray(im_info, dtype=np.float32))
+    t = t.to(torch.float32).reshape(-1)[:3].contiguous()
+    if torch.device(dev).type != "cuda":
+        return t.to(dev)
+    return t.pin_memory().to(dev, non_blocking=True)
+
+
+def rpn_decode(bbox_preds, top_idx, shapes, strides, base_anchors, A, im_info):
     """Fused anchors + bbox_transform + clip_boxes for the pre-NMS top-k of every level (one launch).
     bbox_preds[l] fp32 [4A,h,w] (contiguous), top_idx[l] int64 [k_l] flat (y,x,a) indices, base_anchors float64
-    [L,A,4] on the device.  -> boxes [sum k_l, 4]."""
+    [L,A,4] on the device, im_info the (h, w, scale) row (CUDA float32 [3], or a host row: im_info_device).
+    -> boxes [sum k_l, 4]."""
     L = len(bbox_preds)
     dev = bbox_preds[0].device
     require_cuda(*bbox_preds, *top_idx, base_anchors)
@@ -691,13 +707,14 @@ def rpn_decode(bbox_preds, top_idx, shapes, strides, base_anchors, A, im_h, im_w
     bbox_preds = [f32c(b) for b in bbox_preds]
     top_idx = [t.contiguous() for t in top_idx]
     assert all(t.dtype == torch.int64 for t in top_idx)
+    info = im_info_device(im_info, dev)
     ks = [int(t.numel()) for t in top_idx]
     out = torch.empty((sum(ks), 4), dtype=torch.float32, device=dev)
     vp, ci = C.c_void_p, C.c_int
     with _Timed("rpn_decode", 1, {"bytes": 56.0 * sum(ks)}, dev):
         call("rpn_decode", dev, (vp * L)(*[b.data_ptr() for b in bbox_preds]), (vp * L)(*[t.data_ptr() for t in top_idx]),
              (ci * L)(*ks), (ci * L)(*[int(s[0]) for s in shapes]), (ci * L)(*[int(s[1]) for s in shapes]),
-             (ci * L)(*[int(s) for s in strides]), base_anchors, L, int(A), float(im_h), float(im_w), out)
+             (ci * L)(*[int(s) for s in strides]), base_anchors, L, int(A), info, out)
     return out
 
 
@@ -741,9 +758,10 @@ def rpn_collect(keep, cnt, offs, boxes, scores, post_nms_top_n):
     return rois, out_s, ok
 
 
-def maskroi_prepare(rois, roi_valid, bbox_delta, cls_prob, class_agnostic, score_thresh, weights, im_h, im_w):
+def maskroi_prepare(rois, roi_valid, bbox_delta, cls_prob, class_agnostic, score_thresh, weights, im_info):
     """Fused MaskROI front half -> (sc [n], cls int32 [n], bx [n,4], offs int32 [nseg+1]), n = R*(C-1):
-    candidates first in (segment, score desc, index) order, decoded and clipped."""
+    candidates first in (segment, score desc, index) order, decoded and clipped to the (h, w, scale) row im_info
+    (CUDA float32 [3], or a host row: im_info_device)."""
     require_cuda(rois, roi_valid, bbox_delta, cls_prob)
     rois, bbox_delta, cls_prob = f32c(rois), f32c(bbox_delta), f32c(cls_prob)
     assert roi_valid.dtype == torch.bool and roi_valid.is_contiguous()
@@ -751,6 +769,7 @@ def maskroi_prepare(rois, roi_valid, bbox_delta, cls_prob, class_agnostic, score
     n = R * (Cn - 1)
     dev = rois.device
     nseg = 1 if class_agnostic else Cn - 1
+    info = im_info_device(im_info, dev)
     sc = torch.empty((n,), dtype=torch.float32, device=dev)
     cls = torch.empty((n,), dtype=torch.int32, device=dev)
     bx = torch.empty((n, 4), dtype=torch.float32, device=dev)
@@ -758,8 +777,7 @@ def maskroi_prepare(rois, roi_valid, bbox_delta, cls_prob, class_agnostic, score
     w4 = (C.c_float * 4)(*[float(w) for w in weights])
     with _Timed("maskroi", 1, {"bytes": 4.0 * (rois.numel() + bbox_delta.numel() + cls_prob.numel())}, dev):
         call("maskroi_prepare", dev, rois, roi_valid, bbox_delta, cls_prob, R, Cn,
-             1 if class_agnostic else 0, float(score_thresh), w4, float(im_h), float(im_w),
-             sc, cls, bx, offs)
+             1 if class_agnostic else 0, float(score_thresh), w4, info, sc, cls, bx, offs)
     return sc, cls, bx, offs
 
 
@@ -1217,18 +1235,25 @@ def unified_pan_result(seg, pan, cls_inds, num_seg_classes, num_classes, stuff_a
     return out
 
 
-def prep_image(image_hwc_u8, pixel_means, scale=1.0, stride=32, flip=False):
+def prep_image(image_hwc_u8, pixel_means, scale=1.0, stride=32, flip=False, out=None):
     """dataset/base_dataset.py:143-174 prep_im_for_blob + :898-923 im_list_to_blob on the device: uint8 [h,w,3] (BGR)
     -> fp32 blob [1,3,Hp,Wp] (mean-subtracted, bilinearly resized by `scale`, zero-padded to a multiple of `stride`)
     and the resized (h, w).  flip=True mirrors the image first (get_image_blob's im[:, ::-1, :] for a flipped roidb
-    entry), bit-identical to passing a flipped copy."""
+    entry), bit-identical to passing a flipped copy.  out: a float32 CUDA buffer of at least 3*Hp*Wp elements whose
+    leading part receives the blob (padding written as zeros); the blob returned is then a view of it."""
     require_cuda(image_hwc_u8)
     assert image_hwc_u8.dtype == torch.uint8 and image_hwc_u8.dim() == 3 and image_hwc_u8.shape[2] == 3
     im = image_hwc_u8.contiguous()
     h, w = int(im.shape[0]), int(im.shape[1])
     ho, wo = int(np.rint(h * scale)), int(np.rint(w * scale))              # cvRound(src * f) (cv2.resize dsize rule)
     Hp, Wp = int(math.ceil(ho / float(stride)) * stride), int(math.ceil(wo / float(stride)) * stride)
-    blob = torch.empty((1, 3, Hp, Wp), dtype=torch.float32, device=im.device)
+    if out is None:
+        blob = torch.empty((1, 3, Hp, Wp), dtype=torch.float32, device=im.device)
+    else:
+        assert out.dtype == torch.float32 and out.is_contiguous() and out.device == im.device
+        if out.numel() < 3 * Hp * Wp:
+            raise ValueError("prep_image: out holds %d elements, the blob needs %d" % (out.numel(), 3 * Hp * Wp))
+        blob = out.reshape(-1)[:3 * Hp * Wp].view(1, 3, Hp, Wp)
     pm = (C.c_double * 3)(*[float(v) for v in pixel_means])
     with _Timed("prep_image", 1, {"bytes": 3.0 * h * w + 12.0 * Hp * Wp}, im.device):
         call("prep_image", im.device, im, h, w, float(scale), ho, wo, Hp, Wp, pm, blob, int(bool(flip)))

@@ -59,6 +59,7 @@ from torch.optim.optimizer import required
 
 from . import _lib
 from ._lib import call, f32c, query_bytes, require_cuda
+from .geometry import prep_scale
 from .operators import _weight_cache, prep_image
 
 
@@ -1791,11 +1792,7 @@ class TrainingSample:
 
     def im_scale(self, target_size, h, w):
         """prep_im_for_blob's scale of an h x w image for one target size (base_dataset.py:158-168)."""
-        size_min, size_max = min(h, w), max(h, w)
-        s = float(target_size) / float(size_min)
-        if np.round(s * size_max) > self.max_size:
-            s = float(self.max_size) / float(size_max)
-        return s
+        return prep_scale(target_size, self.max_size, h, w)
 
     def draw_scale(self, h, w):
         """get_image_blob's draw (base_dataset.py:119-121) -> (scale index, im_scale)."""
