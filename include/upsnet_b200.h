@@ -477,6 +477,28 @@ int upsnet_cocoeval_image(int segm, const float *boxes, const float *scores, con
                           int num_categories, const int *class_to_k, int image_slot, upsnet_coco_record *records,
                           int record_cap, int *n_records, long long *npig, int *err, void *workspace,
                           size_t workspace_bytes, void *stream);
+/* upsnet_gt_rle: the ground truths of one image as upsnet_cocoeval_image reads them, COCO.annToRLE on the device
+ * (maskUtils.merge(maskUtils.frPyObjects(segm, h, w)) for a list segmentation).
+ *   Annotation g (of num_anns, in annotation order) is the union of polygons [ann_poly[g], ann_poly[g+1]) (ann_poly int32
+ *   [num_anns + 1]); polygon q has the fp64 vertices verts[poly_vert[q] .. poly_vert[q+1]) (poly_vert int32 [P + 1],
+ *   verts (x, y) pairs, |coordinate| < 4e8).  Each polygon is rasterised as maskApi.c rleFrPoly does at h x w (k =
+ *   its vertex count, 0 and 1 included), and the polygons are united as rleMerge(..., intersect = 0).  A box-list
+ *   segmentation is passed as rleFrBbox's polygons [xs, ys, xs, ye, xe, ye, xe, ys].  An annotation without polygons
+ *   takes src_counts[src_offsets[g] .. src_offsets[g+1]) (uint32, src_offsets int64 [num_anns + 1]) unchanged: the
+ *   uncompressed run lengths of an RLE segmentation, staged from the host.
+ *   Writes gt_counts uint32 (all annotations back to back, the canonical runs: column-major, zeros first, the first run
+ *   possibly 0, every later one > 0, summing to h * w) and gt_offsets int64 [num_anns + 1].  capacity: the gt_counts
+ *   elements available, at least the total run count; for an annotation of polygons, 1 + the sum over its edges of
+ *   min(w, (|X1 - X0| + 1) / 5 + 1) with X = (int)(5 x + .5) bounds its runs.  Over capacity: err (DEVICE int,
+ *   sticky) gets UPSNET_GT_RLE_E_CAPACITY, every offset is 0 and no run is written.  Offsets come from a device scan;
+ *   the call never synchronises.  Deterministic: the same input gives the same bytes.
+ *   Limits: h, w >= 1 and h * w < 2^31, num_anns <= 65535 (else UPSNET_E_UNSUPPORTED).
+ *   Workspace: upsnet_gt_rle_workspace_bytes(num_anns, h, w). */
+#define UPSNET_GT_RLE_E_CAPACITY 64   /* more runs than capacity (the bit is free in the UPSNET_COCOEVAL_E_* flag) */
+int upsnet_gt_rle_workspace_bytes(int num_anns, int h, int w, size_t *bytes);
+int upsnet_gt_rle(int h, int w, int num_anns, const int *ann_poly, const int *poly_vert, const double *verts,
+                  const int64_t *src_offsets, const uint32_t *src_counts, uint32_t *gt_counts, long long capacity,
+                  int64_t *gt_offsets, int *err, void *workspace, size_t workspace_bytes, void *stream);
 int upsnet_cocoeval_accumulate_workspace_bytes(int n_records, size_t *bytes);
 int upsnet_cocoeval_accumulate(const upsnet_coco_record *records, int n_records, const int *image_rank,
                                const long long *npig, int num_categories, double *precision, double *recall,

@@ -12,21 +12,11 @@
 //   3. pt_mask:   one CTA per mask row: the object of largest IoU with the row's box, its polygons rasterised at M x M
 //                 by the rleFrPoly rule (toggles + prefix XOR, below), and the K * M^2 class-specific target row.
 //
-// The rasteriser.  rleFrPoly (cocoapi maskApi.c) walks each edge at 5x, keeps the points where the upsampled x
-// coordinate u changes and min(u) = 5n + 2 (a pixel centre, 0 <= n < M), maps each to (x = n, y = ceil(clamp((min v +
-// .5) / 5 - .5, 0, M))), sorts the column-major indices a = x * M + y, differences them and merges zero runs.  The runs
-// alternate 0 / 1 starting with 0, so pixel i is 1 iff an odd number of points have a <= i: a zero difference (two
-// equal points) cancels a boundary, which is what the merge does.  So each surviving point toggles bit a of a bitmap
-// and a prefix XOR gives the mask; a = M * M (y clamped to M in the last column) falls off the end.  Within an edge u
-// moves by at most 1 per point, monotonically, so each n is crossed at most once: on a shallow edge u = t + xs and the
-// crossing is direct; on a steep edge u(t) = (int)(xs + s*t + .5) and the crossing is found by bisection on that same
-// double expression.  Each edge therefore costs at most M steps whatever its length.  Consecutive edges share the
-// rounded vertex when it is >= 0; when it is negative, (int) truncation can make them differ, but then both u <= 0
-// and the pair is dropped by xd < 0.  Edges are thus independent (tests/proposal_target_oracle.py pins this
-// formulation to the literal rleFrPoly on random polygons).  Every rounding step is an explicit _rn intrinsic: gcc's
-// x86-64 build of maskApi.c and numpy do not contract into FMA.
+// The rasteriser is rleFrPoly's edge walk of poly.cuh at h = w = M: each edge's surviving boundary points toggle bits
+// of a column-major M x M bitmap in shared memory, and a prefix XOR gives the mask.
 #include "common.cuh"
 #include "cta.cuh"
+#include "poly.cuh"
 #include "targets.cuh"
 
 namespace ups {
@@ -223,55 +213,6 @@ __global__ void __launch_bounds__(kPtSample) pt_sample_kernel(const PtParams p) 
   }
 }
 
-// (int)(5 * c + .5) of a float32 coordinate, as rleFrPoly rounds the scaled vertices (double, truncation)
-__device__ __forceinline__ int up5(float c) { return (int)__dadd_rn(__dmul_rn(5.0, (double)c), 0.5); }
-
-__device__ __forceinline__ void toggle(unsigned int* bits, int M, int n, int yv) {
-  double yd = __dsub_rn(__ddiv_rn(__dadd_rn((double)yv, 0.5), 5.0), 0.5);
-  if (yd < 0.0) yd = 0.0;
-  else if (yd > (double)M) yd = (double)M;
-  const int a = n * M + (int)ceil(yd);
-  if (a < M * M) atomicXor(bits + (a >> 5), 1u << (a & 31));
-}
-
-// the surviving boundary points of one edge (X0, Y0) -> (X1, Y1) of rleFrPoly, at most M of them
-__device__ void edge_toggles(unsigned int* bits, int M, int X0, int Y0, int X1, int Y1) {
-  const int dx = abs(X1 - X0), dy = abs(Y1 - Y0);
-  if (dx >= dy) {
-    if (dx == 0) return;            // one point: no u change inside the edge
-    const bool flip = X0 > X1;
-    const int xs = flip ? X1 : X0, ys = flip ? Y1 : Y0, ye = flip ? Y0 : Y1;
-    const double s = __ddiv_rn((double)(ye - ys), (double)dx);
-    const int lo = xs, hi = xs + dx;
-    const int n0 = lo <= 2 ? 0 : (lo - 2 + 4) / 5, n1 = hi < 3 ? -1 : min(M - 1, (hi - 3) / 5);
-    for (int n = n0; n <= n1; ++n) {
-      const int ta = 5 * n + 2 - xs;
-      const int va = (int)__dadd_rn(__dadd_rn((double)ys, __dmul_rn(s, (double)ta)), 0.5);
-      const int vb = (int)__dadd_rn(__dadd_rn((double)ys, __dmul_rn(s, (double)(ta + 1))), 0.5);
-      toggle(bits, M, n, min(va, vb));
-    }
-  } else {
-    const bool flip = Y0 > Y1;
-    const int xs = flip ? X1 : X0, xe = flip ? X0 : X1, ys = flip ? Y1 : Y0;
-    const double s = __ddiv_rn((double)(xe - xs), (double)dy);
-    auto u = [&](int t) { return (int)__dadd_rn(__dadd_rn((double)xs, __dmul_rn(s, (double)t)), 0.5); };
-    const int u0 = u(0), u1 = u(dy);
-    const int lo = min(u0, u1), hi = max(u0, u1);
-    const int n0 = lo <= 2 ? 0 : (lo - 2 + 4) / 5, n1 = hi < 3 ? -1 : min(M - 1, (hi - 3) / 5);
-    for (int n = n0; n <= n1; ++n) {
-      const int xd = 5 * n + 2;
-      int a = 0, b = dy;            // the first t past the crossing: u(t) >= xd + 1 (s > 0) or u(t) <= xd (s < 0)
-      while (b - a > 1) {
-        const int m = (a + b) >> 1;
-        const int um = u(m);
-        if (s > 0.0 ? um >= xd + 1 : um <= xd) b = m;
-        else a = m;
-      }
-      toggle(bits, M, n, ys + b - 1);
-    }
-  }
-}
-
 // 3. one mask row: the class-specific K * M^2 target (-1 outside the class slot)
 __global__ void __launch_bounds__(kPtThreads) pt_mask_kernel(const PtParams p) {
   __shared__ unsigned int bits[kPtMaxM * kPtMaxM / 32 + 1];
@@ -318,7 +259,7 @@ __global__ void __launch_bounds__(kPtThreads) pt_mask_kernel(const PtParams p) {
         const int Y0 = up5(__fdiv_rn(__fmul_rn(__fsub_rn(a[1], b.y), fM), wy));
         const int X1 = up5(__fdiv_rn(__fmul_rn(__fsub_rn(c[0], b.x), fM), wx));
         const int Y1 = up5(__fdiv_rn(__fmul_rn(__fsub_rn(c[1], b.y), fM), wy));
-        edge_toggles(bits, M, X0, Y0, X1, Y1);
+        edge_toggles(bits, M, M, X0, Y0, X1, Y1);
       }
       __syncthreads();
       if (threadIdx.x < 32) {         // prefix XOR over the column-major bits, OR-ed into the union of the polygons

@@ -31,7 +31,8 @@ that bin exists, so gt rows >= C are dropped and predictions >= C alias into lat
 
 `DetectionAP` computes the COCO box or mask AP of the reference's evaluate_boxes / evaluate_masks (pycocotools COCOeval
 with its default Params) without the results JSON: update() matches one image on the device (csrc/cocoeval.cu), reading
-the masks from im_post_rle's run lengths, and summarize() accumulates every image's records on the device and copies
+the masks from im_post_rle's run lengths and rasterising polygon ground truths there too (csrc/gt_rle.cu, COCO.annToRLE
+at the image's size), and summarize() accumulates every image's records on the device and copies
 precision / recall / scores back once.
 """
 import collections
@@ -328,7 +329,8 @@ _AP_ERRORS = ((1, "more than %d detections in one image" % MAX_AP_DET),
               (4, "more than %d ground truths of one category in one image" % MAX_AP_GT_CAT),
               (8, "a detection class index outside [1, number of categories]"),
               (16, "more records than record_capacity (kept detections over all images)"),
-              (32, "a mask RLE that does not cover the image (size mismatch, or im_post_rle's buffer overflowed)"))
+              (32, "a mask RLE that does not cover the image (size mismatch, or im_post_rle's buffer overflowed)"),
+              (64, "rasterised polygon ground truths with more runs than the host's bound (UPSNET_GT_RLE_E_CAPACITY)"))
 
 
 def _mask_counts(mask):
@@ -345,7 +347,8 @@ def _mask_counts(mask):
 
 def gt_rle(segmentation):
     """A ground-truth `segmentation` -> (h, w, uint32 run lengths).  Accepts a compressed or uncompressed COCO RLE dict or
-    a [H,W] mask.  Polygons are rejected: rasterise them first (COCO.annToRLE(ann))."""
+    a [H,W] mask.  Polygons are rejected: DetectionAP.update(..., im_size=(h, w)) rasterises them on the device
+    (operators.ann_to_rle), or pass COCO.annToRLE(ann)."""
     from .operators import rle_from_string
     if isinstance(segmentation, dict):
         h, w = (int(v) for v in segmentation["size"])
@@ -446,9 +449,13 @@ class DetectionAP:
         self._npig = torch.zeros((K, 4), dtype=torch.int64, device=self.device)
         self._err = torch.zeros((1,), dtype=torch.int32, device=self.device)
         self._ws = torch.empty((0,), dtype=torch.uint8, device=self.device)
-        self._stage = [[torch.empty((0,), dtype=torch.uint8), torch.empty((0,), dtype=torch.uint8, device=self.device), None]
-                       for _ in range(self.STAGING_SLOTS)]
+        self._stage_ring = [[torch.empty((0,), dtype=torch.uint8), torch.empty((0,), dtype=torch.uint8, device=self.device),
+                             None] for _ in range(self.STAGING_SLOTS)]
         self._next = 0
+        # polygon ground truths: the rasteriser's output (cocoeval_image's gt_counts / gt_offsets) and workspace
+        self._gt_counts = torch.empty((0,), dtype=torch.int32, device=self.device)
+        self._gt_offsets = torch.empty((0,), dtype=torch.int64, device=self.device)
+        self._gt_ws = torch.empty((0,), dtype=torch.uint8, device=self.device)
         self._image_ids = []
         self._seen = set()
 
@@ -460,8 +467,10 @@ class DetectionAP:
             raise ValueError("%s must have shape %s, got %s" % (name, shape, tuple(x.shape)))
         return x.to(self.device, dtype, non_blocking=True).contiguous()
 
-    def _gt_table(self, gt_anns):
-        """fp64 [9][G] (K index, iscrowd, area, x, y, w, h, rle h, rle w) and, for segm, the run lengths and offsets."""
+    def _gt_table(self, gt_anns, im_size=None):
+        """fp64 [9][G] (K index, iscrowd, area, x, y, w, h, rle h, rle w) and, for segm, the run lengths and offsets.  With
+        im_size, the segmentations are packed for the device rasteriser instead (ops.pack_segmentations at the image's
+        size), and the third value is that PackedSegms."""
         G = len(gt_anns)
         table = np.zeros((9, G), np.float64)
         runs = []
@@ -474,24 +483,31 @@ class DetectionAP:
             table[2, j] = float(ann["area"])
             if self.iou_type == "bbox":
                 table[3:7, j] = [float(v) for v in ann["bbox"]]
-            else:
+            elif im_size is None:
                 h, w, cnts = gt_rle(ann["segmentation"])
                 table[7, j], table[8, j] = h, w
                 runs.append(cnts)
+        if im_size is not None:
+            from .operators import pack_segmentations
+            pk = pack_segmentations([ann["segmentation"] for ann in gt_anns], *im_size)
+            table[7:9] = pk.sizes
+            return table, None, pk
         offs = np.zeros(G + 1, np.int64)
         if runs:
             offs[1:] = np.cumsum([r.size for r in runs])
         counts = np.concatenate(runs).astype(np.uint32) if runs else np.zeros(0, np.uint32)
         return table, offs, counts
 
-    def _stage_gt(self, table, offs, counts):
-        """Copies the ground truths through a ring of pinned buffers; returns device pointers (table, offsets, counts)."""
-        G = table.shape[1]
-        nt, no = 8 * table.size, 8 * offs.size
-        nbytes = nt + no + 4 * counts.size
-        k = self._next % len(self._stage)
+    def _stage(self, arrays):
+        """Copies the arrays (back to back, each 8-byte aligned) through a ring of pinned buffers; returns their device
+        addresses."""
+        at, nbytes = [], 0
+        for a in arrays:
+            at.append(nbytes)
+            nbytes += a.nbytes + (-a.nbytes) % 8
+        k = self._next % len(self._stage_ring)
         self._next += 1
-        host, dev, ev = self._stage[k]
+        host, dev, ev = self._stage_ring[k]
         if ev is not None:
             ev.synchronize()           # the H2D copy that last read this pinned slot (STAGING_SLOTS updates ago)
         if host.numel() < nbytes:
@@ -499,24 +515,42 @@ class DetectionAP:
             host = torch.empty((size,), dtype=torch.uint8, pin_memory=True)
             dev = torch.empty((size,), dtype=torch.uint8, device=self.device)
         h = host.numpy()
-        h[:nt] = table.reshape(-1).view(np.uint8)
-        h[nt:nt + no] = offs.view(np.uint8)
-        h[nt + no:nbytes] = counts.view(np.uint8)
+        for a, o in zip(arrays, at):
+            h[o:o + a.nbytes] = a.reshape(-1).view(np.uint8)
         if nbytes:
             dev[:nbytes].copy_(host[:nbytes], non_blocking=True)
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.device))
-        self._stage[k] = [host, dev, ev]
-        base = dev.data_ptr()
-        return (C.c_void_p(base), C.c_void_p(base + nt), C.c_void_p(base + nt + no)) if G else (None, None, None)
+        self._stage_ring[k] = [host, dev, ev]
+        return [C.c_void_p(dev.data_ptr() + o) for o in at]
+
+    def _rasterise_gt(self, table, pk, H, W):
+        """Stages the table and the packed segmentations, and enqueues upsnet_gt_rle; returns the device pointers
+        (table, offsets, counts) for cocoeval_image."""
+        from . import operators as ops
+        ptrs = self._stage([table] + ops.gt_rle_arrays(pk))
+        G = table.shape[1]
+        if self._gt_counts.numel() < pk.bound:
+            self._gt_counts = torch.empty((max(pk.bound, 2 * self._gt_counts.numel()),), dtype=torch.int32,
+                                          device=self.device)
+        if self._gt_offsets.numel() < G + 1:
+            self._gt_offsets = torch.empty((max(G + 1, 2 * self._gt_offsets.numel()),), dtype=torch.int64,
+                                           device=self.device)
+        nb = query_bytes("gt_rle_workspace_bytes", G, H, W)
+        if self._gt_ws.numel() < nb:
+            self._gt_ws = torch.empty((nb,), dtype=torch.uint8, device=self.device)
+        ops.gt_rle_call(pk, H, W, ptrs[1:], self._gt_counts, self._gt_offsets, self._err, self._gt_ws)
+        return ptrs[0], self._gt_offsets, self._gt_counts
 
     def update(self, image_id, gt_anns, boxes, scores, cls_inds, rle=None, n_dev=None, im_size=None):
         """Adds one image: COCOeval.evaluate() for its detections and ground truths.
         gt_anns: the image's instance annotations (category_id, iscrowd, area, and bbox for 'bbox' / segmentation for
-        'segm', as a compressed or uncompressed RLE or a [H,W] mask).  boxes fp32 [n,4] x1 y1 x2 y2, scores fp32 [n],
+        'segm', as a compressed or uncompressed RLE, a [H,W] mask, or with im_size a polygon list or box list, which is
+        rasterised on the device as COCO.annToRLE does at (H, W) = im_size, the image record's height and width).  boxes fp32 [n,4] x1 y1 x2 y2, scores fp32 [n],
         cls_inds int64 [n] class indices in [1, K], in im_post order.  rle = (counts, run_len) as ops.im_post_rle returns
         them (segm only; they stay on the device).  n_dev: optional device int32 count, as for im_post_rle.  im_size:
-        (H, W) of the detection masks, by default the ground truths' RLE size.  Nothing waits for the device."""
+        (H, W) of the image, the detection masks' size, by default the ground truths' RLE size; needed for polygon
+        ground truths.  Nothing waits for the device (polygon vertices go through the same pinned staging ring)."""
         if image_id in self._seen:
             raise ValueError("image id %r was already added" % (image_id,))
         if len(self._image_ids) >= MAX_AP_IMAGES:
@@ -528,7 +562,9 @@ class DetectionAP:
         segm = self.iou_type == "segm"
         if segm and rle is None:
             raise ValueError("iou_type 'segm' needs rle=(counts, run_len)")
-        table, offs, counts = self._gt_table(gt_anns)
+        # polygon / box-list ground truths are rasterised on the device at the image record's size, given as im_size
+        polys = segm and im_size is not None and any(isinstance(a["segmentation"], list) for a in gt_anns)
+        table, offs, counts = self._gt_table(gt_anns, im_size if polys else None)
         G = table.shape[1]
         cnt, rl, cap, H, W = None, None, 0, 0, 0
         if segm:
@@ -541,15 +577,17 @@ class DetectionAP:
                 H, W = (int(v) for v in im_size)
             elif G:
                 H, W = int(table[7, 0]), int(table[8, 0])
-            nb = query_bytes("cocoeval_workspace_bytes", n, cap, int(counts.size))
+            nb = query_bytes("cocoeval_workspace_bytes", n, cap, counts.bound if polys else int(counts.size))
             if self._ws.numel() < nb:
                 self._ws = torch.empty((nb,), dtype=torch.uint8, device=self.device)
         if n_dev is not None and (not n_dev.is_cuda or n_dev.dtype != torch.int32):
             raise ValueError("n_dev must be a device int32 tensor")
-        if G <= MAX_AP_GT:
-            t_ptr, o_ptr, c_ptr = self._stage_gt(table, offs, counts)
-        else:                          # only counted: the device raises the error flag without reading the table
+        if G > MAX_AP_GT:              # only counted: the device raises the error flag without reading the table
             t_ptr = o_ptr = c_ptr = None
+        elif polys:
+            t_ptr, o_ptr, c_ptr = self._rasterise_gt(table, counts, H, W)
+        else:
+            t_ptr, o_ptr, c_ptr = self._stage([table, offs, counts]) if G else (None, None, None)
         slot = len(self._image_ids)
         call("cocoeval_image", self.device, int(segm), b, s, c, n, n_dev, cnt, cap, rl, H, W,
              t_ptr, G, c_ptr, o_ptr, len(self.cat_ids), self._cls_to_k, slot,

@@ -15,6 +15,7 @@ Reference interfaces mirrored (paths relative to /root/reference/upsnet/):
 Forward only: the inference hot path (SURVEY.md section 8); backward kernels are the training
 config and out of this round's scope.
 """
+import collections
 import ctypes as C
 import math
 
@@ -1347,6 +1348,115 @@ def rle_from_string(s):
             x += cnts[-2]
         cnts.append(x)
     return np.asarray(cnts, np.int64).astype(np.uint32)
+
+
+MAX_POLY_COORD = 4e8       # (int)(5 * c + .5) stays inside int32, as maskApi.c needs
+
+
+# One image's segmentations in upsnet_gt_rle's layout (see pack_segmentations)
+PackedSegms = collections.namedtuple("PackedSegms", "ann_poly poly_vert verts src_off src_counts bound sizes")
+
+
+def pack_segmentations(segms, h, w):
+    """COCO.annToRLE's inputs for upsnet_gt_rle, in annotation order.  A list segmentation is dispatched as
+    maskUtils.frPyObjects does: len(segm[0]) == 4 reads every entry as a box [x, y, bw, bh] (rleFrBbox: the polygon
+    [xs, ys, xs, ye, xe, ye, xe, ys], xe = xs + bw and ye = ys + bh in float64); len(segm[0]) > 4 makes every entry a
+    polygon of k = len(p) // 2 vertices (later ones of 4 or 2 coordinates included); anything else, and an empty list,
+    raises ValueError.  Polygons are rasterised at (h, w), the image record's size.  Any other segmentation (compressed
+    or uncompressed RLE dict, [H,W] mask) is parsed by evaluation.gt_rle into host run lengths that the device copies
+    through.  -> PackedSegms: ann_poly int32 [G+1], poly_vert int32 [P+1], verts float64 [V*2], src_off int64 [G+1],
+    src_counts uint32, bound (int: the run capacity, see upsnet_gt_rle) and sizes int [2, G] (the RLE h, w)."""
+    import itertools
+    from .evaluation import gt_rle
+    h, w = int(h), int(w)
+    if h <= 0 or w <= 0:
+        raise ValueError("image size %dx%d is empty" % (h, w))
+    polys, ann_poly, src, src_len, sizes = [], [0], [], [], []
+    for seg in segms:
+        if isinstance(seg, list):
+            if not seg:
+                raise ValueError("an empty polygon list (pycocotools' frPyObjects indexes segm[0])")
+            n0 = len(seg[0])
+            if n0 == 4:
+                bb = np.asarray(seg, np.float64)            # ragged rows raise, as frBbox's 2-D double buffer does
+                if bb.ndim != 2 or bb.shape[1] != 4:
+                    raise ValueError("a box-list segmentation must be [[x, y, w, h], ...]")
+                xs, ys = bb[:, 0], bb[:, 1]
+                xe, ye = xs + bb[:, 2], ys + bb[:, 3]
+                polys.extend(np.stack([xs, ys, xs, ye, xe, ye, xe, ys], 1))
+            elif n0 > 4:
+                polys.extend(seg)
+            else:
+                raise ValueError("segmentation %r...: input type is not supported (frPyObjects)" % (seg[:1],))
+            src_len.append(0)
+            sizes.append((h, w))
+        else:
+            rh, rw, cnts = gt_rle(seg)
+            src.append(cnts)
+            src_len.append(cnts.size)
+            sizes.append((rh, rw))
+        ann_poly.append(len(polys))
+    k = np.fromiter((len(p) // 2 for p in polys), np.int64, len(polys))
+    poly_vert = np.zeros(len(polys) + 1, np.int64)
+    np.cumsum(k, out=poly_vert[1:])
+    verts = np.fromiter(itertools.chain.from_iterable(p[:2 * n] for p, n in zip(polys, k.tolist())), np.float64,
+                        2 * int(poly_vert[-1]))
+    if not np.all(np.abs(verts) < MAX_POLY_COORD):
+        raise ValueError("polygon coordinates must be finite and below %g in magnitude" % MAX_POLY_COORD)
+    ann_poly = np.asarray(ann_poly, np.int64)
+    src_len = np.asarray(src_len, np.int64)
+    # the run bound: 1 + per edge min(w, (|X1 - X0| + 1) // 5 + 1) over the annotation's polygons, at most h * w + 1
+    X = np.trunc(5.0 * verts[0::2] + .5).astype(np.int64)
+    nxt = np.arange(X.size) + 1
+    full = k > 0
+    nxt[poly_vert[1:][full] - 1] = poly_vert[:-1][full]
+    per_edge = np.minimum(w, (np.abs(X[nxt] - X) + 1) // 5 + 1) if X.size else np.zeros(0, np.int64)
+    ann_of_vert = np.repeat(np.repeat(np.arange(len(segms)), np.diff(ann_poly)), k)
+    edges = np.bincount(ann_of_vert, weights=per_edge, minlength=len(segms)).astype(np.int64)
+    is_poly = np.diff(ann_poly) > 0
+    bound = int(np.where(is_poly, np.minimum(edges + 1, h * w + 1), src_len).sum())
+    src_off = np.zeros(len(segms) + 1, np.int64)
+    np.cumsum(src_len, out=src_off[1:])
+    return PackedSegms(ann_poly=ann_poly.astype(np.int32), poly_vert=poly_vert.astype(np.int32), verts=verts,
+                       src_off=src_off, src_counts=np.concatenate(src).astype(np.uint32) if src else np.zeros(0, np.uint32),
+                       bound=bound, sizes=np.asarray(sizes, np.int64).reshape(-1, 2).T)
+
+
+def gt_rle_arrays(pk):
+    """The host arrays upsnet_gt_rle reads, in the order gt_rle_call takes their device addresses."""
+    return [pk.verts, pk.src_off, pk.ann_poly, pk.poly_vert, pk.src_counts]
+
+
+def gt_rle_call(pk, h, w, ptrs, counts, offsets, err, ws):
+    """Launches upsnet_gt_rle on the current stream for a PackedSegms whose gt_rle_arrays() were staged at the device
+    addresses ptrs; counts int32 [>= pk.bound], offsets int64 [G + 1], err device int32 [1], ws its workspace."""
+    call("gt_rle", counts.device, int(h), int(w), len(pk.ann_poly) - 1, ptrs[2], ptrs[3], ptrs[0], ptrs[1], ptrs[4],
+         counts, counts.numel(), offsets, err, ws, ws.numel())
+
+
+def ann_to_rle(segms, h, w, device=None, err=None):
+    """COCO.annToRLE of one image's segmentations on the device (upsnet_gt_rle), at the image record's (h, w): polygon
+    lists and box lists (see pack_segmentations) are rasterised by maskApi.c's rleFrPoly rule and their parts united,
+    RLE dicts (compressed or uncompressed) and [H,W] masks are copied through.  Returns (counts int32 [>= total] holding
+    the uint32 run lengths back to back, offsets int64 [G+1]) on the device; annotation g's runs are
+    counts[offsets[g]:offsets[g+1]].  err: optional device int32 [1] that gets UPSNET_GT_RLE_E_CAPACITY OR-ed in if the
+    runs outgrow the host's bound (then every offset is 0).  Nothing waits for the device."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    pk = pack_segmentations(segms, h, w)
+    G = len(pk.ann_poly) - 1
+    arrays = gt_rle_arrays(pk)
+    offs = np.cumsum([0] + [a.nbytes + (-a.nbytes) % 8 for a in arrays])
+    host = torch.empty((max(int(offs[-1]), 8),), dtype=torch.uint8, pin_memory=True)
+    for a, o in zip(arrays, offs):
+        host.numpy()[o:o + a.nbytes] = a.view(np.uint8)
+    stage = host.to(dev, non_blocking=True)
+    out = (torch.empty((max(pk.bound, 1),), dtype=torch.int32, device=dev),
+           torch.empty((G + 1,), dtype=torch.int64, device=dev))
+    if err is None:
+        err = torch.zeros((1,), dtype=torch.int32, device=dev)
+    ws = torch.empty((max(query_bytes("gt_rle_workspace_bytes", G, int(h), int(w)), 1),), dtype=torch.uint8, device=dev)
+    gt_rle_call(pk, h, w, [C.c_void_p(stage.data_ptr() + int(o)) for o in offs[:-1]], out[0], out[1], err, ws)
+    return out
 
 
 def im_post_rle(pred_boxes, pred_masks, cls_inds, im_h, im_w, n_dev=None, cap=None):
