@@ -970,6 +970,37 @@ int upsnet_conv_wgrad(const void *x_nhwc, const void *g, float *dw, int N, int H
                       int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int flags, int precision,
                       void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---------------------------------------------------------------------------------------
+ * GroupNorm (csrc/group_norm.cu): nn.GroupNorm(groups, C) semantics -- biased variance, y = (x - mean) / sqrt(var + eps)
+ * * gamma + beta -- over NHWC activations.  Deterministic: no atomics, fixed merge orders.
+ * replaces: nn.GroupNorm(32, C) of models/fpn.py:43-58, rpn.py:37-40, rcnn.py:50-56 and :102-104, fcn.py:49-50.
+ *
+ * upsnet_group_norm_forward: whole maps.  x, y [N,H,W,C] in dtype (F32, BF16, or PAIR: [N,H,W,2C]); statistics cover
+ * all H*W pixels of an image.  Three launches: per-(image, group, CTA) partial (count, mean, M2), their merge by Chan's
+ * formula into stats[N][groups][2] = (mean, 1/sqrt(var + eps)) (fp32, caller-owned, read by the backward), and the
+ * apply.  shift (fp32 [N][C] or NULL) is added after beta; flags: UPSNET_EPI_RELU; UPSNET_EPI_RES_UP2 with residual
+ * [N,H/2,W/2,C] in dtype, read with nearest 2x up-sampling and added before the ReLU (H, W even).  C <= 1024 with
+ * min(C, 256) dividing both 256 and C, else UPSNET_E_UNSUPPORTED.  Workspace: upsnet_group_norm_workspace_bytes.
+ *
+ * upsnet_group_norm_rows: R rows of HW pixels x C channels (NHWC, dtype as above), each row normalised on its own (the
+ * mask branch's 14x14 roi maps, RCNN fc6 as [R,1024,1,1]); one launch, one warp per (row, group), two passes.  flags:
+ * UPSNET_EPI_RELU.  n_dev (int32 device scalar or NULL): rows >= *n_dev are skipped and their output is unspecified.
+ *
+ * upsnet_group_norm_backward: gradients of y = act(GN(x) + shift [+ up2(residual)]), fp32 NHWC.  dy, x, dx [N,H,W,C];
+ * y the forward output (read for the ReLU mask; pass it iff flags has UPSNET_EPI_RELU); stats from the forward.
+ * dgamma, dbeta [C], dshift [N][C] (= per-image dbeta) and dres [N,H/2,W/2,C] (needs UPSNET_EPI_RES_UP2) are each
+ * optional.  Workspace: upsnet_group_norm_backward_workspace_bytes. */
+int upsnet_group_norm_workspace_bytes(int N, int C, int H, int W, int groups, size_t *bytes);
+int upsnet_group_norm_forward(const void *x, const float *gamma, const float *beta, const float *shift,
+                              const void *residual, void *y, float *stats, int N, int C, int H, int W, int groups,
+                              float eps, int dtype, int flags, void *workspace, size_t workspace_bytes, void *stream);
+int upsnet_group_norm_rows(const void *x, const float *gamma, const float *beta, void *y, int R, int C, int HW, int groups,
+                           float eps, int dtype, int flags, const int *n_dev, void *stream);
+int upsnet_group_norm_backward_workspace_bytes(int N, int C, int H, int W, int groups, size_t *bytes);
+int upsnet_group_norm_backward(const float *dy, const float *x, const float *y, const float *stats, const float *gamma,
+                               float *dx, float *dgamma, float *dbeta, float *dshift, float *dres, int N, int C, int H,
+                               int W, int groups, int flags, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

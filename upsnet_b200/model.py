@@ -71,6 +71,12 @@ class UPSNetConfig:
         self.rpn_batch_size = 256
         self.fg_fraction = 0.25
         self.fcn_with_roi_loss = False
+        # network.{fpn,rpn,rcnn,fcn}_with_norm: 'none' or 'group_norm' (nn.GroupNorm(32, C) after each conv of the head);
+        # 'batch_norm' needs the reference's absent distbatchnorm module and is refused by resnet_upsnet
+        self.fpn_with_norm = "none"
+        self.rpn_with_norm = "none"
+        self.rcnn_with_norm = "none"
+        self.fcn_with_norm = "none"
         for k, v in kw.items():
             if not hasattr(self, k):
                 raise AttributeError(k)
@@ -108,7 +114,8 @@ class UPSNetConfig:
                    train_rpn_min_size=int(get("train", "rpn_min_size", 0)),
                    batch_rois=int(get("train", "batch_rois", 512)), rpn_batch_size=int(get("train", "rpn_batch_size", 256)),
                    fg_fraction=float(get("train", "fg_fraction", 0.25)),
-                   fcn_with_roi_loss=bool(get("train", "fcn_with_roi_loss", False)))
+                   fcn_with_roi_loss=bool(get("train", "fcn_with_roi_loss", False)),
+                   **{k: str(get("network", k, "none")) for k in NORM_KEYS})
 
     @classmethod
     def cityscapes_r50(cls):      # experiments/upsnet_resnet50_cityscapes_16gpu.yaml
@@ -122,6 +129,27 @@ class UPSNetConfig:
     def coco_r101_dcn(cls):       # experiments/upsnet_resnet101_dcn_coco_3x_16gpu.yaml
         return cls(num_classes=81, num_seg_classes=133, backbone_with_dconv=3, fpn_with_gap=True,
                    fcn_num_layers=3, fcn_with_roi_loss=True)
+
+
+NORM_KEYS = ("fpn_with_norm", "rpn_with_norm", "rcnn_with_norm", "fcn_with_norm")
+
+
+def _check_norms(cfg):
+    """The reference builds nn.GroupNorm(32, C) for 'group_norm'; its 'batch_norm' is a BatchNorm2d imported only from
+    the absent distbatchnorm module (models/fpn.py:22-23), so it raises NameError there and UpsnetError here.
+    rpn_with_norm is read but unused: models/resnet_upsnet.py:52 builds the RPN without passing it."""
+    for k in NORM_KEYS:
+        v = getattr(cfg, k)
+        if v not in ("none", "group_norm", "batch_norm"):
+            raise _lib.UpsnetError("network.%s: %r is not one of 'none', 'group_norm', 'batch_norm'" % (k, v))
+        if v == "batch_norm" and k != "rpn_with_norm":
+            raise _lib.UpsnetError("network.%s = 'batch_norm' is not built: the reference's BatchNorm2d comes from its "
+                                   "absent distbatchnorm module (SyncBN); use 'group_norm' or 'none'" % k)
+
+
+def _gn_conv(cin, cout, k, padding=0):
+    """conv (no bias) + nn.GroupNorm(32, cout): the reference's normed conv (models/fpn.py:47-54)."""
+    return nn.Sequential(nn.Conv2d(cin, cout, k, padding=padding, bias=False), nn.GroupNorm(32, cout))
 
 
 def _fold_bn(conv_w, bn):
@@ -278,27 +306,52 @@ class ResNetBackbone(nn.Module):
 # FPN / RPN / heads (models/fpn.py, rpn.py, rcnn.py, fcn.py)
 # ---------------------------------------------------------------------------------------------
 class FPN(nn.Module):
-    """models/fpn.py:25-104 (with_norm='none', nearest upsampling, P6 = stride-2 subsample of P5)."""
+    """models/fpn.py:25-104 (with_norm 'none' or 'group_norm', nearest upsampling, P6 = stride-2 subsample of P5)."""
 
-    def __init__(self, feature_dim, with_gap):
+    def __init__(self, feature_dim, with_gap, with_norm="none"):
         super().__init__()
         self.feature_dim = feature_dim
+        self.gn = with_norm == "group_norm"
         if with_gap:
             self.fpn_gap = nn.Linear(2048, feature_dim)
         for name, cin in (("fpn_p5_1x1", 2048), ("fpn_p4_1x1", 1024), ("fpn_p3_1x1", 512), ("fpn_p2_1x1", 256)):
-            setattr(self, name, nn.Conv2d(cin, feature_dim, 1))
+            setattr(self, name, _gn_conv(cin, feature_dim, 1) if self.gn else nn.Conv2d(cin, feature_dim, 1))
         for name in ("fpn_p5", "fpn_p4", "fpn_p3", "fpn_p2"):
-            setattr(self, name, nn.Conv2d(feature_dim, feature_dim, 3, padding=1))
+            setattr(self, name, _gn_conv(feature_dim, feature_dim, 3, 1) if self.gn else
+                    nn.Conv2d(feature_dim, feature_dim, 3, padding=1))
         for m in self.modules():
             if isinstance(m, nn.Conv2d):
                 nn.init.kaiming_uniform_(m.weight.data, a=1)
-                m.bias.data.zero_()
+                if m.bias is not None:
+                    m.bias.data.zero_()
 
     @staticmethod
     def _c(m, x, residual=None, padding=0, up2=False):
         return ops.conv2d(x, m.weight, m.bias, padding=padding, residual=residual, residual_up2=up2)
 
+    def _forward_gn(self, res2, res3, res4, res5):
+        """with_norm = 'group_norm': each conv without bias, then the GN apply with the rest of the reference's sum
+        fused in -- fpn_gap as the extra per-channel shift of P5's lateral, the nearest-2x top-down add as its residual."""
+        def c(name, x, padding=0, **kw):
+            conv, gn = getattr(self, name)
+            t = ops.conv2d(x, conv.weight, None, padding=padding)
+            return ops.group_norm(t, gn.weight, gn.bias, gn.num_groups, gn.eps, **kw)
+        shift = None
+        if hasattr(self, "fpn_gap"):
+            shift = ops.linear(res5.float().mean(dim=(2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, out_dtype=torch.float32)
+        p5_1x1 = c("fpn_p5_1x1", res5, shift=shift)
+        p4_plus = c("fpn_p4_1x1", res4, residual=p5_1x1, residual_up2=True)
+        p3_plus = c("fpn_p3_1x1", res3, residual=p4_plus, residual_up2=True)
+        p2_plus = c("fpn_p2_1x1", res2, residual=p3_plus, residual_up2=True)
+        p5 = c("fpn_p5", p5_1x1, padding=1)
+        p4 = c("fpn_p4", p4_plus, padding=1)
+        p3 = c("fpn_p3", p3_plus, padding=1)
+        p2 = c("fpn_p2", p2_plus, padding=1)
+        return p2, p3, p4, p5, ops.subsample2(p5)
+
     def forward(self, res2, res3, res4, res5):
+        if self.gn:
+            return self._forward_gn(res2, res3, res4, res5)
         p5_1x1 = self._c(self.fpn_p5_1x1, res5)
         if hasattr(self, "fpn_gap"):
             gap = ops.linear(res5.float().mean(dim=(2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, out_dtype=torch.float32)
@@ -321,6 +374,9 @@ class FPN(nn.Module):
         """forward with device gradients (training.conv2d, the same fused top-down add).  With fpn_gap, the context
         vector fpn_gap(GAP(res5)) (models/fpn.py:84-86, added to every P5 lateral pixel) is folded into the bias of the
         P5 lateral conv, so that conv's d bias carries the gradient to both biases, fpn_gap and res5."""
+        if self.gn:
+            return self._forward_train_gn(res2, res3, res4, res5, prec)
+
         def c(m, x, bias=None, **kw):
             return training.conv2d(x, m.weight, m.bias if bias is None else bias, precision=prec, **kw)
         p5_bias = None
@@ -335,6 +391,26 @@ class FPN(nn.Module):
         p3 = c(self.fpn_p3, p3_plus, padding=1)
         p4 = c(self.fpn_p4, p4_plus, padding=1)
         p5 = c(self.fpn_p5, p5_1x1, padding=1)
+        return p2, p3, p4, p5, p5[:, :, ::2, ::2]
+
+    def _forward_train_gn(self, res2, res3, res4, res5, prec):
+        """forward_train with group_norm: training.conv2d without bias, then training.group_norm with the top-down add
+        and the context vector as its residual and shift, so their gradients leave the GN backward."""
+        def c(name, x, padding=0, residual=None, shift=None):
+            conv, gn = getattr(self, name)
+            t = training.conv2d(x, conv.weight, None, padding=padding, precision=prec)
+            return training.group_norm(t, gn.weight, gn.bias, gn.num_groups, gn.eps, residual=residual, shift=shift)
+        shift = None
+        if hasattr(self, "fpn_gap"):        # one image: the context vector is one row
+            shift = training.linear(res5.mean((2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, precision=prec)
+        p5_1x1 = c("fpn_p5_1x1", res5, shift=shift)
+        p4_plus = c("fpn_p4_1x1", res4, residual=p5_1x1)
+        p3_plus = c("fpn_p3_1x1", res3, residual=p4_plus)
+        p2_plus = c("fpn_p2_1x1", res2, residual=p3_plus)
+        p2 = c("fpn_p2", p2_plus, padding=1)
+        p3 = c("fpn_p3", p3_plus, padding=1)
+        p4 = c("fpn_p4", p4_plus, padding=1)
+        p5 = c("fpn_p5", p5_1x1, padding=1)
         return p2, p3, p4, p5, p5[:, :, ::2, ::2]
 
 
@@ -377,11 +453,16 @@ class RPN(nn.Module):
 class RCNN(nn.Module):
     """models/rcnn.py:89-146."""
 
-    def __init__(self, num_classes, num_reg_classes, pool_size=7, dim_in=256, dim_hidden=1024):
+    def __init__(self, num_classes, num_reg_classes, pool_size=7, dim_in=256, dim_hidden=1024, with_norm="none"):
         super().__init__()
         self.pool_size = pool_size
         self.roi_pooling = ops.FPNRoIAlign(pool_size, pool_size, [1.0 / 4, 1.0 / 8, 1.0 / 16, 1.0 / 32])
-        self.fc6 = nn.Sequential(nn.Linear(pool_size ** 2 * dim_in, dim_hidden), nn.ReLU(inplace=True))
+        self.gn = with_norm == "group_norm"
+        if self.gn:     # models/rcnn.py:102: Linear, View(-1, C, 1, 1), GroupNorm, View(-1, C), ReLU
+            self.fc6 = nn.Sequential(nn.Linear(pool_size ** 2 * dim_in, dim_hidden), nn.Unflatten(1, (dim_hidden, 1, 1)),
+                                     nn.GroupNorm(32, dim_hidden), nn.Flatten(), nn.ReLU(inplace=True))
+        else:
+            self.fc6 = nn.Sequential(nn.Linear(pool_size ** 2 * dim_in, dim_hidden), nn.ReLU(inplace=True))
         self.fc7 = nn.Sequential(nn.Linear(dim_hidden, dim_hidden), nn.ReLU(inplace=True))
         self.cls_score = nn.Linear(dim_hidden, num_classes)
         self.bbox_pred = nn.Linear(dim_hidden, num_reg_classes * 4)
@@ -417,7 +498,10 @@ class RCNN(nn.Module):
                 x, w6 = nhwc.reshape(pool.size(0), -1), self._w6_nhwc
             else:
                 x, w6 = pool.reshape(pool.size(0), -1), self.fc6[0].weight
-        fc6 = ops.linear(x, w6, self.fc6[0].bias, relu=True)
+        fc6 = ops.linear(x, w6, self.fc6[0].bias, relu=not self.gn)
+        if self.gn:
+            gn = self.fc6[2]
+            fc6 = ops.group_norm_rows(fc6, gn.weight, gn.bias, gn.num_groups, gn.eps, relu=True)
         fc7 = ops.linear(fc6, self.fc7[0].weight, self.fc7[0].bias, relu=True)
         both = ops.linear(fc7, self._f[0], self._f[1], out_dtype=torch.float32).float()
         return {"cls_score": both[:, :self.num_classes].contiguous(),
@@ -428,8 +512,11 @@ class RCNN(nn.Module):
         two heads as separate training.linear calls."""
         ps = self.pool_size
         pool = training.FPNRoIAlignFunction.apply(rois, ps, ps, self.roi_pooling.spatial_scale, 2, *feat)
-        fc6 = training.linear(pool.reshape(pool.shape[0], -1), self.fc6[0].weight, self.fc6[0].bias, relu=True,
+        fc6 = training.linear(pool.reshape(pool.shape[0], -1), self.fc6[0].weight, self.fc6[0].bias, relu=not self.gn,
                               precision=prec)
+        if self.gn:
+            gn = self.fc6[2]
+            fc6 = training.group_norm(fc6, gn.weight, gn.bias, gn.num_groups, gn.eps, relu=True)
         fc7 = training.linear(fc6, self.fc7[0].weight, self.fc7[0].bias, relu=True, precision=prec)
         return (training.linear(fc7, self.cls_score.weight, self.cls_score.bias, precision=prec),
                 training.linear(fc7, self.bbox_pred.weight, self.bbox_pred.bias, precision=prec))
@@ -438,17 +525,21 @@ class RCNN(nn.Module):
 class MaskBranch(nn.Module):
     """models/rcnn.py:34-87: ROIAlign 14x14 -> 4 x (3x3 + ReLU) -> deconv 2x2/2 + ReLU -> 1x1."""
 
-    def __init__(self, num_classes, mask_size=28, dim_in=256, dim_hidden=256):
+    def __init__(self, num_classes, mask_size=28, dim_in=256, dim_hidden=256, with_norm="none"):
         super().__init__()
         self.roi_pooling = ops.FPNRoIAlign(mask_size // 2, mask_size // 2, [1.0 / 4, 1.0 / 8, 1.0 / 16, 1.0 / 32])
+        self.gn = with_norm == "group_norm"
         for i, cin in enumerate((dim_in, dim_hidden, dim_hidden, dim_hidden), start=1):
-            setattr(self, "mask_conv%d" % i, nn.Sequential(nn.Conv2d(cin, dim_hidden, 3, 1, 1), nn.ReLU(inplace=True)))
+            layers = [nn.Conv2d(cin, dim_hidden, 3, 1, 1, bias=False), nn.GroupNorm(32, dim_hidden)] if self.gn else \
+                [nn.Conv2d(cin, dim_hidden, 3, 1, 1)]
+            setattr(self, "mask_conv%d" % i, nn.Sequential(*layers, nn.ReLU(inplace=True)))
         self.mask_deconv1 = nn.Sequential(nn.ConvTranspose2d(dim_hidden, dim_hidden, 2, 2, 0), nn.ReLU(inplace=True))
         self.mask_score = nn.Conv2d(dim_hidden, num_classes, 1)
         for m in self.modules():
             if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
                 nn.init.kaiming_normal_(m.weight.data, mode="fan_in")
-                m.bias.data.zero_()
+                if m.bias is not None:
+                    m.bias.data.zero_()
         self._f = None
 
     def prepare(self):
@@ -470,8 +561,10 @@ class MaskBranch(nn.Module):
             r = self.roi_pooling
             x = ops.fpn_roi_align(list(feat), rois, r.pooled_height, r.pooled_width, r.spatial_scale, layout="auto", **bound)
         for i in range(1, 5):
-            c = getattr(self, "mask_conv%d" % i)[0]
-            x = ops.conv2d(x, c.weight, c.bias, padding=1, relu=True, **bound)
+            c = getattr(self, "mask_conv%d" % i)
+            x = ops.conv2d(x, c[0].weight, c[0].bias, padding=1, relu=not self.gn, **bound)
+            if self.gn:
+                x = ops.group_norm_rows(x, c[1].weight, c[1].bias, c[1].num_groups, c[1].eps, relu=True, n_dev=n_dev)
         w1, b1, cout = self._f
         if isinstance(x, ops.Pair):
             # pair stream: the deconv-as-1x1 conv writes its four (a, b) groups as [hi Cout][lo Cout] each, i.e. directly
@@ -504,8 +597,10 @@ class MaskBranch(nn.Module):
             return feat[0].new_zeros((0, self.mask_score.weight.shape[0], 2 * M, 2 * M))
         x = training.FPNRoIAlignFunction.apply(rois, M, M, self.roi_pooling.spatial_scale, 2, *feat)
         for i in range(1, 5):
-            c = getattr(self, "mask_conv%d" % i)[0]
-            x = training.conv2d(x, c.weight, c.bias, padding=1, relu=True, precision=prec)
+            c = getattr(self, "mask_conv%d" % i)
+            x = training.conv2d(x, c[0].weight, c[0].bias, padding=1, relu=not self.gn, precision=prec)
+            if self.gn:
+                x = training.group_norm(x, c[1].weight, c[1].bias, c[1].num_groups, c[1].eps, relu=True)
         d = self.mask_deconv1[0]
         x = training.conv_transpose2x2(x, d.weight, d.bias, relu=True, precision=prec)
         return training.conv2d(x, self.mask_score.weight, self.mask_score.bias, precision=prec)
@@ -514,10 +609,11 @@ class MaskBranch(nn.Module):
 class FCNSubNet(nn.Module):
     """models/fcn.py:29-73: num_layers x (DeformConvWithOffset + ReLU); channel drop at layer n-2."""
 
-    def __init__(self, in_channels, out_channels, num_layers):
+    def __init__(self, in_channels, out_channels, num_layers, with_norm="none"):
         super().__init__()
         assert num_layers >= 2
         self.num_layers = num_layers
+        self.gn = with_norm == "group_norm"
         self.conv = nn.ModuleList()
         for i in range(num_layers):
             if i == num_layers - 2:
@@ -525,7 +621,8 @@ class FCNSubNet(nn.Module):
                 in_channels = out_channels
             else:
                 layer = DeformConvWithOffset(in_channels, in_channels, 3, stride=1, padding=1, dilation=1)
-            self.conv.append(nn.Sequential(layer, nn.ReLU(inplace=True)))
+            norm = [nn.GroupNorm(32, in_channels)] if self.gn else []       # models/fcn.py:49-50
+            self.conv.append(nn.Sequential(layer, *norm, nn.ReLU(inplace=True)))
         for m in self.modules():
             if isinstance(m, nn.Conv2d):
                 m.weight.data.fill_(0)
@@ -540,16 +637,31 @@ class FCNSubNet(nn.Module):
             l = self.conv[i][0]
             offset = ops.conv2d(x, l.conv_offset.weight, l.conv_offset.bias, 1, 1, 1, out_format="nchw")
             x = ops.deform_conv(x, offset, l.conv.weight, l.conv.bias, l.conv.stride, l.conv.padding,
-                                l.conv.dilation, l.conv.deformable_groups, relu=True)   # ReLU fused
+                                l.conv.dilation, l.conv.deformable_groups, relu=not self.gn)   # ReLU fused
+            if self.gn:
+                gn = self.conv[i][1]
+                x = ops.group_norm(x, gn.weight, gn.bias, gn.num_groups, gn.eps, relu=True)
+        return x
+
+    def forward_train(self, x):
+        """forward with device gradients: each DeformConvWithOffset (its autograd Functions), then GN + ReLU through
+        training.group_norm or the ReLU alone."""
+        for i in range(self.num_layers):
+            x = self.conv[i][0](x)
+            if self.gn:
+                gn = self.conv[i][1]
+                x = training.group_norm(x, gn.weight, gn.bias, gn.num_groups, gn.eps, relu=True)
+            else:
+                x = F.relu(x)
         return x
 
 
 class FCNHead(nn.Module):
     """models/fcn.py:76-108."""
 
-    def __init__(self, in_channels, num_classes, num_layers, upsample_rate=4):
+    def __init__(self, in_channels, num_classes, num_layers, upsample_rate=4, with_norm="none"):
         super().__init__()
-        self.fcn_subnet = FCNSubNet(in_channels, 128, num_layers)
+        self.fcn_subnet = FCNSubNet(in_channels, 128, num_layers, with_norm)
         self.upsample_rate = upsample_rate
         self.score = nn.Conv2d(512, num_classes, 1)
         nn.init.normal_(self.score.weight.data, 0, 0.01)
@@ -627,8 +739,7 @@ class FCNHead(nn.Module):
         w = self.score.weight
         scores = []
         for l, feat in enumerate((p2, p3, p4, p5)):
-            for i in range(self.fcn_subnet.num_layers):
-                feat = F.relu(self.fcn_subnet.conv[i][0](feat))
+            feat = self.fcn_subnet.forward_train(feat)
             scores.append(training.conv2d(feat, w[:, 128 * l:128 * (l + 1)], self.score.bias if l == 0 else None,
                                           precision=prec))
         return training.FcnScoreFuseFunction.apply(*scores)
@@ -644,12 +755,15 @@ class resnet_upsnet(nn.Module):
         self.cfg = cfg
         self.num_classes, self.num_seg_classes = cfg.num_classes, cfg.num_seg_classes
         self.num_reg_classes = cfg.num_classes
+        _check_norms(cfg)
         self.resnet_backbone = ResNetBackbone(backbone_depth, cfg)
-        self.fpn = FPN(cfg.fpn_feature_dim, cfg.fpn_with_gap)
-        self.rpn = RPN(cfg.num_anchors, cfg.fpn_feature_dim)
-        self.rcnn = RCNN(self.num_classes, self.num_reg_classes, dim_in=cfg.fpn_feature_dim)
-        self.mask_branch = MaskBranch(self.num_classes, cfg.mask_size, dim_in=cfg.fpn_feature_dim)
-        self.fcn_head = FCNHead(cfg.fpn_feature_dim, self.num_seg_classes, cfg.fcn_num_layers)
+        self.fpn = FPN(cfg.fpn_feature_dim, cfg.fpn_with_gap, cfg.fpn_with_norm)
+        self.rpn = RPN(cfg.num_anchors, cfg.fpn_feature_dim)      # rpn_with_norm unused, as in resnet_upsnet.py:52
+        self.rcnn = RCNN(self.num_classes, self.num_reg_classes, dim_in=cfg.fpn_feature_dim, with_norm=cfg.rcnn_with_norm)
+        self.mask_branch = MaskBranch(self.num_classes, cfg.mask_size, dim_in=cfg.fpn_feature_dim,
+                                      with_norm=cfg.rcnn_with_norm)
+        self.fcn_head = FCNHead(cfg.fpn_feature_dim, self.num_seg_classes, cfg.fcn_num_layers,
+                                with_norm=cfg.fcn_with_norm)
         self.enable_void = cfg.panoptic_box_keep_fraction < 1
         assert self.enable_void, "all shipped configs enable the void channel"
         self.pyramid_proposal = ProposalGenerator(cfg.rpn_feat_stride, cfg.anchor_scales, cfg.anchor_ratios,
@@ -970,20 +1084,32 @@ class resnet_upsnet(nn.Module):
 
     def get_params_lr(self):
         """The reference's 13 parameter groups (models/resnet_upsnet.py:260-285, get_params of models/resnet.py:31-51):
-        the (empty) norm group, then for res3-res5, fpn, rcnn, mask_branch, rpn and fcn_head the weights at lr 1 and the
-        biases at lr 2 without weight decay, selected by the same name rule.  Only parameters with requires_grad."""
-        def params(prefixes, suffix):
+        the GroupNorm group (every nn.GroupNorm's weight and bias, at lr 1 without weight decay; empty without
+        group_norm), then for res3-res5, fpn, rcnn, mask_branch, rpn and fcn_head the weights at lr 1 and the biases at
+        lr 2 without weight decay, selected by the same name rule, with the GroupNorm parameters excluded except from
+        the rpn groups (the reference does not exclude them there; its RPN never has any).  Only parameters with
+        requires_grad, except in the GroupNorm group, which the reference does not filter."""
+        gn_params, gn_names = [], set()
+        for n, m in self.named_modules():
+            if isinstance(m, nn.GroupNorm):
+                gn_params += [m.weight, m.bias]
+                gn_names |= {n + ".weight", n + ".bias"}
+
+        def params(prefixes, suffix, exclude=()):
             for name, module in self.named_modules():
                 if name in prefixes:
                     for n, p in module.named_parameters():
                         n = name + "." + n
+                        if n in exclude:
+                            continue
                         if (n.split(".")[-1].startswith(suffix) or n.endswith(suffix)) and p.requires_grad:
                             yield p
-        groups = [{"params": [], "lr": 1, "weight_decay": 0}]
+        groups = [{"params": gn_params, "lr": 1, "weight_decay": 0}]
         for prefixes in (["resnet_backbone.res3", "resnet_backbone.res4", "resnet_backbone.res5"], ["fpn"], ["rcnn"],
                          ["mask_branch"], ["rpn"], ["fcn_head"]):
-            groups.append({"params": list(params(prefixes, "weight")), "lr": 1})
-            groups.append({"params": list(params(prefixes, "bias")), "lr": 2, "weight_decay": 0})
+            ex = gn_names if prefixes[0] in ("fpn", "rcnn", "mask_branch", "fcn_head") else ()
+            groups.append({"params": list(params(prefixes, "weight", ex)), "lr": 1})
+            groups.append({"params": list(params(prefixes, "bias", ex)), "lr": 2, "weight_decay": 0})
         return groups
 
     def forward(self, data, label=None):

@@ -552,6 +552,72 @@ def fcn_score_fuse(s2, s3, s4, s5):
     return out
 
 
+def _gn_store(x, like=None):
+    """(NHWC storage, dtype code) of an activation for the GroupNorm kernels: a Pair's store, or the NHWC storage of a
+    bf16 / fp32 logical [N,C,H,W] tensor (a copy only when it is not channels_last).  With `like`, x is first brought
+    to the format of that storage (the residual of the FPN top-down add)."""
+    if like is not None:
+        if like.dtype == "pair":
+            x = x if isinstance(x, Pair) else Pair.from_float(x)
+        else:
+            x = as_float(x).to(like.dtype)
+    if isinstance(x, Pair):
+        return x.store, _lib.DTYPE_PAIR
+    if x.dtype not in (torch.float32, torch.bfloat16):
+        x = x.float()
+    return _nhwc(x), (_lib.DTYPE_BF16 if x.dtype == torch.bfloat16 else _lib.DTYPE_F32)
+
+
+def _gn_wrap(store, dt):
+    return Pair(store) if dt == _lib.DTYPE_PAIR else store.permute(0, 3, 1, 2)
+
+
+def group_norm(x, weight, bias, groups=32, eps=1e-5, relu=False, residual=None, residual_up2=False, shift=None,
+               return_stats=False):
+    """nn.GroupNorm(groups, C) over whole maps, with the optional epilogue y = act(GN(x) + shift + up2(residual)):
+    shift float32 [N, C] (FPN's context vector, models/fpn.py:84-86), residual [N,C,H/2,W/2] read with nearest 2x
+    up-sampling (the FPN top-down add; residual_up2 must be set), ReLU.  x: a Pair, or a bf16 / fp32 logical [N,C,H,W]
+    tensor; y has x's format (Pair, or NHWC storage viewed as [N,C,H,W]).  With return_stats also the float32
+    [N, groups, 2] (mean, 1 / sqrt(var + eps)) that upsnet_group_norm_backward reads."""
+    require_cuda(x, weight, bias, shift)
+    if (residual is not None) != bool(residual_up2):
+        raise _lib.UpsnetError("group_norm: a residual is read with nearest 2x up-sampling only (residual_up2=True)")
+    N, C, H, W = x.shape
+    xs, dt = _gn_store(x)
+    res = None if residual is None else _gn_store(residual, like=xs if dt != _lib.DTYPE_PAIR else x)[0]
+    y = torch.empty_like(xs)
+    stats = torch.empty((N, groups, 2), dtype=torch.float32, device=xs.device)
+    ws = torch.empty(query_bytes("group_norm_workspace_bytes", N, C, H, W, groups), dtype=torch.uint8, device=xs.device)
+    nbytes = xs.numel() * xs.element_size()
+    work = {"bytes": float(3 * nbytes + (0 if res is None else res.numel() * res.element_size())),
+            "shape": "N%d %dx%d C%d G%d %s%s%s" % (N, H, W, C, groups, {0: "float32", 1: "bfloat16", 2: "pair"}[dt],
+                                                  " +res" if res is not None else "", " +shift" if shift is not None else "")}
+    flags = (_lib.EPI_RELU if relu else 0) | (_lib.EPI_RES_UP2 if res is not None else 0)
+    with _Timed("group_norm", 3, work, xs.device):
+        call("group_norm_forward", xs.device, xs, f32c(weight), f32c(bias), None if shift is None else f32c(shift), res,
+             y, stats, N, C, H, W, groups, float(eps), dt, flags, ws, ws.numel())
+    out = _gn_wrap(y, dt)
+    return (out, stats) if return_stats else out
+
+
+def group_norm_rows(x, weight, bias, groups=32, eps=1e-5, relu=False, n_dev=None):
+    """nn.GroupNorm(groups, C) of every row on its own, one launch: x a Pair or bf16 / fp32 tensor of logical shape
+    [R,C,h,w] (the mask branch's roi maps) or a [R,C] tensor (RCNN fc6, models/rcnn.py:102 views it as [R,C,1,1]).
+    n_dev: optional int32 device count; rows >= n_dev are skipped (their output is unspecified).  y has x's format."""
+    require_cuda(x, weight, bias)
+    flat = not isinstance(x, Pair) and x.dim() == 2
+    xs, dt = _gn_store(x.reshape(x.shape[0], x.shape[1], 1, 1) if flat else x)
+    R, h, w, _ = xs.shape
+    C = weight.shape[0]
+    y = torch.empty_like(xs)
+    work = {"bytes": float(2 * xs.numel() * xs.element_size()),
+            "shape": "R%d %dx%d C%d G%d rows" % (R, h, w, C, groups)}
+    with _Timed("group_norm", 1, work, xs.device):
+        call("group_norm_rows", xs.device, xs, f32c(weight), f32c(bias), y, R, C, h * w, groups, float(eps), dt,
+             _lib.EPI_RELU if relu else 0, _count(n_dev))
+    return y.reshape(R, C) if flat else _gn_wrap(y, dt)
+
+
 def fpn_roi_align(feats, rois, pooled_height, pooled_width, spatial_scales, sampling_ratio=2, layout="nchw",
                   return_levels=False, n_dev=None):
     """FPNRoIAlign.forward in one launch (level assignment on device, output already in roi order).

@@ -10,7 +10,7 @@ def synthetic_model(cfg=None, depth=(3, 4, 6, 3), seed=0, device="cpu"):
     (a) offset convs get non-zero weights/biases so DCN offsets are a few pixels (the reference zero-inits
     them, modules/deform_conv.py:72-73 -- zero offsets would hide DCN bugs), (b) BN statistics are
     randomised so folding is exercised, (c) the class / mask heads are biased so that several dozen
-    detections survive score > 0.6 and reach the panoptic head."""
+    detections survive score > 0.6 and reach the panoptic head, (d) GroupNorm affines are randomised around (1, 0)."""
     from upsnet_b200.model import resnet_upsnet, Bottleneck
     from upsnet_b200.operators import DeformConvWithOffset
     g = torch.Generator().manual_seed(seed)
@@ -58,6 +58,10 @@ def synthetic_model(cfg=None, depth=(3, 4, 6, 3), seed=0, device="cpu"):
         m.rcnn.bbox_pred.weight.copy_(torch.empty_like(m.rcnn.bbox_pred.weight).normal_(0, 0.02, generator=g))
         m.mask_branch.mask_score.bias.fill_(0.2)
         m.fcn_head.score.weight.copy_(torch.empty_like(m.fcn_head.score.weight).normal_(0, 0.1, generator=g))
+        for mod in m.modules():     # group_norm configurations: non-trivial affines (nn.GroupNorm inits 1 and 0)
+            if isinstance(mod, torch.nn.GroupNorm):
+                mod.weight.copy_(torch.empty_like(mod.weight).uniform_(0.5, 1.5, generator=g))
+                mod.bias.copy_(torch.empty_like(mod.bias).normal_(0, 0.1, generator=g))
         if sum(depth) > 16:      # deeper than ResNet-50: keep the residual stream of the random-init stack bounded
             _calibrate_residual_growth(m, g)
         _calibrate_fpn_laterals(m, g)
@@ -124,6 +128,8 @@ def _calibrate_fpn_laterals(m, g):
         feats.append(t)
     for name, f in zip(("fpn_p2_1x1", "fpn_p3_1x1", "fpn_p4_1x1", "fpn_p5_1x1"), feats):
         conv = getattr(m.fpn, name)
+        if isinstance(conv, torch.nn.Sequential):     # group_norm: GN normalises the lateral's scale itself
+            continue
         rms = F.conv2d(f, cpu(conv.weight)).pow(2).mean().sqrt().item()
         conv.weight.mul_(1.0 / max(rms, 1e-6))
 

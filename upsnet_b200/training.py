@@ -380,6 +380,56 @@ def linear(x, weight, bias=None, relu=False, precision="bf16x3"):
     return y.reshape(R, weight.shape[0])
 
 
+class GroupNormFunction(torch.autograd.Function):
+    """y = act(GN(x) + shift + up2(residual)) (ops.group_norm on float32 NHWC) with device gradients
+    (upsnet_group_norm_backward): dx, d weight, d bias, d shift (float32 [N, C], the per-image d bias) and d residual,
+    only what needs_input_grad asks for."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, shift, residual, groups, eps, relu):
+        from . import operators as ops
+        require_cuda(x, weight, bias, shift, residual)
+        xs = ops._nhwc(x.detach().float())
+        y, stats = ops.group_norm(xs.permute(0, 3, 1, 2), weight.detach(), bias.detach(), groups, eps, relu,
+                                  None if residual is None else residual.detach().float(), residual is not None,
+                                  None if shift is None else shift.detach(), return_stats=True)
+        ctx.save_for_backward(xs, y if relu else None, stats, weight)
+        ctx.cfg = (groups, relu, residual is not None)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from . import operators as ops
+        xs, y, stats, weight = ctx.saved_tensors
+        groups, relu, has_res = ctx.cfg
+        ni = ctx.needs_input_grad
+        N, H, W, C = xs.shape
+        dev = xs.device
+        dy = ops._nhwc(grad_out.float())
+        dx = torch.empty_like(xs)
+        dgamma = torch.empty(C, dtype=torch.float32, device=dev) if ni[1] else None
+        dbeta = torch.empty(C, dtype=torch.float32, device=dev) if ni[2] else None
+        dshift = torch.empty((N, C), dtype=torch.float32, device=dev) if ni[3] else None
+        dres = torch.empty((N, H // 2, W // 2, C), dtype=torch.float32, device=dev) if (has_res and ni[4]) else None
+        nb = query_bytes("group_norm_backward_workspace_bytes", N, C, H, W, groups)
+        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        flags = (_lib.EPI_RELU if relu else 0) | (_lib.EPI_RES_UP2 if has_res else 0)
+        call("group_norm_backward", dev, dy, xs, None if y is None else y.permute(0, 2, 3, 1), stats, weight.detach(),
+             dx, dgamma, dbeta, dshift, dres, N, C, H, W, groups, flags, ws, nb)
+        return (dx.permute(0, 3, 1, 2), dgamma, dbeta, dshift, None if dres is None else dres.permute(0, 3, 1, 2),
+                None, None, None)
+
+
+def group_norm(x, weight, bias, groups=32, eps=1e-5, relu=False, residual=None, shift=None):
+    """Differentiable nn.GroupNorm(groups, C) with the fused epilogue of ops.group_norm: x float32 [N,C,H,W] (or [R,C],
+    normalised as [R,C,1,1], RCNN fc6); residual [N,C,H/2,W/2] added after nearest 2x up-sampling; shift [N,C].
+    -> float32 of x's logical shape, channels_last storage."""
+    if x.dim() == 2:
+        R, C = x.shape
+        return GroupNormFunction.apply(x.reshape(R, C, 1, 1), weight, bias, shift, residual, groups, eps, relu).reshape(R, C)
+    return GroupNormFunction.apply(x, weight, bias, shift, residual, groups, eps, relu)
+
+
 class ConvTranspose2x2Function(torch.autograd.Function):
     """ConvTranspose2d(k = 2, s = 2) (+ ReLU) as the 1x1 conv to 4 C channels ordered (a, b, c) that the engine runs
     (MaskBranch.prepare), followed by the pixel shuffle.  Backward reads dY through the 2x2 pixel-unshuffle of
