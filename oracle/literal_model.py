@@ -17,6 +17,11 @@ Reference lines restated (paths relative to /root/reference/upsnet/models/):
   fpn.py:78-104 FPN.forward            rpn.py:52-56 RPN.forward
   fcn.py:29-73 FCNSubNet, :88-108 FCNHead.forward
   rcnn.py:79-87 MaskBranch.forward, :132-146 RCNN.forward
+  with_norm 'group_norm' (network.{fpn,rcnn,fcn}_with_norm), GroupNorm(32) on each layer whose state_dict carries its
+  parameters (fpn.fpn_p5_1x1.{0,1}, fcn_head.fcn_subnet.conv.i.{0,1}, rcnn.fc6.{0,2}, mask_branch.mask_convN.{0,1}):
+    fpn.py:43-58 and :78-104 (conv without bias -> GroupNorm, the context vector added after the GN of fpn_p5_1x1)
+    fcn.py:41-52 (DeformConvWithOffset -> GroupNorm -> ReLU)
+    rcnn.py:50-56 (mask convs without bias -> GroupNorm -> ReLU), :102 (fc6: Linear -> view [R,C,1,1] -> GroupNorm -> ReLU)
   ../operators/modules/fpn_roi_align.py:32-62 FPNRoIAlign.forward (level = floor(2 + log2(sqrt(wh)/224 + 1e-6)) in float32)
   ../operators/modules/deform_conv.py:67-78 DeformConvWithOffset
 Custom CUDA ops are replaced by torchvision's operators of the same lineage (roi_align aligned=False, sampling_ratio 2;
@@ -52,6 +57,11 @@ class LiteralUPSNet:
     def dcn(self, x, offset, wname, padding=1, dilation=1):
         return torchvision.ops.deform_conv2d(x, offset, self.p[wname + ".weight"], self.p.get(wname + ".bias"),
                                              stride=1, padding=padding, dilation=dilation)
+
+    def gn(self, x, name):      # nn.GroupNorm(32, C) where the state_dict carries `name` (with_norm 'group_norm'), else x
+        if name + ".weight" not in self.p:
+            return x
+        return F.group_norm(x, 32, self.p[name + ".weight"], self.p[name + ".bias"], 1e-5)
 
     # ------------------------------------------------------------------ backbone
     def bottleneck(self, x, p, stride, dilation, deformable, has_down):
@@ -96,18 +106,24 @@ class LiteralUPSNet:
         return F.linear(F.adaptive_avg_pool2d(res5, (1, 1)).flatten(1), self.p["fpn.fpn_gap.weight"],
                         self.p["fpn.fpn_gap.bias"]).view(1, -1, 1, 1)
 
+    def fpn_conv(self, x, name, padding=0):
+        """An FPN conv; with group_norm the nn.Sequential of the conv without bias and its GroupNorm (fpn.py:47-54)."""
+        if name + ".1.weight" not in self.p:
+            return self.conv(x, name, 1, padding)
+        return self.gn(self.conv(x, name + ".0", 1, padding), name + ".1")
+
     def fpn(self, res2, res3, res4, res5):
         up = lambda t: F.interpolate(t, scale_factor=2, mode="nearest")     # noqa: E731
-        p5_1x1 = self.conv(res5, "fpn.fpn_p5_1x1")
+        p5_1x1 = self.fpn_conv(res5, "fpn.fpn_p5_1x1")
         if self.with_gap:
             p5_1x1 = p5_1x1 + self.gap(res5)
-        p4_plus = up(p5_1x1) + self.conv(res4, "fpn.fpn_p4_1x1")
-        p3_plus = up(p4_plus) + self.conv(res3, "fpn.fpn_p3_1x1")
-        p2_plus = up(p3_plus) + self.conv(res2, "fpn.fpn_p2_1x1")
-        p2 = self.conv(p2_plus, "fpn.fpn_p2", 1, 1)
-        p3 = self.conv(p3_plus, "fpn.fpn_p3", 1, 1)
-        p4 = self.conv(p4_plus, "fpn.fpn_p4", 1, 1)
-        p5 = self.conv(p5_1x1, "fpn.fpn_p5", 1, 1)
+        p4_plus = up(p5_1x1) + self.fpn_conv(res4, "fpn.fpn_p4_1x1")
+        p3_plus = up(p4_plus) + self.fpn_conv(res3, "fpn.fpn_p3_1x1")
+        p2_plus = up(p3_plus) + self.fpn_conv(res2, "fpn.fpn_p2_1x1")
+        p2 = self.fpn_conv(p2_plus, "fpn.fpn_p2", 1)
+        p3 = self.fpn_conv(p3_plus, "fpn.fpn_p3", 1)
+        p4 = self.fpn_conv(p4_plus, "fpn.fpn_p4", 1)
+        p5 = self.fpn_conv(p5_1x1, "fpn.fpn_p5", 1)
         p6 = F.max_pool2d(p5, 1, 2)
         return p2, p3, p4, p5, p6
 
@@ -121,9 +137,9 @@ class LiteralUPSNet:
     def fcn_level(self, x, level):
         """FCNSubNet on one FPN level; level 0 is P2."""
         for i in range(self.fcn_layers):
-            p = "fcn_head.fcn_subnet.conv.%d.0" % i
-            offset = self.conv(x, p + ".conv_offset", 1, 1, 1)
-            x = F.relu(self.dcn(x, offset, p + ".conv"))
+            p = "fcn_head.fcn_subnet.conv.%d" % i
+            offset = self.conv(x, p + ".0.conv_offset", 1, 1, 1)
+            x = F.relu(self.gn(self.dcn(x, offset, p + ".0.conv"), p + ".1"))
         return x
 
     def fcn_head(self, p2, p3, p4, p5, upsample_rate=4):
@@ -158,7 +174,10 @@ class LiteralUPSNet:
 
     def rcnn(self, feats, rois):
         x = self.fpn_roi_align(feats, rois, 7).flatten(1)
-        fc6 = F.relu(F.linear(x, self.p["rcnn.fc6.0.weight"], self.p["rcnn.fc6.0.bias"]))
+        fc6 = F.linear(x, self.p["rcnn.fc6.0.weight"], self.p["rcnn.fc6.0.bias"])
+        if "rcnn.fc6.2.weight" in self.p:
+            fc6 = self.gn(fc6.view(fc6.shape[0], -1, 1, 1), "rcnn.fc6.2").flatten(1)
+        fc6 = F.relu(fc6)
         fc7 = F.relu(F.linear(fc6, self.p["rcnn.fc7.0.weight"], self.p["rcnn.fc7.0.bias"]))
         return {"cls_score": F.linear(fc7, self.p["rcnn.cls_score.weight"], self.p["rcnn.cls_score.bias"]),
                 "bbox_pred": F.linear(fc7, self.p["rcnn.bbox_pred.weight"], self.p["rcnn.bbox_pred.bias"]), "fc_feat": fc7}
@@ -166,7 +185,7 @@ class LiteralUPSNet:
     def mask_branch(self, feats, rois):
         x = self.fpn_roi_align(feats, rois, 14)
         for i in range(1, 5):
-            x = F.relu(self.conv(x, "mask_branch.mask_conv%d.0" % i, 1, 1))
+            x = F.relu(self.gn(self.conv(x, "mask_branch.mask_conv%d.0" % i, 1, 1), "mask_branch.mask_conv%d.1" % i))
         x = F.relu(F.conv_transpose2d(x, self.p["mask_branch.mask_deconv1.0.weight"], self.p["mask_branch.mask_deconv1.0.bias"], 2))
         return self.conv(x, "mask_branch.mask_score")
 

@@ -15,7 +15,7 @@ Recorded for each norm option ('none', 'group_norm' on all four keys):
   groups are empty);
   gn_fpn_out<i> / gn_rpn_<k>: the group_norm FPN (with fpn_gap, fpn_feature_dim 64) on 8x16 inputs and the RPN on
   its P2, run on the CPU; inputs and parameters (gn_param_names / gn_param_shapes, in named_parameters order) are
-  not stored but defined by tests/gn_literal_model.py fixture_values / fixture_fpn_params.
+  not stored but defined by tests/train_forward_oracle.py fixture_values / fixture_fpn_params.
 
 Import shims (nothing inside the executed code is changed): those of make_reference_modules.py, plus stand-ins for
 the ROIAlign / deformable-conv autograd Functions (CUDA extensions; the constructors do not call them).
@@ -29,7 +29,8 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.dirname(HERE))                    # tests/: gn_literal_model
+sys.path.insert(0, os.path.dirname(HERE))                    # tests/: train_forward_oracle
+sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))   # the repository: oracle, upsnet_b200
 import make_reference_modules as MRM  # noqa: E402  (puts /root/reference first on sys.path)
 
 OUT = os.path.join(HERE, "reference_group_norm.npz")
@@ -110,19 +111,19 @@ def main():
         for i, g in enumerate(param_groups(heads)):
             out["%s_group%d" % (norm, i)] = np.array(g, dtype=str)
     # the group_norm FPN (with the context vector) and RPN, executed at a small size on inputs and parameters that
-    # gn_literal_model.fixture_values defines, so that only their names, shapes and the outputs are stored
-    import gn_literal_model as GL
+    # train_forward_oracle.fixture_values defines, so that only their names, shapes and the outputs are stored
+    import train_forward_oracle as TF
     torch.manual_seed(1)
     heads = build_heads("group_norm", with_gap=True, feature_dim=64)      # 64 channels: a small fixture
     shapes = [(n, tuple(p.shape)) for n, p in heads.named_parameters() if n.startswith(("fpn.", "rpn."))]
-    params = GL.fixture_fpn_params(shapes)
+    params = TF.fixture_fpn_params(shapes)
     out["gn_param_names"] = np.array([n for n, _ in shapes])
     out["gn_param_shapes"] = np.array([",".join(map(str, s_)) for _, s_ in shapes])
     with torch.no_grad():
         named = dict(heads.named_parameters())
         for n, v in params.items():
             named[n].copy_(v)
-        ins = [GL.fixture_values(l, (1, c, 8 >> l, 16 >> l), 4.0) for l, c in enumerate((256, 512, 1024, 2048))]
+        ins = [TF.fixture_values(l, (1, c, 8 >> l, 16 >> l), 4.0) for l, c in enumerate((256, 512, 1024, 2048))]
         fpn = heads.fpn(*ins)
         for l, t in enumerate(fpn):
             out["gn_fpn_out%d" % l] = t.numpy()

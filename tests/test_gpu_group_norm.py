@@ -3,7 +3,7 @@
 Kernels against float64 F.group_norm (and its autograd) at every GN layer shape of cityscapes_r50 (1024x2048) and
 coco_r50 (800x1344), in the three storage formats, with ReLU, the nearest-2x residual and the extra shift; byte
 repeatability and graph replay.  Whole-model inference with all norm keys 'group_norm' against the literal model
-extended by tests/gn_literal_model.py, graphs over mixed sizes, and the training forward against the float64 oracle."""
+(oracle/literal_model.py), graphs over mixed sizes, and the training forward against the float64 oracle."""
 import os
 import sys
 
@@ -14,8 +14,8 @@ import torch.nn.functional as F
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-import gn_literal_model as GL  # noqa: E402
 import train_forward_oracle as TF  # noqa: E402
+from oracle.literal_model import LiteralUPSNet  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda", 0)
@@ -251,9 +251,9 @@ def test_model_inference_vs_literal(name, H, W):
         U.set_precision("fp32")
         m.keep_intermediates = False
     it = out["_intermediates"]
-    lit = GL.LiteralGNUPSNet(m.state_dict(), depth=depth, num_classes=cfg.num_classes, num_seg_classes=cfg.num_seg_classes,
-                             dconv_from=cfg.backbone_with_dconv, fcn_layers=cfg.fcn_num_layers, with_gap=cfg.fpn_with_gap,
-                             dtype=torch.float64, device=DEV)
+    lit = LiteralUPSNet(m.state_dict(), depth=depth, num_classes=cfg.num_classes, num_seg_classes=cfg.num_seg_classes,
+                        dconv_from=cfg.backbone_with_dconv, fcn_layers=cfg.fcn_num_layers, with_gap=cfg.fpn_with_gap,
+                        dtype=torch.float64, device=DEV)
     d = lit.dense(inp["data"])
     errs = {"fpn_p%d" % (l + 2): rel(a, b) for l, (a, b) in enumerate(zip(it["fpn"], d["fpn"]))}
     for l in range(5):
@@ -363,7 +363,7 @@ def test_training_forward_vs_oracle(prec, with_gap):
     for k, p in m.named_parameters():
         assert (p.grad is not None) == (k in trainable), k
     sd = {k: v.detach() for k, v in m.state_dict().items()}
-    orc = GL.GNTrainOracle(sd, TF.trainable_names(m), depth=depth, with_gap=with_gap, dtype=torch.float64, device=DEV)
+    orc = TF.TrainOracle(sd, TF.trainable_names(m), depth=depth, with_gap=with_gap, dtype=torch.float64, device=DEV)
     want, wgrads = orc.step(data["data"], label, out["_intermediates"])
     named = dict(m.named_parameters())
     got = {k: named[k].grad for k in wgrads}

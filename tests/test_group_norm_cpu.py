@@ -10,8 +10,9 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-import gn_literal_model as GL  # noqa: E402
+import train_forward_oracle as TF  # noqa: E402
 
+from oracle.literal_model import LiteralUPSNet  # noqa: E402
 from upsnet_b200._lib import UpsnetError  # noqa: E402
 from upsnet_b200.model import UPSNetConfig, resnet_upsnet  # noqa: E402
 
@@ -84,8 +85,8 @@ def test_reference_style_load_accepts_a_group_norm_checkpoint():
 
 def test_literal_group_norm_fpn_and_rpn_match_the_reference():
     shapes = [(n, tuple(int(v) for v in s.split(","))) for n, s in zip(FIX["gn_param_names"], FIX["gn_param_shapes"])]
-    lit = GL.LiteralGNUPSNet(GL.fixture_fpn_params(shapes), with_gap=True, dtype=torch.float64)
-    ins = [GL.fixture_values(l, (1, c, 8 >> l, 16 >> l), 4.0).double() for l, c in enumerate((256, 512, 1024, 2048))]
+    lit = LiteralUPSNet(TF.fixture_fpn_params(shapes), with_gap=True, dtype=torch.float64)
+    ins = [TF.fixture_values(l, (1, c, 8 >> l, 16 >> l), 4.0).double() for l, c in enumerate((256, 512, 1024, 2048))]
     with torch.no_grad():
         out = lit.fpn(*ins)
         rpn = lit.rpn(out[0])

@@ -236,3 +236,23 @@ def synthetic_entry(seed, h, w, G, num_classes=9):
 def image(seed, h, w):
     g = torch.Generator().manual_seed(seed)
     return torch.randn(1, 3, h, w, generator=g) * 50
+
+
+def fixture_values(seed, shape, scale=1.0, offset=0.0):
+    """Deterministic float32 values, uniform in offset + scale * [-1/2, 1/2), defined by this code alone (splitmix64
+    keys of upsnet_b200.training.draw_keys, top 24 bits): the FPN / RPN inputs and parameters of
+    tests/golden/make_reference_group_norm.py, made again by the test instead of being stored in the fixture."""
+    from upsnet_b200.training import draw_keys
+    n = int(np.prod(shape))
+    u = (draw_keys(seed, n) >> np.uint64(40)).astype(np.float64) / 2.0 ** 24
+    return torch.from_numpy(((u - 0.5) * scale + offset).astype(np.float32).reshape(shape))
+
+
+def fixture_fpn_params(shapes):
+    """{name: tensor} for the (name, shape) list of the reference FPN / RPN parameters, in order: GroupNorm weights
+    around 1, other biases and GN biases around 0 (scale 0.4), weights at scale 0.1."""
+    out = {}
+    for i, (name, shape) in enumerate(shapes):
+        gn_w = name.endswith(".1.weight")
+        out[name] = fixture_values(1000 + i, shape, 0.4 if len(shape) == 1 else 0.1, 1.0 if gn_w else 0.0)
+    return out

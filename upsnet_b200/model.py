@@ -325,92 +325,65 @@ class FPN(nn.Module):
                 if m.bias is not None:
                     m.bias.data.zero_()
 
-    @staticmethod
-    def _c(m, x, residual=None, padding=0, up2=False):
-        return ops.conv2d(x, m.weight, m.bias, padding=padding, residual=residual, residual_up2=up2)
-
-    def _forward_gn(self, res2, res3, res4, res5):
-        """with_norm = 'group_norm': each conv without bias, then the GN apply with the rest of the reference's sum
-        fused in -- fpn_gap as the extra per-channel shift of P5's lateral, the nearest-2x top-down add as its residual."""
-        def c(name, x, padding=0, **kw):
+    def forward(self, res2, res3, res4, res5):
+        """Each lateral 1x1 ends in an epilogue that adds the nearest-2x-upsampled coarser level, so no upsampled tensor
+        is written: with 'none' the conv's, after its bias; with 'group_norm' the GN apply's, after a conv without bias.
+        The context vector fpn_gap(GAP(res5)) is the P5 lateral's GN shift, or with 'none' added to that conv's output."""
+        def step(name, x, padding=0, residual=None, shift=None):
+            up = {"residual": residual, "residual_up2": residual is not None}
+            if not self.gn:
+                m = getattr(self, name)
+                return ops.conv2d(x, m.weight, m.bias, padding=padding, **up)
             conv, gn = getattr(self, name)
             t = ops.conv2d(x, conv.weight, None, padding=padding)
-            return ops.group_norm(t, gn.weight, gn.bias, gn.num_groups, gn.eps, **kw)
-        shift = None
-        if hasattr(self, "fpn_gap"):
-            shift = ops.linear(res5.float().mean(dim=(2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, out_dtype=torch.float32)
-        p5_1x1 = c("fpn_p5_1x1", res5, shift=shift)
-        p4_plus = c("fpn_p4_1x1", res4, residual=p5_1x1, residual_up2=True)
-        p3_plus = c("fpn_p3_1x1", res3, residual=p4_plus, residual_up2=True)
-        p2_plus = c("fpn_p2_1x1", res2, residual=p3_plus, residual_up2=True)
-        p5 = c("fpn_p5", p5_1x1, padding=1)
-        p4 = c("fpn_p4", p4_plus, padding=1)
-        p3 = c("fpn_p3", p3_plus, padding=1)
-        p2 = c("fpn_p2", p2_plus, padding=1)
-        return p2, p3, p4, p5, ops.subsample2(p5)
+            return ops.group_norm(t, gn.weight, gn.bias, gn.num_groups, gn.eps, shift=shift, **up)
 
-    def forward(self, res2, res3, res4, res5):
-        if self.gn:
-            return self._forward_gn(res2, res3, res4, res5)
-        p5_1x1 = self._c(self.fpn_p5_1x1, res5)
-        if hasattr(self, "fpn_gap"):
-            gap = ops.linear(res5.float().mean(dim=(2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, out_dtype=torch.float32)
+        def gap():          # models/fpn.py:84-86, float32 [N, C]; launched where each norm consumes it
+            return ops.linear(res5.float().mean(dim=(2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, out_dtype=torch.float32)
+        with_gap = hasattr(self, "fpn_gap")
+        p5_1x1 = step("fpn_p5_1x1", res5, shift=gap() if with_gap and self.gn else None)
+        if with_gap and not self.gn:
+            g = gap().view(-1, self.feature_dim, 1, 1)
             if isinstance(p5_1x1, ops.Pair):
-                p5_1x1 = ops.Pair.from_float(p5_1x1.float() + gap.view(-1, self.feature_dim, 1, 1))
+                p5_1x1 = ops.Pair.from_float(p5_1x1.float() + g)
             else:
-                p5_1x1 = p5_1x1 + gap.view(-1, self.feature_dim, 1, 1).to(p5_1x1.dtype)
-        # lateral 1x1 + nearest-2x-upsampled coarser level, fused into the conv epilogue (no upsampled tensor)
-        p4_plus = self._c(self.fpn_p4_1x1, res4, residual=p5_1x1, up2=True)
-        p3_plus = self._c(self.fpn_p3_1x1, res3, residual=p4_plus, up2=True)
-        p2_plus = self._c(self.fpn_p2_1x1, res2, residual=p3_plus, up2=True)
-        p5 = self._c(self.fpn_p5, p5_1x1, padding=1)
-        p4 = self._c(self.fpn_p4, p4_plus, padding=1)
-        p3 = self._c(self.fpn_p3, p3_plus, padding=1)
-        p2 = self._c(self.fpn_p2, p2_plus, padding=1)
+                p5_1x1 = p5_1x1 + g.to(p5_1x1.dtype)
+        p4_plus = step("fpn_p4_1x1", res4, residual=p5_1x1)
+        p3_plus = step("fpn_p3_1x1", res3, residual=p4_plus)
+        p2_plus = step("fpn_p2_1x1", res2, residual=p3_plus)
+        p5 = step("fpn_p5", p5_1x1, padding=1)
+        p4 = step("fpn_p4", p4_plus, padding=1)
+        p3 = step("fpn_p3", p3_plus, padding=1)
+        p2 = step("fpn_p2", p2_plus, padding=1)
         p6 = ops.subsample2(p5)                                         # MaxPool2d(kernel 1, stride 2)
         return p2, p3, p4, p5, p6
 
     def forward_train(self, res2, res3, res4, res5, prec):
-        """forward with device gradients (training.conv2d, the same fused top-down add).  With fpn_gap, the context
-        vector fpn_gap(GAP(res5)) (models/fpn.py:84-86, added to every P5 lateral pixel) is folded into the bias of the
-        P5 lateral conv, so that conv's d bias carries the gradient to both biases, fpn_gap and res5."""
-        if self.gn:
-            return self._forward_train_gn(res2, res3, res4, res5, prec)
-
-        def c(m, x, bias=None, **kw):
-            return training.conv2d(x, m.weight, m.bias if bias is None else bias, precision=prec, **kw)
-        p5_bias = None
-        if hasattr(self, "fpn_gap"):        # one image: the context vector is one row
-            gap = training.linear(res5.mean((2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, precision=prec)
-            p5_bias = self.fpn_p5_1x1.bias + gap.reshape(self.feature_dim)
-        p5_1x1 = c(self.fpn_p5_1x1, res5, p5_bias)
-        p4_plus = c(self.fpn_p4_1x1, res4, residual=p5_1x1, residual_up2=True)
-        p3_plus = c(self.fpn_p3_1x1, res3, residual=p4_plus, residual_up2=True)
-        p2_plus = c(self.fpn_p2_1x1, res2, residual=p3_plus, residual_up2=True)
-        p2 = c(self.fpn_p2, p2_plus, padding=1)
-        p3 = c(self.fpn_p3, p3_plus, padding=1)
-        p4 = c(self.fpn_p4, p4_plus, padding=1)
-        p5 = c(self.fpn_p5, p5_1x1, padding=1)
-        return p2, p3, p4, p5, p5[:, :, ::2, ::2]
-
-    def _forward_train_gn(self, res2, res3, res4, res5, prec):
-        """forward_train with group_norm: training.conv2d without bias, then training.group_norm with the top-down add
-        and the context vector as its residual and shift, so their gradients leave the GN backward."""
-        def c(name, x, padding=0, residual=None, shift=None):
+        """forward with device gradients: training.conv2d, then with group_norm training.group_norm, with the same fused
+        top-down add.  The context vector fpn_gap(GAP(res5)) (models/fpn.py:84-86, added to every P5 lateral pixel) is,
+        with 'none', folded into the bias of the P5 lateral conv, so that conv's d bias carries the gradient to both
+        biases, fpn_gap and res5; with 'group_norm' it is the GN apply's shift, whose gradient the GN backward returns."""
+        def step(name, x, padding=0, residual=None, shift=None):
+            if not self.gn:
+                m = getattr(self, name)
+                bias = m.bias if shift is None else m.bias + shift.reshape(self.feature_dim)
+                return training.conv2d(x, m.weight, bias, padding=padding, residual=residual,
+                                       residual_up2=residual is not None, precision=prec)
             conv, gn = getattr(self, name)
             t = training.conv2d(x, conv.weight, None, padding=padding, precision=prec)
             return training.group_norm(t, gn.weight, gn.bias, gn.num_groups, gn.eps, residual=residual, shift=shift)
-        shift = None
+
+        gap = None
         if hasattr(self, "fpn_gap"):        # one image: the context vector is one row
-            shift = training.linear(res5.mean((2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, precision=prec)
-        p5_1x1 = c("fpn_p5_1x1", res5, shift=shift)
-        p4_plus = c("fpn_p4_1x1", res4, residual=p5_1x1)
-        p3_plus = c("fpn_p3_1x1", res3, residual=p4_plus)
-        p2_plus = c("fpn_p2_1x1", res2, residual=p3_plus)
-        p2 = c("fpn_p2", p2_plus, padding=1)
-        p3 = c("fpn_p3", p3_plus, padding=1)
-        p4 = c("fpn_p4", p4_plus, padding=1)
-        p5 = c("fpn_p5", p5_1x1, padding=1)
+            gap = training.linear(res5.mean((2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, precision=prec)
+        p5_1x1 = step("fpn_p5_1x1", res5, shift=gap)
+        p4_plus = step("fpn_p4_1x1", res4, residual=p5_1x1)
+        p3_plus = step("fpn_p3_1x1", res3, residual=p4_plus)
+        p2_plus = step("fpn_p2_1x1", res2, residual=p3_plus)
+        p2 = step("fpn_p2", p2_plus, padding=1)
+        p3 = step("fpn_p3", p3_plus, padding=1)
+        p4 = step("fpn_p4", p4_plus, padding=1)
+        p5 = step("fpn_p5", p5_1x1, padding=1)
         return p2, p3, p4, p5, p5[:, :, ::2, ::2]
 
 
