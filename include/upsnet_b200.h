@@ -40,6 +40,9 @@ extern "C" {
 #define UPSNET_EPI_RES_UP2 2 /* upsnet_igemm_forward only: residual is [N,Ho/2,Wo/2,Cout], read with nearest 2x upsampling */
 #define UPSNET_EPI_STEM_PAIR 8 /* upsnet_stem_forward only: y is a hi/lo pair tensor [N,Ho,Wo,2*Cout] (precision bf16x3) */
 #define UPSNET_EPI_NO_TMA 4  /* upsnet_igemm_forward only: use the cp.async gather kernel even where the TMA-fed one qualifies */
+/* upsnet_group_norm_forward / _backward only, together with UPSNET_EPI_RES_UP2: the half-resolution residual is read
+ * with bilinear 2x up-sampling (align_corners = False, as upsnet_upsample2_bilinear_nhwc) instead of nearest */
+#define UPSNET_EPI_RES_BILINEAR 16
 /* upsnet_igemm_forward, y_dtype PAIR only: store the output channels as [hi G][lo G] per group of G channels instead of
  * [hi Cout][lo Cout] (G % 64 == 0, Cout % G == 0; 0 = Cout).  Lets a 1x1 conv that emulates a 2x2 deconvolution write
  * its four (a,b) sub-pixel groups as four pair pixels (models/rcnn.py:62 mask_deconv1). */
@@ -274,6 +277,21 @@ int upsnet_fcn_score_fuse(const float *s2, const float *s3, const float *s4, con
  * H % 8 == W % 8 == 0 and planes <= 65535, else UPSNET_E_UNSUPPORTED. */
 int upsnet_fcn_score_fuse_backward(const float *dscore, float *ds3, float *ds4, float *ds5, int planes, int H,
                                    int W, void *stream);
+
+/* FPN top-down bilinear 2x up-sampling on NHWC activations (csrc/upsample2.cu), align_corners = False: the rule of
+ * upsnet_upsample_bilinear_nchw with factor 2 (source index (dst + 0.5)/2 - 0.5 clamped at 0, the last row / column
+ * repeated; any h, w, odd ones included).
+ * replaces: models/fpn.py:27-35 fpn_upsample with network.fpn_upsample_method = 'bilinear', applied at :88-93.
+ * x [N,h,w,C] -> y [N,2h,2w,C] in dtype (F32, BF16, or PAIR: [N,h,w,2C] -> [N,2h,2w,2C]); interpolated in fp32 (a
+ * pair's value is hi + lo) and rounded once to dtype.  C % 8 == 0 and 16-byte aligned x, y, else UPSNET_E_UNSUPPORTED.
+ *
+ * upsnet_upsample2_bilinear_nhwc_adjoint: dx = up2^T(dy), fp32 NHWC dy [N,2h,2w,C] -> dx [N,h,w,C], every element
+ * written.  A gather (each coarse pixel sums its 4x4 fine footprint with the forward's weights, along x then y, in a
+ * fixed order), no atomics: the same input gives the same bytes; capturable.  C % 4 == 0 and 16-byte aligned dy, dx,
+ * else UPSNET_E_UNSUPPORTED.
+ * replaces: autograd of that F.interpolate. */
+int upsnet_upsample2_bilinear_nhwc(const void *x, void *y, int N, int h, int w, int C, int dtype, void *stream);
+int upsnet_upsample2_bilinear_nhwc_adjoint(const float *dy, float *dx, int N, int h, int w, int C, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * Detection glue, fused (device-resident; nothing returns to the host).
@@ -979,7 +997,8 @@ int upsnet_conv_wgrad(const void *x_nhwc, const void *g, float *dw, int N, int H
  * all H*W pixels of an image.  Three launches: per-(image, group, CTA) partial (count, mean, M2), their merge by Chan's
  * formula into stats[N][groups][2] = (mean, 1/sqrt(var + eps)) (fp32, caller-owned, read by the backward), and the
  * apply.  shift (fp32 [N][C] or NULL) is added after beta; flags: UPSNET_EPI_RELU; UPSNET_EPI_RES_UP2 with residual
- * [N,H/2,W/2,C] in dtype, read with nearest 2x up-sampling and added before the ReLU (H, W even).  C <= 1024 with
+ * [N,H/2,W/2,C] in dtype, read with nearest 2x up-sampling -- or, adding UPSNET_EPI_RES_BILINEAR, with the four
+ * bilinear taps of upsnet_upsample2_bilinear_nhwc -- and added before the ReLU (H, W even).  C <= 1024 with
  * min(C, 256) dividing both 256 and C, else UPSNET_E_UNSUPPORTED.  Workspace: upsnet_group_norm_workspace_bytes.
  *
  * upsnet_group_norm_rows: R rows of HW pixels x C channels (NHWC, dtype as above), each row normalised on its own (the
@@ -988,8 +1007,9 @@ int upsnet_conv_wgrad(const void *x_nhwc, const void *g, float *dw, int N, int H
  *
  * upsnet_group_norm_backward: gradients of y = act(GN(x) + shift [+ up2(residual)]), fp32 NHWC.  dy, x, dx [N,H,W,C];
  * y the forward output (read for the ReLU mask; pass it iff flags has UPSNET_EPI_RELU); stats from the forward.
- * dgamma, dbeta [C], dshift [N][C] (= per-image dbeta) and dres [N,H/2,W/2,C] (needs UPSNET_EPI_RES_UP2) are each
- * optional.  Workspace: upsnet_group_norm_backward_workspace_bytes. */
+ * dgamma, dbeta [C], dshift [N][C] (= per-image dbeta) and dres [N,H/2,W/2,C] (needs UPSNET_EPI_RES_UP2; with
+ * UPSNET_EPI_RES_BILINEAR too it is the bilinear adjoint of the masked dy, as upsnet_upsample2_bilinear_nhwc_adjoint,
+ * which needs C % 4 == 0) are each optional.  Workspace: upsnet_group_norm_backward_workspace_bytes. */
 int upsnet_group_norm_workspace_bytes(int N, int C, int H, int W, int groups, size_t *bytes);
 int upsnet_group_norm_forward(const void *x, const float *gamma, const float *beta, const float *shift,
                               const void *residual, void *y, float *stats, int N, int C, int H, int W, int groups,

@@ -20,6 +20,7 @@ EPI_RELU = 1
 EPI_RES_UP2 = 2
 EPI_NO_TMA = 4
 EPI_STEM_PAIR = 8
+EPI_RES_BILINEAR = 16
 
 
 def EPI_SIGMOID_FROM(c):

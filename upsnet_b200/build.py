@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libupsnet_b200.so")
-SOURCES = ["roi_align.cu", "nms.cu", "panoptic.cu", "igemm_simt.cu", "igemm_tc.cu", "igemm_tma.cu", "dcn_win.cu", "detection.cu", "pool.cu", "post.cu", "impost.cu", "pq.cu", "sseg.cu", "cocoeval.cu", "gt_rle.cu", "combined.cu", "rpn_target.cu", "proposal_target.cu", "panoptic_loss.cu", "train_loss.cu", "labels.cu", "backward.cu", "conv_backward.cu", "sgd.cu", "group_norm.cu", "capi.cu"]
+SOURCES = ["roi_align.cu", "nms.cu", "panoptic.cu", "igemm_simt.cu", "igemm_tc.cu", "igemm_tma.cu", "dcn_win.cu", "detection.cu", "pool.cu", "post.cu", "impost.cu", "pq.cu", "sseg.cu", "cocoeval.cu", "gt_rle.cu", "combined.cu", "rpn_target.cu", "proposal_target.cu", "panoptic_loss.cu", "train_loss.cu", "labels.cu", "backward.cu", "conv_backward.cu", "sgd.cu", "group_norm.cu", "upsample2.cu", "capi.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

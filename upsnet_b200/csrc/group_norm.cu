@@ -11,6 +11,7 @@
 // a warp reads consecutive channels.
 #include <math.h>
 
+#include "bilin.cuh"
 #include "common.cuh"
 #include "pair.cuh"
 
@@ -146,7 +147,10 @@ __global__ void gn_finalize_kernel(const float* __restrict__ part, int nparts, i
   }
 }
 
-// Phase 2: y = (x - mean) rstd gamma + beta [+ shift[n]] [+ up2(residual)] [ReLU], written in y's format.
+// Phase 2: y = (x - mean) rstd gamma + beta [+ shift[n]] [+ up2(residual)] [ReLU], written in y's format.  up2 is
+// nearest, or with UPSNET_EPI_RES_BILINEAR (BIL) the four taps of bilin.cuh's rule blended in fp32.  BIL is a template
+// argument so that the nearest instantiation keeps its registers.
+template <bool BIL>
 __global__ void __launch_bounds__(kGnThreads)
 gn_apply_kernel(const void* __restrict__ x, const float* __restrict__ stats, const float* __restrict__ gamma,
                 const float* __restrict__ beta, const float* __restrict__ shift, const void* __restrict__ res,
@@ -154,8 +158,8 @@ gn_apply_kernel(const void* __restrict__ x, const float* __restrict__ stats, con
   const int n = blockIdx.y, t = threadIdx.x;
   const int c0 = t % gm.TC, sub = t / gm.TC;
   const int cg = gm.C / gm.groups;
-  const bool relu = flags & UPSNET_EPI_RELU, up2 = res != nullptr;
-  const int Wr = gm.W / 2, HWr = (gm.HW / gm.W / 2) * Wr;
+  const bool relu = flags & UPSNET_EPI_RELU, up2 = res != nullptr, bil = BIL && up2;
+  const int Wr = gm.W / 2, Hr = gm.HW / gm.W / 2, HWr = Hr * Wr;
   float mean[kGnMaxJ], a[kGnMaxJ], b[kGnMaxJ];
 #pragma unroll
   for (int j = 0; j < kGnMaxJ; ++j) {
@@ -169,14 +173,28 @@ gn_apply_kernel(const void* __restrict__ x, const float* __restrict__ stats, con
     const int p1 = min(ch * kGnChunk + kGnChunk, gm.HW);
     for (int p = ch * kGnChunk + sub; p < p1; p += gm.SUB) {
       const size_t pix = (size_t)n * gm.HW + p;
-      size_t rpix = 0;
-      if (up2) rpix = (size_t)n * HWr + (size_t)(p / gm.W / 2) * Wr + (p % gm.W) / 2;
+      size_t rpix = 0, r00 = 0, r01 = 0, r10 = 0, r11 = 0;
+      BilinAxis ay, ax;
+      if (bil) {
+        ay = bilin_axis(p / gm.W, Hr, 2);
+        ax = bilin_axis(p % gm.W, Wr, 2);
+        r00 = (size_t)n * HWr + (size_t)ay.i0 * Wr + ax.i0;
+        r01 = (size_t)n * HWr + (size_t)ay.i0 * Wr + ax.i1;
+        r10 = (size_t)n * HWr + (size_t)ay.i1 * Wr + ax.i0;
+        r11 = (size_t)n * HWr + (size_t)ay.i1 * Wr + ax.i1;
+      } else if (up2) {
+        rpix = (size_t)n * HWr + (size_t)(p / gm.W / 2) * Wr + (p % gm.W) / 2;
+      }
 #pragma unroll
       for (int j = 0; j < kGnMaxJ; ++j) {
         if (j >= gm.J) break;
         const int c = c0 + j * gm.TC;
         float v = (load_elem(x, dtype, pix, gm.C, c) - mean[j]) * a[j] + b[j];
-        if (up2) v += load_elem(res, dtype, rpix, gm.C, c);
+        if (bil)
+          v += bilin_mix(ay, ax, load_elem(res, dtype, r00, gm.C, c), load_elem(res, dtype, r01, gm.C, c),
+                         load_elem(res, dtype, r10, gm.C, c), load_elem(res, dtype, r11, gm.C, c));
+        else if (up2)
+          v += load_elem(res, dtype, rpix, gm.C, c);
         if (relu) v = fmaxf(v, 0.f);
         store_elem(y, dtype, pix, gm.C, c, v);
       }
@@ -402,6 +420,7 @@ extern "C" int upsnet_group_norm_forward(const void* x, const float* gamma, cons
   if (dtype != UPSNET_DTYPE_F32 && dtype != UPSNET_DTYPE_BF16 && dtype != UPSNET_DTYPE_PAIR) return UPSNET_E_BADARG;
   if (!map_ok(N, C, H, W, groups)) return UPSNET_E_UNSUPPORTED;
   if (((flags & UPSNET_EPI_RES_UP2) != 0) != (residual != nullptr)) return UPSNET_E_BADARG;
+  if ((flags & UPSNET_EPI_RES_BILINEAR) && !residual) return UPSNET_E_BADARG;
   if (residual && (H % 2 || W % 2)) return UPSNET_E_UNSUPPORTED;
   size_t need = 0;
   upsnet_group_norm_workspace_bytes(N, C, H, W, groups, &need);
@@ -416,7 +435,10 @@ extern "C" int upsnet_group_norm_forward(const void* x, const float* gamma, cons
   gn_finalize_kernel<<<ceil_div(total, 8), 256, 0, s>>>(part, nb, total, eps, stats);
   UPS_CHECK_LAUNCH();
   const int na = ceil_div(2 * num_sms() * 4, N) < gm.nchunks ? ceil_div(2 * num_sms() * 4, N) : gm.nchunks;
-  gn_apply_kernel<<<dim3(na, N), kGnThreads, 0, s>>>(x, stats, gamma, beta, shift, residual, y, dtype, gm, flags);
+  if (residual && (flags & UPSNET_EPI_RES_BILINEAR))
+    gn_apply_kernel<true><<<dim3(na, N), kGnThreads, 0, s>>>(x, stats, gamma, beta, shift, residual, y, dtype, gm, flags);
+  else
+    gn_apply_kernel<false><<<dim3(na, N), kGnThreads, 0, s>>>(x, stats, gamma, beta, shift, residual, y, dtype, gm, flags);
   UPS_CHECK_LAUNCH();
   return 0;
 }
@@ -455,8 +477,12 @@ extern "C" int upsnet_group_norm_backward(const float* dy, const float* x, const
   if (!dy || !x || !stats || !gamma || !dx || !workspace) return UPSNET_E_BADARG;
   if (((flags & UPSNET_EPI_RELU) != 0) != (y != nullptr)) return UPSNET_E_BADARG;
   if (dres && !(flags & UPSNET_EPI_RES_UP2)) return UPSNET_E_BADARG;
+  const bool bil = flags & UPSNET_EPI_RES_BILINEAR;
+  if (bil && !(flags & UPSNET_EPI_RES_UP2)) return UPSNET_E_BADARG;
   if (!map_ok(N, C, H, W, groups)) return UPSNET_E_UNSUPPORTED;
   if (dres && (H % 2 || W % 2)) return UPSNET_E_UNSUPPORTED;
+  if (dres && bil && (C % 4 || (((uintptr_t)dy) & 15) || (((uintptr_t)dres) & 15) || (((uintptr_t)y) & 15)))
+    return UPSNET_E_UNSUPPORTED;
   size_t need = 0;
   upsnet_group_norm_backward_workspace_bytes(N, C, H, W, groups, &need);
   if (workspace_bytes < need) return UPSNET_E_WORKSPACE;
@@ -476,6 +502,7 @@ extern "C" int upsnet_group_norm_backward(const float* dy, const float* x, const
   }
   gn_bwd_dx_kernel<<<dim3(nb, N), kGnThreads, 0, s>>>(dy, x, y, stats, coef, gamma, gm, dx);
   UPS_CHECK_LAUNCH();
+  if (dres && bil) return up2_bilinear_adjoint_launch(dy, y, dres, N, H / 2, W / 2, C, s);
   if (dres) {
     const size_t total = (size_t)N * (H / 2) * (W / 2) * C;
     const size_t blocks = (total + 255) / 256 < 65535 ? (total + 255) / 256 : 65535;

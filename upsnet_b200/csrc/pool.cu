@@ -5,6 +5,7 @@
 #include <cuda_bf16.h>
 #include <cfloat>
 
+#include "bilin.cuh"
 #include "common.cuh"
 #include "pair.cuh"
 #include "up4.cuh"
@@ -164,17 +165,6 @@ upsample_bilinear_nchw_kernel(const float* __restrict__ x, float* __restrict__ y
 // bilinear up-sampling, models/fcn.py:94-101) summed at P2 resolution in one pass, same bilinear rule and the same order
 // of the three additions as the torch expression it replaces (F.interpolate + add, three times).
 namespace ups {
-__device__ __forceinline__ float bilin_at(const float* __restrict__ pl, int H, int W, int f, int yo, int xo) {
-  const float rf = 1.0f / (float)f;
-  const float sy = fmaxf(rf * ((float)yo + 0.5f) - 0.5f, 0.f), sx = fmaxf(rf * ((float)xo + 0.5f) - 0.5f, 0.f);
-  const int y0 = (int)sy, x0 = (int)sx;
-  const int y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
-  const float ly = sy - (float)y0, lx = sx - (float)x0, hy = 1.f - ly, hx = 1.f - lx;
-  const float* r0 = pl + (size_t)y0 * W;
-  const float* r1 = pl + (size_t)y1 * W;
-  return hy * (hx * __ldg(r0 + x0) + lx * __ldg(r0 + x1)) + ly * (hx * __ldg(r1 + x0) + lx * __ldg(r1 + x1));
-}
-
 __global__ void __launch_bounds__(256)
 fcn_score_fuse_kernel(const float* __restrict__ s2, const float* __restrict__ s3, const float* __restrict__ s4,
                       const float* __restrict__ s5, float* __restrict__ out, int P, int H, int W) {
@@ -213,14 +203,6 @@ extern "C" int upsnet_fcn_score_fuse(const float* s2, const float* s3, const flo
 namespace ups {
 constexpr int kFbTx = 32, kFbTy = 8, kFbThreads = kFbTx * kFbTy;
 constexpr int kFbRows = 8 * kFbTy + 8;       // output rows of the x8 footprint of one tile, the largest
-
-// weight of source sample s in output coordinate o (n source samples, factor f), exactly as bilin_at forms it
-__device__ __forceinline__ float bilin_tap(int o, int s, int n, int f) {
-  const float src = fmaxf((1.0f / (float)f) * ((float)o + 0.5f) - 0.5f, 0.f);
-  const int i0 = (int)src, i1 = i0 + (i0 < n - 1 ? 1 : 0);
-  const float l = src - (float)i0;
-  return (i0 == s ? 1.f - l : 0.f) + (i1 == s ? l : 0.f);
-}
 
 __global__ void __launch_bounds__(kFbThreads)
 fcn_score_fuse_backward_kernel(const float* __restrict__ g, float* __restrict__ d3, float* __restrict__ d4,

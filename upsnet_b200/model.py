@@ -77,6 +77,9 @@ class UPSNetConfig:
         self.rpn_with_norm = "none"
         self.rcnn_with_norm = "none"
         self.fcn_with_norm = "none"
+        # network.fpn_upsample_method: how the FPN's top-down path up-samples the coarser level, 'nearest' or 'bilinear'
+        # (F.interpolate(scale_factor=2, align_corners=False), models/fpn.py:27-35)
+        self.fpn_upsample_method = "nearest"
         for k, v in kw.items():
             if not hasattr(self, k):
                 raise AttributeError(k)
@@ -115,6 +118,7 @@ class UPSNetConfig:
                    batch_rois=int(get("train", "batch_rois", 512)), rpn_batch_size=int(get("train", "rpn_batch_size", 256)),
                    fg_fraction=float(get("train", "fg_fraction", 0.25)),
                    fcn_with_roi_loss=bool(get("train", "fcn_with_roi_loss", False)),
+                   fpn_upsample_method=str(get("network", "fpn_upsample_method", "nearest")),
                    **{k: str(get("network", k, "none")) for k in NORM_KEYS})
 
     @classmethod
@@ -145,6 +149,13 @@ def _check_norms(cfg):
         if v == "batch_norm" and k != "rpn_with_norm":
             raise _lib.UpsnetError("network.%s = 'batch_norm' is not built: the reference's BatchNorm2d comes from its "
                                    "absent distbatchnorm module (SyncBN); use 'group_norm' or 'none'" % k)
+
+
+def _check_fpn_upsample(cfg):
+    """The reference's FPN asserts upsample_method in ['nearest', 'bilinear'] (models/fpn.py:31)."""
+    if cfg.fpn_upsample_method not in ("nearest", "bilinear"):
+        raise _lib.UpsnetError("network.fpn_upsample_method: %r is not one of 'nearest', 'bilinear'"
+                               % (cfg.fpn_upsample_method,))
 
 
 def _gn_conv(cin, cout, k, padding=0):
@@ -306,12 +317,14 @@ class ResNetBackbone(nn.Module):
 # FPN / RPN / heads (models/fpn.py, rpn.py, rcnn.py, fcn.py)
 # ---------------------------------------------------------------------------------------------
 class FPN(nn.Module):
-    """models/fpn.py:25-104 (with_norm 'none' or 'group_norm', nearest upsampling, P6 = stride-2 subsample of P5)."""
+    """models/fpn.py:25-104 (with_norm 'none' or 'group_norm', upsample_method 'nearest' or 'bilinear', P6 = stride-2
+    subsample of P5).  The up-sampling method has no parameters: both build the same module tree."""
 
-    def __init__(self, feature_dim, with_gap, with_norm="none"):
+    def __init__(self, feature_dim, with_gap, with_norm="none", upsample_method="nearest"):
         super().__init__()
         self.feature_dim = feature_dim
         self.gn = with_norm == "group_norm"
+        self.upsample_method = upsample_method
         if with_gap:
             self.fpn_gap = nn.Linear(2048, feature_dim)
         for name, cin in (("fpn_p5_1x1", 2048), ("fpn_p4_1x1", 1024), ("fpn_p3_1x1", 512), ("fpn_p2_1x1", 256)):
@@ -326,17 +339,25 @@ class FPN(nn.Module):
                     m.bias.data.zero_()
 
     def forward(self, res2, res3, res4, res5):
-        """Each lateral 1x1 ends in an epilogue that adds the nearest-2x-upsampled coarser level, so no upsampled tensor
-        is written: with 'none' the conv's, after its bias; with 'group_norm' the GN apply's, after a conv without bias.
-        The context vector fpn_gap(GAP(res5)) is the P5 lateral's GN shift, or with 'none' added to that conv's output."""
+        """Each lateral 1x1 ends in an epilogue that adds the 2x-upsampled coarser level: with 'none' the conv's, after
+        its bias; with 'group_norm' the GN apply's, after a conv without bias.  With 'nearest' both epilogues read the
+        coarser level directly, so no upsampled tensor is written; with 'bilinear' the GN apply reads its four bilinear
+        taps, and with 'none' the up-sampling kernel writes the upsampled map, which the conv adds as a plain residual.
+        The context vector fpn_gap(GAP(res5)) is the P5 lateral's GN shift, or with 'none' added to that conv's output;
+        either way it is in P5's lateral before that is up-sampled (models/fpn.py:84-88)."""
+        bilinear = self.upsample_method == "bilinear"
+
         def step(name, x, padding=0, residual=None, shift=None):
             up = {"residual": residual, "residual_up2": residual is not None}
             if not self.gn:
                 m = getattr(self, name)
+                if bilinear and residual is not None:
+                    up = {"residual": ops.upsample2_bilinear(residual)}
                 return ops.conv2d(x, m.weight, m.bias, padding=padding, **up)
             conv, gn = getattr(self, name)
             t = ops.conv2d(x, conv.weight, None, padding=padding)
-            return ops.group_norm(t, gn.weight, gn.bias, gn.num_groups, gn.eps, shift=shift, **up)
+            return ops.group_norm(t, gn.weight, gn.bias, gn.num_groups, gn.eps, shift=shift,
+                                  upsample=self.upsample_method, **up)
 
         def gap():          # models/fpn.py:84-86, float32 [N, C]; launched where each norm consumes it
             return ops.linear(res5.float().mean(dim=(2, 3)), self.fpn_gap.weight, self.fpn_gap.bias, out_dtype=torch.float32)
@@ -360,18 +381,26 @@ class FPN(nn.Module):
 
     def forward_train(self, res2, res3, res4, res5, prec):
         """forward with device gradients: training.conv2d, then with group_norm training.group_norm, with the same fused
-        top-down add.  The context vector fpn_gap(GAP(res5)) (models/fpn.py:84-86, added to every P5 lateral pixel) is,
-        with 'none', folded into the bias of the P5 lateral conv, so that conv's d bias carries the gradient to both
-        biases, fpn_gap and res5; with 'group_norm' it is the GN apply's shift, whose gradient the GN backward returns."""
+        top-down add ('bilinear' with 'none': training.upsample2_bilinear, whose backward is the adjoint kernel, then
+        the plain residual).  The context vector fpn_gap(GAP(res5)) (models/fpn.py:84-86, added to every P5 lateral
+        pixel) is, with 'none', folded into the bias of the P5 lateral conv, so that conv's d bias carries the gradient
+        to both biases, fpn_gap and res5; with 'group_norm' it is the GN apply's shift, whose gradient the GN backward
+        returns."""
+        bilinear = self.upsample_method == "bilinear"
+
         def step(name, x, padding=0, residual=None, shift=None):
             if not self.gn:
                 m = getattr(self, name)
                 bias = m.bias if shift is None else m.bias + shift.reshape(self.feature_dim)
+                if bilinear and residual is not None:
+                    return training.conv2d(x, m.weight, bias, padding=padding,
+                                           residual=training.upsample2_bilinear(residual), precision=prec)
                 return training.conv2d(x, m.weight, bias, padding=padding, residual=residual,
                                        residual_up2=residual is not None, precision=prec)
             conv, gn = getattr(self, name)
             t = training.conv2d(x, conv.weight, None, padding=padding, precision=prec)
-            return training.group_norm(t, gn.weight, gn.bias, gn.num_groups, gn.eps, residual=residual, shift=shift)
+            return training.group_norm(t, gn.weight, gn.bias, gn.num_groups, gn.eps, residual=residual, shift=shift,
+                                       upsample=self.upsample_method)
 
         gap = None
         if hasattr(self, "fpn_gap"):        # one image: the context vector is one row
@@ -729,8 +758,9 @@ class resnet_upsnet(nn.Module):
         self.num_classes, self.num_seg_classes = cfg.num_classes, cfg.num_seg_classes
         self.num_reg_classes = cfg.num_classes
         _check_norms(cfg)
+        _check_fpn_upsample(cfg)
         self.resnet_backbone = ResNetBackbone(backbone_depth, cfg)
-        self.fpn = FPN(cfg.fpn_feature_dim, cfg.fpn_with_gap, cfg.fpn_with_norm)
+        self.fpn = FPN(cfg.fpn_feature_dim, cfg.fpn_with_gap, cfg.fpn_with_norm, cfg.fpn_upsample_method)
         self.rpn = RPN(cfg.num_anchors, cfg.fpn_feature_dim)      # rpn_with_norm unused, as in resnet_upsnet.py:52
         self.rcnn = RCNN(self.num_classes, self.num_reg_classes, dim_in=cfg.fpn_feature_dim, with_norm=cfg.rcnn_with_norm)
         self.mask_branch = MaskBranch(self.num_classes, cfg.mask_size, dim_in=cfg.fpn_feature_dim,

@@ -539,6 +539,21 @@ def upsample_bilinear(x, factor):
     return y
 
 
+def upsample2_bilinear(x):
+    """F.interpolate(x, scale_factor=2, mode='bilinear', align_corners=False) on the activation stream (models/fpn.py:27-35,
+    network.fpn_upsample_method = 'bilinear'): x a Pair, or a bf16 / fp32 logical [N,C,h,w] tensor (NHWC storage; a
+    copy only when it is not channels_last) -> [N,C,2h,2w] in x's format, interpolated in fp32 and rounded once."""
+    require_cuda(x)
+    N, Cc, h, w = x.shape
+    xs, dt = _gn_store(x)
+    y = torch.empty((N, 2 * h, 2 * w, xs.shape[-1]), dtype=xs.dtype, device=xs.device)
+    work = {"bytes": float((xs.numel() + y.numel()) * xs.element_size()),
+            "shape": "N%d %dx%d C%d %s" % (N, h, w, Cc, {0: "float32", 1: "bfloat16", 2: "pair"}[dt])}
+    with _Timed("upsample2_bilinear", 1, work, xs.device):
+        call("upsample2_bilinear_nhwc", xs.device, xs, y, N, h, w, Cc, dt)
+    return _gn_wrap(y, dt)
+
+
 def fcn_score_fuse(s2, s3, s4, s5):
     """s2 + up2(s3) + up4(s4) + up8(s5) on contiguous NCHW fp32 score maps (models/fcn.py:94-101 after the engine's
     score-before-upsample rewrite), one launch instead of three F.interpolate + three adds."""
@@ -573,15 +588,18 @@ def _gn_wrap(store, dt):
 
 
 def group_norm(x, weight, bias, groups=32, eps=1e-5, relu=False, residual=None, residual_up2=False, shift=None,
-               return_stats=False):
+               return_stats=False, upsample="nearest"):
     """nn.GroupNorm(groups, C) over whole maps, with the optional epilogue y = act(GN(x) + shift + up2(residual)):
-    shift float32 [N, C] (FPN's context vector, models/fpn.py:84-86), residual [N,C,H/2,W/2] read with nearest 2x
-    up-sampling (the FPN top-down add; residual_up2 must be set), ReLU.  x: a Pair, or a bf16 / fp32 logical [N,C,H,W]
+    shift float32 [N, C] (FPN's context vector, models/fpn.py:84-86), residual [N,C,H/2,W/2] read with 2x up-sampling
+    (the FPN top-down add; residual_up2 must be set), nearest or, with upsample='bilinear', bilinear with
+    align_corners=False (network.fpn_upsample_method), ReLU.  x: a Pair, or a bf16 / fp32 logical [N,C,H,W]
     tensor; y has x's format (Pair, or NHWC storage viewed as [N,C,H,W]).  With return_stats also the float32
     [N, groups, 2] (mean, 1 / sqrt(var + eps)) that upsnet_group_norm_backward reads."""
     require_cuda(x, weight, bias, shift)
     if (residual is not None) != bool(residual_up2):
-        raise _lib.UpsnetError("group_norm: a residual is read with nearest 2x up-sampling only (residual_up2=True)")
+        raise _lib.UpsnetError("group_norm: a residual is read with 2x up-sampling only (residual_up2=True)")
+    if upsample not in ("nearest", "bilinear"):
+        raise _lib.UpsnetError("group_norm: upsample %r is not one of 'nearest', 'bilinear'" % (upsample,))
     N, C, H, W = x.shape
     xs, dt = _gn_store(x)
     res = None if residual is None else _gn_store(residual, like=xs if dt != _lib.DTYPE_PAIR else x)[0]
@@ -593,6 +611,9 @@ def group_norm(x, weight, bias, groups=32, eps=1e-5, relu=False, residual=None, 
             "shape": "N%d %dx%d C%d G%d %s%s%s" % (N, H, W, C, groups, {0: "float32", 1: "bfloat16", 2: "pair"}[dt],
                                                   " +res" if res is not None else "", " +shift" if shift is not None else "")}
     flags = (_lib.EPI_RELU if relu else 0) | (_lib.EPI_RES_UP2 if res is not None else 0)
+    if res is not None and upsample == "bilinear":
+        flags |= _lib.EPI_RES_BILINEAR
+        work["shape"] += " bilinear"
     with _Timed("group_norm", 3, work, xs.device):
         call("group_norm_forward", xs.device, xs, f32c(weight), f32c(bias), None if shift is None else f32c(shift), res,
              y, stats, N, C, H, W, groups, float(eps), dt, flags, ws, ws.numel())

@@ -41,6 +41,8 @@
   only and can be replayed from a CUDA graph.  Unlike the reference, the step does not write g + wd p back into p.grad.
 * FcnScoreFuseFunction / fcn_score_fuse_backward: the semantic head's level sum s2 + up2(s3) + up4(s4) + up8(s5) with
   its adjoint on the device (csrc/pool.cu upsnet_fcn_score_fuse_backward), used by the model's training forward.
+* Upsample2BilinearFunction / upsample2_bilinear: the FPN's bilinear top-down up-sampling (network.fpn_upsample_method
+  = 'bilinear') with its adjoint on the device (csrc/upsample2.cu); GroupNormFunction reads its residual the same way.
 
 Scope note: this is the operator / communication layer of the training configuration, the RPN and proposal targets,
 the label maps, every loss of the training forward, the dense convolutions and FC layers with their gradients, and the
@@ -386,22 +388,22 @@ class GroupNormFunction(torch.autograd.Function):
     only what needs_input_grad asks for."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, shift, residual, groups, eps, relu):
+    def forward(ctx, x, weight, bias, shift, residual, groups, eps, relu, upsample):
         from . import operators as ops
         require_cuda(x, weight, bias, shift, residual)
         xs = ops._nhwc(x.detach().float())
         y, stats = ops.group_norm(xs.permute(0, 3, 1, 2), weight.detach(), bias.detach(), groups, eps, relu,
                                   None if residual is None else residual.detach().float(), residual is not None,
-                                  None if shift is None else shift.detach(), return_stats=True)
+                                  None if shift is None else shift.detach(), return_stats=True, upsample=upsample)
         ctx.save_for_backward(xs, y if relu else None, stats, weight)
-        ctx.cfg = (groups, relu, residual is not None)
+        ctx.cfg = (groups, relu, residual is not None, upsample)
         return y
 
     @staticmethod
     def backward(ctx, grad_out):
         from . import operators as ops
         xs, y, stats, weight = ctx.saved_tensors
-        groups, relu, has_res = ctx.cfg
+        groups, relu, has_res, upsample = ctx.cfg
         ni = ctx.needs_input_grad
         N, H, W, C = xs.shape
         dev = xs.device
@@ -414,20 +416,56 @@ class GroupNormFunction(torch.autograd.Function):
         nb = query_bytes("group_norm_backward_workspace_bytes", N, C, H, W, groups)
         ws = torch.empty(nb, dtype=torch.uint8, device=dev)
         flags = (_lib.EPI_RELU if relu else 0) | (_lib.EPI_RES_UP2 if has_res else 0)
+        if has_res and upsample == "bilinear":
+            flags |= _lib.EPI_RES_BILINEAR
         call("group_norm_backward", dev, dy, xs, None if y is None else y.permute(0, 2, 3, 1), stats, weight.detach(),
              dx, dgamma, dbeta, dshift, dres, N, C, H, W, groups, flags, ws, nb)
         return (dx.permute(0, 3, 1, 2), dgamma, dbeta, dshift, None if dres is None else dres.permute(0, 3, 1, 2),
-                None, None, None)
+                None, None, None, None)
 
 
-def group_norm(x, weight, bias, groups=32, eps=1e-5, relu=False, residual=None, shift=None):
+def group_norm(x, weight, bias, groups=32, eps=1e-5, relu=False, residual=None, shift=None, upsample="nearest"):
     """Differentiable nn.GroupNorm(groups, C) with the fused epilogue of ops.group_norm: x float32 [N,C,H,W] (or [R,C],
-    normalised as [R,C,1,1], RCNN fc6); residual [N,C,H/2,W/2] added after nearest 2x up-sampling; shift [N,C].
+    normalised as [R,C,1,1], RCNN fc6); residual [N,C,H/2,W/2] added after 2x up-sampling, nearest or with
+    upsample='bilinear' bilinear (align_corners=False; its gradient is the adjoint of that up-sampling); shift [N,C].
     -> float32 of x's logical shape, channels_last storage."""
     if x.dim() == 2:
         R, C = x.shape
-        return GroupNormFunction.apply(x.reshape(R, C, 1, 1), weight, bias, shift, residual, groups, eps, relu).reshape(R, C)
-    return GroupNormFunction.apply(x, weight, bias, shift, residual, groups, eps, relu)
+        return GroupNormFunction.apply(x.reshape(R, C, 1, 1), weight, bias, shift, residual, groups, eps, relu,
+                                       upsample).reshape(R, C)
+    return GroupNormFunction.apply(x, weight, bias, shift, residual, groups, eps, relu, upsample)
+
+
+def upsample2_bilinear_adjoint(dy):
+    """dx = up2^T(dy) for dy float32 [N,C,2h,2w]: the adjoint of the bilinear 2x up-sampling (align_corners=False) on
+    NHWC storage (upsnet_upsample2_bilinear_nhwc_adjoint) -> float32 [N,C,h,w], channels_last storage."""
+    from . import operators as ops
+    require_cuda(dy)
+    g = ops._nhwc(dy.float())
+    N, H, W, Cc = g.shape
+    dx = torch.empty((N, H // 2, W // 2, Cc), dtype=torch.float32, device=g.device)
+    call("upsample2_bilinear_nhwc_adjoint", g.device, g, dx, N, H // 2, W // 2, Cc)
+    return dx.permute(0, 3, 1, 2)
+
+
+class Upsample2BilinearFunction(torch.autograd.Function):
+    """F.interpolate(x, scale_factor=2, mode='bilinear', align_corners=False) of a float32 map (the FPN top-down path
+    with network.fpn_upsample_method = 'bilinear'): forward ops.upsample2_bilinear, backward its adjoint."""
+
+    @staticmethod
+    def forward(ctx, x):
+        from . import operators as ops
+        return ops.upsample2_bilinear(x.detach().float())
+
+    @staticmethod
+    def backward(ctx, grad):
+        return upsample2_bilinear_adjoint(grad)
+
+
+def upsample2_bilinear(x):
+    """Differentiable bilinear 2x up-sampling (align_corners=False) of x float32 [N,C,h,w] (C % 8 == 0) ->
+    float32 [N,C,2h,2w], channels_last storage."""
+    return Upsample2BilinearFunction.apply(x)
 
 
 class ConvTranspose2x2Function(torch.autograd.Function):
